@@ -126,8 +126,9 @@ static_assert((sizeof(LqSmem) * LQ_WARPS + 1024) * QMB_LQ_MINB <= 232448, "proje
 #ifndef QMB_FL_MINB
 #define QMB_FL_MINB 2
 #endif
-constexpr int FL_WARPS = 4, FL_TILE = 64;   // widest block of the record: a foot (63 doubles)
-constexpr int FL_SMEM = FL_WARPS * 32 * (FL_TILE + 1) * 8;
+constexpr int FL_WARPS = 4, FL_TILE = ne::EE_DBL;   // widest block of the record: the end-effector error and its Jacobian (78 doubles)
+constexpr int FL_UROW = NU + 1;   // the node's input in a shared-memory row per thread (odd length: no bank conflicts), 60 registers the kinematics need more
+constexpr int FL_SMEM = FL_WARPS * 32 * (FL_TILE + 1 + FL_UROW) * 8;   // 110.6 KB: two CTAs per SM
 __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(const DevModel* __restrict__ mdl, int b0, int B, int nmax, MpcProblemDev p, MpcSolutionDev sol, double* __restrict__ rec, const int32_t* __restrict__ status) {
   // Each block of the record is produced straight into the lane's row of the warp's transposition tile (shared memory: the record never lives in thread-local
   // memory - with 34 k resident threads on an H100 a 4 KB stack frame is 138 MB, more than the 50 MB L2) and leaves as one contiguous run per node and store instruction.
@@ -143,14 +144,18 @@ __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(co
   auto flush = [&](int off, int cnt) {   // rows of the tile -> records: 32 (or 64) consecutive doubles of one node per store instruction
     __syncwarp();
 #pragma unroll 4
-    for (int rw = 0; rw < 32; ++rw) if ((active >> rw) & 1u) { double* g = gbase + (size_t)rw * ne::NODE_REC_DBL + off; if (lane < cnt) g[lane] = tile[warp][rw][lane]; if (lane + 32 < cnt) g[lane + 32] = tile[warp][rw][lane + 32]; }
+    for (int rw = 0; rw < 32; ++rw) if ((active >> rw) & 1u) { double* g = gbase + (size_t)rw * ne::NODE_REC_DBL + off;
+#pragma unroll
+      for (int c = lane; c < FL_TILE; c += 32) if (c < cnt) g[c] = tile[warp][rw][c]; }
     __syncwarp(); };
-  double x[NX], u[NU]; ne::BaseKin bk; ne::FlowAcc acc; double t = 0.0, dt = 0.0;
+  double* u = reinterpret_cast<double*>(smem_raw + (size_t)FL_WARPS * 32 * (FL_TILE + 1) * 8) + tid * FL_UROW;
+  double x[NX]; ne::BaseKin bk; ne::FlowAcc acc; double t = 0.0, dt = 0.0;
   if (work) {
     const double* gt = sol.t + (size_t)b * nmax; const int32_t* ge = sol.event + (size_t)b * nmax;
     const double* xk = sol.x + ((size_t)b * nmax + k) * NX; const double* uk = sol.u + ((size_t)b * nmax + k) * NU;
 #pragma unroll
     for (int i = 0; i < NX; ++i) { x[i] = xk[i]; u[i] = terminal ? 0.0 : uk[i]; }
+    asm volatile("" ::: "memory");   // u is read back from the row where it is used, not held in registers
     t = interval_start(gt[k], ge[k]); dt = terminal ? 0.0 : interval_end(gt[k + 1], ge[k + 1]) - t;
     ne::base_eval<true>(mdl, x, bk); ne::flow_acc_init(acc);
   }
@@ -166,16 +171,10 @@ __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(co
 #pragma unroll
     for (int i = 0; i < 12; ++i) f1[i] = fl->f[i]; }
   flush(4 * ne::FOOT_DBL, ne::FLOW_DBL);
-  { ne::EeRec ee;   // end-effector error and its Jacobian: 78 doubles, two flushes
-    if (work) { const int nk = clamp_targets(p.n_target[b]); const ne::TargetSeg sg = ne::target_segment(p.target_times + (size_t)b * KMAX, p.target_states + (size_t)b * KMAX * TARGET_DIM, nk, t);
-      double pref[3], qref[4]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<true>(mdl, x, bk, pref, qref, ee.e, ee.Je);
-#pragma unroll
-      for (int j = 0; j < 39; ++j) row[j] = reinterpret_cast<const double*>(&ee)[j]; }
-    flush(4 * ne::FOOT_DBL + ne::FLOW_DBL, 39);
-    if (work) {
-#pragma unroll
-      for (int j = 0; j < 39; ++j) row[j] = reinterpret_cast<const double*>(&ee)[39 + j]; }
-    flush(4 * ne::FOOT_DBL + ne::FLOW_DBL + 39, 39); }
+  if (work) { ne::EeRec* ee = reinterpret_cast<ne::EeRec*>(row);   // end-effector error and its Jacobian
+    const int nk = clamp_targets(p.n_target[b]); const ne::TargetSeg sg = ne::target_segment(p.target_times + (size_t)b * KMAX, p.target_states + (size_t)b * KMAX * TARGET_DIM, nk, t);
+    double pref[3], qref[4]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<true>(mdl, x, bk, pref, qref, ee->e, ee->Je); }
+  flush(4 * ne::FOOT_DBL + ne::FLOW_DBL, ne::EE_DBL);
   const bool stage2 = work && !terminal;
   if (stage2) {   // second RK2 stage at x + c dt k1 (rows 12:30 of the flow map are the joint-velocity inputs)
     const double cdt = mdl->rk_c * dt;
@@ -822,7 +821,7 @@ __global__ void __launch_bounds__(RIC_THREADS, 4) mpc_riccati_kernel(const DevMo
 // =====================================================================================================
 // K4: filter line search (one CTA per robot; warps stride over nodes) + trajectory update + input fix-up
 // One THREAD per node (node_eval.cuh): the trial point's kinematics, flow maps, cost and constraint residuals are chains of scalar work with 3..9 useful lanes in
-// the warp-per-node form; here every lane carries a node, nothing lives in shared memory, and the per-robot sums are a block reduction.
+// the warp-per-node form; here every lane carries a node (its trial point in a shared-memory row) and the per-robot sums are a block reduction.
 __device__ __forceinline__ void fixup_inputs(MpcSolutionDev sol, int b, int nmax, int n, int tid, int nthreads) {
   // toPrimalSolution [upstream]: input at a pre-event node repeats the previous one; last input repeated
   const int32_t* ge = sol.event + (size_t)b * nmax; double* gu = sol.u + (size_t)b * nmax * NU;
@@ -831,11 +830,17 @@ __device__ __forceinline__ void fixup_inputs(MpcSolutionDev sol, int b, int nmax
 }
 
 #ifndef QMB_LS_MINB
-#define QMB_LS_MINB 4
+#define QMB_LS_MINB 2
 #endif
+// The trial point (x, u: 60 doubles) and the first flow stage (12) live in a shared-memory row per thread: in registers they would take 144 of them next to the
+// kinematics, and what does not fit spills to a stack frame (2 KB per thread, 135 MB at 4 CTAs per SM on 132 SMs: more than the L2).  An odd row length in
+// doubles keeps the warp's accesses to one element free of bank conflicts.  74.8 KB per CTA.  Two CTAs per SM (255 registers, no spills) measured faster on
+// H100 than three (168 registers, 192 B of spills): 2.0 vs 2.5 ms at 8192 robots.
+constexpr int LS_ROW = NX + NU + 12 + 1, LS_SMEM = 32 * LS_WARPS * LS_ROW * 8;
 __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_kernel(const DevModel* __restrict__ mdl, int b0, int B, int nmax, MpcProblemDev p, MpcSolutionDev sol, const double* __restrict__ dxo, const double* __restrict__ duo,
                                                                      const double* __restrict__ robot, int32_t* __restrict__ status, double* __restrict__ step_info, int iteration) {
   __shared__ double red[LS_WARPS][3]; __shared__ int decision; __shared__ double s_ev[EMAX]; __shared__ unsigned char s_modes[EMAX + 8];
+  extern __shared__ double s_tp[];   // [32 * LS_WARPS][LS_ROW]: the thread's trial point (x then u)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31; const int b = b0 + blockIdx.x; if (b >= B) return;
   if (status[b] & MST_CONVERGED) return;
   const int n = sol.n_nodes[b]; const int N = n - 1;
@@ -852,35 +857,42 @@ __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_ker
   while (!failed) {
     double cost = 0.0, dyn = 0.0, eq = 0.0;
     for (int k = tid; k <= N; k += 32 * LS_WARPS) {
-      double xa[NX], ua[NU]; const bool terminal = (k == N);
-#pragma unroll
+      double* xa = s_tp + tid * LS_ROW; double* ua = xa + NX; const bool terminal = (k == N);
+#pragma unroll 6
       for (int i = 0; i < NX; ++i) { xa[i] = gx[(size_t)k * NX + i] + alpha * gdx[(size_t)k * NX + i]; ua[i] = terminal ? 0.0 : gu[(size_t)k * NU + i] + alpha * gdu[(size_t)k * NU + i]; }
+      asm volatile("" ::: "memory");   // the evaluation reads the row back where it needs an element: forwarding the 60 stored values would keep them in registers
       if (k == 0) { double s = 0.0; for (int i = 0; i < NX; ++i) { const double d = p.x0[(size_t)b * NX + i] - xa[i]; s = fma(d, d, s); } dyn += s; }
       if (!terminal && ge[k] == 1) { double s = 0.0; for (int i = 0; i < NX; ++i) { const double d = xa[i] - (gx[(size_t)(k + 1) * NX + i] + alpha * gdx[(size_t)(k + 1) * NX + i]); s = fma(d, d, s); } dyn += s; continue; }
       const double t = interval_start(gt[k], ge[k]);
       const double dt = terminal ? 1.0 : interval_end(gt[k + 1], ge[k + 1]) - t; const int mode = mode_at_time(ev, modes, ne, t); const int fm = terminal ? 0 : flag_mask(mode);
-      ne::BaseKin bk; ne::FlowAcc acc; double f1[12];
+      ne::BaseKin bk; ne::FlowAcc acc; double* f1 = ua + NU;
       ne::base_eval<false>(mdl, xa, bk); ne::flow_acc_init(acc);
-      { double fe[4][3], pf[4][3];
+      { double es = 0.0; bool ok = true;
 #pragma unroll 1
-        for (int i = 0; i < 4; ++i) { double d[3], Jl[9]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, pf[i], Jl, nullptr, nullptr); if (!terminal) ne::foot_velocity_1<false>(mdl, xa, ua, bk, i, d, Jl, nullptr, fe[i], nullptr); }
-        if (!terminal) eq += dt * ne::equality_ss(mdl, ua, fe, pf, fm, ev, modes, ne, t, nullptr); }
+        for (int i = 0; i < 4; ++i) { double d[3], Jl[9], pf[3]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, pf, Jl, nullptr, nullptr);
+          if (!terminal) { double fe[3]; ne::foot_velocity_1<false>(mdl, xa, ua, bk, i, d, Jl, nullptr, fe, nullptr); ne::equality_add(mdl, ua, fe, pf, fm, ev, modes, ne, t, i, es, ok); } }
+        if (!terminal) eq += dt * es; }
       ne::flow_finish<false>(mdl, xa, bk, acc, f1, nullptr);
+      asm volatile("" ::: "memory");   // f1 is read back after the cost, not held in registers across it
       { const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, xa, bk, pref, qref, ee, nullptr);
         cost += dt * ne::cost_value(mdl, xa, ua, sg, ee, fm, terminal); }
       if (terminal) continue;
       const double cdt = mdl->rk_c * dt;   // second stage in place (the trial state is re-read from L2 for the defect)
 #pragma unroll
-      for (int i = 0; i < NX; ++i) xa[i] += cdt * (i < 12 ? f1[i < 12 ? i : 0] : ua[i]);
+      for (int i = 0; i < 12; ++i) xa[i] += cdt * f1[i];
+#pragma unroll 6
+      for (int i = 12; i < NX; ++i) xa[i] += cdt * ua[i];
       double f2[12]; ne::base_eval<false>(mdl, xa, bk); ne::flow_acc_init(acc);
 #pragma unroll 1
       for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr); }
       ne::flow_finish<false>(mdl, xa, bk, acc, f2, nullptr);
       double s = 0.0;
+      auto defect = [&](int i, double fa, double fb) { const double x0i = gx[(size_t)k * NX + i] + alpha * gdx[(size_t)k * NX + i];
+        const double d = x0i + dt * (w1 * fa + w2 * fb) - (gx[(size_t)(k + 1) * NX + i] + alpha * gdx[(size_t)(k + 1) * NX + i]); s = fma(d, d, s); };
 #pragma unroll
-      for (int i = 0; i < NX; ++i) { const double fa = (i < 12) ? f1[i < 12 ? i : 0] : ua[i], fb = (i < 12) ? f2[i < 12 ? i : 0] : ua[i];   // rows 12:30 of the flow map are the joint-velocity inputs
-        const double x0i = gx[(size_t)k * NX + i] + alpha * gdx[(size_t)k * NX + i];
-        const double d = x0i + dt * (w1 * fa + w2 * fb) - (gx[(size_t)(k + 1) * NX + i] + alpha * gdx[(size_t)(k + 1) * NX + i]); s = fma(d, d, s); }
+      for (int i = 0; i < 12; ++i) defect(i, f1[i], f2[i]);
+#pragma unroll 6
+      for (int i = 12; i < NX; ++i) defect(i, ua[i], ua[i]);   // rows 12:30 of the flow map are the joint-velocity inputs
       dyn += dt * s;
     }
     cost = warp_sum(cost); dyn = warp_sum(dyn); eq = warp_sum(eq);
@@ -945,10 +957,11 @@ constexpr int RO_THREADS = 128, RO_MAXTRIALS = 32;
 template <bool PERF, class MT>
 __device__ __forceinline__ void rollout_step(const DevModel* __restrict__ mdl, double* x, const double* u, double t, double dt, int fm, const double* ev, const MT* modes, int ne, const double* tt, const double* ts, int nk, double& cost, double& eq) {
   ne::BaseKin bk; ne::FlowAcc acc; double f1[12], x2[NX]; ne::base_eval<false>(mdl, x, bk); ne::flow_acc_init(acc);
-  if (PERF) { double fe[4][3], pf[4][3];
+  if (PERF) { double es = 0.0; bool ok = true;
 #pragma unroll 1
-    for (int i = 0; i < 4; ++i) { double d[3], Jl[9]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, pf[i], Jl, nullptr, nullptr); ne::foot_velocity_1<false>(mdl, x, u, bk, i, d, Jl, nullptr, fe[i], nullptr); }
-    eq += dt * ne::equality_ss(mdl, u, fe, pf, fm, ev, modes, ne, t, nullptr);
+    for (int i = 0; i < 4; ++i) { double d[3], Jl[9], pf[3], fe[3]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, pf, Jl, nullptr, nullptr); ne::foot_velocity_1<false>(mdl, x, u, bk, i, d, Jl, nullptr, fe, nullptr);
+      ne::equality_add(mdl, u, fe, pf, fm, ev, modes, ne, t, i, es, ok); }
+    eq += dt * es;
     const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, x, bk, pref, qref, ee, nullptr);
     cost += dt * ne::cost_value(mdl, x, u, sg, ee, fm, false);
   } else {
@@ -1127,6 +1140,7 @@ bool mpc_alloc(MpcBuffers& m, int B, int nmax, std::string& err, std::vector<voi
 int mpc_configure_device() {
   cudaError_t e = cudaFuncSetAttribute(mpc_setup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);   // 48 B per node and warp: opt-in beyond nmax ~ 250
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_flow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FL_SMEM);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_linesearch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LS_SMEM);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_rollout_trials_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RO_RPC_MAX * GAIN_DBL * 8);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_lq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LqSmem) * LQ_WARPS));
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_riccati_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RicSmem));
@@ -1155,7 +1169,7 @@ int mpc_solve_launch(const DevModel* mdl, const DevModel& hm, MpcBuffers& m, con
     if (ev && it == iters - 1) cudaEventRecord(ev[3], stream);
     if (ddp) { mpc_rollout_trials_kernel<<<(nb + ro_rpc - 1) / ro_rpc, ro_rpc * tr_pitch, (size_t)ro_rpc * GAIN_DBL * 8, stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.ddp_trial, m.robot, m.status, n_trials, tr_pitch, ro_rpc);   // all step lengths side by side
       mpc_rollout_kernel<<<ro_grid, RO_THREADS, 0, stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.ddp_trial, m.robot, m.status, m.step_info, 2, n_trials, tr_pitch, it); ++launched; }   // decision + in-place rollout of the accepted step
-    else mpc_linesearch_kernel<<<nb, 32 * LS_WARPS, 0, stream>>>(mdl, b0, b1, nmax, p, next, m.dx, m.du, m.robot, m.status, m.step_info, it);
+    else mpc_linesearch_kernel<<<nb, 32 * LS_WARPS, LS_SMEM, stream>>>(mdl, b0, b1, nmax, p, next, m.dx, m.du, m.robot, m.status, m.step_info, it);
     launched += 4;
   }
   if (ev) cudaEventRecord(ev[4], stream);

@@ -35,16 +35,20 @@ struct BaseKin { double tr[6], R0[9], T[9], Tinv[9], W[9], c[3], rcom[3], omega[
 // sums over the feet that the flow map needs
 struct FlowAcc { double fsum[3], hang[3], hth[3][3]; };
 
-// one serial chain from the base: joints first .. first + NJC - 1; returns the last body's frame, every joint's origin and axis (world)
+// a[3 * s + c] for a block s in 0..3 known only at run time (a foot's forces, a leg's joints): a chain of selects with static register indices.  Indexing the
+// thread's array with s directly would place the whole array in local memory.
+QMB_HD double pick3(const double* a, int s, int c) { return s == 0 ? a[c] : (s == 1 ? a[3 + c] : (s == 2 ? a[6 + c] : a[9 + c])); }
+
+// one serial chain from the base: joints first .. first + NJC - 1 at angles q[0 .. NJC - 1]; returns the last body's frame, every joint's origin and axis (world)
 template <int NJC>
-QMB_HD void chain_fk(const DevModel* __restrict__ mdl, const double* R0, const double* p0, const double* qj, int first, double* Rl, double* pl, double (*org)[3], double (*axs)[3]) {
+QMB_HD void chain_fk(const DevModel* __restrict__ mdl, const double* R0, const double* p0, const double* q, int first, double* Rl, double* pl, double (*org)[3], double (*axs)[3]) {
   double Rp[9], pp[3];
 #pragma unroll
   for (int i = 0; i < 9; ++i) Rp[i] = R0[i];
   pp[0] = p0[0]; pp[1] = p0[1]; pp[2] = p0[2];
 #pragma unroll
   for (int jj = 0; jj < NJC; ++jj) {
-    const int j = first + jj; double s, c; sincos(qj[j], &s, &c);
+    const int j = first + jj; double s, c; sincos(q[jj], &s, &c);
     const int ax = mdl->axis[j]; const double* Rj = mdl->Rj[j]; double Rlq[9];
 #pragma unroll
     for (int i = 0; i < 3; ++i) { const double r0 = Rj[3 * i], r1 = Rj[3 * i + 1], r2 = Rj[3 * i + 2];   // Rj * Rq(axis, q): Rq mixes the two columns after the axis
@@ -90,10 +94,11 @@ QMB_HD void flow_acc_init(FlowAcc& acc) { for (int a = 0; a < 3; ++a) { acc.fsum
 template <bool JAC>
 QMB_HD void foot_eval(const DevModel* __restrict__ mdl, const double* x, const double* u, const BaseKin& bk, int i, FlowAcc& acc, double* d, double* pf, double* Jl, double* al, double* JxF) {
   const int first = mdl->foot_leg[i]; double Rl[9], pl[3], org[3][3], axs[3][3];
-  chain_fk<3>(mdl, bk.R0, x + 6, x + 12, first, Rl, pl, org, axs);
+  const double q[3] = {pick3(x + 12, first / 3, 0), pick3(x + 12, first / 3, 1), pick3(x + 12, first / 3, 2)};
+  chain_fk<3>(mdl, bk.R0, x + 6, q, first, Rl, pl, org, axs);
   double pw[3]; matvec3(Rl, mdl->foot_p[i], pw);
   for (int a = 0; a < 3; ++a) { pw[a] += pl[a]; d[a] = pw[a] - bk.rcom[a]; if (pf) pf[a] = pw[a]; }
-  const double* F = u + 3 * i; const double im = 1.0 / mdl->total_mass;
+  const double F[3] = {pick3(u, i, 0), pick3(u, i, 1), pick3(u, i, 2)}; const double im = 1.0 / mdl->total_mass;
   for (int a = 0; a < 3; ++a) acc.fsum[a] += F[a];
   cross3_add(d, F, acc.hang);
   for (int j = 0; j < 3; ++j) { const double r[3] = {pw[0] - org[j][0], pw[1] - org[j][1], pw[2] - org[j][2]}; double col[3]; cross3(axs[j], r, col);
@@ -132,7 +137,7 @@ QMB_HD void flow_finish(const DevModel* __restrict__ mdl, const double* x, const
 // foot velocity v_i = h_lin + omega x d_i + sum_j Jl_j qd_j (+ its state Jacobian on the 12 support columns), foot_velocity<> of mpc_device.cuh for one foot
 template <bool JAC>
 QMB_HD void foot_velocity_1(const DevModel* __restrict__ mdl, const double* x, const double* u, const BaseKin& bk, int i, const double* d, const double* Jli, const double* ali, double* e, double (*C)[12]) {
-  const int first = mdl->foot_leg[i]; const double* om = bk.omega; const double qd[3] = {u[12 + first], u[12 + first + 1], u[12 + first + 2]};
+  const int leg = mdl->foot_leg[i] / 3; const double* om = bk.omega; const double qd[3] = {pick3(u + 12, leg, 0), pick3(u + 12, leg, 1), pick3(u + 12, leg, 2)};
   double w[3] = {0, 0, 0}; for (int j = 0; j < 3; ++j) for (int a = 0; a < 3; ++a) w[a] += Jli[3 * j + a] * qd[j];
   double v[3]; cross3(om, d, v); for (int a = 0; a < 3; ++a) e[a] = v[a] + x[a] + w[a];
   if (JAC) {
@@ -172,7 +177,7 @@ QMB_HD void target_pose(const TargetSeg& sg, int nk, double* pref, double* qref)
 template <bool JAC>
 QMB_HD void ee_eval(const DevModel* __restrict__ mdl, const double* x, const BaseKin& bk, const double* pref, const double* qref, double* e, double* Je /*[6][12]*/) {
   double Rl[9], pl[3], org[6][3], axs[6][3];
-  chain_fk<6>(mdl, bk.R0, x + 6, x + 12, 12, Rl, pl, org, axs);
+  chain_fk<6>(mdl, bk.R0, x + 6, x + 24, 12, Rl, pl, org, axs);
   double R[9]; matmul3(Rl, mdl->ee_R, R); double pw[3]; matvec3(Rl, mdl->ee_p, pw);
   for (int a = 0; a < 3; ++a) { pw[a] += pl[a]; e[a] = pw[a] - pref[a]; }
   double q[4]; const double tr = R[0] + R[4] + R[8];   // rotation -> quaternion (w,x,y,z); sign free (quadratic penalty), same q used for e and its Jacobian
@@ -200,14 +205,17 @@ QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, cons
   double value = 0.0;
   if (!terminal) {
     int nst = 0; for (int i = 0; i < 4; ++i) nst += (flagmask >> i) & 1;
-    double dx[NX], du[NU];
-    for (int i = 0; i < NX; ++i) { dx[i] = x[i] - (sg.a * sg.l[i] + (1.0 - sg.a) * sg.rr[i]); double un = 0.0; if (i < 12 && (i % 3) == 2 && ((flagmask >> (i / 3)) & 1)) un = mdl->total_mass * 9.81 / nst; du[i] = u[i] - un; }
+    // deviations from the references element by element where they are used: whole dx[30] / du[30] arrays would not fit in registers next to (x, u)
+    auto dx = [&](int i) { return x[i] - (sg.a * sg.l[i] + (1.0 - sg.a) * sg.rr[i]); };
+    const double un = mdl->total_mass * 9.81 / nst;
     double acc = 0.0;
-    if (mdl->q_is_diag) { for (int i = 0; i < NX; ++i) acc = fma(dx[i] * mdl->Qdiag[i], dx[i], acc); }
-    else { for (int i = 0; i < NX; ++i) { double qd = 0.0; for (int j = 0; j < NX; ++j) qd = fma(mdl->Q[i * NX + j], dx[j], qd); acc = fma(dx[i], qd, acc); } }
-    for (int blk = 0; blk < 8; ++blk) { const double* Rb = mdl->Rblk[blk]; const double* d3 = du + 3 * blk;
+    if (mdl->q_is_diag) { for (int i = 0; i < NX; ++i) { const double d = dx(i); acc = fma(d * mdl->Qdiag[i], d, acc); } }
+    else { for (int i = 0; i < NX; ++i) { double qd = 0.0; for (int j = 0; j < NX; ++j) qd = fma(mdl->Q[i * NX + j], dx(j), qd); acc = fma(dx(i), qd, acc); } }
+#pragma unroll
+    for (int blk = 0; blk < 8; ++blk) { const double* Rb = mdl->Rblk[blk];   // blocks 0..3: the feet's forces (weight compensation on the z force of a stance foot)
+      const double d3[3] = {u[3 * blk], u[3 * blk + 1], u[3 * blk + 2] - ((blk < 4 && ((flagmask >> blk) & 1)) ? un : 0.0)};
       for (int r = 0; r < 3; ++r) acc = fma(d3[r], fma(Rb[3 * r], d3[0], fma(Rb[3 * r + 1], d3[1], Rb[3 * r + 2] * d3[2])), acc); }
-    for (int i = 0; i < 6; ++i) acc = fma(du[24 + i] * mdl->Rarm[i], du[24 + i], acc);
+    for (int i = 0; i < 6; ++i) acc = fma(u[24 + i] * mdl->Rarm[i], u[24 + i], acc);
     value += 0.5 * acc;
   }
   { const double mup = terminal ? mdl->mu_final_ee_pos : mdl->mu_ee_pos, muo = terminal ? mdl->mu_final_ee_ori : mdl->mu_ee_ori;
@@ -231,15 +239,18 @@ QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, cons
   return value;
 }
 
+// foot i's terms of equality_ss added to es (feet in contact order, so a caller can add them foot by foot without keeping every foot's e and pf)
+template <class MT>
+QMB_HD void equality_add(const DevModel* __restrict__ mdl, const double* u, const double* e, const double* pf, int flagmask, const double* ev, const MT* modes, int ne, double t, int i, double& es, bool& ok) {
+  if ((flagmask >> i) & 1) { for (int a = 0; a < 3; ++a) es += e[a] * e[a]; }
+  else { double zp, zv; ok &= swing_reference(mdl, ev, modes, ne, i, t, zp, zv); double ez = e[2] - zv; if (mdl->position_error_gain != 0.0) ez += mdl->position_error_gain * (pf[2] - zp);
+    es += ez * ez; for (int a = 0; a < 3; ++a) { const double F = pick3(u, i, a); es += F * F; } }
+}
 // squared equality-constraint residual of a node (ZeroVelocity on stance feet; ZeroForce + NormalVelocity on swing feet); swing_ok reports an unenclosed swing phase
 template <class MT>
 QMB_HD double equality_ss(const DevModel* __restrict__ mdl, const double* u, const double (*e)[3], const double (*pf)[3], int flagmask, const double* ev, const MT* modes, int ne, double t, bool* swing_ok) {
   double es = 0.0; bool ok = true;
-  for (int i = 0; i < 4; ++i) {
-    if ((flagmask >> i) & 1) { for (int a = 0; a < 3; ++a) es += e[i][a] * e[i][a]; }
-    else { double zp, zv; ok &= swing_reference(mdl, ev, modes, ne, i, t, zp, zv); double ez = e[i][2] - zv; if (mdl->position_error_gain != 0.0) ez += mdl->position_error_gain * (pf[i][2] - zp);
-      es += ez * ez; for (int a = 0; a < 3; ++a) es += u[3 * i + a] * u[3 * i + a]; }
-  }
+  for (int i = 0; i < 4; ++i) equality_add(mdl, u, e[i], pf[i], flagmask, ev, modes, ne, t, i, es, ok);
   if (swing_ok) *swing_ok = ok;
   return es;
 }
