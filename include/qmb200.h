@@ -203,6 +203,35 @@ int qmb200_hw_write_dev(qmb200_handle* h, const double* time, const double* peri
 /* gazebo/delay (qm_gazebo/config/default.yaml:2; QMHWSim.cpp:33-35 defaults to 0); clears the FIFO */
 int qmb200_hw_set_delay(qmb200_handle* h, double delay);
 
+/* ---- plant: Gazebo's physics step behind QMHWSim (one writeSim → physics step → readSim cycle) plus the contact flags QMHWSim::readSim reports to the
+ *      ContactSensorInterface (qm_gazebo/src/QMHWSim.cpp:71-90), batched on the device.  Forward dynamics of the 24-DoF tree with a compliant contact
+ *      between each foot's collision sphere and a flat ground plane (this project's contact law, not Gazebo/ODE's: DESIGN.md §4.6).  The caller owns
+ *      the plant state q[24] = [p_base, euler ZYX, joints], v[24] = dq/dt. */
+typedef struct {
+  double ground_height;        /* plane z = ground_height (m); default 0 */
+  double foot_radius;          /* foot collision sphere, centred on the *_FOOT frame (m); default 0.0265 (robot.urdf *_FOOT <collision>) */
+  double stiffness;            /* normal force F_n = max(0, stiffness * delta - damping * dz/dt), delta = penetration (N/m); default 1e6 */
+  double damping;              /* (N s/m); default 1e3 */
+  double tangential_damping;   /* friction F_t = -v_t * min(tangential_damping, friction_mu * F_n / |v_t|) (N s/m); default 1e3 */
+  double friction_mu;          /* default 0.6 (robot.urdf mu1 / mu2 of the feet) */
+  double joint_damping[18];    /* viscous joint damping (N m s/rad); default robot.urdf <dynamics damping>: 0.05 legs, 0 arm */
+  int32_t substeps_per_ms;     /* semi-implicit Euler substeps per simulated millisecond; default 4 */
+} qmb200_sim_params;
+int qmb200_sim_get_params(const qmb200_handle* h, qmb200_sim_params* out);
+/* rejects non-finite values, foot_radius / stiffness / damping / tangential_damping / friction_mu <= 0, joint_damping < 0, substeps_per_ms < 1 */
+int qmb200_sim_set_params(qmb200_handle* h, const qmb200_sim_params* p);
+/* Advance every robot by `duration` s (0 < duration <= 1) with the effort held, as one writeSim → physics step: effort is clipped to the URDF effort
+ * limits (gazebo_ros_control DefaultRobotHWSim), q and v are updated in place; rbd = the measured state at the end (qm_estimation's ground-truth
+ * layout, EE pose included); contact = 4-bit mask of the feet with a positive normal force in the last substep (LF=8 RF=4 LH=2 RH=1);
+ * status = QMB200_ST_NAN (non-finite state) | QMB200_ST_NOT_PD (mass matrix not positive definite: the robot stops at that substep).
+ * status is this plant's own word: nothing is OR-ed into the controller's. */
+int qmb200_sim_step(qmb200_handle* h, double duration, const double* effort /*[B][18]*/, double* q /*[B][24] in-out*/, double* v /*[B][24] in-out*/,
+                    double* rbd /*[B][55]*/, int32_t* contact /*[B]*/, int32_t* status /*[B]*/);
+int qmb200_sim_step_dev(qmb200_handle* h, double duration, const double* effort, double* q, double* v, double* rbd, int32_t* contact, int32_t* status, void* cuda_stream);
+/* Host utility: the nominal standing configuration (defaultJointState, base at the given x, y, yaw, zero roll and pitch) with the base height at
+ * which the four foot spheres carry m g / 4 each at the static penetration of the current params; v = 0. */
+int qmb200_sim_standing_state(const qmb200_handle* h, int32_t n, const double* xy_yaw /*[n][3]*/, double* q /*[n][24]*/, double* v /*[n][24]*/);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

@@ -28,6 +28,12 @@ class WbcGains(C.Structure):
                [("kp_arm_joint", C.c_double * 6), ("kd_arm_joint", C.c_double * 6), ("kp_ee_linear", C.c_double * 3), ("kd_ee_linear", C.c_double * 3), ("kp_ee_angular", C.c_double * 3), ("kd_ee_angular", C.c_double * 3)]
 
 
+class SimParams(C.Structure):
+    """qmb200_sim_params: the plant's contact and joint constants (include/qmb200.h, DESIGN.md §4.6)."""
+    _fields_ = [(n, C.c_double) for n in ("ground_height", "foot_radius", "stiffness", "damping", "tangential_damping", "friction_mu")] + \
+               [("joint_damping", C.c_double * 18), ("substeps_per_ms", C.c_int32)]
+
+
 # every symbol include/qmb200.h declares (checked by the CPU test-suite)
 SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_dims", "qmb200_get_model_info", "qmb200_get_joint_name",
            "qmb200_wbc_update", "qmb200_wbc_update_dev", "qmb200_wbc_set_input_last", "qmb200_wbc_get_input_last", "qmb200_wbc_get_gains", "qmb200_wbc_set_gains", "qmb200_wbc_get_diagnostics", "qmb200_wbc_set_iteration_caps",
@@ -37,7 +43,8 @@ SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_d
            "qmb200_gait_create", "qmb200_gait_destroy", "qmb200_gait_insert_template", "qmb200_gait_get_mode_schedule",
            "qmb200_observation_update", "qmb200_observation_update_dev", "qmb200_target_trajectories", "qmb200_target_trajectories_dev", "qmb200_initial_ee_target",
            "qmb200_control_law", "qmb200_control_law_dev", "qmb200_set_arm_gains", "qmb200_hw_write", "qmb200_hw_write_dev", "qmb200_hw_set_delay", "qmb200_update", "qmb200_update_dev",
-           "qmb200_debug_model_blob", "qmb200_comm_get_unique_id", "qmb200_comm_init", "qmb200_comm_destroy", "qmb200_comm_info", "qmb200_allgather_torque", "qmb200_gait_bin_permutation", "qmb200_set_pipeline", "qmb200_set_profiling", "qmb200_collect_kernel_times", "qmb200_get_kernel_times", "qmb200_get_flow_kernel_time", "qmb200_measure_fp64_peak"]
+           "qmb200_debug_model_blob", "qmb200_comm_get_unique_id", "qmb200_comm_init", "qmb200_comm_destroy", "qmb200_comm_info", "qmb200_allgather_torque", "qmb200_gait_bin_permutation", "qmb200_set_pipeline", "qmb200_set_profiling", "qmb200_collect_kernel_times", "qmb200_get_kernel_times", "qmb200_get_flow_kernel_time", "qmb200_measure_fp64_peak",
+           "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state"]
 
 _lib = None
 
@@ -65,6 +72,9 @@ def load_library():
     lib.qmb200_hw_set_delay.argtypes = [C.c_void_p, C.c_double]
     lib.qmb200_mpc_set_iterations.argtypes = [C.c_void_p, C.c_int32, C.c_double]
     lib.qmb200_initial_ee_target.restype = None
+    lib.qmb200_sim_step.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 6
+    lib.qmb200_sim_step_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 7
+    lib.qmb200_sim_standing_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.qmb200_gait_destroy.restype = None
     lib.qmb200_gait_destroy.argtypes = [C.c_void_p]
     lib.qmb200_gait_insert_template.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_double, C.c_double]

@@ -1,0 +1,99 @@
+"""Closed-loop batched simulation on one GPU: the controller of qm_controllers (QMController) driving the plant step of this library, at the
+reference's rates, entirely on device buffers of one CUDA stream (INTEGRATION.md §3).
+
+Per simulated millisecond (Gazebo's default physics step, 1 kHz):
+  every 10 ms (mpcDesiredFrequency 100, task.info)  target_trajectories_dev (cmd_vel) → mpc_solve_dev          (the MPC node + target publisher)
+  every WBC period (default 2 ms)                     update_dev: observation → evaluatePolicy → WBC → control law (QMController::update)
+  every 1 ms                                          hw_write_dev (QMHWSim::writeSim, 9 ms command delay of qm_gazebo/config/default.yaml)
+                                                      → sim_step_dev (physics step + QMHWSim::readSim's contact flags)
+The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
+the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
+tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
+"""
+import numpy as np
+
+from ._lib import EMAX, KMAX, NX, RBD, TARGET
+from .interface import gait_schedule
+
+MPC_PERIOD_MS = 10         # mpcDesiredFrequency 100 (task.info)
+HW_DELAY = 0.009           # gazebo/delay (qm_gazebo/config/default.yaml:2)
+T_START = 10.0             # QMController::updateControlLaw drives the legs only once time > 10 s
+
+
+def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None):
+    """Run `duration` s of closed loop for all solver.batch robots.
+
+    gait: a gait.info template name ("stance", "trot", ...), started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the base frame, same for every
+    robot; xy_yaw: [B, 3] initial base x, y, yaw (default zeros), each robot starts in qmb200_sim_standing_state.
+    sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
+    Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
+    safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end)."""
+    import torch
+    B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
+    n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
+    assert MPC_PERIOD_MS % wbc_period_ms == 0, "the WBC period must divide the MPC period"
+    stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
+    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+    i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
+
+    # ---- plant state, the first measurement, the controller's members (host → device once) ----
+    xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
+    q0, v0 = solver.sim_standing_state(xy)
+    t_obs0 = t_start - wbc_period_ms * 1e-3   # observation clock of `starting`; the first update brings it to t_start, the plant's clock
+    ev, md, ne = gait_schedule(gait, t_start, t_obs0, t_start + duration + solver.time_horizon + 1.0) if gait != "stance" else (np.zeros(EMAX), np.full(EMAX + 1, 15, dtype=np.int32), 0)
+    if ne >= EMAX:
+        raise ValueError("closed_loop.run: the %s schedule of %.2f s needs more than %d events" % (gait, duration, EMAX))
+    with torch.cuda.stream(stream):
+        q = f64(q0); v = f64(v0); rbd = torch.zeros((B, RBD), dtype=torch.float64, device=dev)
+        contact = torch.zeros(B, dtype=torch.int32, device=dev); sim_st = torch.zeros_like(contact); hw_st = torch.zeros_like(contact); ctl_st = torch.zeros_like(contact)
+        acc_st = torch.zeros_like(contact)
+        effort = torch.zeros((B, 18), dtype=torch.float64, device=dev); jpos = torch.zeros_like(effort); jvel = torch.zeros_like(effort)
+    stream.synchronize()
+    solver.sim_step_dev(1e-6, effort, q, v, rbd, contact, sim_st, s)   # a 1 us physics step with zero effort reads the first measured state
+    stream.synchronize()
+    rbd_h = rbd.cpu().numpy()
+    x_obs0 = solver.centroidal_state_from_rbd(rbd_h)
+    with torch.cuda.stream(stream):
+        t_obs = f64(np.full(B, t_obs0)); x_obs = f64(x_obs0)
+        joint_cmd = torch.zeros((B, 18, 5), dtype=torch.float64, device=dev); arm_pos = torch.zeros((B, 6), dtype=torch.float64, device=dev); last_time = f64(np.full(B, t_obs0))
+        cmd54 = torch.zeros((B, 54), dtype=torch.float64, device=dev)
+        cmd7 = torch.zeros((B, 7), dtype=torch.float64, device=dev); cmd7[:, :4] = f64(np.asarray(cmd_vel, dtype=np.float64)[None, :4])
+        last_ee = f64(solver.initial_ee_target()); ee_state = torch.zeros((B, 7), dtype=torch.float64, device=dev)
+        prob = dict(t0=t_obs, x0=x_obs, n_events=i32(np.full(B, ne)), event_times=f64(np.tile(ev, (B, 1))), modes=i32(np.tile(md, (B, 1))),
+                    n_target=torch.zeros(B, dtype=torch.int32, device=dev), target_times=torch.zeros((B, KMAX), dtype=torch.float64, device=dev),
+                    target_states=torch.zeros((B, KMAX, TARGET), dtype=torch.float64, device=dev))
+        period = f64(np.full(B, wbc_period_ms * 1e-3)); hw_period = f64(np.full(B, 1e-3)); hw_time = torch.zeros(B, dtype=torch.float64, device=dev)
+        ticks = n_ms // MPC_PERIOD_MS
+        rec_base = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev); rec_ee = torch.zeros((ticks, B, 7), dtype=torch.float64, device=dev)
+        rec_st = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
+    stream.synchronize()
+    solver.hw_set_delay(HW_DELAY)
+
+    def mpc_tick():
+        ee_state.copy_(rbd[:, 48:55])
+        solver.target_trajectories_dev(0, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
+        solver.mpc_solve_dev(prob, s)
+
+    with torch.cuda.stream(stream):
+        mpc_tick(); stream.synchronize()          # QMController::starting: one blocking solve before the loop
+        for k in range(n_ms):
+            if k % MPC_PERIOD_MS == 0 and k > 0:
+                mpc_tick()
+            if k % wbc_period_ms == 0:
+                solver.update_dev(rbd, period, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, ctl_st, s)
+                acc_st.bitwise_or_(ctl_st)
+            hw_time.fill_(t_start + k * 1e-3); jpos.copy_(q[:, 6:]); jvel.copy_(v[:, 6:])
+            solver.hw_write_dev(hw_time, hw_period, joint_cmd, jpos, jvel, effort, hw_st, s)
+            if sim_timer:
+                sim_timer(True)
+            solver.sim_step_dev(1e-3, effort, q, v, rbd, contact, sim_st, s)
+            if sim_timer:
+                sim_timer(False)
+            acc_st.bitwise_or_(hw_st).bitwise_or_(sim_st)
+            if (k + 1) % MPC_PERIOD_MS == 0:
+                i = (k + 1) // MPC_PERIOD_MS - 1
+                rec_base[i, :, 0:3] = rbd[:, 3:6]; rec_base[i, :, 3:6] = rbd[:, 0:3]; rec_ee[i] = rbd[:, 48:55]; rec_st[i] = acc_st; acc_st.zero_()
+    stream.synchronize()
+    t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
+    return dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
+                start_base=np.c_[q0[:, 0:3], q0[:, 3:6]], start_ee=rbd_h[:, 48:55])

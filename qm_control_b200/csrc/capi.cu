@@ -13,6 +13,7 @@
 #include "host/qm_config.h"
 #include "kernels/mpc_api.cuh"
 #include "kernels/ctrl_api.cuh"
+#include "kernels/sim_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -48,6 +49,7 @@ struct qmb200_handle {
                                *c_jpos = nullptr, *c_jvel = nullptr, *c_effort = nullptr, *c_ttimes = nullptr, *c_tstates = nullptr; int32_t *c_status = nullptr, *c_ntarget = nullptr;
   double hw_delay = 0.0; double *hw_ring_cmd = nullptr, *hw_ring_stamp = nullptr; int32_t* hw_ring_state = nullptr;   // QMHWSim command-delay FIFO
   void* comm = nullptr; int comm_ranks = 0, comm_rank = 0; double* d_send = nullptr;   // NCCL communicator of this handle (capi_comm.inc) and the packed torque rows
+  SimParams sim_prm{}; double *s_effort = nullptr, *s_q = nullptr, *s_v = nullptr, *s_rbd = nullptr; int32_t *s_contact = nullptr, *s_status = nullptr;   // plant step (capi_sim.inc)
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
 
@@ -57,6 +59,7 @@ template <class T> bool dalloc(qmb200_handle* h, T** p, size_t count) {
   if (e != cudaSuccess) { h->err = std::string("cudaMalloc failed: ") + cudaGetErrorString(e); return false; }
   cudaMemsetAsync(q, 0, count * sizeof(T), h->stream); h->allocs.push_back(q); *p = static_cast<T*>(q); return true;   // zeroed in stream order with the handle's work (lazy allocators synchronise once, see ctrl_alloc)
 }
+SimParams default_sim_params();   // capi_sim.inc
 int fail(qmb200_handle* h, const std::string& msg) { if (h) h->err = msg; else g_create_error = msg; return -1; }
 #define QMB_CUDA(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(h, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
 }  // namespace
@@ -79,6 +82,7 @@ int qmb200_create(const qmb200_config* cfg, qmb200_handle** out) {
   if (cfg->time_horizon > 0) h->hm.dev.time_horizon = cfg->time_horizon;
   if (cfg->dt > 0) h->hm.dev.dt = cfg->dt;
   h->task_file = cfg->task_file;
+  h->sim_prm = default_sim_params();
   h->B = cfg->batch; h->variant = cfg->wbc_variant; h->device = cfg->device; h->law_prm.variant = cfg->wbc_variant == QMB200_WBC_HIERARCHICAL_MPC ? 1 : 0;
   const int nint = (int)std::ceil(h->hm.dev.time_horizon / h->hm.dev.dt - 1e-9);
   h->nmax = cfg->max_nodes > 0 ? cfg->max_nodes : nint + 1 + 20;
@@ -207,3 +211,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_mpc.inc"
 #include "capi_ctrl.inc"
 #include "capi_comm.inc"
+#include "capi_sim.inc"

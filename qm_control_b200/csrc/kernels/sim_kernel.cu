@@ -1,0 +1,133 @@
+// Batched plant step: the physics Gazebo runs behind QMHWSim (qm_gazebo/src/QMHWSim.cpp), restated as forward dynamics of the 24-DoF tree with
+// compliant foot-ground contact, so that the controller's joint efforts (qmb200_hw_write) turn into the next measured state rbd[55] on the device.
+//
+// One warp owns one robot (lanes over bodies / generalised coordinates, as in rbd.cuh).  One launch advances every robot by `substeps`
+// semi-implicit Euler steps of length h with the effort held; q, v stay in shared memory between substeps.  Per substep, at (q, v):
+//   M, nle                 rbd_kinematics<true> → rbd_inertias(gravity) → rbd_accumulate → rbd_mass_matrix_nle
+//   contact (lanes 0..3)   foot sphere of radius r centred on the *_FOOT frame against the plane z = ground:
+//                          penetration delta = ground - (p_z - r); F_n = max(0, k delta - d pdot_z) for delta > 0, else 0;
+//                          F_t = -v_t min(gamma, mu F_n / |v_t|) (regularised Coulomb).  The force acts at the sphere centre, so the
+//                          sphere's rolling is not modelled: the contact point is the foot frame's point, not the lowest point of the sphere.
+//   Q                      [0_6; sat(effort) - damping .* qdot_j] + sum_f J_f^T F_f - nle      (J_f: point_jacobian of the foot frame)
+//   solve                  M qddot = Q by the warp Cholesky (wlinalg.cuh); v += h qddot; q += h v
+// After the last substep one kinematics-only pass at the final q gives the measured state rbd[55] (include/qmb200.h layout) with the
+// end-effector pose as qm_estimation fills it from ground truth.
+#include "rbd.cuh"
+#include "sim_api.cuh"
+#include "wlinalg.cuh"
+#include "../../../include/qmb200.h"
+
+namespace qmb {
+
+namespace {
+constexpr int SIM_WARPS = 2;   // robots per CTA: 2 x 15.2 KB of static shared memory
+constexpr int NTRI = NQ * (NQ + 1) / 2;
+
+struct SimWs {
+  RbdWs rb;
+  double q[NQ], v[NQ], nle[NQ], Q[NQ];
+  double M[NQ * NQ];   // dense mass matrix; once packed into L it holds the four foot Jacobians (12 x 24)
+  double L[NTRI];      // packed lower triangle of M, then its Cholesky factor
+  double fc[4][3];     // contact force of each foot (world)
+  double pf[4][3];     // foot frame origin (world)
+};
+
+// Eigen::Quaterniond(const Matrix3d&) (Shepperd's method, largest diagonal pivot); out = x, y, z, w
+__device__ __forceinline__ void rot_to_quat_xyzw(const double* m, double* o) {
+  const double t = m[0] + m[4] + m[8];
+  if (t > 0.0) {
+    double s = sqrt(t + 1.0); o[3] = 0.5 * s; s = 0.5 / s;
+    o[0] = (m[7] - m[5]) * s; o[1] = (m[2] - m[6]) * s; o[2] = (m[3] - m[1]) * s;
+  } else if (m[8] > (m[4] > m[0] ? m[4] : m[0])) {   // pivot z (the three pivots written out: no run-time register indices)
+    double s = sqrt(m[8] - m[0] - m[4] + 1.0); o[2] = 0.5 * s; s = 0.5 / s;
+    o[3] = (m[3] - m[1]) * s; o[0] = (m[2] + m[6]) * s; o[1] = (m[5] + m[7]) * s;
+  } else if (m[4] > m[0]) {                           // pivot y
+    double s = sqrt(m[4] - m[8] - m[0] + 1.0); o[1] = 0.5 * s; s = 0.5 / s;
+    o[3] = (m[2] - m[6]) * s; o[2] = (m[7] + m[5]) * s; o[0] = (m[1] + m[3]) * s;
+  } else {                                            // pivot x
+    double s = sqrt(m[0] - m[4] - m[8] + 1.0); o[0] = 0.5 * s; s = 0.5 / s;
+    o[3] = (m[7] - m[5]) * s; o[1] = (m[3] + m[1]) * s; o[2] = (m[6] + m[2]) * s;
+  }
+}
+}  // namespace
+
+__global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel* __restrict__ mdl, SimParams prm, int B, int substeps, double h,
+                                                                  const double* __restrict__ effort /*[B][18]*/, double* __restrict__ q_io /*[B][24]*/,
+                                                                  double* __restrict__ v_io /*[B][24]*/, double* __restrict__ rbd /*[B][55]*/,
+                                                                  int32_t* __restrict__ contact, int32_t* __restrict__ status) {
+  __shared__ SimWs s_ws[SIM_WARPS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * SIM_WARPS + warp;
+  if (b >= B) return;   // the whole warp leaves together
+  SimWs* w = &s_ws[warp]; RbdWs* ws = &w->rb;
+  double tau = 0.0, jdamp = 0.0;   // lane c >= 6: saturated effort and viscous damping of joint c - 6
+  if (lane < NQ) { w->q[lane] = q_io[(size_t)b * NQ + lane]; w->v[lane] = v_io[(size_t)b * NQ + lane]; }
+  if (lane >= 6 && lane < NQ) {
+    const int j = lane - 6; const double lim = mdl->effort[j];
+    tau = fmin(fmax(effort[(size_t)b * NJ + j], -lim), lim); jdamp = prm.joint_damping[j];
+  }
+  __syncwarp();
+  int st = 0; unsigned in_contact = 0;
+  for (int k = 0; k < substeps; ++k) {
+    rbd_kinematics<true>(mdl, w->q, w->v, ws, lane);
+    rbd_inertias(mdl, ws, lane, 1);
+    rbd_accumulate(mdl, ws, lane, true);
+    rbd_mass_matrix_nle(mdl, ws, w->M, NQ, w->nle, lane);
+    if (lane < NQ) { const double* row = w->M + lane * NQ; double* out = w->L + tri(lane); for (int c = 0; c <= lane; ++c) out[c] = row[c]; }
+    double fn = 0.0;
+    if (lane < 4) {
+      const int f = lane, body = mdl->foot_body[f];
+      double pw[3]; matvec3(ws->R[body], mdl->foot_p[f], pw); pw[0] += ws->p[body][0]; pw[1] += ws->p[body][1]; pw[2] += ws->p[body][2];
+      double vel[3], acc[3]; point_vel_acc(ws, body, pw, vel, acc);
+      const double pen = prm.ground_height - (pw[2] - prm.foot_radius);
+      if (pen > 0.0) fn = fmax(0.0, prm.stiffness * pen - prm.damping * vel[2]);
+      double fx = 0.0, fy = 0.0; const double vt = sqrt(vel[0] * vel[0] + vel[1] * vel[1]);
+      if (fn > 0.0 && vt > 0.0) { const double c = fmin(prm.tangential_damping, prm.friction_mu * fn / vt); fx = -c * vel[0]; fy = -c * vel[1]; }
+      w->fc[f][0] = fx; w->fc[f][1] = fy; w->fc[f][2] = fn;
+      w->pf[f][0] = pw[0]; w->pf[f][1] = pw[1]; w->pf[f][2] = pw[2];
+    }
+    const unsigned bal = __ballot_sync(FULL, lane < 4 && fn > 0.0);
+    in_contact = ((bal & 1u) << 3) | ((bal & 2u) << 1) | ((bal & 4u) >> 1) | ((bal & 8u) >> 3);   // foot f → bit 3 - f (LF=8 RF=4 LH=2 RH=1)
+    __syncwarp();
+    for (int f = 0; f < 4; ++f) { const int j = mdl->foot_body[f] - 1; point_jacobian(ws, w->pf[f], mdl->chain_start[j], j, w->M + 3 * f * NQ, NQ, lane); }
+    __syncwarp();
+    if (lane < NQ) {
+      double g = tau - jdamp * w->v[lane] - w->nle[lane];
+#pragma unroll
+      for (int f = 0; f < 4; ++f) g += w->M[(3 * f) * NQ + lane] * w->fc[f][0] + w->M[(3 * f + 1) * NQ + lane] * w->fc[f][1] + w->M[(3 * f + 2) * NQ + lane] * w->fc[f][2];
+      w->Q[lane] = g;
+    }
+    __syncwarp();
+    if (!w_cholesky(w->L, NQ, lane)) { st |= QMB200_ST_NOT_PD; break; }
+    w_chol_solve(w->L, NQ, w->Q, lane);
+    if (lane < NQ) { const double vn = w->v[lane] + h * w->Q[lane]; w->v[lane] = vn; w->q[lane] += h * vn; }
+    __syncwarp();
+  }
+  const bool bad = lane < NQ && !(isfinite(w->q[lane]) && isfinite(w->v[lane]));
+  if (__any_sync(FULL, bad)) st |= QMB200_ST_NAN;
+  rbd_kinematics<false>(mdl, w->q, w->v, ws, lane);
+  double* r = rbd + (size_t)b * QMB200_RBD;
+  if (lane < NQ) {
+    q_io[(size_t)b * NQ + lane] = w->q[lane]; v_io[(size_t)b * NQ + lane] = w->v[lane];
+    r[lane < 3 ? lane + 3 : (lane < 6 ? lane - 3 : lane)] = w->q[lane];                 // [euler ZYX, pos, joints]
+    if (lane < 3) r[NQ + 3 + lane] = w->v[lane]; else if (lane >= 6) r[NQ + lane] = w->v[lane];   // v_lin, joint velocities
+  }
+  if (lane == 0) {
+    double T[9]; euler_rate_map_sc(ws->trig, T); const double ed[3] = {w->v[3], w->v[4], w->v[5]}; double om[3]; matvec3(T, ed, om);
+    r[NQ] = om[0]; r[NQ + 1] = om[1]; r[NQ + 2] = om[2];                                  // w_world = T(zyx) zyx_rates
+    const int eb = mdl->ee_body; double Rb[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) Rb[i] = ws->R[eb][i];
+    double pe[3]; matvec3(Rb, mdl->ee_p, pe); double Re[9]; matmul3(Rb, mdl->ee_R, Re);
+    r[48] = pe[0] + ws->p[eb][0]; r[49] = pe[1] + ws->p[eb][1]; r[50] = pe[2] + ws->p[eb][2];
+    rot_to_quat_xyzw(Re, r + 51);
+    contact[b] = (int32_t)in_contact; status[b] = st;
+  }
+}
+
+int launch_sim_step(const DevModel* mdl, const SimParams& prm, int B, int substeps, double h, const double* effort, double* q, double* v, double* rbd, int32_t* contact,
+                    int32_t* status, cudaStream_t s) {
+  sim_step_kernel<<<(B + SIM_WARPS - 1) / SIM_WARPS, 32 * SIM_WARPS, 0, s>>>(mdl, prm, B, substeps, h, effort, q, v, rbd, contact, status);
+  return 1;
+}
+
+}  // namespace qmb

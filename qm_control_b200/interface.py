@@ -291,6 +291,54 @@ class Solver:
         self._chk(self.lib.qmb200_update(self.h, _p(_f64(rbd, (B, RBD))), _p(_f64(period, (B,))), _p(t), _p(x), _p(jc), _p(ap), _p(lt), _p(cmd), _p(st)), "qmb200_update")
         return t, x, jc, ap, lt, cmd, st
 
+    # device-pointer variants of the controller side (torch-cuda tensors, no synchronisation)
+    def target_trajectories_dev(self, kind, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, stream=None):
+        self._chk(self.lib.qmb200_target_trajectories_dev(self.h, int(kind), _p(cmd), _p(t_obs), _p(x_obs), _p(ee_state), _p(last_ee_target), _p(n_target), _p(target_times), _p(target_states),
+                                                          C.c_void_p(stream) if stream else None), "qmb200_target_trajectories_dev")
+
+    def update_dev(self, rbd, period, t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time, cmd, status, stream=None):
+        self._chk(self.lib.qmb200_update_dev(self.h, _p(rbd), _p(period), _p(t_obs), _p(x_obs), _p(joint_cmd), _p(arm_pos_cmd), _p(last_time), _p(cmd), _p(status), C.c_void_p(stream) if stream else None),
+                  "qmb200_update_dev")
+
+    def hw_write_dev(self, time, period, joint_cmd, joint_pos, joint_vel, effort, status, stream=None):
+        self._chk(self.lib.qmb200_hw_write_dev(self.h, _p(time), _p(period), _p(joint_cmd), _p(joint_pos), _p(joint_vel), _p(effort), _p(status), C.c_void_p(stream) if stream else None),
+                  "qmb200_hw_write_dev")
+
+    # ---------------- plant (include/qmb200.h: Gazebo's physics step behind QMHWSim + readSim's contact flags) ----------------
+    def sim_get_params(self):
+        """→ dict of qmb200_sim_params (joint_damping as a list of 18)."""
+        p = _lib.SimParams(); self._chk(self.lib.qmb200_sim_get_params(self.h, C.byref(p)), "qmb200_sim_get_params")
+        return {n: (list(getattr(p, n)) if n == "joint_damping" else getattr(p, n)) for n, _ in _lib.SimParams._fields_}
+
+    def sim_set_params(self, **params):
+        """Keyword per field of qmb200_sim_params; unspecified fields keep their value."""
+        p = _lib.SimParams(); self._chk(self.lib.qmb200_sim_get_params(self.h, C.byref(p)), "qmb200_sim_get_params")
+        for k, v in params.items():
+            if k == "joint_damping":
+                for i, x in enumerate(v):
+                    p.joint_damping[i] = float(x)
+            elif k == "substeps_per_ms":
+                p.substeps_per_ms = int(v)
+            else:
+                setattr(p, k, float(v))
+        self._chk(self.lib.qmb200_sim_set_params(self.h, C.byref(p)), "qmb200_sim_set_params")
+
+    def sim_step(self, duration, effort, q, v):
+        """One physics step of every robot (effort held for `duration` s) → (q, v, rbd[B,55], contact[B], status[B])."""
+        B = self.batch; q = _f64(q, (B, 24)).copy(); v = _f64(v, (B, 24)).copy(); rbd = np.zeros((B, RBD)); contact = np.zeros(B, dtype=np.int32); st = np.zeros(B, dtype=np.int32)
+        self._chk(self.lib.qmb200_sim_step(self.h, float(duration), _p(_f64(effort, (B, 18))), _p(q), _p(v), _p(rbd), _p(contact), _p(st)), "qmb200_sim_step")
+        return q, v, rbd, contact, st
+
+    def sim_step_dev(self, duration, effort, q, v, rbd, contact, status, stream=None):
+        """Device-pointer variant: q, v updated in place; no synchronisation."""
+        self._chk(self.lib.qmb200_sim_step_dev(self.h, float(duration), _p(effort), _p(q), _p(v), _p(rbd), _p(contact), _p(status), C.c_void_p(stream) if stream else None), "qmb200_sim_step_dev")
+
+    def sim_standing_state(self, xy_yaw):
+        """Nominal standing configuration at the given base (x, y, yaw) rows → (q[n,24], v[n,24])."""
+        xy = _f64(xy_yaw).reshape(-1, 3); n = xy.shape[0]; q = np.zeros((n, 24)); v = np.zeros((n, 24))
+        self._chk(self.lib.qmb200_sim_standing_state(self.h, n, _p(xy), _p(q), _p(v)), "qmb200_sim_standing_state")
+        return q, v
+
     # ---------------- utilities ----------------
     def centroidal_state_from_rbd(self, rbd):
         rbd = _f64(rbd); n = rbd.shape[0]; x = np.empty((n, NX))

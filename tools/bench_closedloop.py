@@ -1,0 +1,73 @@
+"""Closed-loop benchmark on one GPU (qm_control_b200.closed_loop): the controller at the reference's rates driving this library's plant step.
+
+Default: 8192 robots, trot at cmd_vel 0.3 m/s, 1 s simulated after a warm-up run of the same length.  Prints one JSON line with the wall time per
+simulated second, the plant step's device time per call (CUDA events) and its share of the loop, and quality lines (base distance, end-effector
+deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
+
+    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def card():
+    """GPU name and power limit as nvidia-smi reports them (read-only query); None where unavailable."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30).stdout.strip()
+        name, limit = [s.strip() for s in out.split(",")[:2]]
+        return name, limit
+    except Exception:
+        return None, None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
+    ap.add_argument("--gait", default="trot"); ap.add_argument("--vx", type=float, default=0.3)
+    args = ap.parse_args()
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch; sim_s = args.duration; cmd = (args.vx, 0.0, 0.0, 0.0)
+    solver = q.Solver(batch=B, device=0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)   # robots do not interact; spread for readability only
+    closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy)   # warm-up run of the same length
+    pairs = []
+
+    def sim_timer(start):
+        if start:
+            pairs.append([torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)]); pairs[-1][0].record()
+        else:
+            pairs[-1][1].record()
+    torch.cuda.synchronize(dev); t0 = time.perf_counter()
+    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer)
+    torch.cuda.synchronize(dev); wall = time.perf_counter() - t0
+    sim_ms = float(np.sum([a.elapsed_time(b) for a, b in pairs])); per_call = sim_ms / len(pairs)
+    dist = np.linalg.norm(r["base"][-1, :, :2] - r["start_base"][:, :2], axis=1)
+    dpos = np.max(np.linalg.norm(r["ee"][:, :, :3] - r["start_ee"][None, :, :3], axis=2), axis=0) * 1e3
+    dot = np.clip(np.abs(np.sum(r["ee"][:, :, 3:] * r["start_ee"][None, :, 3:], axis=2)), 0.0, 1.0); dang = np.max(np.degrees(2.0 * np.arccos(dot)), axis=0)
+    pct = lambda a: {"p50": float(np.percentile(a, 50)), "p95": float(np.percentile(a, 95)), "max": float(np.max(a))}
+    name, limit = card()
+    print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
+                      "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
+                      "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
+                      "quality": {"label": "this project's compliant-contact plant, not Gazebo/ODE: not comparable to README.md:116", "base_distance_m": pct(dist),
+                                  "ee_max_pos_dev_mm": pct(dpos), "ee_max_ori_dev_deg": pct(dang),
+                                  "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(r["status"], axis=0))),
+                                  "min_base_height_m": float(np.min(r["base"][:, :, 2])), "max_abs_roll_pitch_rad": float(np.max(np.abs(r["base"][:, :, 4:6])))},
+                      "config": {"workload": "closed loop: %s, cmd_vel %.2f m/s, MPC 100 Hz / WBC 500 Hz / plant 1 kHz (4 substeps), 9 ms command delay" % (args.gait, args.vx),
+                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length"}}))
+
+
+if __name__ == "__main__":
+    main()
