@@ -228,6 +228,26 @@ int qmb200_sim_set_params(qmb200_handle* h, const qmb200_sim_params* p);
 int qmb200_sim_step(qmb200_handle* h, double duration, const double* effort /*[B][18]*/, double* q /*[B][24] in-out*/, double* v /*[B][24] in-out*/,
                     double* rbd /*[B][55]*/, int32_t* contact /*[B]*/, int32_t* status /*[B]*/);
 int qmb200_sim_step_dev(qmb200_handle* h, double duration, const double* effort, double* q, double* v, double* rbd, int32_t* contact, int32_t* status, void* cuda_stream);
+/* Per-robot plant variation, kept in the handle and applied by every qmb200_sim_step(_ext)(_dev) call (plant properties, like qmb200_sim_params):
+ *   friction_mu[B]   the feet's Coulomb coefficient of robot b, in place of qmb200_sim_params.friction_mu
+ *   payload[B][8]    layout: [m_ee, o_ee_x, o_ee_y, o_ee_z, m_base, o_base_x, o_base_y, o_base_z]
+ *                    two point masses (kg) rigidly attached at o_ee (m, end-effector frame) and o_base (m, base frame); no rotational inertia.
+ * The controller (MPC model, WBC) is not told about the payload: the model mismatch is the experiment.  qmb200_sim_standing_state ignores the
+ * robot params, so a payload shifts the static pre-load of the standing state (by micrometres per kilogram at the default stiffness).
+ * Host arrays, copied to the device; synchronous (waits for the device).  NULL clears that override.  Rejects a non-finite or <= 0 friction_mu,
+ * a non-finite payload entry and a negative mass; on rejection the stored values stay unchanged. */
+int qmb200_sim_set_robot_params(qmb200_handle* h, const double* friction_mu /*[B] or NULL*/, const double* payload /*[B][8] or NULL*/);
+/* The stored values; where an override is not set: friction_mu = qmb200_sim_params.friction_mu, payload = 0.  set_mask: 1 = friction_mu, 2 = payload.
+ * Any output may be NULL. */
+int qmb200_sim_get_robot_params(const qmb200_handle* h, double* friction_mu /*[B]*/, double* payload /*[B][8]*/, int32_t* set_mask);
+/* qmb200_sim_step(_dev) plus external wrenches held over the whole step; wrench NULL = qmb200_sim_step(_dev).
+ *   wrench[B][12]    layout: [f_base_x, f_base_y, f_base_z, n_base_x, n_base_y, n_base_z, f_ee_x, f_ee_y, f_ee_z, n_ee_x, n_ee_y, n_ee_z]
+ *                    forces (N) and moments (N m) in the world frame; each moment is about its own frame's origin (the base origin q[0:3], the
+ *                    end-effector frame origin).  Not validated: a non-finite wrench shows as QMB200_ST_NAN. */
+int qmb200_sim_step_ext(qmb200_handle* h, double duration, const double* effort /*[B][18]*/, const double* wrench /*[B][12] or NULL*/, double* q /*[B][24] in-out*/,
+                        double* v /*[B][24] in-out*/, double* rbd /*[B][55]*/, int32_t* contact /*[B]*/, int32_t* status /*[B]*/);
+int qmb200_sim_step_ext_dev(qmb200_handle* h, double duration, const double* effort, const double* wrench, double* q, double* v, double* rbd, int32_t* contact,
+                            int32_t* status, void* cuda_stream);
 /* Host utility: the nominal standing configuration (defaultJointState, base at the given x, y, yaw, zero roll and pitch) with the base height at
  * which the four foot spheres carry m g / 4 each at the static penetration of the current params; v = 0. */
 int qmb200_sim_standing_state(const qmb200_handle* h, int32_t n, const double* xy_yaw /*[n][3]*/, double* q /*[n][24]*/, double* v /*[n][24]*/);

@@ -34,6 +34,11 @@ class SimParams(C.Structure):
                [("joint_damping", C.c_double * 18), ("substeps_per_ms", C.c_int32)]
 
 
+# per-robot plant variation (include/qmb200.h: qmb200_sim_set_robot_params, qmb200_sim_step_ext): the column layouts of payload[B][8] and wrench[B][12]
+PAYLOAD_LAYOUT = ("m_ee", "o_ee_x", "o_ee_y", "o_ee_z", "m_base", "o_base_x", "o_base_y", "o_base_z")
+WRENCH_LAYOUT = ("f_base_x", "f_base_y", "f_base_z", "n_base_x", "n_base_y", "n_base_z", "f_ee_x", "f_ee_y", "f_ee_z", "n_ee_x", "n_ee_y", "n_ee_z")
+
+
 # every symbol include/qmb200.h declares (checked by the CPU test-suite)
 SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_dims", "qmb200_get_model_info", "qmb200_get_joint_name",
            "qmb200_wbc_update", "qmb200_wbc_update_dev", "qmb200_wbc_set_input_last", "qmb200_wbc_get_input_last", "qmb200_wbc_get_gains", "qmb200_wbc_set_gains", "qmb200_wbc_get_diagnostics", "qmb200_wbc_set_iteration_caps",
@@ -44,7 +49,8 @@ SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_d
            "qmb200_observation_update", "qmb200_observation_update_dev", "qmb200_target_trajectories", "qmb200_target_trajectories_dev", "qmb200_initial_ee_target",
            "qmb200_control_law", "qmb200_control_law_dev", "qmb200_set_arm_gains", "qmb200_hw_write", "qmb200_hw_write_dev", "qmb200_hw_set_delay", "qmb200_update", "qmb200_update_dev",
            "qmb200_debug_model_blob", "qmb200_comm_get_unique_id", "qmb200_comm_init", "qmb200_comm_destroy", "qmb200_comm_info", "qmb200_allgather_torque", "qmb200_gait_bin_permutation", "qmb200_set_pipeline", "qmb200_set_profiling", "qmb200_collect_kernel_times", "qmb200_get_kernel_times", "qmb200_get_flow_kernel_time", "qmb200_measure_fp64_peak",
-           "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state"]
+           "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state",
+           "qmb200_sim_set_robot_params", "qmb200_sim_get_robot_params", "qmb200_sim_step_ext", "qmb200_sim_step_ext_dev"]
 
 _lib = None
 
@@ -74,6 +80,10 @@ def load_library():
     lib.qmb200_initial_ee_target.restype = None
     lib.qmb200_sim_step.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 6
     lib.qmb200_sim_step_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 7
+    lib.qmb200_sim_step_ext.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 7
+    lib.qmb200_sim_step_ext_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 8
+    lib.qmb200_sim_set_robot_params.argtypes = [C.c_void_p] * 3
+    lib.qmb200_sim_get_robot_params.argtypes = [C.c_void_p] * 4
     lib.qmb200_sim_standing_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.qmb200_gait_destroy.restype = None
     lib.qmb200_gait_destroy.argtypes = [C.c_void_p]

@@ -6,6 +6,9 @@ Per simulated millisecond (Gazebo's default physics step, 1 kHz):
   every WBC period (default 2 ms)                     update_dev: observation → evaluatePolicy → WBC → control law (QMController::update)
   every 1 ms                                          hw_write_dev (QMHWSim::writeSim, 9 ms command delay of qm_gazebo/config/default.yaml)
                                                       → sim_step_dev (physics step + QMHWSim::readSim's contact flags)
+Per-robot experiments (robustness sweeps): cmd_vel and gait may differ per robot, and the plant may vary per robot through the handle's robot
+params (floor friction, end-effector and base payloads: Solver.sim_set_robot_params) and external pushes held over whole plant steps.  The
+controller is not told about any of them.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -20,18 +23,54 @@ HW_DELAY = 0.009           # gazebo/delay (qm_gazebo/config/default.yaml:2)
 T_START = 10.0             # QMController::updateControlLaw drives the legs only once time > 10 s
 
 
-def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None):
+def _schedules(gait, B, t_start, t_obs0, t_end):
+    """Mode schedules of one gait name, or of a sequence of B names (tiled once per distinct name) → (event_times[B, EMAX], modes[B, EMAX+1], n_events[B])."""
+    names = [gait] * B if isinstance(gait, str) else list(gait)
+    if len(names) != B:
+        raise ValueError("closed_loop.run: gait must be one name or a sequence of %d names, got %d" % (B, len(names)))
+    tiles = {}
+    for name in dict.fromkeys(names):
+        ev, md, ne = gait_schedule(name, t_start, t_obs0, t_end) if name != "stance" else (np.zeros(EMAX), np.full(EMAX + 1, 15, dtype=np.int32), 0)
+        if ne >= EMAX:
+            raise ValueError("closed_loop.run: the %s schedule of %.2f s needs more than %d events" % (name, t_end - t_start, EMAX))
+        tiles[name] = (ev, md, ne)
+    return (np.array([tiles[n][0] for n in names]), np.array([tiles[n][1] for n in names], dtype=np.int32), np.array([tiles[n][2] for n in names], dtype=np.int32))
+
+
+def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
+        friction_mu=None, payload=None, pushes=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
-    gait: a gait.info template name ("stance", "trot", ...), started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the base frame, same for every
-    robot; xy_yaw: [B, 3] initial base x, y, yaw (default zeros), each robot starts in qmb200_sim_standing_state.
+    gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
+    base frame, (4,) for every robot or [B, 4]; xy_yaw: [B, 3] initial base x, y, yaw (default zeros), each robot starts in qmb200_sim_standing_state.
+    friction_mu: scalar or [B], payload: [B, 8] (_lib.PAYLOAD_LAYOUT): set as the handle's robot params for this run (None keeps the handle's own);
+    the previous robot params are restored when run returns.  pushes: (t_on[B], duration[B], wrench[B, 12]) with t_on in seconds after the start
+    and wrench in _lib.WRENCH_LAYOUT: robot b's wrench acts in every 1 ms plant step whose start lies in [t_on, t_on + duration).
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end)."""
+    if friction_mu is None and payload is None:
+        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes)
+    prev = solver.sim_get_robot_params()
+    solver.sim_set_robot_params(friction_mu=prev["friction_mu"] if friction_mu is None else friction_mu, payload=prev["payload"] if payload is None else payload)
+    try:
+        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes)
+    finally:
+        solver.sim_set_robot_params(**prev)
+
+
+def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
     assert MPC_PERIOD_MS % wbc_period_ms == 0, "the WBC period must divide the MPC period"
+    cmd_vel = np.asarray(cmd_vel, dtype=np.float64)
+    if cmd_vel.shape not in ((4,), (B, 4)):
+        raise ValueError("closed_loop.run: cmd_vel must have shape (4,) or (%d, 4), got %s" % (B, cmd_vel.shape))
+    if pushes is not None:
+        t_on, t_dur, wrench = (np.asarray(a, dtype=np.float64) for a in pushes)
+        if t_on.shape != (B,) or t_dur.shape != (B,) or wrench.shape != (B, 12):
+            raise ValueError("closed_loop.run: pushes must be (t_on[%d], duration[%d], wrench[%d, 12])" % (B, B, B))
     stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
     f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
     i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
@@ -40,9 +79,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
     q0, v0 = solver.sim_standing_state(xy)
     t_obs0 = t_start - wbc_period_ms * 1e-3   # observation clock of `starting`; the first update brings it to t_start, the plant's clock
-    ev, md, ne = gait_schedule(gait, t_start, t_obs0, t_start + duration + solver.time_horizon + 1.0) if gait != "stance" else (np.zeros(EMAX), np.full(EMAX + 1, 15, dtype=np.int32), 0)
-    if ne >= EMAX:
-        raise ValueError("closed_loop.run: the %s schedule of %.2f s needs more than %d events" % (gait, duration, EMAX))
+    ev, md, ne = _schedules(gait, B, t_start, t_obs0, t_start + duration + solver.time_horizon + 1.0)
     with torch.cuda.stream(stream):
         q = f64(q0); v = f64(v0); rbd = torch.zeros((B, RBD), dtype=torch.float64, device=dev)
         contact = torch.zeros(B, dtype=torch.int32, device=dev); sim_st = torch.zeros_like(contact); hw_st = torch.zeros_like(contact); ctl_st = torch.zeros_like(contact)
@@ -57,15 +94,19 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         t_obs = f64(np.full(B, t_obs0)); x_obs = f64(x_obs0)
         joint_cmd = torch.zeros((B, 18, 5), dtype=torch.float64, device=dev); arm_pos = torch.zeros((B, 6), dtype=torch.float64, device=dev); last_time = f64(np.full(B, t_obs0))
         cmd54 = torch.zeros((B, 54), dtype=torch.float64, device=dev)
-        cmd7 = torch.zeros((B, 7), dtype=torch.float64, device=dev); cmd7[:, :4] = f64(np.asarray(cmd_vel, dtype=np.float64)[None, :4])
+        cmd7 = torch.zeros((B, 7), dtype=torch.float64, device=dev); cmd7[:, :4] = f64(cmd_vel[None, :4] if cmd_vel.ndim == 1 else cmd_vel)
         last_ee = f64(solver.initial_ee_target()); ee_state = torch.zeros((B, 7), dtype=torch.float64, device=dev)
-        prob = dict(t0=t_obs, x0=x_obs, n_events=i32(np.full(B, ne)), event_times=f64(np.tile(ev, (B, 1))), modes=i32(np.tile(md, (B, 1))),
+        prob = dict(t0=t_obs, x0=x_obs, n_events=i32(ne), event_times=f64(ev), modes=i32(md),
                     n_target=torch.zeros(B, dtype=torch.int32, device=dev), target_times=torch.zeros((B, KMAX), dtype=torch.float64, device=dev),
                     target_states=torch.zeros((B, KMAX, TARGET), dtype=torch.float64, device=dev))
         period = f64(np.full(B, wbc_period_ms * 1e-3)); hw_period = f64(np.full(B, 1e-3)); hw_time = torch.zeros(B, dtype=torch.float64, device=dev)
         ticks = n_ms // MPC_PERIOD_MS
         rec_base = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev); rec_ee = torch.zeros((ticks, B, 7), dtype=torch.float64, device=dev)
         rec_st = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
+        push = None
+        if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
+            push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench), zero=torch.zeros((B, 12), dtype=torch.float64, device=dev),
+                        now=torch.zeros((B, 12), dtype=torch.float64, device=dev))
     stream.synchronize()
     solver.hw_set_delay(HW_DELAY)
 
@@ -86,7 +127,9 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             solver.hw_write_dev(hw_time, hw_period, joint_cmd, jpos, jvel, effort, hw_st, s)
             if sim_timer:
                 sim_timer(True)
-            solver.sim_step_dev(1e-3, effort, q, v, rbd, contact, sim_st, s)
+            if push is not None:
+                torch.where(((push["on"] <= k) & (push["off"] > k))[:, None], push["wrench"], push["zero"], out=push["now"])
+            solver.sim_step_dev(1e-3, effort, q, v, rbd, contact, sim_st, s, wrench=None if push is None else push["now"])
             if sim_timer:
                 sim_timer(False)
             acc_st.bitwise_or_(hw_st).bitwise_or_(sim_st)

@@ -50,6 +50,7 @@ struct qmb200_handle {
   double hw_delay = 0.0; double *hw_ring_cmd = nullptr, *hw_ring_stamp = nullptr; int32_t* hw_ring_state = nullptr;   // QMHWSim command-delay FIFO
   void* comm = nullptr; int comm_ranks = 0, comm_rank = 0; double* d_send = nullptr;   // NCCL communicator of this handle (capi_comm.inc) and the packed torque rows
   SimParams sim_prm{}; double *s_effort = nullptr, *s_q = nullptr, *s_v = nullptr, *s_rbd = nullptr; int32_t *s_contact = nullptr, *s_status = nullptr;   // plant step (capi_sim.inc)
+  std::vector<double> r_mu, r_payload; double *s_mu = nullptr, *s_payload = nullptr, *s_wrench = nullptr;   // per-robot plant variation: host copy (empty = not set), device copy
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
 

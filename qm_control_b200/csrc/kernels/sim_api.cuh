@@ -19,7 +19,8 @@ struct SimParams {
   int substeps_per_ms;         // semi-implicit Euler steps per millisecond of simulated time
 };
 
+// mu [B], payload [B][8], wrench [B][12]: optional per-robot plant variation (NULL = not used; sim_kernel.cu has the layouts)
 int launch_sim_step(const DevModel* mdl, const SimParams& prm, int B, int substeps, double h, const double* effort, double* q, double* v, double* rbd, int32_t* contact,
-                    int32_t* status, cudaStream_t s);
+                    int32_t* status, const double* mu, const double* payload, const double* wrench, cudaStream_t s);
 
 }  // namespace qmb

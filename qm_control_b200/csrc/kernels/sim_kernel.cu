@@ -12,6 +12,15 @@
 //   solve                  M qddot = Q by the warp Cholesky (wlinalg.cuh); v += h qddot; q += h v
 // After the last substep one kinematics-only pass at the final q gives the measured state rbd[55] (include/qmb200.h layout) with the
 // end-effector pose as qm_estimation fills it from ground truth.
+//
+// Per-robot plant variation (each input optional: a NULL pointer is the same for the whole grid, so there is one code path):
+//   mu[B]            the feet's Coulomb coefficient in place of prm.friction_mu
+//   payload[B][8]    [m_ee, o_ee(3), m_base, o_base(3)]: point masses rigidly attached at o_ee (end-effector frame) and o_base (base frame).
+//                    After rbd_inertias, lanes 0 / 1 add each one's spatial inertia about the world origin [m, m c, m(|c|^2 1 - c c^T)] to Ic and its
+//                    RNEA force I_p (A + g) + V x* I_p V to F of the body it is fixed to, so M and nle include it through the existing passes.
+//   wrench[B][12]    [f_base, n_base, f_ee, n_ee], world frame, each moment about its own frame's origin, held over the step: W = [n + p x f; f]
+//                    about the world origin, Q_c += S_c . W over the base columns (base wrench) and the base + arm chain columns (EE wrench).
+// A zero payload or wrench adds exact zeros and mu[b] == prm.friction_mu is the shared law, so neutral variation is bit-identical.
 #include "rbd.cuh"
 #include "sim_api.cuh"
 #include "wlinalg.cuh"
@@ -30,6 +39,7 @@ struct SimWs {
   double L[NTRI];      // packed lower triangle of M, then its Cholesky factor
   double fc[4][3];     // contact force of each foot (world)
   double pf[4][3];     // foot frame origin (world)
+  double W[2][6];      // external wrench [nO; f] about the world origin: [0] end effector, [1] base
 };
 
 // Eigen::Quaterniond(const Matrix3d&) (Shepperd's method, largest diagonal pivot); out = x, y, z, w
@@ -49,12 +59,43 @@ __device__ __forceinline__ void rot_to_quat_xyzw(const double* m, double* o) {
     o[3] = (m[7] - m[5]) * s; o[1] = (m[3] + m[1]) * s; o[2] = (m[6] + m[2]) * s;
   }
 }
+
+// Lane 0: the end-effector frame, lane 1: the base frame.  Adds the payload point mass to Ic / F of the frame's body and writes the wrench about
+// the world origin to w->W[lane] (sim_step_kernel's header has the layouts).
+__device__ __forceinline__ void frame_loads(const DevModel* __restrict__ mdl, SimWs* w, int lane, const double* __restrict__ payload, const double* __restrict__ wrench) {
+  RbdWs* ws = &w->rb; const int body = lane == 0 ? mdl->ee_body : 0;
+  double R[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) R[i] = ws->R[body][i];
+  double po[3] = {0.0, 0.0, 0.0}; if (lane == 0) matvec3(R, mdl->ee_p, po);
+  po[0] += ws->p[body][0]; po[1] += ws->p[body][1]; po[2] += ws->p[body][2];   // frame origin (world)
+  if (payload) {
+    const double m = payload[0]; const double ol[3] = {payload[1], payload[2], payload[3]}; double ob[3] = {ol[0], ol[1], ol[2]};
+    if (lane == 0) matvec3(mdl->ee_R, ol, ob);                                    // offset in the body's axes
+    double c[3]; matvec3(R, ob, c); c[0] += po[0]; c[1] += po[1]; c[2] += po[2];   // point mass position (world)
+    const double cc = dot3(c, c);
+    double I[10] = {m, m * c[0], m * c[1], m * c[2], m * (cc - c[0] * c[0]), -m * c[0] * c[1], -m * c[0] * c[2], m * (cc - c[1] * c[1]), -m * c[1] * c[2], m * (cc - c[2] * c[2])};
+    double acc[6]; for (int i = 0; i < 6; ++i) acc[i] = ws->A[body][i]; acc[5] += 9.81;
+    double f1[6], mom[6]; inertia_apply(I, acc, f1); inertia_apply(I, ws->V[body], mom);
+    const double* wv = ws->V[body]; const double* vv = ws->V[body] + 3;
+    double t1[3], t2[3]; cross3(wv, mom, t1); cross3_add(vv, mom + 3, t1); cross3(wv, mom + 3, t2);   // V x* [n; f] = [w x n + v x f; w x f]
+    double* Ic = ws->Ic[body]; double* F = ws->F[body];
+#pragma unroll
+    for (int i = 0; i < 10; ++i) Ic[i] += I[i];
+    F[0] += f1[0] + t1[0]; F[1] += f1[1] + t1[1]; F[2] += f1[2] + t1[2]; F[3] += f1[3] + t2[0]; F[4] += f1[4] + t2[1]; F[5] += f1[5] + t2[2];
+  }
+  if (wrench) {
+    const double f[3] = {wrench[0], wrench[1], wrench[2]}; double* W = w->W[lane];
+    cross3(po, f, W); W[0] += wrench[3]; W[1] += wrench[4]; W[2] += wrench[5]; W[3] = f[0]; W[4] = f[1]; W[5] = f[2];
+  }
+}
 }  // namespace
 
 __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel* __restrict__ mdl, SimParams prm, int B, int substeps, double h,
                                                                   const double* __restrict__ effort /*[B][18]*/, double* __restrict__ q_io /*[B][24]*/,
                                                                   double* __restrict__ v_io /*[B][24]*/, double* __restrict__ rbd /*[B][55]*/,
-                                                                  int32_t* __restrict__ contact, int32_t* __restrict__ status) {
+                                                                  int32_t* __restrict__ contact, int32_t* __restrict__ status, const double* __restrict__ mu_b /*[B] or NULL*/,
+                                                                  const double* __restrict__ payload /*[B][8] or NULL*/, const double* __restrict__ wrench /*[B][12] or NULL*/) {
   __shared__ SimWs s_ws[SIM_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * SIM_WARPS + warp;
   if (b >= B) return;   // the whole warp leaves together
@@ -65,11 +106,20 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
     const int j = lane - 6; const double lim = mdl->effort[j];
     tau = fmin(fmax(effort[(size_t)b * NJ + j], -lim), lim); jdamp = prm.joint_damping[j];
   }
+  const double mu = mu_b ? mu_b[b] : prm.friction_mu;
+  const double* pl = payload && lane < 2 ? payload + (size_t)b * 8 + 4 * lane : nullptr;      // lane 0: [m_ee, o_ee], lane 1: [m_base, o_base]
+  const double* wr = wrench && lane < 2 ? wrench + (size_t)b * 12 + 6 * (1 - lane) : nullptr;  // lane 0: [f_ee, n_ee], lane 1: [f_base, n_base]
+  const int je = mdl->ee_body - 1;
+  const bool ee_col = lane < 6 || (lane - 6 >= mdl->chain_start[je] && lane - 6 <= je);   // columns of the EE's point_jacobian
   __syncwarp();
   int st = 0; unsigned in_contact = 0;
   for (int k = 0; k < substeps; ++k) {
     rbd_kinematics<true>(mdl, w->q, w->v, ws, lane);
     rbd_inertias(mdl, ws, lane, 1);
+    if (payload || wrench) {
+      if (lane < 2) frame_loads(mdl, w, lane, pl, wr);
+      __syncwarp();
+    }
     rbd_accumulate(mdl, ws, lane, true);
     rbd_mass_matrix_nle(mdl, ws, w->M, NQ, w->nle, lane);
     if (lane < NQ) { const double* row = w->M + lane * NQ; double* out = w->L + tri(lane); for (int c = 0; c <= lane; ++c) out[c] = row[c]; }
@@ -81,7 +131,7 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
       const double pen = prm.ground_height - (pw[2] - prm.foot_radius);
       if (pen > 0.0) fn = fmax(0.0, prm.stiffness * pen - prm.damping * vel[2]);
       double fx = 0.0, fy = 0.0; const double vt = sqrt(vel[0] * vel[0] + vel[1] * vel[1]);
-      if (fn > 0.0 && vt > 0.0) { const double c = fmin(prm.tangential_damping, prm.friction_mu * fn / vt); fx = -c * vel[0]; fy = -c * vel[1]; }
+      if (fn > 0.0 && vt > 0.0) { const double c = fmin(prm.tangential_damping, mu * fn / vt); fx = -c * vel[0]; fy = -c * vel[1]; }
       w->fc[f][0] = fx; w->fc[f][1] = fy; w->fc[f][2] = fn;
       w->pf[f][0] = pw[0]; w->pf[f][1] = pw[1]; w->pf[f][2] = pw[2];
     }
@@ -94,6 +144,10 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
       double g = tau - jdamp * w->v[lane] - w->nle[lane];
 #pragma unroll
       for (int f = 0; f < 4; ++f) g += w->M[(3 * f) * NQ + lane] * w->fc[f][0] + w->M[(3 * f + 1) * NQ + lane] * w->fc[f][1] + w->M[(3 * f + 2) * NQ + lane] * w->fc[f][2];
+      if (wrench) {
+        if (lane < 6) g += dot6(ws->S[lane], w->W[1]);
+        if (ee_col) g += dot6(ws->S[lane], w->W[0]);
+      }
       w->Q[lane] = g;
     }
     __syncwarp();
@@ -125,8 +179,8 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
 }
 
 int launch_sim_step(const DevModel* mdl, const SimParams& prm, int B, int substeps, double h, const double* effort, double* q, double* v, double* rbd, int32_t* contact,
-                    int32_t* status, cudaStream_t s) {
-  sim_step_kernel<<<(B + SIM_WARPS - 1) / SIM_WARPS, 32 * SIM_WARPS, 0, s>>>(mdl, prm, B, substeps, h, effort, q, v, rbd, contact, status);
+                    int32_t* status, const double* mu, const double* payload, const double* wrench, cudaStream_t s) {
+  sim_step_kernel<<<(B + SIM_WARPS - 1) / SIM_WARPS, 32 * SIM_WARPS, 0, s>>>(mdl, prm, B, substeps, h, effort, q, v, rbd, contact, status, mu, payload, wrench);
   return 1;
 }
 

@@ -323,15 +323,38 @@ class Solver:
                 setattr(p, k, float(v))
         self._chk(self.lib.qmb200_sim_set_params(self.h, C.byref(p)), "qmb200_sim_set_params")
 
-    def sim_step(self, duration, effort, q, v):
-        """One physics step of every robot (effort held for `duration` s) → (q, v, rbd[B,55], contact[B], status[B])."""
+    def sim_step(self, duration, effort, q, v, wrench=None):
+        """One physics step of every robot (effort held for `duration` s) → (q, v, rbd[B,55], contact[B], status[B]).
+        wrench: optional [B, 12] external wrenches held over the step (layout _lib.WRENCH_LAYOUT, include/qmb200.h: qmb200_sim_step_ext)."""
         B = self.batch; q = _f64(q, (B, 24)).copy(); v = _f64(v, (B, 24)).copy(); rbd = np.zeros((B, RBD)); contact = np.zeros(B, dtype=np.int32); st = np.zeros(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_sim_step(self.h, float(duration), _p(_f64(effort, (B, 18))), _p(q), _p(v), _p(rbd), _p(contact), _p(st)), "qmb200_sim_step")
+        if wrench is None:
+            self._chk(self.lib.qmb200_sim_step(self.h, float(duration), _p(_f64(effort, (B, 18))), _p(q), _p(v), _p(rbd), _p(contact), _p(st)), "qmb200_sim_step")
+        else:
+            self._chk(self.lib.qmb200_sim_step_ext(self.h, float(duration), _p(_f64(effort, (B, 18))), _p(_f64(wrench, (B, 12))), _p(q), _p(v), _p(rbd), _p(contact), _p(st)),
+                      "qmb200_sim_step_ext")
         return q, v, rbd, contact, st
 
-    def sim_step_dev(self, duration, effort, q, v, rbd, contact, status, stream=None):
-        """Device-pointer variant: q, v updated in place; no synchronisation."""
-        self._chk(self.lib.qmb200_sim_step_dev(self.h, float(duration), _p(effort), _p(q), _p(v), _p(rbd), _p(contact), _p(status), C.c_void_p(stream) if stream else None), "qmb200_sim_step_dev")
+    def sim_step_dev(self, duration, effort, q, v, rbd, contact, status, stream=None, wrench=None):
+        """Device-pointer variant: q, v updated in place; no synchronisation.  wrench: optional [B, 12] device tensor."""
+        if wrench is None:
+            self._chk(self.lib.qmb200_sim_step_dev(self.h, float(duration), _p(effort), _p(q), _p(v), _p(rbd), _p(contact), _p(status), C.c_void_p(stream) if stream else None), "qmb200_sim_step_dev")
+        else:
+            self._chk(self.lib.qmb200_sim_step_ext_dev(self.h, float(duration), _p(effort), _p(wrench), _p(q), _p(v), _p(rbd), _p(contact), _p(status), C.c_void_p(stream) if stream else None),
+                      "qmb200_sim_step_ext_dev")
+
+    def sim_set_robot_params(self, friction_mu=None, payload=None):
+        """Per-robot plant variation kept in the handle: friction_mu [B] (a scalar is broadcast), payload [B, 8] (layout _lib.PAYLOAD_LAYOUT).
+        None clears that override.  The controller does not know about the payload.  Synchronous."""
+        B = self.batch
+        mu = None if friction_mu is None else _f64(np.broadcast_to(np.asarray(friction_mu, dtype=np.float64), (B,)), (B,))
+        pl = None if payload is None else _f64(payload, (B, 8))
+        self._chk(self.lib.qmb200_sim_set_robot_params(self.h, _p(mu), _p(pl)), "qmb200_sim_set_robot_params")
+
+    def sim_get_robot_params(self):
+        """→ dict(friction_mu [B] or None, payload [B, 8] or None): None where that override is not set."""
+        B = self.batch; mu = np.zeros(B); pl = np.zeros((B, 8)); mask = C.c_int32()
+        self._chk(self.lib.qmb200_sim_get_robot_params(self.h, _p(mu), _p(pl), C.byref(mask)), "qmb200_sim_get_robot_params")
+        return dict(friction_mu=mu if mask.value & 1 else None, payload=pl if mask.value & 2 else None)
 
     def sim_standing_state(self, xy_yaw):
         """Nominal standing configuration at the given base (x, y, yaw) rows → (q[n,24], v[n,24])."""

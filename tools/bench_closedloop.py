@@ -4,7 +4,12 @@ Default: 8192 robots, trot at cmd_vel 0.3 m/s, 1 s simulated after a warm-up run
 simulated second, the plant step's device time per call (CUDA events) and its share of the loop, and quality lines (base distance, end-effector
 deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
 
-    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
+    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary]
+
+--vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
+mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
+gains "vary": the quality per condition bin of each axis (fallen robots, base distance, end-effector deviation).  The controller is not told about
+any of it.
 """
 import argparse
 import json
@@ -32,6 +37,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
     ap.add_argument("--gait", default="trot"); ap.add_argument("--vx", type=float, default=0.3)
+    ap.add_argument("--vary", action="store_true", help="per-robot sweep of EE payload, floor friction and a lateral base push")
     args = ap.parse_args()
     import torch
     import qm_control_b200 as q
@@ -41,7 +47,14 @@ def main():
     dev = torch.device("cuda", 0); B = args.batch; sim_s = args.duration; cmd = (args.vx, 0.0, 0.0, 0.0)
     solver = q.Solver(batch=B, device=0)
     xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)   # robots do not interact; spread for readability only
-    closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy)   # warm-up run of the same length
+    kw = {}
+    if args.vary:
+        b = np.arange(B); bins = dict(payload_kg=np.linspace(0.0, 2.0, 5), mu=np.linspace(0.15, 1.0, 5), push_N=np.array([0.0, 60.0, 120.0, 180.0]))
+        idx = dict(payload_kg=b % 5, mu=(b // 5) % 5, push_N=(b // 25) % 4)
+        pl = np.zeros((B, 8)); pl[:, 0] = bins["payload_kg"][idx["payload_kg"]]
+        w = np.zeros((B, 12)); w[:, 1] = bins["push_N"][idx["push_N"]]
+        kw = dict(payload=pl, friction_mu=bins["mu"][idx["mu"]], pushes=(np.full(B, 0.4), np.full(B, 0.1), w))
+    closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw)   # warm-up run of the same length
     pairs = []
 
     def sim_timer(start):
@@ -50,7 +63,7 @@ def main():
         else:
             pairs[-1][1].record()
     torch.cuda.synchronize(dev); t0 = time.perf_counter()
-    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer)
+    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer, **kw)
     torch.cuda.synchronize(dev); wall = time.perf_counter() - t0
     sim_ms = float(np.sum([a.elapsed_time(b) for a, b in pairs])); per_call = sim_ms / len(pairs)
     dist = np.linalg.norm(r["base"][-1, :, :2] - r["start_base"][:, :2], axis=1)
@@ -58,6 +71,15 @@ def main():
     dot = np.clip(np.abs(np.sum(r["ee"][:, :, 3:] * r["start_ee"][None, :, 3:], axis=2)), 0.0, 1.0); dang = np.max(np.degrees(2.0 * np.arccos(dot)), axis=0)
     pct = lambda a: {"p50": float(np.percentile(a, 50)), "p95": float(np.percentile(a, 95)), "max": float(np.max(a))}
     name, limit = card()
+    extra = {}
+    if args.vary:
+        base = r["base"]
+        fallen = ~(np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3))
+        extra["vary"] = {"label": "per-robot sweep; fallen = min base z <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite", "push": "lateral +y base force for 0.1 s from 0.4 s",
+                         "bins": {axis: [{"value": float(val), "robots": int(np.sum(idx[axis] == i)), "fallen": int(np.sum(fallen[idx[axis] == i])),
+                                          "base_distance_m_p50": float(np.percentile(dist[idx[axis] == i], 50)),
+                                          "ee_max_pos_dev_mm": pct(dpos[idx[axis] == i]), "ee_max_ori_dev_deg_p50": float(np.percentile(dang[idx[axis] == i], 50))}
+                                         for i, val in enumerate(bins[axis])] for axis in bins}}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
@@ -66,7 +88,7 @@ def main():
                                   "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(r["status"], axis=0))),
                                   "min_base_height_m": float(np.min(r["base"][:, :, 2])), "max_abs_roll_pitch_rad": float(np.max(np.abs(r["base"][:, :, 4:6])))},
                       "config": {"workload": "closed loop: %s, cmd_vel %.2f m/s, MPC 100 Hz / WBC 500 Hz / plant 1 kHz (4 substeps), 9 ms command delay" % (args.gait, args.vx),
-                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length"}}))
+                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length"}, **extra}))
 
 
 if __name__ == "__main__":
