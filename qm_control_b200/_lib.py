@@ -36,6 +36,9 @@ class SimParams(C.Structure):
 
 # per-robot plant variation (include/qmb200.h: qmb200_sim_set_robot_params, qmb200_sim_step_ext): the column layouts of payload[B][8] and wrench[B][12]
 PAYLOAD_LAYOUT = ("m_ee", "o_ee_x", "o_ee_y", "o_ee_z", "m_base", "o_base_x", "o_base_y", "o_base_z")
+# the controller's model payload (qmb200_set_model_payload) has PAYLOAD_LAYOUT too; per robot it yields SRBD_LAYOUT (qmb200_debug_srbd_constants)
+SRBD_LAYOUT = ("m",) + tuple("I_nom_%d%d" % (i, j) for i in range(3) for j in range(3)) + tuple("I_nom_inv_%d%d" % (i, j) for i in range(3) for j in range(3)) + \
+              ("c_nom_x", "c_nom_y", "c_nom_z", "pad0", "pad1")
 WRENCH_LAYOUT = ("f_base_x", "f_base_y", "f_base_z", "n_base_x", "n_base_y", "n_base_z", "f_ee_x", "f_ee_y", "f_ee_z", "n_ee_x", "n_ee_y", "n_ee_z")
 
 
@@ -50,7 +53,8 @@ SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_d
            "qmb200_control_law", "qmb200_control_law_dev", "qmb200_set_arm_gains", "qmb200_hw_write", "qmb200_hw_write_dev", "qmb200_hw_set_delay", "qmb200_update", "qmb200_update_dev",
            "qmb200_debug_model_blob", "qmb200_comm_get_unique_id", "qmb200_comm_init", "qmb200_comm_destroy", "qmb200_comm_info", "qmb200_allgather_torque", "qmb200_gait_bin_permutation", "qmb200_set_pipeline", "qmb200_set_profiling", "qmb200_collect_kernel_times", "qmb200_get_kernel_times", "qmb200_get_flow_kernel_time", "qmb200_measure_fp64_peak",
            "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state",
-           "qmb200_sim_set_robot_params", "qmb200_sim_get_robot_params", "qmb200_sim_step_ext", "qmb200_sim_step_ext_dev"]
+           "qmb200_sim_set_robot_params", "qmb200_sim_get_robot_params", "qmb200_sim_step_ext", "qmb200_sim_step_ext_dev",
+           "qmb200_set_model_payload", "qmb200_get_model_payload", "qmb200_debug_srbd_constants"]
 
 _lib = None
 
@@ -84,6 +88,9 @@ def load_library():
     lib.qmb200_sim_step_ext_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 8
     lib.qmb200_sim_set_robot_params.argtypes = [C.c_void_p] * 3
     lib.qmb200_sim_get_robot_params.argtypes = [C.c_void_p] * 4
+    lib.qmb200_set_model_payload.argtypes = [C.c_void_p] * 2
+    lib.qmb200_get_model_payload.argtypes = [C.c_void_p] * 3
+    lib.qmb200_debug_srbd_constants.argtypes = [C.POINTER(Config), C.c_int32, C.c_void_p, C.c_void_p]
     lib.qmb200_sim_standing_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.qmb200_gait_destroy.restype = None
     lib.qmb200_gait_destroy.argtypes = [C.c_void_p]

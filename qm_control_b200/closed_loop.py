@@ -8,7 +8,7 @@ Per simulated millisecond (Gazebo's default physics step, 1 kHz):
                                                       → sim_step_dev (physics step + QMHWSim::readSim's contact flags)
 Per-robot experiments (robustness sweeps): cmd_vel and gait may differ per robot, and the plant may vary per robot through the handle's robot
 params (floor friction, end-effector and base payloads: Solver.sim_set_robot_params) and external pushes held over whole plant steps.  The
-controller is not told about any of them.
+controller is not told about any of them unless the run sets its model payload (Solver.set_model_payload), e.g. to the plant's payload.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -38,7 +38,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
-        friction_mu=None, payload=None, pushes=None):
+        friction_mu=None, payload=None, pushes=None, model_payload=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -46,9 +46,23 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     friction_mu: scalar or [B], payload: [B, 8] (_lib.PAYLOAD_LAYOUT): set as the handle's robot params for this run (None keeps the handle's own);
     the previous robot params are restored when run returns.  pushes: (t_on[B], duration[B], wrench[B, 12]) with t_on in seconds after the start
     and wrench in _lib.WRENCH_LAYOUT: robot b's wrench acts in every 1 ms plant step whose start lies in [t_on, t_on + duration).
+    model_payload: the controller's model payload for this run (Solver.set_model_payload): None keeps the handle's own, "plant" copies this run's plant
+    payload (zeros where the plant carries none), or an array [B, 8]; the previous model payload is restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end)."""
+    if model_payload is not None:
+        prev_model = solver.get_model_payload()
+        try:
+            if isinstance(model_payload, str):
+                if model_payload != "plant":
+                    raise ValueError("closed_loop.run: model_payload must be None, \"plant\" or an array [%d, 8], got %r" % (solver.batch, model_payload))
+                plant = payload if payload is not None else solver.sim_get_robot_params()["payload"]
+                model_payload = np.zeros((solver.batch, 8)) if plant is None else plant
+            solver.set_model_payload(model_payload)
+            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes)
+        finally:
+            solver.set_model_payload(prev_model)
     if friction_mu is None and payload is None:
         return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes)
     prev = solver.sim_get_robot_params()

@@ -17,7 +17,8 @@
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
-                       double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0 = 0, int b1 = -1, int32_t* diag = nullptr);
+                       double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0 = 0, int b1 = -1, int32_t* diag = nullptr,
+                       const double* srbd = nullptr, const double* payload = nullptr);   // srbd [B][SRBD_DBL] / payload [B][8]: the model payload (NULL: none)
 int wbc_configure_device();   // per-device kernel attributes (opt-in shared memory): wbc_kernel.cu / mpc_kernels.cu
 int mpc_configure_device();
 }
@@ -51,6 +52,10 @@ struct qmb200_handle {
   void* comm = nullptr; int comm_ranks = 0, comm_rank = 0; double* d_send = nullptr;   // NCCL communicator of this handle (capi_comm.inc) and the packed torque rows
   SimParams sim_prm{}; double *s_effort = nullptr, *s_q = nullptr, *s_v = nullptr, *s_rbd = nullptr; int32_t *s_contact = nullptr, *s_status = nullptr;   // plant step (capi_sim.inc)
   std::vector<double> r_mu, r_payload; double *s_mu = nullptr, *s_payload = nullptr, *s_wrench = nullptr;   // per-robot plant variation: host copy (empty = not set), device copy
+  // the controller's model payload (qmb200_set_model_payload): host copies of the payload rows and of the robots' SRBD constants (empty = not set), device copies
+  std::vector<double> m_payload, m_srbd; double *d_mpayload = nullptr, *d_srbd = nullptr;
+  const double* srbd_dev() const { return m_payload.empty() ? nullptr : d_srbd; }
+  const double* mpayload_dev() const { return m_payload.empty() ? nullptr : d_mpayload; }
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
 
@@ -126,6 +131,55 @@ int64_t qmb200_debug_model_blob(const qmb200_config* cfg, void* out, int64_t cap
   } catch (const std::exception& e) { g_create_error = e.what(); return -2; }
 }
 
+// ------------------------------------------------------------------ model payload
+static_assert(SRBD_DBL == QMB200_SRBD, "per-robot SRBD block of include/qmb200.h");
+}  // extern "C"
+namespace {
+// payload rows [n][8] as qmb200_sim_set_robot_params accepts them: finite, masses >= 0; "" when valid
+std::string payload_error(const double* payload, size_t n, const char* who) {
+  for (size_t b = 0; b < n; ++b) {
+    const double* p = payload + 8 * b;
+    for (int i = 0; i < 8; ++i) if (!std::isfinite(p[i])) return std::string(who) + ": payload must be finite";
+    if (p[0] < 0.0 || p[4] < 0.0) return std::string(who) + ": payload masses must be >= 0";
+  }
+  return "";
+}
+// SRBD constants of n robots with payload rows [n][8] (NULL: none)
+void srbd_rows(const HostModel& hm, const double* payload, size_t n, double* out) {
+  for (size_t b = 0; b < n; ++b) srbd_constants(hm.dev, hm.default_joint_state, payload ? payload + 8 * b : nullptr, out + SRBD_DBL * b);
+}
+}  // namespace
+extern "C" {
+
+int qmb200_set_model_payload(qmb200_handle* h, const double* payload) {
+  if (!h) return -1; const size_t B = (size_t)h->B;
+  if (payload) { const std::string e = payload_error(payload, B, "qmb200_set_model_payload"); if (!e.empty()) return fail(h, e); }
+  std::vector<double> srbd; if (payload) { srbd.resize(B * SRBD_DBL); srbd_rows(h->hm, payload, B, srbd.data()); }
+  QMB_CUDA(h, cudaSetDevice(h->device));
+  if (payload && !h->d_srbd && !(dalloc(h, &h->d_srbd, B * SRBD_DBL) && dalloc(h, &h->d_mpayload, B * 8))) return -4;
+  // work still queued on any stream may read the current arrays: the copy waits for the device
+  QMB_CUDA(h, cudaDeviceSynchronize());
+  if (payload) { QMB_CUDA(h, cudaMemcpy(h->d_srbd, srbd.data(), B * SRBD_DBL * 8, cudaMemcpyHostToDevice)); QMB_CUDA(h, cudaMemcpy(h->d_mpayload, payload, B * 64, cudaMemcpyHostToDevice)); }
+  if (payload) { h->m_payload.assign(payload, payload + B * 8); h->m_srbd.swap(srbd); } else { h->m_payload.clear(); h->m_srbd.clear(); }
+  return 0;
+}
+int qmb200_get_model_payload(const qmb200_handle* h, double* payload, int32_t* is_set) {
+  if (!h) return -1; const size_t B = (size_t)h->B;
+  if (payload) { if (h->m_payload.empty()) std::memset(payload, 0, B * 64); else std::memcpy(payload, h->m_payload.data(), B * 64); }
+  if (is_set) *is_set = h->m_payload.empty() ? 0 : 1;
+  return 0;
+}
+int qmb200_debug_srbd_constants(const qmb200_config* cfg, int32_t n, const double* payload, double* out) {
+  if (!cfg || !cfg->task_file || !cfg->urdf_file || !cfg->reference_file) { g_create_error = "qmb200_debug_srbd_constants: task/urdf/reference file required"; return -1; }
+  if (n < 0 || (n > 0 && !out)) { g_create_error = "qmb200_debug_srbd_constants: n must be >= 0 and out non-null"; return -1; }
+  if (payload) { const std::string e = payload_error(payload, (size_t)n, "qmb200_debug_srbd_constants"); if (!e.empty()) { g_create_error = e; return -1; } }
+  try {
+    HostModel hm = build_host_model(cfg->task_file, cfg->urdf_file, cfg->reference_file, cfg->wbc_gains_file ? cfg->wbc_gains_file : "");
+    srbd_rows(hm, payload, (size_t)n, out);
+    return 0;
+  } catch (const std::exception& e) { g_create_error = e.what(); return -2; }
+}
+
 int qmb200_get_dims(const qmb200_handle* h, int32_t* batch, int32_t* nmax, int32_t* emax, int32_t* kmax) {
   if (!h) return -1; if (batch) *batch = h->B; if (nmax) *nmax = h->nmax; if (emax) *emax = QMB200_EMAX; if (kmax) *kmax = QMB200_KMAX; return 0;
 }
@@ -147,7 +201,8 @@ int qmb200_wbc_update_dev(qmb200_handle* h, const double* x_des, const double* u
                           double* cmd, int32_t* status, void* cuda_stream) {
   if (!h) return -1; if (!x_des || !u_des || !rbd || !mode || !period || !time || !cmd || !status) return fail(h, "qmb200_wbc_update_dev: null buffer");
   QMB_CUDA(h, cudaSetDevice(h->device));
-  launch_wbc_update(h->d_model, h->B, x_des, u_des, rbd, mode, period, time, h->d_input_last, h->variant, cmd, status, cuda_stream ? (cudaStream_t)cuda_stream : h->stream, 0, -1, h->d_wbc_diag);
+  launch_wbc_update(h->d_model, h->B, x_des, u_des, rbd, mode, period, time, h->d_input_last, h->variant, cmd, status, cuda_stream ? (cudaStream_t)cuda_stream : h->stream, 0, -1, h->d_wbc_diag,
+                    h->srbd_dev(), h->mpayload_dev());
   h->launches += 1;
   QMB_CUDA(h, cudaGetLastError());
   return 0;

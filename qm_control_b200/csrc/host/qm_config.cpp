@@ -164,7 +164,33 @@ int axis_index(const double* a, const std::string& name) {
   if (a[0] == 1 && a[1] == 0 && a[2] == 0) return 0; if (a[0] == 0 && a[1] == 1 && a[2] == 0) return 1; if (a[0] == 0 && a[1] == 0 && a[2] == 1) return 2;
   throw std::runtime_error("URDF: joint " + name + " has an axis other than +x/+y/+z (unsupported)");
 }
+// world rotation / origin of every body at q [24]
+void host_fk(const DevModel& d, const double* q, Rot* Rw, double (*pw)[3]) {
+  const double rz[3] = {q[5], q[4], q[3]}; Rw[0] = from_rpy(rz); for (int i = 0; i < 3; ++i) pw[0][i] = q[i];   // Rz(q3) Ry(q4) Rx(q5)
+  for (int j = 0; j < NJ; ++j) { const int pb = d.parent[j]; Rot Rl; std::memcpy(Rl.m, d.Rj[j], sizeof(Rl.m)); Rw[j + 1] = mul(mul(Rw[pb], Rl), about_axis(d.axis[j], q[6 + j])); apply(Rw[pb], d.pj[j], pw[j + 1]); for (int i = 0; i < 3; ++i) pw[j + 1][i] += pw[pb][i]; }
+}
 }  // namespace
+
+void srbd_constants(const DevModel& d, const double* default_joint_state, const double* payload, double* out) {
+  Rot Rw[NB]; double pw[NB][3];
+  double qn[NQ] = {0}; for (int j = 0; j < NJ; ++j) qn[6 + j] = default_joint_state[j]; host_fk(d, qn, Rw, pw);
+  Lump whole; for (int b = 0; b < NB; ++b) { double c[3]; apply(Rw[b], d.com[b], c); for (int i = 0; i < 3; ++i) c[i] += pw[b][i]; Rot I0; std::memcpy(I0.m, d.Ib[b], sizeof(I0.m)); Rot Iw = mul(mul(Rw[b], I0), transpose(Rw[b])); lump_add(whole, d.mass[b], c, Iw.m); }
+  double mass = d.total_mass;
+  for (int k = 0; payload && k < 2; ++k) {   // [m_ee, o_ee] at o_ee in the end-effector frame, [m_base, o_base] at o_base in the base frame
+    const double m = payload[4 * k]; if (m == 0.0) continue;   // a zero mass adds nothing, so the nominal constants stay bit-identical
+    const int body = k == 0 ? d.ee_body : 0; double cb[3] = {payload[4 * k + 1], payload[4 * k + 2], payload[4 * k + 3]};
+    if (k == 0) { Rot Re; std::memcpy(Re.m, d.ee_R, sizeof(Re.m)); double o[3]; apply(Re, cb, o); for (int i = 0; i < 3; ++i) cb[i] = o[i] + d.ee_p[i]; }
+    double c[3]; apply(Rw[body], cb, c); for (int i = 0; i < 3; ++i) c[i] += pw[body][i];
+    const double I0[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; lump_add(whole, m, c, I0); mass += m;
+  }
+  SrbdConst s; s.m = mass;
+  std::memcpy(s.I_nom, whole.I, sizeof(whole.I)); for (int i = 0; i < 3; ++i) s.c_nom[i] = -whole.c[i];
+  const double* m = s.I_nom; const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6]; const double id = 1.0 / (m[0] * c00 + m[1] * c01 + m[2] * c02);
+  double* o = s.I_nom_inv; o[0] = c00 * id; o[1] = (m[2] * m[7] - m[1] * m[8]) * id; o[2] = (m[1] * m[5] - m[2] * m[4]) * id; o[3] = c01 * id; o[4] = (m[0] * m[8] - m[2] * m[6]) * id; o[5] = (m[2] * m[3] - m[0] * m[5]) * id;
+  o[6] = c02 * id; o[7] = (m[1] * m[6] - m[0] * m[7]) * id; o[8] = (m[0] * m[4] - m[1] * m[3]) * id;
+  for (int i = 0; i < SRBD_DBL; ++i) out[i] = 0.0;
+  std::memcpy(out, &s, sizeof(s));
+}
 
 HostModel build_host_model(const std::string& task_file, const std::string& urdf_file, const std::string& reference_file, const std::string& gains_file) {
   InfoFile task(task_file); UrdfRobot urdf = read_urdf(urdf_file); InfoFile reference(reference_file);
@@ -219,17 +245,8 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
 
   // --- CentroidalModelInfo, SRBD (createCentroidalModelInfo [upstream]) ---
   { auto djs = reference.matrix("defaultJointState", NJ, 1); for (int i = 0; i < NJ; ++i) hm.default_joint_state[i] = djs[i]; }
+  { double s[SRBD_DBL]; srbd_constants(d, hm.default_joint_state, nullptr, s); std::memcpy(&d.total_mass, s, sizeof(SrbdConst)); }
   Rot Rw[NB]; double pw[NB][3];
-  auto host_fk = [&](const double* q /*24*/) {
-    const double rz[3] = {q[5], q[4], q[3]}; Rw[0] = from_rpy(rz); for (int i = 0; i < 3; ++i) pw[0][i] = q[i];   // Rz(q3) Ry(q4) Rx(q5)
-    for (int j = 0; j < NJ; ++j) { const int pb = d.parent[j]; Rot Rl; std::memcpy(Rl.m, d.Rj[j], sizeof(Rl.m)); Rw[j + 1] = mul(mul(Rw[pb], Rl), about_axis(d.axis[j], q[6 + j])); apply(Rw[pb], d.pj[j], pw[j + 1]); for (int i = 0; i < 3; ++i) pw[j + 1][i] += pw[pb][i]; }
-  };
-  { double qn[NQ] = {0}; for (int j = 0; j < NJ; ++j) qn[6 + j] = hm.default_joint_state[j]; host_fk(qn);
-    Lump whole; for (int b = 0; b < NB; ++b) { double c[3]; apply(Rw[b], d.com[b], c); for (int i = 0; i < 3; ++i) c[i] += pw[b][i]; Rot I0; std::memcpy(I0.m, d.Ib[b], sizeof(I0.m)); Rot Iw = mul(mul(Rw[b], I0), transpose(Rw[b])); lump_add(whole, d.mass[b], c, Iw.m); }
-    std::memcpy(d.I_nom, whole.I, sizeof(whole.I)); for (int i = 0; i < 3; ++i) d.c_nom[i] = -whole.c[i];
-    const double* m = d.I_nom; const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6]; const double id = 1.0 / (m[0] * c00 + m[1] * c01 + m[2] * c02);
-    double* o = d.I_nom_inv; o[0] = c00 * id; o[1] = (m[2] * m[7] - m[1] * m[8]) * id; o[2] = (m[1] * m[5] - m[2] * m[4]) * id; o[3] = c01 * id; o[4] = (m[0] * m[8] - m[2] * m[6]) * id; o[5] = (m[2] * m[3] - m[0] * m[5]) * id;
-    o[6] = c02 * id; o[7] = (m[1] * m[6] - m[0] * m[7]) * id; o[8] = (m[0] * m[4] - m[1] * m[3]) * id; }
 
   // --- WBC gains (wbcWigeht.cfg defaults; optional override file) and friction (WbcBase.cpp:584-594) ---
   d.kp_swing = 350; d.kd_swing = 37; d.base_height_kp = 400; d.base_height_kd = 140; d.base_linear_kp = 400; d.base_linear_kd = 100; d.base_angular_kp = 400; d.base_angular_kd = 140;
@@ -248,7 +265,7 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
   { auto init = task.matrix("initialState", NX, 1); for (int i = 0; i < NX; ++i) hm.initial_state[i] = init[i]; }
   { auto Q = task.matrix("Q", NX, NX); std::memcpy(d.Q, Q.data(), sizeof(d.Q)); auto Rt = task.matrix("R", NU, NU); std::memcpy(d.R, Rt.data(), sizeof(d.R));
     // initializeInputCostWeight (QMInterface.cpp:274-299): R[12:24,12:24] = J^T Rtask[12:24,12:24] J, J = d(foot pos)/d(leg joints) at initialState
-    host_fk(hm.initial_state + 6); double J[12][12] = {{0}};
+    host_fk(d, hm.initial_state + 6, Rw, pw); double J[12][12] = {{0}};
     for (int f = 0; f < 4; ++f) { const int body = d.foot_body[f]; double pf[3]; apply(Rw[body], d.foot_p[f], pf); for (int i = 0; i < 3; ++i) pf[i] += pw[body][i];
       for (int k = 0; k < 3; ++k) { const int j = d.foot_leg[f] + k; const int ax = d.axis[j]; const double a[3] = {Rw[j + 1].m[ax], Rw[j + 1].m[3 + ax], Rw[j + 1].m[6 + ax]}; const double r[3] = {pf[0] - pw[j + 1][0], pf[1] - pw[j + 1][1], pf[2] - pw[j + 1][2]};
         J[3 * f + 0][j] = a[1] * r[2] - a[2] * r[1]; J[3 * f + 1][j] = a[2] * r[0] - a[0] * r[2]; J[3 * f + 2][j] = a[0] * r[1] - a[1] * r[0]; } }

@@ -52,6 +52,12 @@ struct HostModel {
 // from task.info (Q, R with the leg-velocity block mapped through the foot Jacobians, QMInterface.cpp:274-299).
 HostModel build_host_model(const std::string& task_file, const std::string& urdf_file, const std::string& reference_file, const std::string& gains_file);
 
+// The SRBD constants (SrbdConst, padded to SRBD_DBL doubles) of the model at defaultJointState, as createCentroidalModelInfo folds the bodies: the composite
+// mass, inertia about the composite COM and the base-to-COM offset.  `payload` (include/qmb200.h layout [m_ee, o_ee(3), m_base, o_base(3)], or null) adds
+// two point masses without rotational inertia, at o_ee in the end-effector frame and at o_base in the base frame - what a URDF with an extra fixed link carrying
+// each mass would give.  Zero masses add nothing: build_host_model's DevModel fields are this function with no payload.
+void srbd_constants(const DevModel& d, const double* default_joint_state, const double* payload, double* out /*[SRBD_DBL]*/);
+
 // gait.info / reference.info mode-sequence templates (ocs2 ModeSequenceTemplate) and name → mode number
 struct ModeTemplate { std::vector<double> switching_times; std::vector<int> modes; };
 int mode_from_name(const std::string& name);

@@ -24,7 +24,7 @@ struct ControlLawParams {
   double arm_kp, arm_kd;      // dynamic_reconfigure kp_arm_wbc / kd_arm_wbc (qm_controllers/cfg/weight.cfg:7-8: 0.0, 0.5)
 };
 
-int launch_observation(const DevModel* mdl, int B, const double* rbd, const double* period, double* t_obs, double* x_obs, cudaStream_t s);
+int launch_observation(const DevModel* mdl, int B, const double* rbd, const double* period, double* t_obs, double* x_obs, cudaStream_t s, const double* srbd /*[B][SRBD_DBL] or NULL*/);
 int launch_target(const TargetParams& prm, int kind, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state, double* last_ee_target,
                   int32_t* n_target, double* target_times, double* target_states, cudaStream_t s);
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,

@@ -45,9 +45,10 @@ __device__ __forceinline__ void quat_to_rot(double w, double x, double y, double
 
 // -----------------------------------------------------------------------------------------------------------------
 // Observation: rbd[55] → centroidal state (SRBD mapping, the same arithmetic as qmb200_centroidal_state_from_rbd:
-// CentroidalModelRbdConversions::computeCentroidalStateFromRbdModel [upstream, recalled]) with the controller's yaw unwrap.
+// CentroidalModelRbdConversions::computeCentroidalStateFromRbdModel [upstream, recalled]) with the controller's yaw unwrap.  srbd: per-robot SRBD constants
+// [B][SRBD_DBL] of a model payload, or NULL for the model's.
 __global__ void __launch_bounds__(OBS_ROBOTS) ctrl_observation_kernel(const DevModel* __restrict__ mdl, int B, const double* __restrict__ rbd, const double* __restrict__ period,
-                                                                       double* __restrict__ t_obs, double* __restrict__ x_obs) {
+                                                                       double* __restrict__ t_obs, double* __restrict__ x_obs, const double* __restrict__ srbd) {
   __shared__ double s_rbd[OBS_ROBOTS * 55];   // leading dimension 55 (odd)
   __shared__ double s_x[OBS_ROBOTS * 31];
   const int b0 = blockIdx.x * OBS_ROBOTS, rows = min(OBS_ROBOTS, B - b0), r = threadIdx.x;
@@ -57,10 +58,11 @@ __global__ void __launch_bounds__(OBS_ROBOTS) ctrl_observation_kernel(const DevM
     const double* s = s_rbd + r * 55; double* o = s_x + r * 31;
     double R[9]; rot_zyx(s[0], s[1], s[2], R);
     const double w[3] = {s[NQ], s[NQ + 1], s[NQ + 2]};
-    double c[3]; matvec3(R, mdl->c_nom, c);
+    const SrbdConst* sc = srbd_of(mdl, srbd, b0 + r);
+    double c[3]; matvec3(R, sc->c_nom, c);
     double cw[3]; cross3(c, w, cw);                                     // h_lin/m = v_lin + (R c_nom) x w
-    double Rtw[3], IRtw[3], L[3]; matTvec3(R, w, Rtw); matvec3(mdl->I_nom, Rtw, IRtw); matvec3(R, IRtw, L);   // h_ang = R I R^T w
-    const double inv_m = 1.0 / mdl->total_mass;
+    double Rtw[3], IRtw[3], L[3]; matTvec3(R, w, Rtw); matvec3(sc->I_nom, Rtw, IRtw); matvec3(R, IRtw, L);   // h_ang = R I R^T w
+    const double inv_m = 1.0 / sc->m;
 #pragma unroll
     for (int i = 0; i < 3; ++i) { o[i] = s[NQ + 3 + i] + cw[i]; o[3 + i] = L[i] * inv_m; o[6 + i] = s[3 + i]; o[9 + i] = s[i]; }
 #pragma unroll
@@ -187,8 +189,8 @@ __global__ void __launch_bounds__(ControlLawParams::THREADS) ctrl_hw_write_kerne
 }
 
 // -----------------------------------------------------------------------------------------------------------------
-int launch_observation(const DevModel* mdl, int B, const double* rbd, const double* period, double* t_obs, double* x_obs, cudaStream_t s) {
-  ctrl_observation_kernel<<<(B + OBS_ROBOTS - 1) / OBS_ROBOTS, OBS_ROBOTS, 0, s>>>(mdl, B, rbd, period, t_obs, x_obs); return 1;
+int launch_observation(const DevModel* mdl, int B, const double* rbd, const double* period, double* t_obs, double* x_obs, cudaStream_t s, const double* srbd) {
+  ctrl_observation_kernel<<<(B + OBS_ROBOTS - 1) / OBS_ROBOTS, OBS_ROBOTS, 0, s>>>(mdl, B, rbd, period, t_obs, x_obs, srbd); return 1;
 }
 int launch_target(const TargetParams& prm, int kind, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state, double* last_ee_target,
                   int32_t* n_target, double* target_times, double* target_states, cudaStream_t s) {

@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stddef.h>
 #include <stdint.h>
 
 // Scalar helpers are host + device: tests/nodeeval_host.cpp compiles the one-thread-per-node evaluator (node_eval.cuh) with g++ and checks it against the
@@ -67,6 +68,17 @@ struct DevModel {
   int wbc_iter_cap0, wbc_iter_cap;   // WBC iteration caps: level-0 semismooth passes (30) and active-set iterations per level (80); qmb200_wbc_set_iteration_caps (diagnostics / tests)
   double cost_tol; int sqp_iterations;   // sqp.sqpIteration (task.info:28) and costTol [upstream ocs2_sqp default 1e-4]: SqpSolver::runImpl loop + checkConvergence
 };
+
+// The SRBD constants of one robot (createCentroidalModelInfo [upstream]): robotMass, centroidalInertiaNominal, its inverse, comToBasePositionNominal, in the order
+// DevModel keeps the nominal robot's.  A robot with a model payload (qmb200_set_model_payload) has its own block of SRBD_DBL doubles in this order, so the kernels
+// read either through one pointer: srbd_of(mdl, srbd, b) with srbd = the per-robot blocks, or NULL for the nominal model.
+struct SrbdConst { double m, I_nom[9], I_nom_inv[9], c_nom[3]; };
+constexpr int SRBD_DBL = 24;   // SrbdConst padded to 16-byte rows
+static_assert(offsetof(DevModel, I_nom) == offsetof(DevModel, total_mass) + offsetof(SrbdConst, I_nom) && offsetof(DevModel, I_nom_inv) == offsetof(DevModel, total_mass) + offsetof(SrbdConst, I_nom_inv) &&
+              offsetof(DevModel, c_nom) == offsetof(DevModel, total_mass) + offsetof(SrbdConst, c_nom) && sizeof(SrbdConst) <= SRBD_DBL * 8, "DevModel's SRBD fields have SrbdConst's layout");
+QMB_HD const SrbdConst* srbd_of(const DevModel* mdl, const double* srbd, int b) {
+  return srbd ? reinterpret_cast<const SrbdConst*>(srbd + (size_t)SRBD_DBL * b) : reinterpret_cast<const SrbdConst*>(&mdl->total_mass);
+}
 
 #ifdef __CUDACC__
 __device__ __forceinline__ double warp_sum(double v) {

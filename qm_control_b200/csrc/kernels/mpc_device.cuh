@@ -19,16 +19,16 @@ __device__ __forceinline__ double target_xnom(const double* tt, const double* ts
 }
 
 // Intermediate (or terminal) cost value and its quadratic model in the compact form of QuadWs (NOT scaled by dt).  ws: {x[30], u[30]} of the node; cw: end-effector
-// error e[6] and its Jacobian Je[6][12] (flow kernel); xnom: this lane's state reference; `flagmask` = contact flags (bit i = foot i).  Returns the value (lane-uniform).
+// error e[6] and its Jacobian Je[6][12] (flow kernel); sc: the robot's SRBD constants (srbd_of); xnom: this lane's state reference; `flagmask` = contact flags (bit i = foot i).  Returns the value (lane-uniform).
 template <class WS, class CW>
-__device__ __forceinline__ double stage_cost_quad(const DevModel* __restrict__ mdl, const WS* ws, const CW* cw, QuadWs* qw, double xnom, int flagmask, bool terminal, int lane) {
+__device__ __forceinline__ double stage_cost_quad(const DevModel* __restrict__ mdl, const SrbdConst* sc, const WS* ws, const CW* cw, QuadWs* qw, double xnom, int flagmask, bool terminal, int lane) {
   double value = 0.0;
   for (int e = lane; e < 144; e += 32) qw->E[e] = 0.0; for (int e = lane; e < 36; e += 32) qw->fric[e] = 0.0; if (lane < NX) { qw->qdiag[lane] = 0.0; qw->rdiag[lane] = 0.0; qw->qf[lane] = 0.0; qw->rf[lane] = 0.0; } __syncwarp();
   int nst = 0; for (int i = 0; i < 4; ++i) nst += (flagmask >> i) & 1;
   if (!terminal) {
     // tracking cost: 1/2 dx'Q dx + 1/2 du'R du, u_nom = weightCompensatingInput(contact flags)
     double dx = 0.0, du = 0.0;
-    if (lane < NX) { dx = ws->x[lane] - xnom; double un = 0.0; if (lane < 12 && (lane % 3) == 2 && ((flagmask >> (lane / 3)) & 1)) un = mdl->total_mass * 9.81 / nst; du = ws->u[lane] - un; }
+    if (lane < NX) { dx = ws->x[lane] - xnom; double un = 0.0; if (lane < 12 && (lane % 3) == 2 && ((flagmask >> (lane / 3)) & 1)) un = sc->m * 9.81 / nst; du = ws->u[lane] - un; }
     double qd = 0.0, rd = 0.0;
     if (mdl->q_is_diag) { if (lane < NX) qd = mdl->Qdiag[lane] * dx; }
     else { const double* Qr = mdl->Q + (lane < NX ? lane : 0) * NX;

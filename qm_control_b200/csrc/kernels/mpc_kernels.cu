@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(32 * SETUP_WARPS) mpc_setup_kernel(const DevMo
   for (int k = 0; k < n - 1; ++k) {
     const int flag = sflag[k]; const SetupIdx ix = sidx[k]; double uk = 0.0;
     if (flag == 1) { uk = lerp(pu, ix.iu, ix.au); xk = lerp(px, ix.ix, ix.ax); }
-    else if (flag == 0) { const int mode = ix.iu; int nst = 0; for (int i = 0; i < 4; ++i) nst += contact_flag(mode, i); if (lane < 12 && (lane % 3) == 2 && contact_flag(mode, lane / 3)) uk = mdl->total_mass * 9.81 / nst; }
+    else if (flag == 0) { const int mode = ix.iu; int nst = 0; for (int i = 0; i < 4; ++i) nst += contact_flag(mode, i); if (lane < 12 && (lane % 3) == 2 && contact_flag(mode, lane / 3)) uk = srbd_of(mdl, p.srbd, b)->m * 9.81 / nst; }
     if (lane < NX) { gu[(size_t)k * NU + lane] = uk; gx[(size_t)(k + 1) * NX + lane] = xk; }
   }
   if (lane < NX && n >= 1) gu[(size_t)(n - 1) * NU + lane] = 0.0;
@@ -140,6 +140,7 @@ __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(co
   const bool terminal = work && (k == n - 1);
   if (work && !terminal && sol.event[(size_t)b * nmax + k] == 1) work = false;   // event node: identity jump map, nothing to evaluate
   const unsigned active = __ballot_sync(FULL, work); if (!active) return;
+  const SrbdConst* sc = srbd_of(mdl, p.srbd, work ? b : b0);   // the robot's SRBD constants (qmb200_set_model_payload), the model's without a model payload
   double* row = &tile[warp][lane][0]; double* gbase = rec + ((size_t)b0 * nmax + (size_t)(gid - lane)) * ne::NODE_REC_DBL;   // node index = robot * nmax + k, as K2b reads it
   auto flush = [&](int off, int cnt) {   // rows of the tile -> records: 32 (or 64) consecutive doubles of one node per store instruction
     __syncwarp();
@@ -157,17 +158,17 @@ __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(co
     for (int i = 0; i < NX; ++i) { x[i] = xk[i]; u[i] = terminal ? 0.0 : uk[i]; }
     asm volatile("" ::: "memory");   // u is read back from the row where it is used, not held in registers
     t = interval_start(gt[k], ge[k]); dt = terminal ? 0.0 : interval_end(gt[k + 1], ge[k + 1]) - t;
-    ne::base_eval<true>(mdl, x, bk); ne::flow_acc_init(acc);
+    ne::base_eval<true>(mdl, x, bk, sc); ne::flow_acc_init(acc);
   }
 #pragma unroll 1
   for (int i = 0; i < 4; ++i) {   // foot blocks: kinematics of the leg, foot-velocity rows
     if (work) { ne::FootBlk* fb = reinterpret_cast<ne::FootBlk*>(row); double al[9];
-      ne::foot_eval<true>(mdl, x, u, bk, i, acc, fb->d, fb->pf, fb->Jl, al, fb->JxF);
+      ne::foot_eval<true>(mdl, x, u, bk, i, acc, fb->d, fb->pf, fb->Jl, al, fb->JxF, sc);
       if (!terminal) ne::foot_velocity_1<true>(mdl, x, u, bk, i, fb->d, fb->Jl, al, fb->e, fb->C); }
     flush(i * ne::FOOT_DBL, ne::FOOT_DBL);
   }
   double f1[12];
-  if (work) { ne::FlowBlk* fl = reinterpret_cast<ne::FlowBlk*>(row); ne::flow_finish<true>(mdl, x, bk, acc, fl->f, fl);
+  if (work) { ne::FlowBlk* fl = reinterpret_cast<ne::FlowBlk*>(row); ne::flow_finish<true>(mdl, x, bk, acc, fl->f, fl, sc);
 #pragma unroll
     for (int i = 0; i < 12; ++i) f1[i] = fl->f[i]; }
   flush(4 * ne::FOOT_DBL, ne::FLOW_DBL);
@@ -180,12 +181,12 @@ __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(co
     const double cdt = mdl->rk_c * dt;
 #pragma unroll
     for (int i = 0; i < NX; ++i) x[i] += cdt * (i < 12 ? f1[i < 12 ? i : 0] : u[i]);
-    ne::base_eval<true>(mdl, x, bk); ne::flow_acc_init(acc);
+    ne::base_eval<true>(mdl, x, bk, sc); ne::flow_acc_init(acc);
 #pragma unroll 1
-    for (int i = 0; i < 4; ++i) { ne::Foot2Blk* f2 = reinterpret_cast<ne::Foot2Blk*>(row) + i; ne::foot_eval<true>(mdl, x, u, bk, i, acc, f2->d, nullptr, nullptr, nullptr, f2->JxF); }
+    for (int i = 0; i < 4; ++i) { ne::Foot2Blk* f2 = reinterpret_cast<ne::Foot2Blk*>(row) + i; ne::foot_eval<true>(mdl, x, u, bk, i, acc, f2->d, nullptr, nullptr, nullptr, f2->JxF, sc); }
   }
   flush(4 * ne::FOOT_DBL + ne::FLOW_DBL + ne::EE_DBL, 4 * ne::FOOT2_DBL);
-  if (stage2) { ne::FlowBlk* fl = reinterpret_cast<ne::FlowBlk*>(row); ne::flow_finish<true>(mdl, x, bk, acc, fl->f, fl); }
+  if (stage2) { ne::FlowBlk* fl = reinterpret_cast<ne::FlowBlk*>(row); ne::flow_finish<true>(mdl, x, bk, acc, fl->f, fl, sc); }
   flush(4 * ne::FOOT_DBL + ne::FLOW_DBL + ne::EE_DBL + 4 * ne::FOOT2_DBL, ne::FLOW_DBL);
 }
 
@@ -231,6 +232,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   if (!work) return;
   double* sg = stage + node * STAGE_DBL;
   const bool terminal = (k == n - 1);
+  const SrbdConst* sc = srbd_of(mdl, p.srbd, b);
   if (lane < NX) { sm.x[lane] = xv; sm.u[lane] = terminal ? 0.0 : uv; }   // the next node's state (defect) stays in the lane's register
   __syncwarp();
   if (!terminal && ek == 1) {   // event node: identity jump map, no input, no cost (setupEventNode)
@@ -254,7 +256,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   {
   // ---- cost quadratic model at (x, u) (the end-effector error and its Jacobian come with the record) ----
   struct XU { double x[NX], u[NU]; }; static_assert(offsetof(LqSmem, u) == offsetof(LqSmem, x) + NX * 8, "x then u");
-  cost_val = stage_cost_quad(mdl, reinterpret_cast<const XU*>(sm.x), &sm.rec.ee, &sm.quad, target_xnom(tt, ts, nk, t, lane), fm, terminal, lane);
+  cost_val = stage_cost_quad(mdl, sc, reinterpret_cast<const XU*>(sm.x), &sm.rec.ee, &sm.quad, target_xnom(tt, ts, nk, t, lane), fm, terminal, lane);
   if (terminal) {   // setupTerminalNode: finalEndEffector soft constraint only (QMInterface.cpp:104)
     double* tl = sg + ST_TAIL; int32_t* si = reinterpret_cast<int32_t*>(tl + T_INT);
     for (int r = 0; r < NX; ++r) { const int a = ee_pos(r); if (lane < q_row_padded(r)) { const int cc = (lane <= r) ? ee_pos(lane) : -1; sg[ST_Q + q_row_offset(r) + lane] = (a >= 0 && cc >= 0) ? sm.quad.E[a * 12 + cc] : 0.0; } }   // final cost: packed lower triangle
@@ -317,7 +319,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
     sm.rs[lane] = sv;
   }
   // continuous-time Jacobians of the two RK2 stages from the record's blocks
-  const double imr = 1.0 / mdl->total_mass;
+  const double imr = 1.0 / sc->m;
   expand_flow(sm.rec.s1, sm.rec.foot[0].JxF, ne::FOOT_DBL, sm.A1r, lfp, lane); expand_flow(sm.rec.s2, sm.rec.foot2[0].JxF, ne::FOOT2_DBL, sm.Ar, lfp, lane);
   // force block of rows 3:6 of df/du at both stages, column c = lane < 12 (foot i = c / 3, axis a = c % 3): cross(d_i, e_a)[r] / m - three entries per stage, kept in registers
   // (the foot blocks of the record are about to be overlaid by the RK2 combination's outputs)
@@ -326,7 +328,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
     for (int r = 0; r < 3; ++r) if (r != a) { const double sgn = ((a - r + 3) % 3 == 1) ? -imr : imr; b1v[r] = sgn * d1[3 - r - a]; b2v[r] = sgn * d2[3 - r - a]; } }
   __syncwarp();
   }
-  const double w1 = mdl->rk_w1, w2 = mdl->rk_w2, cdt = mdl->rk_c * dt, mass = mdl->total_mass, dtw = dt * (w1 + w2), imass = 1.0 / mass;
+  const double w1 = mdl->rk_w1, w2 = mdl->rk_w2, cdt = mdl->rk_c * dt, mass = sc->m, dtw = dt * (w1 + w2), imass = 1.0 / mass;
   double bb = 0.0; if (lane < NX) { const double fa = lane < 12 ? sm.rec.s1.f[lane < 12 ? lane : 0] : sm.u[lane], fb = lane < 12 ? sm.rec.s2.f[lane < 12 ? lane : 0] : sm.u[lane];   // rows 12:30 of the flow map: the joint-velocity inputs
     bb = xv + dt * (w1 * fa + w2 * fb) - xnv; lt.bvec[lane] = bb; }   // defect
   const double dyn_ss = warp_sum(bb * bb);
@@ -583,7 +585,7 @@ __global__ void __launch_bounds__(RIC_THREADS, 4) mpc_riccati_kernel(const DevMo
   if (status[b] & MST_CONVERGED) return;
   const int n = sol.n_nodes[b]; const int N = n - 1;
   const double* sgb = stage + (size_t)b * nmax * STAGE_DBL; double* gb = gains + (size_t)b * nmax * GAIN_DBL;
-  const int lfp = pack_leg_foot(mdl); const double imass = 1.0 / mdl->total_mass;
+  const int lfp = pack_leg_foot(mdl); const double imass = 1.0 / srbd_of(mdl, p.srbd, b)->m;
   for (int e = tid; e < (int)(sizeof(RicSmem) / 8); e += RIC_THREADS) reinterpret_cast<double*>(&sm)[e] = 0.0;   // zero everything once (padding columns, static zero rows)
   __syncthreads();
   if (tid < NX && (tid < 3 || tid >= 24)) sm.A[tid * LDX + tid] = 1.0;   // identity rows of A~ that no node ever changes
@@ -853,7 +855,7 @@ __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_ker
   const double* rb = robot + (size_t)b * ROBOT_DBL; const double armijo = rb[0], base_cost = rb[1], base_viol = sqrt(rb[2] + rb[3]), dxn = rb[4], dun = rb[5];
   const bool failed = (status[b] & MST_NOT_PD) != 0;
   double alpha = 1.0; bool accepted = false; double sc = base_cost, sd = rb[2], se = rb[3];
-  const double w1 = mdl->rk_w1, w2 = mdl->rk_w2;
+  const double w1 = mdl->rk_w1, w2 = mdl->rk_w2; const SrbdConst* srb = srbd_of(mdl, p.srbd, b);
   while (!failed) {
     double cost = 0.0, dyn = 0.0, eq = 0.0;
     for (int k = tid; k <= N; k += 32 * LS_WARPS) {
@@ -866,26 +868,26 @@ __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_ker
       const double t = interval_start(gt[k], ge[k]);
       const double dt = terminal ? 1.0 : interval_end(gt[k + 1], ge[k + 1]) - t; const int mode = mode_at_time(ev, modes, ne, t); const int fm = terminal ? 0 : flag_mask(mode);
       ne::BaseKin bk; ne::FlowAcc acc; double* f1 = ua + NU;
-      ne::base_eval<false>(mdl, xa, bk); ne::flow_acc_init(acc);
+      ne::base_eval<false>(mdl, xa, bk, srb); ne::flow_acc_init(acc);
       { double es = 0.0; bool ok = true;
 #pragma unroll 1
-        for (int i = 0; i < 4; ++i) { double d[3], Jl[9], pf[3]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, pf, Jl, nullptr, nullptr);
+        for (int i = 0; i < 4; ++i) { double d[3], Jl[9], pf[3]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, pf, Jl, nullptr, nullptr, srb);
           if (!terminal) { double fe[3]; ne::foot_velocity_1<false>(mdl, xa, ua, bk, i, d, Jl, nullptr, fe, nullptr); ne::equality_add(mdl, ua, fe, pf, fm, ev, modes, ne, t, i, es, ok); } }
         if (!terminal) eq += dt * es; }
-      ne::flow_finish<false>(mdl, xa, bk, acc, f1, nullptr);
+      ne::flow_finish<false>(mdl, xa, bk, acc, f1, nullptr, srb);
       asm volatile("" ::: "memory");   // f1 is read back after the cost, not held in registers across it
       { const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, xa, bk, pref, qref, ee, nullptr);
-        cost += dt * ne::cost_value(mdl, xa, ua, sg, ee, fm, terminal); }
+        cost += dt * ne::cost_value(mdl, xa, ua, sg, ee, fm, terminal, srb); }
       if (terminal) continue;
       const double cdt = mdl->rk_c * dt;   // second stage in place (the trial state is re-read from L2 for the defect)
 #pragma unroll
       for (int i = 0; i < 12; ++i) xa[i] += cdt * f1[i];
 #pragma unroll 6
       for (int i = 12; i < NX; ++i) xa[i] += cdt * ua[i];
-      double f2[12]; ne::base_eval<false>(mdl, xa, bk); ne::flow_acc_init(acc);
+      double f2[12]; ne::base_eval<false>(mdl, xa, bk, srb); ne::flow_acc_init(acc);
 #pragma unroll 1
-      for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr); }
-      ne::flow_finish<false>(mdl, xa, bk, acc, f2, nullptr);
+      for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, xa, ua, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr, srb); }
+      ne::flow_finish<false>(mdl, xa, bk, acc, f2, nullptr, srb);
       double s = 0.0;
       auto defect = [&](int i, double fa, double fb) { const double x0i = gx[(size_t)k * NX + i] + alpha * gdx[(size_t)k * NX + i];
         const double d = x0i + dt * (w1 * fa + w2 * fb) - (gx[(size_t)(k + 1) * NX + i] + alpha * gdx[(size_t)(k + 1) * NX + i]); s = fma(d, d, s); };
@@ -955,26 +957,26 @@ __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_ker
 constexpr int RO_THREADS = 128, RO_MAXTRIALS = 32;
 // one RK2 step of the flow map from (x, u); with PERF also the node's cost (unscaled by dt) and equality SSE at (x, u).  x is replaced by the next state.
 template <bool PERF, class MT>
-__device__ __forceinline__ void rollout_step(const DevModel* __restrict__ mdl, double* x, const double* u, double t, double dt, int fm, const double* ev, const MT* modes, int ne, const double* tt, const double* ts, int nk, double& cost, double& eq) {
-  ne::BaseKin bk; ne::FlowAcc acc; double f1[12], x2[NX]; ne::base_eval<false>(mdl, x, bk); ne::flow_acc_init(acc);
+__device__ __forceinline__ void rollout_step(const DevModel* __restrict__ mdl, const SrbdConst* sc, double* x, const double* u, double t, double dt, int fm, const double* ev, const MT* modes, int ne, const double* tt, const double* ts, int nk, double& cost, double& eq) {
+  ne::BaseKin bk; ne::FlowAcc acc; double f1[12], x2[NX]; ne::base_eval<false>(mdl, x, bk, sc); ne::flow_acc_init(acc);
   if (PERF) { double es = 0.0; bool ok = true;
 #pragma unroll 1
-    for (int i = 0; i < 4; ++i) { double d[3], Jl[9], pf[3], fe[3]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, pf, Jl, nullptr, nullptr); ne::foot_velocity_1<false>(mdl, x, u, bk, i, d, Jl, nullptr, fe, nullptr);
+    for (int i = 0; i < 4; ++i) { double d[3], Jl[9], pf[3], fe[3]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, pf, Jl, nullptr, nullptr, sc); ne::foot_velocity_1<false>(mdl, x, u, bk, i, d, Jl, nullptr, fe, nullptr);
       ne::equality_add(mdl, u, fe, pf, fm, ev, modes, ne, t, i, es, ok); }
     eq += dt * es;
     const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, x, bk, pref, qref, ee, nullptr);
-    cost += dt * ne::cost_value(mdl, x, u, sg, ee, fm, false);
+    cost += dt * ne::cost_value(mdl, x, u, sg, ee, fm, false, sc);
   } else {
 #pragma unroll 1
-    for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr); } }
-  ne::flow_finish<false>(mdl, x, bk, acc, f1, nullptr);
+    for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr, sc); } }
+  ne::flow_finish<false>(mdl, x, bk, acc, f1, nullptr, sc);
   const double cdt = mdl->rk_c * dt, w1 = mdl->rk_w1, w2 = mdl->rk_w2;
 #pragma unroll
   for (int i = 0; i < NX; ++i) x2[i] = x[i] + cdt * (i < 12 ? f1[i < 12 ? i : 0] : u[i]);
-  double f2[12]; ne::base_eval<false>(mdl, x2, bk); ne::flow_acc_init(acc);
+  double f2[12]; ne::base_eval<false>(mdl, x2, bk, sc); ne::flow_acc_init(acc);
 #pragma unroll 1
-  for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, x2, u, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr); }
-  ne::flow_finish<false>(mdl, x2, bk, acc, f2, nullptr);
+  for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, x2, u, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr, sc); }
+  ne::flow_finish<false>(mdl, x2, bk, acc, f2, nullptr, sc);
 #pragma unroll
   for (int i = 0; i < NX; ++i) x[i] += dt * (w1 * (i < 12 ? f1[i < 12 ? i : 0] : u[i]) + w2 * (i < 12 ? f2[i < 12 ? i : 0] : u[i]));
 }
@@ -1016,7 +1018,7 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_kernel(co
       if (ge[k] != 1) { const double t = interval_start(gt[k], ge[k]); const double dt = interval_end(gt[k + 1], ge[k + 1]) - t; double u[NU];
 #pragma unroll
         for (int i = 0; i < NU; ++i) u[i] = gu[(size_t)k * NU + i];
-        rollout_step<false>(mdl, xa, u, t, dt, 0, ev, modes, ne, tt, ts, nk, cost, eq); }
+        rollout_step<false>(mdl, srbd_of(mdl, p.srbd, b), xa, u, t, dt, 0, ev, modes, ne, tt, ts, nk, cost, eq); }
 #pragma unroll
       for (int i = 0; i < NX; ++i) gx[(size_t)(k + 1) * NX + i] = xa[i];
     }
@@ -1047,7 +1049,7 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_kernel(co
         rollout_input(tl, gb + (size_t)k * GAIN_DBL, gu + (size_t)k * NU, dxv, alpha, lfp, un);
         for (int i = 0; i < NU; ++i) gu[(size_t)k * NU + i] = un[i];
         const double t = interval_start(gt[k], ge[k]); const double dt = interval_end(gt[k + 1], ge[k + 1]) - t; const int fm = flag_mask(mode_at_time(ev, modes, ne, t));
-        rollout_step<false>(mdl, xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
+        rollout_step<false>(mdl, srbd_of(mdl, p.srbd, b), xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
       }
       // the nominal state of the next node is read before the new one replaces it (in-place commit)
 #pragma unroll
@@ -1098,16 +1100,16 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_trials_ke
         for (int i = 0; i < NX; ++i) dxv[i] = xa[i] - xnom[i];
         rollout_input(tl, sK + r * GAIN_DBL, gu + (size_t)k * NU, dxv, alpha, lfp, un);
         const double t = interval_start(gt[k], ge[k]); const double dt = interval_end(gt[k + 1], ge[k + 1]) - t; const int fm = flag_mask(mode_at_time(ev, modes, ne, t));
-        rollout_step<true>(mdl, xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
+        rollout_step<true>(mdl, srbd_of(mdl, p.srbd, (int)bb), xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
       }
 #pragma unroll
       for (int i = 0; i < NX; ++i) xnom[i] = gx[(size_t)(k + 1) * NX + i];
     }
   }
   if (active) {   // final cost at x_N
-    const double t = interval_start(gt[N], ge[N]); ne::BaseKin bk; ne::base_eval<false>(mdl, xa, bk); double u0[NU]; for (int i = 0; i < NU; ++i) u0[i] = 0.0;
+    const double t = interval_start(gt[N], ge[N]); ne::BaseKin bk; ne::base_eval<false>(mdl, xa, bk, srbd_of(mdl, p.srbd, b)); double u0[NU]; for (int i = 0; i < NU; ++i) u0[i] = 0.0;
     const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, xa, bk, pref, qref, ee, nullptr);
-    cost += ne::cost_value(mdl, xa, u0, sg, ee, 0, true);
+    cost += ne::cost_value(mdl, xa, u0, sg, ee, 0, true, srbd_of(mdl, p.srbd, b));
     double* tb = trial + (size_t)b * RO_MAXTRIALS * 2; tb[2 * tr] = cost; tb[2 * tr + 1] = eq; }
 }
 

@@ -39,6 +39,9 @@ struct FlowAcc { double fsum[3], hang[3], hth[3][3]; };
 // thread's array with s directly would place the whole array in local memory.
 QMB_HD double pick3(const double* a, int s, int c) { return s == 0 ? a[c] : (s == 1 ? a[3 + c] : (s == 2 ? a[6 + c] : a[9 + c])); }
 
+// The SRBD constants the flow map and the cost use (base_eval, foot_eval, flow_finish, cost_value take the robot's as `sc`): the model's when sc is null.
+QMB_HD const SrbdConst& srbd_or_nominal(const DevModel* __restrict__ mdl, const SrbdConst* sc) { return sc ? *sc : *srbd_of(mdl, nullptr, 0); }
+
 // one serial chain from the base: joints first .. first + NJC - 1 at angles q[0 .. NJC - 1]; returns the last body's frame, every joint's origin and axis (world)
 template <int NJC>
 QMB_HD void chain_fk(const DevModel* __restrict__ mdl, const double* R0, const double* p0, const double* q, int first, double* Rl, double* pl, double (*org)[3], double (*axs)[3]) {
@@ -69,10 +72,10 @@ QMB_HD void chain_fk(const DevModel* __restrict__ mdl, const double* R0, const d
 }
 
 template <bool JAC>
-QMB_HD void base_eval(const DevModel* __restrict__ mdl, const double* x, BaseKin& bk) {
+QMB_HD void base_eval(const DevModel* __restrict__ mdl, const double* x, BaseKin& bk, const SrbdConst* sc = nullptr) {
   sincos(x[9], &bk.tr[0], &bk.tr[1]); sincos(x[10], &bk.tr[2], &bk.tr[3]); sincos(x[11], &bk.tr[4], &bk.tr[5]);
   rot_zyx_sc(bk.tr, bk.R0); euler_rate_map_sc(bk.tr, bk.T); inv3(bk.T, bk.Tinv);
-  const double m = mdl->total_mass; const double* R = bk.R0; const double* Ii = mdl->I_nom_inv; const double* ha = x + 3;
+  const SrbdConst& S = srbd_or_nominal(mdl, sc); const double m = S.m; const double* R = bk.R0; const double* Ii = S.I_nom_inv; const double* ha = x + 3;
 #pragma unroll
   for (int i = 0; i < 3; ++i)
 #pragma unroll
@@ -80,7 +83,7 @@ QMB_HD void base_eval(const DevModel* __restrict__ mdl, const double* x, BaseKin
 #pragma unroll
       for (int bq = 0; bq < 3; ++bq) { const double rib = R[3 * i] * Ii[bq] + R[3 * i + 1] * Ii[3 + bq] + R[3 * i + 2] * Ii[6 + bq]; acc = fma(rib, R[3 * jj + bq], acc); }
       bk.W[3 * i + jj] = m * acc; }
-  matvec3(R, mdl->c_nom, bk.c);
+  matvec3(R, S.c_nom, bk.c);
   for (int a = 0; a < 3; ++a) bk.rcom[a] = x[6 + a] - bk.c[a];
   matvec3(bk.W, ha, bk.omega); matvec3(bk.Tinv, bk.omega, bk.thd);
   if (JAC) { for (int k = 0; k < 3; ++k) { const double Tk[3] = {bk.T[k], bk.T[3 + k], bk.T[6 + k]}; double t1[3], t2[3], t3[3];
@@ -92,13 +95,14 @@ QMB_HD void flow_acc_init(FlowAcc& acc) { for (int a = 0; a < 3; ++a) { acc.fsum
 // One foot (contact order i; its leg's joints foot_leg[i] .. + 2): chain kinematics, foot - com, leg Jacobian columns Jl[3 * j + a] (+ joint axes al, same layout),
 // the foot's share of the flow map (accumulated in acc) and, with JAC, (J_j x F_i) / m.  Jl / al / pf / JxF may be null.
 template <bool JAC>
-QMB_HD void foot_eval(const DevModel* __restrict__ mdl, const double* x, const double* u, const BaseKin& bk, int i, FlowAcc& acc, double* d, double* pf, double* Jl, double* al, double* JxF) {
+QMB_HD void foot_eval(const DevModel* __restrict__ mdl, const double* x, const double* u, const BaseKin& bk, int i, FlowAcc& acc, double* d, double* pf, double* Jl, double* al, double* JxF,
+                      const SrbdConst* sc = nullptr) {
   const int first = mdl->foot_leg[i]; double Rl[9], pl[3], org[3][3], axs[3][3];
   const double q[3] = {pick3(x + 12, first / 3, 0), pick3(x + 12, first / 3, 1), pick3(x + 12, first / 3, 2)};
   chain_fk<3>(mdl, bk.R0, x + 6, q, first, Rl, pl, org, axs);
   double pw[3]; matvec3(Rl, mdl->foot_p[i], pw);
   for (int a = 0; a < 3; ++a) { pw[a] += pl[a]; d[a] = pw[a] - bk.rcom[a]; if (pf) pf[a] = pw[a]; }
-  const double F[3] = {pick3(u, i, 0), pick3(u, i, 1), pick3(u, i, 2)}; const double im = 1.0 / mdl->total_mass;
+  const double F[3] = {pick3(u, i, 0), pick3(u, i, 1), pick3(u, i, 2)}; const double im = 1.0 / srbd_or_nominal(mdl, sc).m;
   for (int a = 0; a < 3; ++a) acc.fsum[a] += F[a];
   cross3_add(d, F, acc.hang);
   for (int j = 0; j < 3; ++j) { const double r[3] = {pw[0] - org[j][0], pw[1] - org[j][1], pw[2] - org[j][2]}; double col[3]; cross3(axs[j], r, col);
@@ -110,8 +114,8 @@ QMB_HD void foot_eval(const DevModel* __restrict__ mdl, const double* x, const d
 
 // rows 0:12 of the flow map from the accumulated foot terms (+ the base-frame Jacobian blocks)
 template <bool JAC>
-QMB_HD void flow_finish(const DevModel* __restrict__ mdl, const double* x, const BaseKin& bk, const FlowAcc& acc, double* f, FlowBlk* fb) {
-  const double im = 1.0 / mdl->total_mass; const double* om = bk.omega; const double* c = bk.c;
+QMB_HD void flow_finish(const DevModel* __restrict__ mdl, const double* x, const BaseKin& bk, const FlowAcc& acc, double* f, FlowBlk* fb, const SrbdConst* sc = nullptr) {
+  const double im = 1.0 / srbd_or_nominal(mdl, sc).m; const double* om = bk.omega; const double* c = bk.c;
   for (int a = 0; a < 3; ++a) { f[a] = acc.fsum[a] * im + (a == 2 ? -9.81 : 0.0); f[3 + a] = acc.hang[a] * im; f[9 + a] = bk.thd[a]; }
   { double oc[3]; cross3(om, c, oc); for (int a = 0; a < 3; ++a) f[6 + a] = x[a] + oc[a]; }
   if (JAC) {
@@ -201,13 +205,13 @@ QMB_HD void ee_eval(const DevModel* __restrict__ mdl, const double* x, const Bas
 }
 
 // Intermediate (or terminal) cost VALUE at (x, u) given the end-effector error (stage_cost<false> of mpc_device.cuh; unscaled by dt)
-QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, const double* u, const TargetSeg& sg, const double* ee, int flagmask, bool terminal) {
+QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, const double* u, const TargetSeg& sg, const double* ee, int flagmask, bool terminal, const SrbdConst* sc = nullptr) {
   double value = 0.0;
   if (!terminal) {
     int nst = 0; for (int i = 0; i < 4; ++i) nst += (flagmask >> i) & 1;
     // deviations from the references element by element where they are used: whole dx[30] / du[30] arrays would not fit in registers next to (x, u)
     auto dx = [&](int i) { return x[i] - (sg.a * sg.l[i] + (1.0 - sg.a) * sg.rr[i]); };
-    const double un = mdl->total_mass * 9.81 / nst;
+    const double un = srbd_or_nominal(mdl, sc).m * 9.81 / nst;
     double acc = 0.0;
     if (mdl->q_is_diag) { for (int i = 0; i < NX; ++i) { const double d = dx(i); acc = fma(d * mdl->Qdiag[i], d, acc); } }
     else { for (int i = 0; i < NX; ++i) { double qd = 0.0; for (int j = 0; j < NX; ++j) qd = fma(mdl->Q[i * NX + j], dx(j), qd); acc = fma(dx(i), qd, acc); } }

@@ -21,7 +21,7 @@
 //   wrench[B][12]    [f_base, n_base, f_ee, n_ee], world frame, each moment about its own frame's origin, held over the step: W = [n + p x f; f]
 //                    about the world origin, Q_c += S_c . W over the base columns (base wrench) and the base + arm chain columns (EE wrench).
 // A zero payload or wrench adds exact zeros and mu[b] == prm.friction_mu is the shared law, so neutral variation is bit-identical.
-#include "rbd.cuh"
+#include "payload.cuh"
 #include "sim_api.cuh"
 #include "wlinalg.cuh"
 #include "../../../include/qmb200.h"
@@ -60,30 +60,11 @@ __device__ __forceinline__ void rot_to_quat_xyzw(const double* m, double* o) {
   }
 }
 
-// Lane 0: the end-effector frame, lane 1: the base frame.  Adds the payload point mass to Ic / F of the frame's body and writes the wrench about
+// Lane 0: the end-effector frame, lane 1: the base frame.  Adds the payload point mass to Ic / F of the frame's body (payload.cuh) and writes the wrench about
 // the world origin to w->W[lane] (sim_step_kernel's header has the layouts).
 __device__ __forceinline__ void frame_loads(const DevModel* __restrict__ mdl, SimWs* w, int lane, const double* __restrict__ payload, const double* __restrict__ wrench) {
-  RbdWs* ws = &w->rb; const int body = lane == 0 ? mdl->ee_body : 0;
-  double R[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) R[i] = ws->R[body][i];
-  double po[3] = {0.0, 0.0, 0.0}; if (lane == 0) matvec3(R, mdl->ee_p, po);
-  po[0] += ws->p[body][0]; po[1] += ws->p[body][1]; po[2] += ws->p[body][2];   // frame origin (world)
-  if (payload) {
-    const double m = payload[0]; const double ol[3] = {payload[1], payload[2], payload[3]}; double ob[3] = {ol[0], ol[1], ol[2]};
-    if (lane == 0) matvec3(mdl->ee_R, ol, ob);                                    // offset in the body's axes
-    double c[3]; matvec3(R, ob, c); c[0] += po[0]; c[1] += po[1]; c[2] += po[2];   // point mass position (world)
-    const double cc = dot3(c, c);
-    double I[10] = {m, m * c[0], m * c[1], m * c[2], m * (cc - c[0] * c[0]), -m * c[0] * c[1], -m * c[0] * c[2], m * (cc - c[1] * c[1]), -m * c[1] * c[2], m * (cc - c[2] * c[2])};
-    double acc[6]; for (int i = 0; i < 6; ++i) acc[i] = ws->A[body][i]; acc[5] += 9.81;
-    double f1[6], mom[6]; inertia_apply(I, acc, f1); inertia_apply(I, ws->V[body], mom);
-    const double* wv = ws->V[body]; const double* vv = ws->V[body] + 3;
-    double t1[3], t2[3]; cross3(wv, mom, t1); cross3_add(vv, mom + 3, t1); cross3(wv, mom + 3, t2);   // V x* [n; f] = [w x n + v x f; w x f]
-    double* Ic = ws->Ic[body]; double* F = ws->F[body];
-#pragma unroll
-    for (int i = 0; i < 10; ++i) Ic[i] += I[i];
-    F[0] += f1[0] + t1[0]; F[1] += f1[1] + t1[1]; F[2] += f1[2] + t1[2]; F[3] += f1[3] + t2[0]; F[4] += f1[4] + t2[1]; F[5] += f1[5] + t2[2];
-  }
+  RbdWs* ws = &w->rb; double R[9], po[3]; const int body = payload_frame(mdl, ws, lane, R, po);   // po: frame origin (world)
+  if (payload) payload_add(mdl, ws, lane, body, R, po, payload, true);
   if (wrench) {
     const double f[3] = {wrench[0], wrench[1], wrench[2]}; double* W = w->W[lane];
     cross3(po, f, W); W[0] += wrench[3]; W[1] += wrench[4]; W[2] += wrench[5]; W[3] = f[0]; W[4] = f[1]; W[5] = f[2];

@@ -18,7 +18,7 @@
 // primal active set on the step.  The cascade optimum is basis independent, so the result equals the
 // reference's wherever that optimum is unique (DESIGN.md §WBC).
 #include "dev_common.cuh"
-#include "rbd.cuh"
+#include "payload.cuh"
 #include "wlinalg.cuh"
 
 namespace qmb {
@@ -307,7 +307,10 @@ __device__ int solve_level(WbcSmem& sm, const IneqCtx& ic, int rows, int off, in
 __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevModel* __restrict__ mdl, int b0, int B, const double* __restrict__ x_des, const double* __restrict__ u_des,
                                                                    const double* __restrict__ rbd_meas, const int32_t* __restrict__ mode_in, const double* __restrict__ period_in,
                                                                    const double* __restrict__ time_in, double* __restrict__ input_last, int variant,
-                                                                   double* __restrict__ cmd_out, int32_t* __restrict__ status_out, int32_t* __restrict__ diag_out) {
+                                                                   double* __restrict__ cmd_out, int32_t* __restrict__ status_out, int32_t* __restrict__ diag_out,
+                                                                   const double* __restrict__ srbd, const double* __restrict__ payload) {
+  // srbd [B][SRBD_DBL] / payload [B][8]: the robot's model payload (qmb200_set_model_payload) - its SRBD constants and the point masses the rigid-body passes add
+  // (payload.cuh); both NULL without one (the same for the whole grid)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = b0 + blockIdx.x * (int)(blockDim.x >> 5) + warp;   // robots per CTA = warps per CTA, chosen at launch (the warps of a CTA never synchronise with each other)
@@ -335,6 +338,7 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   RbdWs* ws = &sm.qp.za.rbd; EeWs& ee = sm.qp.ah.ee;   // the end-effector block sits outside the rigid-body overlay
   rbd_kinematics<true>(mdl, sm.q, sm.v, ws, lane);
   rbd_inertias(mdl, ws, lane, 1);
+  if (payload) { if (lane < 2) payload_load(mdl, ws, lane, payload + (size_t)b * 8 + 4 * lane, true); __syncwarp(); }   // lane 0: [m_ee, o_ee], lane 1: [m_base, o_base]
   rbd_accumulate(mdl, ws, lane, true);
   rbd_mass_matrix_nle(mdl, ws, sm.M, LDM, sm.nle, lane);
   for (int f = 0; f < 4; ++f) {
@@ -362,17 +366,19 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   if (lane < NU) input_last[(size_t)b * NU + lane] = udes[lane];
   double A22inv[9], A12[9];   // SRBD blocks at qDesired (kept in lane 0's registers; bound BEFORE dccrba in the reference)
   if (lane == 0) {
+    const SrbdConst* sc = srbd_of(mdl, srbd, b);
     double R[9], T[9]; rot_zyx(sm.qd[3], sm.qd[4], sm.qd[5], R); euler_rate_map(sm.qd[3], sm.qd[4], T);
-    double c[3]; matvec3(R, mdl->c_nom, c);
-    double RI[9], RIRt[9], A22[9]; matmul3(R, mdl->I_nom, RI); matmul3_nt(RI, R, RIRt); matmul3(RIRt, T, A22); inv3(A22, A22inv);
-    const double Sx[9] = {0, -c[2], c[1], c[2], 0, -c[0], -c[1], c[0], 0}; double ST[9]; matmul3(Sx, T, ST); for (int i = 0; i < 9; ++i) A12[i] = mdl->total_mass * ST[i];
-    double ha[3] = {mdl->total_mass * xdes[3], mdl->total_mass * xdes[4], mdl->total_mass * xdes[5]}, ed[3]; matvec3(A22inv, ha, ed);
+    double c[3]; matvec3(R, sc->c_nom, c);
+    double RI[9], RIRt[9], A22[9]; matmul3(R, sc->I_nom, RI); matmul3_nt(RI, R, RIRt); matmul3(RIRt, T, A22); inv3(A22, A22inv);
+    const double Sx[9] = {0, -c[2], c[1], c[2], 0, -c[0], -c[1], c[0], 0}; double ST[9]; matmul3(Sx, T, ST); for (int i = 0; i < 9; ++i) A12[i] = sc->m * ST[i];
+    double ha[3] = {sc->m * xdes[3], sc->m * xdes[4], sc->m * xdes[5]}, ed[3]; matvec3(A22inv, ha, ed);
     double t[3]; matvec3(A12, ed, t);
-    for (int a = 0; a < 3; ++a) { sm.vd[a] = xdes[a] - t[a] / mdl->total_mass; sm.vd[3 + a] = ed[a]; }
+    for (int a = 0; a < 3; ++a) { sm.vd[a] = xdes[a] - t[a] / sc->m; sm.vd[3 + a] = ed[a]; }
   }
   __syncwarp();
   rbd_kinematics<true>(mdl, sm.qd, sm.vd, ws, lane);
   rbd_inertias(mdl, ws, lane, 2);            // bias forces WITHOUT gravity: sum = dAg * v about the origin
+  if (payload) { if (lane < 2) payload_load(mdl, ws, lane, payload + (size_t)b * 8 + 4 * lane, false); __syncwarp(); }
   rbd_accumulate(mdl, ws, lane, true);
   // Aj * jointAccel: sum_j (Ic_{j+1} S_j) qdd_j  (full-model centroidal momentum matrix columns, after dccrba)
   double Phi[6] = {0, 0, 0, 0, 0, 0};
@@ -389,15 +395,16 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
     double vel[3], acc[3]; point_vel_acc(ws, body, pw, vel, acc); for (int a = 0; a < 3; ++a) { ee.ee_d_pos[a] = pw[a]; ee.ee_d_vel[a] = vel[a]; }
     matmul3(ws->R[body], mdl->ee_R, ee.ee_d_rot);
     // centroidalMomentumRate = m*getNormalizedCentroidalMomentumRate(u) [true COM] - dAg v - Aj qdd_j ; baseAcc = AbInv(SRBD) * that
+    const SrbdConst* sc = srbd_of(mdl, srbd, b);
     const double mt = ws->Ic[0][0]; const double com[3] = {ws->Ic[0][1] / mt, ws->Ic[0][2] / mt, ws->Ic[0][3] / mt};
-    double lin[3] = {0, 0, -9.81 * mdl->total_mass}, ang[3] = {0, 0, 0};
+    double lin[3] = {0, 0, -9.81 * sc->m}, ang[3] = {0, 0, 0};
     for (int f = 0; f < 4; ++f) { const double* F = sm.fdes + 3 * f; const double r[3] = {sm.fpos_d[3 * f] - com[0], sm.fpos_d[3 * f + 1] - com[1], sm.fpos_d[3 * f + 2] - com[2]}; lin[0] += F[0]; lin[1] += F[1]; lin[2] += F[2]; cross3_add(r, F, ang); }
     // spatial force about the origin → about the COM: n_com = nO - com x f
     const double* Fb = ws->F[0]; double cf[3]; cross3(com, Fb + 3, cf);
     double cp[3]; cross3(com, Phi + 3, cp);
     for (int a = 0; a < 3; ++a) { lin[a] -= Fb[3 + a] + Phi[3 + a]; ang[a] -= (Fb[a] - cf[a]) + (Phi[a] - cp[a]); }
     double ed[3]; matvec3(A22inv, ang, ed); double t[3]; matvec3(A12, ed, t);
-    for (int a = 0; a < 3; ++a) { sm.base_acc[a] = (lin[a] - t[a]) / mdl->total_mass; sm.base_acc[3 + a] = ed[a]; }
+    for (int a = 0; a < 3; ++a) { sm.base_acc[a] = (lin[a] - t[a]) / sc->m; sm.base_acc[3 + a] = ed[a]; }
   }
   __syncwarp();
 
@@ -470,14 +477,14 @@ static_assert(sizeof(WbcSmem) * WBC_WARPS <= 227 * 1024, "WBC shared-memory budg
 size_t wbc_smem_bytes() { return sizeof(WbcSmem) * WBC_WARPS; }
 
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
-                       double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0, int b1, int32_t* diag) {
+                       double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0, int b1, int32_t* diag, const double* srbd, const double* payload) {
   if (b1 < 0) b1 = B; if (b1 <= b0) return;
   // Eight robots per CTA, one CTA per SM (8 x 28 KB of shared memory: the same 227 KB budget per block on H100).  Smaller CTAs would even out the per-CTA tail, but
   // the kernel is ~24 k SASS instructions (sm_90a build) and the warps of one CTA run in phase and share the instruction cache; a batch of one wave takes the time of its slowest
   // robot whatever the CTA shape.
   const int nb = b1 - b0; const int wpc = WBC_WARPS;
   const int grid = (nb + wpc - 1) / wpc;
-  wbc_update_kernel<<<grid, 32 * wpc, sizeof(WbcSmem) * wpc, stream>>>(mdl, b0, b1, x_des, u_des, rbd, mode, period, time, input_last, variant, cmd, status, diag);
+  wbc_update_kernel<<<grid, 32 * wpc, sizeof(WbcSmem) * wpc, stream>>>(mdl, b0, b1, x_des, u_des, rbd, mode, period, time, input_last, variant, cmd, status, diag, srbd, payload);
 }
 
 // cudaFuncSetAttribute is per device: called from qmb200_create after cudaSetDevice (one handle per GPU, several handles / devices per process allowed)

@@ -356,6 +356,19 @@ class Solver:
         self._chk(self.lib.qmb200_sim_get_robot_params(self.h, _p(mu), _p(pl), C.byref(mask)), "qmb200_sim_get_robot_params")
         return dict(friction_mu=mu if mask.value & 1 else None, payload=pl if mask.value & 2 else None)
 
+    def set_model_payload(self, payload=None):
+        """The controller's model payload [B, 8] (layout _lib.PAYLOAD_LAYOUT): what the MPC and the WBC believe each robot carries, as if its URDF had a
+        fixed link with the point mass at o_ee in the end-effector frame and one at o_base in the base frame.  Independent of the plant's
+        sim_set_robot_params.  None clears it.  Synchronous."""
+        pl = None if payload is None else _f64(payload, (self.batch, 8))
+        self._chk(self.lib.qmb200_set_model_payload(self.h, _p(pl)), "qmb200_set_model_payload")
+
+    def get_model_payload(self):
+        """→ the model payload [B, 8], or None when none is set."""
+        pl = np.zeros((self.batch, 8)); is_set = C.c_int32()
+        self._chk(self.lib.qmb200_get_model_payload(self.h, _p(pl), C.byref(is_set)), "qmb200_get_model_payload")
+        return pl if is_set.value else None
+
     def sim_standing_state(self, xy_yaw):
         """Nominal standing configuration at the given base (x, y, yaw) rows → (q[n,24], v[n,24])."""
         xy = _f64(xy_yaw).reshape(-1, 3); n = xy.shape[0]; q = np.zeros((n, 24)); v = np.zeros((n, 24))

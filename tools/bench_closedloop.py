@@ -9,7 +9,9 @@ deviation from the initial pose, as percentiles over the robots) of this project
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
 gains "vary": the quality per condition bin of each axis (fallen robots, base distance, end-effector deviation).  The controller is not told about
-any of it.
+any of it, unless --model-payload plant sets the controller's model payload to the plant's (closed_loop.run(model_payload="plant")): the timed run
+and the bins are then those of the told controller, and "vary" gains "payload_kg_not_told", the payload bins of the same sweep with the controller
+not told, from one more (untimed) run.
 """
 import argparse
 import json
@@ -38,6 +40,7 @@ def main():
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
     ap.add_argument("--gait", default="trot"); ap.add_argument("--vx", type=float, default=0.3)
     ap.add_argument("--vary", action="store_true", help="per-robot sweep of EE payload, floor friction and a lateral base push")
+    ap.add_argument("--model-payload", choices=["plant"], help="tell the controller the plant's payload (its model payload, Solver.set_model_payload)")
     args = ap.parse_args()
     import torch
     import qm_control_b200 as q
@@ -54,7 +57,8 @@ def main():
         pl = np.zeros((B, 8)); pl[:, 0] = bins["payload_kg"][idx["payload_kg"]]
         w = np.zeros((B, 12)); w[:, 1] = bins["push_N"][idx["push_N"]]
         kw = dict(payload=pl, friction_mu=bins["mu"][idx["mu"]], pushes=(np.full(B, 0.4), np.full(B, 0.1), w))
-    closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw)   # warm-up run of the same length
+    told = dict(model_payload=args.model_payload) if args.model_payload else {}
+    closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told)   # warm-up run of the same length
     pairs = []
 
     def sim_timer(start):
@@ -63,23 +67,33 @@ def main():
         else:
             pairs[-1][1].record()
     torch.cuda.synchronize(dev); t0 = time.perf_counter()
-    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer, **kw)
+    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer, **kw, **told)
     torch.cuda.synchronize(dev); wall = time.perf_counter() - t0
     sim_ms = float(np.sum([a.elapsed_time(b) for a, b in pairs])); per_call = sim_ms / len(pairs)
-    dist = np.linalg.norm(r["base"][-1, :, :2] - r["start_base"][:, :2], axis=1)
-    dpos = np.max(np.linalg.norm(r["ee"][:, :, :3] - r["start_ee"][None, :, :3], axis=2), axis=0) * 1e3
-    dot = np.clip(np.abs(np.sum(r["ee"][:, :, 3:] * r["start_ee"][None, :, 3:], axis=2)), 0.0, 1.0); dang = np.max(np.degrees(2.0 * np.arccos(dot)), axis=0)
     pct = lambda a: {"p50": float(np.percentile(a, 50)), "p95": float(np.percentile(a, 95)), "max": float(np.max(a))}
+
+    def quality(r):
+        dist = np.linalg.norm(r["base"][-1, :, :2] - r["start_base"][:, :2], axis=1)
+        dpos = np.max(np.linalg.norm(r["ee"][:, :, :3] - r["start_ee"][None, :, :3], axis=2), axis=0) * 1e3
+        dot = np.clip(np.abs(np.sum(r["ee"][:, :, 3:] * r["start_ee"][None, :, 3:], axis=2)), 0.0, 1.0); dang = np.max(np.degrees(2.0 * np.arccos(dot)), axis=0)
+        return dist, dpos, dang
+
+    def vary_bins(r, axis):
+        dist, dpos, dang = quality(r); base = r["base"]
+        fallen = ~(np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3))
+        return [{"value": float(val), "robots": int(np.sum(idx[axis] == i)), "fallen": int(np.sum(fallen[idx[axis] == i])),
+                 "base_distance_m_p50": float(np.percentile(dist[idx[axis] == i], 50)),
+                 "ee_max_pos_dev_mm": pct(dpos[idx[axis] == i]), "ee_max_ori_dev_deg_p50": float(np.percentile(dang[idx[axis] == i], 50))}
+                for i, val in enumerate(bins[axis])]
+    dist, dpos, dang = quality(r)
     name, limit = card()
     extra = {}
     if args.vary:
-        base = r["base"]
-        fallen = ~(np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3))
         extra["vary"] = {"label": "per-robot sweep; fallen = min base z <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite", "push": "lateral +y base force for 0.1 s from 0.4 s",
-                         "bins": {axis: [{"value": float(val), "robots": int(np.sum(idx[axis] == i)), "fallen": int(np.sum(fallen[idx[axis] == i])),
-                                          "base_distance_m_p50": float(np.percentile(dist[idx[axis] == i], 50)),
-                                          "ee_max_pos_dev_mm": pct(dpos[idx[axis] == i]), "ee_max_ori_dev_deg_p50": float(np.percentile(dang[idx[axis] == i], 50))}
-                                         for i, val in enumerate(bins[axis])] for axis in bins}}
+                         "bins": {axis: vary_bins(r, axis) for axis in bins}}
+        if args.model_payload:
+            extra["vary"]["model_payload"] = "the controller is told the plant's payload (bins); payload_kg_not_told: the same sweep, controller not told"
+            extra["vary"]["payload_kg_not_told"] = vary_bins(closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw), "payload_kg")
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
@@ -88,7 +102,7 @@ def main():
                                   "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(r["status"], axis=0))),
                                   "min_base_height_m": float(np.min(r["base"][:, :, 2])), "max_abs_roll_pitch_rad": float(np.max(np.abs(r["base"][:, :, 4:6])))},
                       "config": {"workload": "closed loop: %s, cmd_vel %.2f m/s, MPC 100 Hz / WBC 500 Hz / plant 1 kHz (4 substeps), 9 ms command delay" % (args.gait, args.vx),
-                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length"}, **extra}))
+                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length", **({"model_payload": args.model_payload} if args.model_payload else {})}, **extra}))
 
 
 if __name__ == "__main__":
