@@ -27,6 +27,12 @@ using namespace qmb;
 
 static thread_local std::string g_create_error;
 
+// A per-robot array the kernels read, `width` doubles per robot: the host copy (empty = not set) and its device copy, allocated on the first set.
+struct RobotArray {
+  int width; std::vector<double> host; double* d = nullptr;
+  const double* dev() const { return host.empty() ? nullptr : d; }
+};
+
 struct qmb200_handle {
   HostModel hm;
   DevModel* d_model = nullptr;
@@ -34,9 +40,10 @@ struct qmb200_handle {
   cudaStream_t stream = nullptr;
   std::string err, task_file;   // task_file: qmb200_mpc_set_solver re-reads the sqp{} / ipm{} / ddp{} block
   int64_t launches = 0;
-  // staging for the host-pointer API
-  double *d_xdes = nullptr, *d_udes = nullptr, *d_rbd = nullptr, *d_period = nullptr, *d_time = nullptr, *d_cmd = nullptr, *d_input_last = nullptr, *d_teval = nullptr;
-  int32_t *d_mode = nullptr, *d_status = nullptr, *d_wbc_diag = nullptr;   // d_wbc_diag: per-robot WBC iteration counts (qmb200_wbc_get_diagnostics), kept out of the status word
+  // intermediates of the tick and update chains (policy evaluation → WBC → control law), WBC state, and the update chain's safety word
+  double *d_xdes = nullptr, *d_udes = nullptr, *d_input_last = nullptr;
+  int32_t *d_mode = nullptr, *d_wbc_diag = nullptr, *d_safety = nullptr;   // d_wbc_diag: per-robot WBC iteration counts (qmb200_wbc_get_diagnostics), kept out of the status word
+  char* stage = nullptr; size_t stage_bytes = 0;   // device arena of the host-pointer entry points (Staging)
   MpcBuffers mpc;   // device buffers of the MPC path (kernels/mpc_api.cuh)
   std::vector<void*> allocs;
   bool profiling = false; cudaEvent_t ev[8] = {nullptr};   // [0..4] MPC kernels, [5..6] policy / wbc brackets, [7] flow kernel | LQ kernel
@@ -44,18 +51,12 @@ struct qmb200_handle {
   // tick pipeline: the batch is cut into `chunks` robot ranges, each running its MPC → policy → WBC chain on its own stream, so that
   // kernels with different bottlenecks (LQ: instruction latency, Riccati: shared-memory bandwidth, WBC) share the SMs
   static constexpr int MAX_CHUNKS = 8;
-  // controller-side constants and staging (capi_ctrl.inc)
-  TargetParams target_prm{}; ControlLawParams law_prm{0, 0.0, 0.5};
-  bool c_ready = false; double *c_tobs = nullptr, *c_xobs = nullptr, *c_jcmd = nullptr, *c_armpos = nullptr, *c_lasttime = nullptr, *c_cmd7 = nullptr, *c_ee = nullptr, *c_lastee = nullptr,
-                               *c_jpos = nullptr, *c_jvel = nullptr, *c_effort = nullptr, *c_ttimes = nullptr, *c_tstates = nullptr; int32_t *c_status = nullptr, *c_ntarget = nullptr;
+  TargetParams target_prm{}; ControlLawParams law_prm{0, 0.0, 0.5};   // controller-side constants (capi_ctrl.inc)
   double hw_delay = 0.0; double *hw_ring_cmd = nullptr, *hw_ring_stamp = nullptr; int32_t* hw_ring_state = nullptr;   // QMHWSim command-delay FIFO
   void* comm = nullptr; int comm_ranks = 0, comm_rank = 0; double* d_send = nullptr;   // NCCL communicator of this handle (capi_comm.inc) and the packed torque rows
-  SimParams sim_prm{}; double *s_effort = nullptr, *s_q = nullptr, *s_v = nullptr, *s_rbd = nullptr; int32_t *s_contact = nullptr, *s_status = nullptr;   // plant step (capi_sim.inc)
-  std::vector<double> r_mu, r_payload; double *s_mu = nullptr, *s_payload = nullptr, *s_wrench = nullptr;   // per-robot plant variation: host copy (empty = not set), device copy
-  // the controller's model payload (qmb200_set_model_payload): host copies of the payload rows and of the robots' SRBD constants (empty = not set), device copies
-  std::vector<double> m_payload, m_srbd; double *d_mpayload = nullptr, *d_srbd = nullptr;
-  const double* srbd_dev() const { return m_payload.empty() ? nullptr : d_srbd; }
-  const double* mpayload_dev() const { return m_payload.empty() ? nullptr : d_mpayload; }
+  SimParams sim_prm{};   // plant step (capi_sim.inc)
+  RobotArray mu{1}, payload{8};   // per-robot plant variation (qmb200_sim_set_robot_params)
+  RobotArray mpayload{8}, srbd{SRBD_DBL};   // the controller's model payload (qmb200_set_model_payload) and the robots' SRBD constants it gives
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
 
@@ -63,11 +64,86 @@ namespace {
 template <class T> bool dalloc(qmb200_handle* h, T** p, size_t count) {
   void* q = nullptr; cudaError_t e = cudaMalloc(&q, count * sizeof(T));
   if (e != cudaSuccess) { h->err = std::string("cudaMalloc failed: ") + cudaGetErrorString(e); return false; }
-  cudaMemsetAsync(q, 0, count * sizeof(T), h->stream); h->allocs.push_back(q); *p = static_cast<T*>(q); return true;   // zeroed in stream order with the handle's work (lazy allocators synchronise once, see ctrl_alloc)
+  cudaMemsetAsync(q, 0, count * sizeof(T), h->stream); h->allocs.push_back(q); *p = static_cast<T*>(q); return true;   // zeroed in stream order with the handle's work
 }
 SimParams default_sim_params();   // capi_sim.inc
 int fail(qmb200_handle* h, const std::string& msg) { if (h) h->err = msg; else g_create_error = msg; return -1; }
 #define QMB_CUDA(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(h, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
+
+// The model a config describes: the default WBC gains unless a gains file is given, time_horizon / dt overridden when > 0.
+HostModel config_model(const qmb200_config* cfg) {
+  HostModel hm = build_host_model(cfg->task_file, cfg->urdf_file, cfg->reference_file, cfg->wbc_gains_file ? cfg->wbc_gains_file : "");
+  if (cfg->time_horizon > 0) hm.dev.time_horizon = cfg->time_horizon;
+  if (cfg->dt > 0) hm.dev.dt = cfg->dt;
+  return hm;
+}
+// Stream-ordered update of the replicated constants from h->hm.dev: kernels already queued keep the old values, later ones see the new.
+int push_model(qmb200_handle* h) {
+  QMB_CUDA(h, cudaMemcpyAsync(h->d_model, &h->hm.dev, sizeof(DevModel), cudaMemcpyHostToDevice, h->stream)); QMB_CUDA(h, cudaStreamSynchronize(h->stream)); return 0;
+}
+
+// Sets each array to `rows` ([B][width]; NULL clears it).  Work still queued on any stream may read the current device copies, so the copy waits
+// for the device.  On failure the host copies, which say what is set, stay unchanged.
+struct RobotRows { RobotArray* a; const double* rows; };
+int set_robot_arrays(qmb200_handle* h, std::initializer_list<RobotRows> sets) {
+  const size_t B = (size_t)h->B;
+  QMB_CUDA(h, cudaSetDevice(h->device));
+  for (const RobotRows& s : sets) if (s.rows && !s.a->d && !dalloc(h, &s.a->d, B * s.a->width)) return -4;
+  QMB_CUDA(h, cudaDeviceSynchronize());
+  for (const RobotRows& s : sets) if (s.rows) QMB_CUDA(h, cudaMemcpy(s.a->d, s.rows, B * s.a->width * 8, cudaMemcpyHostToDevice));
+  for (const RobotRows& s : sets) { if (s.rows) s.a->host.assign(s.rows, s.rows + B * s.a->width); else s.a->host.clear(); }
+  return 0;
+}
+
+// A host-pointer entry point is its _dev twin on the handle's stream, with the caller's arrays staged through one device arena per handle:
+// in() copies an array to the device, inout() also copies it back after the call, out() only copies it back.  done(rc) queues the copies back,
+// waits for the stream and reports the first CUDA error; when the _dev call failed it returns that call's code and copies nothing back.
+// Every array declared out must be written in full by the kernels, since the arena holds whatever the previous call left there.
+class Staging {
+ public:
+  // The widest entry point, qmb200_control_law, stages 242 doubles and one int32 per robot (qmb200_update: 238 and one); each of its at most
+  // STAGE_SLICES slices starts on a 256-byte boundary, the alignment cudaMalloc gives.
+  static constexpr size_t ROBOT_BYTES = 243 * 8, ALIGN = 256, STAGE_SLICES = 10;
+  explicit Staging(qmb200_handle* h) : h_(h) {}
+  int open() {
+    QMB_CUDA(h_, cudaSetDevice(h_->device));
+    if (!h_->stage) {
+      const size_t bytes = (size_t)h_->B * ROBOT_BYTES + STAGE_SLICES * ALIGN;
+      if (!dalloc(h_, &h_->stage, bytes)) return -4;   // zeroed on h->stream, the only stream that uses the arena
+      h_->stage_bytes = bytes;
+    }
+    return 0;
+  }
+  template <class T> const T* in(const T* src, size_t n) {
+    if (!src) return nullptr;
+    T* d = slice<T>(n); note(cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, h_->stream)); return d;
+  }
+  template <class T> T* inout(T* p, size_t n) { T* d = const_cast<T*>(in<T>(p, n)); back_.push_back({p, d, n * sizeof(T)}); return d; }
+  template <class T> T* out(T* p, size_t n) { T* d = slice<T>(n); back_.push_back({p, d, n * sizeof(T)}); return d; }
+  int done(int rc) {
+    if (rc) return rc;
+    for (const Back& b : back_) note(cudaMemcpyAsync(b.host, b.dev, b.bytes, cudaMemcpyDeviceToHost, h_->stream));
+    note(cudaStreamSynchronize(h_->stream));
+    return err_.empty() ? 0 : fail(h_, err_);
+  }
+
+ private:
+  struct Back { void* host; const void* dev; size_t bytes; };
+  qmb200_handle* h_; size_t used_ = 0; std::vector<Back> back_; std::string err_;
+  void note(cudaError_t e) { if (e != cudaSuccess && err_.empty()) err_ = std::string("staging copy: ") + cudaGetErrorString(e); }
+  template <class T> T* slice(size_t n) {
+    const size_t at = used_, bytes = n * sizeof(T);
+    if (at + bytes > h_->stage_bytes) { if (err_.empty()) err_ = "staging arena too small"; return reinterpret_cast<T*>(h_->stage); }
+    used_ = (at + bytes + ALIGN - 1) / ALIGN * ALIGN; return reinterpret_cast<T*>(h_->stage + at);
+  }
+};
+
+// WbcBase::update of robots [b0, b1) with the handle's model, WBC state (input_last, diagnostics) and model payload
+void wbc_launch(qmb200_handle* h, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time, double* cmd,
+                int32_t* status, cudaStream_t s, int b0 = 0, int b1 = -1) {
+  launch_wbc_update(h->d_model, h->B, x_des, u_des, rbd, mode, period, time, h->d_input_last, h->variant, cmd, status, s, b0, b1, h->d_wbc_diag, h->srbd.dev(), h->mpayload.dev());
+  h->launches += 1;
+}
 }  // namespace
 
 extern "C" {
@@ -78,15 +154,13 @@ int qmb200_create(const qmb200_config* cfg, qmb200_handle** out) {
   if (cfg->batch < 1) return fail(nullptr, "qmb200_create: batch must be >= 1");
   qmb200_handle* h = new qmb200_handle();
   try {
-    h->hm = build_host_model(cfg->task_file, cfg->urdf_file, cfg->reference_file, cfg->wbc_gains_file ? cfg->wbc_gains_file : "");
+    h->hm = config_model(cfg);
     // constants of the target publisher node (QmTargetTrajectoriesPublisher_node.cpp:225-229)
     InfoFile ref(cfg->reference_file), task(cfg->task_file);
     h->target_prm.com_height = ref.number("comHeight"); h->target_prm.target_displacement_velocity = ref.number("targetDisplacementVelocity");
     h->target_prm.target_rotation_velocity = ref.number("targetRotationVelocity"); h->target_prm.time_to_target = task.number("mpc.timeHorizon");
     for (int j = 0; j < NJ; ++j) h->target_prm.default_joint_state[j] = h->hm.default_joint_state[j];
   } catch (const std::exception& e) { g_create_error = e.what(); delete h; return -2; }
-  if (cfg->time_horizon > 0) h->hm.dev.time_horizon = cfg->time_horizon;
-  if (cfg->dt > 0) h->hm.dev.dt = cfg->dt;
   h->task_file = cfg->task_file;
   h->sim_prm = default_sim_params();
   h->B = cfg->batch; h->variant = cfg->wbc_variant; h->device = cfg->device; h->law_prm.variant = cfg->wbc_variant == QMB200_WBC_HIERARCHICAL_MPC ? 1 : 0;
@@ -99,12 +173,11 @@ int qmb200_create(const qmb200_config* cfg, qmb200_handle** out) {
   // kernel attributes are per device: set them for THIS handle's device (a process may hold handles on several GPUs)
   if (wbc_configure_device() != 0 || mpc_configure_device() != 0) { g_create_error = std::string("qmb200_create: cudaFuncSetAttribute failed: ") + cudaGetErrorString(cudaGetLastError()); qmb200_destroy(h); return -3; }
   const size_t B = (size_t)h->B;
-  bool ok = dalloc(h, &h->d_model, 1) && dalloc(h, &h->d_xdes, B * NX) && dalloc(h, &h->d_udes, B * NU) && dalloc(h, &h->d_rbd, B * QMB200_RBD) && dalloc(h, &h->d_period, B) &&
-            dalloc(h, &h->d_time, B) && dalloc(h, &h->d_cmd, B * QMB200_CMD) && dalloc(h, &h->d_input_last, B * NU) && dalloc(h, &h->d_mode, B) && dalloc(h, &h->d_status, B) && dalloc(h, &h->d_teval, B) && dalloc(h, &h->d_wbc_diag, B);
+  bool ok = dalloc(h, &h->d_model, 1) && dalloc(h, &h->d_xdes, B * NX) && dalloc(h, &h->d_udes, B * NU) && dalloc(h, &h->d_input_last, B * NU) && dalloc(h, &h->d_mode, B) &&
+            dalloc(h, &h->d_wbc_diag, B) && dalloc(h, &h->d_safety, B) && dalloc(h, &h->d_send, B * NJ);
   if (ok) { std::string merr; ok = mpc_alloc(h->mpc, h->B, h->nmax, merr, h->allocs, h->stream); if (!ok) h->err = merr; }
   if (!ok) { g_create_error = h->err; qmb200_destroy(h); return -4; }
-  cudaMemcpyAsync(h->d_model, &h->hm.dev, sizeof(DevModel), cudaMemcpyHostToDevice, h->stream);
-  if (cudaStreamSynchronize(h->stream) != cudaSuccess) { g_create_error = std::string("qmb200_create: ") + cudaGetErrorString(cudaGetLastError()); qmb200_destroy(h); return -4; }   // buffers zeroed, constants resident before any (user-stream) launch
+  if (push_model(h)) { g_create_error = "qmb200_create: " + h->err; qmb200_destroy(h); return -4; }   // buffers zeroed, constants resident before any (user-stream) launch
   *out = h; return 0;
 }
 
@@ -124,8 +197,7 @@ const char* qmb200_last_error(const qmb200_handle* h) { return h ? h->err.c_str(
 int64_t qmb200_debug_model_blob(const qmb200_config* cfg, void* out, int64_t capacity) {
   if (!cfg || !cfg->task_file || !cfg->urdf_file || !cfg->reference_file) { g_create_error = "qmb200_debug_model_blob: task/urdf/reference file required"; return -1; }
   try {
-    HostModel hm = build_host_model(cfg->task_file, cfg->urdf_file, cfg->reference_file, cfg->wbc_gains_file ? cfg->wbc_gains_file : "");
-    if (cfg->time_horizon > 0) hm.dev.time_horizon = cfg->time_horizon; if (cfg->dt > 0) hm.dev.dt = cfg->dt;
+    const HostModel hm = config_model(cfg);
     if (out && capacity >= (int64_t)sizeof(DevModel)) std::memcpy(out, &hm.dev, sizeof(DevModel));
     return (int64_t)sizeof(DevModel);
   } catch (const std::exception& e) { g_create_error = e.what(); return -2; }
@@ -135,7 +207,7 @@ int64_t qmb200_debug_model_blob(const qmb200_config* cfg, void* out, int64_t cap
 static_assert(SRBD_DBL == QMB200_SRBD, "per-robot SRBD block of include/qmb200.h");
 }  // extern "C"
 namespace {
-// payload rows [n][8] as qmb200_sim_set_robot_params accepts them: finite, masses >= 0; "" when valid
+// payload rows [n][8] as qmb200_sim_set_robot_params and qmb200_set_model_payload accept them: finite, masses >= 0; "" when valid
 std::string payload_error(const double* payload, size_t n, const char* who) {
   for (size_t b = 0; b < n; ++b) {
     const double* p = payload + 8 * b;
@@ -155,18 +227,13 @@ int qmb200_set_model_payload(qmb200_handle* h, const double* payload) {
   if (!h) return -1; const size_t B = (size_t)h->B;
   if (payload) { const std::string e = payload_error(payload, B, "qmb200_set_model_payload"); if (!e.empty()) return fail(h, e); }
   std::vector<double> srbd; if (payload) { srbd.resize(B * SRBD_DBL); srbd_rows(h->hm, payload, B, srbd.data()); }
-  QMB_CUDA(h, cudaSetDevice(h->device));
-  if (payload && !h->d_srbd && !(dalloc(h, &h->d_srbd, B * SRBD_DBL) && dalloc(h, &h->d_mpayload, B * 8))) return -4;
-  // work still queued on any stream may read the current arrays: the copy waits for the device
-  QMB_CUDA(h, cudaDeviceSynchronize());
-  if (payload) { QMB_CUDA(h, cudaMemcpy(h->d_srbd, srbd.data(), B * SRBD_DBL * 8, cudaMemcpyHostToDevice)); QMB_CUDA(h, cudaMemcpy(h->d_mpayload, payload, B * 64, cudaMemcpyHostToDevice)); }
-  if (payload) { h->m_payload.assign(payload, payload + B * 8); h->m_srbd.swap(srbd); } else { h->m_payload.clear(); h->m_srbd.clear(); }
-  return 0;
+  return set_robot_arrays(h, {{&h->mpayload, payload}, {&h->srbd, payload ? srbd.data() : nullptr}});
 }
 int qmb200_get_model_payload(const qmb200_handle* h, double* payload, int32_t* is_set) {
   if (!h) return -1; const size_t B = (size_t)h->B;
-  if (payload) { if (h->m_payload.empty()) std::memset(payload, 0, B * 64); else std::memcpy(payload, h->m_payload.data(), B * 64); }
-  if (is_set) *is_set = h->m_payload.empty() ? 0 : 1;
+  const std::vector<double>& p = h->mpayload.host;
+  if (payload) { if (p.empty()) std::memset(payload, 0, B * 64); else std::memcpy(payload, p.data(), B * 64); }
+  if (is_set) *is_set = p.empty() ? 0 : 1;
   return 0;
 }
 int qmb200_debug_srbd_constants(const qmb200_config* cfg, int32_t n, const double* payload, double* out) {
@@ -174,8 +241,7 @@ int qmb200_debug_srbd_constants(const qmb200_config* cfg, int32_t n, const doubl
   if (n < 0 || (n > 0 && !out)) { g_create_error = "qmb200_debug_srbd_constants: n must be >= 0 and out non-null"; return -1; }
   if (payload) { const std::string e = payload_error(payload, (size_t)n, "qmb200_debug_srbd_constants"); if (!e.empty()) { g_create_error = e; return -1; } }
   try {
-    HostModel hm = build_host_model(cfg->task_file, cfg->urdf_file, cfg->reference_file, cfg->wbc_gains_file ? cfg->wbc_gains_file : "");
-    srbd_rows(hm, payload, (size_t)n, out);
+    srbd_rows(config_model(cfg), payload, (size_t)n, out);
     return 0;
   } catch (const std::exception& e) { g_create_error = e.what(); return -2; }
 }
@@ -201,24 +267,16 @@ int qmb200_wbc_update_dev(qmb200_handle* h, const double* x_des, const double* u
                           double* cmd, int32_t* status, void* cuda_stream) {
   if (!h) return -1; if (!x_des || !u_des || !rbd || !mode || !period || !time || !cmd || !status) return fail(h, "qmb200_wbc_update_dev: null buffer");
   QMB_CUDA(h, cudaSetDevice(h->device));
-  launch_wbc_update(h->d_model, h->B, x_des, u_des, rbd, mode, period, time, h->d_input_last, h->variant, cmd, status, cuda_stream ? (cudaStream_t)cuda_stream : h->stream, 0, -1, h->d_wbc_diag,
-                    h->srbd_dev(), h->mpayload_dev());
-  h->launches += 1;
+  wbc_launch(h, x_des, u_des, rbd, mode, period, time, cmd, status, cuda_stream ? (cudaStream_t)cuda_stream : h->stream);
   QMB_CUDA(h, cudaGetLastError());
   return 0;
 }
 
 int qmb200_wbc_update(qmb200_handle* h, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time, double* cmd, int32_t* status) {
   if (!h) return -1; if (!x_des || !u_des || !rbd || !mode || !period || !time || !cmd || !status) return fail(h, "qmb200_wbc_update: null buffer");
-  QMB_CUDA(h, cudaSetDevice(h->device));
-  const size_t B = (size_t)h->B; cudaStream_t s = h->stream;
-  QMB_CUDA(h, cudaMemcpyAsync(h->d_xdes, x_des, B * NX * 8, cudaMemcpyHostToDevice, s)); QMB_CUDA(h, cudaMemcpyAsync(h->d_udes, u_des, B * NU * 8, cudaMemcpyHostToDevice, s));
-  QMB_CUDA(h, cudaMemcpyAsync(h->d_rbd, rbd, B * QMB200_RBD * 8, cudaMemcpyHostToDevice, s)); QMB_CUDA(h, cudaMemcpyAsync(h->d_mode, mode, B * 4, cudaMemcpyHostToDevice, s));
-  QMB_CUDA(h, cudaMemcpyAsync(h->d_period, period, B * 8, cudaMemcpyHostToDevice, s)); QMB_CUDA(h, cudaMemcpyAsync(h->d_time, time, B * 8, cudaMemcpyHostToDevice, s));
-  int rc = qmb200_wbc_update_dev(h, h->d_xdes, h->d_udes, h->d_rbd, h->d_mode, h->d_period, h->d_time, h->d_cmd, h->d_status, s); if (rc) return rc;
-  QMB_CUDA(h, cudaMemcpyAsync(cmd, h->d_cmd, B * QMB200_CMD * 8, cudaMemcpyDeviceToHost, s)); QMB_CUDA(h, cudaMemcpyAsync(status, h->d_status, B * 4, cudaMemcpyDeviceToHost, s));
-  QMB_CUDA(h, cudaStreamSynchronize(s));
-  return 0;
+  Staging st(h); if (int rc = st.open()) return rc; const size_t B = (size_t)h->B;
+  return st.done(qmb200_wbc_update_dev(h, st.in(x_des, B * NX), st.in(u_des, B * NU), st.in(rbd, B * QMB200_RBD), st.in(mode, B), st.in(period, B), st.in(time, B),
+                                       st.out(cmd, B * QMB200_CMD), st.out(status, B), h->stream));
 }
 int qmb200_wbc_set_input_last(qmb200_handle* h, const double* input_last) {
   if (!h) return -1; QMB_CUDA(h, cudaSetDevice(h->device));
@@ -245,8 +303,7 @@ int qmb200_wbc_set_gains(qmb200_handle* h, const qmb200_wbc_gains* g) {
   d.base_angular_kp = g->kp_base_angular; d.base_angular_kd = g->kd_base_angular;
   for (int i = 0; i < 6; ++i) { d.arm_joint_kp[i] = g->kp_arm_joint[i]; d.arm_joint_kd[i] = g->kd_arm_joint[i]; }
   for (int i = 0; i < 3; ++i) { d.ee_linear_kp[i] = g->kp_ee_linear[i]; d.ee_linear_kd[i] = g->kd_ee_linear[i]; d.ee_angular_kp[i] = g->kp_ee_angular[i]; d.ee_angular_kd[i] = g->kd_ee_angular[i]; }
-  // stream-ordered update of the replicated constants: kernels already queued keep the old gains, later ones see the new
-  QMB_CUDA(h, cudaMemcpyAsync(h->d_model, &h->hm.dev, sizeof(DevModel), cudaMemcpyHostToDevice, h->stream)); QMB_CUDA(h, cudaStreamSynchronize(h->stream)); return 0;
+  return push_model(h);
 }
 
 // Per-robot WBC diagnostics of the last update on this handle: it0 | it1 << 8 | it2 << 16 | nw << 24 (level-0 semismooth passes, active-set iterations of
@@ -259,7 +316,7 @@ int qmb200_wbc_get_diagnostics(qmb200_handle* h, int32_t* diag) {
 int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32_t active_set_iterations) {
   if (!h) return -1; QMB_CUDA(h, cudaSetDevice(h->device));
   if (level0_passes > 0) h->hm.dev.wbc_iter_cap0 = level0_passes; if (active_set_iterations > 0) h->hm.dev.wbc_iter_cap = active_set_iterations;
-  QMB_CUDA(h, cudaMemcpyAsync(h->d_model, &h->hm.dev, sizeof(DevModel), cudaMemcpyHostToDevice, h->stream)); QMB_CUDA(h, cudaStreamSynchronize(h->stream)); return 0;
+  return push_model(h);
 }
 
 }  // extern "C"
