@@ -223,10 +223,11 @@ int qmb200_hw_set_delay(qmb200_handle* h, double delay);
 
 /* ---- plant: Gazebo's physics step behind QMHWSim (one writeSim → physics step → readSim cycle) plus the contact flags QMHWSim::readSim reports to the
  *      ContactSensorInterface (qm_gazebo/src/QMHWSim.cpp:71-90), batched on the device.  Forward dynamics of the 24-DoF tree with a compliant contact
- *      between each foot's collision sphere and a flat ground plane (this project's contact law, not Gazebo/ODE's: DESIGN.md §4.6).  The caller owns
+ *      between each foot's collision sphere and the ground: a flat plane, or per robot a heightfield tile (qmb200_sim_set_terrain) (this project's
+ *      contact law, not Gazebo/ODE's: DESIGN.md §4.6).  The caller owns
  *      the plant state q[24] = [p_base, euler ZYX, joints], v[24] = dq/dt. */
 typedef struct {
-  double ground_height;        /* plane z = ground_height (m); default 0 */
+  double ground_height;        /* plane z = ground_height (m) under robots without a terrain tile; default 0 */
   double foot_radius;          /* foot collision sphere, centred on the *_FOOT frame (m); default 0.0265 (robot.urdf *_FOOT <collision>) */
   double stiffness;            /* normal force F_n = max(0, stiffness * delta - damping * dz/dt), delta = penetration (N/m); default 1e6 */
   double damping;              /* (N s/m); default 1e3 */
@@ -251,8 +252,8 @@ int qmb200_sim_step_dev(qmb200_handle* h, double duration, const double* effort,
  *   payload[B][8]    layout: [m_ee, o_ee_x, o_ee_y, o_ee_z, m_base, o_base_x, o_base_y, o_base_z]
  *                    two point masses (kg) rigidly attached at o_ee (m, end-effector frame) and o_base (m, base frame); no rotational inertia.
  * These are plant properties only: the controller's model (MPC, WBC) is set apart with qmb200_set_model_payload, so a run can tell the controller the
- * truth, an estimate or nothing (the model mismatch is then the experiment).  qmb200_sim_standing_state ignores the
- * robot params, so a payload shifts the static pre-load of the standing state (by micrometres per kilogram at the default stiffness).
+ * truth, an estimate or nothing (the model mismatch is then the experiment).  qmb200_sim_standing_state ignores friction_mu and payload, so
+ * a payload shifts the static pre-load of the standing state (by micrometres per kilogram at the default stiffness); it does follow the robot terrain.
  * Host arrays, copied to the device; synchronous (waits for the device).  NULL clears that override.  Rejects a non-finite or <= 0 friction_mu,
  * a non-finite payload entry and a negative mass; on rejection the stored values stay unchanged. */
 int qmb200_sim_set_robot_params(qmb200_handle* h, const double* friction_mu /*[B] or NULL*/, const double* payload /*[B][8] or NULL*/);
@@ -267,8 +268,28 @@ int qmb200_sim_step_ext(qmb200_handle* h, double duration, const double* effort 
                         double* v /*[B][24] in-out*/, double* rbd /*[B][55]*/, int32_t* contact /*[B]*/, int32_t* status /*[B]*/);
 int qmb200_sim_step_ext_dev(qmb200_handle* h, double duration, const double* effort, const double* wrench, double* q, double* v, double* rbd, int32_t* contact,
                             int32_t* status, void* cuda_stream);
+/* Per-robot terrain: heightfield tiles under the feet in place of the plane z = ground_height, applied by every qmb200_sim_step(_ext)(_dev) call.
+ * The library holds n_tiles tiles on one grid of nx x ny nodes (both >= 2) with spacing cell (m); heights[n_tiles][ny][nx] are absolute world z (m).
+ * Robot b stands on tile[b] (-1: the plane z = ground_height) whose node (0, 0) lies at world origin[b] = (x, y), so node (i, j) lies at
+ * origin + (i cell, j cell).  At a foot centre (x, y, z) the ground is bilinear in the cell under (x, y), with height H and gradient (gx, gy); outside the
+ * tile the border height continues with zero gradient across the clamped axis.  Contact is against the local tangent plane: s = sqrt(1 + gx^2 + gy^2),
+ * n = (-gx, -gy, 1) / s, penetration delta = (H - (z - r s)) / s, F_n = max(0, stiffness delta - damping v.n) for delta > 0, v_t = v - (v.n) n, friction
+ * as above on v_t; F = F_n n + F_t.  With zero gradient this is the plane law bit for bit, so tile -1 or a constant tile at ground_height changes nothing.
+ * No link other than the feet collides; tiles are not rotated.
+ * qmb200_sim_set_terrain: heights NULL clears the library and with it the robot terrain.  Rejects n_tiles < 1, nx or ny < 2, a non-finite or
+ * non-positive cell, a non-finite height, a library whose byte count overflows, and a library with fewer tiles than a robot references.
+ * qmb200_sim_set_robot_terrain: tile NULL clears the robot terrain (every robot on the plane); rejects a tile outside [-1, n_tiles) and a non-finite origin.
+ * Both are synchronous (they wait for the device); on rejection the stored values stay unchanged. */
+int qmb200_sim_set_terrain(qmb200_handle* h, int32_t n_tiles, int32_t nx, int32_t ny, double cell, const double* heights /*[n_tiles][ny][nx] or NULL: clear*/);
+/* The library: n_tiles = 0 (nx = ny = 0, cell = 0) when none is set; heights [n_tiles][ny][nx] is written when non-NULL.  Any output may be NULL. */
+int qmb200_sim_get_terrain(const qmb200_handle* h, int32_t* n_tiles, int32_t* nx, int32_t* ny, double* cell, double* heights /*or NULL*/);
+int qmb200_sim_set_robot_terrain(qmb200_handle* h, const int32_t* tile /*[B] or NULL: clear*/, const double* origin /*[B][2]*/);
+/* The robot terrain; where none is set tile = -1, origin = 0 and is_set = 0.  Any output may be NULL. */
+int qmb200_sim_get_robot_terrain(const qmb200_handle* h, int32_t* tile /*[B]*/, double* origin /*[B][2]*/, int32_t* is_set);
 /* Host utility: the nominal standing configuration (defaultJointState, base at the given x, y, yaw, zero roll and pitch) with the base height at
- * which the four foot spheres carry m g / 4 each at the static penetration of the current params; v = 0. */
+ * which the four foot spheres carry m g / 4 each at the static penetration of the current params; v = 0.  With robot terrain set n must equal the
+ * batch size and row r stands on robot r's ground: roll and pitch tilt the base onto the plane fitted through the ground heights under the four feet
+ * (a few fixed-point iterations, since the feet move with the tilt), and the base height puts the deepest foot at the static penetration m g / (4 k). */
 int qmb200_sim_standing_state(const qmb200_handle* h, int32_t n, const double* xy_yaw /*[n][3]*/, double* q /*[n][24]*/, double* v /*[n][24]*/);
 
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update

@@ -54,6 +54,7 @@ SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_d
            "qmb200_debug_model_blob", "qmb200_comm_get_unique_id", "qmb200_comm_init", "qmb200_comm_destroy", "qmb200_comm_info", "qmb200_allgather_torque", "qmb200_gait_bin_permutation", "qmb200_set_pipeline", "qmb200_set_profiling", "qmb200_collect_kernel_times", "qmb200_get_kernel_times", "qmb200_get_flow_kernel_time", "qmb200_measure_fp64_peak",
            "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state",
            "qmb200_sim_set_robot_params", "qmb200_sim_get_robot_params", "qmb200_sim_step_ext", "qmb200_sim_step_ext_dev",
+           "qmb200_sim_set_terrain", "qmb200_sim_get_terrain", "qmb200_sim_set_robot_terrain", "qmb200_sim_get_robot_terrain",
            "qmb200_set_model_payload", "qmb200_get_model_payload", "qmb200_debug_srbd_constants"]
 
 _lib = None
@@ -88,6 +89,10 @@ def load_library():
     lib.qmb200_sim_step_ext_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 8
     lib.qmb200_sim_set_robot_params.argtypes = [C.c_void_p] * 3
     lib.qmb200_sim_get_robot_params.argtypes = [C.c_void_p] * 4
+    lib.qmb200_sim_set_terrain.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p]
+    lib.qmb200_sim_get_terrain.argtypes = [C.c_void_p] * 6
+    lib.qmb200_sim_set_robot_terrain.argtypes = [C.c_void_p] * 3
+    lib.qmb200_sim_get_robot_terrain.argtypes = [C.c_void_p] * 4
     lib.qmb200_set_model_payload.argtypes = [C.c_void_p] * 2
     lib.qmb200_get_model_payload.argtypes = [C.c_void_p] * 3
     lib.qmb200_debug_srbd_constants.argtypes = [C.POINTER(Config), C.c_int32, C.c_void_p, C.c_void_p]

@@ -7,7 +7,8 @@ Per simulated millisecond (Gazebo's default physics step, 1 kHz):
   every 1 ms                                          hw_write_dev (QMHWSim::writeSim, 9 ms command delay of qm_gazebo/config/default.yaml)
                                                       → sim_step_dev (physics step + QMHWSim::readSim's contact flags)
 Per-robot experiments (robustness sweeps): cmd_vel and gait may differ per robot, and the plant may vary per robot through the handle's robot
-params (floor friction, end-effector and base payloads: Solver.sim_set_robot_params) and external pushes held over whole plant steps.  The
+params (floor friction, end-effector and base payloads: Solver.sim_set_robot_params), heightfield terrain under the feet
+(Solver.sim_set_terrain / sim_set_robot_terrain) and external pushes held over whole plant steps.  The
 controller is not told about any of them unless the run sets its model payload (Solver.set_model_payload), e.g. to the plant's payload.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
@@ -38,7 +39,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
-        friction_mu=None, payload=None, pushes=None, model_payload=None):
+        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -48,9 +49,27 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     and wrench in _lib.WRENCH_LAYOUT: robot b's wrench acts in every 1 ms plant step whose start lies in [t_on, t_on + duration).
     model_payload: the controller's model payload for this run (Solver.set_model_payload): None keeps the handle's own, "plant" copies this run's plant
     payload (zeros where the plant carries none), or an array [B, 8]; the previous model payload is restored when run returns.
+    terrain: dict(tiles [T, ny, nx], cell, tile [B], origin [B, 2]) (qm_control_b200.terrain builds tiles): the plant's ground for this run
+    (Solver.sim_set_terrain / sim_set_robot_terrain), each robot starting in the standing state on its own ground; the previous terrain is restored
+    when run returns.  The controller does not see the terrain.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end)."""
+    if terrain is not None:
+        prev_lib, prev_robot = solver.sim_get_terrain(), solver.sim_get_robot_terrain()
+        try:
+            solver.sim_set_robot_terrain(None)
+            solver.sim_set_terrain(terrain["tiles"], terrain["cell"])
+            solver.sim_set_robot_terrain(terrain["tile"], terrain["origin"])
+            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, model_payload)
+        finally:
+            solver.sim_set_robot_terrain(None)   # the previous library may have fewer tiles than this run's robots reference
+            if prev_lib is None:
+                solver.sim_set_terrain(None)
+            else:
+                solver.sim_set_terrain(**prev_lib)
+            if prev_robot is not None:
+                solver.sim_set_robot_terrain(**prev_robot)
     if model_payload is not None:
         prev_model = solver.get_model_payload()
         try:

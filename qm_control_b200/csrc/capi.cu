@@ -56,6 +56,8 @@ struct qmb200_handle {
   void* comm = nullptr; int comm_ranks = 0, comm_rank = 0; double* d_send = nullptr;   // NCCL communicator of this handle (capi_comm.inc) and the packed torque rows
   SimParams sim_prm{};   // plant step (capi_sim.inc)
   RobotArray mu{1}, payload{8};   // per-robot plant variation (qmb200_sim_set_robot_params)
+  RobotArray terrain{3};          // per-robot [tile, origin_x, origin_y] on the tile library (qmb200_sim_set_robot_terrain)
+  struct { std::vector<double> host; double* d = nullptr; int n_tiles = 0, nx = 0, ny = 0; double cell = 0.0; } tiles;   // heightfield library (qmb200_sim_set_terrain)
   RobotArray mpayload{8}, srbd{SRBD_DBL};   // the controller's model payload (qmb200_set_model_payload) and the robots' SRBD constants it gives
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
@@ -189,6 +191,7 @@ void qmb200_destroy(qmb200_handle* h) {
   for (int c = 0; c < qmb200_handle::MAX_CHUNKS; ++c) { if (h->cs[c]) { cudaStreamSynchronize(h->cs[c]); cudaStreamDestroy(h->cs[c]); } if (h->join_ev[c]) cudaEventDestroy(h->join_ev[c]); }
   if (h->fork_ev) cudaEventDestroy(h->fork_ev);
   for (void* p : h->allocs) cudaFree(p);
+  if (h->tiles.d) cudaFree(h->tiles.d);
   delete h;
 }
 

@@ -4,10 +4,14 @@
 // One warp owns one robot (lanes over bodies / generalised coordinates, as in rbd.cuh).  One launch advances every robot by `substeps`
 // semi-implicit Euler steps of length h with the effort held; q, v stay in shared memory between substeps.  Per substep, at (q, v):
 //   M, nle                 rbd_kinematics<true> → rbd_inertias(gravity) → rbd_accumulate → rbd_mass_matrix_nle
-//   contact (lanes 0..3)   foot sphere of radius r centred on the *_FOOT frame against the plane z = ground:
-//                          penetration delta = ground - (p_z - r); F_n = max(0, k delta - d pdot_z) for delta > 0, else 0;
-//                          F_t = -v_t min(gamma, mu F_n / |v_t|) (regularised Coulomb).  The force acts at the sphere centre, so the
+//   contact (lanes 0..3)   foot sphere of radius r centred on the *_FOOT frame against the local tangent plane of the ground under its centre:
+//                          height H and gradient (gx, gy) there (sim_api.cuh: ground_at; the plane z = ground: H = ground, g = 0),
+//                          s = sqrt(1 + gx^2 + gy^2), normal n = (-gx, -gy, 1) / s, penetration delta = (H - (p_z - r s)) / s;
+//                          F_n = max(0, k delta - d pdot.n) for delta > 0, else 0; v_t = pdot - (pdot.n) n;
+//                          F = F_n n - v_t min(gamma, mu F_n / |v_t|) (regularised Coulomb).  The force acts at the sphere centre, so the
 //                          sphere's rolling is not modelled: the contact point is the foot frame's point, not the lowest point of the sphere.
+//                          With g = 0 every operation of the law reduces exactly (s = 1, r 1, / 1, n.pdot = pdot_z, v_t = (pdot_x, pdot_y, 0)),
+//                          so flat ground, and a constant tile at height ground, give the plane law bit for bit.
 //   Q                      [0_6; sat(effort) - damping .* qdot_j] + sum_f J_f^T F_f - nle      (J_f: point_jacobian of the foot frame)
 //   solve                  M qddot = Q by the warp Cholesky (wlinalg.cuh); v += h qddot; q += h v
 // After the last substep one kinematics-only pass at the final q gives the measured state rbd[55] (include/qmb200.h layout) with the
@@ -20,6 +24,7 @@
 //                    RNEA force I_p (A + g) + V x* I_p V to F of the body it is fixed to, so M and nle include it through the existing passes.
 //   wrench[B][12]    [f_base, n_base, f_ee, n_ee], world frame, each moment about its own frame's origin, held over the step: W = [n + p x f; f]
 //                    about the world origin, Q_c += S_c . W over the base columns (base wrench) and the base + arm chain columns (EE wrench).
+//   terrain          heightfield tile and origin per robot (SimTerrain); terrain.robot == NULL or tile -1 is the plane z = prm.ground_height
 // A zero payload or wrench adds exact zeros and mu[b] == prm.friction_mu is the shared law, so neutral variation is bit-identical.
 #include "payload.cuh"
 #include "sim_api.cuh"
@@ -72,11 +77,15 @@ __device__ __forceinline__ void frame_loads(const DevModel* __restrict__ mdl, Si
 }
 }  // namespace
 
+// TERRAIN: compiled once with the ground lookup and once for the plane alone (terrain.robot == NULL), which keeps the plane's register budget and its
+// seven CTAs per SM; both run the same contact law, and the law gives the plane bit for bit at zero gradient.
+template <bool TERRAIN>
 __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel* __restrict__ mdl, SimParams prm, int B, int substeps, double h,
                                                                   const double* __restrict__ effort /*[B][18]*/, double* __restrict__ q_io /*[B][24]*/,
                                                                   double* __restrict__ v_io /*[B][24]*/, double* __restrict__ rbd /*[B][55]*/,
                                                                   int32_t* __restrict__ contact, int32_t* __restrict__ status, const double* __restrict__ mu_b /*[B] or NULL*/,
-                                                                  const double* __restrict__ payload /*[B][8] or NULL*/, const double* __restrict__ wrench /*[B][12] or NULL*/) {
+                                                                  const double* __restrict__ payload /*[B][8] or NULL*/, const double* __restrict__ wrench /*[B][12] or NULL*/,
+                                                                  SimTerrain terrain) {
   __shared__ SimWs s_ws[SIM_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * SIM_WARPS + warp;
   if (b >= B) return;   // the whole warp leaves together
@@ -90,6 +99,7 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
   const double mu = mu_b ? mu_b[b] : prm.friction_mu;
   const double* pl = payload && lane < 2 ? payload + (size_t)b * 8 + 4 * lane : nullptr;      // lane 0: [m_ee, o_ee], lane 1: [m_base, o_base]
   const double* wr = wrench && lane < 2 ? wrench + (size_t)b * 12 + 6 * (1 - lane) : nullptr;  // lane 0: [f_ee, n_ee], lane 1: [f_base, n_base]
+  const double* ter = terrain.robot ? terrain.robot + (size_t)b * 3 : nullptr;                   // [tile, origin_x, origin_y]
   const int je = mdl->ee_body - 1;
   const bool ee_col = lane < 6 || (lane - 6 >= mdl->chain_start[je] && lane - 6 <= je);   // columns of the EE's point_jacobian
   __syncwarp();
@@ -109,11 +119,18 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
       const int f = lane, body = mdl->foot_body[f];
       double pw[3]; matvec3(ws->R[body], mdl->foot_p[f], pw); pw[0] += ws->p[body][0]; pw[1] += ws->p[body][1]; pw[2] += ws->p[body][2];
       double vel[3], acc[3]; point_vel_acc(ws, body, pw, vel, acc);
-      const double pen = prm.ground_height - (pw[2] - prm.foot_radius);
-      if (pen > 0.0) fn = fmax(0.0, prm.stiffness * pen - prm.damping * vel[2]);
-      double fx = 0.0, fy = 0.0; const double vt = sqrt(vel[0] * vel[0] + vel[1] * vel[1]);
-      if (fn > 0.0 && vt > 0.0) { const double c = fmin(prm.tangential_damping, mu * fn / vt); fx = -c * vel[0]; fy = -c * vel[1]; }
-      w->fc[f][0] = fx; w->fc[f][1] = fy; w->fc[f][2] = fn;
+      double H = prm.ground_height, gx = 0.0, gy = 0.0;
+      if (TERRAIN) ground_at(terrain, ter, prm.ground_height, pw[0], pw[1], H, gx, gy);
+      const double s = sqrt(1.0 + gx * gx + gy * gy), n[3] = {-gx / s, -gy / s, 1.0 / s};
+      const double pen = (H - (pw[2] - prm.foot_radius * s)) / s, vn = vel[0] * n[0] + vel[1] * n[1] + vel[2] * n[2];
+      if (pen > 0.0) fn = fmax(0.0, prm.stiffness * pen - prm.damping * vn);
+      const double t[3] = {vel[0] - vn * n[0], vel[1] - vn * n[1], vel[2] - vn * n[2]}, vt = sqrt(t[0] * t[0] + t[1] * t[1] + t[2] * t[2]);
+      double F[3] = {0.0, 0.0, 0.0};
+      if (fn > 0.0) {
+        F[0] = fn * n[0]; F[1] = fn * n[1]; F[2] = fn * n[2];
+        if (vt > 0.0) { const double c = fmin(prm.tangential_damping, mu * fn / vt); F[0] -= c * t[0]; F[1] -= c * t[1]; F[2] -= c * t[2]; }
+      }
+      w->fc[f][0] = F[0]; w->fc[f][1] = F[1]; w->fc[f][2] = F[2];
       w->pf[f][0] = pw[0]; w->pf[f][1] = pw[1]; w->pf[f][2] = pw[2];
     }
     const unsigned bal = __ballot_sync(FULL, lane < 4 && fn > 0.0);
@@ -160,8 +177,10 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
 }
 
 int launch_sim_step(const DevModel* mdl, const SimParams& prm, int B, int substeps, double h, const double* effort, double* q, double* v, double* rbd, int32_t* contact,
-                    int32_t* status, const double* mu, const double* payload, const double* wrench, cudaStream_t s) {
-  sim_step_kernel<<<(B + SIM_WARPS - 1) / SIM_WARPS, 32 * SIM_WARPS, 0, s>>>(mdl, prm, B, substeps, h, effort, q, v, rbd, contact, status, mu, payload, wrench);
+                    int32_t* status, const double* mu, const double* payload, const double* wrench, const SimTerrain& terrain, cudaStream_t s) {
+  const dim3 grid((B + SIM_WARPS - 1) / SIM_WARPS), block(32 * SIM_WARPS);
+  if (terrain.robot) sim_step_kernel<true><<<grid, block, 0, s>>>(mdl, prm, B, substeps, h, effort, q, v, rbd, contact, status, mu, payload, wrench, terrain);
+  else sim_step_kernel<false><<<grid, block, 0, s>>>(mdl, prm, B, substeps, h, effort, q, v, rbd, contact, status, mu, payload, wrench, terrain);
   return 1;
 }
 

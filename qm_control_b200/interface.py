@@ -369,8 +369,45 @@ class Solver:
         self._chk(self.lib.qmb200_get_model_payload(self.h, _p(pl), C.byref(is_set)), "qmb200_get_model_payload")
         return pl if is_set.value else None
 
+    def sim_set_terrain(self, tiles=None, cell=None):
+        """Heightfield tile library of the plant: tiles [T, ny, nx] absolute world z (m) on nodes `cell` m apart (qm_control_b200.terrain builds them).
+        None clears the library and every robot's terrain.  Synchronous."""
+        if tiles is None:
+            self._chk(self.lib.qmb200_sim_set_terrain(self.h, 0, 0, 0, 0.0, None), "qmb200_sim_set_terrain"); return
+        t = _f64(tiles)
+        if t.ndim != 3:
+            raise ValueError("expected tiles of shape [T, ny, nx], got %s" % (t.shape,))
+        self._chk(self.lib.qmb200_sim_set_terrain(self.h, t.shape[0], t.shape[2], t.shape[1], float(cell), _p(t)), "qmb200_sim_set_terrain")
+
+    def sim_get_terrain(self):
+        """→ dict(tiles [T, ny, nx], cell), or None when no library is set."""
+        n, nx, ny, cell = C.c_int32(), C.c_int32(), C.c_int32(), C.c_double()
+        self._chk(self.lib.qmb200_sim_get_terrain(self.h, C.byref(n), C.byref(nx), C.byref(ny), C.byref(cell), None), "qmb200_sim_get_terrain")
+        if n.value == 0:
+            return None
+        t = np.zeros((n.value, ny.value, nx.value))
+        self._chk(self.lib.qmb200_sim_get_terrain(self.h, None, None, None, None, _p(t)), "qmb200_sim_get_terrain")
+        return dict(tiles=t, cell=cell.value)
+
+    def sim_set_robot_terrain(self, tile=None, origin=None):
+        """Per-robot terrain: tile [B] (-1: the flat plane; a scalar is broadcast) with its node (0, 0) at world origin [B, 2] (default zeros).
+        None clears it.  Synchronous."""
+        B = self.batch
+        if tile is None:
+            self._chk(self.lib.qmb200_sim_set_robot_terrain(self.h, None, None), "qmb200_sim_set_robot_terrain"); return
+        t = _i32(np.broadcast_to(np.asarray(tile), (B,)), (B,))
+        o = _f64(np.zeros((B, 2)) if origin is None else np.broadcast_to(np.asarray(origin, dtype=np.float64), (B, 2)), (B, 2))
+        self._chk(self.lib.qmb200_sim_set_robot_terrain(self.h, _p(t), _p(o)), "qmb200_sim_set_robot_terrain")
+
+    def sim_get_robot_terrain(self):
+        """→ dict(tile [B], origin [B, 2]), or None when no robot terrain is set."""
+        t = np.zeros(self.batch, dtype=np.int32); o = np.zeros((self.batch, 2)); is_set = C.c_int32()
+        self._chk(self.lib.qmb200_sim_get_robot_terrain(self.h, _p(t), _p(o), C.byref(is_set)), "qmb200_sim_get_robot_terrain")
+        return dict(tile=t, origin=o) if is_set.value else None
+
     def sim_standing_state(self, xy_yaw):
-        """Nominal standing configuration at the given base (x, y, yaw) rows → (q[n,24], v[n,24])."""
+        """Nominal standing configuration at the given base (x, y, yaw) rows → (q[n,24], v[n,24]).  With robot terrain set there is one row per robot,
+        each standing on its own ground."""
         xy = _f64(xy_yaw).reshape(-1, 3); n = xy.shape[0]; q = np.zeros((n, 24)); v = np.zeros((n, 24))
         self._chk(self.lib.qmb200_sim_standing_state(self.h, n, _p(xy), _p(q), _p(v)), "qmb200_sim_standing_state")
         return q, v

@@ -4,7 +4,7 @@ Default: 8192 robots, trot at cmd_vel 0.3 m/s, 1 s simulated after a warm-up run
 simulated second, the plant step's device time per call (CUDA events) and its share of the loop, and quality lines (base distance, end-effector
 deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
 
-    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary]
+    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -12,6 +12,12 @@ gains "vary": the quality per condition bin of each axis (fallen robots, base di
 any of it, unless --model-payload plant sets the controller's model payload to the plant's (closed_loop.run(model_payload="plant")): the timed run
 and the bins are then those of the told controller, and "vary" gains "payload_kg_not_told", the payload bins of the same sweep with the controller
 not told, from one more (untimed) run.
+
+--terrain runs the loop on heightfield terrain (qm_control_b200.terrain): robot b's tile rises beyond 0.35 m ahead of its start, as a ramp of 0/5/10/15
+degrees and steps of 0/3/6/9 cm rise every 0.3 m on it, every combination equally often; the controller does not see the terrain.  The JSON line gains
+"terrain": fallen robots (height above the ground under the base <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite) and base distance per bin of
+each axis, and the plant step's device time at this batch with and without terrain (CUDA events, the two alternated in one process, from one standing
+state).
 """
 import argparse
 import json
@@ -35,13 +41,48 @@ def card():
         return None, None
 
 
+def plant_step_times(solver, ter, xy_yaw, reps=7, calls=20):
+    """Device time per 1 ms plant step (4 substeps) of the whole batch, with the sweep's terrain and without any, alternated `reps` times: each block of
+    `calls` steps starts from the same terrain standing state with zero effort, timed with CUDA events → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)   # a stream of its own: the legacy stream's handle 0 would select the handle's stream
+    solver.sim_set_terrain(ter["tiles"], ter["cell"]); solver.sim_set_robot_terrain(ter["tile"], ter["origin"])
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q0t = torch.as_tensor(q0, device=dev); v0t = torch.as_tensor(v0, device=dev); q = q0t.clone(); v = v0t.clone()
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    times = {"terrain": [], "flat": []}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode in ("terrain", "flat"):
+                if mode == "terrain":
+                    solver.sim_set_robot_terrain(ter["tile"], ter["origin"])
+                else:
+                    solver.sim_set_robot_terrain(None)
+                q.copy_(q0t); v.copy_(v0t); torch.cuda.synchronize(dev)   # every block starts from the same state
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.sim_set_terrain(None)
+    return {"label": "device time per 1 ms plant step of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            "ms_per_call_terrain": float(np.median(times["terrain"])), "ms_per_call_flat": float(np.median(times["flat"])),
+            "spread_terrain": [float(min(times["terrain"])), float(max(times["terrain"]))], "spread_flat": [float(min(times["flat"])), float(max(times["flat"]))]}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
     ap.add_argument("--gait", default="trot"); ap.add_argument("--vx", type=float, default=0.3)
     ap.add_argument("--vary", action="store_true", help="per-robot sweep of EE payload, floor friction and a lateral base push")
     ap.add_argument("--model-payload", choices=["plant"], help="tell the controller the plant's payload (its model payload, Solver.set_model_payload)")
+    ap.add_argument("--terrain", action="store_true", help="per-robot sweep of ramp angle and step rise under the feet")
     args = ap.parse_args()
+    if args.vary and args.terrain:
+        ap.error("--vary and --terrain are separate sweeps")
     import torch
     import qm_control_b200 as q
     from qm_control_b200 import closed_loop
@@ -57,6 +98,13 @@ def main():
         pl = np.zeros((B, 8)); pl[:, 0] = bins["payload_kg"][idx["payload_kg"]]
         w = np.zeros((B, 12)); w[:, 1] = bins["push_N"][idx["push_N"]]
         kw = dict(payload=pl, friction_mu=bins["mu"][idx["mu"]], pushes=(np.full(B, 0.4), np.full(B, 0.1), w))
+    if args.terrain:
+        from qm_control_b200 import terrain as T
+        b = np.arange(B); bins = dict(ramp_deg=np.array([0.0, 5.0, 10.0, 15.0]), step_rise_m=np.array([0.0, 0.03, 0.06, 0.09]))
+        idx = dict(ramp_deg=b % 4, step_rise_m=(b // 4) % 4)
+        tiles = np.stack([T.ramp(a, start=0.35) + T.stairs(r, 0.3, start=0.35) for a in bins["ramp_deg"] for r in bins["step_rise_m"]])
+        ter = dict(tiles=tiles, cell=T.CELL, tile=idx["ramp_deg"] * 4 + idx["step_rise_m"], origin=T.centred_origin(xy[:, :2]))
+        kw = dict(terrain=ter)
     told = dict(model_payload=args.model_payload) if args.model_payload else {}
     closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told)   # warm-up run of the same length
     pairs = []
@@ -79,11 +127,14 @@ def main():
         return dist, dpos, dang
 
     def vary_bins(r, axis):
-        dist, dpos, dang = quality(r); base = r["base"]
-        fallen = ~(np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3))
+        dist, dpos, dang = quality(r); base = r["base"]; ground = 0.0
+        if args.terrain:   # height above the ground under the base
+            ground = T.height(ter["tiles"], ter["cell"], ter["tile"][None], ter["origin"][None], base[:, :, :2])
+        fallen = ~(np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2] - ground, axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3))
         return [{"value": float(val), "robots": int(np.sum(idx[axis] == i)), "fallen": int(np.sum(fallen[idx[axis] == i])),
                  "base_distance_m_p50": float(np.percentile(dist[idx[axis] == i], 50)),
-                 "ee_max_pos_dev_mm": pct(dpos[idx[axis] == i]), "ee_max_ori_dev_deg_p50": float(np.percentile(dang[idx[axis] == i], 50))}
+                 **({"base_distance_m": pct(dist[idx[axis] == i])} if args.terrain else
+                    {"ee_max_pos_dev_mm": pct(dpos[idx[axis] == i]), "ee_max_ori_dev_deg_p50": float(np.percentile(dang[idx[axis] == i], 50))})}
                 for i, val in enumerate(bins[axis])]
     dist, dpos, dang = quality(r)
     name, limit = card()
@@ -94,6 +145,10 @@ def main():
         if args.model_payload:
             extra["vary"]["model_payload"] = "the controller is told the plant's payload (bins); payload_kg_not_told: the same sweep, controller not told"
             extra["vary"]["payload_kg_not_told"] = vary_bins(closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw), "payload_kg")
+    if args.terrain:
+        extra["terrain"] = {"label": "per-robot sweep, controller blind to the terrain; fallen = height above the ground under the base <= 0.3 m or |roll|, |pitch| >= 0.3 rad "
+                                     "or non-finite", "tiles": "ground z = 0 up to 0.35 m ahead of the start, then a ramp (deg) with steps (rise m, run 0.3 m) on it",
+                            "bins": {axis: vary_bins(r, axis) for axis in bins}, "plant_step": plant_step_times(solver, ter, xy)}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
