@@ -158,8 +158,48 @@ int qmb200_centroidal_state_from_rbd(const qmb200_handle* h, int32_t n, const do
  * negative mass; on rejection the stored payload stays unchanged. */
 #define QMB200_SRBD 24   /* per-robot SRBD constants: [robotMass, centroidalInertiaNominal(9, row-major), its inverse(9), comToBasePositionNominal(3), 0, 0] */
 int qmb200_set_model_payload(qmb200_handle* h, const double* payload /*[B][8] or NULL*/);
-/* The stored payload (zeros where none is set); is_set = 1 when one is set.  Either output may be NULL. */
+/* The stored payload (zeros where none is set); is_set = 1 when one is set.  Either output may be NULL.  After a qmb200_payload_est_commit_dev it waits
+ * for the device and returns the rows the kernels read. */
 int qmb200_get_model_payload(const qmb200_handle* h, double* payload /*[B][8]*/, int32_t* is_set);
+
+/* ---- online estimate of the end-effector payload (DESIGN.md §4.6): per-robot recursive least squares on the six arm rows of the nominal model, which see
+ *      an end-effector load through its ten inertial parameters theta = [m, m c_x, m c_y, m c_z, I_xx, I_xy, I_xz, I_yy, I_yz, I_zz] (end-effector frame,
+ *      about its origin) and see neither the foot contacts nor a base payload.  It reads only what the controller reads (the measurement rbd and the effort
+ *      sent) and commits its estimate to the model payload on the device, so it can run inside a loop without host synchronisation.
+ *      An external wrench on the end effector is indistinguishable from a load and biases the estimate while it acts; a wrench on the base does not.
+ *   forgetting       RLS forgetting factor lambda in (0, 1]
+ *   p0_mass, p0_first_moment, p0_inertia   prior variances of m (kg^2), of m c (kg^2 m^2) and of I (kg^2 m^4): P = diag(p0) at the reset
+ *   trace_max        P is scaled down to this trace whenever it exceeds it (directions the motion does not excite would otherwise grow as lambda^-k)
+ *   mass_min         below this estimated mass the committed offset is 0 (m c / m is noise there)
+ *   mass_max         committed mass = clamp(m, 0, mass_max)
+ *   offset_max       committed offset = m c / m with its norm clipped to offset_max (m) */
+typedef struct qmb200_payload_est_params {
+  double forgetting, p0_mass, p0_first_moment, p0_inertia, trace_max, mass_min, mass_max, offset_max;
+} qmb200_payload_est_params;
+int qmb200_payload_est_get_params(const qmb200_handle* h, qmb200_payload_est_params* out);
+/* rejects non-finite values, forgetting outside (0, 1], a variance, trace_max, mass_min, mass_max or offset_max <= 0 and mass_min > mass_max */
+int qmb200_payload_est_set_params(qmb200_handle* h, const qmb200_payload_est_params* p);
+/* (Re)starts the estimator of every robot: theta = the end-effector point mass of prior [B][8] (layout as qmb200_set_model_payload; NULL: the current model
+ * payload, zeros when none is set), P = diag(p0), no stored sample.  Sets the model payload to prior through qmb200_set_model_payload, so the kernels read
+ * per-robot rows from then on.  Synchronous. */
+int qmb200_payload_est_reset(qmb200_handle* h, const double* prior /*[B][8] or NULL*/);
+/* One RLS update per robot from the measurement rbd (the plant's output, include/qmb200.h layout) and the effort [B][18] held over the dt seconds that ended
+ * at it (clipped to the URDF effort limits as the plant does).  The first call after a reset only stores its sample.  status [B] (written, not OR-ed):
+ * QMB200_ST_NAN for a non-finite input (nothing is stored) or update, QMB200_ST_NOT_PD when the innovation covariance fails its Cholesky; the robot
+ * then keeps its theta and P. */
+int qmb200_payload_est_step(qmb200_handle* h, double dt, const double* effort /*[B][18]*/, const double* rbd /*[B][55]*/, int32_t* status /*[B]*/);
+int qmb200_payload_est_step_dev(qmb200_handle* h, double dt, const double* effort, const double* rbd, int32_t* status, void* cuda_stream);
+/* In stream order on cuda_stream (NULL: the handle's): m = clamp(theta_0, 0, mass_max) and o = theta_1:4 / theta_0 (0 when theta_0 < mass_min, norm clipped to
+ * offset_max) into the end-effector half [m_ee, o_ee] of every robot's model payload row, and the robot's SRBD constants from the whole row, as
+ * qmb200_set_model_payload computes them.  The base half is left as it was.  No host copy. */
+int qmb200_payload_est_commit_dev(qmb200_handle* h, void* cuda_stream);
+/* Synchronous: theta [B][10], the diagonal of P [B][10] and the samples stored since the reset [B].  Any output may be NULL. */
+int qmb200_payload_est_get(qmb200_handle* h, double* theta /*[B][10]*/, double* p_diag /*[B][10]*/, int32_t* samples /*[B]*/);
+/* Releases the estimator state; the model payload keeps its last committed rows.  Step, commit and get fail until the next reset. */
+int qmb200_payload_est_stop(qmb200_handle* h);
+/* The model payload rows the kernels read, copied in stream order into payload (device, [B][8]) on cuda_stream (NULL: the handle's): a record of the committed
+ * estimate without host synchronisation.  Fails when no model payload is set. */
+int qmb200_get_model_payload_dev(const qmb200_handle* h, double* payload /*[B][8] device*/, void* cuda_stream);
 
 /* ---- gait front-end: GaitSchedule::getModeSchedule tiling of a ModeSequenceTemplate (QMInterface.cpp:455-480, gait.info) for one robot:
  *      STANCE until t_start, then the template repeated; window [lo, hi]; returns the number of events written (<= EMAX) or negative. */

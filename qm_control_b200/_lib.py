@@ -34,6 +34,14 @@ class SimParams(C.Structure):
                [("joint_damping", C.c_double * 18), ("substeps_per_ms", C.c_int32)]
 
 
+class PayloadEstParams(C.Structure):
+    """qmb200_payload_est_params: the online payload estimator's constants (include/qmb200.h, DESIGN.md §4.6)."""
+    _fields_ = [(n, C.c_double) for n in ("forgetting", "p0_mass", "p0_first_moment", "p0_inertia", "trace_max", "mass_min", "mass_max", "offset_max")]
+
+
+# the payload estimator's parameter vector theta: the load's inertial parameters in the end-effector frame about its origin (include/qmb200.h)
+THETA_LAYOUT = ("m", "mc_x", "mc_y", "mc_z", "I_xx", "I_xy", "I_xz", "I_yy", "I_yz", "I_zz")
+
 # per-robot plant variation (include/qmb200.h: qmb200_sim_set_robot_params, qmb200_sim_step_ext): the column layouts of payload[B][8] and wrench[B][12]
 PAYLOAD_LAYOUT = ("m_ee", "o_ee_x", "o_ee_y", "o_ee_z", "m_base", "o_base_x", "o_base_y", "o_base_z")
 # the controller's model payload (qmb200_set_model_payload) has PAYLOAD_LAYOUT too; per robot it yields SRBD_LAYOUT (qmb200_debug_srbd_constants)
@@ -55,7 +63,9 @@ SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_d
            "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state",
            "qmb200_sim_set_robot_params", "qmb200_sim_get_robot_params", "qmb200_sim_step_ext", "qmb200_sim_step_ext_dev",
            "qmb200_sim_set_terrain", "qmb200_sim_get_terrain", "qmb200_sim_set_robot_terrain", "qmb200_sim_get_robot_terrain",
-           "qmb200_set_model_payload", "qmb200_get_model_payload", "qmb200_debug_srbd_constants"]
+           "qmb200_set_model_payload", "qmb200_get_model_payload", "qmb200_debug_srbd_constants",
+           "qmb200_payload_est_get_params", "qmb200_payload_est_set_params", "qmb200_payload_est_reset", "qmb200_payload_est_step", "qmb200_payload_est_step_dev",
+           "qmb200_payload_est_commit_dev", "qmb200_payload_est_get", "qmb200_payload_est_stop", "qmb200_get_model_payload_dev"]
 
 _lib = None
 
@@ -96,6 +106,15 @@ def load_library():
     lib.qmb200_set_model_payload.argtypes = [C.c_void_p] * 2
     lib.qmb200_get_model_payload.argtypes = [C.c_void_p] * 3
     lib.qmb200_debug_srbd_constants.argtypes = [C.POINTER(Config), C.c_int32, C.c_void_p, C.c_void_p]
+    lib.qmb200_payload_est_get_params.argtypes = [C.c_void_p, C.POINTER(PayloadEstParams)]
+    lib.qmb200_payload_est_set_params.argtypes = [C.c_void_p, C.POINTER(PayloadEstParams)]
+    lib.qmb200_payload_est_reset.argtypes = [C.c_void_p] * 2
+    lib.qmb200_payload_est_step.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 3
+    lib.qmb200_payload_est_step_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 4
+    lib.qmb200_payload_est_commit_dev.argtypes = [C.c_void_p] * 2
+    lib.qmb200_payload_est_get.argtypes = [C.c_void_p] * 4
+    lib.qmb200_payload_est_stop.argtypes = [C.c_void_p]
+    lib.qmb200_get_model_payload_dev.argtypes = [C.c_void_p] * 3
     lib.qmb200_sim_standing_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.qmb200_gait_destroy.restype = None
     lib.qmb200_gait_destroy.argtypes = [C.c_void_p]

@@ -10,6 +10,8 @@ Per-robot experiments (robustness sweeps): cmd_vel and gait may differ per robot
 params (floor friction, end-effector and base payloads: Solver.sim_set_robot_params), heightfield terrain under the feet
 (Solver.sim_set_terrain / sim_set_robot_terrain) and external pushes held over whole plant steps.  The
 controller is not told about any of them unless the run sets its model payload (Solver.set_model_payload), e.g. to the plant's payload.
+With payload_estimator set, an online estimate of each robot's end-effector payload (Solver.payload_est_*) runs beside the plant on what the
+controller sees: it steps after every plant step and is committed to the model payload right before every MPC tick.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -39,7 +41,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
-        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None):
+        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -52,16 +54,24 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     terrain: dict(tiles [T, ny, nx], cell, tile [B], origin [B, 2]) (qm_control_b200.terrain builds tiles): the plant's ground for this run
     (Solver.sim_set_terrain / sim_set_robot_terrain), each robot starting in the standing state on its own ground; the previous terrain is restored
     when run returns.  The controller does not see the terrain.
+    payload_estimator: True, or a dict of qmb200_payload_est_params overrides (Solver.payload_est_set_params), runs the online payload estimate from the model
+    payload in force (model_payload's value, or the handle's own): one step after every plant step with the same effort and measurement, one commit right
+    before every MPC tick, so the targets, solve, updates and observation of one 10 ms window share one model.  Its status is OR-ed into the record's.
+    The estimator is stopped and the previous model payload and estimator parameters restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
-    safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end)."""
+    safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
+    payload_est[ticks, B, 8] = the model payload rows committed at each record's MPC tick)."""
+    if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
+        raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
     if terrain is not None:
         prev_lib, prev_robot = solver.sim_get_terrain(), solver.sim_get_robot_terrain()
         try:
             solver.sim_set_robot_terrain(None)
             solver.sim_set_terrain(terrain["tiles"], terrain["cell"])
             solver.sim_set_robot_terrain(terrain["tile"], terrain["origin"])
-            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, model_payload)
+            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, model_payload,
+                       payload_estimator=payload_estimator)
         finally:
             solver.sim_set_robot_terrain(None)   # the previous library may have fewer tiles than this run's robots reference
             if prev_lib is None:
@@ -79,20 +89,35 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
                 plant = payload if payload is not None else solver.sim_get_robot_params()["payload"]
                 model_payload = np.zeros((solver.batch, 8)) if plant is None else plant
             solver.set_model_payload(model_payload)
-            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes)
+            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, payload_estimator=payload_estimator)
         finally:
             solver.set_model_payload(prev_model)
+    if payload_estimator is not None:
+        prev_model, prev_params = solver.get_model_payload(), solver.payload_est_get_params()
+        try:
+            if isinstance(payload_estimator, dict):
+                solver.payload_est_set_params(**payload_estimator)
+            solver.payload_est_reset()
+            return _plant_params(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, True)
+        finally:
+            solver.payload_est_stop()
+            solver.set_model_payload(prev_model)
+            solver.payload_est_set_params(**prev_params)
+    return _plant_params(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, False)
+
+
+def _plant_params(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, est):
     if friction_mu is None and payload is None:
-        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes)
+        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est)
     prev = solver.sim_get_robot_params()
     solver.sim_set_robot_params(friction_mu=prev["friction_mu"] if friction_mu is None else friction_mu, payload=prev["payload"] if payload is None else payload)
     try:
-        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes)
+        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est)
     finally:
         solver.sim_set_robot_params(**prev)
 
 
-def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes):
+def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -136,6 +161,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         ticks = n_ms // MPC_PERIOD_MS
         rec_base = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev); rec_ee = torch.zeros((ticks, B, 7), dtype=torch.float64, device=dev)
         rec_st = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
+        if est:
+            est_st = torch.zeros_like(contact); rec_pl = torch.zeros((ticks, B, 8), dtype=torch.float64, device=dev)   # row i: the rows of window i's MPC tick
         push = None
         if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
             push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench), zero=torch.zeros((B, 12), dtype=torch.float64, device=dev),
@@ -143,16 +170,18 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     stream.synchronize()
     solver.hw_set_delay(HW_DELAY)
 
-    def mpc_tick():
+    def mpc_tick(i):
+        if est:
+            solver.payload_est_commit_dev(s); solver.get_model_payload_dev(rec_pl[i], s)
         ee_state.copy_(rbd[:, 48:55])
         solver.target_trajectories_dev(0, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
         solver.mpc_solve_dev(prob, s)
 
     with torch.cuda.stream(stream):
-        mpc_tick(); stream.synchronize()          # QMController::starting: one blocking solve before the loop
+        mpc_tick(0); stream.synchronize()          # QMController::starting: one blocking solve before the loop
         for k in range(n_ms):
             if k % MPC_PERIOD_MS == 0 and k > 0:
-                mpc_tick()
+                mpc_tick(k // MPC_PERIOD_MS)
             if k % wbc_period_ms == 0:
                 solver.update_dev(rbd, period, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, ctl_st, s)
                 acc_st.bitwise_or_(ctl_st)
@@ -166,10 +195,16 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             if sim_timer:
                 sim_timer(False)
             acc_st.bitwise_or_(hw_st).bitwise_or_(sim_st)
+            if est:
+                solver.payload_est_step_dev(1e-3, effort, rbd, est_st, s)
+                acc_st.bitwise_or_(est_st)
             if (k + 1) % MPC_PERIOD_MS == 0:
                 i = (k + 1) // MPC_PERIOD_MS - 1
                 rec_base[i, :, 0:3] = rbd[:, 3:6]; rec_base[i, :, 3:6] = rbd[:, 0:3]; rec_ee[i] = rbd[:, 48:55]; rec_st[i] = acc_st; acc_st.zero_()
     stream.synchronize()
     t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
-    return dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
-                start_base=np.c_[q0[:, 0:3], q0[:, 3:6]], start_ee=rbd_h[:, 48:55])
+    out = dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
+               start_base=np.c_[q0[:, 0:3], q0[:, 3:6]], start_ee=rbd_h[:, 48:55])
+    if est:
+        out["payload_est"] = rec_pl.cpu().numpy()
+    return out

@@ -14,6 +14,7 @@
 #include "kernels/mpc_api.cuh"
 #include "kernels/ctrl_api.cuh"
 #include "kernels/sim_api.cuh"
+#include "kernels/payload_est_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -59,6 +60,8 @@ struct qmb200_handle {
   RobotArray terrain{3};          // per-robot [tile, origin_x, origin_y] on the tile library (qmb200_sim_set_robot_terrain)
   struct { std::vector<double> host; double* d = nullptr; int n_tiles = 0, nx = 0, ny = 0; double cell = 0.0; } tiles;   // heightfield library (qmb200_sim_set_terrain)
   RobotArray mpayload{8}, srbd{SRBD_DBL};   // the controller's model payload (qmb200_set_model_payload) and the robots' SRBD constants it gives
+  qmb200_payload_est_params est_prm{}; double* d_est = nullptr;   // payload estimator (capi_est.inc): parameters and state [B][EST_DBL], NULL when not running
+  bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
 
@@ -69,6 +72,7 @@ template <class T> bool dalloc(qmb200_handle* h, T** p, size_t count) {
   cudaMemsetAsync(q, 0, count * sizeof(T), h->stream); h->allocs.push_back(q); *p = static_cast<T*>(q); return true;   // zeroed in stream order with the handle's work
 }
 SimParams default_sim_params();   // capi_sim.inc
+qmb200_payload_est_params default_est_params();   // capi_est.inc
 int fail(qmb200_handle* h, const std::string& msg) { if (h) h->err = msg; else g_create_error = msg; return -1; }
 #define QMB_CUDA(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(h, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
 
@@ -164,7 +168,7 @@ int qmb200_create(const qmb200_config* cfg, qmb200_handle** out) {
     for (int j = 0; j < NJ; ++j) h->target_prm.default_joint_state[j] = h->hm.default_joint_state[j];
   } catch (const std::exception& e) { g_create_error = e.what(); delete h; return -2; }
   h->task_file = cfg->task_file;
-  h->sim_prm = default_sim_params();
+  h->sim_prm = default_sim_params(); h->est_prm = default_est_params();
   h->B = cfg->batch; h->variant = cfg->wbc_variant; h->device = cfg->device; h->law_prm.variant = cfg->wbc_variant == QMB200_WBC_HIERARCHICAL_MPC ? 1 : 0;
   const int nint = (int)std::ceil(h->hm.dev.time_horizon / h->hm.dev.dt - 1e-9);
   h->nmax = cfg->max_nodes > 0 ? cfg->max_nodes : nint + 1 + 20;
@@ -192,6 +196,7 @@ void qmb200_destroy(qmb200_handle* h) {
   if (h->fork_ev) cudaEventDestroy(h->fork_ev);
   for (void* p : h->allocs) cudaFree(p);
   if (h->tiles.d) cudaFree(h->tiles.d);
+  if (h->d_est) cudaFree(h->d_est);
   delete h;
 }
 
@@ -219,9 +224,19 @@ std::string payload_error(const double* payload, size_t n, const char* who) {
   }
   return "";
 }
+// After a payload estimator commit the device holds the model payload rows: wait for it and copy them into the host copies, which say what is set
+int model_rows_sync(const qmb200_handle* hc) {
+  qmb200_handle* h = const_cast<qmb200_handle*>(hc);
+  if (!h->model_on_device) return 0;
+  const size_t B = (size_t)h->B;
+  QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());
+  QMB_CUDA(h, cudaMemcpy(h->mpayload.host.data(), h->mpayload.d, B * 8 * 8, cudaMemcpyDeviceToHost));
+  QMB_CUDA(h, cudaMemcpy(h->srbd.host.data(), h->srbd.d, B * SRBD_DBL * 8, cudaMemcpyDeviceToHost));
+  h->model_on_device = false; return 0;
+}
 // SRBD constants of n robots with payload rows [n][8] (NULL: none)
 void srbd_rows(const HostModel& hm, const double* payload, size_t n, double* out) {
-  for (size_t b = 0; b < n; ++b) srbd_constants(hm.dev, hm.default_joint_state, payload ? payload + 8 * b : nullptr, out + SRBD_DBL * b);
+  for (size_t b = 0; b < n; ++b) srbd_constants(hm.dev, payload ? payload + 8 * b : nullptr, out + SRBD_DBL * b);
 }
 }  // namespace
 extern "C" {
@@ -230,10 +245,13 @@ int qmb200_set_model_payload(qmb200_handle* h, const double* payload) {
   if (!h) return -1; const size_t B = (size_t)h->B;
   if (payload) { const std::string e = payload_error(payload, B, "qmb200_set_model_payload"); if (!e.empty()) return fail(h, e); }
   std::vector<double> srbd; if (payload) { srbd.resize(B * SRBD_DBL); srbd_rows(h->hm, payload, B, srbd.data()); }
-  return set_robot_arrays(h, {{&h->mpayload, payload}, {&h->srbd, payload ? srbd.data() : nullptr}});
+  const int rc = set_robot_arrays(h, {{&h->mpayload, payload}, {&h->srbd, payload ? srbd.data() : nullptr}});
+  if (!rc) h->model_on_device = false;   // set_robot_arrays waited for the device: the rows just written replace any committed ones
+  return rc;
 }
 int qmb200_get_model_payload(const qmb200_handle* h, double* payload, int32_t* is_set) {
   if (!h) return -1; const size_t B = (size_t)h->B;
+  if (int rc = model_rows_sync(h)) return rc;
   const std::vector<double>& p = h->mpayload.host;
   if (payload) { if (p.empty()) std::memset(payload, 0, B * 64); else std::memcpy(payload, p.data(), B * 64); }
   if (is_set) *is_set = p.empty() ? 0 : 1;
@@ -328,3 +346,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_ctrl.inc"
 #include "capi_comm.inc"
 #include "capi_sim.inc"
+#include "capi_est.inc"

@@ -150,16 +150,6 @@ Rot from_rpy(const double* rpy) {   // URDF fixed-axis roll-pitch-yaw = Rz(y) Ry
 Rot identity() { return Rot{{1, 0, 0, 0, 1, 0, 0, 0, 1}}; }
 Rot about_axis(int ax, double q) { const double s = sin(q), c = cos(q); if (ax == 0) return Rot{{1, 0, 0, 0, c, -s, 0, s, c}}; if (ax == 1) return Rot{{c, 0, s, 0, 1, 0, -s, 0, c}}; return Rot{{c, -s, 0, s, c, 0, 0, 0, 1}}; }
 
-struct Lump { double m = 0, c[3] = {0, 0, 0}, I[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; };
-// add rigid body (mass, com, inertia about com) expressed in the same frame
-void lump_add(Lump& a, double m, const double* c, const double* I) {
-  if (m == 0.0) { for (int i = 0; i < 9; ++i) a.I[i] += I[i]; return; }
-  const double mt = a.m + m; double cn[3]; for (int i = 0; i < 3; ++i) cn[i] = (a.m * a.c[i] + m * c[i]) / mt;
-  auto shifted = [&](double mm, const double* cc, const double* II, double* out) { double d[3] = {cc[0] - cn[0], cc[1] - cn[1], cc[2] - cn[2]}; const double dd = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) out[3 * i + j] = II[3 * i + j] + mm * ((i == j ? dd : 0.0) - d[i] * d[j]); };
-  double I1[9], I2[9]; shifted(a.m, a.c, a.I, I1); shifted(m, c, I, I2);
-  for (int i = 0; i < 9; ++i) a.I[i] = I1[i] + I2[i]; a.m = mt; for (int i = 0; i < 3; ++i) a.c[i] = cn[i];
-}
 int axis_index(const double* a, const std::string& name) {
   if (a[0] == 1 && a[1] == 0 && a[2] == 0) return 0; if (a[0] == 0 && a[1] == 1 && a[2] == 0) return 1; if (a[0] == 0 && a[1] == 0 && a[2] == 1) return 2;
   throw std::runtime_error("URDF: joint " + name + " has an axis other than +x/+y/+z (unsupported)");
@@ -171,26 +161,7 @@ void host_fk(const DevModel& d, const double* q, Rot* Rw, double (*pw)[3]) {
 }
 }  // namespace
 
-void srbd_constants(const DevModel& d, const double* default_joint_state, const double* payload, double* out) {
-  Rot Rw[NB]; double pw[NB][3];
-  double qn[NQ] = {0}; for (int j = 0; j < NJ; ++j) qn[6 + j] = default_joint_state[j]; host_fk(d, qn, Rw, pw);
-  Lump whole; for (int b = 0; b < NB; ++b) { double c[3]; apply(Rw[b], d.com[b], c); for (int i = 0; i < 3; ++i) c[i] += pw[b][i]; Rot I0; std::memcpy(I0.m, d.Ib[b], sizeof(I0.m)); Rot Iw = mul(mul(Rw[b], I0), transpose(Rw[b])); lump_add(whole, d.mass[b], c, Iw.m); }
-  double mass = d.total_mass;
-  for (int k = 0; payload && k < 2; ++k) {   // [m_ee, o_ee] at o_ee in the end-effector frame, [m_base, o_base] at o_base in the base frame
-    const double m = payload[4 * k]; if (m == 0.0) continue;   // a zero mass adds nothing, so the nominal constants stay bit-identical
-    const int body = k == 0 ? d.ee_body : 0; double cb[3] = {payload[4 * k + 1], payload[4 * k + 2], payload[4 * k + 3]};
-    if (k == 0) { Rot Re; std::memcpy(Re.m, d.ee_R, sizeof(Re.m)); double o[3]; apply(Re, cb, o); for (int i = 0; i < 3; ++i) cb[i] = o[i] + d.ee_p[i]; }
-    double c[3]; apply(Rw[body], cb, c); for (int i = 0; i < 3; ++i) c[i] += pw[body][i];
-    const double I0[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; lump_add(whole, m, c, I0); mass += m;
-  }
-  SrbdConst s; s.m = mass;
-  std::memcpy(s.I_nom, whole.I, sizeof(whole.I)); for (int i = 0; i < 3; ++i) s.c_nom[i] = -whole.c[i];
-  const double* m = s.I_nom; const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6]; const double id = 1.0 / (m[0] * c00 + m[1] * c01 + m[2] * c02);
-  double* o = s.I_nom_inv; o[0] = c00 * id; o[1] = (m[2] * m[7] - m[1] * m[8]) * id; o[2] = (m[1] * m[5] - m[2] * m[4]) * id; o[3] = c01 * id; o[4] = (m[0] * m[8] - m[2] * m[6]) * id; o[5] = (m[2] * m[3] - m[0] * m[5]) * id;
-  o[6] = c02 * id; o[7] = (m[1] * m[6] - m[0] * m[7]) * id; o[8] = (m[0] * m[4] - m[1] * m[3]) * id;
-  for (int i = 0; i < SRBD_DBL; ++i) out[i] = 0.0;
-  std::memcpy(out, &s, sizeof(s));
-}
+void srbd_constants(const DevModel& d, const double* payload, double* out) { srbd_payload_fold(d, payload, out); }
 
 HostModel build_host_model(const std::string& task_file, const std::string& urdf_file, const std::string& reference_file, const std::string& gains_file) {
   InfoFile task(task_file); UrdfRobot urdf = read_urdf(urdf_file); InfoFile reference(reference_file);
@@ -199,7 +170,7 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
   std::map<std::string, bool> is_child; for (auto& kv : urdf.joints) is_child[kv.second.child] = true;
   std::string root; for (auto& kv : urdf.links) if (!is_child.count(kv.first)) root = kv.first;
   if (root.empty()) throw std::runtime_error("URDF: no root link");
-  Lump lumps[NB]; int nj = 0;
+  SrbdLump lumps[NB]; int nj = 0;
   auto add_link_inertia = [&](int body, const UrdfLink& l, const Rot& R, const double* p) {
     if (!l.has_inertial) return; Rot Rin = from_rpy(l.rpy); Rot Rt = mul(R, Rin);
     const double Il[9] = {l.inertia[0], l.inertia[1], l.inertia[2], l.inertia[1], l.inertia[3], l.inertia[4], l.inertia[2], l.inertia[4], l.inertia[5]};
@@ -245,8 +216,14 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
 
   // --- CentroidalModelInfo, SRBD (createCentroidalModelInfo [upstream]) ---
   { auto djs = reference.matrix("defaultJointState", NJ, 1); for (int i = 0; i < NJ; ++i) hm.default_joint_state[i] = djs[i]; }
-  { double s[SRBD_DBL]; srbd_constants(d, hm.default_joint_state, nullptr, s); std::memcpy(&d.total_mass, s, sizeof(SrbdConst)); }
+  // the nominal SRBD block: the bodies folded at defaultJointState with the base at the origin, level (srbd_payload_fold adds payloads to it)
   Rot Rw[NB]; double pw[NB][3];
+  {
+    double qn[NQ] = {0}; for (int j = 0; j < NJ; ++j) qn[6 + j] = hm.default_joint_state[j]; host_fk(d, qn, Rw, pw);
+    SrbdLump whole; for (int b = 0; b < NB; ++b) { double c[3]; apply(Rw[b], d.com[b], c); for (int i = 0; i < 3; ++i) c[i] += pw[b][i]; Rot I0; std::memcpy(I0.m, d.Ib[b], sizeof(I0.m)); Rot Iw = mul(mul(Rw[b], I0), transpose(Rw[b])); lump_add(whole, d.mass[b], c, Iw.m); }
+    std::memcpy(d.ee_body_R0, Rw[d.ee_body].m, sizeof(d.ee_body_R0)); std::memcpy(d.ee_body_p0, pw[d.ee_body], sizeof(d.ee_body_p0));
+    std::memcpy(d.I_nom, whole.I, sizeof(whole.I)); for (int i = 0; i < 3; ++i) d.c_nom[i] = -whole.c[i]; inv3(d.I_nom, d.I_nom_inv);
+  }
 
   // --- WBC gains (wbcWigeht.cfg defaults; optional override file) and friction (WbcBase.cpp:584-594) ---
   d.kp_swing = 350; d.kd_swing = 37; d.base_height_kp = 400; d.base_height_kd = 140; d.base_linear_kp = 400; d.base_linear_kd = 100; d.base_angular_kp = 400; d.base_angular_kd = 140;

@@ -55,8 +55,9 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
 // The SRBD constants (SrbdConst, padded to SRBD_DBL doubles) of the model at defaultJointState, as createCentroidalModelInfo folds the bodies: the composite
 // mass, inertia about the composite COM and the base-to-COM offset.  `payload` (include/qmb200.h layout [m_ee, o_ee(3), m_base, o_base(3)], or null) adds
 // two point masses without rotational inertia, at o_ee in the end-effector frame and at o_base in the base frame - what a URDF with an extra fixed link carrying
-// each mass would give.  Zero masses add nothing: build_host_model's DevModel fields are this function with no payload.
-void srbd_constants(const DevModel& d, const double* default_joint_state, const double* payload, double* out /*[SRBD_DBL]*/);
+// each mass would give.  build_host_model folds the bodies into DevModel's nominal block; this is srbd_payload_fold (dev_common.cuh) on that block, the
+// function the payload estimator's commit kernel calls on the device.  Zero masses add nothing: no payload gives the nominal block bit for bit.
+void srbd_constants(const DevModel& d, const double* payload, double* out /*[SRBD_DBL]*/);
 
 // gait.info / reference.info mode-sequence templates (ocs2 ModeSequenceTemplate) and name → mode number
 struct ModeTemplate { std::vector<double> switching_times; std::vector<int> modes; };

@@ -42,6 +42,7 @@ struct DevModel {
   int leg_foot[4];         // inverse map: leg (first joint / 3) → foot index
   double foot_p[4][3];
   int ee_body; double ee_R[9]; double ee_p[3];
+  double ee_body_R0[9], ee_body_p0[3];       // world pose of ee_body at defaultJointState (base at the origin, level): where srbd_payload_fold places o_ee
   double total_mass;
   double I_nom[9], I_nom_inv[9], c_nom[3];   // SRBD centroidalInertiaNominal, its inverse, comToBasePositionNominal
   double effort[NJ];
@@ -205,6 +206,45 @@ QMB_HD void rotation_error_world(const double* L, const double* Rr, double* e) {
   if (s < 1e-12) { e[0] = 0.5 * w[0]; e[1] = 0.5 * w[1]; e[2] = 0.5 * w[2]; return; }
   const double k = atan2(s, c) / (2.0 * s); e[0] = k * w[0]; e[1] = k * w[1]; e[2] = k * w[2];
 }
+// A composite rigid body being folded: mass, COM and inertia about the COM, all in one frame.  lump_add adds a body (mass m, COM c, inertia I about c) to it.
+struct SrbdLump { double m = 0.0, c[3] = {0, 0, 0}, I[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; };
+QMB_HD void lump_shift(double mm, const double* cc, const double* II, const double* cn, double* out) {   // II about cc → about cn (parallel axis)
+  const double d[3] = {cc[0] - cn[0], cc[1] - cn[1], cc[2] - cn[2]}; const double dd = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) out[3 * i + j] = II[3 * i + j] + mm * ((i == j ? dd : 0.0) - d[i] * d[j]);
+}
+QMB_HD void lump_add(SrbdLump& a, double m, const double* c, const double* I) {
+  if (m == 0.0) { for (int i = 0; i < 9; ++i) a.I[i] += I[i]; return; }
+  const double mt = a.m + m; double cn[3]; for (int i = 0; i < 3; ++i) cn[i] = (a.m * a.c[i] + m * c[i]) / mt;
+  double I1[9], I2[9]; lump_shift(a.m, a.c, a.I, cn, I1); lump_shift(m, c, I, cn, I2);
+  for (int i = 0; i < 9; ++i) a.I[i] = I1[i] + I2[i];
+  a.m = mt; for (int i = 0; i < 3; ++i) a.c[i] = cn[i];
+}
+
+// The SRBD constants of one robot with model payload pl = [m_ee, o_ee(3), m_base, o_base(3)] (or NULL) → out[SRBD_DBL]: DevModel's nominal block (the fold of the
+// bodies at defaultJointState: total_mass, I_nom about the composite COM, -c_nom) with each point mass added at its position in the default joint state, o_ee
+// in the end-effector frame (ee_body at ee_body_R0 / ee_body_p0) and o_base in the base frame (at the origin, level), then the cofactor inverse of the inertia.
+// A zero mass is skipped, and with both skipped out is the nominal block bit for bit.  The host's srbd_constants and the payload estimator's commit kernel
+// both call this function.
+QMB_HD void srbd_payload_fold(const DevModel& d, const double* pl, double* out) {
+  const SrbdConst& nom = *reinterpret_cast<const SrbdConst*>(&d.total_mass);
+  SrbdLump whole; whole.m = nom.m; for (int i = 0; i < 3; ++i) whole.c[i] = -nom.c_nom[i]; for (int i = 0; i < 9; ++i) whole.I[i] = nom.I_nom[i];
+  double mass = nom.m; bool added = false;
+  for (int k = 0; pl && k < 2; ++k) {
+    const double m = pl[4 * k]; if (m == 0.0) continue;
+    double cb[3] = {pl[4 * k + 1], pl[4 * k + 2], pl[4 * k + 3]};
+    const double I3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, z3[3] = {0, 0, 0};
+    const double* R = k == 0 ? d.ee_body_R0 : I3; const double* p = k == 0 ? d.ee_body_p0 : z3;
+    if (k == 0) { double o[3]; matvec3(d.ee_R, cb, o); for (int i = 0; i < 3; ++i) cb[i] = o[i] + d.ee_p[i]; }
+    double c[3]; matvec3(R, cb, c); for (int i = 0; i < 3; ++i) c[i] += p[i];
+    const double I0[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; lump_add(whole, m, c, I0); mass += m; added = true;
+  }
+  double* o = out; o[0] = mass;
+  for (int i = 0; i < 9; ++i) o[1 + i] = whole.I[i];
+  if (added) inv3(whole.I, o + 10); else for (int i = 0; i < 9; ++i) o[10 + i] = nom.I_nom_inv[i];
+  for (int i = 0; i < 3; ++i) o[19 + i] = -whole.c[i];
+  for (int i = 22; i < SRBD_DBL; ++i) o[i] = 0.0;
+}
+
 // modeNumber2StanceLeg: bit3 LF, bit2 RF, bit1 LH, bit0 RH (contact order LF,RF,LH,RH)
 QMB_HD bool contact_flag(int mode, int foot) { return (mode >> (3 - foot)) & 1; }
 

@@ -369,6 +369,56 @@ class Solver:
         self._chk(self.lib.qmb200_get_model_payload(self.h, _p(pl), C.byref(is_set)), "qmb200_get_model_payload")
         return pl if is_set.value else None
 
+    # ---------------- online payload estimate (include/qmb200.h: qmb200_payload_est_*; DESIGN.md §4.6) ----------------
+    def payload_est_get_params(self):
+        """→ dict of qmb200_payload_est_params."""
+        p = _lib.PayloadEstParams(); self._chk(self.lib.qmb200_payload_est_get_params(self.h, C.byref(p)), "qmb200_payload_est_get_params")
+        return {n: getattr(p, n) for n, _ in _lib.PayloadEstParams._fields_}
+
+    def payload_est_set_params(self, **params):
+        """Keyword per field of qmb200_payload_est_params; unspecified fields keep their value."""
+        p = _lib.PayloadEstParams(); self._chk(self.lib.qmb200_payload_est_get_params(self.h, C.byref(p)), "qmb200_payload_est_get_params")
+        names = [n for n, _ in _lib.PayloadEstParams._fields_]
+        for k, v in params.items():
+            if k not in names:
+                raise ValueError("payload_est_set_params: unknown parameter %r (one of %s)" % (k, ", ".join(names)))
+            setattr(p, k, float(v))
+        self._chk(self.lib.qmb200_payload_est_set_params(self.h, C.byref(p)), "qmb200_payload_est_set_params")
+
+    def payload_est_reset(self, prior=None):
+        """(Re)start the estimator of every robot from prior [B, 8] (layout _lib.PAYLOAD_LAYOUT; None: the current model payload, zeros when none is set).
+        Sets the model payload to prior.  Synchronous."""
+        pl = None if prior is None else _f64(prior, (self.batch, 8))
+        self._chk(self.lib.qmb200_payload_est_reset(self.h, _p(pl)), "qmb200_payload_est_reset")
+
+    def payload_est_step(self, dt, effort, rbd):
+        """One RLS update per robot from the measurement rbd [B, 55] and the effort [B, 18] held over the dt s that ended at it → status [B]."""
+        B = self.batch; st = np.zeros(B, dtype=np.int32)
+        self._chk(self.lib.qmb200_payload_est_step(self.h, float(dt), _p(_f64(effort, (B, 18))), _p(_f64(rbd, (B, RBD))), _p(st)), "qmb200_payload_est_step")
+        return st
+
+    def payload_est_step_dev(self, dt, effort, rbd, status, stream=None):
+        """Device-pointer variant: status [B] int32 written; no synchronisation."""
+        self._chk(self.lib.qmb200_payload_est_step_dev(self.h, float(dt), _p(effort), _p(rbd), _p(status), C.c_void_p(stream) if stream else None), "qmb200_payload_est_step_dev")
+
+    def payload_est_commit_dev(self, stream=None):
+        """The estimate → the end-effector half of every robot's model payload and its SRBD constants, in stream order; no synchronisation."""
+        self._chk(self.lib.qmb200_payload_est_commit_dev(self.h, C.c_void_p(stream) if stream else None), "qmb200_payload_est_commit_dev")
+
+    def payload_est_get(self):
+        """→ dict(theta [B, 10] (layout _lib.THETA_LAYOUT), p_diag [B, 10], samples [B]).  Synchronous."""
+        B = self.batch; th = np.zeros((B, 10)); pd = np.zeros((B, 10)); n = np.zeros(B, dtype=np.int32)
+        self._chk(self.lib.qmb200_payload_est_get(self.h, _p(th), _p(pd), _p(n)), "qmb200_payload_est_get")
+        return dict(theta=th, p_diag=pd, samples=n)
+
+    def payload_est_stop(self):
+        """Release the estimator state; the model payload keeps its last committed rows."""
+        self._chk(self.lib.qmb200_payload_est_stop(self.h), "qmb200_payload_est_stop")
+
+    def get_model_payload_dev(self, out, stream=None):
+        """Copy the model payload rows the kernels read into the device tensor out [B, 8] in stream order (no synchronisation)."""
+        self._chk(self.lib.qmb200_get_model_payload_dev(self.h, _p(out), C.c_void_p(stream) if stream else None), "qmb200_get_model_payload_dev")
+
     def sim_set_terrain(self, tiles=None, cell=None):
         """Heightfield tile library of the plant: tiles [T, ny, nx] absolute world z (m) on nodes `cell` m apart (qm_control_b200.terrain builds them).
         None clears the library and every robot's terrain.  Synchronous."""

@@ -13,6 +13,10 @@ any of it, unless --model-payload plant sets the controller's model payload to t
 and the bins are then those of the told controller, and "vary" gains "payload_kg_not_told", the payload bins of the same sweep with the controller
 not told, from one more (untimed) run.
 
+--model-payload estimate runs the online payload estimator in the loop (closed_loop.run(payload_estimator=True)): the timed run and the bins are then those
+of the estimating controller; "vary" gains "payload_kg_not_told" as above and, per payload bin, the p50 / max of |m_hat - m| at the end; the JSON line
+gains "payload_est": the estimator's device time per call at this batch (CUDA events, alternated with blocks of plant steps).
+
 --terrain runs the loop on heightfield terrain (qm_control_b200.terrain): robot b's tile rises beyond 0.35 m ahead of its start, as a ramp of 0/5/10/15
 degrees and steps of 0/3/6/9 cm rise every 0.3 m on it, every combination equally often; the controller does not see the terrain.  The JSON line gains
 "terrain": fallen robots (height above the ground under the base <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite) and base distance per bin of
@@ -73,12 +77,45 @@ def plant_step_times(solver, ter, xy_yaw, reps=7, calls=20):
             "spread_terrain": [float(min(times["terrain"])), float(max(times["terrain"]))], "spread_flat": [float(min(times["flat"])), float(max(times["flat"]))]}
 
 
+def est_step_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per payload-estimator call and per 1 ms plant step of the whole batch, alternated `reps` times in blocks of `calls` from one standing
+    state (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    prev = solver.get_model_payload(); solver.payload_est_reset(np.zeros((B, 8)))
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+    times = {"estimator": [], "plant": []}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode in ("estimator", "plant"):
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    if mode == "estimator":
+                        solver.payload_est_step_dev(1e-3, eff, rbd, st, s.cuda_stream)
+                    else:
+                        solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.payload_est_stop(); solver.set_model_payload(prev)
+    return {"label": "device time per payload-estimator call and per 1 ms plant step of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            "ms_per_call": float(np.median(times["estimator"])), "ms_per_plant_step": float(np.median(times["plant"])),
+            "spread": [float(min(times["estimator"])), float(max(times["estimator"]))]}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
     ap.add_argument("--gait", default="trot"); ap.add_argument("--vx", type=float, default=0.3)
     ap.add_argument("--vary", action="store_true", help="per-robot sweep of EE payload, floor friction and a lateral base push")
-    ap.add_argument("--model-payload", choices=["plant"], help="tell the controller the plant's payload (its model payload, Solver.set_model_payload)")
+    ap.add_argument("--model-payload", choices=["plant", "estimate"],
+                    help="plant: tell the controller the plant's payload (its model payload, Solver.set_model_payload); estimate: run the online payload estimator")
     ap.add_argument("--terrain", action="store_true", help="per-robot sweep of ramp angle and step rise under the feet")
     args = ap.parse_args()
     if args.vary and args.terrain:
@@ -105,7 +142,7 @@ def main():
         tiles = np.stack([T.ramp(a, start=0.35) + T.stairs(r, 0.3, start=0.35) for a in bins["ramp_deg"] for r in bins["step_rise_m"]])
         ter = dict(tiles=tiles, cell=T.CELL, tile=idx["ramp_deg"] * 4 + idx["step_rise_m"], origin=T.centred_origin(xy[:, :2]))
         kw = dict(terrain=ter)
-    told = dict(model_payload=args.model_payload) if args.model_payload else {}
+    told = {"plant": dict(model_payload="plant"), "estimate": dict(payload_estimator=True), None: {}}[args.model_payload]
     closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told)   # warm-up run of the same length
     pairs = []
 
@@ -142,13 +179,20 @@ def main():
     if args.vary:
         extra["vary"] = {"label": "per-robot sweep; fallen = min base z <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite", "push": "lateral +y base force for 0.1 s from 0.4 s",
                          "bins": {axis: vary_bins(r, axis) for axis in bins}}
+        if args.model_payload == "estimate":
+            err = np.abs(r["payload_est"][-1, :, 0] - kw["payload"][:, 0])
+            extra["vary"]["payload_estimate_error_kg"] = [{"value": float(val), "p50": float(np.percentile(err[idx["payload_kg"] == i], 50)), "max": float(np.max(err[idx["payload_kg"] == i]))}
+                                                          for i, val in enumerate(bins["payload_kg"])]
         if args.model_payload:
-            extra["vary"]["model_payload"] = "the controller is told the plant's payload (bins); payload_kg_not_told: the same sweep, controller not told"
+            extra["vary"]["model_payload"] = {"plant": "the controller is told the plant's payload (bins)", "estimate": "the controller runs the online payload estimate (bins)"}[
+                args.model_payload] + "; payload_kg_not_told: the same sweep, controller not told"
             extra["vary"]["payload_kg_not_told"] = vary_bins(closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw), "payload_kg")
     if args.terrain:
         extra["terrain"] = {"label": "per-robot sweep, controller blind to the terrain; fallen = height above the ground under the base <= 0.3 m or |roll|, |pitch| >= 0.3 rad "
                                      "or non-finite", "tiles": "ground z = 0 up to 0.35 m ahead of the start, then a ramp (deg) with steps (rise m, run 0.3 m) on it",
                             "bins": {axis: vary_bins(r, axis) for axis in bins}, "plant_step": plant_step_times(solver, ter, xy)}
+    if args.model_payload == "estimate":
+        extra["payload_est"] = {**est_step_times(solver, xy), "gpu": name, "power_limit": limit}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
