@@ -16,6 +16,8 @@ The start mirrors QMController::starting (QMController.cpp:98-126): the first ob
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
 """
+import contextlib
+
 import numpy as np
 
 from ._lib import EMAX, KMAX, NX, RBD, TARGET
@@ -64,55 +66,73 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     payload_est[ticks, B, 8] = the model payload rows committed at each record's MPC tick)."""
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
-    if terrain is not None:
-        prev_lib, prev_robot = solver.sim_get_terrain(), solver.sim_get_robot_terrain()
-        try:
-            solver.sim_set_robot_terrain(None)
-            solver.sim_set_terrain(terrain["tiles"], terrain["cell"])
-            solver.sim_set_robot_terrain(terrain["tile"], terrain["origin"])
-            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, model_payload,
-                       payload_estimator=payload_estimator)
-        finally:
-            solver.sim_set_robot_terrain(None)   # the previous library may have fewer tiles than this run's robots reference
-            if prev_lib is None:
-                solver.sim_set_terrain(None)
-            else:
-                solver.sim_set_terrain(**prev_lib)
-            if prev_robot is not None:
-                solver.sim_set_robot_terrain(**prev_robot)
-    if model_payload is not None:
-        prev_model = solver.get_model_payload()
-        try:
-            if isinstance(model_payload, str):
-                if model_payload != "plant":
-                    raise ValueError("closed_loop.run: model_payload must be None, \"plant\" or an array [%d, 8], got %r" % (solver.batch, model_payload))
-                plant = payload if payload is not None else solver.sim_get_robot_params()["payload"]
-                model_payload = np.zeros((solver.batch, 8)) if plant is None else plant
-            solver.set_model_payload(model_payload)
-            return run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, payload_estimator=payload_estimator)
-        finally:
-            solver.set_model_payload(prev_model)
-    if payload_estimator is not None:
-        prev_model, prev_params = solver.get_model_payload(), solver.payload_est_get_params()
-        try:
-            if isinstance(payload_estimator, dict):
-                solver.payload_est_set_params(**payload_estimator)
-            solver.payload_est_reset()
-            return _plant_params(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, True)
-        finally:
-            solver.payload_est_stop()
-            solver.set_model_payload(prev_model)
-            solver.payload_est_set_params(**prev_params)
-    return _plant_params(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, False)
+    # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
+    with contextlib.ExitStack() as scope:
+        if terrain is not None:
+            scope.enter_context(_terrain(solver, terrain))
+        if model_payload is not None:
+            scope.enter_context(_model_payload(solver, model_payload, payload))
+        if payload_estimator is not None:
+            scope.enter_context(_payload_estimator(solver, payload_estimator))
+        if friction_mu is not None or payload is not None:
+            scope.enter_context(_robot_params(solver, friction_mu, payload))
+        return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
+                    torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None)
 
 
-def _plant_params(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, friction_mu, payload, pushes, est):
-    if friction_mu is None and payload is None:
-        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est)
+@contextlib.contextmanager
+def _terrain(solver, terrain):
+    prev_lib, prev_robot = solver.sim_get_terrain(), solver.sim_get_robot_terrain()
+    try:
+        solver.sim_set_robot_terrain(None)
+        solver.sim_set_terrain(terrain["tiles"], terrain["cell"])
+        solver.sim_set_robot_terrain(terrain["tile"], terrain["origin"])
+        yield
+    finally:
+        solver.sim_set_robot_terrain(None)   # the previous library may have fewer tiles than this run's robots reference
+        if prev_lib is None:
+            solver.sim_set_terrain(None)
+        else:
+            solver.sim_set_terrain(**prev_lib)
+        if prev_robot is not None:
+            solver.sim_set_robot_terrain(**prev_robot)
+
+
+@contextlib.contextmanager
+def _model_payload(solver, model_payload, payload):
+    prev_model = solver.get_model_payload()
+    try:
+        if isinstance(model_payload, str):
+            if model_payload != "plant":
+                raise ValueError("closed_loop.run: model_payload must be None, \"plant\" or an array [%d, 8], got %r" % (solver.batch, model_payload))
+            plant = payload if payload is not None else solver.sim_get_robot_params()["payload"]
+            model_payload = np.zeros((solver.batch, 8)) if plant is None else plant
+        solver.set_model_payload(model_payload)
+        yield
+    finally:
+        solver.set_model_payload(prev_model)
+
+
+@contextlib.contextmanager
+def _payload_estimator(solver, params):
+    prev_model, prev_params = solver.get_model_payload(), solver.payload_est_get_params()
+    try:
+        if isinstance(params, dict):
+            solver.payload_est_set_params(**params)
+        solver.payload_est_reset()
+        yield
+    finally:
+        solver.payload_est_stop()
+        solver.set_model_payload(prev_model)
+        solver.payload_est_set_params(**prev_params)
+
+
+@contextlib.contextmanager
+def _robot_params(solver, friction_mu, payload):
     prev = solver.sim_get_robot_params()
     solver.sim_set_robot_params(friction_mu=prev["friction_mu"] if friction_mu is None else friction_mu, payload=prev["payload"] if payload is None else payload)
     try:
-        return _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est)
+        yield
     finally:
         solver.sim_set_robot_params(**prev)
 

@@ -31,7 +31,7 @@ def run(oracle, duration=0.2, cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, t_s
     twin = SimTwin(); tgt = TargetOracle(); hw = HwSimOracle(delay)
     add = recorder.add if recorder is not None else (lambda stage, inp, out: None)
     if recorder is not None:
-        recorder.meta.update(friction_mu=None, payload=None, model_payload=None)
+        recorder.meta.update(friction_mu=None, payload=None, model_payload=None, terrain=None)
     a1 = lambda v: np.array([v], dtype=np.float64)
 
     def step(duration, effort, q, v):

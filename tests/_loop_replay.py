@@ -16,18 +16,16 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from _oracle import TASK, HwSimOracle, TargetOracle
-from _parity import CMD_BLOCKS, MPC_TOL, WBC_TOL, cmd_errors, traj_errors
+from _parity import CMD_BLOCKS, MPC_TOL, PLANT_TOL, Q_BLOCKS, RBD_BLOCKS, WBC_TOL, block_errors, cmd_errors, traj_errors
+from _sim_twin_terrain import robot_terrain
 
 NOT_PD, NO_STEP, SAFETY = 8, 16, 0x10000
 NEAR = 1e-9           # relative distance of a line-search acceptance test from its threshold that round-off can cross
-PLANT_TOL = 1e-8      # per block, as tests/test_sim_variation_gpu.py
-Q_BLOCKS = {"pos": slice(0, 3), "euler": slice(3, 6), "joints": slice(6, 24)}
-RBD_BLOCKS = {"euler": slice(0, 3), "pos": slice(3, 6), "joints": slice(6, 24), "w": slice(24, 27), "v_lin": slice(27, 30), "joint_vel": slice(30, 48), "ee_pos": slice(48, 51),
-              "ee_quat": slice(51, 55)}
 
 
 class Record:
-    """meta: friction_mu [B] or None, payload [B, 8] or None (the plant's), model_payload [B, 8] or None; calls: (stage, inputs, outputs) in call order."""
+    """meta: friction_mu [B] or None, payload [B, 8] or None (the plant's), model_payload [B, 8] or None, terrain dict(tiles [T, ny, nx] or None, cell or
+    None, tile [B], origin [B, 2]) or None (the plant's ground); calls: (stage, inputs, outputs) in call order."""
 
     def __init__(self):
         self.meta = {}; self.calls = []
@@ -68,6 +66,8 @@ def record(solver, fn):
             torch.cuda.synchronize()
             if not rec.meta:
                 p = solver.sim_get_robot_params(); rec.meta.update(friction_mu=p["friction_mu"], payload=p["payload"], model_payload=solver.get_model_payload())
+                lib, robot = solver.sim_get_terrain(), solver.sim_get_robot_terrain()
+                rec.meta["terrain"] = None if robot is None else dict(tiles=None if lib is None else lib["tiles"], cell=None if lib is None else lib["cell"], **robot)
             inp = {("prob" if k == "prob_dev" else k): _host(a[k]) for k in ins}
             if stage == "mpc":
                 inp["before"] = solver.mpc_get_solution()
@@ -255,24 +255,21 @@ def replay_hw_write(rec, delay):
 
 
 # ---------------- plant ----------------
-def _rel(a, b, blocks):
-    return {k: float(np.max(np.abs(a[s] - b[s])) / max(1.0, float(np.max(np.abs(b[s]))))) for k, s in blocks.items()}
-
-
 def replay_plant(rec, twin, every=1):
-    """Every `every`-th plant step of every robot on the twin with the robot's friction, payload and wrench of that step, at PLANT_TOL per block;
-    contact mask and status exact."""
-    mu, pl = rec.meta.get("friction_mu"), rec.meta.get("payload"); worst = {}; n = 0; pushed = 0
+    """Every `every`-th plant step of every robot on the twin (a tests/_sim_twin_terrain.SimTwinTerrain) with the robot's friction, payload, wrench and
+    ground of that step, at PLANT_TOL per block; contact mask and status exact."""
+    mu, pl, ter = rec.meta.get("friction_mu"), rec.meta.get("payload"), rec.meta.get("terrain"); worst = {}; n = 0; pushed = 0
     for i, (inp, out) in enumerate(rec.of("sim")):
         if i % every:
             continue
         B = len(inp["q"]); w = inp["wrench"]
         for b in range(B):
             wb = None if w is None else w[b]; pushed += int(wb is not None and np.any(wb != 0))
-            q, v, rbd, c, st = twin.step_ext(inp["duration"], inp["effort"][b], inp["q"][b], inp["v"][b], None if mu is None else mu[b], None if pl is None else pl[b], wb)
+            q, v, rbd, c, st = twin.step_ext(inp["duration"], inp["effort"][b], inp["q"][b], inp["v"][b], None if mu is None else mu[b], None if pl is None else pl[b], wb,
+                                             terrain=robot_terrain(ter, b))
             assert out["contact"][b] == c and out["status"][b] == st, ("plant step %d robot %d" % (i, b), out["contact"][b], c, out["status"][b], st)
             for name, a, r, blocks in (("q", out["q"][b], q, Q_BLOCKS), ("v", out["v"][b], v, Q_BLOCKS), ("rbd", out["rbd"][b], rbd, RBD_BLOCKS)):
-                err = _rel(a, r, blocks)
+                err = block_errors(a, r, blocks)
                 assert max(err.values()) < PLANT_TOL, ("plant step %d robot %d" % (i, b), name, err)
                 for k, e in err.items():
                     worst[name + ":" + k] = max(worst.get(name + ":" + k, 0.0), e)

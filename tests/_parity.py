@@ -21,11 +21,15 @@ WBC_TOL = 1e-8           # asserted: one WbcBase::update on identical inputs, pe
 MPCWBC_TOL = 1e-8        # asserted: HierarchicalMpcWbc (arm torque limits active, arm accelerations of 1e4 rad/s^2 behind a 3e3-conditioned 6x6 block); both sides are KKT
                          # points to 1e-11 once the oracle refines its levels on the active set, observed agreement ~1e-11
 TICK_TOL = 1e-6          # asserted: MPC -> evaluatePolicy -> WBC chain (the WBC's PD laws multiply the MPC's ~1e-11 by gains up to 6000: still a decade below the contract)
+PLANT_TOL = 1e-8         # asserted: one plant step against the CPU plant twin, per block of q, v and the measurement rbd
 
 # name -> (lo, hi, floor)
 X_BLOCKS = {"h_lin/m": (0, 3, 0.1), "h_ang/m": (3, 6, 0.05), "base_pos": (6, 9, 0.1), "base_zyx": (9, 12, 0.1), "leg_q": (12, 24, 0.1), "arm_q": (24, 30, 0.1)}
 U_BLOCKS = {"force": (0, 12, 10.0), "leg_qd": (12, 24, 0.1), "arm_qd": (24, 30, 0.1)}
 CMD_BLOCKS = {"base_lin_acc": (0, 3, 1.0), "base_ang_acc": (3, 6, 1.0), "leg_acc": (6, 18, 1.0), "arm_acc": (18, 24, 1.0), "force": (24, 36, 10.0), "leg_torque": (36, 48, 1.0), "arm_torque": (48, 54, 1.0)}
+Q_BLOCKS = {"pos": (0, 3, 1.0), "euler": (3, 6, 1.0), "joints": (6, 24, 1.0)}                    # the plant's q [24] and v [24]
+RBD_BLOCKS = {"euler": (0, 3, 1.0), "pos": (3, 6, 1.0), "joints": (6, 24, 1.0), "w": (24, 27, 1.0), "v_lin": (27, 30, 1.0), "joint_vel": (30, 48, 1.0), "ee_pos": (48, 51, 1.0),
+              "ee_quat": (51, 55, 1.0)}                                                            # the plant's measurement rbd [55]
 
 _LOG = os.environ.get("QMB_PARITY_LOG")
 

@@ -9,7 +9,7 @@ import pytest
 import _closed_loop_cpu
 import _loop_replay as R
 from _oracle import Oracle
-from _sim_twin_ext import SimTwinExt
+from _sim_twin_terrain import SimTwinTerrain
 
 T_START, DURATION = 10.0, 0.1
 
@@ -36,7 +36,7 @@ def test_replay_reproduces_the_rehearsal_exactly(rehearsal):
     assert up["replayed"] == 50 and up["swing"] > 0 and up["certified"] == 0
     assert all(v == 0.0 for v in up["worst"].values()), up["worst"]
     assert R.replay_hw_write(rec, 0.009)["replayed"] == 100
-    pl = R.replay_plant(rec, SimTwinExt())
+    pl = R.replay_plant(rec, SimTwinTerrain())
     assert pl["replayed"] == 101 and pl["pushed"] == 0 and all(v == 0.0 for v in pl["worst"].values()), pl
 
 

@@ -14,7 +14,7 @@ import pytest
 import _loop_replay as R
 from _oracle import Oracle
 from _payload_urdf import edited_urdf
-from _sim_twin_ext import SimTwinExt
+from _sim_twin_terrain import SimTwinTerrain
 from qm_control_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -71,7 +71,7 @@ def test_closed_loop_replays_call_by_call(tmp_path):
     n_solves, n_updates = int(round(DURATION * 100)), int(round(DURATION * 500))
 
     stages = dict(targets=lambda: R.replay_targets(rec), mpc=lambda: R.replay_mpc(rec, oracles), invariant=lambda: R.replay_invariant(rec),
-                  update=lambda: R.replay_update(rec, oracles), hw_write=lambda: R.replay_hw_write(rec, 0.009), plant=lambda: R.replay_plant(rec, SimTwinExt()))
+                  update=lambda: R.replay_update(rec, oracles), hw_write=lambda: R.replay_hw_write(rec, 0.009), plant=lambda: R.replay_plant(rec, SimTwinTerrain()))
     out = {}; failed = {}; secs = {}
     for name, replay in stages.items():          # every stage runs and reports before the first failure is raised
         t1 = time.time()

@@ -4,17 +4,12 @@ import numpy as np
 import pytest
 
 import _closed_loop_cpu
+from _parity import PLANT_TOL, Q_BLOCKS, RBD_BLOCKS, block_errors
 from _sim_twin import DEFAULTS, SimTwin
 
 pytestmark = pytest.mark.gpu
 
 B = 256
-BLOCKS = {"pos": slice(0, 3), "euler": slice(3, 6), "joints": slice(6, 24)}
-RBD_BLOCKS = {"euler": slice(0, 3), "pos": slice(3, 6), "joints": slice(6, 24), "w": slice(24, 27), "v_lin": slice(27, 30), "joint_vel": slice(30, 48), "ee_pos": slice(48, 51), "ee_quat": slice(51, 55)}
-
-
-def _rel(a, b, blocks):
-    return {k: float(np.max(np.abs(a[:, s] - b[:, s])) / max(1.0, float(np.max(np.abs(b[:, s]))))) for k, s in blocks.items()}
 
 
 @pytest.fixture(scope="module")
@@ -67,9 +62,9 @@ def test_sim_step_matches_the_twin(solver, twin, oracle):
     np.testing.assert_array_equal(cg, ct)
     g = np.arange(B) // 32
     assert np.all(ct[g == 0] == 0) and np.count_nonzero(ct) >= B // 8 and len(set(ct.tolist())) >= 5, ct   # a foot pushed in deep rebounds within the 1 ms
-    for name, a, b, blocks in (("q", qg, qt, BLOCKS), ("v", vg, vt, BLOCKS), ("rbd", rg, rt, RBD_BLOCKS)):
-        err = _rel(a, b, blocks)
-        assert max(err.values()) < 1e-8, (name, err)
+    for name, a, b, blocks in (("q", qg, qt, Q_BLOCKS), ("v", vg, vt, Q_BLOCKS), ("rbd", rg, rt, RBD_BLOCKS)):
+        err = block_errors(a, b, blocks)
+        assert max(err.values()) < PLANT_TOL, (name, err)
 
 
 def test_batch_position_invariance(solver, twin, oracle):

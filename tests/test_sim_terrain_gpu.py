@@ -7,18 +7,17 @@ import numpy as np
 import pytest
 
 import _loop_replay as R
-import _loop_replay_terrain as RT
 from _oracle import Oracle
+from _parity import PLANT_TOL, Q_BLOCKS, RBD_BLOCKS, block_errors
 from _sim_twin import DEFAULTS
 from _sim_twin_terrain import SimTwinTerrain
 from qm_control_b200 import terrain as T
-from test_sim_variation_gpu import BLOCKS, RBD_BLOCKS, _rel, _states, _variation
+from test_sim_variation_gpu import _states, _variation
 
 pytestmark = pytest.mark.gpu
 
 B = 256                  # the state groups of test_sim_gpu.py / test_sim_variation_gpu.py
 SIZE, CELL = 4.0, 0.02
-TOL = 1e-8
 
 
 @pytest.fixture(scope="module")
@@ -66,9 +65,9 @@ def _compare(got, ref, tag):
     assert np.all(sg == 0) and np.all(st == 0), tag
     np.testing.assert_array_equal(cg, ct, err_msg=tag)
     worst = {}
-    for name, a, b, blocks in (("q", qg, qt, BLOCKS), ("v", vg, vt, BLOCKS), ("rbd", rg, rt, RBD_BLOCKS)):
-        err = _rel(a, b, blocks); worst[name] = max(err.values())
-        assert worst[name] < TOL, (tag, name, err)
+    for name, a, b, blocks in (("q", qg, qt, Q_BLOCKS), ("v", vg, vt, Q_BLOCKS), ("rbd", rg, rt, RBD_BLOCKS)):
+        err = block_errors(a, b, blocks); worst[name] = max(err.values())
+        assert worst[name] < PLANT_TOL, (tag, name, err)
     return worst
 
 
@@ -237,7 +236,7 @@ def _rotation_errors(on_ramp, n_ms):
         if a[2][54] < 0:
             a[2][51:55] *= -1
         b = _rotate_back(qk[1], vk[1], rk[1], centre[1], psi)
-        errs.append(max(max(_rel(x[None], y[None], bl).values()) for x, y, bl in zip(a, b, (BLOCKS, BLOCKS, RBD_BLOCKS))))
+        errs.append(max(max(block_errors(x, y, bl).values()) for x, y, bl in zip(a, b, (Q_BLOCKS, Q_BLOCKS, RBD_BLOCKS))))
         assert ck[0] == ck[1], k
     return np.array(errs)
 
@@ -376,13 +375,13 @@ def test_closed_loop_on_a_ramp_replays_call_by_call():
         xy = np.zeros((n, 3)); xy[:, 0] = 2.0 * np.arange(n)
         tiles = np.stack([T.ramp(8.0, 0.0, start=0.3), T.ramp(6.0, 90.0)]); tile = np.arange(n) % 2
         ter = dict(tiles=tiles, cell=CELL, tile=tile, origin=T.centred_origin(xy[:, :2]))
-        res, rec = RT.record(s, lambda: closed_loop.run(s, duration=0.1, gait="trot", cmd_vel=(0.3, 0.0, 0.0, 0.0), xy_yaw=xy, terrain=ter))
+        res, rec = R.record(s, lambda: closed_loop.run(s, duration=0.1, gait="trot", cmd_vel=(0.3, 0.0, 0.0, 0.0), xy_yaw=xy, terrain=ter))
     finally:
         s.close()
     np.testing.assert_array_equal(rec.meta["terrain"]["tile"], tile); np.testing.assert_array_equal(rec.meta["terrain"]["tiles"], tiles)
     oracles = [Oracle()] * n
     tg = R.replay_targets(rec); mpc = R.replay_mpc(rec, oracles); up = R.replay_update(rec, oracles); hw = R.replay_hw_write(rec, 0.009)
-    pl = RT.replay_plant(rec, SimTwinTerrain())
+    pl = R.replay_plant(rec, SimTwinTerrain())
     print("ramp closed loop replay: plant %d robot-steps, worst %s; mpc %d robot-solves; update %d; hw_write %d; targets %d" % (
         pl["replayed"], {k: "%.1e" % e for k, e in pl["worst"].items()}, mpc["replayed"], up["replayed"], hw["replayed"], tg["replayed"]))
     assert pl["replayed"] == 101 * n and hw["replayed"] == 100 * n and up["replayed"] == 50 * n and mpc["replayed"] + mpc["excused"] == 10 * n

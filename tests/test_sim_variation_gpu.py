@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 import _closed_loop_cpu
+from _parity import PLANT_TOL, Q_BLOCKS, RBD_BLOCKS, block_errors
 from _sim_twin import DEFAULTS
 from _sim_twin_ext import SimTwinExt
 from qm_control_b200 import _lib
@@ -11,14 +12,8 @@ from qm_control_b200 import _lib
 pytestmark = pytest.mark.gpu
 
 B = 256
-BLOCKS = {"pos": slice(0, 3), "euler": slice(3, 6), "joints": slice(6, 24)}
 PL = {n: i for i, n in enumerate(_lib.PAYLOAD_LAYOUT)}
 WR = {n: i for i, n in enumerate(_lib.WRENCH_LAYOUT)}
-RBD_BLOCKS = {"euler": slice(0, 3), "pos": slice(3, 6), "joints": slice(6, 24), "w": slice(24, 27), "v_lin": slice(27, 30), "joint_vel": slice(30, 48), "ee_pos": slice(48, 51), "ee_quat": slice(51, 55)}
-
-
-def _rel(a, b, blocks):
-    return {k: float(np.max(np.abs(a[:, s] - b[:, s])) / max(1.0, float(np.max(np.abs(b[:, s]))))) for k, s in blocks.items()}
 
 
 @pytest.fixture(scope="module")
@@ -84,9 +79,9 @@ def test_step_ext_matches_the_twin(solver, twin, oracle, kind):
     qt, vt, rt, ct, st = twin.step_batch_ext(1e-3, eff, q, v, mu=mu, payload=pl, wrench=wr)
     assert np.all(sg == 0) and np.all(st == 0)
     np.testing.assert_array_equal(cg, ct)
-    for name, a, b, blocks in (("q", qg, qt, BLOCKS), ("v", vg, vt, BLOCKS), ("rbd", rg, rt, RBD_BLOCKS)):
-        err = _rel(a, b, blocks)
-        assert max(err.values()) < 1e-8, (kind, name, err)
+    for name, a, b, blocks in (("q", qg, qt, Q_BLOCKS), ("v", vg, vt, Q_BLOCKS), ("rbd", rg, rt, RBD_BLOCKS)):
+        err = block_errors(a, b, blocks)
+        assert max(err.values()) < PLANT_TOL, (kind, name, err)
     qp, vp, _, _, _ = solver.sim_step(1e-3, eff, q, v)   # the variation changes the step
     assert np.max(np.abs(vp - vg)) > 1e-6
 
