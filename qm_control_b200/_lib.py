@@ -50,22 +50,98 @@ SRBD_LAYOUT = ("m",) + tuple("I_nom_%d%d" % (i, j) for i in range(3) for j in ra
 WRENCH_LAYOUT = ("f_base_x", "f_base_y", "f_base_z", "n_base_x", "n_base_y", "n_base_z", "f_ee_x", "f_ee_y", "f_ee_z", "n_ee_x", "n_ee_y", "n_ee_z")
 
 
-# every symbol include/qmb200.h declares (checked by the CPU test-suite)
-SYMBOLS = ["qmb200_create", "qmb200_destroy", "qmb200_last_error", "qmb200_get_dims", "qmb200_get_model_info", "qmb200_get_joint_name",
-           "qmb200_wbc_update", "qmb200_wbc_update_dev", "qmb200_wbc_set_input_last", "qmb200_wbc_get_input_last", "qmb200_wbc_get_gains", "qmb200_wbc_set_gains", "qmb200_wbc_get_diagnostics", "qmb200_wbc_set_iteration_caps",
-           "qmb200_mpc_solve", "qmb200_mpc_solve_dev", "qmb200_mpc_set_iterations", "qmb200_mpc_set_solver", "qmb200_mpc_get_solver", "qmb200_mpc_reset", "qmb200_mpc_set_solution", "qmb200_mpc_get_solution",
-           "qmb200_policy_eval", "qmb200_policy_eval_dev", "qmb200_tick", "qmb200_tick_dev", "qmb200_centroidal_state_from_rbd",
-           "qmb200_gait_schedule", "qmb200_launch_count", "qmb200_stream", "qmb200_debug_get_step",
-           "qmb200_gait_create", "qmb200_gait_destroy", "qmb200_gait_insert_template", "qmb200_gait_get_mode_schedule",
-           "qmb200_observation_update", "qmb200_observation_update_dev", "qmb200_target_trajectories", "qmb200_target_trajectories_dev", "qmb200_initial_ee_target",
-           "qmb200_control_law", "qmb200_control_law_dev", "qmb200_set_arm_gains", "qmb200_hw_write", "qmb200_hw_write_dev", "qmb200_hw_set_delay", "qmb200_update", "qmb200_update_dev",
-           "qmb200_debug_model_blob", "qmb200_comm_get_unique_id", "qmb200_comm_init", "qmb200_comm_destroy", "qmb200_comm_info", "qmb200_allgather_torque", "qmb200_gait_bin_permutation", "qmb200_set_pipeline", "qmb200_set_profiling", "qmb200_collect_kernel_times", "qmb200_get_kernel_times", "qmb200_get_flow_kernel_time", "qmb200_measure_fp64_peak",
-           "qmb200_sim_get_params", "qmb200_sim_set_params", "qmb200_sim_step", "qmb200_sim_step_dev", "qmb200_sim_standing_state",
-           "qmb200_sim_set_robot_params", "qmb200_sim_get_robot_params", "qmb200_sim_step_ext", "qmb200_sim_step_ext_dev",
-           "qmb200_sim_set_terrain", "qmb200_sim_get_terrain", "qmb200_sim_set_robot_terrain", "qmb200_sim_get_robot_terrain",
-           "qmb200_set_model_payload", "qmb200_get_model_payload", "qmb200_debug_srbd_constants",
-           "qmb200_payload_est_get_params", "qmb200_payload_est_set_params", "qmb200_payload_est_reset", "qmb200_payload_est_step", "qmb200_payload_est_step_dev",
-           "qmb200_payload_est_commit_dev", "qmb200_payload_est_get", "qmb200_payload_est_stop", "qmb200_get_model_payload_dev"]
+# every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
+# None), except the file-name strings and the config struct; int and int32_t are c_int32.  The CPU test-suite checks each slot against the header.
+P, I32, I64, D, S, CFG = C.c_void_p, C.c_int32, C.c_int64, C.c_double, C.c_char_p, C.POINTER(Config)
+PROTOTYPES = {
+    "qmb200_create": (I32, [CFG, P]),
+    "qmb200_destroy": (None, [P]),
+    "qmb200_last_error": (S, [P]),
+    "qmb200_get_dims": (I32, [P] * 5),
+    "qmb200_get_model_info": (I32, [P] * 6),
+    "qmb200_get_joint_name": (I32, [P, I32, P, I32]),
+    "qmb200_wbc_update": (I32, [P] * 9),
+    "qmb200_wbc_update_dev": (I32, [P] * 10),
+    "qmb200_wbc_set_input_last": (I32, [P] * 2),
+    "qmb200_wbc_get_input_last": (I32, [P] * 2),
+    "qmb200_wbc_get_gains": (I32, [P] * 2),
+    "qmb200_wbc_set_gains": (I32, [P] * 2),
+    "qmb200_wbc_get_diagnostics": (I32, [P] * 2),
+    "qmb200_wbc_set_iteration_caps": (I32, [P, I32, I32]),
+    "qmb200_mpc_solve": (I32, [P] * 16),
+    "qmb200_mpc_solve_dev": (I32, [P] * 10),
+    "qmb200_mpc_set_iterations": (I32, [P, I32, D]),
+    "qmb200_mpc_reset": (I32, [P]),
+    "qmb200_mpc_set_solution": (I32, [P] * 6),
+    "qmb200_mpc_get_solution": (I32, [P] * 8),
+    "qmb200_policy_eval": (I32, [P] * 5),
+    "qmb200_policy_eval_dev": (I32, [P] * 6),
+    "qmb200_tick": (I32, [P] * 14),
+    "qmb200_tick_dev": (I32, [P] * 15),
+    "qmb200_centroidal_state_from_rbd": (I32, [P, I32, P, P]),
+    "qmb200_set_model_payload": (I32, [P] * 2),
+    "qmb200_get_model_payload": (I32, [P] * 3),
+    "qmb200_payload_est_get_params": (I32, [P] * 2),
+    "qmb200_payload_est_set_params": (I32, [P] * 2),
+    "qmb200_payload_est_reset": (I32, [P] * 2),
+    "qmb200_payload_est_step": (I32, [P, D] + [P] * 3),
+    "qmb200_payload_est_step_dev": (I32, [P, D] + [P] * 4),
+    "qmb200_payload_est_commit_dev": (I32, [P] * 2),
+    "qmb200_payload_est_get": (I32, [P] * 4),
+    "qmb200_payload_est_stop": (I32, [P]),
+    "qmb200_get_model_payload_dev": (I32, [P] * 3),
+    "qmb200_gait_schedule": (I32, [S, S, D, D, D, P, P]),
+    "qmb200_gait_create": (I32, [S, S, P]),
+    "qmb200_gait_destroy": (None, [P]),
+    "qmb200_gait_insert_template": (I32, [P, S, S, D, D]),
+    "qmb200_gait_get_mode_schedule": (I32, [P, D, D, P, P]),
+    "qmb200_observation_update": (I32, [P] * 5),
+    "qmb200_observation_update_dev": (I32, [P] * 6),
+    "qmb200_target_trajectories": (I32, [P, I32] + [P] * 8),
+    "qmb200_target_trajectories_dev": (I32, [P, I32] + [P] * 9),
+    "qmb200_initial_ee_target": (None, [P]),
+    "qmb200_control_law": (I32, [P] * 10),
+    "qmb200_control_law_dev": (I32, [P] * 11),
+    "qmb200_set_arm_gains": (I32, [P, D, D]),
+    "qmb200_hw_write": (I32, [P] * 8),
+    "qmb200_hw_write_dev": (I32, [P] * 9),
+    "qmb200_hw_set_delay": (I32, [P, D]),
+    "qmb200_sim_get_params": (I32, [P] * 2),
+    "qmb200_sim_set_params": (I32, [P] * 2),
+    "qmb200_sim_step": (I32, [P, D] + [P] * 6),
+    "qmb200_sim_step_dev": (I32, [P, D] + [P] * 7),
+    "qmb200_sim_set_robot_params": (I32, [P] * 3),
+    "qmb200_sim_get_robot_params": (I32, [P] * 4),
+    "qmb200_sim_step_ext": (I32, [P, D] + [P] * 7),
+    "qmb200_sim_step_ext_dev": (I32, [P, D] + [P] * 8),
+    "qmb200_sim_set_terrain": (I32, [P, I32, I32, I32, D, P]),
+    "qmb200_sim_get_terrain": (I32, [P] * 6),
+    "qmb200_sim_set_robot_terrain": (I32, [P] * 3),
+    "qmb200_sim_get_robot_terrain": (I32, [P] * 4),
+    "qmb200_sim_standing_state": (I32, [P, I32, P, P, P]),
+    "qmb200_update": (I32, [P] * 10),
+    "qmb200_update_dev": (I32, [P] * 11),
+    "qmb200_set_pipeline": (I32, [P, I32]),
+    "qmb200_set_profiling": (I32, [P, I32]),
+    "qmb200_collect_kernel_times": (I32, [P]),
+    "qmb200_get_kernel_times": (I32, [P] * 2),
+    "qmb200_get_flow_kernel_time": (I32, [P] * 2),
+    "qmb200_measure_fp64_peak": (I32, [P] * 2),
+    "qmb200_debug_get_step": (I32, [P] * 4),
+    "qmb200_mpc_set_solver": (I32, [P, I32]),
+    "qmb200_mpc_get_solver": (I32, [P] * 6),
+    "qmb200_comm_get_unique_id": (I32, [P]),
+    "qmb200_comm_init": (I32, [P, I32, I32, P]),
+    "qmb200_comm_destroy": (I32, [P]),
+    "qmb200_comm_info": (I32, [P] * 4),
+    "qmb200_allgather_torque": (I32, [P] * 6),
+    "qmb200_gait_bin_permutation": (I32, [I32] + [P] * 5),
+    "qmb200_debug_model_blob": (I64, [CFG, P, I64]),
+    "qmb200_debug_srbd_constants": (I32, [CFG, I32, P, P]),
+    "qmb200_launch_count": (I64, [P]),
+    "qmb200_stream": (P, [P]),
+}
+SYMBOLS = list(PROTOTYPES)
 
 _lib = None
 
@@ -78,50 +154,9 @@ def load_library():
     if not os.path.exists(LIB_PATH):
         raise QmbError("libqmb200.so not built (%s): run `python -c 'import __graft_entry__ as g; g.build()'` — there is no CPU fallback" % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    lib.qmb200_last_error.restype = C.c_char_p
-    lib.qmb200_last_error.argtypes = [C.c_void_p]
-    lib.qmb200_create.argtypes = [C.POINTER(Config), C.POINTER(C.c_void_p)]
-    lib.qmb200_destroy.argtypes = [C.c_void_p]
-    lib.qmb200_destroy.restype = None
-    lib.qmb200_debug_model_blob.restype = C.c_int64
-    lib.qmb200_debug_model_blob.argtypes = [C.POINTER(Config), C.c_void_p, C.c_int64]
-    lib.qmb200_launch_count.restype = C.c_int64
-    lib.qmb200_launch_count.argtypes = [C.c_void_p]
-    lib.qmb200_stream.restype = C.c_void_p
-    lib.qmb200_stream.argtypes = [C.c_void_p]
-    lib.qmb200_set_arm_gains.argtypes = [C.c_void_p, C.c_double, C.c_double]
-    lib.qmb200_hw_set_delay.argtypes = [C.c_void_p, C.c_double]
-    lib.qmb200_mpc_set_iterations.argtypes = [C.c_void_p, C.c_int32, C.c_double]
-    lib.qmb200_initial_ee_target.restype = None
-    lib.qmb200_sim_step.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 6
-    lib.qmb200_sim_step_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 7
-    lib.qmb200_sim_step_ext.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 7
-    lib.qmb200_sim_step_ext_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 8
-    lib.qmb200_sim_set_robot_params.argtypes = [C.c_void_p] * 3
-    lib.qmb200_sim_get_robot_params.argtypes = [C.c_void_p] * 4
-    lib.qmb200_sim_set_terrain.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p]
-    lib.qmb200_sim_get_terrain.argtypes = [C.c_void_p] * 6
-    lib.qmb200_sim_set_robot_terrain.argtypes = [C.c_void_p] * 3
-    lib.qmb200_sim_get_robot_terrain.argtypes = [C.c_void_p] * 4
-    lib.qmb200_set_model_payload.argtypes = [C.c_void_p] * 2
-    lib.qmb200_get_model_payload.argtypes = [C.c_void_p] * 3
-    lib.qmb200_debug_srbd_constants.argtypes = [C.POINTER(Config), C.c_int32, C.c_void_p, C.c_void_p]
-    lib.qmb200_payload_est_get_params.argtypes = [C.c_void_p, C.POINTER(PayloadEstParams)]
-    lib.qmb200_payload_est_set_params.argtypes = [C.c_void_p, C.POINTER(PayloadEstParams)]
-    lib.qmb200_payload_est_reset.argtypes = [C.c_void_p] * 2
-    lib.qmb200_payload_est_step.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 3
-    lib.qmb200_payload_est_step_dev.argtypes = [C.c_void_p, C.c_double] + [C.c_void_p] * 4
-    lib.qmb200_payload_est_commit_dev.argtypes = [C.c_void_p] * 2
-    lib.qmb200_payload_est_get.argtypes = [C.c_void_p] * 4
-    lib.qmb200_payload_est_stop.argtypes = [C.c_void_p]
-    lib.qmb200_get_model_payload_dev.argtypes = [C.c_void_p] * 3
-    lib.qmb200_sim_standing_state.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.qmb200_gait_destroy.restype = None
-    lib.qmb200_gait_destroy.argtypes = [C.c_void_p]
-    lib.qmb200_gait_insert_template.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_double, C.c_double]
-    lib.qmb200_gait_get_mode_schedule.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_void_p]
-    for name in SYMBOLS:
-        getattr(lib, name)
+    for name, (restype, argtypes) in PROTOTYPES.items():
+        fn = getattr(lib, name)   # AttributeError when the build lacks a declared symbol
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 

@@ -10,7 +10,7 @@ import os
 import numpy as np
 
 from . import _lib
-from ._lib import NX, NU, RBD, CMD, TARGET, EMAX, KMAX, Config, QmbError, dp, ip
+from ._lib import NX, NU, RBD, CMD, TARGET, EMAX, KMAX, Config, QmbError
 
 
 class QMInterface:
@@ -80,9 +80,11 @@ class Solver:
         except Exception:
             pass
 
-    def _chk(self, rc, what):
+    def _call(self, name, *args):
+        """qmb200_<name>(h, *args); a non-zero return code raises QmbError with the handle's last error."""
+        rc = getattr(self.lib, "qmb200_" + name)(self.h, *args)
         if rc != 0:
-            raise QmbError("%s failed (%d): %s" % (what, rc, self.lib.qmb200_last_error(self.h).decode()))
+            raise QmbError("qmb200_%s failed (%d): %s" % (name, rc, self.lib.qmb200_last_error(self.h).decode()))
 
     @property
     def launch_count(self):
@@ -103,20 +105,20 @@ class Solver:
         B = self.batch
         x_des = _f64(x_des, (B, NX)); u_des = _f64(u_des, (B, NU)); rbd = _f64(rbd, (B, RBD)); mode = _i32(mode, (B,)); period = _f64(period, (B,)); time = _f64(time, (B,))
         cmd = np.empty((B, CMD)); status = np.empty(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_wbc_update(self.h, _p(x_des), _p(u_des), _p(rbd), _p(mode), _p(period), _p(time), _p(cmd), _p(status)), "qmb200_wbc_update")
+        self._call("wbc_update", _p(x_des), _p(u_des), _p(rbd), _p(mode), _p(period), _p(time), _p(cmd), _p(status))
         return cmd, status
 
     def wbc_update_dev(self, x_des, u_des, rbd, mode, period, time, cmd, status, stream=None):
-        self._chk(self.lib.qmb200_wbc_update_dev(self.h, _p(x_des), _p(u_des), _p(rbd), _p(mode), _p(period), _p(time), _p(cmd), _p(status), C.c_void_p(stream) if stream else None), "qmb200_wbc_update_dev")
+        self._call("wbc_update_dev", _p(x_des), _p(u_des), _p(rbd), _p(mode), _p(period), _p(time), _p(cmd), _p(status), stream)
 
     def wbc_get_gains(self):
         """→ dict of the task-formulator PD gains (WbcBase::dynamicCallback fields)."""
-        g = _lib.WbcGains(); self._chk(self.lib.qmb200_wbc_get_gains(self.h, C.byref(g)), "qmb200_wbc_get_gains")
+        g = _lib.WbcGains(); self._call("wbc_get_gains", C.byref(g))
         return {n: (list(getattr(g, n)) if hasattr(getattr(g, n), "__len__") else getattr(g, n)) for n, _ in _lib.WbcGains._fields_}
 
     def wbc_set_gains(self, **gains):
         """Dynamic reconfigure of the WBC gains: keyword per field of qmb200_wbc_gains; unspecified fields keep their value."""
-        g = _lib.WbcGains(); self._chk(self.lib.qmb200_wbc_get_gains(self.h, C.byref(g)), "qmb200_wbc_get_gains")
+        g = _lib.WbcGains(); self._call("wbc_get_gains", C.byref(g))
         for k, v in gains.items():
             cur = getattr(g, k)
             if hasattr(cur, "__len__"):
@@ -124,21 +126,21 @@ class Solver:
                     cur[i] = float(x)
             else:
                 setattr(g, k, float(v))
-        self._chk(self.lib.qmb200_wbc_set_gains(self.h, C.byref(g)), "qmb200_wbc_set_gains")
+        self._call("wbc_set_gains", C.byref(g))
 
     def wbc_set_input_last(self, input_last=None):
-        self._chk(self.lib.qmb200_wbc_set_input_last(self.h, _p(_f64(input_last, (self.batch, NU))) if input_last is not None else None), "qmb200_wbc_set_input_last")
+        self._call("wbc_set_input_last", _p(_f64(input_last, (self.batch, NU))) if input_last is not None else None)
 
     def wbc_get_diagnostics(self):
         """→ dict(level0_passes, level1_iterations, level2_iterations, working_set) of the last WBC update, per robot."""
-        d = np.zeros(self.batch, dtype=np.int32); self._chk(self.lib.qmb200_wbc_get_diagnostics(self.h, _p(d)), "qmb200_wbc_get_diagnostics")
+        d = np.zeros(self.batch, dtype=np.int32); self._call("wbc_get_diagnostics", _p(d))
         return dict(level0_passes=d & 0xFF, level1_iterations=(d >> 8) & 0xFF, level2_iterations=(d >> 16) & 0xFF, working_set=(d >> 24) & 0xFF)
 
     def wbc_set_iteration_caps(self, level0_passes=0, active_set_iterations=0):
-        self._chk(self.lib.qmb200_wbc_set_iteration_caps(self.h, int(level0_passes), int(active_set_iterations)), "qmb200_wbc_set_iteration_caps")
+        self._call("wbc_set_iteration_caps", int(level0_passes), int(active_set_iterations))
 
     def wbc_get_input_last(self):
-        out = np.empty((self.batch, NU)); self._chk(self.lib.qmb200_wbc_get_input_last(self.h, _p(out)), "qmb200_wbc_get_input_last"); return out
+        out = np.empty((self.batch, NU)); self._call("wbc_get_input_last", _p(out)); return out
 
     # ---------------- MPC ----------------
     def _prob(self, prob):
@@ -150,18 +152,18 @@ class Solver:
         B, N = self.batch, self.nmax; a = self._prob(prob)
         out = dict(n_nodes=np.zeros(B, dtype=np.int32), t=np.zeros((B, N)), event=np.zeros((B, N), dtype=np.int32), x=np.zeros((B, N, NX)), u=np.zeros((B, N, NU)),
                    status=np.zeros(B, dtype=np.int32), step_info=np.zeros((B, 4)))
-        self._chk(self.lib.qmb200_mpc_solve(self.h, *[_p(v) for v in a], _p(out["n_nodes"]), _p(out["t"]), _p(out["event"]), _p(out["x"]), _p(out["u"]), _p(out["status"]), _p(out["step_info"])), "qmb200_mpc_solve")
+        self._call("mpc_solve", *[_p(v) for v in a], _p(out["n_nodes"]), _p(out["t"]), _p(out["event"]), _p(out["x"]), _p(out["u"]), _p(out["status"]), _p(out["step_info"]))
         return out
 
     def mpc_solve_dev(self, prob_dev, stream=None):
         keys = ("t0", "x0", "n_events", "event_times", "modes", "n_target", "target_times", "target_states")
-        self._chk(self.lib.qmb200_mpc_solve_dev(self.h, *[_p(prob_dev[k]) for k in keys], C.c_void_p(stream) if stream else None), "qmb200_mpc_solve_dev")
+        self._call("mpc_solve_dev", *[_p(prob_dev[k]) for k in keys], stream)
 
     SOLVERS = {"sqp": 0, "ipm": 1, "ddp": 2}
 
     def mpc_set_solver(self, solver):
         """'sqp' (SqpMpc, what QMController runs), 'ipm' (ipm{} block) or 'ddp' (ddp{} block, discrete-time form): include/qmb200.h."""
-        self._chk(self.lib.qmb200_mpc_set_solver(self.h, self.SOLVERS[solver] if isinstance(solver, str) else int(solver)), "qmb200_mpc_set_solver")
+        self._call("mpc_set_solver", self.SOLVERS[solver] if isinstance(solver, str) else int(solver))
 
     def mpc_get_solver(self):
         s, it = C.c_int32(), C.c_int32(); dt, gx, gn = C.c_double(), C.c_double(), C.c_double()
@@ -170,36 +172,36 @@ class Solver:
 
     def mpc_set_iterations(self, sqp_iterations=0, cost_tol=0.0):
         """sqp.sqpIteration / costTol (SqpSolver::runImpl loop bound and checkConvergence tolerance)."""
-        self._chk(self.lib.qmb200_mpc_set_iterations(self.h, int(sqp_iterations), float(cost_tol)), "qmb200_mpc_set_iterations")
+        self._call("mpc_set_iterations", int(sqp_iterations), float(cost_tol))
 
     def mpc_reset(self):
-        self._chk(self.lib.qmb200_mpc_reset(self.h), "qmb200_mpc_reset")
+        self._call("mpc_reset")
 
     def mpc_set_solution(self, sol):
         B, N = self.batch, self.nmax
-        self._chk(self.lib.qmb200_mpc_set_solution(self.h, _p(_i32(sol["n_nodes"], (B,))), _p(_f64(sol["t"], (B, N))), _p(_i32(sol["event"], (B, N))), _p(_f64(sol["x"], (B, N, NX))), _p(_f64(sol["u"], (B, N, NU)))), "qmb200_mpc_set_solution")
+        self._call("mpc_set_solution", _p(_i32(sol["n_nodes"], (B,))), _p(_f64(sol["t"], (B, N))), _p(_i32(sol["event"], (B, N))), _p(_f64(sol["x"], (B, N, NX))), _p(_f64(sol["u"], (B, N, NU))))
 
     def mpc_get_solution(self):
         B, N = self.batch, self.nmax
         out = dict(n_nodes=np.zeros(B, dtype=np.int32), t=np.zeros((B, N)), event=np.zeros((B, N), dtype=np.int32), x=np.zeros((B, N, NX)), u=np.zeros((B, N, NU)),
                    status=np.zeros(B, dtype=np.int32), step_info=np.zeros((B, 4)))
-        self._chk(self.lib.qmb200_mpc_get_solution(self.h, _p(out["n_nodes"]), _p(out["t"]), _p(out["event"]), _p(out["x"]), _p(out["u"]), _p(out["status"]), _p(out["step_info"])), "qmb200_mpc_get_solution")
+        self._call("mpc_get_solution", _p(out["n_nodes"]), _p(out["t"]), _p(out["event"]), _p(out["x"]), _p(out["u"]), _p(out["status"]), _p(out["step_info"]))
         return out
 
     def policy_eval(self, t):
         B = self.batch; t = _f64(t, (B,)); xd = np.empty((B, NX)); ud = np.empty((B, NU)); mode = np.empty(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_policy_eval(self.h, _p(t), _p(xd), _p(ud), _p(mode)), "qmb200_policy_eval")
+        self._call("policy_eval", _p(t), _p(xd), _p(ud), _p(mode))
         return xd, ud, mode
 
     def tick(self, prob, t_eval, rbd, period):
         B = self.batch; a = self._prob(prob); t_eval = _f64(t_eval, (B,)); rbd = _f64(rbd, (B, RBD)); period = _f64(period, (B,))
         cmd = np.empty((B, CMD)); status = np.empty(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_tick(self.h, *[_p(v) for v in a], _p(t_eval), _p(rbd), _p(period), _p(cmd), _p(status)), "qmb200_tick")
+        self._call("tick", *[_p(v) for v in a], _p(t_eval), _p(rbd), _p(period), _p(cmd), _p(status))
         return cmd, status
 
     def tick_dev(self, prob_dev, t_eval, rbd, period, cmd, status, stream=None):
         keys = ("t0", "x0", "n_events", "event_times", "modes", "n_target", "target_times", "target_states")
-        self._chk(self.lib.qmb200_tick_dev(self.h, *[_p(prob_dev[k]) for k in keys], _p(t_eval), _p(rbd), _p(period), _p(cmd), _p(status), C.c_void_p(stream) if stream else None), "qmb200_tick_dev")
+        self._call("tick_dev", *[_p(prob_dev[k]) for k in keys], _p(t_eval), _p(rbd), _p(period), _p(cmd), _p(status), stream)
 
     # ---------------- multi-GPU (include/qmb200.h: one NCCL all-gather of the torque rows per tick, driven from the C++ host) ----------------
     def comm_unique_id(self):
@@ -210,14 +212,14 @@ class Solver:
         return buf.raw
 
     def comm_init(self, nranks, rank, unique_id):
-        self._chk(self.lib.qmb200_comm_init(self.h, int(nranks), int(rank), C.c_char_p(bytes(unique_id))), "qmb200_comm_init")
+        self._call("comm_init", int(nranks), int(rank), C.c_char_p(bytes(unique_id)))
 
     def comm_info(self):
         n, r, v = C.c_int32(), C.c_int32(), C.c_int32(); self.lib.qmb200_comm_info(self.h, C.byref(n), C.byref(r), C.byref(v)); return n.value, r.value, v.value
 
     def allgather_torque(self, cmd_dev, torque_all_dev, perm_dev=None, stream=None):
         """torque_all[r * B + i] = cmd[i, 36:54] of rank r (original robot order when perm_dev is given); device tensors."""
-        self._chk(self.lib.qmb200_allgather_torque(self.h, None, _p(cmd_dev), _p(perm_dev), _p(torque_all_dev), C.c_void_p(stream) if stream else None), "qmb200_allgather_torque")
+        self._call("allgather_torque", None, _p(cmd_dev), _p(perm_dev), _p(torque_all_dev), stream)
 
     def gait_bin_permutation(self, prob):
         """Host: perm[p] = original index of the robot at position p after sorting by contact phase (qmb200_gait_bin_permutation)."""
@@ -229,90 +231,87 @@ class Solver:
 
     def set_pipeline(self, chunks):
         """Number of robot ranges the tick runs as concurrent stream chains (include/qmb200.h: qmb200_set_pipeline)."""
-        self._chk(self.lib.qmb200_set_pipeline(self.h, int(chunks)), "qmb200_set_pipeline")
+        self._call("set_pipeline", int(chunks))
 
     def set_profiling(self, on=True):
-        self._chk(self.lib.qmb200_set_profiling(self.h, 1 if on else 0), "qmb200_set_profiling")
+        self._call("set_profiling", 1 if on else 0)
 
     def collect_kernel_times(self):
         self.lib.qmb200_collect_kernel_times(self.h)
 
     def kernel_times(self):
-        ms = np.zeros(6); self._chk(self.lib.qmb200_get_kernel_times(self.h, _p(ms)), "qmb200_get_kernel_times")
+        ms = np.zeros(6); self._call("get_kernel_times", _p(ms))
         d = dict(zip(("setup", "lq", "riccati", "linesearch", "policy_eval", "wbc"), ms.tolist()))
-        v = C.c_double(); self._chk(self.lib.qmb200_get_flow_kernel_time(self.h, C.byref(v)), "qmb200_get_flow_kernel_time"); d["lq_flow"] = v.value   # part of "lq"
+        v = C.c_double(); self._call("get_flow_kernel_time", C.byref(v)); d["lq_flow"] = v.value   # part of "lq"
         return d
 
     def measure_fp64_peak(self):
-        v = C.c_double(); self._chk(self.lib.qmb200_measure_fp64_peak(self.h, C.byref(v)), "qmb200_measure_fp64_peak"); return v.value
+        v = C.c_double(); self._call("measure_fp64_peak", C.byref(v)); return v.value
 
     def debug_get_step(self):
         B, N = self.batch, self.nmax; dx = np.zeros((B, N, NX)); du = np.zeros((B, N, NU)); robot = np.zeros((B, 8))
-        self._chk(self.lib.qmb200_debug_get_step(self.h, _p(dx), _p(du), _p(robot)), "qmb200_debug_get_step"); return dx, du, robot
+        self._call("debug_get_step", _p(dx), _p(du), _p(robot)); return dx, du, robot
 
     # ---------------- controller side (SURVEY §8f): observation, targets, control law, plant law, QMController::update ----------------
     def observation_update(self, rbd, period, t_obs, x_obs):
         """QMController::updateStateEstimation tail (QMController.cpp:236-243) → (t_obs, x_obs) advanced."""
         B = self.batch; rbd = _f64(rbd, (B, RBD)); period = _f64(period, (B,)); t = _f64(t_obs, (B,)).copy(); x = _f64(x_obs, (B, NX)).copy()
-        self._chk(self.lib.qmb200_observation_update(self.h, _p(rbd), _p(period), _p(t), _p(x)), "qmb200_observation_update"); return t, x
+        self._call("observation_update", _p(rbd), _p(period), _p(t), _p(x)); return t, x
 
     def target_trajectories(self, kind, cmd, t_obs, x_obs, ee_state, last_ee_target):
         """QmTargetTrajectoriesPublisher_node.cpp:44-208 → (n_target, target_times, target_states, last_ee_target)."""
         B = self.batch; c = np.zeros((B, 7)); cmd = np.asarray(cmd, dtype=np.float64).reshape(B, -1); c[:, :cmd.shape[1]] = cmd
         t = _f64(t_obs, (B,)); x = _f64(x_obs, (B, NX)); ee = _f64(ee_state, (B, 7)); le = _f64(last_ee_target, (B, 7)).copy()
         nt = np.zeros(B, dtype=np.int32); tt = np.zeros((B, KMAX)); ts = np.zeros((B, KMAX, TARGET))
-        self._chk(self.lib.qmb200_target_trajectories(self.h, int(kind), _p(c), _p(t), _p(x), _p(ee), _p(le), _p(nt), _p(tt), _p(ts)), "qmb200_target_trajectories"); return nt, tt, ts, le
+        self._call("target_trajectories", int(kind), _p(c), _p(t), _p(x), _p(ee), _p(le), _p(nt), _p(tt), _p(ts)); return nt, tt, ts, le
 
     def initial_ee_target(self):
         v = np.zeros(7); self.lib.qmb200_initial_ee_target(_p(v)); return np.tile(v, (self.batch, 1))
 
     def set_arm_gains(self, kp, kd):
-        self._chk(self.lib.qmb200_set_arm_gains(self.h, float(kp), float(kd)), "qmb200_set_arm_gains")
+        self._call("set_arm_gains", float(kp), float(kd))
 
     def control_law(self, x_des, u_des, wbc_cmd, t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time):
         """SafetyChecker + updateControlLaw (QMController.cpp:159-190 / 427-445) → (joint_cmd, arm_pos_cmd, last_time, status)."""
         B = self.batch; jc = _f64(joint_cmd, (B, 18, 5)).copy(); ap = _f64(arm_pos_cmd, (B, 6)).copy(); lt = _f64(last_time, (B,)).copy(); st = np.zeros(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_control_law(self.h, _p(_f64(x_des, (B, NX))), _p(_f64(u_des, (B, NU))), _p(_f64(wbc_cmd, (B, CMD))), _p(_f64(t_obs, (B,))), _p(_f64(x_obs, (B, NX))), _p(jc), _p(ap), _p(lt), _p(st)),
-                  "qmb200_control_law"); return jc, ap, lt, st
+        self._call("control_law", _p(_f64(x_des, (B, NX))), _p(_f64(u_des, (B, NU))), _p(_f64(wbc_cmd, (B, CMD))), _p(_f64(t_obs, (B,))), _p(_f64(x_obs, (B, NX))),
+                   _p(jc), _p(ap), _p(lt), _p(st)); return jc, ap, lt, st
 
     def hw_set_delay(self, delay):
-        self._chk(self.lib.qmb200_hw_set_delay(self.h, float(delay)), "qmb200_hw_set_delay")
+        self._call("hw_set_delay", float(delay))
 
     def hw_write(self, time, period, joint_cmd, joint_pos, joint_vel):
         """QMHWSim::writeSim (QMHWSim.cpp:98-116) → (effort[B,18], status)."""
         B = self.batch; eff = np.zeros((B, 18)); st = np.zeros(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_hw_write(self.h, _p(_f64(time, (B,))), _p(_f64(period, (B,))), _p(_f64(joint_cmd, (B, 18, 5))), _p(_f64(joint_pos, (B, 18))), _p(_f64(joint_vel, (B, 18))), _p(eff), _p(st)), "qmb200_hw_write")
+        self._call("hw_write", _p(_f64(time, (B,))), _p(_f64(period, (B,))), _p(_f64(joint_cmd, (B, 18, 5))), _p(_f64(joint_pos, (B, 18))), _p(_f64(joint_vel, (B, 18))), _p(eff), _p(st))
         return eff, st
 
     def update(self, rbd, period, t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time):
         """QMController::update (QMController.cpp:128-175) on the stored policy → (t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time, cmd[B,54], status)."""
         B = self.batch; t = _f64(t_obs, (B,)).copy(); x = _f64(x_obs, (B, NX)).copy(); jc = _f64(joint_cmd, (B, 18, 5)).copy(); ap = _f64(arm_pos_cmd, (B, 6)).copy(); lt = _f64(last_time, (B,)).copy()
         cmd = np.zeros((B, CMD)); st = np.zeros(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_update(self.h, _p(_f64(rbd, (B, RBD))), _p(_f64(period, (B,))), _p(t), _p(x), _p(jc), _p(ap), _p(lt), _p(cmd), _p(st)), "qmb200_update")
+        self._call("update", _p(_f64(rbd, (B, RBD))), _p(_f64(period, (B,))), _p(t), _p(x), _p(jc), _p(ap), _p(lt), _p(cmd), _p(st))
         return t, x, jc, ap, lt, cmd, st
 
     # device-pointer variants of the controller side (torch-cuda tensors, no synchronisation)
     def target_trajectories_dev(self, kind, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, stream=None):
-        self._chk(self.lib.qmb200_target_trajectories_dev(self.h, int(kind), _p(cmd), _p(t_obs), _p(x_obs), _p(ee_state), _p(last_ee_target), _p(n_target), _p(target_times), _p(target_states),
-                                                          C.c_void_p(stream) if stream else None), "qmb200_target_trajectories_dev")
+        self._call("target_trajectories_dev", int(kind), _p(cmd), _p(t_obs), _p(x_obs), _p(ee_state), _p(last_ee_target), _p(n_target), _p(target_times), _p(target_states), stream)
 
     def update_dev(self, rbd, period, t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time, cmd, status, stream=None):
-        self._chk(self.lib.qmb200_update_dev(self.h, _p(rbd), _p(period), _p(t_obs), _p(x_obs), _p(joint_cmd), _p(arm_pos_cmd), _p(last_time), _p(cmd), _p(status), C.c_void_p(stream) if stream else None),
-                  "qmb200_update_dev")
+        self._call("update_dev", _p(rbd), _p(period), _p(t_obs), _p(x_obs), _p(joint_cmd), _p(arm_pos_cmd), _p(last_time), _p(cmd), _p(status), stream)
 
     def hw_write_dev(self, time, period, joint_cmd, joint_pos, joint_vel, effort, status, stream=None):
-        self._chk(self.lib.qmb200_hw_write_dev(self.h, _p(time), _p(period), _p(joint_cmd), _p(joint_pos), _p(joint_vel), _p(effort), _p(status), C.c_void_p(stream) if stream else None),
-                  "qmb200_hw_write_dev")
+        self._call("hw_write_dev", _p(time), _p(period), _p(joint_cmd), _p(joint_pos), _p(joint_vel), _p(effort), _p(status), stream)
 
     # ---------------- plant (include/qmb200.h: Gazebo's physics step behind QMHWSim + readSim's contact flags) ----------------
     def sim_get_params(self):
         """→ dict of qmb200_sim_params (joint_damping as a list of 18)."""
-        p = _lib.SimParams(); self._chk(self.lib.qmb200_sim_get_params(self.h, C.byref(p)), "qmb200_sim_get_params")
+        p = _lib.SimParams(); self._call("sim_get_params", C.byref(p))
         return {n: (list(getattr(p, n)) if n == "joint_damping" else getattr(p, n)) for n, _ in _lib.SimParams._fields_}
 
     def sim_set_params(self, **params):
         """Keyword per field of qmb200_sim_params; unspecified fields keep their value."""
-        p = _lib.SimParams(); self._chk(self.lib.qmb200_sim_get_params(self.h, C.byref(p)), "qmb200_sim_get_params")
+        p = _lib.SimParams(); self._call("sim_get_params", C.byref(p))
         for k, v in params.items():
             if k == "joint_damping":
                 for i, x in enumerate(v):
@@ -321,26 +320,24 @@ class Solver:
                 p.substeps_per_ms = int(v)
             else:
                 setattr(p, k, float(v))
-        self._chk(self.lib.qmb200_sim_set_params(self.h, C.byref(p)), "qmb200_sim_set_params")
+        self._call("sim_set_params", C.byref(p))
 
     def sim_step(self, duration, effort, q, v, wrench=None):
         """One physics step of every robot (effort held for `duration` s) → (q, v, rbd[B,55], contact[B], status[B]).
         wrench: optional [B, 12] external wrenches held over the step (layout _lib.WRENCH_LAYOUT, include/qmb200.h: qmb200_sim_step_ext)."""
         B = self.batch; q = _f64(q, (B, 24)).copy(); v = _f64(v, (B, 24)).copy(); rbd = np.zeros((B, RBD)); contact = np.zeros(B, dtype=np.int32); st = np.zeros(B, dtype=np.int32)
         if wrench is None:
-            self._chk(self.lib.qmb200_sim_step(self.h, float(duration), _p(_f64(effort, (B, 18))), _p(q), _p(v), _p(rbd), _p(contact), _p(st)), "qmb200_sim_step")
+            self._call("sim_step", float(duration), _p(_f64(effort, (B, 18))), _p(q), _p(v), _p(rbd), _p(contact), _p(st))
         else:
-            self._chk(self.lib.qmb200_sim_step_ext(self.h, float(duration), _p(_f64(effort, (B, 18))), _p(_f64(wrench, (B, 12))), _p(q), _p(v), _p(rbd), _p(contact), _p(st)),
-                      "qmb200_sim_step_ext")
+            self._call("sim_step_ext", float(duration), _p(_f64(effort, (B, 18))), _p(_f64(wrench, (B, 12))), _p(q), _p(v), _p(rbd), _p(contact), _p(st))
         return q, v, rbd, contact, st
 
     def sim_step_dev(self, duration, effort, q, v, rbd, contact, status, stream=None, wrench=None):
         """Device-pointer variant: q, v updated in place; no synchronisation.  wrench: optional [B, 12] device tensor."""
         if wrench is None:
-            self._chk(self.lib.qmb200_sim_step_dev(self.h, float(duration), _p(effort), _p(q), _p(v), _p(rbd), _p(contact), _p(status), C.c_void_p(stream) if stream else None), "qmb200_sim_step_dev")
+            self._call("sim_step_dev", float(duration), _p(effort), _p(q), _p(v), _p(rbd), _p(contact), _p(status), stream)
         else:
-            self._chk(self.lib.qmb200_sim_step_ext_dev(self.h, float(duration), _p(effort), _p(wrench), _p(q), _p(v), _p(rbd), _p(contact), _p(status), C.c_void_p(stream) if stream else None),
-                      "qmb200_sim_step_ext_dev")
+            self._call("sim_step_ext_dev", float(duration), _p(effort), _p(wrench), _p(q), _p(v), _p(rbd), _p(contact), _p(status), stream)
 
     def sim_set_robot_params(self, friction_mu=None, payload=None):
         """Per-robot plant variation kept in the handle: friction_mu [B] (a scalar is broadcast), payload [B, 8] (layout _lib.PAYLOAD_LAYOUT).
@@ -348,12 +345,12 @@ class Solver:
         B = self.batch
         mu = None if friction_mu is None else _f64(np.broadcast_to(np.asarray(friction_mu, dtype=np.float64), (B,)), (B,))
         pl = None if payload is None else _f64(payload, (B, 8))
-        self._chk(self.lib.qmb200_sim_set_robot_params(self.h, _p(mu), _p(pl)), "qmb200_sim_set_robot_params")
+        self._call("sim_set_robot_params", _p(mu), _p(pl))
 
     def sim_get_robot_params(self):
         """→ dict(friction_mu [B] or None, payload [B, 8] or None): None where that override is not set."""
         B = self.batch; mu = np.zeros(B); pl = np.zeros((B, 8)); mask = C.c_int32()
-        self._chk(self.lib.qmb200_sim_get_robot_params(self.h, _p(mu), _p(pl), C.byref(mask)), "qmb200_sim_get_robot_params")
+        self._call("sim_get_robot_params", _p(mu), _p(pl), C.byref(mask))
         return dict(friction_mu=mu if mask.value & 1 else None, payload=pl if mask.value & 2 else None)
 
     def set_model_payload(self, payload=None):
@@ -361,82 +358,82 @@ class Solver:
         fixed link with the point mass at o_ee in the end-effector frame and one at o_base in the base frame.  Independent of the plant's
         sim_set_robot_params.  None clears it.  Synchronous."""
         pl = None if payload is None else _f64(payload, (self.batch, 8))
-        self._chk(self.lib.qmb200_set_model_payload(self.h, _p(pl)), "qmb200_set_model_payload")
+        self._call("set_model_payload", _p(pl))
 
     def get_model_payload(self):
         """→ the model payload [B, 8], or None when none is set."""
         pl = np.zeros((self.batch, 8)); is_set = C.c_int32()
-        self._chk(self.lib.qmb200_get_model_payload(self.h, _p(pl), C.byref(is_set)), "qmb200_get_model_payload")
+        self._call("get_model_payload", _p(pl), C.byref(is_set))
         return pl if is_set.value else None
 
     # ---------------- online payload estimate (include/qmb200.h: qmb200_payload_est_*; DESIGN.md §4.6) ----------------
     def payload_est_get_params(self):
         """→ dict of qmb200_payload_est_params."""
-        p = _lib.PayloadEstParams(); self._chk(self.lib.qmb200_payload_est_get_params(self.h, C.byref(p)), "qmb200_payload_est_get_params")
+        p = _lib.PayloadEstParams(); self._call("payload_est_get_params", C.byref(p))
         return {n: getattr(p, n) for n, _ in _lib.PayloadEstParams._fields_}
 
     def payload_est_set_params(self, **params):
         """Keyword per field of qmb200_payload_est_params; unspecified fields keep their value."""
-        p = _lib.PayloadEstParams(); self._chk(self.lib.qmb200_payload_est_get_params(self.h, C.byref(p)), "qmb200_payload_est_get_params")
+        p = _lib.PayloadEstParams(); self._call("payload_est_get_params", C.byref(p))
         names = [n for n, _ in _lib.PayloadEstParams._fields_]
         for k, v in params.items():
             if k not in names:
                 raise ValueError("payload_est_set_params: unknown parameter %r (one of %s)" % (k, ", ".join(names)))
             setattr(p, k, float(v))
-        self._chk(self.lib.qmb200_payload_est_set_params(self.h, C.byref(p)), "qmb200_payload_est_set_params")
+        self._call("payload_est_set_params", C.byref(p))
 
     def payload_est_reset(self, prior=None):
         """(Re)start the estimator of every robot from prior [B, 8] (layout _lib.PAYLOAD_LAYOUT; None: the current model payload, zeros when none is set).
         Sets the model payload to prior.  Synchronous."""
         pl = None if prior is None else _f64(prior, (self.batch, 8))
-        self._chk(self.lib.qmb200_payload_est_reset(self.h, _p(pl)), "qmb200_payload_est_reset")
+        self._call("payload_est_reset", _p(pl))
 
     def payload_est_step(self, dt, effort, rbd):
         """One RLS update per robot from the measurement rbd [B, 55] and the effort [B, 18] held over the dt s that ended at it → status [B]."""
         B = self.batch; st = np.zeros(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_payload_est_step(self.h, float(dt), _p(_f64(effort, (B, 18))), _p(_f64(rbd, (B, RBD))), _p(st)), "qmb200_payload_est_step")
+        self._call("payload_est_step", float(dt), _p(_f64(effort, (B, 18))), _p(_f64(rbd, (B, RBD))), _p(st))
         return st
 
     def payload_est_step_dev(self, dt, effort, rbd, status, stream=None):
         """Device-pointer variant: status [B] int32 written; no synchronisation."""
-        self._chk(self.lib.qmb200_payload_est_step_dev(self.h, float(dt), _p(effort), _p(rbd), _p(status), C.c_void_p(stream) if stream else None), "qmb200_payload_est_step_dev")
+        self._call("payload_est_step_dev", float(dt), _p(effort), _p(rbd), _p(status), stream)
 
     def payload_est_commit_dev(self, stream=None):
         """The estimate → the end-effector half of every robot's model payload and its SRBD constants, in stream order; no synchronisation."""
-        self._chk(self.lib.qmb200_payload_est_commit_dev(self.h, C.c_void_p(stream) if stream else None), "qmb200_payload_est_commit_dev")
+        self._call("payload_est_commit_dev", stream)
 
     def payload_est_get(self):
         """→ dict(theta [B, 10] (layout _lib.THETA_LAYOUT), p_diag [B, 10], samples [B]).  Synchronous."""
         B = self.batch; th = np.zeros((B, 10)); pd = np.zeros((B, 10)); n = np.zeros(B, dtype=np.int32)
-        self._chk(self.lib.qmb200_payload_est_get(self.h, _p(th), _p(pd), _p(n)), "qmb200_payload_est_get")
+        self._call("payload_est_get", _p(th), _p(pd), _p(n))
         return dict(theta=th, p_diag=pd, samples=n)
 
     def payload_est_stop(self):
         """Release the estimator state; the model payload keeps its last committed rows."""
-        self._chk(self.lib.qmb200_payload_est_stop(self.h), "qmb200_payload_est_stop")
+        self._call("payload_est_stop")
 
     def get_model_payload_dev(self, out, stream=None):
         """Copy the model payload rows the kernels read into the device tensor out [B, 8] in stream order (no synchronisation)."""
-        self._chk(self.lib.qmb200_get_model_payload_dev(self.h, _p(out), C.c_void_p(stream) if stream else None), "qmb200_get_model_payload_dev")
+        self._call("get_model_payload_dev", _p(out), stream)
 
     def sim_set_terrain(self, tiles=None, cell=None):
         """Heightfield tile library of the plant: tiles [T, ny, nx] absolute world z (m) on nodes `cell` m apart (qm_control_b200.terrain builds them).
         None clears the library and every robot's terrain.  Synchronous."""
         if tiles is None:
-            self._chk(self.lib.qmb200_sim_set_terrain(self.h, 0, 0, 0, 0.0, None), "qmb200_sim_set_terrain"); return
+            self._call("sim_set_terrain", 0, 0, 0, 0.0, None); return
         t = _f64(tiles)
         if t.ndim != 3:
             raise ValueError("expected tiles of shape [T, ny, nx], got %s" % (t.shape,))
-        self._chk(self.lib.qmb200_sim_set_terrain(self.h, t.shape[0], t.shape[2], t.shape[1], float(cell), _p(t)), "qmb200_sim_set_terrain")
+        self._call("sim_set_terrain", t.shape[0], t.shape[2], t.shape[1], float(cell), _p(t))
 
     def sim_get_terrain(self):
         """→ dict(tiles [T, ny, nx], cell), or None when no library is set."""
         n, nx, ny, cell = C.c_int32(), C.c_int32(), C.c_int32(), C.c_double()
-        self._chk(self.lib.qmb200_sim_get_terrain(self.h, C.byref(n), C.byref(nx), C.byref(ny), C.byref(cell), None), "qmb200_sim_get_terrain")
+        self._call("sim_get_terrain", C.byref(n), C.byref(nx), C.byref(ny), C.byref(cell), None)
         if n.value == 0:
             return None
         t = np.zeros((n.value, ny.value, nx.value))
-        self._chk(self.lib.qmb200_sim_get_terrain(self.h, None, None, None, None, _p(t)), "qmb200_sim_get_terrain")
+        self._call("sim_get_terrain", None, None, None, None, _p(t))
         return dict(tiles=t, cell=cell.value)
 
     def sim_set_robot_terrain(self, tile=None, origin=None):
@@ -444,34 +441,34 @@ class Solver:
         None clears it.  Synchronous."""
         B = self.batch
         if tile is None:
-            self._chk(self.lib.qmb200_sim_set_robot_terrain(self.h, None, None), "qmb200_sim_set_robot_terrain"); return
+            self._call("sim_set_robot_terrain", None, None); return
         t = _i32(np.broadcast_to(np.asarray(tile), (B,)), (B,))
         o = _f64(np.zeros((B, 2)) if origin is None else np.broadcast_to(np.asarray(origin, dtype=np.float64), (B, 2)), (B, 2))
-        self._chk(self.lib.qmb200_sim_set_robot_terrain(self.h, _p(t), _p(o)), "qmb200_sim_set_robot_terrain")
+        self._call("sim_set_robot_terrain", _p(t), _p(o))
 
     def sim_get_robot_terrain(self):
         """→ dict(tile [B], origin [B, 2]), or None when no robot terrain is set."""
         t = np.zeros(self.batch, dtype=np.int32); o = np.zeros((self.batch, 2)); is_set = C.c_int32()
-        self._chk(self.lib.qmb200_sim_get_robot_terrain(self.h, _p(t), _p(o), C.byref(is_set)), "qmb200_sim_get_robot_terrain")
+        self._call("sim_get_robot_terrain", _p(t), _p(o), C.byref(is_set))
         return dict(tile=t, origin=o) if is_set.value else None
 
     def sim_standing_state(self, xy_yaw):
         """Nominal standing configuration at the given base (x, y, yaw) rows → (q[n,24], v[n,24]).  With robot terrain set there is one row per robot,
         each standing on its own ground."""
         xy = _f64(xy_yaw).reshape(-1, 3); n = xy.shape[0]; q = np.zeros((n, 24)); v = np.zeros((n, 24))
-        self._chk(self.lib.qmb200_sim_standing_state(self.h, n, _p(xy), _p(q), _p(v)), "qmb200_sim_standing_state")
+        self._call("sim_standing_state", n, _p(xy), _p(q), _p(v))
         return q, v
 
     # ---------------- utilities ----------------
     def centroidal_state_from_rbd(self, rbd):
         rbd = _f64(rbd); n = rbd.shape[0]; x = np.empty((n, NX))
-        self._chk(self.lib.qmb200_centroidal_state_from_rbd(self.h, n, _p(rbd), _p(x)), "qmb200_centroidal_state_from_rbd"); return x
+        self._call("centroidal_state_from_rbd", n, _p(rbd), _p(x)); return x
 
 
 def gait_schedule(gait_name, t_start, lo, hi, gait_file=None):
     """GaitSchedule tiling of a gait.info template → (event_times[EMAX], mode_sequence[EMAX+1], n_events)."""
     lib = _lib.load_library(); ev = np.zeros(EMAX); md = np.full(EMAX + 1, 15, dtype=np.int32)
-    n = lib.qmb200_gait_schedule((gait_file or _lib.asset("qm_gait.info")).encode(), gait_name.encode(), C.c_double(t_start), C.c_double(lo), C.c_double(hi), _p(ev), _p(md))
+    n = lib.qmb200_gait_schedule((gait_file or _lib.asset("qm_gait.info")).encode(), gait_name.encode(), float(t_start), float(lo), float(hi), _p(ev), _p(md))
     if n < 0:
         raise QmbError("qmb200_gait_schedule failed: " + lib.qmb200_last_error(None).decode())
     return ev, md, n

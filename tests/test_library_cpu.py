@@ -15,14 +15,48 @@ from qm_control_b200.interface import gait_schedule
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_library_exports_every_declared_symbol():
+def _c_kind(decl):
+    """Kind of a C type, with or without a parameter name: ptr / str (const char*) / int32 / int64 / double / void."""
+    if "*" in decl:
+        return "str" if re.fullmatch(r"const\s+char\s*\*\s*\w*", decl) else "ptr"
+    return {"int": "int32", "int32_t": "int32", "int64_t": "int64", "double": "double", "void": "void"}[decl.replace("const ", "").split()[0]]
+
+
+def _ctypes_kind(t):
+    if t is None:
+        return "void"
+    if t is C.c_char_p:
+        return "str"
+    if t is C.c_void_p or issubclass(t, C._Pointer):
+        return "ptr"
+    return {C.c_int32: "int32", C.c_int64: "int64", C.c_double: "double"}[t]
+
+
+def _header_prototypes():
+    """name → (return kind, [argument kinds]) of every function include/qmb200.h declares, in header order."""
     hdr = open(os.path.join(ROOT, "include", "qmb200.h")).read()
-    declared = sorted(set(re.findall(r"\b(qmb200_[a-z_0-9]+)\s*\(", hdr)))
+    code = re.sub(r"^\s*#.*$", "", re.sub(r"/\*.*?\*/|//[^\n]*", "", hdr, flags=re.S), flags=re.M)
+    protos = {}
+    for ret, name, params in re.findall(r"([\w\s*]+?)\b(qmb200_\w+)\s*\(([^()]*)\)\s*;", code):
+        params = [p.strip() for p in params.split(",")] if params.strip() not in ("", "void") else []
+        assert name not in protos, name
+        protos[name] = (_c_kind(ret.strip()), [_c_kind(p) for p in params])
+    assert set(protos) == set(re.findall(r"\b(qmb200_[a-z_0-9]+)\s*\(", hdr)), "a declaration the prototype parser missed"
+    return protos
+
+
+def test_library_exports_every_declared_symbol():
+    """The binding's prototype table has every function of include/qmb200.h, in header order, with the same return and argument kinds."""
+    declared = _header_prototypes()
     assert len(declared) >= 24
+    assert list(_lib.PROTOTYPES) == list(declared) and _lib.SYMBOLS == list(declared)
+    for name, (ret, args) in declared.items():
+        restype, argtypes = _lib.PROTOTYPES[name]
+        assert (_ctypes_kind(restype), [_ctypes_kind(t) for t in argtypes]) == (ret, args), name
     lib = q.load_library()
-    for name in declared:
-        assert hasattr(lib, name), name
-    assert sorted(set(_lib.SYMBOLS)) == declared   # the python binding tracks the header
+    for name, (restype, argtypes) in _lib.PROTOTYPES.items():
+        fn = getattr(lib, name)
+        assert fn.restype is restype and list(fn.argtypes) == list(argtypes), name
 
 
 def test_create_fails_loudly_without_gpu_or_files():
