@@ -107,17 +107,18 @@ __global__ void __launch_bounds__(32 * SETUP_WARPS) mpc_setup_kernel(const DevMo
 // (3x12 blocks) and written straight into the dense stage record the Riccati kernel consumes.
 struct LqLate { double BrdF[9 * 12], BrdJ[3 * NJ], bvec[NX]; };                // produced by the RK2 combination, after the cost / projection blocks have consumed rec.foot and rec.ee
 struct alignas(16) LqSmem {   // 16-byte vector loads of the record: every warp's slice starts 16-byte aligned
-  ne::NodeRec rec;                                                             // the node's record from the flow kernel (K2a); LqLate overlays rec.foot[] once the cost / projection / Jacobian expansion have consumed it
+  ne::NodeRec rec;                                                             // the node's record from the flow kernel (K2a); LqLate overlays rec.foot[] once the cost / projection / flow columns have consumed it
   QuadWs quad; LegWs leg[4];
   double x[NX], u[NU];                                                         // (x, u) of the node in the layout stage_cost_quad reads (x then u)
-  double A1r[9 * NX], Ar[9 * NX];                                              // rows 3:12 of df/dx at the two RK2 stages; A1r becomes A_d - I in place.  Until expand_flow fills it, Ar holds the robot's mode schedule
+  double Rw[NU][3];                                                            // the node's input weight (quad_R, read from the model once): row i < 24 on the columns of its triple, arm row i: [i][0] = diagonal
   double Pe_full[NU], rs[NU];
+  double ev[EMAX];                                                             // the robot's mode schedule: the binary searches and the swing-interval scans hit shared memory
   int dep_idx[MAXDEP], free_idx[MU], col_of_input[NU];
+  unsigned char modes[EMAX + 1];
 };
-static_assert(9 * NX * 8 >= EMAX * 8 + EMAX + 8, "the mode schedule (event times + modes) is staged in the Ar buffer until the flow Jacobians are expanded");
 static_assert(sizeof(LqLate) <= 4 * sizeof(ne::FootBlk) && offsetof(ne::NodeRec, foot) == 0, "LqLate overlays the foot blocks of the record");
 static_assert(sizeof(LqSmem) % 16 == 0 && offsetof(LqSmem, rec) == 0, "aligned record slice");
-static_assert((sizeof(LqSmem) * LQ_WARPS + 1024) * QMB_LQ_MINB <= 232448, "projection kernel: QMB_LQ_MINB CTAs of LQ_WARPS warps per SM (13.8 KB per node: four CTAs of four warps = 16 nodes in flight)");
+static_assert((sizeof(LqSmem) * LQ_WARPS + 1024) * QMB_LQ_MINB <= 232448, "projection kernel: QMB_LQ_MINB CTAs of LQ_WARPS warps per SM (10.0 KB per node: four CTAs of four warps = 16 nodes in flight; 20 warps would fit the shared memory, not the 96-register budget)");
 
 // =====================================================================================================
 // K2a: flow kernel - one THREAD per node (node_eval.cuh).  Kinematics of the five chains, both RK2 stages of the flow map with their Jacobian blocks, the
@@ -194,19 +195,25 @@ __global__ void __launch_bounds__(32 * FL_WARPS, QMB_FL_MINB) mpc_flow_kernel(co
 // K2b: cost quadratic model, equality constraints, projection, RK2 sensitivities and the structured stage record of one node (one warp per node), on the
 // record of the flow kernel.
 // (A CTA-wide re-alignment of the warps at phase boundaries - instruction-cache sharing - was tried and dropped: it made the kernel slower.)
-// rows 3:12 of df/dx (9 x 30, two thirds zeros) from the Jacobian blocks of a flow record: fill, then lane = column writes
-// its own non-zeros (the fill and the column writes are separated by a warp barrier)
-__device__ __forceinline__ void expand_flow(const ne::FlowBlk& fb, const double* jxf0, int fstride /*doubles between two feet*/, double* Ar, int lfp, int lane) {
-  for (int e = lane; e < 9 * NX; e += 32) Ar[e] = 0.0;
-  __syncwarp();
-  if (lane < 24) {
-    const int col = lane;
-    if (col < 3) Ar[(3 + col) * NX + col] = 1.0;                                                         // d pdot / d h_lin = I
-    else if (col < 6) { for (int a = 0; a < 3; ++a) { Ar[(3 + a) * NX + col] = fb.Mpc[3 * a + col - 3]; Ar[(6 + a) * NX + col] = fb.Mtw[3 * a + col - 3]; } }   // d / d h_ang
-    else if (col >= 9 && col < 12) { for (int a = 0; a < 3; ++a) { Ar[a * NX + col] = fb.hth[col - 9][a]; Ar[(3 + a) * NX + col] = fb.vp[col - 9][a]; Ar[(6 + a) * NX + col] = fb.vt[col - 9][a]; } }   // d / d theta
-    else if (col >= 12) { const int j12 = col - 12; const double* jf = jxf0 + foot_of_leg_joint(lfp, j12) * fstride + 3 * (j12 % 3); for (int a = 0; a < 3; ++a) Ar[a * NX + col] = jf[a]; }   // d hdot_ang / d q_leg = (J_j x F) / m
-  }
-  __syncwarp();
+// column `col` of rows 3:12 of df/dx (9 x 30, two thirds zeros) from the Jacobian blocks of a flow record, into registers
+__device__ __forceinline__ void flow_column(const ne::FlowBlk& fb, const double* jxf0, int fstride /*doubles between two feet*/, int lfp, int col, double (&a)[9]) {
+#pragma unroll
+  for (int q = 0; q < 9; ++q) a[q] = (q >= 3 && q < 6 && col == q - 3) ? 1.0 : 0.0;                      // d pdot / d h_lin = I
+  if (col >= 3 && col < 6) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r) { a[3 + r] = fb.Mpc[3 * r + col - 3]; a[6 + r] = fb.Mtw[3 * r + col - 3]; } }   // d / d h_ang
+  else if (col >= 9 && col < 12) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r) { a[r] = fb.hth[col - 9][r]; a[3 + r] = fb.vp[col - 9][r]; a[6 + r] = fb.vt[col - 9][r]; } }   // d / d theta
+  else if (col >= 12 && col < 24) { const int j12 = col - 12; const double* jf = jxf0 + foot_of_leg_joint(lfp, j12) * fstride + 3 * (j12 % 3);
+#pragma unroll
+    for (int r = 0; r < 3; ++r) a[r] = jf[r]; }   // d hdot_ang / d q_leg = (J_j x F) / m
+}
+// entry (r, 3 + q) of rows 3:12 of df/dx, q < 9 (the columns h_ang, p, theta that multiply the first stage's rows 3:12 in A2 A1); zero where the structure is
+__device__ __forceinline__ double flow_inner(const ne::FlowBlk& fb, int r, int q) {
+  if (q < 3) return r < 3 ? 0.0 : (r < 6 ? fb.Mpc[3 * (r - 3) + q] : fb.Mtw[3 * (r - 6) + q]);
+  if (q < 6) return 0.0;
+  return r < 3 ? fb.hth[q - 6][r] : (r < 6 ? fb.vp[q - 6][r - 3] : fb.vt[q - 6][r - 6]);
 }
 __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(const DevModel* __restrict__ mdl, int b0, int B, int nmax, MpcProblemDev p, MpcSolutionDev sol, const double* __restrict__ rec, double* __restrict__ stage, int32_t* __restrict__ status) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -225,7 +232,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   const double xv = (lane < NX) ? xk[lane] : 0.0, uv = (lane < NU) ? uk[lane] : 0.0, xnv = (lane < NX && has_next) ? xk[NX + lane] : 0.0;
   const double* gt = sol.t + (size_t)b * nmax; const int32_t* ge = sol.event + (size_t)b * nmax;
   const double tk = gt[k], tk1 = has_next ? gt[k + 1] : 0.0; const int ek = ge[k], ek1 = has_next ? ge[k + 1] : 0;
-  const int ne = clamp_events(p.n_events[b]); double* s_ev = sm.Ar; unsigned char* s_modes = reinterpret_cast<unsigned char*>(sm.Ar + EMAX); const double* ev = s_ev; const unsigned char* modes = s_modes;   // staged once per node: the binary searches and the swing-interval scans hit shared memory
+  const int ne = clamp_events(p.n_events[b]); double* s_ev = sm.ev; unsigned char* s_modes = sm.modes; const double* ev = s_ev; const unsigned char* modes = s_modes;
   { const double* gev = p.event_times + (size_t)b * EMAX; const int32_t* gmodes = p.modes + (size_t)b * (EMAX + 1); s_ev[lane] = (lane < ne) ? gev[lane] : 0.0; s_modes[lane] = (unsigned char)((lane <= ne) ? gmodes[lane] : 15); if (lane == 0) s_modes[EMAX] = (unsigned char)((EMAX <= ne) ? gmodes[EMAX] : 15); }
   const int n = sol.n_nodes[b];
   const bool work = k < n && !(status[b] & MST_CONVERGED);   // MST_CONVERGED: SqpSolver::runImpl left the iteration loop for this robot
@@ -252,7 +259,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   const double dt = terminal ? 0.0 : interval_end(tk1, ek1) - t;
   const int mode = mode_at_time(ev, modes, ne, t); const int fm = terminal ? 0 : flag_mask(mode);
   if (!terminal && !(dt > 0.0) && lane == 0) atomicOr(&status[b], MST_NEG_DT);   // getIntervalDuration <= 0: an event within weakEpsilon of a grid node (QMB200_ST_NEG_DT)
-  double cost_val = 0.0, eq_ss = 0.0; int ndep = 0, m = 0; double b1v[3] = {0.0, 0.0, 0.0}, b2v[3] = {0.0, 0.0, 0.0};
+  double cost_val = 0.0, eq_ss = 0.0; int ndep = 0, m = 0; double b1v[3] = {0.0, 0.0, 0.0}, b2v[3] = {0.0, 0.0, 0.0}, a1[9], a2[9];
   {
   // ---- cost quadratic model at (x, u) (the end-effector error and its Jacobian come with the record) ----
   struct XU { double x[NX], u[NU]; }; static_assert(offsetof(LqSmem, u) == offsetof(LqSmem, x) + NX * 8, "x then u");
@@ -267,7 +274,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   int nd_before = 0; for (int i = 0; i < 4; ++i) if (i < lane) nd_before += ((fm >> i) & 1) ? 3 : 4;
   ndep = 0; for (int i = 0; i < 4; ++i) ndep += ((fm >> i) & 1) ? 3 : 4;
   m = NU - ndep;
-  if (lane < NU) sm.Pe_full[lane] = 0.0;
+  for (int e = lane; e < NU * 3; e += 32) { const int i = e / 3, c = e - 3 * i; sm.Rw[i][c] = (i < 24) ? quad_R(mdl, &sm.quad, i, 3 * (i / 3) + c) : (c == 0 ? quad_R(mdl, &sm.quad, i, i) : 0.0); }
   bool swing_ok = true; int pivot = -1;
   if (lane < 4) {   // lane = foot (contact order); its leg's first joint = foot_leg
     const int i = lane; const int first = mdl->foot_leg[i]; LegWs& L = sm.leg[i]; L.first = first; L.stance = (fm >> i) & 1;
@@ -289,43 +296,51 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   bool is_dep = false; if (lane < NU) for (int d = 0; d < ndep; ++d) is_dep |= (sm.dep_idx[d] == lane);
   const unsigned free_mask = __ballot_sync(FULL, lane < NU && !is_dep);
   if (lane < NU) { const int rank = __popc(free_mask & ((1u << lane) - 1u)); sm.col_of_input[lane] = is_dep ? -1 : rank; if (!is_dep) sm.free_idx[rank] = lane; }
-  __syncwarp();
   // ---- per-leg projection blocks (structured elimination; the projected optimum does not depend on the null-space basis) ----
+  // lane = foot: the 3x3 elimination matrix G of the leg; every entry of P_x, P_e and r + R P_e is then one lane's short dot product
   if (lane < 4) {
-    const int i = lane; LegWs& L = sm.leg[i]; const int first = L.first;
-    for (int a = 0; a < 3; ++a) for (int c = 0; c < 3; ++c) L.Rl[3 * a + c] = quad_R(mdl, &sm.quad, 12 + first + a, 12 + first + c);
-    for (int j = 0; j < 3; ++j) { L.free_col[j] = sm.col_of_input[12 + first + j]; L.Pe[j] = 0.0; for (int c = 0; c < 12; ++c) L.Px[j][c] = 0.0; }
+    const int i = lane; LegWs& L = sm.leg[i]; const ne::FootBlk& fb = sm.rec.foot[i];
     L.Pu2[0] = L.Pu2[1] = 0.0;
     if (L.stance) {   // zero velocity: Jl dqd = -(C dx + e)  →  dqd = -Jl^{-1} (C dx + e)
-      double Jm[9], Ji[9]; for (int a = 0; a < 3; ++a) for (int j = 0; j < 3; ++j) Jm[3 * a + j] = sm.rec.foot[i].Jl[3 * j + a]; inv3(Jm, Ji);
-      for (int j = 0; j < 3; ++j) { double pe = 0.0; for (int a = 0; a < 3; ++a) pe -= Ji[3 * j + a] * sm.rec.foot[i].e[a]; L.Pe[j] = pe; sm.Pe_full[12 + first + j] = pe;
-        for (int c = 0; c < 12; ++c) { double sv = 0.0; for (int a = 0; a < 3; ++a) sv -= Ji[3 * j + a] * sm.rec.foot[i].C[a][c]; L.Px[j][c] = sv; } }
+      double Jm[9], Ji[9]; for (int a = 0; a < 3; ++a) for (int j = 0; j < 3; ++j) Jm[3 * a + j] = fb.Jl[3 * j + a]; inv3(Jm, Ji);
+      for (int e = 0; e < 9; ++e) L.G[e] = -Ji[e];
     } else {          // zero force: dF = -F ; normal velocity: pivot joint eliminated
-      for (int a = 0; a < 3; ++a) sm.Pe_full[3 * i + a] = -sm.u[3 * i + a];
-      const double piv = sm.rec.foot[i].Jl[3 * pivot + 2], nip = -1.0 / piv;
-      L.Pe[pivot] = sm.rec.foot[i].e[2] * nip; sm.Pe_full[12 + first + pivot] = L.Pe[pivot];
-      for (int c = 0; c < 12; ++c) L.Px[pivot][c] = sm.rec.foot[i].C[2][c] * nip;
-      int nf = 0; for (int j = 0; j < 3; ++j) if (j != pivot) L.Pu2[nf++] = sm.rec.foot[i].Jl[3 * j + 2] * nip;
+      const double nip = -1.0 / fb.Jl[3 * pivot + 2];
+      for (int e = 0; e < 9; ++e) L.G[e] = (e == 3 * pivot + 2) ? nip : 0.0;
+      int nf = 0; for (int j = 0; j < 3; ++j) if (j != pivot) L.Pu2[nf++] = fb.Jl[3 * j + 2] * nip;
     }
-    // rs = r + R Pe on the leg's joint inputs (the product Rl Px is formed where it is used: Q~ needs Px' (Rl Px), one 3-vector per row)
-    for (int a = 0; a < 3; ++a) { double sv = sm.quad.rf[12 + first + a]; for (int j = 0; j < 3; ++j) sv += L.Rl[3 * a + j] * L.Pe[j]; L.rs[a] = sv; }
   }
   __syncwarp();
-  // rs of every input: r + R Pe (R couples joint velocities only inside a leg; forces and arm inputs only with themselves)
+  if (lane < 16) { const int i = lane >> 2, j = lane & 3; if (j < 3) sm.leg[i].free_col[j] = sm.col_of_input[12 + sm.leg[i].first + j]; }
+  for (int e = lane; e < 144; e += 32) {   // P_x: (foot, row, support column)
+    const int i = e / 36, jc = e - 36 * i, j = jc / 12, c = jc - 12 * j; LegWs& L = sm.leg[i]; const ne::FootBlk& fb = sm.rec.foot[i];
+    double sv = 0.0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) sv = fma(L.G[3 * j + a], fb.C[a][c], sv);
+    L.Px[j][c] = sv;
+  }
+  if (lane < NU) {   // P_e of every input: -F for the forces of swing feet, G e for the leg joints (zero for the free joints of swing legs)
+    double pe = 0.0;
+    if (lane < 12) { if (!sm.leg[lane / 3].stance) pe = -sm.u[lane]; }
+    else if (lane < 24) { const int jl = lane - 12; const int i = foot_of_leg_joint(lfp, jl), j = jl % 3; const LegWs& L = sm.leg[i]; const double* e = sm.rec.foot[i].e;
+#pragma unroll
+      for (int a = 0; a < 3; ++a) pe = fma(L.G[3 * j + a], e[a], pe); }
+    sm.Pe_full[lane] = pe;
+  }
+  __syncwarp();
+  // rs of every input: r + R Pe (R couples forces and leg-joint velocities only inside their triple, the arm inputs only with themselves)
   if (lane < NU) {
     double sv = sm.quad.rf[lane];
-    if (lane < 12) { const int f = lane / 3; for (int a = 0; a < 3; ++a) sv += quad_R(mdl, &sm.quad, lane, 3 * f + a) * sm.Pe_full[3 * f + a]; }
-    else if (lane < 24) { const int i = foot_of_leg_joint(lfp, lane - 12); sv = sm.leg[i].rs[(lane - 12) % 3]; }
+    if (lane < 24) { const int f = lane / 3; for (int a = 0; a < 3; ++a) sv += sm.Rw[lane][a] * sm.Pe_full[3 * f + a]; }
     sm.rs[lane] = sv;
   }
-  // continuous-time Jacobians of the two RK2 stages from the record's blocks
-  const double imr = 1.0 / sc->m;
-  expand_flow(sm.rec.s1, sm.rec.foot[0].JxF, ne::FOOT_DBL, sm.A1r, lfp, lane); expand_flow(sm.rec.s2, sm.rec.foot2[0].JxF, ne::FOOT2_DBL, sm.Ar, lfp, lane);
   // force block of rows 3:6 of df/du at both stages, column c = lane < 12 (foot i = c / 3, axis a = c % 3): cross(d_i, e_a)[r] / m - three entries per stage, kept in registers
-  // (the foot blocks of the record are about to be overlaid by the RK2 combination's outputs)
+  const double imr = 1.0 / sc->m;
   if (lane < 12) { const int i = lane / 3, a = lane - 3 * i; const double* d1 = sm.rec.foot[i].d; const double* d2 = sm.rec.foot2[i].d;
 #pragma unroll
     for (int r = 0; r < 3; ++r) if (r != a) { const double sgn = ((a - r + 3) % 3 == 1) ? -imr : imr; b1v[r] = sgn * d1[3 - r - a]; b2v[r] = sgn * d2[3 - r - a]; } }
+  // column c = lane of rows 3:12 of df/dx at both RK2 stages, straight from the record's blocks (the foot blocks are about to be overlaid by the RK2 combination's outputs)
+  if (lane < NX) { flow_column(sm.rec.s1, sm.rec.foot[0].JxF, ne::FOOT_DBL, lfp, lane, a1); flow_column(sm.rec.s2, sm.rec.foot2[0].JxF, ne::FOOT2_DBL, lfp, lane, a2); }
   __syncwarp();
   }
   const double w1 = mdl->rk_w1, w2 = mdl->rk_w2, cdt = mdl->rk_c * dt, mass = sc->m, dtw = dt * (w1 + w2), imass = 1.0 / mass;
@@ -333,54 +348,53 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
     bb = xv + dt * (w1 * fa + w2 * fb) - xnv; lt.bvec[lane] = bb; }   // defect
   const double dyn_ss = warp_sum(bb * bb);
   // A_d - I (rows 3:12) = dt (w1 A1 + w2 (A2 + c dt A2 A1)) ; B_d rows 3:12 = dt (w1 B1 + w2 (B2 + c dt A2 B1)): force columns (9x12), joint columns only in the h_ang rows (3x18)
-  if (lane < NX) {   // lane = column c: needs column c of A1 only, so A1r can be overwritten in place
-    const int c = lane; double a1[9], out[9];
+  double out[9];   // lane = column c: column c of A_d - I, rows 3:12 (the inner products run over the non-zero entries of A2's columns 3:12 only)
+  if (lane < NX) {
+    const int c = lane; const ne::FlowBlk& f2 = sm.rec.s2;
 #pragma unroll
-    for (int q = 0; q < 9; ++q) a1[q] = sm.A1r[q * NX + c];
+    for (int r = 0; r < 9; ++r) { double aa = 0.0;
 #pragma unroll
-    for (int r = 0; r < 9; ++r) { const double* a2 = sm.Ar + r * NX; double aa = 0.0;
+      for (int q = 0; q < 9; ++q) if (!(q >= 3 && q < 6) && !(q < 3 && r < 3)) aa = fma(flow_inner(f2, r, q), a1[q], aa);
+      out[r] = dt * (w1 * a1[r] + w2 * (a2[r] + cdt * aa));
+      if (c < 12) { double b1 = 0.0, b2 = 0.0; if (r < 3) { b1 = b1v[r < 3 ? r : 0]; b2 = b2v[r < 3 ? r : 0]; } double ab = (r == 3 + c % 3) ? imass : 0.0;   // d / d h_lin of stage 2 times d h_lin / dF
+        if (r >= 3) {
 #pragma unroll
-      for (int q = 0; q < 9; ++q) aa = fma(a2[3 + q], a1[q], aa);
-      out[r] = dt * (w1 * a1[r] + w2 * (a2[c] + cdt * aa));
-      if (c < 12) { double b1 = 0.0, b2 = 0.0; if (r < 3) { b1 = b1v[r < 3 ? r : 0]; b2 = b2v[r < 3 ? r : 0]; } double ab = a2[c % 3] * imass;
-#pragma unroll
-        for (int q = 0; q < 3; ++q) ab += a2[3 + q] * b1v[q]; lt.BrdF[r * 12 + c] = dt * (w1 * b1 + w2 * (b2 + cdt * ab)); }
-      else if (r < 3) lt.BrdJ[r * NJ + c - 12] = dt * w2 * cdt * a2[c]; }
-#pragma unroll
-    for (int r = 0; r < 9; ++r) sm.A1r[r * NX + c] = out[r];
+          for (int q = 0; q < 3; ++q) ab += flow_inner(f2, r, q) * b1v[q]; }
+        lt.BrdF[r * 12 + c] = dt * (w1 * b1 + w2 * (b2 + cdt * ab)); }
+      else if (r < 3) lt.BrdJ[r * NJ + c - 12] = dt * w2 * cdt * a2[r]; }
   }
   __syncwarp();
-  // ---- projected dynamics: b~ = b + B_d Pe (lane = state row) ; rows 3:12 of A~ = A_d + B_d Px (the h_ang rows pick up the dependent joint velocities) ----
+  // ---- projected dynamics: b~ = b + B_d Pe (lane = state row) ; rows 3:12 of A~ = A_d + B_d Px (lane = column; the h_ang rows pick up the dependent joint velocities) ----
   double* tl = sg + ST_TAIL; int32_t* si = reinterpret_cast<int32_t*>(tl + T_INT);
   if (lane < NX) {
     const int r = lane; double bt = lt.bvec[r];
-    if (r >= 3 && r < 6) {       // + sum_legs BrdJ[r][joint] * Px_joint (accumulated in the shared-memory row, own thread)
-      double* arow = sm.A1r + (r - 3) * NX; double acc[12];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { const LegWs& L = sm.leg[i];
-#pragma unroll
-        for (int c = 0; c < 12; ++c) acc[c] = 0.0;
-        for (int j = 0; j < 3; ++j) if (L.dep[j]) { const double coef = lt.BrdJ[(r - 3) * NJ + L.first + j]; bt += coef * L.Pe[j];
-#pragma unroll
-          for (int c = 0; c < 12; ++c) acc[c] = fma(coef, L.Px[j][c], acc[c]); }
-#pragma unroll
-        for (int c = 0; c < 12; ++c) arow[sup_col(c, L.first)] += acc[c];
-      }
-    }
+    if (r >= 3 && r < 6) for (int i = 0; i < 4; ++i) { const LegWs& L = sm.leg[i]; for (int j = 0; j < 3; ++j) if (L.dep[j]) bt += lt.BrdJ[(r - 3) * NJ + L.first + j] * sm.Pe_full[12 + L.first + j]; }
     if (r >= 12 && r < 24) {     // dependent joint-velocity rows: I + dtw * Px
-      const int i = foot_of_leg_joint(lfp, r - 12); const LegWs& L = sm.leg[i]; const int j = (r - 12) % 3;
-      if (L.dep[j]) bt += dtw * L.Pe[j];
+      const LegWs& L = sm.leg[foot_of_leg_joint(lfp, r - 12)];
+      if (L.dep[(r - 12) % 3]) bt += dtw * sm.Pe_full[r];
     }
     if (r < 3) for (int f = 0; f < 4; ++f) bt += (dtw * imass) * sm.Pe_full[3 * f + r];
     if (r >= 3 && r < 12) for (int f = 0; f < 4; ++f) if (!sm.leg[f].stance) for (int a = 0; a < 3; ++a) bt += lt.BrdF[(r - 3) * 12 + 3 * f + a] * sm.Pe_full[3 * f + a];
     tl[T_b + r] = bt;
     if (r >= 3 && r < 12) sg[ST_AR + (r - 3) * LDX + NX] = bt;   // b~[3:12] also rides in column 30 of the dense A~ rows (K3's vector recursion)
-  }
-  if (lane >= 3 && lane < 12) sm.A1r[(lane - 3) * NX + lane] += 1.0;   // A1r rows become rows 3:12 of A~ themselves (own row of each lane: no hazard with the h_ang update above)
-  __syncwarp();
-  // rows 3:12 of A~ with K3's shared-memory pitch (one 240-byte run per store instruction), zero padding columns 31..35
+    const int c = lane; const int pos_all = c < 6 ? c : ((c >= 9 && c < 12) ? c - 3 : -1);   // support position of column c in every leg's block (-1: only the own leg's joints, or none)
 #pragma unroll
-  for (int r = 0; r < 9; ++r) { if (lane < NX) sg[ST_AR + r * LDX + lane] = sm.A1r[r * NX + lane]; else if (lane == 31) sg[ST_AR + r * LDX + 31] = 0.0; }
+    for (int rr = 0; rr < 3; ++rr) {   // + sum_legs BrdJ[rr][joint] * Px_joint[c], legs in order
+      double v = out[rr];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { const LegWs& L = sm.leg[i]; const int first = L.first;
+        const int pos = pos_all >= 0 ? pos_all : ((c >= 12 + first && c < 15 + first) ? 9 + c - 12 - first : -1);
+        if (pos >= 0) { double acc = 0.0;
+          for (int j = 0; j < 3; ++j) if (L.dep[j]) acc = fma(lt.BrdJ[rr * NJ + first + j], L.Px[j][pos], acc);
+          v += acc; } }
+      out[rr] = v;
+    }
+#pragma unroll
+    for (int rr = 0; rr < 9; ++rr) { if (c == rr + 3) out[rr] += 1.0; sg[ST_AR + rr * LDX + c] = out[rr]; }   // rows 3:12 of A~ with K3's shared-memory pitch (one 240-byte run per store instruction)
+  } else if (lane == 31) {
+#pragma unroll
+    for (int rr = 0; rr < 9; ++rr) sg[ST_AR + rr * LDX + 31] = 0.0;   // zero padding columns 31..35
+  }
   for (int e = lane; e < 36; e += 32) sg[ST_AR + (e >> 2) * LDX + 32 + (e & 3)] = 0.0;
   // Px rows of the 12 leg-joint velocity inputs on their support columns: K3 rebuilds rows 12:24 of A~ (I + dtw Px) and the dependent inputs of the rollout from them
   for (int e = lane; e < 144; e += 32) { const int j12 = e / 12, c = e - 12 * j12; const LegWs& L = sm.leg[foot_of_leg_joint(lfp, j12)]; const int j = j12 % 3; tl[T_PXJ + e] = L.dep[j] ? L.Px[j][c] : 0.0; }
@@ -418,9 +432,9 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
 #pragma unroll
         for (int c = 0; c < 12; ++c) blk[c] = 0.0;
         double w3[3] = {0.0, 0.0, 0.0};   // row pr of Px' Rl ; then blk = w3' Px  (= row pr of Px' Rl Px)
-        for (int j = 0; j < 3; ++j) if (L.dep[j]) { const double pj = L.Px[j][pr]; qv = fma(pj, L.rs[j], qv);
+        for (int j = 0; j < 3; ++j) if (L.dep[j]) { const double pj = L.Px[j][pr]; qv = fma(pj, sm.rs[12 + first + j], qv);
 #pragma unroll
-          for (int a = 0; a < 3; ++a) w3[a] = fma(pj, L.Rl[3 * j + a], w3[a]); }
+          for (int a = 0; a < 3; ++a) w3[a] = fma(pj, sm.Rw[12 + first + j][a], w3[a]); }
         for (int a = 0; a < 3; ++a) if (L.dep[a]) { const double wa = w3[a];
 #pragma unroll
           for (int c = 0; c < 12; ++c) blk[c] = fma(wa, L.Px[a][c], blk[c]); }
@@ -451,21 +465,22 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
       const int fa = sm.free_idx[a]; double rv = sm.rs[fa]; int li = -1, jf = -1;
       if (fa >= 12 && fa < 24) { li = foot_of_leg_joint(lfp, fa - 12); jf = (fa - 12) % 3; }
       const bool swing_joint = li >= 0 && !sm.leg[li].stance;
+      const double* Rl = sm.Rw[jf >= 0 ? fa - jf : 0];   // swing joint: rows of the leg's 3x3 input-weight block, Rl[3 * j + k] = R[first + j][first + k]
       if (swing_joint) {   // free joint of a swing leg: coupled to the pivot through R_leg and Pu
         const LegWs& L = sm.leg[li]; const int pv = L.pivot; const int jfi = jf > pv ? jf - 1 : jf; const double pu = L.Pu2[jfi];
-        rv += pu * L.rs[pv];
-        const double coef = L.Rl[3 * jf + pv]; double* Srow = tl + T_SJ + (2 * li + jfi) * 12;
-        const double cf = dt * (coef + pu * L.Rl[3 * pv + pv]);   // only the pivot row of Px is non-zero in a swing leg: (Rl Px)[pv] = Rl[pv][pv] Px[pv]
+        rv += pu * sm.rs[fa - jf + pv];
+        const double coef = Rl[3 * jf + pv]; double* Srow = tl + T_SJ + (2 * li + jfi) * 12;
+        const double cf = dt * (coef + pu * Rl[3 * pv + pv]);   // only the pivot row of Px is non-zero in a swing leg: (Rl Px)[pv] = Rl[pv][pv] Px[pv]
         for (int c = 0; c < 12; ++c) Srow[c] = cf * L.Px[pv][c];
       }
       rtil = dt * rv;
       // R is block diagonal (3x3 blocks over force / leg-joint triples, diagonal over the arm): only the free inputs of fa's own block contribute to row a
-      if (fa >= 24) rt[0] = dt * quad_R(mdl, &sm.quad, fa, fa);
+      if (fa >= 24) rt[0] = dt * sm.Rw[fa][0];
       else { const int bi = fa / 3;
         for (int jc = 0; jc < 3; ++jc) { const int fc = 3 * bi + jc; if (sm.col_of_input[fc] < 0) continue;
-          double v = quad_R(mdl, &sm.quad, fa, fc);
+          double v = sm.Rw[fa][jc];
           if (swing_joint) { const LegWs& L = sm.leg[li]; const int pv = L.pivot; const double pa = L.Pu2[jf > pv ? jf - 1 : jf], pc = L.Pu2[jc > pv ? jc - 1 : jc];
-            v += pa * L.Rl[3 * pv + jc] + L.Rl[3 * jf + pv] * pc + pa * L.Rl[3 * pv + pv] * pc; }
+            v += pa * Rl[3 * pv + jc] + Rl[3 * jf + pv] * pc + pa * Rl[3 * pv + pv] * pc; }
           rt[jc] = dt * v; } }
     }
     tl[T_r + a] = rtil; tl[T_RT + 3 * a] = rt[0]; tl[T_RT + 3 * a + 1] = rt[1]; tl[T_RT + 3 * a + 2] = rt[2];

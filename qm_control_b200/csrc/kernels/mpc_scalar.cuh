@@ -40,9 +40,11 @@ template <class MT> QMB_HD bool swing_reference(const DevModel* __restrict__ mdl
   zp = ((c3 * tn + c2) * tn + c1) * tn + c0; zv = ((3.0 * c3 * tn + 2.0 * c2) * tn + c1) * idt; return true;
 }
 // ocs2 RelaxedBarrierPenalty [upstream]
+// (one logarithm of the selected argument: lanes of a warp that fall on different sides of delta do not evaluate it twice)
 QMB_HD void relaxed_barrier(double mu, double delta, double h, double& p0, double& p1, double& p2) {
-  if (h > delta) { const double ih = 1.0 / h; p0 = -mu * log(h); p1 = -mu * ih; p2 = mu * ih * ih; }
-  else { const double t = (h - 2.0 * delta) / delta; p0 = mu * (-log(delta) + 0.5 * t * t - 0.5); p1 = mu * (h - 2.0 * delta) / (delta * delta); p2 = mu / (delta * delta); }
+  const bool inside = h > delta; const double lg = log(inside ? h : delta);
+  if (inside) { const double ih = 1.0 / h; p0 = -mu * lg; p1 = -mu * ih; p2 = mu * ih * ih; }
+  else { const double t = (h - 2.0 * delta) / delta; p0 = mu * (-lg + 0.5 * t * t - 0.5); p1 = mu * (h - 2.0 * delta) / (delta * delta); p2 = mu / (delta * delta); }
 }
 
 QMB_HD int ee_pos(int c) { return (c >= 6 && c < 12) ? c - 6 : (c >= 24 ? c - 18 : -1); }
@@ -62,8 +64,7 @@ QMB_HD double quad_R(const DevModel* __restrict__ mdl, const QuadWs* q, int i, i
 // joint-velocity inputs, the input weight couples joint velocities only inside a leg
 struct LegWs {
   double Px[3][12];     // rows of P_x of the dependent joint-velocity inputs of this leg on the support columns (stance: 3 rows; swing: pivot row only)
-  double Rl[9];         // 3x3 input-weight block of the leg (incl. diagonal additions)
-  double Pe[3], rs[3];  // P_e of the dependent joints ; r + R P_e on the leg's joint inputs
+  double G[9];          // elimination matrix: P_x row j = sum_a G[3j+a] C[a], P_e[j] = sum_a G[3j+a] e[a] (stance: minus the inverse of the foot's joint-velocity Jacobian; swing: -1 / pivot entry at (pivot, z), zero elsewhere)
   double Pu2[2];        // swing: coupling of the pivot joint to the two free joints
   int dep[3];           // is joint j of this leg dependent
   int pivot, stance, first, free_col[3];   // projected-input column of each free joint (-1 if dependent)
