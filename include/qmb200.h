@@ -332,6 +332,63 @@ int qmb200_sim_get_robot_terrain(const qmb200_handle* h, int32_t* tile /*[B]*/, 
  * (a few fixed-point iterations, since the feet move with the tilt), and the base height puts the deepest foot at the static penetration m g / (4 k). */
 int qmb200_sim_standing_state(const qmb200_handle* h, int32_t n, const double* xy_yaw /*[n][3]*/, double* q /*[n][24]*/, double* v /*[n][24]*/);
 
+/* ---- sensors of the plant: the IMU block of QMHWSim::readSim (qm_gazebo/src/QMHWSim.cpp:51-69) and the joint handles it fills, batched on the device.
+ *      The IMU link unitree_imu sits at the base origin with the base's axes (robot.urdf), so with R = R(zyx) and w the world angular velocity:
+ *        sensors[QMB200_SENSORS] = [quat xyzw(4) of R exp([n_o]x), gyro(3) = R^T w + n_g, accel(3) = R^T((v_lin - v_prev_lin) / dt - g) + n_a, joint pos(18)
+ *                                   = q[6:24] + n_q, joint vel(18) = v[6:24] + n_v],  g = (0, 0, -9.81)
+ *      The accelerometer reads the mean acceleration over the step that started at v_prev.  The contact flags are the mask qmb200_sim_step returns.
+ *      Each noise term is sigma * N(0, 1), drawn as a pure function of (seed, robot, sample, channel): a counter-based integer hash and Box-Muller, so a
+ *      draw depends neither on the batch nor on the launch; robot = the robot's index in the handle's batch plus rank * batch with a communicator
+ *      (qmb200_comm_init).  The orientation noise n_o ~ N(0, sigma_orientation^2 1) is a rotation vector in the body frame.  All sigmas default to 0 (the
+ *      reference's readSim, whose noise is a TODO); qm_gazebo/config/default.yaml:3-8 gives the covariances 0.0012 / 0.0004 / 0.01 of orientation,
+ *      angular velocity and linear acceleration, i.e. sigma 0.0346 rad, 0.02 rad/s and 0.1 m/s^2. */
+#define QMB200_SENSORS 46
+typedef struct qmb200_sensor_params {
+  uint64_t seed;
+  double sigma_orientation, sigma_gyro, sigma_accel, sigma_joint_pos, sigma_joint_vel;   /* rad, rad/s, m/s^2, rad, rad/s */
+} qmb200_sensor_params;
+int qmb200_sim_get_sensor_params(const qmb200_handle* h, qmb200_sensor_params* out);
+/* rejects a non-finite or negative sigma; on rejection the stored values stay unchanged */
+int qmb200_sim_set_sensor_params(qmb200_handle* h, const qmb200_sensor_params* p);
+/* sensors [B][46] of the plant state (q, v) [B][24] after a step of dt s (finite, > 0) that started at velocity v_prev [B][24] (owned by the caller);
+ * sample numbers the reading for the noise. */
+int qmb200_sim_read_sensors(qmb200_handle* h, double dt, int64_t sample, const double* q /*[B][24]*/, const double* v /*[B][24]*/, const double* v_prev /*[B][24]*/,
+                            double* sensors /*[B][46]*/);
+int qmb200_sim_read_sensors_dev(qmb200_handle* h, double dt, int64_t sample, const double* q, const double* v, const double* v_prev, double* sensors, void* cuda_stream);
+
+/* ---- base state estimation, the seam of StateEstimateBase::update (qm_estimation/src/StateEstimateBase.cpp:41-78, fed by
+ *      QMController::updateStateEstimation, qm_controllers/src/QMController.cpp:202-244): a linear Kalman filter per robot on
+ *      x = [p_base(3), v_base(3), p_foot(4 x 3, contact order LF, RF, LH, RH)] in the world frame, from the sensors above and the contact mask.
+ *      Orientation and angular velocity come from the IMU as read (zyx from the quaternion, yaw in (-pi, pi]; w = R gyro); the legs' kinematics at the
+ *      encoder readings give each foot's offset r_i from the base and its velocity.  Predict: p += v dt + a dt^2 / 2, v += a dt with a = R accel + g,
+ *      feet constant, P = A P A^T + dt diag(process).  Update with 28 rows: p_base - p_foot_i = -r_i, v_base = -dr_i/dt and p_foot_i,z = foot_height per
+ *      foot.  A foot not in contact has its process and measurement variances scaled by swing_scale.  The rows assume the plane: no terrain.
+ *   process_base_pos, process_base_vel, process_foot    process noise per second: m^2/s, (m/s)^2/s, m^2/s
+ *   meas_foot_pos, meas_foot_vel, meas_foot_height      measurement variances: m^2, (m/s)^2, m^2
+ *   swing_scale                                         factor on a swing foot's variances
+ *   foot_height                                         world z of a stance foot frame: ground_height + foot_radius - m g / (4 stiffness); the default is that of
+ *                                                       the default plant params and the model's mass
+ *   p0_base_pos, p0_base_vel, p0_foot                   P = diag(p0) at the reset (m^2, (m/s)^2, m^2) */
+typedef struct qmb200_state_est_params {
+  double process_base_pos, process_base_vel, process_foot, meas_foot_pos, meas_foot_vel, meas_foot_height, swing_scale, foot_height, p0_base_pos, p0_base_vel, p0_foot;
+} qmb200_state_est_params;
+int qmb200_state_est_get_params(const qmb200_handle* h, qmb200_state_est_params* out);
+/* rejects a non-finite value and a negative one (foot_height may take any finite value); on rejection the stored values stay unchanged */
+int qmb200_state_est_set_params(qmb200_handle* h, const qmb200_state_est_params* p);
+/* (Re)starts the filter of every robot: p_base = base_pos [B][3] (required), v_base = 0, P = diag(p0), no call yet.  Synchronous. */
+int qmb200_state_est_reset(qmb200_handle* h, const double* base_pos /*[B][3]*/);
+/* One filter call per robot from sensors [B][46] (qmb200_sim_read_sensors) and the contact mask [B] (qmb200_sim_step) of a step of dt s (finite, > 0):
+ * writes rbd_est [B][55] (include/qmb200.h layout: zyx, p, joints, w, v, joint rates, end-effector pose) for the controller.  The first call after a reset
+ * only places the feet at p_base + r_i.  status [B] (written, not OR-ed): QMB200_ST_NAN for a non-finite input (nothing is written) or update,
+ * QMB200_ST_NOT_PD when the innovation covariance fails its Cholesky; the robot then keeps x and P, and rbd_est is written from them. */
+int qmb200_state_est_step(qmb200_handle* h, double dt, const double* sensors /*[B][46]*/, const int32_t* contact /*[B]*/, double* rbd_est /*[B][55]*/, int32_t* status /*[B]*/);
+int qmb200_state_est_step_dev(qmb200_handle* h, double dt, const double* sensors, const int32_t* contact, double* rbd_est, int32_t* status, void* cuda_stream);
+/* Synchronous: x [B][18], the diagonal of P [B][18] and the calls since the reset [B].  Any output may be NULL. */
+int qmb200_state_est_get(qmb200_handle* h, double* x /*[B][18]*/, double* p_diag /*[B][18]*/, int32_t* samples /*[B]*/);
+/* Releases the filter state.  Step and get fail until the next reset.  Stopping a filter that is not running does nothing and returns 0, as
+ * qmb200_payload_est_stop does, so a caller's clean-up may stop unconditionally. */
+int qmb200_state_est_stop(qmb200_handle* h);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

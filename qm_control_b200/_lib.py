@@ -39,6 +39,27 @@ class PayloadEstParams(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("forgetting", "p0_mass", "p0_first_moment", "p0_inertia", "trace_max", "mass_min", "mass_max", "offset_max")]
 
 
+SENSORS = 46   # QMB200_SENSORS
+
+
+class SensorParams(C.Structure):
+    """qmb200_sensor_params: the noise of the plant's IMU and encoder readings (include/qmb200.h, DESIGN.md §4.6)."""
+    _fields_ = [("seed", C.c_uint64)] + [(n, C.c_double) for n in ("sigma_orientation", "sigma_gyro", "sigma_accel", "sigma_joint_pos", "sigma_joint_vel")]
+
+
+class StateEstParams(C.Structure):
+    """qmb200_state_est_params: the base state estimator's constants (include/qmb200.h, DESIGN.md §4.6)."""
+    _fields_ = [(n, C.c_double) for n in ("process_base_pos", "process_base_vel", "process_foot", "meas_foot_pos", "meas_foot_vel", "meas_foot_height", "swing_scale",
+                                          "foot_height", "p0_base_pos", "p0_base_vel", "p0_foot")]
+
+
+# the sensor reading's columns (qmb200_sim_read_sensors) and the state estimator's state x (qmb200_state_est_get)
+SENSOR_LAYOUT = ("quat_x", "quat_y", "quat_z", "quat_w", "gyro_x", "gyro_y", "gyro_z", "accel_x", "accel_y", "accel_z") + \
+                tuple("joint_pos_%d" % j for j in range(18)) + tuple("joint_vel_%d" % j for j in range(18))
+STATE_EST_LAYOUT = ("p_x", "p_y", "p_z", "v_x", "v_y", "v_z") + tuple("foot_%s_%s" % (f, a) for f in ("LF", "RF", "LH", "RH") for a in "xyz")
+# the reference sensor noise of qm_gazebo/config/default.yaml:3-8 (covariances 0.0012, 0.0004, 0.01 of orientation, angular velocity, linear acceleration)
+SENSOR_NOISE_REFERENCE = dict(sigma_orientation=0.0012 ** 0.5, sigma_gyro=0.0004 ** 0.5, sigma_accel=0.01 ** 0.5)
+
 # the payload estimator's parameter vector theta: the load's inertial parameters in the end-effector frame about its origin (include/qmb200.h)
 THETA_LAYOUT = ("m", "mc_x", "mc_y", "mc_z", "I_xx", "I_xy", "I_xz", "I_yy", "I_yz", "I_zz")
 
@@ -119,6 +140,17 @@ PROTOTYPES = {
     "qmb200_sim_set_robot_terrain": (I32, [P] * 3),
     "qmb200_sim_get_robot_terrain": (I32, [P] * 4),
     "qmb200_sim_standing_state": (I32, [P, I32, P, P, P]),
+    "qmb200_sim_get_sensor_params": (I32, [P] * 2),
+    "qmb200_sim_set_sensor_params": (I32, [P] * 2),
+    "qmb200_sim_read_sensors": (I32, [P, D, I64] + [P] * 4),
+    "qmb200_sim_read_sensors_dev": (I32, [P, D, I64] + [P] * 5),
+    "qmb200_state_est_get_params": (I32, [P] * 2),
+    "qmb200_state_est_set_params": (I32, [P] * 2),
+    "qmb200_state_est_reset": (I32, [P] * 2),
+    "qmb200_state_est_step": (I32, [P, D] + [P] * 4),
+    "qmb200_state_est_step_dev": (I32, [P, D] + [P] * 5),
+    "qmb200_state_est_get": (I32, [P] * 4),
+    "qmb200_state_est_stop": (I32, [P]),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

@@ -12,6 +12,9 @@ params (floor friction, end-effector and base payloads: Solver.sim_set_robot_par
 controller is not told about any of them unless the run sets its model payload (Solver.set_model_payload), e.g. to the plant's payload.
 With payload_estimator set, an online estimate of each robot's end-effector payload (Solver.payload_est_*) runs beside the plant on what the
 controller sees: it steps after every plant step and is committed to the model payload right before every MPC tick.
+With state_estimator set, the controller no longer reads the plant's true state: after every plant step the IMU and encoders are read
+(Solver.sim_read_sensors_dev) and a base state estimator (Solver.state_est_*) turns them and the contact flags into the measurement every consumer on
+the controller side reads (the updates, the targets' end-effector state, the payload estimator).  The plant and the record keep the truth.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -20,7 +23,8 @@ import contextlib
 
 import numpy as np
 
-from ._lib import EMAX, KMAX, NX, RBD, TARGET
+from . import _lib
+from ._lib import EMAX, KMAX, NX, RBD, SENSORS, TARGET
 from .interface import gait_schedule
 
 MPC_PERIOD_MS = 10         # mpcDesiredFrequency 100 (task.info)
@@ -43,7 +47,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
-        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None):
+        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -60,12 +64,28 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     payload in force (model_payload's value, or the handle's own): one step after every plant step with the same effort and measurement, one commit right
     before every MPC tick, so the targets, solve, updates and observation of one 10 ms window share one model.  Its status is OR-ed into the record's.
     The estimator is stopped and the previous model payload and estimator parameters restored when run returns.
+    state_estimator: True, or a dict of qmb200_state_est_params overrides (Solver.state_est_set_params), closes the loop on estimated base states: after
+    every plant step (1 ms step k) the sensors are read with sample = k (-1 for the reading of the start) and the estimator steps; update_dev, the
+    targets' end-effector state and the payload estimator read its rbd_est.  It starts at the plant's start position.  Its status is OR-ed into the
+    record's.  Not with terrain: the estimator's foot-height rows assume the plane.
+    sensor_noise: None (noise-free readings), "reference" (_lib.SENSOR_NOISE_REFERENCE, the IMU covariances of qm_gazebo/config/default.yaml) or a dict
+    of qmb200_sensor_params overrides; only with state_estimator.  The estimator is stopped and the previous sensor and estimator parameters restored
+    when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
-    payload_est[ticks, B, 8] = the model payload rows committed at each record's MPC tick)."""
+    payload_est[ticks, B, 8] = the model payload rows committed at each record's MPC tick; with state_estimator also base_est[ticks, B, 6], the estimated base in
+    the layout of base)."""
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
+    if state_estimator is not None and state_estimator is not True and not isinstance(state_estimator, dict):
+        raise ValueError("closed_loop.run: state_estimator must be None, True or a dict of estimator parameters, got %r" % (state_estimator,))
+    if sensor_noise is not None and sensor_noise != "reference" and not isinstance(sensor_noise, dict):
+        raise ValueError("closed_loop.run: sensor_noise must be None, \"reference\" or a dict of sensor parameters, got %r" % (sensor_noise,))
+    if sensor_noise is not None and state_estimator is None:
+        raise ValueError("closed_loop.run: sensor_noise needs state_estimator (the controller reads the plant's true state otherwise)")
+    if state_estimator is not None and terrain is not None:
+        raise ValueError("closed_loop.run: state_estimator does not support terrain (its foot-height rows assume the plane)")
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
         if terrain is not None:
@@ -74,10 +94,12 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_model_payload(solver, model_payload, payload))
         if payload_estimator is not None:
             scope.enter_context(_payload_estimator(solver, payload_estimator))
+        if state_estimator is not None:
+            scope.enter_context(_state_estimator(solver, state_estimator, sensor_noise))
         if friction_mu is not None or payload is not None:
             scope.enter_context(_robot_params(solver, friction_mu, payload))
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
-                    torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None)
+                    torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None)
 
 
 @contextlib.contextmanager
@@ -128,6 +150,21 @@ def _payload_estimator(solver, params):
 
 
 @contextlib.contextmanager
+def _state_estimator(solver, params, noise):
+    prev_params, prev_noise = solver.state_est_get_params(), solver.sim_get_sensor_params()
+    try:
+        if isinstance(params, dict):
+            solver.state_est_set_params(**params)
+        if noise is not None:
+            solver.sim_set_sensor_params(**(_lib.SENSOR_NOISE_REFERENCE if noise == "reference" else noise))
+        yield   # _run resets the estimator once it knows the start position
+    finally:
+        solver.state_est_stop()
+        solver.sim_set_sensor_params(**prev_noise)
+        solver.state_est_set_params(**prev_params)
+
+
+@contextlib.contextmanager
 def _robot_params(solver, friction_mu, payload):
     prev = solver.sim_get_robot_params()
     solver.sim_set_robot_params(friction_mu=prev["friction_mu"] if friction_mu is None else friction_mu, payload=prev["payload"] if payload is None else payload)
@@ -137,7 +174,7 @@ def _robot_params(solver, friction_mu, payload):
         solver.sim_set_robot_params(**prev)
 
 
-def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False):
+def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -163,11 +200,21 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         contact = torch.zeros(B, dtype=torch.int32, device=dev); sim_st = torch.zeros_like(contact); hw_st = torch.zeros_like(contact); ctl_st = torch.zeros_like(contact)
         acc_st = torch.zeros_like(contact)
         effort = torch.zeros((B, 18), dtype=torch.float64, device=dev); jpos = torch.zeros_like(effort); jvel = torch.zeros_like(effort)
+        if se:   # the controller's measurement: the estimator's rbd_est in place of the plant's rbd
+            v_prev = torch.zeros_like(v); sensors = torch.zeros((B, SENSORS), dtype=torch.float64, device=dev); rbd_est = torch.zeros_like(rbd)
+            se_st = torch.zeros_like(contact); v_prev.copy_(v)
     stream.synchronize()
     solver.sim_step_dev(1e-6, effort, q, v, rbd, contact, sim_st, s)   # a 1 us physics step with zero effort reads the first measured state
+    meas = rbd
+    if se:
+        solver.sim_read_sensors_dev(1e-6, -1, q, v, v_prev, sensors, s)
+        stream.synchronize()
+        solver.state_est_reset(q0[:, 0:3])
+        solver.state_est_step_dev(1e-6, sensors, contact, rbd_est, se_st, s)   # the first call after the reset places the feet
+        meas = rbd_est
     stream.synchronize()
     rbd_h = rbd.cpu().numpy()
-    x_obs0 = solver.centroidal_state_from_rbd(rbd_h)
+    x_obs0 = solver.centroidal_state_from_rbd(meas.cpu().numpy())
     with torch.cuda.stream(stream):
         t_obs = f64(np.full(B, t_obs0)); x_obs = f64(x_obs0)
         joint_cmd = torch.zeros((B, 18, 5), dtype=torch.float64, device=dev); arm_pos = torch.zeros((B, 6), dtype=torch.float64, device=dev); last_time = f64(np.full(B, t_obs0))
@@ -183,6 +230,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         rec_st = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
         if est:
             est_st = torch.zeros_like(contact); rec_pl = torch.zeros((ticks, B, 8), dtype=torch.float64, device=dev)   # row i: the rows of window i's MPC tick
+        if se:
+            rec_base_est = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev)
         push = None
         if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
             push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench), zero=torch.zeros((B, 12), dtype=torch.float64, device=dev),
@@ -193,7 +242,7 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     def mpc_tick(i):
         if est:
             solver.payload_est_commit_dev(s); solver.get_model_payload_dev(rec_pl[i], s)
-        ee_state.copy_(rbd[:, 48:55])
+        ee_state.copy_(meas[:, 48:55])
         solver.target_trajectories_dev(0, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
         solver.mpc_solve_dev(prob, s)
 
@@ -203,10 +252,12 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             if k % MPC_PERIOD_MS == 0 and k > 0:
                 mpc_tick(k // MPC_PERIOD_MS)
             if k % wbc_period_ms == 0:
-                solver.update_dev(rbd, period, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, ctl_st, s)
+                solver.update_dev(meas, period, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, ctl_st, s)
                 acc_st.bitwise_or_(ctl_st)
             hw_time.fill_(t_start + k * 1e-3); jpos.copy_(q[:, 6:]); jvel.copy_(v[:, 6:])
             solver.hw_write_dev(hw_time, hw_period, joint_cmd, jpos, jvel, effort, hw_st, s)
+            if se:
+                v_prev.copy_(v)
             if sim_timer:
                 sim_timer(True)
             if push is not None:
@@ -215,16 +266,24 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             if sim_timer:
                 sim_timer(False)
             acc_st.bitwise_or_(hw_st).bitwise_or_(sim_st)
+            if se:
+                solver.sim_read_sensors_dev(1e-3, k, q, v, v_prev, sensors, s)
+                solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, se_st, s)
+                acc_st.bitwise_or_(se_st)
             if est:
-                solver.payload_est_step_dev(1e-3, effort, rbd, est_st, s)
+                solver.payload_est_step_dev(1e-3, effort, meas, est_st, s)
                 acc_st.bitwise_or_(est_st)
             if (k + 1) % MPC_PERIOD_MS == 0:
                 i = (k + 1) // MPC_PERIOD_MS - 1
                 rec_base[i, :, 0:3] = rbd[:, 3:6]; rec_base[i, :, 3:6] = rbd[:, 0:3]; rec_ee[i] = rbd[:, 48:55]; rec_st[i] = acc_st; acc_st.zero_()
+                if se:
+                    rec_base_est[i, :, 0:3] = rbd_est[:, 3:6]; rec_base_est[i, :, 3:6] = rbd_est[:, 0:3]
     stream.synchronize()
     t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
     out = dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
                start_base=np.c_[q0[:, 0:3], q0[:, 3:6]], start_ee=rbd_h[:, 48:55])
     if est:
         out["payload_est"] = rec_pl.cpu().numpy()
+    if se:
+        out["base_est"] = rec_base_est.cpu().numpy()
     return out

@@ -191,6 +191,23 @@ QMB_HD void euler_rate_map_dot_times_sc(const double* tr, const double* ed, doub
   o[1] = (-sz * zd) * ed[1] + (-sy * yd * sz + cy * cz * zd) * ed[2];
   o[2] = (-cy * yd) * ed[2];
 }
+// Eigen::Quaterniond(const Matrix3d&) (Shepperd's method, largest diagonal pivot); out = x, y, z, w
+QMB_HD void rot_to_quat_xyzw(const double* m, double* o) {
+  const double t = m[0] + m[4] + m[8];
+  if (t > 0.0) {
+    double s = sqrt(t + 1.0); o[3] = 0.5 * s; s = 0.5 / s;
+    o[0] = (m[7] - m[5]) * s; o[1] = (m[2] - m[6]) * s; o[2] = (m[3] - m[1]) * s;
+  } else if (m[8] > (m[4] > m[0] ? m[4] : m[0])) {   // pivot z (the three pivots written out: no run-time register indices)
+    double s = sqrt(m[8] - m[0] - m[4] + 1.0); o[2] = 0.5 * s; s = 0.5 / s;
+    o[3] = (m[3] - m[1]) * s; o[0] = (m[2] + m[6]) * s; o[1] = (m[5] + m[7]) * s;
+  } else if (m[4] > m[0]) {                           // pivot y
+    double s = sqrt(m[4] - m[8] - m[0] + 1.0); o[1] = 0.5 * s; s = 0.5 / s;
+    o[3] = (m[2] - m[6]) * s; o[2] = (m[7] + m[5]) * s; o[0] = (m[1] + m[3]) * s;
+  } else {                                            // pivot x
+    double s = sqrt(m[0] - m[4] - m[8] + 1.0); o[0] = 0.5 * s; s = 0.5 / s;
+    o[3] = (m[7] - m[5]) * s; o[1] = (m[3] + m[1]) * s; o[2] = (m[6] + m[2]) * s;
+  }
+}
 QMB_HD void inv3(const double* m, double* o) {
   const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
   const double id = 1.0 / (m[0] * c00 + m[1] * c01 + m[2] * c02);

@@ -47,24 +47,6 @@ struct SimWs {
   double W[2][6];      // external wrench [nO; f] about the world origin: [0] end effector, [1] base
 };
 
-// Eigen::Quaterniond(const Matrix3d&) (Shepperd's method, largest diagonal pivot); out = x, y, z, w
-__device__ __forceinline__ void rot_to_quat_xyzw(const double* m, double* o) {
-  const double t = m[0] + m[4] + m[8];
-  if (t > 0.0) {
-    double s = sqrt(t + 1.0); o[3] = 0.5 * s; s = 0.5 / s;
-    o[0] = (m[7] - m[5]) * s; o[1] = (m[2] - m[6]) * s; o[2] = (m[3] - m[1]) * s;
-  } else if (m[8] > (m[4] > m[0] ? m[4] : m[0])) {   // pivot z (the three pivots written out: no run-time register indices)
-    double s = sqrt(m[8] - m[0] - m[4] + 1.0); o[2] = 0.5 * s; s = 0.5 / s;
-    o[3] = (m[3] - m[1]) * s; o[0] = (m[2] + m[6]) * s; o[1] = (m[5] + m[7]) * s;
-  } else if (m[4] > m[0]) {                           // pivot y
-    double s = sqrt(m[4] - m[8] - m[0] + 1.0); o[1] = 0.5 * s; s = 0.5 / s;
-    o[3] = (m[2] - m[6]) * s; o[2] = (m[7] + m[5]) * s; o[0] = (m[1] + m[3]) * s;
-  } else {                                            // pivot x
-    double s = sqrt(m[0] - m[4] - m[8] + 1.0); o[0] = 0.5 * s; s = 0.5 / s;
-    o[3] = (m[7] - m[5]) * s; o[1] = (m[3] + m[1]) * s; o[2] = (m[6] + m[2]) * s;
-  }
-}
-
 // Lane 0: the end-effector frame, lane 1: the base frame.  Adds the payload point mass to Ic / F of the frame's body (payload.cuh) and writes the wrench about
 // the world origin to w->W[lane] (sim_step_kernel's header has the layouts).
 __device__ __forceinline__ void frame_loads(const DevModel* __restrict__ mdl, SimWs* w, int lane, const double* __restrict__ payload, const double* __restrict__ wrench) {

@@ -459,6 +459,74 @@ class Solver:
         self._call("sim_standing_state", n, _p(xy), _p(q), _p(v))
         return q, v
 
+    # ---------------- sensors and base state estimate (include/qmb200.h: qmb200_sim_read_sensors, qmb200_state_est_*; DESIGN.md §4.6) ----------------
+    def sim_get_sensor_params(self):
+        """→ dict of qmb200_sensor_params (seed an int, the sigmas floats)."""
+        p = _lib.SensorParams(); self._call("sim_get_sensor_params", C.byref(p))
+        return {n: getattr(p, n) for n, _ in _lib.SensorParams._fields_}
+
+    def sim_set_sensor_params(self, **params):
+        """Keyword per field of qmb200_sensor_params; unspecified fields keep their value."""
+        p = _lib.SensorParams(); self._call("sim_get_sensor_params", C.byref(p))
+        names = [n for n, _ in _lib.SensorParams._fields_]
+        for k, v in params.items():
+            if k not in names:
+                raise ValueError("sim_set_sensor_params: unknown parameter %r (one of %s)" % (k, ", ".join(names)))
+            setattr(p, k, int(v) if k == "seed" else float(v))
+        self._call("sim_set_sensor_params", C.byref(p))
+
+    def sim_read_sensors(self, dt, sample, q, v, v_prev):
+        """IMU and encoder readings of the plant state (q, v) [B, 24] after a step of dt s that started at v_prev → sensors [B, 46] (_lib.SENSOR_LAYOUT)."""
+        B = self.batch; out = np.zeros((B, _lib.SENSORS)); q, v, v_prev = _f64(q, (B, 24)), _f64(v, (B, 24)), _f64(v_prev, (B, 24))   # held until the call returns
+        self._call("sim_read_sensors", float(dt), int(sample), _p(q), _p(v), _p(v_prev), _p(out))
+        return out
+
+    def sim_read_sensors_dev(self, dt, sample, q, v, v_prev, sensors, stream=None):
+        """Device-pointer variant: sensors [B, 46] written; no synchronisation."""
+        self._call("sim_read_sensors_dev", float(dt), int(sample), _p(q), _p(v), _p(v_prev), _p(sensors), stream)
+
+    def state_est_get_params(self):
+        """→ dict of qmb200_state_est_params."""
+        p = _lib.StateEstParams(); self._call("state_est_get_params", C.byref(p))
+        return {n: getattr(p, n) for n, _ in _lib.StateEstParams._fields_}
+
+    def state_est_set_params(self, **params):
+        """Keyword per field of qmb200_state_est_params; unspecified fields keep their value."""
+        p = _lib.StateEstParams(); self._call("state_est_get_params", C.byref(p))
+        names = [n for n, _ in _lib.StateEstParams._fields_]
+        for k, v in params.items():
+            if k not in names:
+                raise ValueError("state_est_set_params: unknown parameter %r (one of %s)" % (k, ", ".join(names)))
+            setattr(p, k, float(v))
+        self._call("state_est_set_params", C.byref(p))
+
+    def state_est_reset(self, base_pos):
+        """(Re)start the base state estimator of every robot at base_pos [B, 3], at rest, P = diag(p0).  Synchronous."""
+        base_pos = _f64(base_pos, (self.batch, 3))   # a copy of a strided view must live until the call returns
+        self._call("state_est_reset", _p(base_pos))
+
+    def state_est_step(self, dt, sensors, contact, rbd_est=None):
+        """One filter call per robot from sensors [B, 46] and the contact mask [B] → (rbd_est [B, 55], status [B]).  rbd_est: what a robot with a
+        non-finite input keeps (default zeros)."""
+        B = self.batch; out = np.zeros((B, RBD)) if rbd_est is None else _f64(rbd_est, (B, RBD)).copy(); st = np.zeros(B, dtype=np.int32)
+        sensors, contact = _f64(sensors, (B, _lib.SENSORS)), _i32(contact, (B,))   # held until the call returns
+        self._call("state_est_step", float(dt), _p(sensors), _p(contact), _p(out), _p(st))
+        return out, st
+
+    def state_est_step_dev(self, dt, sensors, contact, rbd_est, status, stream=None):
+        """Device-pointer variant: rbd_est [B, 55] and status [B] int32 written; no synchronisation."""
+        self._call("state_est_step_dev", float(dt), _p(sensors), _p(contact), _p(rbd_est), _p(status), stream)
+
+    def state_est_get(self):
+        """→ dict(x [B, 18] (layout _lib.STATE_EST_LAYOUT), p_diag [B, 18], samples [B]).  Synchronous."""
+        B = self.batch; x = np.zeros((B, 18)); pd = np.zeros((B, 18)); n = np.zeros(B, dtype=np.int32)
+        self._call("state_est_get", _p(x), _p(pd), _p(n))
+        return dict(x=x, p_diag=pd, samples=n)
+
+    def state_est_stop(self):
+        """Release the estimator state."""
+        self._call("state_est_stop")
+
     # ---------------- utilities ----------------
     def centroidal_state_from_rbd(self, rbd):
         rbd = _f64(rbd); n = rbd.shape[0]; x = np.empty((n, NX))

@@ -4,7 +4,7 @@ Default: 8192 robots, trot at cmd_vel 0.3 m/s, 1 s simulated after a warm-up run
 simulated second, the plant step's device time per call (CUDA events) and its share of the loop, and quality lines (base distance, end-effector
 deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
 
-    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain]
+    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference]]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -22,6 +22,13 @@ degrees and steps of 0/3/6/9 cm rise every 0.3 m on it, every combination equall
 "terrain": fallen robots (height above the ground under the base <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite) and base distance per bin of
 each axis, and the plant step's device time at this batch with and without terrain (CUDA events, the two alternated in one process, from one standing
 state).
+
+--state-estimator closes the loop on the base state estimate (closed_loop.run(state_estimator=True)): the controller reads what the IMU, the encoders
+and the contact flags give, with --sensor-noise reference the IMU noise of qm_gazebo/config/default.yaml.  The timed run and the quality lines are then
+those of the estimating controller.  The JSON line gains "state_est": the device time per call of the sensor reading and the estimator step together at
+this batch (CUDA events, alternated with blocks of plant steps); percentiles over the robots of |z_hat - z| and |v_hat - v| (over the run and at the
+end) and of the xy drift at the end (taken in the warm-up run, which is the timed run's twin); and the quality lines of a ground-truth run of the same
+sweep (one more untimed run in the same process).  Each of these runs starts from a cold MPC and WBC state (Solver.mpc_reset, wbc_set_input_last).
 """
 import argparse
 import json
@@ -109,6 +116,60 @@ def est_step_times(solver, xy_yaw, reps=7, calls=20):
             "spread": [float(min(times["estimator"])), float(max(times["estimator"]))]}
 
 
+def state_est_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per sensor reading + estimator step and per 1 ms plant step of the whole batch, alternated `reps` times in blocks of `calls` from one
+    standing state (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev); v_prev = v.clone()
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev); rbd_est = torch.zeros_like(rbd)
+    sensors = torch.zeros((B, 46), dtype=torch.float64, device=dev); contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    solver.state_est_reset(q0[:, 0:3])
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+    times = {"estimator": [], "plant": []}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode in ("estimator", "plant"):
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for k in range(calls):
+                    if mode == "estimator":
+                        solver.sim_read_sensors_dev(1e-3, k, q, v, v_prev, sensors, s.cuda_stream)
+                        solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, st, s.cuda_stream)
+                    else:
+                        solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.state_est_stop()
+    return {"label": "device time per sensor reading + estimator step and per 1 ms plant step of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            "ms_per_call": float(np.median(times["estimator"])), "ms_per_plant_step": float(np.median(times["plant"])),
+            "spread": [float(min(times["estimator"])), float(max(times["estimator"]))]}
+
+
+def watch_state_est(solver):
+    """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z| and |v_hat - v| on the device (no
+    synchronisation) → (box, unwrap); box["max"] [B, 2], box["last"] [B, 2] after the run."""
+    import torch
+    orig_sim, orig_est = solver.sim_step_dev, solver.state_est_step_dev; box = {}
+
+    def sim(duration, effort, q, v, rbd, contact, status, stream=None, wrench=None):
+        box["rbd"] = rbd; orig_sim(duration, effort, q, v, rbd, contact, status, stream, wrench=wrench)
+
+    def est(dt, sensors, contact, rbd_est, status, stream=None):
+        orig_est(dt, sensors, contact, rbd_est, status, stream)
+        with torch.cuda.stream(torch.cuda.ExternalStream(stream)):
+            e = torch.stack([(rbd_est[:, 5] - box["rbd"][:, 5]).abs(), (rbd_est[:, 27:30] - box["rbd"][:, 27:30]).norm(dim=1)], 1)
+            box["last"] = e; box["max"] = e if "max" not in box else torch.maximum(box["max"], e)
+
+    def unwrap():
+        del solver.sim_step_dev, solver.state_est_step_dev
+    solver.sim_step_dev, solver.state_est_step_dev = sim, est
+    return box, unwrap
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
@@ -117,9 +178,15 @@ def main():
     ap.add_argument("--model-payload", choices=["plant", "estimate"],
                     help="plant: tell the controller the plant's payload (its model payload, Solver.set_model_payload); estimate: run the online payload estimator")
     ap.add_argument("--terrain", action="store_true", help="per-robot sweep of ramp angle and step rise under the feet")
+    ap.add_argument("--state-estimator", action="store_true", help="the controller reads the base state estimate from the IMU, encoders and contact flags")
+    ap.add_argument("--sensor-noise", choices=["reference"], help="with --state-estimator: the IMU noise of qm_gazebo/config/default.yaml")
     args = ap.parse_args()
     if args.vary and args.terrain:
         ap.error("--vary and --terrain are separate sweeps")
+    if args.sensor_noise and not args.state_estimator:
+        ap.error("--sensor-noise needs --state-estimator")
+    if args.state_estimator and args.terrain:
+        ap.error("--state-estimator assumes the plane: it cannot be combined with --terrain")
     import torch
     import qm_control_b200 as q
     from qm_control_b200 import closed_loop
@@ -143,7 +210,19 @@ def main():
         ter = dict(tiles=tiles, cell=T.CELL, tile=idx["ramp_deg"] * 4 + idx["step_rise_m"], origin=T.centred_origin(xy[:, :2]))
         kw = dict(terrain=ter)
     told = {"plant": dict(model_payload="plant"), "estimate": dict(payload_estimator=True), None: {}}[args.model_payload]
-    closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told)   # warm-up run of the same length
+    se = dict(state_estimator=True, sensor_noise=args.sensor_noise) if args.state_estimator else {}
+    def fresh():
+        """with --state-estimator every run starts from a cold MPC and WBC state: a run whose robots fell leaves warm starts the next run must not inherit"""
+        if args.state_estimator:
+            solver.mpc_reset(); solver.wbc_set_input_last(None)
+    if args.state_estimator:
+        box, unwrap = watch_state_est(solver)
+    try:
+        fresh()
+        warm = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told, **se)   # warm-up run of the same length
+    finally:
+        if args.state_estimator:
+            unwrap()
     pairs = []
 
     def sim_timer(start):
@@ -151,8 +230,8 @@ def main():
             pairs.append([torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)]); pairs[-1][0].record()
         else:
             pairs[-1][1].record()
-    torch.cuda.synchronize(dev); t0 = time.perf_counter()
-    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer, **kw, **told)
+    fresh(); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+    r = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, sim_timer=sim_timer, **kw, **told, **se)
     torch.cuda.synchronize(dev); wall = time.perf_counter() - t0
     sim_ms = float(np.sum([a.elapsed_time(b) for a, b in pairs])); per_call = sim_ms / len(pairs)
     pct = lambda a: {"p50": float(np.percentile(a, 50)), "p95": float(np.percentile(a, 95)), "max": float(np.max(a))}
@@ -173,6 +252,9 @@ def main():
                  **({"base_distance_m": pct(dist[idx[axis] == i])} if args.terrain else
                     {"ee_max_pos_dev_mm": pct(dpos[idx[axis] == i]), "ee_max_ori_dev_deg_p50": float(np.percentile(dang[idx[axis] == i], 50))})}
                 for i, val in enumerate(bins[axis])]
+    def upright(r):
+        base = r["base"]
+        return np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3)
     dist, dpos, dang = quality(r)
     name, limit = card()
     extra = {}
@@ -193,6 +275,17 @@ def main():
                             "bins": {axis: vary_bins(r, axis) for axis in bins}, "plant_step": plant_step_times(solver, ter, xy)}
     if args.model_payload == "estimate":
         extra["payload_est"] = {**est_step_times(solver, xy), "gpu": name, "power_limit": limit}
+    if args.state_estimator:
+        mx, last = box["max"].cpu().numpy(), box["last"].cpu().numpy()
+        drift = np.linalg.norm(warm["base_est"][-1, :, 0:2] - warm["base"][-1, :, 0:2], axis=1)
+        fresh(); truth = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told)
+        t_dist, t_dpos, t_dang = quality(truth)
+        extra["state_est"] = {**state_est_times(solver, xy), "gpu": name, "power_limit": limit, "sensor_noise": args.sensor_noise or "none",
+                              "errors": {"label": "over the robots, from the warm-up run (the timed run's twin)", "z_abs_m_over_run": pct(mx[:, 0]), "z_abs_m_at_end": pct(last[:, 0]),
+                                         "v_abs_m_s_over_run": pct(mx[:, 1]), "v_abs_m_s_at_end": pct(last[:, 1]), "xy_drift_m_at_end": pct(drift)},
+                              "fallen": int(np.sum(~upright(r))), "fallen_warmup": int(np.sum(~upright(warm))), "ground_truth": {"label": "the same sweep, controller reading the plant's true state", "fallen": int(np.sum(~upright(truth))),
+                                                                                    "base_distance_m": pct(t_dist), "ee_max_pos_dev_mm": pct(t_dpos), "ee_max_ori_dev_deg": pct(t_dang),
+                                                                                    "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(truth["status"], axis=0)))}}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
@@ -201,7 +294,8 @@ def main():
                                   "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(r["status"], axis=0))),
                                   "min_base_height_m": float(np.min(r["base"][:, :, 2])), "max_abs_roll_pitch_rad": float(np.max(np.abs(r["base"][:, :, 4:6])))},
                       "config": {"workload": "closed loop: %s, cmd_vel %.2f m/s, MPC 100 Hz / WBC 500 Hz / plant 1 kHz (4 substeps), 9 ms command delay" % (args.gait, args.vx),
-                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length", **({"model_payload": args.model_payload} if args.model_payload else {})}, **extra}))
+                                 "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length", **({"model_payload": args.model_payload} if args.model_payload else {}),
+                                 **({"state_estimator": True, "sensor_noise": args.sensor_noise or "none"} if args.state_estimator else {})}, **extra}))
 
 
 if __name__ == "__main__":
