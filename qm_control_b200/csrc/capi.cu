@@ -218,6 +218,7 @@ int64_t qmb200_debug_model_blob(const qmb200_config* cfg, void* out, int64_t cap
 
 // ------------------------------------------------------------------ model payload
 static_assert(SRBD_DBL == QMB200_SRBD, "per-robot SRBD block of include/qmb200.h");
+static_assert(RBD_EE_QUAT + 4 == QMB200_RBD, "rbd layout of include/qmb200.h");
 }  // extern "C"
 namespace {
 // payload rows [n][8] as qmb200_sim_set_robot_params and qmb200_set_model_payload accept them: finite, masses >= 0; "" when valid

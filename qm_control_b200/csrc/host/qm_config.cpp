@@ -148,18 +148,25 @@ Rot from_rpy(const double* rpy) {   // URDF fixed-axis roll-pitch-yaw = Rz(y) Ry
   return Rot{{cy * cp, cy * sp * sr - sy * cr, cy * sp * cr + sy * sr, sy * cp, sy * sp * sr + cy * cr, sy * sp * cr - cy * sr, -sp, cp * sr, cp * cr}};
 }
 Rot identity() { return Rot{{1, 0, 0, 0, 1, 0, 0, 0, 1}}; }
+Rot as_rot(const double* m) { Rot r; std::memcpy(r.m, m, sizeof(r.m)); return r; }
 Rot about_axis(int ax, double q) { const double s = sin(q), c = cos(q); if (ax == 0) return Rot{{1, 0, 0, 0, c, -s, 0, s, c}}; if (ax == 1) return Rot{{c, 0, s, 0, 1, 0, -s, 0, c}}; return Rot{{c, -s, 0, s, c, 0, 0, 0, 1}}; }
 
 int axis_index(const double* a, const std::string& name) {
   if (a[0] == 1 && a[1] == 0 && a[2] == 0) return 0; if (a[0] == 0 && a[1] == 1 && a[2] == 0) return 1; if (a[0] == 0 && a[1] == 0 && a[2] == 1) return 2;
   throw std::runtime_error("URDF: joint " + name + " has an axis other than +x/+y/+z (unsupported)");
 }
-// world rotation / origin of every body at q [24]
-void host_fk(const DevModel& d, const double* q, Rot* Rw, double (*pw)[3]) {
-  const double rz[3] = {q[5], q[4], q[3]}; Rw[0] = from_rpy(rz); for (int i = 0; i < 3; ++i) pw[0][i] = q[i];   // Rz(q3) Ry(q4) Rx(q5)
-  for (int j = 0; j < NJ; ++j) { const int pb = d.parent[j]; Rot Rl; std::memcpy(Rl.m, d.Rj[j], sizeof(Rl.m)); Rw[j + 1] = mul(mul(Rw[pb], Rl), about_axis(d.axis[j], q[6 + j])); apply(Rw[pb], d.pj[j], pw[j + 1]); for (int i = 0; i < 3; ++i) pw[j + 1][i] += pw[pb][i]; }
-}
 }  // namespace
+
+void host_fk(const DevModel& d, const double* q, double Rw[NB][9], double pw[NB][3]) {
+  const double rz[3] = {q[5], q[4], q[3]}; std::memcpy(Rw[0], from_rpy(rz).m, sizeof(Rw[0])); for (int i = 0; i < 3; ++i) pw[0][i] = q[i];   // Rz(q3) Ry(q4) Rx(q5)
+  for (int j = 0; j < NJ; ++j) {
+    const int pb = d.parent[j]; const Rot Rp = as_rot(Rw[pb]);
+    std::memcpy(Rw[j + 1], mul(mul(Rp, as_rot(d.Rj[j])), about_axis(d.axis[j], q[6 + j])).m, sizeof(Rw[0])); apply(Rp, d.pj[j], pw[j + 1]); for (int i = 0; i < 3; ++i) pw[j + 1][i] += pw[pb][i];
+  }
+}
+void host_feet(const DevModel& d, const double Rw[NB][9], const double pw[NB][3], double pf[4][3]) {
+  for (int f = 0; f < 4; ++f) { const int body = d.foot_body[f]; apply(as_rot(Rw[body]), d.foot_p[f], pf[f]); for (int i = 0; i < 3; ++i) pf[f][i] += pw[body][i]; }
+}
 
 void srbd_constants(const DevModel& d, const double* payload, double* out) { srbd_payload_fold(d, payload, out); }
 
@@ -217,11 +224,11 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
   // --- CentroidalModelInfo, SRBD (createCentroidalModelInfo [upstream]) ---
   { auto djs = reference.matrix("defaultJointState", NJ, 1); for (int i = 0; i < NJ; ++i) hm.default_joint_state[i] = djs[i]; }
   // the nominal SRBD block: the bodies folded at defaultJointState with the base at the origin, level (srbd_payload_fold adds payloads to it)
-  Rot Rw[NB]; double pw[NB][3];
+  double Rw[NB][9], pw[NB][3];
   {
     double qn[NQ] = {0}; for (int j = 0; j < NJ; ++j) qn[6 + j] = hm.default_joint_state[j]; host_fk(d, qn, Rw, pw);
-    SrbdLump whole; for (int b = 0; b < NB; ++b) { double c[3]; apply(Rw[b], d.com[b], c); for (int i = 0; i < 3; ++i) c[i] += pw[b][i]; Rot I0; std::memcpy(I0.m, d.Ib[b], sizeof(I0.m)); Rot Iw = mul(mul(Rw[b], I0), transpose(Rw[b])); lump_add(whole, d.mass[b], c, Iw.m); }
-    std::memcpy(d.ee_body_R0, Rw[d.ee_body].m, sizeof(d.ee_body_R0)); std::memcpy(d.ee_body_p0, pw[d.ee_body], sizeof(d.ee_body_p0));
+    SrbdLump whole; for (int b = 0; b < NB; ++b) { const Rot R = as_rot(Rw[b]); double c[3]; apply(R, d.com[b], c); for (int i = 0; i < 3; ++i) c[i] += pw[b][i]; Rot Iw = mul(mul(R, as_rot(d.Ib[b])), transpose(R)); lump_add(whole, d.mass[b], c, Iw.m); }
+    std::memcpy(d.ee_body_R0, Rw[d.ee_body], sizeof(d.ee_body_R0)); std::memcpy(d.ee_body_p0, pw[d.ee_body], sizeof(d.ee_body_p0));
     std::memcpy(d.I_nom, whole.I, sizeof(whole.I)); for (int i = 0; i < 3; ++i) d.c_nom[i] = -whole.c[i]; inv3(d.I_nom, d.I_nom_inv);
   }
 
@@ -242,9 +249,9 @@ HostModel build_host_model(const std::string& task_file, const std::string& urdf
   { auto init = task.matrix("initialState", NX, 1); for (int i = 0; i < NX; ++i) hm.initial_state[i] = init[i]; }
   { auto Q = task.matrix("Q", NX, NX); std::memcpy(d.Q, Q.data(), sizeof(d.Q)); auto Rt = task.matrix("R", NU, NU); std::memcpy(d.R, Rt.data(), sizeof(d.R));
     // initializeInputCostWeight (QMInterface.cpp:274-299): R[12:24,12:24] = J^T Rtask[12:24,12:24] J, J = d(foot pos)/d(leg joints) at initialState
-    host_fk(d, hm.initial_state + 6, Rw, pw); double J[12][12] = {{0}};
-    for (int f = 0; f < 4; ++f) { const int body = d.foot_body[f]; double pf[3]; apply(Rw[body], d.foot_p[f], pf); for (int i = 0; i < 3; ++i) pf[i] += pw[body][i];
-      for (int k = 0; k < 3; ++k) { const int j = d.foot_leg[f] + k; const int ax = d.axis[j]; const double a[3] = {Rw[j + 1].m[ax], Rw[j + 1].m[3 + ax], Rw[j + 1].m[6 + ax]}; const double r[3] = {pf[0] - pw[j + 1][0], pf[1] - pw[j + 1][1], pf[2] - pw[j + 1][2]};
+    host_fk(d, hm.initial_state + 6, Rw, pw); double feet[4][3]; host_feet(d, Rw, pw, feet); double J[12][12] = {{0}};
+    for (int f = 0; f < 4; ++f) { const double* pf = feet[f];
+      for (int k = 0; k < 3; ++k) { const int j = d.foot_leg[f] + k; const int ax = d.axis[j]; const double a[3] = {Rw[j + 1][ax], Rw[j + 1][3 + ax], Rw[j + 1][6 + ax]}; const double r[3] = {pf[0] - pw[j + 1][0], pf[1] - pw[j + 1][1], pf[2] - pw[j + 1][2]};
         J[3 * f + 0][j] = a[1] * r[2] - a[2] * r[1]; J[3 * f + 1][j] = a[2] * r[0] - a[0] * r[2]; J[3 * f + 2][j] = a[0] * r[1] - a[1] * r[0]; } }
     for (int a = 0; a < 12; ++a) for (int b = 0; b < 12; ++b) { double s = 0; for (int i = 0; i < 12; ++i) for (int k = 0; k < 12; ++k) s += J[i][a] * Rt[(size_t)(12 + i) * NU + 12 + k] * J[k][b]; d.R[(12 + a) * NU + 12 + b] = s; }
     // compact block form used by the kernels; anything outside the blocks is refused (the structured projection relies on it)

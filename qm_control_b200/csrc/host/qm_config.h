@@ -52,6 +52,11 @@ struct HostModel {
 // from task.info (Q, R with the leg-velocity block mapped through the foot Jacobians, QMInterface.cpp:274-299).
 HostModel build_host_model(const std::string& task_file, const std::string& urdf_file, const std::string& reference_file, const std::string& gains_file);
 
+// Forward kinematics of the model on the host at q[24] = [p, zyx, joints]: world rotation Rw (row-major) and origin pw of every body.  build_host_model derives
+// the model's constants from it.  host_feet: the world origins of the four foot frames (contact order) from its output.
+void host_fk(const DevModel& d, const double* q, double Rw[NB][9], double pw[NB][3]);
+void host_feet(const DevModel& d, const double Rw[NB][9], const double pw[NB][3], double pf[4][3]);
+
 // The SRBD constants (SrbdConst, padded to SRBD_DBL doubles) of the model at defaultJointState, as createCentroidalModelInfo folds the bodies: the composite
 // mass, inertia about the composite COM and the base-to-COM offset.  `payload` (include/qmb200.h layout [m_ee, o_ee(3), m_base, o_base(3)], or null) adds
 // two point masses without rotational inertia, at o_ee in the end-effector frame and at o_base in the base frame - what a URDF with an extra fixed link carrying

@@ -44,9 +44,8 @@ __device__ __forceinline__ void quat_to_rot(double w, double x, double y, double
 }  // namespace
 
 // -----------------------------------------------------------------------------------------------------------------
-// Observation: rbd[55] → centroidal state (SRBD mapping, the same arithmetic as qmb200_centroidal_state_from_rbd:
-// CentroidalModelRbdConversions::computeCentroidalStateFromRbdModel [upstream, recalled]) with the controller's yaw unwrap.  srbd: per-robot SRBD constants
-// [B][SRBD_DBL] of a model payload, or NULL for the model's.
+// Observation: rbd[55] → centroidal state (centroidal_from_rbd, as qmb200_centroidal_state_from_rbd) with the controller's yaw unwrap.  srbd: per-robot SRBD
+// constants [B][SRBD_DBL] of a model payload, or NULL for the model's.
 __global__ void __launch_bounds__(OBS_ROBOTS) ctrl_observation_kernel(const DevModel* __restrict__ mdl, int B, const double* __restrict__ rbd, const double* __restrict__ period,
                                                                        double* __restrict__ t_obs, double* __restrict__ x_obs, const double* __restrict__ srbd) {
   __shared__ double s_rbd[OBS_ROBOTS * 55];   // leading dimension 55 (odd)
@@ -55,18 +54,8 @@ __global__ void __launch_bounds__(OBS_ROBOTS) ctrl_observation_kernel(const DevM
   tile_load<55, 55>(s_rbd, rbd + (size_t)b0 * 55, rows);
   __syncthreads();
   if (r < rows) {
-    const double* s = s_rbd + r * 55; double* o = s_x + r * 31;
-    double R[9]; rot_zyx(s[0], s[1], s[2], R);
-    const double w[3] = {s[NQ], s[NQ + 1], s[NQ + 2]};
-    const SrbdConst* sc = srbd_of(mdl, srbd, b0 + r);
-    double c[3]; matvec3(R, sc->c_nom, c);
-    double cw[3]; cross3(c, w, cw);                                     // h_lin/m = v_lin + (R c_nom) x w
-    double Rtw[3], IRtw[3], L[3]; matTvec3(R, w, Rtw); matvec3(sc->I_nom, Rtw, IRtw); matvec3(R, IRtw, L);   // h_ang = R I R^T w
-    const double inv_m = 1.0 / sc->m;
-#pragma unroll
-    for (int i = 0; i < 3; ++i) { o[i] = s[NQ + 3 + i] + cw[i]; o[3 + i] = L[i] * inv_m; o[6 + i] = s[3 + i]; o[9 + i] = s[i]; }
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) o[12 + j] = s[6 + j];
+    double* o = s_x + r * 31;
+    centroidal_from_rbd(*srbd_of(mdl, srbd, b0 + r), s_rbd + r * 55, o);
     const double yaw_last = x_obs[(size_t)(b0 + r) * NX + 9];           // currentObservation_.state(9) of the previous update
     o[9] = yaw_last + shortest_angular_distance(yaw_last, o[9]);
     t_obs[b0 + r] += period[b0 + r];

@@ -24,6 +24,9 @@ constexpr int NX = 30;   // centroidal state
 constexpr int NU = 30;   // input: 12 contact forces (LF,RF,LH,RH) + 18 joint velocities
 constexpr int NDEC = 36; // WBC decision vector [vdot(24); F(12)]
 constexpr unsigned FULL = 0xffffffffu;
+// The measured state rbd[55] (include/qmb200.h): euler ZYX, base position, joint positions, world angular velocity, base linear velocity, joint velocities,
+// end-effector position and orientation quaternion xyzw
+constexpr int RBD_ZYX = 0, RBD_POS = 3, RBD_JPOS = 6, RBD_W = 24, RBD_V = 27, RBD_JVEL = 30, RBD_EE_POS = 48, RBD_EE_QUAT = 51;
 
 // Model + settings constants, replicated per GPU (read-only, L1/L2 resident).
 struct DevModel {
@@ -153,7 +156,8 @@ QMB_HD void matmul3_nt(const double* A, const double* B, double* C) {
 #pragma unroll
     for (int j = 0; j < 3; ++j) C[3 * i + j] = A[3 * i] * B[3 * j] + A[3 * i + 1] * B[3 * j + 1] + A[3 * i + 2] * B[3 * j + 2];
 }
-// R = Rz(z) Ry(y) Rx(x)   (ocs2 getRotationMatrixFromZyxEulerAngles)
+// R = Rz(z) Ry(y) Rx(x)   (ocs2 getRotationMatrixFromZyxEulerAngles).  The formula of rot_zyx_sc, written out: computed through rot_zyx_sc, nvcc
+// contracts the WBC's desired-side rotation into different FMAs and its commands move in the last bits.
 QMB_HD void rot_zyx(double z, double y, double x, double* R) {
   double sz, cz, sy, cy, sx, cx; sincos(z, &sz, &cz); sincos(y, &sy, &cy); sincos(x, &sx, &cx);
   R[0] = cz * cy; R[1] = cz * sy * sx - sz * cx; R[2] = cz * sy * cx + sz * sx;
@@ -235,6 +239,22 @@ QMB_HD void lump_add(SrbdLump& a, double m, const double* c, const double* I) {
   double I1[9], I2[9]; lump_shift(a.m, a.c, a.I, cn, I1); lump_shift(m, c, I, cn, I2);
   for (int i = 0; i < 9; ++i) a.I[i] = I1[i] + I2[i];
   a.m = mt; for (int i = 0; i < 3; ++i) a.c[i] = cn[i];
+}
+
+// rbd row s[55] → centroidal state x[30] = [h_lin / m, h_ang / m, base position, euler ZYX, joints] by the SRBD mapping of robot constants sc
+// (CentroidalModelRbdConversions::computeCentroidalStateFromRbdModel [upstream, recalled]): h_lin / m = v_lin + (R c_nom) x w, h_ang = R I_nom R^T w.
+// The yaw is copied as measured; the controller's observation unwraps it.
+QMB_HD void centroidal_from_rbd(const SrbdConst& sc, const double* s, double* x) {
+  double R[9]; rot_zyx(s[RBD_ZYX], s[RBD_ZYX + 1], s[RBD_ZYX + 2], R);
+  const double w[3] = {s[RBD_W], s[RBD_W + 1], s[RBD_W + 2]};
+  double c[3]; matvec3(R, sc.c_nom, c);
+  double cw[3]; cross3(c, w, cw);
+  double Rtw[3], IRtw[3], L[3]; matTvec3(R, w, Rtw); matvec3(sc.I_nom, Rtw, IRtw); matvec3(R, IRtw, L);
+  const double inv_m = 1.0 / sc.m;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) { x[i] = s[RBD_V + i] + cw[i]; x[3 + i] = L[i] * inv_m; x[6 + i] = s[RBD_POS + i]; x[9 + i] = s[RBD_ZYX + i]; }
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) x[12 + j] = s[RBD_JPOS + j];
 }
 
 // The SRBD constants of one robot with model payload pl = [m_ee, o_ee(3), m_base, o_base(3)] (or NULL) → out[SRBD_DBL]: DevModel's nominal block (the fold of the

@@ -24,14 +24,12 @@ __device__ __forceinline__ void payload_add(const DevModel* __restrict__ mdl, Rb
   double c[3]; matvec3(R, ob, c); c[0] += po[0]; c[1] += po[1]; c[2] += po[2];   // point mass position (world)
   const double cc = dot3(c, c);
   double I[10] = {m, m * c[0], m * c[1], m * c[2], m * (cc - c[0] * c[0]), -m * c[0] * c[1], -m * c[0] * c[2], m * (cc - c[1] * c[1]), -m * c[1] * c[2], m * (cc - c[2] * c[2])};
-  double acc[6]; for (int i = 0; i < 6; ++i) acc[i] = ws->A[body][i]; if (gravity) acc[5] += 9.81;
-  double f1[6], mom[6]; inertia_apply(I, acc, f1); inertia_apply(I, ws->V[body], mom);
-  const double* wv = ws->V[body]; const double* vv = ws->V[body] + 3;
-  double t1[3], t2[3]; cross3(wv, mom, t1); cross3_add(vv, mom + 3, t1); cross3(wv, mom + 3, t2);   // V x* [n; f] = [w x n + v x f; w x f]
   double* Ic = ws->Ic[body]; double* F = ws->F[body];
 #pragma unroll
   for (int i = 0; i < 10; ++i) Ic[i] += I[i];
-  F[0] += f1[0] + t1[0]; F[1] += f1[1] + t1[1]; F[2] += f1[2] + t1[2]; F[3] += f1[3] + t2[0]; F[4] += f1[4] + t2[1]; F[5] += f1[5] + t2[2];
+  double f[6]; rnea_force(I, ws->V[body], ws->A[body], gravity, f);
+#pragma unroll
+  for (int i = 0; i < 6; ++i) F[i] += f[i];
 }
 
 // both steps for the frame's payload pl

@@ -10,7 +10,7 @@
 //
 // One warp owns one robot (lanes over bodies / columns, as in rbd.cuh and sim_kernel.cu).  Per call, from the measurement rbd [55] and the effort held over the
 // interval of length dt that ended at it:
-//   (q, v)      rbd → q, and v with euler rates = T(zyx)^-1 w_world, as the WBC's measured pass
+//   (q, v)      rbd → q, and v with euler rates = T(zyx)^-1 w_world (rbd_read, as the WBC's measured pass)
 //   qdd         (v - v_prev) / dt, with the previous sample from the estimator state; M, nle, the end-effector twist and acceleration at the midpoint
 //               state ((q + q_prev) / 2 with the euler difference unwrapped, (v + v_prev) / 2): rbd_kinematics<true> → rbd_inertias → rbd_accumulate →
 //               rbd_mass_matrix_nle, then the end-effector body's acceleration A + sum_c S_c qdd_c
@@ -58,10 +58,7 @@ __global__ void __launch_bounds__(32 * EST_WARPS) payload_est_step_kernel(const 
   const double* rb = rbd + (size_t)b * QMB200_RBD; double* st = state + (size_t)b * EST_DBL;
 
   // ---- the sample: q, v (euler rates) as the WBC's measured pass reads them ----
-  if (lane < 3) { w->q[lane] = rb[3 + lane]; w->q[3 + lane] = rb[lane]; w->v[lane] = rb[NQ + 3 + lane]; }
-  if (lane < NJ) { w->q[6 + lane] = rb[6 + lane]; w->v[6 + lane] = rb[NQ + 6 + lane]; }
-  __syncwarp();
-  if (lane == 0) { double T[9], Ti[9]; euler_rate_map(w->q[3], w->q[4], T); inv3(T, Ti); const double om[3] = {rb[NQ], rb[NQ + 1], rb[NQ + 2]}; matvec3(Ti, om, w->v + 3); }
+  rbd_read(rb, w->q, w->v, nullptr, lane);
   __syncwarp();
   double qk = 0.0, vk = 0.0, tau = 0.0;
   if (lane < NQ) { qk = w->q[lane]; vk = w->v[lane]; }
@@ -94,19 +91,14 @@ __global__ void __launch_bounds__(32 * EST_WARPS) payload_est_step_kernel(const 
     w->y[lane - a0] = acc;
   }
   if (lane == 0) {   // end-effector frame kinematics at the midpoint: pose, twist, acceleration with qdd
-    const int eb = mdl->ee_body; double Rb[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) Rb[i] = ws->R[eb][i];
-    double pe[3]; matvec3(Rb, mdl->ee_p, pe); pe[0] += ws->p[eb][0]; pe[1] += ws->p[eb][1]; pe[2] += ws->p[eb][2];
-    double Re[9]; matmul3(Rb, mdl->ee_R, Re);
+    const int eb = mdl->ee_body;
+    double pe[3], Re[9]; ee_pose(mdl, ws, pe, Re);
     double Af[6]; for (int i = 0; i < 6; ++i) Af[i] = ws->A[eb][i];
     for (int c = 0; c <= 6 + je; ++c) {
       if (c >= 6 && c < a0) continue;
       const double qd = w->qdd[c]; for (int i = 0; i < 6; ++i) Af[i] += ws->S[c][i] * qd;
     }
-    const double* V = ws->V[eb]; double vel[3], acc[3];
-    cross3(V, pe, vel); vel[0] += V[3]; vel[1] += V[4]; vel[2] += V[5];
-    cross3(Af, pe, acc); acc[0] += Af[3]; acc[1] += Af[4]; acc[2] += Af[5]; cross3_add(V, vel, acc);
+    const double* V = ws->V[eb]; double vel[3], acc[3]; point_vel_acc(V, Af, pe, vel, acc);
     acc[2] += 9.81;                                           // a - g with g = -9.81 z (rbd_inertias' gravity)
     matTvec3(Re, V, w->kin); matTvec3(Re, Af, w->kin + 3); matTvec3(Re, acc, w->kin + 6);
     for (int i = 0; i < 9; ++i) w->Re[i] = Re[i];
@@ -119,7 +111,7 @@ __global__ void __launch_bounds__(32 * EST_WARPS) payload_est_step_kernel(const 
 
   // ---- regressor rows: Phi[r] = -(J_v^T f + J_w^T n) per unit parameter, with the column's end-effector Jacobian in the frame's axes ----
   if (lane >= a0 && lane <= 6 + je) {
-    const double* S = ws->S[lane]; double jv[3]; cross3(S, w->pe, jv); jv[0] += S[3]; jv[1] += S[4]; jv[2] += S[5];
+    const double* S = ws->S[lane]; double jv[3]; point_vel(S, w->pe, jv);
     double wf[3], wn[3]; matTvec3(w->Re, jv, wf); matTvec3(w->Re, S, wn);
     const double* om = w->kin; const double* al = w->kin + 3; const double* a = w->kin + 6;
     double* phi = w->Phi[lane - a0];

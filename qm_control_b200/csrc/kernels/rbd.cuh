@@ -35,6 +35,27 @@ __device__ __forceinline__ void inertia_apply(const double* I, const double* mv,
   out[5] = m * v[2] + (w[0] * h[1] - w[1] * h[0]);
 }
 __device__ __forceinline__ double dot6(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2] + a[3] * b[3] + a[4] * b[4] + a[5] * b[5]; }
+// RNEA force of the inertia I moving with V under the bias acceleration A: F = I (A + g) + V x* I V, with g = +9.81 z (the base acceleration trick) or 0
+__device__ __forceinline__ void rnea_force(const double* I, const double* V, const double* A, bool gravity, double* F) {
+  double acc[6]; for (int i = 0; i < 6; ++i) acc[i] = A[i]; if (gravity) acc[5] += 9.81;
+  double f1[6], mom[6]; inertia_apply(I, acc, f1); inertia_apply(I, V, mom);
+  const double* w = V; const double* vv = V + 3;
+  // V x* [n; f] = [w x n + v x f; w x f]
+  double t1[3], t2[3]; cross3(w, mom, t1); cross3_add(vv, mom + 3, t1); cross3(w, mom + 3, t2);
+  F[0] = f1[0] + t1[0]; F[1] = f1[1] + t1[1]; F[2] = f1[2] + t1[2]; F[3] = f1[3] + t2[0]; F[4] = f1[4] + t2[1]; F[5] = f1[5] + t2[2];
+}
+
+// The measured state rbd[55] as the rigid-body passes take it: q = [p, zyx, joints], v = [v_lin, zyx rates = T^-1 w_world, joint rates], into shared memory.
+// T (euler_rate_map at zyx) is also stored when the caller keeps it, else pass NULL.  Lane 0 writes v[3..5] last: the caller synchronises the warp after.
+__device__ __forceinline__ void rbd_read(const double* __restrict__ rb, double* q, double* v, double* T, int lane) {
+  if (lane < 3) { q[lane] = rb[RBD_POS + lane]; q[3 + lane] = rb[RBD_ZYX + lane]; v[lane] = rb[RBD_V + lane]; }
+  if (lane < NJ) { q[6 + lane] = rb[RBD_JPOS + lane]; v[6 + lane] = rb[RBD_JVEL + lane]; }
+  __syncwarp();
+  if (lane == 0) {
+    double Tl[9], Ti[9]; double* Tm = T ? T : Tl; euler_rate_map(q[3], q[4], Tm); inv3(Tm, Ti);
+    const double w[3] = {rb[RBD_W], rb[RBD_W + 1], rb[RBD_W + 2]}; matvec3(Ti, w, v + 3);
+  }
+}
 
 // Pass 1: kinematics (+ optional velocities / bias accelerations).  q,v are in shared memory (24 each).
 // Lane L < 19 owns body L.  with_vel: 0 = positions only, 1 = V and A as well.  max_depth limits the tree levels that are updated
@@ -125,14 +146,7 @@ __device__ __forceinline__ void rbd_inertias(const DevModel* __restrict__ mdl, R
     double* I = ws->Ic[b]; I[0] = m; I[1] = m * c[0]; I[2] = m * c[1]; I[3] = m * c[2];
     I[4] = Iw[0] + m * (cc - c[0] * c[0]); I[5] = Iw[1] - m * c[0] * c[1]; I[6] = Iw[2] - m * c[0] * c[2];
     I[7] = Iw[4] + m * (cc - c[1] * c[1]); I[8] = Iw[5] - m * c[1] * c[2]; I[9] = Iw[8] + m * (cc - c[2] * c[2]);
-    if (with_force) {
-      double acc[6]; for (int i = 0; i < 6; ++i) acc[i] = ws->A[b][i]; if (with_force == 1) acc[5] += 9.81;
-      double f1[6], mom[6]; inertia_apply(I, acc, f1); inertia_apply(I, ws->V[b], mom);
-      const double* w = ws->V[b]; const double* vv = ws->V[b] + 3;
-      // V x* [n; f] = [w x n + v x f; w x f]
-      double t1[3], t2[3]; cross3(w, mom, t1); cross3_add(vv, mom + 3, t1); cross3(w, mom + 3, t2);
-      double* F = ws->F[b]; F[0] = f1[0] + t1[0]; F[1] = f1[1] + t1[1]; F[2] = f1[2] + t1[2]; F[3] = f1[3] + t2[0]; F[4] = f1[4] + t2[1]; F[5] = f1[5] + t2[2];
-    }
+    if (with_force) rnea_force(I, ws->V[b], ws->A[b], with_force == 1, ws->F[b]);
   }
   __syncwarp();
 }
@@ -181,20 +195,32 @@ __device__ __forceinline__ void rbd_mass_matrix_nle(const DevModel* __restrict__
   __syncwarp();
 }
 
+// velocity of the point pw (world) fixed on a body moving with the spatial velocity V = [w; vO]: w x pw + vO
+__device__ __forceinline__ void point_vel(const double* V, const double* pw, double* vel) { cross3(V, pw, vel); vel[0] += V[3]; vel[1] += V[4]; vel[2] += V[5]; }
+
 // Linear velocity Jacobian row block (3 x 24, LOCAL_WORLD_ALIGNED) of a point pw fixed on `body` whose chain
 // covers joints [chain_first, chain_last]; lanes over columns.
 __device__ __forceinline__ void point_jacobian(const RbdWs* ws, const double* pw, int chain_first, int chain_last, double* J, int ldj, int lane) {
   if (lane < NQ) {
     const int c = lane; double col[3] = {0, 0, 0};
-    if (c < 6 || (c - 6 >= chain_first && c - 6 <= chain_last)) { const double* S = ws->S[c]; cross3(S, pw, col); col[0] += S[3]; col[1] += S[4]; col[2] += S[5]; }
+    if (c < 6 || (c - 6 >= chain_first && c - 6 <= chain_last)) point_vel(ws->S[c], pw, col);
     J[c] = col[0]; J[ldj + c] = col[1]; J[2 * ldj + c] = col[2];
   }
 }
-// classical velocity / bias acceleration (Jdot*v) of a point fixed on `body`
-__device__ __forceinline__ void point_vel_acc(const RbdWs* ws, int body, const double* pw, double* vel, double* acc) {
-  const double* V = ws->V[body]; const double* A = ws->A[body];
-  cross3(V, pw, vel); vel[0] += V[3]; vel[1] += V[4]; vel[2] += V[5];
-  cross3(A, pw, acc); acc[0] += A[3]; acc[1] += A[4]; acc[2] += A[5]; cross3_add(V, vel, acc);
+// classical velocity / bias acceleration (Jdot*v) of a point fixed on a body moving with V, A
+__device__ __forceinline__ void point_vel_acc(const double* V, const double* A, const double* pw, double* vel, double* acc) {
+  point_vel(V, pw, vel); point_vel(A, pw, acc); cross3_add(V, vel, acc);
+}
+
+// world position of the point pl (body axes) fixed on `body`
+__device__ __forceinline__ void body_point(const RbdWs* ws, int body, const double* pl, double* pw) {
+  matvec3(ws->R[body], pl, pw); pw[0] += ws->p[body][0]; pw[1] += ws->p[body][1]; pw[2] += ws->p[body][2];
+}
+// origin of foot frame f (world)
+__device__ __forceinline__ void foot_point(const DevModel* __restrict__ mdl, const RbdWs* ws, int f, double* pw) { body_point(ws, mdl->foot_body[f], mdl->foot_p[f], pw); }
+// end-effector frame: origin pe and, unless Re is NULL, rotation Re (world)
+__device__ __forceinline__ void ee_pose(const DevModel* __restrict__ mdl, const RbdWs* ws, double* pe, double* Re) {
+  const int eb = mdl->ee_body; body_point(ws, eb, mdl->ee_p, pe); if (Re) matmul3(ws->R[eb], mdl->ee_R, Re);
 }
 
 }  // namespace qmb

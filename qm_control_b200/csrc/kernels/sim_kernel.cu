@@ -98,9 +98,8 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
     if (lane < NQ) { const double* row = w->M + lane * NQ; double* out = w->L + tri(lane); for (int c = 0; c <= lane; ++c) out[c] = row[c]; }
     double fn = 0.0;
     if (lane < 4) {
-      const int f = lane, body = mdl->foot_body[f];
-      double pw[3]; matvec3(ws->R[body], mdl->foot_p[f], pw); pw[0] += ws->p[body][0]; pw[1] += ws->p[body][1]; pw[2] += ws->p[body][2];
-      double vel[3], acc[3]; point_vel_acc(ws, body, pw, vel, acc);
+      const int f = lane;
+      double pw[3], vel[3]; foot_point(mdl, ws, f, pw); point_vel(ws->V[mdl->foot_body[f]], pw, vel);
       double H = prm.ground_height, gx = 0.0, gy = 0.0;
       if (TERRAIN) ground_at(terrain, ter, prm.ground_height, pw[0], pw[1], H, gx, gy);
       const double s = sqrt(1.0 + gx * gx + gy * gy), n[3] = {-gx / s, -gy / s, 1.0 / s};
@@ -142,18 +141,15 @@ __global__ void __launch_bounds__(32 * SIM_WARPS) sim_step_kernel(const DevModel
   double* r = rbd + (size_t)b * QMB200_RBD;
   if (lane < NQ) {
     q_io[(size_t)b * NQ + lane] = w->q[lane]; v_io[(size_t)b * NQ + lane] = w->v[lane];
-    r[lane < 3 ? lane + 3 : (lane < 6 ? lane - 3 : lane)] = w->q[lane];                 // [euler ZYX, pos, joints]
-    if (lane < 3) r[NQ + 3 + lane] = w->v[lane]; else if (lane >= 6) r[NQ + lane] = w->v[lane];   // v_lin, joint velocities
+    r[lane < 3 ? RBD_POS + lane : (lane < 6 ? RBD_ZYX + lane - 3 : RBD_JPOS + lane - 6)] = w->q[lane];
+    if (lane < 3) r[RBD_V + lane] = w->v[lane]; else if (lane >= 6) r[RBD_JVEL + lane - 6] = w->v[lane];
   }
   if (lane == 0) {
     double T[9]; euler_rate_map_sc(ws->trig, T); const double ed[3] = {w->v[3], w->v[4], w->v[5]}; double om[3]; matvec3(T, ed, om);
-    r[NQ] = om[0]; r[NQ + 1] = om[1]; r[NQ + 2] = om[2];                                  // w_world = T(zyx) zyx_rates
-    const int eb = mdl->ee_body; double Rb[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) Rb[i] = ws->R[eb][i];
-    double pe[3]; matvec3(Rb, mdl->ee_p, pe); double Re[9]; matmul3(Rb, mdl->ee_R, Re);
-    r[48] = pe[0] + ws->p[eb][0]; r[49] = pe[1] + ws->p[eb][1]; r[50] = pe[2] + ws->p[eb][2];
-    rot_to_quat_xyzw(Re, r + 51);
+    r[RBD_W] = om[0]; r[RBD_W + 1] = om[1]; r[RBD_W + 2] = om[2];                        // w_world = T(zyx) zyx_rates
+    double pe[3], Re[9]; ee_pose(mdl, ws, pe, Re);
+    r[RBD_EE_POS] = pe[0]; r[RBD_EE_POS + 1] = pe[1]; r[RBD_EE_POS + 2] = pe[2];
+    rot_to_quat_xyzw(Re, r + RBD_EE_QUAT);
     contact[b] = (int32_t)in_contact; status[b] = st;
   }
 }

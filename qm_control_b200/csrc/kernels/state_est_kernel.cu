@@ -120,16 +120,13 @@ __global__ void __launch_bounds__(32 * SE_WARPS) state_est_step_kernel(const Dev
   if (lane < 3) { zyx = w->e[lane]; om = w->e[3 + lane]; }
   rbd_kinematics<true>(mdl, w->q, w->v, ws, lane);
   if (lane < 4) {
-    const int f = lane, body = mdl->foot_body[f];
-    double pw[3], vel[3]; matvec3(ws->R[body], mdl->foot_p[f], pw); pw[0] += ws->p[body][0]; pw[1] += ws->p[body][1]; pw[2] += ws->p[body][2];
-    const double* V = ws->V[body]; cross3(V, pw, vel); vel[0] += V[3]; vel[1] += V[4]; vel[2] += V[5];
+    const int f = lane;
+    double pw[3], vel[3]; foot_point(mdl, ws, f, pw); point_vel(ws->V[mdl->foot_body[f]], pw, vel);
     for (int k = 0; k < 3; ++k) { w->r[f][k] = pw[k]; w->rd[f][k] = vel[k]; }
   }
   if (lane == 4) {
-    const int eb = mdl->ee_body; double Rb[9];
-    for (int i = 0; i < 9; ++i) Rb[i] = ws->R[eb][i];
-    double pe[3], Re[9]; matvec3(Rb, mdl->ee_p, pe); matmul3(Rb, mdl->ee_R, Re);
-    for (int k = 0; k < 3; ++k) w->ee[k] = pe[k] + ws->p[eb][k];
+    double pe[3], Re[9]; ee_pose(mdl, ws, pe, Re);
+    for (int k = 0; k < 3; ++k) w->ee[k] = pe[k];
     rot_to_quat_xyzw(Re, w->ee + 3);
   }
   if (lane < SE_NX) w->x[lane] = st[SE_X + lane];
@@ -215,10 +212,10 @@ __global__ void __launch_bounds__(32 * SE_WARPS) state_est_step_kernel(const Dev
     for (int t = lane; t < SE_TRI; t += 32) st[SE_P + t] = w->P[t];
   }
   // ---- the measurement the controller reads, from the stored state (lane i < 18 wrote st[i] itself) ----
-  if (lane < 6) out[lane < 3 ? 3 + lane : 24 + lane] = st[SE_X + lane];   // p -> [3, 6), v -> [27, 30)
-  if (lane < 3) { out[lane] = zyx; out[24 + lane] = om; }
-  if (lane < NJ) { out[6 + lane] = w->q[6 + lane]; out[30 + lane] = w->v[6 + lane]; }
-  if (lane < 7) out[48 + lane] = lane < 3 ? w->ee[lane] + st[SE_X + lane] : w->ee[lane];
+  if (lane < 6) out[lane < 3 ? RBD_POS + lane : RBD_V + lane - 3] = st[SE_X + lane];
+  if (lane < 3) { out[RBD_ZYX + lane] = zyx; out[RBD_W + lane] = om; }
+  if (lane < NJ) { out[RBD_JPOS + lane] = w->q[6 + lane]; out[RBD_JVEL + lane] = w->v[6 + lane]; }
+  if (lane < 7) out[RBD_EE_POS + lane] = lane < 3 ? w->ee[lane] + st[SE_X + lane] : w->ee[lane];   // position, then the quaternion at RBD_EE_QUAT
   if (lane == 0) { st[SE_N] = n_prev + 1.0; status[b] = code; }
 }
 
