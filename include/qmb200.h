@@ -389,6 +389,35 @@ int qmb200_state_est_get(qmb200_handle* h, double* x /*[B][18]*/, double* p_diag
  * qmb200_payload_est_stop does, so a caller's clean-up may stop unconditionally. */
 int qmb200_state_est_stop(qmb200_handle* h);
 
+/* ---- attitude filter, between the sensors and the state estimator: a multiplicative (error-state) Kalman filter per robot on SO(3) with gyro-bias
+ *      states.  The reference has none (StateEstimateBase::updateImu passes the IMU quaternion through); a real robot's IMU filters on board.
+ *      Nominal q_hat (world <- body) and b_hat, error [dtheta, db] with R = R_hat Exp(dtheta) (body frame), P 6x6.  Per call, on the row sensors[46]
+ *      (qmb200_sim_read_sensors): predict q_hat <- q_hat (x) Exp((gyro - b_hat) dt), P <- F P F^T + dt diag(process), F = [[Exp(w dt)^T, -dt 1], [0, 1]];
+ *      update with the row's quaternion q_m: r = Log(q_hat^-1 (x) q_m) (sign with w >= 0, so q_m and -q_m agree), S = P_tt + meas_orientation 1,
+ *      K = P H^T S^-1, q_hat <- q_hat (x) Exp(K_t r), b_hat += K_b r, P <- P - K H P.  The accelerometer is not used.  The row is rewritten in place:
+ *      quaternion = q_hat (w >= 0), gyro = gyro - b_hat; every other column is untouched, so qmb200_state_est_step reads the filtered row unchanged.
+ *   process_attitude, process_gyro_bias    process noise per second: rad^2/s (gyro white noise as angle random walk), (rad/s)^2/s (bias random walk)
+ *   meas_orientation                       variance of each axis of the orientation reading's error, rad^2 (> 0)
+ *   p0_attitude, p0_gyro_bias              P = diag(p0) at the reset: rad^2, (rad/s)^2 */
+typedef struct qmb200_attitude_params {
+  double process_attitude, process_gyro_bias, meas_orientation, p0_attitude, p0_gyro_bias;   /* rad^2/s, (rad/s)^2/s, rad^2, rad^2, (rad/s)^2 */
+} qmb200_attitude_params;
+int qmb200_attitude_get_params(const qmb200_handle* h, qmb200_attitude_params* out);
+/* rejects a non-finite or negative value and meas_orientation <= 0; on rejection the stored values stay unchanged */
+int qmb200_attitude_set_params(qmb200_handle* h, const qmb200_attitude_params* p);
+/* (Re)starts the filter of every robot: b_hat = 0, P = diag(p0), no call yet; the next call takes q_hat from its reading.  Synchronous. */
+int qmb200_attitude_reset(qmb200_handle* h);
+/* One filter call per robot on sensors [B][46] (in-out) of a step of dt s (finite, > 0).  The first call after a reset sets q_hat to the normalised
+ * reading.  status [B] (written, not OR-ed): QMB200_ST_NAN for a non-finite quaternion or gyro input (neither the row nor the state is touched) or
+ * update (the robot keeps its state and the row is written from it). */
+int qmb200_attitude_step(qmb200_handle* h, double dt, double* sensors /*[B][46] in-out*/, int32_t* status /*[B]*/);
+int qmb200_attitude_step_dev(qmb200_handle* h, double dt, double* sensors, int32_t* status, void* cuda_stream);
+/* Synchronous: q_hat [B][4] (xyzw, as stored: its sign is continuous from call to call), b_hat [B][3], the diagonal of P [B][6] and the calls since the
+ * reset [B].  Any output may be NULL. */
+int qmb200_attitude_get(qmb200_handle* h, double* quat /*[B][4]*/, double* gyro_bias /*[B][3]*/, double* p_diag /*[B][6]*/, int32_t* samples /*[B]*/);
+/* Releases the filter state.  Step and get fail until the next reset.  Stopping a filter that is not running does nothing and returns 0. */
+int qmb200_attitude_stop(qmb200_handle* h);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

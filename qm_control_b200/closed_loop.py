@@ -15,6 +15,7 @@ controller sees: it steps after every plant step and is committed to the model p
 With state_estimator set, the controller no longer reads the plant's true state: after every plant step the IMU and encoders are read
 (Solver.sim_read_sensors_dev) and a base state estimator (Solver.state_est_*) turns them and the contact flags into the measurement every consumer on
 the controller side reads (the updates, the targets' end-effector state, the payload estimator).  The plant and the record keep the truth.
+With attitude_filter set as well, an attitude filter (Solver.attitude_*) rewrites each reading's orientation and gyro columns before the estimator reads them.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -47,7 +48,8 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
-        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None):
+        friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
+        attitude_filter=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -71,6 +73,10 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     sensor_noise: None (noise-free readings), "reference" (_lib.SENSOR_NOISE_REFERENCE, the IMU covariances of qm_gazebo/config/default.yaml) or a dict
     of qmb200_sensor_params overrides; only with state_estimator.  The estimator is stopped and the previous sensor and estimator parameters restored
     when run returns.
+    attitude_filter: True, or a dict of qmb200_attitude_params overrides (Solver.attitude_set_params); only with state_estimator.  After every sensor
+    reading (the start's included) an attitude filter step replaces the reading's quaternion and gyro with the filtered orientation and the
+    bias-corrected rate, and the estimator steps on that.  Its status is OR-ed into the record's.  The filter is stopped and its previous parameters
+    restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
@@ -86,6 +92,10 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         raise ValueError("closed_loop.run: sensor_noise needs state_estimator (the controller reads the plant's true state otherwise)")
     if state_estimator is not None and terrain is not None:
         raise ValueError("closed_loop.run: state_estimator does not support terrain (its foot-height rows assume the plane)")
+    if attitude_filter is not None and attitude_filter is not True and not isinstance(attitude_filter, dict):
+        raise ValueError("closed_loop.run: attitude_filter must be None, True or a dict of attitude filter parameters, got %r" % (attitude_filter,))
+    if attitude_filter is not None and state_estimator is None:
+        raise ValueError("closed_loop.run: attitude_filter needs state_estimator (it filters the sensor readings the estimator reads)")
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
         if terrain is not None:
@@ -96,10 +106,13 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_payload_estimator(solver, payload_estimator))
         if state_estimator is not None:
             scope.enter_context(_state_estimator(solver, state_estimator, sensor_noise))
+        if attitude_filter is not None:
+            scope.enter_context(_attitude_filter(solver, attitude_filter))
         if friction_mu is not None or payload is not None:
             scope.enter_context(_robot_params(solver, friction_mu, payload))
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
-                    torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None)
+                    torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
+                    att=attitude_filter is not None)
 
 
 @contextlib.contextmanager
@@ -165,6 +178,18 @@ def _state_estimator(solver, params, noise):
 
 
 @contextlib.contextmanager
+def _attitude_filter(solver, params):
+    prev_params = solver.attitude_get_params()
+    try:
+        if isinstance(params, dict):
+            solver.attitude_set_params(**params)
+        yield   # _run resets the filter right before its first reading
+    finally:
+        solver.attitude_stop()
+        solver.attitude_set_params(**prev_params)
+
+
+@contextlib.contextmanager
 def _robot_params(solver, friction_mu, payload):
     prev = solver.sim_get_robot_params()
     solver.sim_set_robot_params(friction_mu=prev["friction_mu"] if friction_mu is None else friction_mu, payload=prev["payload"] if payload is None else payload)
@@ -174,7 +199,7 @@ def _robot_params(solver, friction_mu, payload):
         solver.sim_set_robot_params(**prev)
 
 
-def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False):
+def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -203,6 +228,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         if se:   # the controller's measurement: the estimator's rbd_est in place of the plant's rbd
             v_prev = torch.zeros_like(v); sensors = torch.zeros((B, SENSORS), dtype=torch.float64, device=dev); rbd_est = torch.zeros_like(rbd)
             se_st = torch.zeros_like(contact); v_prev.copy_(v)
+            if att:
+                at_st = torch.zeros_like(contact)
     stream.synchronize()
     solver.sim_step_dev(1e-6, effort, q, v, rbd, contact, sim_st, s)   # a 1 us physics step with zero effort reads the first measured state
     meas = rbd
@@ -210,6 +237,9 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         solver.sim_read_sensors_dev(1e-6, -1, q, v, v_prev, sensors, s)
         stream.synchronize()
         solver.state_est_reset(q0[:, 0:3])
+        if att:
+            solver.attitude_reset()
+            solver.attitude_step_dev(1e-6, sensors, at_st, s)   # the first call after the reset takes the reading
         solver.state_est_step_dev(1e-6, sensors, contact, rbd_est, se_st, s)   # the first call after the reset places the feet
         meas = rbd_est
     stream.synchronize()
@@ -268,6 +298,9 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             acc_st.bitwise_or_(hw_st).bitwise_or_(sim_st)
             if se:
                 solver.sim_read_sensors_dev(1e-3, k, q, v, v_prev, sensors, s)
+                if att:
+                    solver.attitude_step_dev(1e-3, sensors, at_st, s)
+                    acc_st.bitwise_or_(at_st)
                 solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, se_st, s)
                 acc_st.bitwise_or_(se_st)
             if est:

@@ -527,6 +527,47 @@ class Solver:
         """Release the estimator state."""
         self._call("state_est_stop")
 
+    # ---------------- attitude filter (include/qmb200.h: qmb200_attitude_*; DESIGN.md §4.6) ----------------
+    def attitude_get_params(self):
+        """→ dict of qmb200_attitude_params."""
+        p = _lib.AttitudeParams(); self._call("attitude_get_params", C.byref(p))
+        return {n: getattr(p, n) for n, _ in _lib.AttitudeParams._fields_}
+
+    def attitude_set_params(self, **params):
+        """Keyword per field of qmb200_attitude_params; unspecified fields keep their value."""
+        p = _lib.AttitudeParams(); self._call("attitude_get_params", C.byref(p))
+        names = [n for n, _ in _lib.AttitudeParams._fields_]
+        for k, v in params.items():
+            if k not in names:
+                raise ValueError("attitude_set_params: unknown parameter %r (one of %s)" % (k, ", ".join(names)))
+            setattr(p, k, float(v))
+        self._call("attitude_set_params", C.byref(p))
+
+    def attitude_reset(self):
+        """(Re)start the attitude filter of every robot: b_hat = 0, P = diag(p0); the next call takes its reading.  Synchronous."""
+        self._call("attitude_reset")
+
+    def attitude_step(self, dt, sensors):
+        """One filter call per robot on sensors [B, 46] → (sensors [B, 46] with the filtered quaternion and the bias-corrected gyro, status [B]).  The
+        input is not modified."""
+        B = self.batch; out = _f64(sensors, (B, _lib.SENSORS)).copy(); st = np.zeros(B, dtype=np.int32)
+        self._call("attitude_step", float(dt), _p(out), _p(st))
+        return out, st
+
+    def attitude_step_dev(self, dt, sensors, status, stream=None):
+        """Device-pointer variant: sensors [B, 46] rewritten in place, status [B] int32 written; no synchronisation."""
+        self._call("attitude_step_dev", float(dt), _p(sensors), _p(status), stream)
+
+    def attitude_get(self):
+        """→ dict(quat [B, 4] (xyzw as stored), gyro_bias [B, 3], p_diag [B, 6], samples [B]).  Synchronous."""
+        B = self.batch; qt = np.zeros((B, 4)); bias = np.zeros((B, 3)); pd = np.zeros((B, 6)); n = np.zeros(B, dtype=np.int32)
+        self._call("attitude_get", _p(qt), _p(bias), _p(pd), _p(n))
+        return dict(quat=qt, gyro_bias=bias, p_diag=pd, samples=n)
+
+    def attitude_stop(self):
+        """Release the filter state."""
+        self._call("attitude_stop")
+
     # ---------------- utilities ----------------
     def centroidal_state_from_rbd(self, rbd):
         rbd = _f64(rbd); n = rbd.shape[0]; x = np.empty((n, NX))

@@ -4,7 +4,7 @@ Default: 8192 robots, trot at cmd_vel 0.3 m/s, 1 s simulated after a warm-up run
 simulated second, the plant step's device time per call (CUDA events) and its share of the loop, and quality lines (base distance, end-effector
 deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
 
-    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference]]
+    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter]]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -29,6 +29,12 @@ those of the estimating controller.  The JSON line gains "state_est": the device
 this batch (CUDA events, alternated with blocks of plant steps); percentiles over the robots of |z_hat - z| and |v_hat - v| (over the run and at the
 end) and of the xy drift at the end (taken in the warm-up run, which is the timed run's twin); and the quality lines of a ground-truth run of the same
 sweep (one more untimed run in the same process).  Each of these runs starts from a cold MPC and WBC state (Solver.mpc_reset, wbc_set_input_last).
+The error percentiles include the wrapped zyx orientation error of rbd_est against the plant (the largest of the three angles).
+
+--attitude-filter (with --state-estimator) runs the attitude filter between the sensors and the estimator (closed_loop.run(attitude_filter=True)): the
+timed run and the quality lines are then those of the filtered chain.  The JSON line gains "attitude": the filter's device time per call at this batch
+(CUDA events, alternated with blocks of plant steps), and the fallen count and quality lines of the same sweep on the estimate without the filter (one
+more untimed run in the same process).
 """
 import argparse
 import json
@@ -149,9 +155,42 @@ def state_est_times(solver, xy_yaw, reps=7, calls=20):
             "spread": [float(min(times["estimator"])), float(max(times["estimator"]))]}
 
 
+def attitude_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per attitude filter call and per 1 ms plant step of the whole batch, alternated `reps` times in blocks of `calls` from one standing
+    state (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    sensors = torch.zeros((B, 46), dtype=torch.float64, device=dev); contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+    solver.sim_read_sensors_dev(1e-3, 0, q, v, v, sensors, s.cuda_stream); torch.cuda.synchronize(dev)
+    solver.attitude_reset(); solver.attitude_step_dev(1e-3, sensors, st, s.cuda_stream)   # past the first call, which only takes the reading
+    times = {"attitude": [], "plant": []}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode in ("attitude", "plant"):
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    if mode == "attitude":
+                        solver.attitude_step_dev(1e-3, sensors, st, s.cuda_stream)
+                    else:
+                        solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.attitude_stop()
+    return {"label": "device time per attitude filter call and per 1 ms plant step of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            "ms_per_call": float(np.median(times["attitude"])), "ms_per_plant_step": float(np.median(times["plant"])),
+            "spread": [float(min(times["attitude"])), float(max(times["attitude"]))]}
+
+
 def watch_state_est(solver):
-    """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z| and |v_hat - v| on the device (no
-    synchronisation) → (box, unwrap); box["max"] [B, 2], box["last"] [B, 2] after the run."""
+    """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
+    error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
     import torch
     orig_sim, orig_est = solver.sim_step_dev, solver.state_est_step_dev; box = {}
 
@@ -161,7 +200,8 @@ def watch_state_est(solver):
     def est(dt, sensors, contact, rbd_est, status, stream=None):
         orig_est(dt, sensors, contact, rbd_est, status, stream)
         with torch.cuda.stream(torch.cuda.ExternalStream(stream)):
-            e = torch.stack([(rbd_est[:, 5] - box["rbd"][:, 5]).abs(), (rbd_est[:, 27:30] - box["rbd"][:, 27:30]).norm(dim=1)], 1)
+            e = torch.stack([(rbd_est[:, 5] - box["rbd"][:, 5]).abs(), (rbd_est[:, 27:30] - box["rbd"][:, 27:30]).norm(dim=1),
+                             torch.remainder(rbd_est[:, 0:3] - box["rbd"][:, 0:3] + np.pi, 2 * np.pi).sub_(np.pi).abs().amax(dim=1)], 1)
             box["last"] = e; box["max"] = e if "max" not in box else torch.maximum(box["max"], e)
 
     def unwrap():
@@ -180,11 +220,14 @@ def main():
     ap.add_argument("--terrain", action="store_true", help="per-robot sweep of ramp angle and step rise under the feet")
     ap.add_argument("--state-estimator", action="store_true", help="the controller reads the base state estimate from the IMU, encoders and contact flags")
     ap.add_argument("--sensor-noise", choices=["reference"], help="with --state-estimator: the IMU noise of qm_gazebo/config/default.yaml")
+    ap.add_argument("--attitude-filter", action="store_true", help="with --state-estimator: filter the IMU orientation before the estimator reads it")
     args = ap.parse_args()
     if args.vary and args.terrain:
         ap.error("--vary and --terrain are separate sweeps")
     if args.sensor_noise and not args.state_estimator:
         ap.error("--sensor-noise needs --state-estimator")
+    if args.attitude_filter and not args.state_estimator:
+        ap.error("--attitude-filter needs --state-estimator")
     if args.state_estimator and args.terrain:
         ap.error("--state-estimator assumes the plane: it cannot be combined with --terrain")
     import torch
@@ -210,7 +253,7 @@ def main():
         ter = dict(tiles=tiles, cell=T.CELL, tile=idx["ramp_deg"] * 4 + idx["step_rise_m"], origin=T.centred_origin(xy[:, :2]))
         kw = dict(terrain=ter)
     told = {"plant": dict(model_payload="plant"), "estimate": dict(payload_estimator=True), None: {}}[args.model_payload]
-    se = dict(state_estimator=True, sensor_noise=args.sensor_noise) if args.state_estimator else {}
+    se = dict(state_estimator=True, sensor_noise=args.sensor_noise, **({"attitude_filter": True} if args.attitude_filter else {})) if args.state_estimator else {}
     def fresh():
         """with --state-estimator every run starts from a cold MPC and WBC state: a run whose robots fell leaves warm starts the next run must not inherit"""
         if args.state_estimator:
@@ -282,10 +325,18 @@ def main():
         t_dist, t_dpos, t_dang = quality(truth)
         extra["state_est"] = {**state_est_times(solver, xy), "gpu": name, "power_limit": limit, "sensor_noise": args.sensor_noise or "none",
                               "errors": {"label": "over the robots, from the warm-up run (the timed run's twin)", "z_abs_m_over_run": pct(mx[:, 0]), "z_abs_m_at_end": pct(last[:, 0]),
-                                         "v_abs_m_s_over_run": pct(mx[:, 1]), "v_abs_m_s_at_end": pct(last[:, 1]), "xy_drift_m_at_end": pct(drift)},
+                                         "v_abs_m_s_over_run": pct(mx[:, 1]), "v_abs_m_s_at_end": pct(last[:, 1]), "xy_drift_m_at_end": pct(drift),
+                                         "zyx_abs_rad_over_run": pct(mx[:, 2]), "zyx_abs_rad_at_end": pct(last[:, 2])},
                               "fallen": int(np.sum(~upright(r))), "fallen_warmup": int(np.sum(~upright(warm))), "ground_truth": {"label": "the same sweep, controller reading the plant's true state", "fallen": int(np.sum(~upright(truth))),
                                                                                     "base_distance_m": pct(t_dist), "ee_max_pos_dev_mm": pct(t_dpos), "ee_max_ori_dev_deg": pct(t_dang),
                                                                                     "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(truth["status"], axis=0)))}}
+        if args.attitude_filter:
+            fresh(); raw = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told, state_estimator=True, sensor_noise=args.sensor_noise)
+            n_dist, n_dpos, n_dang = quality(raw)
+            extra["attitude"] = {**attitude_times(solver, xy), "gpu": name, "power_limit": limit,
+                                 "without_filter": {"label": "the same sweep on the estimate, without the attitude filter", "fallen": int(np.sum(~upright(raw))),
+                                                    "base_distance_m": pct(n_dist), "ee_max_pos_dev_mm": pct(n_dpos), "ee_max_ori_dev_deg": pct(n_dang),
+                                                    "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(raw["status"], axis=0)))}}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
@@ -295,7 +346,8 @@ def main():
                                   "min_base_height_m": float(np.min(r["base"][:, :, 2])), "max_abs_roll_pitch_rad": float(np.max(np.abs(r["base"][:, :, 4:6])))},
                       "config": {"workload": "closed loop: %s, cmd_vel %.2f m/s, MPC 100 Hz / WBC 500 Hz / plant 1 kHz (4 substeps), 9 ms command delay" % (args.gait, args.vx),
                                  "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length", **({"model_payload": args.model_payload} if args.model_payload else {}),
-                                 **({"state_estimator": True, "sensor_noise": args.sensor_noise or "none"} if args.state_estimator else {})}, **extra}))
+                                 **({"state_estimator": True, "sensor_noise": args.sensor_noise or "none", "attitude_filter": args.attitude_filter} if args.state_estimator else {})},
+                      **extra}))
 
 
 if __name__ == "__main__":
