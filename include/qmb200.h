@@ -418,6 +418,39 @@ int qmb200_attitude_get(qmb200_handle* h, double* quat /*[B][4]*/, double* gyro_
 /* Releases the filter state.  Step and get fail until the next reset.  Stopping a filter that is not running does nothing and returns 0. */
 int qmb200_attitude_stop(qmb200_handle* h);
 
+/* ---- slip detector, between the sensors (and the attitude filter) and the state estimator: per robot and foot in contact, a test of the foot's
+ *      velocity against the estimator's prior.  The estimator's leg-velocity rows (v_base = -dr_i/dt) assume a stance foot at rest; a foot that slides
+ *      breaks them.  Per call, from the row sensors[46] (the legs as qmb200_state_est_step reads them) and the estimator's stored state (read only):
+ *      v- = v_hat + a dt (a = R accel + g), Sigma- = P_vv + dt process_base_vel 1; per foot i in contact u_i = v- + dr_i/dt (the world velocity of the
+ *      foot point) and d2_i = u_i^T (Sigma- + meas_slip 1)^-1 u_i.  A foot becomes slipping when d2_i > gate and is trusted again after hold consecutive
+ *      calls with d2_i < release (hold 0 acts as 1); a foot out of contact is cleared.  stance = contact & ~slip is the mask to pass to
+ *      qmb200_state_est_step in place of the plant's: a slipping foot is then handled as a swing foot.
+ *   gate, release     thresholds on d2 (chi-square, 3 degrees of freedom), 0 < release <= gate
+ *   meas_slip         variance added per axis for a stance foot's own velocity (its creep under the compliant contact), (m/s)^2, >= 0
+ *   hold              calls below release before a slipping foot is trusted again, >= 0 */
+typedef struct qmb200_slip_params {
+  double gate, release, meas_slip;   /* -, -, (m/s)^2 */
+  int32_t hold;                      /* calls */
+} qmb200_slip_params;
+int qmb200_slip_get_params(const qmb200_handle* h, qmb200_slip_params* out);
+/* rejects non-finite values, gate <= 0, release outside (0, gate], meas_slip < 0 and hold < 0; on rejection the stored values stay unchanged */
+int qmb200_slip_set_params(qmb200_handle* h, const qmb200_slip_params* p);
+/* (Re)starts the detector of every robot: no foot slipping, counters zero.  Synchronous. */
+int qmb200_slip_reset(qmb200_handle* h);
+/* One detector call per robot of a step of dt s (finite, > 0), before the estimator's step on the same row: from sensors [B][46] and the contact mask
+ * contact_in [B], writes stance_out [B] = contact_in & ~slip_out and slip_out [B] (the feet in contact flagged as slipping, contact bit order).  Needs
+ * the detector and the state estimator running.  Before the estimator's first call after its reset, and for a robot with a non-finite reading
+ * (status QMB200_ST_NAN), contact_in passes through and the robot's detector state is untouched.  status [B] is written, not OR-ed. */
+int qmb200_slip_step(qmb200_handle* h, double dt, const double* sensors /*[B][46]*/, const int32_t* contact_in /*[B]*/, int32_t* stance_out /*[B]*/,
+                     int32_t* slip_out /*[B]*/, int32_t* status /*[B]*/);
+int qmb200_slip_step_dev(qmb200_handle* h, double dt, const double* sensors, const int32_t* contact_in, int32_t* stance_out, int32_t* slip_out, int32_t* status,
+                         void* cuda_stream);
+/* Synchronous: the slip mask [B], per foot the calls below release counted towards hold [B][4] and the onsets since the reset [B][4] (feet in contact
+ * order LF, RF, LH, RH).  Any output may be NULL. */
+int qmb200_slip_get(qmb200_handle* h, int32_t* mask /*[B]*/, int32_t* hold /*[B][4]*/, int32_t* onsets /*[B][4]*/);
+/* Releases the detector state.  Step and get fail until the next reset.  Stopping a detector that is not running does nothing and returns 0. */
+int qmb200_slip_stop(qmb200_handle* h);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

@@ -58,6 +58,11 @@ class AttitudeParams(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("process_attitude", "process_gyro_bias", "meas_orientation", "p0_attitude", "p0_gyro_bias")]
 
 
+class SlipParams(C.Structure):
+    """qmb200_slip_params: the slip detector's thresholds (include/qmb200.h, DESIGN.md §4.6)."""
+    _fields_ = [("gate", C.c_double), ("release", C.c_double), ("meas_slip", C.c_double), ("hold", C.c_int32)]
+
+
 # the sensor reading's columns (qmb200_sim_read_sensors) and the state estimator's state x (qmb200_state_est_get)
 SENSOR_LAYOUT = ("quat_x", "quat_y", "quat_z", "quat_w", "gyro_x", "gyro_y", "gyro_z", "accel_x", "accel_y", "accel_z") + \
                 tuple("joint_pos_%d" % j for j in range(18)) + tuple("joint_vel_%d" % j for j in range(18))
@@ -163,6 +168,13 @@ PROTOTYPES = {
     "qmb200_attitude_step_dev": (I32, [P, D] + [P] * 3),
     "qmb200_attitude_get": (I32, [P] * 5),
     "qmb200_attitude_stop": (I32, [P]),
+    "qmb200_slip_get_params": (I32, [P] * 2),
+    "qmb200_slip_set_params": (I32, [P] * 2),
+    "qmb200_slip_reset": (I32, [P]),
+    "qmb200_slip_step": (I32, [P, D] + [P] * 5),
+    "qmb200_slip_step_dev": (I32, [P, D] + [P] * 6),
+    "qmb200_slip_get": (I32, [P] * 4),
+    "qmb200_slip_stop": (I32, [P]),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

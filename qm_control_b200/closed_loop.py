@@ -16,6 +16,7 @@ With state_estimator set, the controller no longer reads the plant's true state:
 (Solver.sim_read_sensors_dev) and a base state estimator (Solver.state_est_*) turns them and the contact flags into the measurement every consumer on
 the controller side reads (the updates, the targets' end-effector state, the payload estimator).  The plant and the record keep the truth.
 With attitude_filter set as well, an attitude filter (Solver.attitude_*) rewrites each reading's orientation and gyro columns before the estimator reads them.
+With slip_detector set as well, a slip detector (Solver.slip_*) removes the stance feet that slide from the contact mask the estimator reads.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -49,7 +50,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None):
+        attitude_filter=None, slip_detector=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -77,11 +78,14 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     reading (the start's included) an attitude filter step replaces the reading's quaternion and gyro with the filtered orientation and the
     bias-corrected rate, and the estimator steps on that.  Its status is OR-ed into the record's.  The filter is stopped and its previous parameters
     restored when run returns.
+    slip_detector: True, or a dict of qmb200_slip_params overrides (Solver.slip_set_params); only with state_estimator.  After every sensor reading
+    (and attitude filter step) a detector step turns the plant's contact mask into the mask of trusted stance feet, and the estimator steps on that
+    mask.  Its status is OR-ed into the record's.  The detector is stopped and its previous parameters restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
     payload_est[ticks, B, 8] = the model payload rows committed at each record's MPC tick; with state_estimator also base_est[ticks, B, 6], the estimated base in
-    the layout of base)."""
+    the layout of base; with slip_detector also slip[ticks, B], the OR of the detector's slip masks over each record's 10 ms window)."""
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
     if state_estimator is not None and state_estimator is not True and not isinstance(state_estimator, dict):
@@ -96,6 +100,10 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         raise ValueError("closed_loop.run: attitude_filter must be None, True or a dict of attitude filter parameters, got %r" % (attitude_filter,))
     if attitude_filter is not None and state_estimator is None:
         raise ValueError("closed_loop.run: attitude_filter needs state_estimator (it filters the sensor readings the estimator reads)")
+    if slip_detector is not None and slip_detector is not True and not isinstance(slip_detector, dict):
+        raise ValueError("closed_loop.run: slip_detector must be None, True or a dict of slip detector parameters, got %r" % (slip_detector,))
+    if slip_detector is not None and state_estimator is None:
+        raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
         if terrain is not None:
@@ -108,11 +116,13 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_state_estimator(solver, state_estimator, sensor_noise))
         if attitude_filter is not None:
             scope.enter_context(_attitude_filter(solver, attitude_filter))
+        if slip_detector is not None:
+            scope.enter_context(_slip_detector(solver, slip_detector))
         if friction_mu is not None or payload is not None:
             scope.enter_context(_robot_params(solver, friction_mu, payload))
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None)
+                    att=attitude_filter is not None, sl=slip_detector is not None)
 
 
 @contextlib.contextmanager
@@ -190,6 +200,18 @@ def _attitude_filter(solver, params):
 
 
 @contextlib.contextmanager
+def _slip_detector(solver, params):
+    prev_params = solver.slip_get_params()
+    try:
+        if isinstance(params, dict):
+            solver.slip_set_params(**params)
+        yield   # _run resets the detector with the estimator
+    finally:
+        solver.slip_stop()
+        solver.slip_set_params(**prev_params)
+
+
+@contextlib.contextmanager
 def _robot_params(solver, friction_mu, payload):
     prev = solver.sim_get_robot_params()
     solver.sim_set_robot_params(friction_mu=prev["friction_mu"] if friction_mu is None else friction_mu, payload=prev["payload"] if payload is None else payload)
@@ -199,7 +221,7 @@ def _robot_params(solver, friction_mu, payload):
         solver.sim_set_robot_params(**prev)
 
 
-def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False):
+def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -230,6 +252,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             se_st = torch.zeros_like(contact); v_prev.copy_(v)
             if att:
                 at_st = torch.zeros_like(contact)
+            if sl:   # the estimator reads the trusted stance mask in place of the plant's contact mask
+                stance = torch.zeros_like(contact); slip = torch.zeros_like(contact); sl_st = torch.zeros_like(contact); slip_acc = torch.zeros_like(contact)
     stream.synchronize()
     solver.sim_step_dev(1e-6, effort, q, v, rbd, contact, sim_st, s)   # a 1 us physics step with zero effort reads the first measured state
     meas = rbd
@@ -240,7 +264,12 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         if att:
             solver.attitude_reset()
             solver.attitude_step_dev(1e-6, sensors, at_st, s)   # the first call after the reset takes the reading
-        solver.state_est_step_dev(1e-6, sensors, contact, rbd_est, se_st, s)   # the first call after the reset places the feet
+        se_contact = contact
+        if sl:
+            solver.slip_reset()
+            solver.slip_step_dev(1e-6, sensors, contact, stance, slip, sl_st, s)   # passes the contact mask through: the estimator has had no call yet
+            se_contact = stance
+        solver.state_est_step_dev(1e-6, sensors, se_contact, rbd_est, se_st, s)   # the first call after the reset places the feet
         meas = rbd_est
     stream.synchronize()
     rbd_h = rbd.cpu().numpy()
@@ -262,6 +291,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             est_st = torch.zeros_like(contact); rec_pl = torch.zeros((ticks, B, 8), dtype=torch.float64, device=dev)   # row i: the rows of window i's MPC tick
         if se:
             rec_base_est = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev)
+        if sl:
+            rec_slip = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
         push = None
         if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
             push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench), zero=torch.zeros((B, 12), dtype=torch.float64, device=dev),
@@ -301,7 +332,10 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                 if att:
                     solver.attitude_step_dev(1e-3, sensors, at_st, s)
                     acc_st.bitwise_or_(at_st)
-                solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, se_st, s)
+                if sl:
+                    solver.slip_step_dev(1e-3, sensors, contact, stance, slip, sl_st, s)
+                    acc_st.bitwise_or_(sl_st); slip_acc.bitwise_or_(slip)
+                solver.state_est_step_dev(1e-3, sensors, se_contact, rbd_est, se_st, s)
                 acc_st.bitwise_or_(se_st)
             if est:
                 solver.payload_est_step_dev(1e-3, effort, meas, est_st, s)
@@ -311,6 +345,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                 rec_base[i, :, 0:3] = rbd[:, 3:6]; rec_base[i, :, 3:6] = rbd[:, 0:3]; rec_ee[i] = rbd[:, 48:55]; rec_st[i] = acc_st; acc_st.zero_()
                 if se:
                     rec_base_est[i, :, 0:3] = rbd_est[:, 3:6]; rec_base_est[i, :, 3:6] = rbd_est[:, 0:3]
+                if sl:
+                    rec_slip[i] = slip_acc; slip_acc.zero_()
     stream.synchronize()
     t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
     out = dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
@@ -319,4 +355,6 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         out["payload_est"] = rec_pl.cpu().numpy()
     if se:
         out["base_est"] = rec_base_est.cpu().numpy()
+    if sl:
+        out["slip"] = rec_slip.cpu().numpy()
     return out

@@ -17,6 +17,7 @@
 #include "kernels/payload_est_api.cuh"
 #include "kernels/state_est_api.cuh"
 #include "kernels/attitude_api.cuh"
+#include "kernels/slip_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -66,6 +67,7 @@ struct qmb200_handle {
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
   qmb200_state_est_params se_prm{}; double* d_se = nullptr;        // base state estimator: parameters and state [B][SE_DBL], NULL when not running
   qmb200_attitude_params at_prm{}; double* d_at = nullptr;         // attitude filter (capi_attitude.inc): parameters and state [B][AT_DBL], NULL when not running
+  qmb200_slip_params sl_prm{}; double* d_sl = nullptr;             // slip detector (capi_slip.inc): parameters and state [B][SL_DBL], NULL when not running
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
@@ -80,6 +82,7 @@ SimParams default_sim_params();   // capi_sim.inc
 qmb200_payload_est_params default_est_params();   // capi_est.inc
 qmb200_state_est_params default_state_est_params(const DevModel& d);   // capi_state_est.inc
 qmb200_attitude_params default_attitude_params();   // capi_attitude.inc
+qmb200_slip_params default_slip_params();   // capi_slip.inc
 int fail(qmb200_handle* h, const std::string& msg) { if (h) h->err = msg; else g_create_error = msg; return -1; }
 #define QMB_CUDA(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(h, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
 
@@ -176,6 +179,7 @@ int qmb200_create(const qmb200_config* cfg, qmb200_handle** out) {
   } catch (const std::exception& e) { g_create_error = e.what(); delete h; return -2; }
   h->task_file = cfg->task_file;
   h->sim_prm = default_sim_params(); h->est_prm = default_est_params(); h->se_prm = default_state_est_params(h->hm.dev); h->at_prm = default_attitude_params();
+  h->sl_prm = default_slip_params();
   h->B = cfg->batch; h->variant = cfg->wbc_variant; h->device = cfg->device; h->law_prm.variant = cfg->wbc_variant == QMB200_WBC_HIERARCHICAL_MPC ? 1 : 0;
   const int nint = (int)std::ceil(h->hm.dev.time_horizon / h->hm.dev.dt - 1e-9);
   h->nmax = cfg->max_nodes > 0 ? cfg->max_nodes : nint + 1 + 20;
@@ -206,6 +210,7 @@ void qmb200_destroy(qmb200_handle* h) {
   if (h->d_est) cudaFree(h->d_est);
   if (h->d_se) cudaFree(h->d_se);
   if (h->d_at) cudaFree(h->d_at);
+  if (h->d_sl) cudaFree(h->d_sl);
   delete h;
 }
 
@@ -359,3 +364,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_est.inc"
 #include "capi_state_est.inc"
 #include "capi_attitude.inc"
+#include "capi_slip.inc"

@@ -19,7 +19,15 @@
 // The first call after a reset only places the feet at p + r_i.  rbd_est[55] = [zyx, p, joints, w, v, joint rates, end-effector pose].
 // status: QMB200_ST_NAN for a non-finite input (nothing is written) or update (x and P are kept); QMB200_ST_NOT_PD when S fails the Cholesky (x and P are
 // kept).  rbd_est is written in both of the last two cases, from the kept state.
+//
+// slip_step_kernel, one warp per robot, between the sensor reading (and the attitude filter) and the estimator step: the legs as the estimator reads
+// them (read_legs), then for each foot f in contact u_f = v- + rd_f, the world velocity of the foot point under the estimator's prior v- = v_hat + a dt,
+// and d^2_f = u_f^T (P_vv + dt process_base_vel 1 + meas_slip 1)^-1 u_f.  A foot becomes slipping when d^2_f > gate and is trusted again after hold
+// consecutive calls with d^2_f < release; a foot out of contact is cleared.  stance = contact & ~slip is the mask the estimator step reads in place of
+// contact, so a slipping foot is handled as a swing foot.  Before the estimator's first call after its reset (SE_N = 0) and on a non-finite reading
+// (QMB200_ST_NAN) the contact mask passes through and the detector's state is untouched.
 #include "state_est_api.cuh"
+#include "slip_api.cuh"
 #include "rbd.cuh"
 #include "wlinalg.cuh"
 
@@ -54,6 +62,54 @@ __device__ __forceinline__ int tri_row(int t) {
   if (tri(i) > t) --i; else if (tri(i + 1) <= t) ++i;
   return i;
 }
+
+// The reading of one sensor row sn, shared by the estimator and the slip detector.  Lane 0: R and zyx from the quaternion, w = R gyro, a = R accel + g;
+// lanes < NJ: the encoders; then rbd_kinematics<true> at q = [0, zyx, joints], v = [0, T^-1 w, joint rates] and, per foot f (lane f < 4), its offset
+// r_f from the base and its velocity rd_f in world axes; with EE also the end-effector pose relative to the base (lane 4).  W: a warp workspace with
+// rb, q, v, a, r, rd, a scratch e[>= 6] and, with EE, ee.  zyx and om: lane i < 3's euler angle and world angular velocity component.  Lanes 0..4 leave
+// without a final __syncwarp: the caller syncs before it reads r, rd or ee from another lane.
+template <bool EE, class W>
+__device__ __forceinline__ void read_legs(const DevModel* __restrict__ mdl, const double* sn, W* w, int lane, double& zyx, double& om) {
+  RbdWs* ws = &w->rb;
+  if (lane == 0) {
+    double qt[4] = {sn[SEN_QUAT], sn[SEN_QUAT + 1], sn[SEN_QUAT + 2], sn[SEN_QUAT + 3]};
+    const double nn = 1.0 / sqrt(qt[0] * qt[0] + qt[1] * qt[1] + qt[2] * qt[2] + qt[3] * qt[3]);
+    const double x = qt[0] * nn, y = qt[1] * nn, z = qt[2] * nn, qw = qt[3] * nn;
+    const double R[9] = {1.0 - 2.0 * (y * y + z * z), 2.0 * (x * y - z * qw), 2.0 * (x * z + y * qw),
+                         2.0 * (x * y + z * qw), 1.0 - 2.0 * (x * x + z * z), 2.0 * (y * z - x * qw),
+                         2.0 * (x * z - y * qw), 2.0 * (y * z + x * qw), 1.0 - 2.0 * (x * x + y * y)};
+    const double e[3] = {atan2(R[3], R[0]), asin(fmin(fmax(-R[6], -1.0), 1.0)), atan2(R[7], R[8])};
+    const double gy[3] = {sn[SEN_GYRO], sn[SEN_GYRO + 1], sn[SEN_GYRO + 2]}, ac[3] = {sn[SEN_ACCEL], sn[SEN_ACCEL + 1], sn[SEN_ACCEL + 2]};
+    double wv[3], a[3], T[9], Ti[9], ed[3]; matvec3(R, gy, wv); matvec3(R, ac, a); a[2] -= 9.81;
+    euler_rate_map(e[0], e[1], T); inv3(T, Ti); matvec3(Ti, wv, ed);
+    for (int i = 0; i < 3; ++i) { w->q[i] = 0.0; w->v[i] = 0.0; w->q[3 + i] = e[i]; w->v[3 + i] = ed[i]; w->a[i] = a[i]; w->e[i] = e[i]; w->e[3 + i] = wv[i]; }
+  }
+  if (lane < NJ) { w->q[6 + lane] = sn[SEN_JPOS + lane]; w->v[6 + lane] = sn[SEN_JVEL + lane]; }
+  __syncwarp();
+  if (lane < 3) { zyx = w->e[lane]; om = w->e[3 + lane]; }
+  rbd_kinematics<true>(mdl, w->q, w->v, ws, lane);
+  if (lane < 4) {
+    const int f = lane;
+    double pw[3], vel[3]; foot_point(mdl, ws, f, pw); point_vel(ws->V[mdl->foot_body[f]], pw, vel);
+    for (int k = 0; k < 3; ++k) { w->r[f][k] = pw[k]; w->rd[f][k] = vel[k]; }
+  }
+  if constexpr (EE) {
+    if (lane == 4) {
+      double pe[3], Re[9]; ee_pose(mdl, ws, pe, Re);
+      for (int k = 0; k < 3; ++k) w->ee[k] = pe[k];
+      rot_to_quat_xyzw(Re, w->ee + 3);
+    }
+  }
+}
+
+constexpr int SL_WARPS = 4;   // robots per CTA of the slip detector
+struct SlWs {
+  RbdWs rb;
+  double q[NQ], v[NQ];
+  double r[4][3], rd[4][3];   // foot offsets from the base and their velocities (world axes)
+  double a[3];                // base acceleration a = R accel + g (world)
+  double e[6];                // read_legs' scratch
+};
 }  // namespace
 
 __global__ void read_sensors_kernel(qmb200_sensor_params prm, int B, int64_t robot0, double dt, int64_t sample, const double* __restrict__ q,
@@ -94,41 +150,14 @@ __global__ void __launch_bounds__(32 * SE_WARPS) state_est_step_kernel(const Dev
   __shared__ SeWs s_ws[SE_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * SE_WARPS + warp;
   if (b >= B) return;   // the whole warp leaves together
-  SeWs* w = &s_ws[warp]; RbdWs* ws = &w->rb;
+  SeWs* w = &s_ws[warp];
   const double* sn = sensors + (size_t)b * QMB200_SENSORS; double* st = state + (size_t)b * SE_DBL; double* out = rbd_est + (size_t)b * QMB200_RBD;
   const double s0 = sn[lane], s1 = lane + 32 < QMB200_SENSORS ? sn[lane + 32] : 0.0;
   if (__any_sync(FULL, !(isfinite(s0) && isfinite(s1)))) { if (lane == 0) status[b] = QMB200_ST_NAN; return; }   // dt: checked by the API
   const int mask = contact[b];
 
-  // ---- attitude from the IMU, joints from the encoders ----
   double zyx = 0.0, om = 0.0;   // lanes 0..2: this lane's euler angle and world angular velocity component
-  if (lane == 0) {
-    double qt[4] = {sn[SEN_QUAT], sn[SEN_QUAT + 1], sn[SEN_QUAT + 2], sn[SEN_QUAT + 3]};
-    const double nn = 1.0 / sqrt(qt[0] * qt[0] + qt[1] * qt[1] + qt[2] * qt[2] + qt[3] * qt[3]);
-    const double x = qt[0] * nn, y = qt[1] * nn, z = qt[2] * nn, qw = qt[3] * nn;
-    const double R[9] = {1.0 - 2.0 * (y * y + z * z), 2.0 * (x * y - z * qw), 2.0 * (x * z + y * qw),
-                         2.0 * (x * y + z * qw), 1.0 - 2.0 * (x * x + z * z), 2.0 * (y * z - x * qw),
-                         2.0 * (x * z - y * qw), 2.0 * (y * z + x * qw), 1.0 - 2.0 * (x * x + y * y)};
-    const double e[3] = {atan2(R[3], R[0]), asin(fmin(fmax(-R[6], -1.0), 1.0)), atan2(R[7], R[8])};
-    const double gy[3] = {sn[SEN_GYRO], sn[SEN_GYRO + 1], sn[SEN_GYRO + 2]}, ac[3] = {sn[SEN_ACCEL], sn[SEN_ACCEL + 1], sn[SEN_ACCEL + 2]};
-    double wv[3], a[3], T[9], Ti[9], ed[3]; matvec3(R, gy, wv); matvec3(R, ac, a); a[2] -= 9.81;
-    euler_rate_map(e[0], e[1], T); inv3(T, Ti); matvec3(Ti, wv, ed);
-    for (int i = 0; i < 3; ++i) { w->q[i] = 0.0; w->v[i] = 0.0; w->q[3 + i] = e[i]; w->v[3 + i] = ed[i]; w->a[i] = a[i]; w->e[i] = e[i]; w->e[3 + i] = wv[i]; }
-  }
-  if (lane < NJ) { w->q[6 + lane] = sn[SEN_JPOS + lane]; w->v[6 + lane] = sn[SEN_JVEL + lane]; }
-  __syncwarp();
-  if (lane < 3) { zyx = w->e[lane]; om = w->e[3 + lane]; }
-  rbd_kinematics<true>(mdl, w->q, w->v, ws, lane);
-  if (lane < 4) {
-    const int f = lane;
-    double pw[3], vel[3]; foot_point(mdl, ws, f, pw); point_vel(ws->V[mdl->foot_body[f]], pw, vel);
-    for (int k = 0; k < 3; ++k) { w->r[f][k] = pw[k]; w->rd[f][k] = vel[k]; }
-  }
-  if (lane == 4) {
-    double pe[3], Re[9]; ee_pose(mdl, ws, pe, Re);
-    for (int k = 0; k < 3; ++k) w->ee[k] = pe[k];
-    rot_to_quat_xyzw(Re, w->ee + 3);
-  }
+  read_legs<true>(mdl, sn, w, lane, zyx, om);
   if (lane < SE_NX) w->x[lane] = st[SE_X + lane];
   for (int t = lane; t < SE_TRI; t += 32) w->P[t] = st[SE_P + t];
   const double n_prev = st[SE_N];
@@ -217,6 +246,67 @@ __global__ void __launch_bounds__(32 * SE_WARPS) state_est_step_kernel(const Dev
   if (lane < NJ) { out[RBD_JPOS + lane] = w->q[6 + lane]; out[RBD_JVEL + lane] = w->v[6 + lane]; }
   if (lane < 7) out[RBD_EE_POS + lane] = lane < 3 ? w->ee[lane] + st[SE_X + lane] : w->ee[lane];   // position, then the quaternion at RBD_EE_QUAT
   if (lane == 0) { st[SE_N] = n_prev + 1.0; status[b] = code; }
+}
+
+__global__ void __launch_bounds__(32 * SL_WARPS) slip_step_kernel(const DevModel* __restrict__ mdl, qmb200_slip_params prm, double process_base_vel, int B,
+                                                                  double dt, const double* __restrict__ sensors, const int32_t* __restrict__ contact,
+                                                                  const double* __restrict__ se, double* __restrict__ state, int32_t* __restrict__ stance,
+                                                                  int32_t* __restrict__ slip, int32_t* __restrict__ status) {
+  __shared__ SlWs s_ws[SL_WARPS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * SL_WARPS + warp;
+  if (b >= B) return;   // the whole warp leaves together
+  SlWs* w = &s_ws[warp];
+  const double* sn = sensors + (size_t)b * QMB200_SENSORS; const double* sx = se + (size_t)b * SE_DBL; double* st = state + (size_t)b * SL_DBL;
+  const int mask = contact[b];
+  const double s0 = sn[lane], s1 = lane + 32 < QMB200_SENSORS ? sn[lane + 32] : 0.0;
+  int code = 0;
+  if (__any_sync(FULL, !(isfinite(s0) && isfinite(s1)))) code = QMB200_ST_NAN;
+  if (code || sx[SE_N] == 0.0) {   // a non-finite reading, or the estimator's next call only places the feet: the contact mask passes through
+    if (lane == 0) { stance[b] = mask; slip[b] = 0; status[b] = code; }
+    return;
+  }
+  double zyx, om; read_legs<false>(mdl, sn, w, lane, zyx, om);
+  __syncwarp();
+
+  // ---- lane f < 4: d^2 of foot f's world velocity u = v- + rd_f under the prior N(v-, Sigma-) of the estimator's next prediction ----
+  double d2 = 0.0; bool bad = false;
+  if (lane < 4) {
+    const int f = lane;
+    double S[9], Si[9], u[3];
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) S[3 * i + j] = sx[SE_P + (i >= j ? tri(3 + i) + 3 + j : tri(3 + j) + 3 + i)];
+      S[4 * i] += dt * process_base_vel + prm.meas_slip;
+      u[i] = sx[SE_X + 3 + i] + dt * w->a[i] + w->rd[f][i];
+    }
+    inv3(S, Si);
+    for (int i = 0; i < 3; ++i) d2 += u[i] * (Si[3 * i] * u[0] + Si[3 * i + 1] * u[1] + Si[3 * i + 2] * u[2]);
+    bad = contact_flag(mask, f) && !isfinite(d2);
+  }
+  if (__any_sync(FULL, bad)) {   // not reached on a finite estimator state (Sigma >= meas_slip 1 > 0); the state is kept
+    if (lane == 0) { stance[b] = mask; slip[b] = 0; status[b] = QMB200_ST_NAN; }
+    return;
+  }
+  // ---- hysteresis: slipping above gate, trusted again after hold consecutive calls below release; a foot out of contact is cleared ----
+  unsigned bit = 0u;
+  if (lane < 4) {
+    const int f = lane;
+    bool sl = ((int)st[SL_MASK] >> (3 - f)) & 1; double hold = st[SL_HOLD + f], onset = st[SL_ONSET + f];
+    if (!contact_flag(mask, f)) { sl = false; hold = 0.0; }
+    else if (sl) {
+      if (d2 < prm.release) { hold += 1.0; if (hold >= (double)prm.hold) { sl = false; hold = 0.0; } }
+      else hold = 0.0;
+    } else if (d2 > prm.gate) { sl = true; hold = 0.0; onset += 1.0; }
+    st[SL_HOLD + f] = hold; st[SL_ONSET + f] = onset;
+    bit = sl ? 1u << (3 - f) : 0u;
+  }
+  const int sm = (int)__reduce_or_sync(FULL, bit);
+  if (lane == 0) { st[SL_MASK] = (double)sm; stance[b] = mask & ~sm; slip[b] = sm; status[b] = 0; }
+}
+
+int launch_slip_step(const DevModel* mdl, const qmb200_slip_params& prm, const qmb200_state_est_params& se_prm, int B, double dt, const double* sensors,
+                     const int32_t* contact, const double* se, double* state, int32_t* stance, int32_t* slip, int32_t* status, cudaStream_t s) {
+  slip_step_kernel<<<(B + SL_WARPS - 1) / SL_WARPS, 32 * SL_WARPS, 0, s>>>(mdl, prm, se_prm.process_base_vel, B, dt, sensors, contact, se, state, stance, slip, status);
+  return 1;
 }
 
 int launch_read_sensors(const qmb200_sensor_params& prm, int B, int64_t robot0, double dt, int64_t sample, const double* q, const double* v, const double* v_prev,

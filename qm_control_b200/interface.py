@@ -568,6 +568,50 @@ class Solver:
         """Release the filter state."""
         self._call("attitude_stop")
 
+    # ---------------- slip detector (include/qmb200.h: qmb200_slip_*; DESIGN.md §4.6) ----------------
+    def slip_get_params(self):
+        """→ dict of qmb200_slip_params."""
+        p = _lib.SlipParams(); self._call("slip_get_params", C.byref(p))
+        return {n: getattr(p, n) for n, _ in _lib.SlipParams._fields_}
+
+    def slip_set_params(self, **params):
+        """Keyword per field of qmb200_slip_params; unspecified fields keep their value."""
+        p = _lib.SlipParams(); self._call("slip_get_params", C.byref(p))
+        names = [n for n, _ in _lib.SlipParams._fields_]
+        for k, v in params.items():
+            if k not in names:
+                raise ValueError("slip_set_params: unknown parameter %r (one of %s)" % (k, ", ".join(names)))
+            if k == "hold" and v != int(v):
+                raise ValueError("slip_set_params: hold must be a whole number of calls, got %r" % (v,))
+            setattr(p, k, int(v) if k == "hold" else float(v))
+        self._call("slip_set_params", C.byref(p))
+
+    def slip_reset(self):
+        """(Re)start the slip detector of every robot: no foot slipping, counters zero.  Synchronous."""
+        self._call("slip_reset")
+
+    def slip_step(self, dt, sensors, contact):
+        """One detector call per robot from sensors [B, 46] and the contact mask [B] → (stance [B], slip [B], status [B]); stance is the mask to pass to
+        state_est_step.  Needs the state estimator running."""
+        B = self.batch; stance = np.zeros(B, dtype=np.int32); slip = np.zeros(B, dtype=np.int32); st = np.zeros(B, dtype=np.int32)
+        sensors, contact = _f64(sensors, (B, _lib.SENSORS)), _i32(contact, (B,))   # held until the call returns
+        self._call("slip_step", float(dt), _p(sensors), _p(contact), _p(stance), _p(slip), _p(st))
+        return stance, slip, st
+
+    def slip_step_dev(self, dt, sensors, contact, stance, slip, status, stream=None):
+        """Device-pointer variant: stance [B], slip [B] and status [B] int32 written; no synchronisation."""
+        self._call("slip_step_dev", float(dt), _p(sensors), _p(contact), _p(stance), _p(slip), _p(status), stream)
+
+    def slip_get(self):
+        """→ dict(mask [B], hold [B, 4] (calls below release while slipping), onsets [B, 4]).  Synchronous."""
+        B = self.batch; m = np.zeros(B, dtype=np.int32); hold = np.zeros((B, 4), dtype=np.int32); on = np.zeros((B, 4), dtype=np.int32)
+        self._call("slip_get", _p(m), _p(hold), _p(on))
+        return dict(mask=m, hold=hold, onsets=on)
+
+    def slip_stop(self):
+        """Release the detector state."""
+        self._call("slip_stop")
+
     # ---------------- utilities ----------------
     def centroidal_state_from_rbd(self, rbd):
         rbd = _f64(rbd); n = rbd.shape[0]; x = np.empty((n, NX))

@@ -4,7 +4,7 @@ Default: 8192 robots, trot at cmd_vel 0.3 m/s, 1 s simulated after a warm-up run
 simulated second, the plant step's device time per call (CUDA events) and its share of the loop, and quality lines (base distance, end-effector
 deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
 
-    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter]]
+    python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter] [--slip-detector]]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -35,6 +35,12 @@ The error percentiles include the wrapped zyx orientation error of rbd_est again
 timed run and the quality lines are then those of the filtered chain.  The JSON line gains "attitude": the filter's device time per call at this batch
 (CUDA events, alternated with blocks of plant steps), and the fallen count and quality lines of the same sweep on the estimate without the filter (one
 more untimed run in the same process).
+
+--slip-detector (with --state-estimator) runs the slip detector before every estimator step (closed_loop.run(slip_detector=True)): the timed run and the
+quality lines are then those of the chain with the detector.  The JSON line gains "slip": the detector's device time per call at this batch (CUDA
+events, alternated with blocks of plant steps); the robots with any foot flagged; and, for the warm-up run (the timed run's twin) and for one more
+untimed run of the same sweep without the detector, the fallen robots, the xy drift of the estimate at the end (p50 / p95) and |v_hat - v| over the run
+from the error watch.  With --vary these come per friction bin as well.
 """
 import argparse
 import json
@@ -188,6 +194,41 @@ def attitude_times(solver, xy_yaw, reps=7, calls=20):
             "spread": [float(min(times["attitude"])), float(max(times["attitude"]))]}
 
 
+def slip_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per slip detector call and per 1 ms plant step of the whole batch, alternated `reps` times in blocks of `calls` from one standing
+    state past the estimator's first call (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev); rbd_est = torch.zeros_like(rbd)
+    sensors = torch.zeros((B, 46), dtype=torch.float64, device=dev); contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    stance, slip = torch.zeros_like(contact), torch.zeros_like(contact)
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+    solver.sim_read_sensors_dev(1e-3, 0, q, v, v, sensors, s.cuda_stream); torch.cuda.synchronize(dev)
+    solver.state_est_reset(q0[:, 0:3]); solver.slip_reset()
+    solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, st, s.cuda_stream)   # past the estimator's first call, before which the mask passes through
+    times = {"slip": [], "plant": []}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode in ("slip", "plant"):
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    if mode == "slip":
+                        solver.slip_step_dev(1e-3, sensors, contact, stance, slip, st, s.cuda_stream)
+                    else:
+                        solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.slip_stop(); solver.state_est_stop()
+    return {"label": "device time per slip detector call and per 1 ms plant step of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            "ms_per_call": float(np.median(times["slip"])), "ms_per_plant_step": float(np.median(times["plant"])),
+            "spread": [float(min(times["slip"])), float(max(times["slip"]))]}
+
+
 def watch_state_est(solver):
     """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
     error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
@@ -221,6 +262,7 @@ def main():
     ap.add_argument("--state-estimator", action="store_true", help="the controller reads the base state estimate from the IMU, encoders and contact flags")
     ap.add_argument("--sensor-noise", choices=["reference"], help="with --state-estimator: the IMU noise of qm_gazebo/config/default.yaml")
     ap.add_argument("--attitude-filter", action="store_true", help="with --state-estimator: filter the IMU orientation before the estimator reads it")
+    ap.add_argument("--slip-detector", action="store_true", help="with --state-estimator: keep slipping stance feet out of the estimate")
     args = ap.parse_args()
     if args.vary and args.terrain:
         ap.error("--vary and --terrain are separate sweeps")
@@ -228,6 +270,8 @@ def main():
         ap.error("--sensor-noise needs --state-estimator")
     if args.attitude_filter and not args.state_estimator:
         ap.error("--attitude-filter needs --state-estimator")
+    if args.slip_detector and not args.state_estimator:
+        ap.error("--slip-detector needs --state-estimator")
     if args.state_estimator and args.terrain:
         ap.error("--state-estimator assumes the plane: it cannot be combined with --terrain")
     import torch
@@ -253,7 +297,8 @@ def main():
         ter = dict(tiles=tiles, cell=T.CELL, tile=idx["ramp_deg"] * 4 + idx["step_rise_m"], origin=T.centred_origin(xy[:, :2]))
         kw = dict(terrain=ter)
     told = {"plant": dict(model_payload="plant"), "estimate": dict(payload_estimator=True), None: {}}[args.model_payload]
-    se = dict(state_estimator=True, sensor_noise=args.sensor_noise, **({"attitude_filter": True} if args.attitude_filter else {})) if args.state_estimator else {}
+    se = dict(state_estimator=True, sensor_noise=args.sensor_noise, **({"attitude_filter": True} if args.attitude_filter else {}),
+              **({"slip_detector": True} if args.slip_detector else {})) if args.state_estimator else {}
     def fresh():
         """with --state-estimator every run starts from a cold MPC and WBC state: a run whose robots fell leaves warm starts the next run must not inherit"""
         if args.state_estimator:
@@ -337,6 +382,27 @@ def main():
                                  "without_filter": {"label": "the same sweep on the estimate, without the attitude filter", "fallen": int(np.sum(~upright(raw))),
                                                     "base_distance_m": pct(n_dist), "ee_max_pos_dev_mm": pct(n_dpos), "ee_max_ori_dev_deg": pct(n_dang),
                                                     "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(raw["status"], axis=0)))}}
+        if args.slip_detector:
+            box2, unwrap2 = watch_state_est(solver)
+            try:
+                fresh(); nodet = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told, **{k: v for k, v in se.items() if k != "slip_detector"})
+            finally:
+                unwrap2()
+            arms = {"with_detector": (warm, mx[:, 1]), "without_detector": (nodet, box2["max"].cpu().numpy()[:, 1])}
+
+            def slip_arm(run, verr, sel):
+                d = np.linalg.norm(run["base_est"][-1, sel, 0:2] - run["base"][-1, sel, 0:2], axis=1)
+                return {"robots": int(np.sum(sel)), "fallen": int(np.sum(~upright(run)[sel])), "xy_drift_m_at_end_p50": float(np.percentile(d, 50)),
+                        "xy_drift_m_at_end_p95": float(np.percentile(d, 95)), "v_abs_m_s_over_run_p50": float(np.percentile(verr[sel], 50)),
+                        "v_abs_m_s_over_run_p95": float(np.percentile(verr[sel], 95)),
+                        **({"robots_flagged": int(np.sum(run["slip"].any(axis=0)[sel]))} if "slip" in run else {})}
+            every = np.ones(B, dtype=bool)
+            extra["slip"] = {**slip_times(solver, xy), "gpu": name, "power_limit": limit, "robots_flagged_timed_run": int(np.sum(r["slip"].any(axis=0))),
+                             "label": "with_detector: the warm-up run (the timed run's twin); without_detector: the same sweep without the detector, in the same process",
+                             **{tag: slip_arm(run, verr, every) for tag, (run, verr) in arms.items()}}
+            if args.vary:
+                extra["slip"]["mu_bins"] = [{"mu": float(val), **{tag: slip_arm(run, verr, idx["mu"] == i) for tag, (run, verr) in arms.items()}}
+                                            for i, val in enumerate(bins["mu"])]
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
@@ -346,7 +412,8 @@ def main():
                                   "min_base_height_m": float(np.min(r["base"][:, :, 2])), "max_abs_roll_pitch_rad": float(np.max(np.abs(r["base"][:, :, 4:6])))},
                       "config": {"workload": "closed loop: %s, cmd_vel %.2f m/s, MPC 100 Hz / WBC 500 Hz / plant 1 kHz (4 substeps), 9 ms command delay" % (args.gait, args.vx),
                                  "batch": B, "simulated_s": sim_s, "warmup": "one run of the same length", **({"model_payload": args.model_payload} if args.model_payload else {}),
-                                 **({"state_estimator": True, "sensor_noise": args.sensor_noise or "none", "attitude_filter": args.attitude_filter} if args.state_estimator else {})},
+                                 **({"state_estimator": True, "sensor_noise": args.sensor_noise or "none", "attitude_filter": args.attitude_filter,
+                                     "slip_detector": args.slip_detector} if args.state_estimator else {})},
                       **extra}))
 
 
