@@ -316,8 +316,9 @@ int qmb200_sim_step_ext_dev(qmb200_handle* h, double duration, const double* eff
  * n = (-gx, -gy, 1) / s, penetration delta = (H - (z - r s)) / s, F_n = max(0, stiffness delta - damping v.n) for delta > 0, v_t = v - (v.n) n, friction
  * as above on v_t; F = F_n n + F_t.  With zero gradient this is the plane law bit for bit, so tile -1 or a constant tile at ground_height changes nothing.
  * No link other than the feet collides; tiles are not rotated.
- * qmb200_sim_set_terrain: heights NULL clears the library and with it the robot terrain.  Rejects n_tiles < 1, nx or ny < 2, a non-finite or
- * non-positive cell, a non-finite height, a library whose byte count overflows, and a library with fewer tiles than a robot references.
+ * qmb200_sim_set_terrain: heights NULL clears the library and with it the robot terrain and the state estimator's ground map.  Rejects n_tiles < 1, nx
+ * or ny < 2, a non-finite or non-positive cell, a non-finite height, a library whose byte count overflows, and a library with fewer tiles than a robot
+ * or the estimator's ground map (qmb200_state_est_set_ground) references.
  * qmb200_sim_set_robot_terrain: tile NULL clears the robot terrain (every robot on the plane); rejects a tile outside [-1, n_tiles) and a non-finite origin.
  * Both are synchronous (they wait for the device); on rejection the stored values stay unchanged. */
 int qmb200_sim_set_terrain(qmb200_handle* h, int32_t n_tiles, int32_t nx, int32_t ny, double cell, const double* heights /*[n_tiles][ny][nx] or NULL: clear*/);
@@ -362,7 +363,8 @@ int qmb200_sim_read_sensors_dev(qmb200_handle* h, double dt, int64_t sample, con
  *      Orientation and angular velocity come from the IMU as read (zyx from the quaternion, yaw in (-pi, pi]; w = R gyro); the legs' kinematics at the
  *      encoder readings give each foot's offset r_i from the base and its velocity.  Predict: p += v dt + a dt^2 / 2, v += a dt with a = R accel + g,
  *      feet constant, P = A P A^T + dt diag(process).  Update with 28 rows: p_base - p_foot_i = -r_i, v_base = -dr_i/dt and p_foot_i,z = foot_height per
- *      foot.  A foot not in contact has its process and measurement variances scaled by swing_scale.  The rows assume the plane: no terrain.
+ *      foot.  A foot not in contact has its process and measurement variances scaled by swing_scale.  The foot-height rows assume the plane
+ *      z = ground_height unless a ground map is set (qmb200_state_est_set_ground below).
  *   process_base_pos, process_base_vel, process_foot    process noise per second: m^2/s, (m/s)^2/s, m^2/s
  *   meas_foot_pos, meas_foot_vel, meas_foot_height      measurement variances: m^2, (m/s)^2, m^2
  *   swing_scale                                         factor on a swing foot's variances
@@ -388,6 +390,17 @@ int qmb200_state_est_get(qmb200_handle* h, double* x /*[B][18]*/, double* p_diag
 /* Releases the filter state.  Step and get fail until the next reset.  Stopping a filter that is not running does nothing and returns 0, as
  * qmb200_payload_est_stop does, so a caller's clean-up may stop unconditionally. */
 int qmb200_state_est_stop(qmb200_handle* h);
+/* The estimator's ground map: per robot a tile of the plant's library (qmb200_sim_set_terrain; -1: the plane) with its node (0, 0) at world origin[b],
+ * as qmb200_sim_set_robot_terrain takes them but held apart from the plant's own rows, so a run may give the estimator a map that differs from the
+ * ground.  With a map, foot f's height row is h_f = p_f,z - H(p_f,x, p_f,y) = s_f (foot_height - ground_height), s_f = sqrt(1 + gx^2 + gy^2): the
+ * plant's contact law holds a stance sphere centre at r - delta along the normal of the local tangent plane.  H and its gradient come from the plant's
+ * lookup at the predicted foot position, ground_height is the plant's when the step is launched, and the row is linearised there (-gx, -gy at the
+ * foot's x and y).  A tile of -1 or a constant tile at ground_height gives the plane's numbers bit for bit.  tile NULL clears the map; rejects a tile
+ * outside [-1, n_tiles) and a non-finite origin.  Synchronous; on rejection the stored map stays unchanged.  The map survives qmb200_state_est_reset
+ * and _stop; qmb200_sim_set_terrain refuses a library without a tile the map references, and clearing the library clears the map. */
+int qmb200_state_est_set_ground(qmb200_handle* h, const int32_t* tile /*[B] or NULL: clear*/, const double* origin /*[B][2]*/);
+/* The ground map; where none is set tile = -1, origin = 0 and is_set = 0.  Any output may be NULL. */
+int qmb200_state_est_get_ground(const qmb200_handle* h, int32_t* tile /*[B]*/, double* origin /*[B][2]*/, int32_t* is_set);
 
 /* ---- attitude filter, between the sensors and the state estimator: a multiplicative (error-state) Kalman filter per robot on SO(3) with gyro-bias
  *      states.  The reference has none (StateEstimateBase::updateImu passes the IMU quaternion through); a real robot's IMU filters on board.

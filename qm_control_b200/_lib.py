@@ -161,6 +161,8 @@ PROTOTYPES = {
     "qmb200_state_est_step_dev": (I32, [P, D] + [P] * 5),
     "qmb200_state_est_get": (I32, [P] * 4),
     "qmb200_state_est_stop": (I32, [P]),
+    "qmb200_state_est_set_ground": (I32, [P] * 3),
+    "qmb200_state_est_get_ground": (I32, [P] * 4),
     "qmb200_attitude_get_params": (I32, [P] * 2),
     "qmb200_attitude_set_params": (I32, [P] * 2),
     "qmb200_attitude_reset": (I32, [P]),

@@ -17,6 +17,7 @@ With state_estimator set, the controller no longer reads the plant's true state:
 the controller side reads (the updates, the targets' end-effector state, the payload estimator).  The plant and the record keep the truth.
 With attitude_filter set as well, an attitude filter (Solver.attitude_*) rewrites each reading's orientation and gyro columns before the estimator reads them.
 With slip_detector set as well, a slip detector (Solver.slip_*) removes the stance feet that slide from the contact mask the estimator reads.
+On terrain the estimator needs ground_map, its own map of the run's tile library (Solver.state_est_set_ground); the controller still sees no terrain.
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  The mode schedule is
 tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -50,7 +51,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None):
+        attitude_filter=None, slip_detector=None, ground_map=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -70,7 +71,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     state_estimator: True, or a dict of qmb200_state_est_params overrides (Solver.state_est_set_params), closes the loop on estimated base states: after
     every plant step (1 ms step k) the sensors are read with sample = k (-1 for the reading of the start) and the estimator steps; update_dev, the
     targets' end-effector state and the payload estimator read its rbd_est.  It starts at the plant's start position.  Its status is OR-ed into the
-    record's.  Not with terrain: the estimator's foot-height rows assume the plane.
+    record's.  With terrain only together with ground_map: the estimator's foot-height rows assume the plane otherwise.
     sensor_noise: None (noise-free readings), "reference" (_lib.SENSOR_NOISE_REFERENCE, the IMU covariances of qm_gazebo/config/default.yaml) or a dict
     of qmb200_sensor_params overrides; only with state_estimator.  The estimator is stopped and the previous sensor and estimator parameters restored
     when run returns.
@@ -81,6 +82,10 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     slip_detector: True, or a dict of qmb200_slip_params overrides (Solver.slip_set_params); only with state_estimator.  After every sensor reading
     (and attitude filter step) a detector step turns the plant's contact mask into the mask of trusted stance feet, and the estimator steps on that
     mask.  Its status is OR-ed into the record's.  The detector is stopped and its previous parameters restored when run returns.
+    ground_map: True, or dict(tile [B], origin [B, 2]); needs state_estimator and terrain.  The estimator's ground map for this run
+    (Solver.state_est_set_ground), on this run's tile library: True gives it the run's own terrain rows (a perfect map), a dict rows of its own (a
+    wrong tile, a shifted origin).  Its foot-height rows then follow the mapped ground under each foot.  The controller still does not see the terrain.
+    The previous map is restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
@@ -94,8 +99,12 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         raise ValueError("closed_loop.run: sensor_noise must be None, \"reference\" or a dict of sensor parameters, got %r" % (sensor_noise,))
     if sensor_noise is not None and state_estimator is None:
         raise ValueError("closed_loop.run: sensor_noise needs state_estimator (the controller reads the plant's true state otherwise)")
-    if state_estimator is not None and terrain is not None:
-        raise ValueError("closed_loop.run: state_estimator does not support terrain (its foot-height rows assume the plane)")
+    if ground_map is not None and ground_map is not True and not isinstance(ground_map, dict):
+        raise ValueError("closed_loop.run: ground_map must be None, True or dict(tile, origin), got %r" % (ground_map,))
+    if ground_map is not None and (state_estimator is None or terrain is None):
+        raise ValueError("closed_loop.run: ground_map needs state_estimator and terrain (it maps the run's tile library for the estimator)")
+    if state_estimator is not None and terrain is not None and ground_map is None:
+        raise ValueError("closed_loop.run: state_estimator on terrain needs ground_map (without one its foot-height rows assume the plane)")
     if attitude_filter is not None and attitude_filter is not True and not isinstance(attitude_filter, dict):
         raise ValueError("closed_loop.run: attitude_filter must be None, True or a dict of attitude filter parameters, got %r" % (attitude_filter,))
     if attitude_filter is not None and state_estimator is None:
@@ -108,6 +117,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     with contextlib.ExitStack() as scope:
         if terrain is not None:
             scope.enter_context(_terrain(solver, terrain))
+        if ground_map is not None:
+            scope.enter_context(_ground_map(solver, terrain if ground_map is True else ground_map))
         if model_payload is not None:
             scope.enter_context(_model_payload(solver, model_payload, payload))
         if payload_estimator is not None:
@@ -141,6 +152,18 @@ def _terrain(solver, terrain):
             solver.sim_set_terrain(**prev_lib)
         if prev_robot is not None:
             solver.sim_set_robot_terrain(**prev_robot)
+
+
+@contextlib.contextmanager
+def _ground_map(solver, rows):
+    prev = solver.state_est_get_ground()   # entered after _terrain: the previous map has survived its library change
+    try:
+        solver.state_est_set_ground(rows["tile"], rows["origin"])
+        yield
+    finally:
+        solver.state_est_set_ground(None)
+        if prev is not None:
+            solver.state_est_set_ground(**prev)
 
 
 @contextlib.contextmanager

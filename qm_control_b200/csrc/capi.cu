@@ -66,6 +66,7 @@ struct qmb200_handle {
   qmb200_payload_est_params est_prm{}; double* d_est = nullptr;   // payload estimator (capi_est.inc): parameters and state [B][EST_DBL], NULL when not running
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
   qmb200_state_est_params se_prm{}; double* d_se = nullptr;        // base state estimator: parameters and state [B][SE_DBL], NULL when not running
+  RobotArray se_ground{3};        // the estimator's ground map: per-robot [tile, origin_x, origin_y] on the tile library (qmb200_state_est_set_ground)
   qmb200_attitude_params at_prm{}; double* d_at = nullptr;         // attitude filter (capi_attitude.inc): parameters and state [B][AT_DBL], NULL when not running
   qmb200_slip_params sl_prm{}; double* d_sl = nullptr;             // slip detector (capi_slip.inc): parameters and state [B][SL_DBL], NULL when not running
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read

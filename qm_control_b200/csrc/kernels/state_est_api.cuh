@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include "dev_common.cuh"
+#include "sim_api.cuh"
 #include "../../../include/qmb200.h"
 
 namespace qmb {
@@ -37,8 +38,9 @@ constexpr int SE_X = 0, SE_P = SE_X + SE_NX, SE_N = SE_P + SE_TRI, SE_DBL = SE_N
 // sensors of robots [0, B) at the plant state (q, v) after a step of dt seconds that started at velocity v_prev; robot b draws its noise as robot robot0 + b
 int launch_read_sensors(const qmb200_sensor_params& prm, int B, int64_t robot0, double dt, int64_t sample, const double* q, const double* v, const double* v_prev,
                         double* sensors, cudaStream_t s);
-// one filter call per robot from sensors [B][46] and the contact mask [B]; writes rbd_est [B][55] and status [B]
+// one filter call per robot from sensors [B][46] and the contact mask [B]; writes rbd_est [B][55] and status [B].  map: the estimator's ground map on
+// the plant's tile library (map.robot [B][3] = [tile, origin_x, origin_y]; NULL: every foot-height row on the plane), ground_height: the plant's plane
 int launch_state_est_step(const DevModel* mdl, const qmb200_state_est_params& prm, int B, double dt, const double* sensors, const int32_t* contact, double* state,
-                          double* rbd_est, int32_t* status, cudaStream_t s);
+                          double* rbd_est, int32_t* status, const SimTerrain& map, double ground_height, cudaStream_t s);
 
 }  // namespace qmb

@@ -16,6 +16,11 @@
 //                foot's variances scaled by swing_scale.  Every row of C is +1 at column a_r and -1 at column b_r (or nothing), so P C^T and
 //                S = C P C^T + R are gathered from P by index; S by the warp Cholesky, K = P C^T S^-1 (one lane per row of K), x += K (y - C x),
 //                P -= K C P symmetrised
+//   ground map   (optional, per robot a tile of the plant's library and its origin) foot f's height row becomes h_f(x) = p_f,z - H(p_f,x, p_f,y) =
+//                s_f c with c = foot_height - ground_height and s_f = sqrt(1 + gx_f^2 + gy_f^2): the plant holds a stance sphere centre at r - delta
+//                along the normal of the local tangent plane.  H, g = (gx, gy) and s come from ground_at (sim_api.cuh) at the predicted foot xy,
+//                and the row of C gains -gx_f, -gy_f at p_f,x, p_f,y; G = P C^T and S pick up those two terms, K and the updates are unchanged.
+//                A tile of -1 is the plane row.
 // The first call after a reset only places the feet at p + r_i.  rbd_est[55] = [zyx, p, joints, w, v, joint rates, end-effector pose].
 // status: QMB200_ST_NAN for a non-finite input (nothing is written) or update (x and P are kept); QMB200_ST_NOT_PD when S fails the Cholesky (x and P are
 // kept).  rbd_est is written in both of the last two cases, from the kept state.
@@ -27,6 +32,8 @@
 // contact, so a slipping foot is handled as a swing foot.  Before the estimator's first call after its reset (SE_N = 0) and on a non-finite reading
 // (QMB200_ST_NAN) the contact mask passes through and the detector's state is untouched.
 #include "state_est_api.cuh"
+#include <type_traits>
+
 #include "slip_api.cuh"
 #include "rbd.cuh"
 #include "wlinalg.cuh"
@@ -48,6 +55,10 @@ struct SeWs {
   double K[SE_NX][SE_NY + 1];
   double S[SE_STRI];          // C P C^T + R, packed lower, then its Cholesky factor
   double e[SE_NY];            // innovation y - C x
+};
+// with a ground map: per foot f the ground under its predicted position, (H_f, gx_f, gy_f, s_f = sqrt(1 + gx_f^2 + gy_f^2))
+struct SeWsMap : SeWs {
+  double hg[4][4];
 };
 
 // columns of measurement row r: +1 at a_r, -1 at b_r (b_r < 0: none)
@@ -144,13 +155,17 @@ __global__ void read_sensors_kernel(qmb200_sensor_params prm, int B, int64_t rob
   }
 }
 
+// MAP: compiled once with the ground map's foot-height rows and once for the plane alone (map.robot == NULL), which keeps the plane's code as it was.
+template <bool MAP>
 __global__ void __launch_bounds__(32 * SE_WARPS) state_est_step_kernel(const DevModel* __restrict__ mdl, qmb200_state_est_params prm, int B, double dt,
                                                                        const double* __restrict__ sensors, const int32_t* __restrict__ contact,
-                                                                       double* __restrict__ state, double* __restrict__ rbd_est, int32_t* __restrict__ status) {
-  __shared__ SeWs s_ws[SE_WARPS];
+                                                                       double* __restrict__ state, double* __restrict__ rbd_est, int32_t* __restrict__ status,
+                                                                       SimTerrain map, double ground_height) {
+  using Ws = typename std::conditional<MAP, SeWsMap, SeWs>::type;
+  __shared__ Ws s_ws[SE_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * SE_WARPS + warp;
   if (b >= B) return;   // the whole warp leaves together
-  SeWs* w = &s_ws[warp];
+  Ws* w = &s_ws[warp];
   const double* sn = sensors + (size_t)b * QMB200_SENSORS; double* st = state + (size_t)b * SE_DBL; double* out = rbd_est + (size_t)b * QMB200_RBD;
   const double s0 = sn[lane], s1 = lane + 32 < QMB200_SENSORS ? sn[lane + 32] : 0.0;
   if (__any_sync(FULL, !(isfinite(s0) && isfinite(s1)))) { if (lane == 0) status[b] = QMB200_ST_NAN; return; }   // dt: checked by the API
@@ -191,18 +206,41 @@ __global__ void __launch_bounds__(32 * SE_WARPS) state_est_step_kernel(const Dev
     for (int h = 0; h < 6; ++h) { const int t = lane + 32 * h; if (t < SE_TRI) w->P[t] = pn[h]; }
     if (lane < SE_NX) w->x[lane] = xn;
     __syncwarp();
+    if constexpr (MAP) {   // the ground under each foot's predicted (= stored) position, from the plant's lookup
+      if (lane < 4) {
+        const int f = lane; double H, gx, gy;
+        ground_at(map, map.robot + (size_t)b * 3, ground_height, w->x[6 + 3 * f], w->x[7 + 3 * f], H, gx, gy);
+        w->hg[f][0] = H; w->hg[f][1] = gx; w->hg[f][2] = gy; w->hg[f][3] = sqrt(1.0 + gx * gx + gy * gy);
+      }
+      __syncwarp();
+    }
 
     // ---- update: G = P C^T, S = C G + R, e = y - C x ----
-    for (int t = lane; t < SE_NX * SE_NY; t += 32) { const int j = t / SE_NY, r = t % SE_NY; w->G[j][r] = pk(w->P, j, col_a(r)) - gpk(w->P, j, col_b(r)); }
+    // With a map, height row 24 + f is h_f(x) = p_f,z - H(p_f,x, p_f,y) = s_f c, c = foot_height - ground_height: its row of C adds -gx_f at p_f,x and
+    // -gy_f at p_f,y to the +1 at p_f,z.  A zero gradient and H = ground_height give the plane's numbers bit for bit.
+    for (int t = lane; t < SE_NX * SE_NY; t += 32) {
+      const int j = t / SE_NY, r = t % SE_NY;
+      double g = pk(w->P, j, col_a(r)) - gpk(w->P, j, col_b(r));
+      if constexpr (MAP) {
+        if (r >= 24) { const int f = r - 24; g -= w->hg[f][1] * pk(w->P, j, 6 + 3 * f) + w->hg[f][2] * pk(w->P, j, 7 + 3 * f); }
+      }
+      w->G[j][r] = g;
+    }
     if (lane < SE_NY) {
       const int r = lane, f = row_foot(r), a = col_a(r), bb = col_b(r);
-      const double yr = r < 12 ? -w->r[f][r % 3] : (r < 24 ? -w->rd[f][(r - 12) % 3] : prm.foot_height);
+      double yr = r < 12 ? -w->r[f][r % 3] : (r < 24 ? -w->rd[f][(r - 12) % 3] : prm.foot_height);
+      if constexpr (MAP) {   // y_f - H_f = s_f c - H_f written so that H_f = ground_height, s_f = 1 leaves foot_height
+        if (r >= 24) yr = prm.foot_height + (w->hg[f][0] - ground_height) + (w->hg[f][3] - 1.0) * (prm.foot_height - ground_height);
+      }
       w->e[r] = yr - (w->x[a] - (bb < 0 ? 0.0 : w->x[bb]));
     }
     __syncwarp();
     for (int t = lane; t < SE_STRI; t += 32) {
       const int r = tri_row(t), c = t - tri(r), bb = col_b(r);
       double s = w->G[col_a(r)][c] - (bb < 0 ? 0.0 : w->G[bb][c]);
+      if constexpr (MAP) {
+        if (r >= 24) { const int f = r - 24; s -= w->hg[f][1] * w->G[6 + 3 * f][c] + w->hg[f][2] * w->G[7 + 3 * f][c]; }
+      }
       if (r == c) s += (r < 12 ? prm.meas_foot_pos : (r < 24 ? prm.meas_foot_vel : prm.meas_foot_height)) * (contact_flag(mask, row_foot(r)) ? 1.0 : prm.swing_scale);
       w->S[t] = s;
     }
@@ -315,8 +353,10 @@ int launch_read_sensors(const qmb200_sensor_params& prm, int B, int64_t robot0, 
   return 1;
 }
 int launch_state_est_step(const DevModel* mdl, const qmb200_state_est_params& prm, int B, double dt, const double* sensors, const int32_t* contact, double* state,
-                          double* rbd_est, int32_t* status, cudaStream_t s) {
-  state_est_step_kernel<<<(B + SE_WARPS - 1) / SE_WARPS, 32 * SE_WARPS, 0, s>>>(mdl, prm, B, dt, sensors, contact, state, rbd_est, status);
+                          double* rbd_est, int32_t* status, const SimTerrain& map, double ground_height, cudaStream_t s) {
+  const int grid = (B + SE_WARPS - 1) / SE_WARPS;
+  if (map.robot) state_est_step_kernel<true><<<grid, 32 * SE_WARPS, 0, s>>>(mdl, prm, B, dt, sensors, contact, state, rbd_est, status, map, ground_height);
+  else state_est_step_kernel<false><<<grid, 32 * SE_WARPS, 0, s>>>(mdl, prm, B, dt, sensors, contact, state, rbd_est, status, map, ground_height);
   return 1;
 }
 

@@ -527,6 +527,23 @@ class Solver:
         """Release the estimator state."""
         self._call("state_est_stop")
 
+    def state_est_set_ground(self, tile=None, origin=None):
+        """The estimator's ground map on the plant's tile library: tile [B] (-1: the plane; a scalar is broadcast) with its node (0, 0) at world
+        origin [B, 2] (default zeros), held apart from the plant's robot terrain.  None clears it.  It survives state_est_reset and state_est_stop.
+        Synchronous."""
+        B = self.batch
+        if tile is None:
+            self._call("state_est_set_ground", None, None); return
+        t = _i32(np.broadcast_to(np.asarray(tile), (B,)), (B,))
+        o = _f64(np.zeros((B, 2)) if origin is None else np.broadcast_to(np.asarray(origin, dtype=np.float64), (B, 2)), (B, 2))
+        self._call("state_est_set_ground", _p(t), _p(o))
+
+    def state_est_get_ground(self):
+        """→ dict(tile [B], origin [B, 2]), or None when no ground map is set."""
+        t = np.zeros(self.batch, dtype=np.int32); o = np.zeros((self.batch, 2)); is_set = C.c_int32()
+        self._call("state_est_get_ground", _p(t), _p(o), C.byref(is_set))
+        return dict(tile=t, origin=o) if is_set.value else None
+
     # ---------------- attitude filter (include/qmb200.h: qmb200_attitude_*; DESIGN.md §4.6) ----------------
     def attitude_get_params(self):
         """→ dict of qmb200_attitude_params."""

@@ -30,6 +30,9 @@ this batch (CUDA events, alternated with blocks of plant steps); percentiles ove
 end) and of the xy drift at the end (taken in the warm-up run, which is the timed run's twin); and the quality lines of a ground-truth run of the same
 sweep (one more untimed run in the same process).  Each of these runs starts from a cold MPC and WBC state (Solver.mpc_reset, wbc_set_input_last).
 The error percentiles include the wrapped zyx orientation error of rbd_est against the plant (the largest of the three angles).
+With --terrain the estimator runs on a perfect ground map (closed_loop.run(ground_map=True)), and "terrain" gains "state_est": per ramp and step bin
+the fallen robots of the estimate arm and of the true-state arm and |z_hat - z| p50 / p95 over the run, and the estimator step's device time at this
+batch with the map and without it (CUDA events, alternated).
 
 --attitude-filter (with --state-estimator) runs the attitude filter between the sensors and the estimator (closed_loop.run(attitude_filter=True)): the
 timed run and the quality lines are then those of the filtered chain.  The JSON line gains "attitude": the filter's device time per call at this batch
@@ -161,6 +164,41 @@ def state_est_times(solver, xy_yaw, reps=7, calls=20):
             "spread": [float(min(times["estimator"])), float(max(times["estimator"]))]}
 
 
+def ground_map_times(solver, ter, xy_yaw, reps=7, calls=20):
+    """Device time per estimator step of the whole batch with the sweep's terrain as the estimator's ground map and without a map, alternated `reps`
+    times in blocks of `calls` from one terrain standing state past the estimator's first call (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    solver.sim_set_terrain(ter["tiles"], ter["cell"]); solver.sim_set_robot_terrain(ter["tile"], ter["origin"])
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev); rbd_est = torch.zeros_like(rbd)
+    sensors = torch.zeros((B, 46), dtype=torch.float64, device=dev); contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)
+    solver.sim_read_sensors_dev(1e-3, 0, q, v, v, sensors, s.cuda_stream); torch.cuda.synchronize(dev)
+    solver.state_est_reset(q0[:, 0:3]); solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, st, s.cuda_stream)   # past the first call
+    times = {"map": [], "plane": []}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode in ("map", "plane"):
+                if mode == "map":
+                    solver.state_est_set_ground(ter["tile"], ter["origin"])
+                else:
+                    solver.state_est_set_ground(None)
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    solver.state_est_step_dev(1e-3, sensors, contact, rbd_est, st, s.cuda_stream)
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.state_est_stop(); solver.sim_set_terrain(None)
+    return {"label": "device time per estimator step of %d robots with the ground map and without, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            "ms_per_call_map": float(np.median(times["map"])), "ms_per_call_plane": float(np.median(times["plane"])),
+            "spread_map": [float(min(times["map"])), float(max(times["map"]))], "spread_plane": [float(min(times["plane"])), float(max(times["plane"]))]}
+
+
 def attitude_times(solver, xy_yaw, reps=7, calls=20):
     """Device time per attitude filter call and per 1 ms plant step of the whole batch, alternated `reps` times in blocks of `calls` from one standing
     state (CUDA events) → median ms per call of each."""
@@ -272,8 +310,6 @@ def main():
         ap.error("--attitude-filter needs --state-estimator")
     if args.slip_detector and not args.state_estimator:
         ap.error("--slip-detector needs --state-estimator")
-    if args.state_estimator and args.terrain:
-        ap.error("--state-estimator assumes the plane: it cannot be combined with --terrain")
     import torch
     import qm_control_b200 as q
     from qm_control_b200 import closed_loop
@@ -298,7 +334,7 @@ def main():
         kw = dict(terrain=ter)
     told = {"plant": dict(model_payload="plant"), "estimate": dict(payload_estimator=True), None: {}}[args.model_payload]
     se = dict(state_estimator=True, sensor_noise=args.sensor_noise, **({"attitude_filter": True} if args.attitude_filter else {}),
-              **({"slip_detector": True} if args.slip_detector else {})) if args.state_estimator else {}
+              **({"slip_detector": True} if args.slip_detector else {}), **({"ground_map": True} if args.terrain else {})) if args.state_estimator else {}
     def fresh():
         """with --state-estimator every run starts from a cold MPC and WBC state: a run whose robots fell leaves warm starts the next run must not inherit"""
         if args.state_estimator:
@@ -375,8 +411,20 @@ def main():
                               "fallen": int(np.sum(~upright(r))), "fallen_warmup": int(np.sum(~upright(warm))), "ground_truth": {"label": "the same sweep, controller reading the plant's true state", "fallen": int(np.sum(~upright(truth))),
                                                                                     "base_distance_m": pct(t_dist), "ee_max_pos_dev_mm": pct(t_dpos), "ee_max_ori_dev_deg": pct(t_dang),
                                                                                     "robots_with_status_bits": int(np.count_nonzero(np.bitwise_or.reduce(truth["status"], axis=0)))}}
+        if args.terrain:
+            def fallen(run):
+                base = run["base"]; ground = T.height(ter["tiles"], ter["cell"], ter["tile"][None], ter["origin"][None], base[:, :, :2])
+                return ~(np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2] - ground, axis=0) > 0.3) & (np.max(np.abs(base[:, :, 4:6]), axis=(0, 2)) < 0.3))
+            f_est, f_truth = fallen(warm), fallen(truth)
+            extra["terrain"]["state_est"] = {
+                "label": "per bin: the estimate arm (the warm-up run, the timed run's twin, the estimator on a perfect ground map) and the true-state arm of the "
+                         "same sweep; |z_hat - z| over the run from the error watch", **ground_map_times(solver, ter, xy), "gpu": name, "power_limit": limit,
+                "bins": {axis: [{"value": float(val), "robots": int(np.sum(idx[axis] == i)), "fallen_estimate": int(np.sum(f_est[idx[axis] == i])),
+                                 "fallen_truth": int(np.sum(f_truth[idx[axis] == i])), "z_abs_m_over_run_p50": float(np.percentile(mx[idx[axis] == i, 0], 50)),
+                                 "z_abs_m_over_run_p95": float(np.percentile(mx[idx[axis] == i, 0], 95))} for i, val in enumerate(bins[axis])] for axis in bins}}
         if args.attitude_filter:
-            fresh(); raw = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told, state_estimator=True, sensor_noise=args.sensor_noise)
+            fresh(); raw = closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw, **told, state_estimator=True, sensor_noise=args.sensor_noise,
+                                           **({"ground_map": True} if args.terrain else {}))
             n_dist, n_dpos, n_dang = quality(raw)
             extra["attitude"] = {**attitude_times(solver, xy), "gpu": name, "power_limit": limit,
                                  "without_filter": {"label": "the same sweep on the estimate, without the attitude filter", "fallen": int(np.sum(~upright(raw))),
