@@ -219,6 +219,45 @@ int qmb200_gait_insert_template(qmb200_gait* g, const char* gait_file, const cha
 /* GaitSchedule::getModeSchedule(lowerBoundTime, upperBoundTime): returns the number of events written (<= EMAX) or negative */
 int qmb200_gait_get_mode_schedule(qmb200_gait* g, double lower_bound_time, double upper_bound_time, double* event_times /*[EMAX]*/, int32_t* mode_sequence /*[EMAX+1]*/);
 
+/* ---- device gait front-end: the GaitSchedule protocol above for every robot of the handle, on the device, rolled once per MPC tick so that a
+ *      closed loop can switch gaits per robot without a host synchronisation (DESIGN.md §4.7).  Each robot holds a schedule of at most
+ *      QMB200_GAIT_CAP events, its active template and a cursor into its own command timeline.  The arithmetic is that of qmb200_gait_insert_template /
+ *      qmb200_gait_get_mode_schedule: a robot's windows equal, bit for bit, those of a qmb200_gait object driven through the same protocol. */
+#define QMB200_GAIT_CAP 64    /* events of one robot's schedule while a step works on it */
+#define QMB200_GAIT_MAXM 16   /* modes of one template */
+/* The template table: templates names[0..n) of gait_file, in that order (a template's id is its index).  Rejects a name the file lacks, more than
+ * QMB200_GAIT_MAXM modes and switching times that are not finite and strictly increasing.  Fails while the schedule runs (qmb200_gait_dev_stop first). */
+int qmb200_gait_dev_set_templates(qmb200_handle* h, const char* gait_file, const char* const* names, int32_t n);
+/* (Re)starts every robot's schedule: what qmb200_gait_create builds (reference.info's initialModeSchedule, task.info's phaseTransitionStanceTime)
+ * followed by qmb200_gait_insert_template(template[b], t_start[b], T) with T the handle's time horizon: stance until t_start, then the template.
+ * Clears the command timeline.  Rejects a template outside the table and a non-finite t_start.  Synchronous. */
+int qmb200_gait_dev_reset(qmb200_handle* h, const int32_t* tmpl /*[B]*/, const double* t_start /*[B]*/);
+/* The command timeline, n_cmd commands per robot (host arrays, copied): robot b's command c is due at t[b][c] (same clock as t_obs; sorted per robot,
+ * +inf pads), inserts template tmpl[b][c] (-1: none) and sets cmd_vel[b][c] (vx, vy, vz, yaw rate; a NaN row: none).  Every cursor goes back to 0;
+ * n_cmd = 0 clears the timeline.  Rejects a NaN time, unsorted times, a template outside [-1, n_templates) and a cmd_vel row neither finite nor all
+ * NaN.  Synchronous. */
+int qmb200_gait_dev_set_commands(qmb200_handle* h, int32_t n_cmd, const double* t /*[B][n_cmd]*/, const int32_t* tmpl /*[B][n_cmd]*/, const double* cmd_vel /*[B][n_cmd][4]*/);
+/* One step per robot at t = t_obs[b], right before the MPC tick's target_trajectories: (1) every command of the robot due at t (time <= t) and not yet
+ * applied, in order: a template is inserted with qmb200_gait_insert_template's arithmetic at (t + T, T) (GaitReceiver::preSolverRun: start = the
+ * solve's final time, final = the time horizon), a cmd_vel row is written to cmd[b][0:4] (the target front-end's cmd[B][7]); (2) the window
+ * getModeSchedule(t - T, t + 2T) is written to the MPC problem rows n_events[b], event_times[b][EMAX] (0 past the count) and modes[b][EMAX+1] (stance
+ * past the count).  All or nothing per robot: status QMB200_ST_NAN (non-finite t) or QMB200_ST_OVERFLOW (the window would hold more than QMB200_EMAX
+ * events, where qmb200_gait_get_mode_schedule returns -2, or the schedule more than QMB200_GAIT_CAP) leaves the robot's schedule, cursor, MPC rows and
+ * cmd row as they were, so its due commands are applied by a later step.  status [B] is written, not OR-ed; tmpl [B] (active template) and mode [B]
+ * (the stored schedule's mode at t, as the MPC reads it) are written when non-NULL. */
+int qmb200_gait_dev_step(qmb200_handle* h, const double* t_obs /*[B]*/, int32_t* n_events /*[B] in-out*/, double* event_times /*[B][EMAX] in-out*/,
+                         int32_t* mode_sequence /*[B][EMAX+1] in-out*/, double* cmd /*[B][7] in-out*/, int32_t* tmpl /*[B] or NULL*/, int32_t* mode /*[B] or NULL*/,
+                         int32_t* status /*[B]*/);
+int qmb200_gait_dev_step_dev(qmb200_handle* h, const double* t_obs, int32_t* n_events, double* event_times, int32_t* mode_sequence, double* cmd, int32_t* tmpl,
+                             int32_t* mode, int32_t* status, void* cuda_stream);
+/* Synchronous: each robot's stored schedule (count, event times [B][GAIT_CAP] with 0 past the count, modes [B][GAIT_CAP+1] with stance past it), active
+ * template and cursor.  Any output may be NULL. */
+int qmb200_gait_dev_get(qmb200_handle* h, int32_t* n_events /*[B]*/, double* event_times /*[B][QMB200_GAIT_CAP]*/, int32_t* mode_sequence /*[B][QMB200_GAIT_CAP+1]*/,
+                        int32_t* tmpl /*[B]*/, int32_t* cursor /*[B]*/);
+/* Releases the schedules and the timeline; the template table stays.  Step and get fail until the next reset.  Stopping a schedule that is not
+ * running does nothing and returns 0. */
+int qmb200_gait_dev_stop(qmb200_handle* h);
+
 /* ---- controller side of the path (SURVEY.md section 8f): the steps of QMController::update around evaluatePolicy / WbcBase::update and the
  *      publisher that feeds the solver, batched on the device.  The caller owns the per-robot controller state these functions read and
  *      write (the members of QMController / QmTargetTrajectoriesInteractiveMarker they mirror); `_dev` variants take device pointers. */

@@ -8,6 +8,7 @@ LIB_PATH = os.environ.get("QMB200_LIB", os.path.join(HERE, "libqmb200.so"))   # 
 ASSETS = os.path.join(ROOT, "assets")
 
 NX, NU, RBD, CMD, TARGET, EMAX, KMAX = 30, 30, 55, 54, 37, 32, 4
+GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
 
 dp = C.POINTER(C.c_double)
 ip = C.POINTER(C.c_int32)
@@ -126,6 +127,13 @@ PROTOTYPES = {
     "qmb200_gait_destroy": (None, [P]),
     "qmb200_gait_insert_template": (I32, [P, S, S, D, D]),
     "qmb200_gait_get_mode_schedule": (I32, [P, D, D, P, P]),
+    "qmb200_gait_dev_set_templates": (I32, [P, S, P, I32]),
+    "qmb200_gait_dev_reset": (I32, [P] * 3),
+    "qmb200_gait_dev_set_commands": (I32, [P, I32] + [P] * 3),
+    "qmb200_gait_dev_step": (I32, [P] * 9),
+    "qmb200_gait_dev_step_dev": (I32, [P] * 10),
+    "qmb200_gait_dev_get": (I32, [P] * 6),
+    "qmb200_gait_dev_stop": (I32, [P]),
     "qmb200_observation_update": (I32, [P] * 5),
     "qmb200_observation_update_dev": (I32, [P] * 6),
     "qmb200_target_trajectories": (I32, [P, I32] + [P] * 8),

@@ -18,6 +18,7 @@
 #include "kernels/state_est_api.cuh"
 #include "kernels/attitude_api.cuh"
 #include "kernels/slip_api.cuh"
+#include "kernels/gait_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -42,7 +43,7 @@ struct qmb200_handle {
   DevModel* d_model = nullptr;
   int B = 0, nmax = 0, variant = 0, device = 0;
   cudaStream_t stream = nullptr;
-  std::string err, task_file;   // task_file: qmb200_mpc_set_solver re-reads the sqp{} / ipm{} / ddp{} block
+  std::string err, task_file, reference_file;   // task_file: qmb200_mpc_set_solver re-reads the sqp{} / ipm{} / ddp{} block; both: qmb200_gait_dev_reset
   int64_t launches = 0;
   // intermediates of the tick and update chains (policy evaluation → WBC → control law), WBC state, and the update chain's safety word
   double *d_xdes = nullptr, *d_udes = nullptr, *d_input_last = nullptr;
@@ -69,6 +70,10 @@ struct qmb200_handle {
   RobotArray se_ground{3};        // the estimator's ground map: per-robot [tile, origin_x, origin_y] on the tile library (qmb200_state_est_set_ground)
   qmb200_attitude_params at_prm{}; double* d_at = nullptr;         // attitude filter (capi_attitude.inc): parameters and state [B][AT_DBL], NULL when not running
   qmb200_slip_params sl_prm{}; double* d_sl = nullptr;             // slip detector (capi_slip.inc): parameters and state [B][SL_DBL], NULL when not running
+  struct {   // device gait schedule (capi_gait.inc): template table, per-robot state (NULL when not running) and command timeline [B][n_cmd]
+    std::vector<GsTemplate> table; GsTemplate* d_table = nullptr; GsRobot* d_robots = nullptr; int32_t* d_cursor = nullptr;
+    double* d_t = nullptr; int32_t* d_tmpl = nullptr; double* d_vel = nullptr; int n_cmd = 0; double stance_time = 0.0;
+  } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
@@ -178,7 +183,7 @@ int qmb200_create(const qmb200_config* cfg, qmb200_handle** out) {
     h->target_prm.target_rotation_velocity = ref.number("targetRotationVelocity"); h->target_prm.time_to_target = task.number("mpc.timeHorizon");
     for (int j = 0; j < NJ; ++j) h->target_prm.default_joint_state[j] = h->hm.default_joint_state[j];
   } catch (const std::exception& e) { g_create_error = e.what(); delete h; return -2; }
-  h->task_file = cfg->task_file;
+  h->task_file = cfg->task_file; h->reference_file = cfg->reference_file;
   h->sim_prm = default_sim_params(); h->est_prm = default_est_params(); h->se_prm = default_state_est_params(h->hm.dev); h->at_prm = default_attitude_params();
   h->sl_prm = default_slip_params();
   h->B = cfg->batch; h->variant = cfg->wbc_variant; h->device = cfg->device; h->law_prm.variant = cfg->wbc_variant == QMB200_WBC_HIERARCHICAL_MPC ? 1 : 0;
@@ -212,6 +217,7 @@ void qmb200_destroy(qmb200_handle* h) {
   if (h->d_se) cudaFree(h->d_se);
   if (h->d_at) cudaFree(h->d_at);
   if (h->d_sl) cudaFree(h->d_sl);
+  cudaFree(h->gs.d_table); cudaFree(h->gs.d_robots); cudaFree(h->gs.d_cursor); cudaFree(h->gs.d_t); cudaFree(h->gs.d_tmpl); cudaFree(h->gs.d_vel);
   delete h;
 }
 
@@ -366,3 +372,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_state_est.inc"
 #include "capi_attitude.inc"
 #include "capi_slip.inc"
+#include "capi_gait.inc"

@@ -1,0 +1,101 @@
+// Device gait schedule (gait_kernel.cu): per robot, ocs2::legged_robot::GaitSchedule as the host object qmb200_gait keeps it (capi_mpc.inc), on
+// fixed-capacity arrays, with a timeline of gait and cmd_vel commands, rolled once per MPC tick (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7).
+// The core (gs_*) is host + device: tests/gait_host.cpp compiles it with g++ and checks it against the host objects on the CPU.  Its arithmetic is
+// that of qmb200_gait_insert_template / qmb200_gait_get_mode_schedule: the event times come out bit for bit equal.
+#pragma once
+#include "dev_common.cuh"
+#include "../../../include/qmb200.h"
+
+namespace qmb {
+
+constexpr int GS_MAXM = QMB200_GAIT_MAXM;   // modes of one template
+constexpr int GS_CAP = QMB200_GAIT_CAP;     // events of one robot's schedule while a step works on it (a window holds at most QMB200_EMAX)
+constexpr int GS_STANCE = 15;
+
+// one ModeSequenceTemplate: modes md[n], switching times sw[n + 1] (strictly increasing)
+struct GsTemplate { int32_t n; int32_t md[GS_MAXM]; double sw[GS_MAXM + 1]; };
+// one robot's schedule: event times ev[n] (strictly increasing) and the n + 1 modes md[0..n] before, between and after them
+struct GsSchedule { int32_t n; int32_t md[GS_CAP + 1]; double ev[GS_CAP]; };
+// one robot's device state: the stored schedule and the active template (its index in the handle's table)
+struct GsRobot { GsSchedule s; int32_t tmpl; };
+// one robot's commands (robot-major arrays [B][n_cmd]): time t (sorted per robot), template (-1: none), cmd_vel row [4] (NaN: none)
+struct GsCommands { int n; const double* t; const int32_t* tmpl; const double* vel; };
+
+QMB_HD int gs_lower_bound(const double* a, int n, double t) { int lo = 0, hi = n; while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < t) lo = mid + 1; else hi = mid; } return lo; }
+
+// GaitSchedule::tileModeSequenceTemplate(startTime, finalTime): [.. last mode] start [template repeated until the last event >= final] STANCE.
+// -2 when start is not after the last event (as the host) or the events would exceed GS_CAP; s is then partly written.
+QMB_HD int gs_tile(GsSchedule& s, const GsTemplate& t, double start, double final_time) {
+  if (s.n > 0 && start <= s.ev[s.n - 1]) return -2;
+  if (s.n >= GS_CAP) return -2;
+  s.ev[s.n++] = start;
+  while (s.ev[s.n - 1] < final_time)
+    for (int i = 0; i < t.n; ++i) {
+      if (s.n >= GS_CAP) return -2;
+      s.md[s.n] = t.md[i]; s.ev[s.n] = s.ev[s.n - 1] + (t.sw[i + 1] - t.sw[i]); ++s.n;
+    }
+  s.md[s.n] = GS_STANCE; return 0;
+}
+
+// GaitSchedule::insertModeSequenceTemplate(template, startTime, finalTime): drop the events from start on, stance_time of stance unless the
+// schedule already ends standing, then the template.  0 or -2 (s partly written).
+QMB_HD int gs_insert(GsSchedule& s, const GsTemplate& t, double start, double final_time, double stance_time) {
+  const int idx = gs_lower_bound(s.ev, s.n, start);
+  if (idx < s.n) s.n = idx;
+  const double stance = s.md[s.n] == GS_STANCE ? 0.0 : stance_time;
+  if (stance > 0.0) { if (s.n >= GS_CAP) return -2; s.ev[s.n++] = start; s.md[s.n] = GS_STANCE; }
+  return gs_tile(s, t, start + stance, final_time);
+}
+
+// GaitSchedule::getModeSchedule(lower, upper): keep one event before lower (its mode forced to stance), drop the final stance phase, re-tile from
+// the last event to upper.  The schedule then is the window: returns its event count (<= QMB200_EMAX) or -2 (s partly written).
+// A schedule is never empty here: every tile leaves at least its start event.
+QMB_HD int gs_get(GsSchedule& s, const GsTemplate& t, double lower, double upper) {
+  const int idx = gs_lower_bound(s.ev, s.n, lower);
+  if (idx > 0) {
+    const int d = idx - 1; s.n -= d;
+    for (int i = 0; i < s.n; ++i) { s.ev[i] = s.ev[i + d]; s.md[i] = s.md[i + d]; }
+    s.md[s.n] = s.md[s.n + d]; s.md[0] = GS_STANCE;
+  }
+  const double tiling_start = s.ev[s.n - 1];
+  --s.n;
+  if (int rc = gs_tile(s, t, tiling_start, upper)) return rc;
+  return s.n > QMB200_EMAX ? -2 : s.n;
+}
+
+// One step of robot b at time t: the robot's commands due at t (time <= t, from *cursor on) in order: a template is inserted at t + horizon with
+// final horizon (GaitReceiver::preSolverRun), a cmd_vel row goes to cmd[0:4]; then the window [t - horizon, t + 2 horizon] is taken.  All or
+// nothing: status QMB200_ST_NAN (non-finite t) or QMB200_ST_OVERFLOW (a window above QMB200_EMAX events, or GS_CAP exceeded) leaves r, *cursor,
+// the MPC rows and cmd untouched.  Otherwise writes n_events, event_times[EMAX] (0 past the count), modes[EMAX + 1] (stance past the count) and cmd.
+// Returns the status.
+QMB_HD int gs_step(GsRobot& r, int32_t* cursor, const GsTemplate* table, const GsCommands& c, int b, double t, double horizon, double stance_time,
+                   int32_t* n_events, double* event_times, int32_t* modes, double* cmd) {
+  if (!isfinite(t)) return QMB200_ST_NAN;
+  GsRobot w = r; int cur = *cursor; double vel[4]; bool has_vel = false;
+  for (; cur < c.n && c.t[(size_t)b * c.n + cur] <= t; ++cur) {
+    const size_t k = (size_t)b * c.n + cur;
+    if (c.tmpl[k] >= 0) {
+      if (gs_insert(w.s, table[c.tmpl[k]], t + horizon, horizon, stance_time)) return QMB200_ST_OVERFLOW;
+      w.tmpl = c.tmpl[k];
+    }
+    if (!isnan(c.vel[4 * k])) { for (int i = 0; i < 4; ++i) vel[i] = c.vel[4 * k + i]; has_vel = true; }
+  }
+  const int n = gs_get(w.s, table[w.tmpl], t - horizon, t + 2.0 * horizon);
+  if (n < 0) return QMB200_ST_OVERFLOW;
+  *n_events = n;
+  for (int i = 0; i < QMB200_EMAX; ++i) event_times[i] = i < n ? w.s.ev[i] : 0.0;
+  for (int i = 0; i <= QMB200_EMAX; ++i) modes[i] = i <= n ? w.s.md[i] : GS_STANCE;
+  if (has_vel) for (int i = 0; i < 4; ++i) cmd[i] = vel[i];
+  r = w; *cursor = cur;
+  return 0;
+}
+
+// the mode of schedule s at t, as the MPC reads it (mode_at_time: the mode after the last event before t)
+QMB_HD int gs_mode_at(const GsSchedule& s, double t) { return s.md[gs_lower_bound(s.ev, s.n, t)]; }
+
+// one step per robot (gs_step) at t_obs [B] on the MPC problem rows n_events [B], event_times [B][EMAX], modes [B][EMAX + 1] and cmd [B][7];
+// writes status [B], and tmpl [B] (active template) and mode [B] (gs_mode_at t_obs of the stored schedule) when non-NULL
+int launch_gait_step(int B, const GsTemplate* table, GsRobot* robots, int32_t* cursor, GsCommands c, double horizon, double stance_time, const double* t_obs,
+                     int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, cudaStream_t s);
+
+}  // namespace qmb

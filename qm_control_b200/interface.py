@@ -629,6 +629,64 @@ class Solver:
         """Release the detector state."""
         self._call("slip_stop")
 
+    # ---------------- device gait schedule (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7) ----------------
+    def gait_dev_set_templates(self, names=None, gait_file=None):
+        """Load the template table: names (default: every template of the gait file, in the order of its list) → the names, a template's id being its
+        index.  Fails while the schedule runs."""
+        gait_file = gait_file or self.interface.gaitFile
+        names = list(gait_template_names(gait_file) if names is None else names)
+        arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
+        self._call("gait_dev_set_templates", gait_file.encode(), C.cast(arr, C.c_void_p), len(names))
+        self.gait_templates = names
+        return names
+
+    def gait_template_ids(self, names):
+        """Template names → int32 ids in the loaded table; ValueError on a name the table lacks."""
+        table = getattr(self, "gait_templates", None) or []
+        unknown = sorted({n for n in names if n not in table})
+        if unknown:
+            raise ValueError("unknown gait template(s) %s (loaded: %s)" % (", ".join(unknown), ", ".join(table)))
+        return np.array([table.index(n) for n in names], dtype=np.int32)
+
+    def gait_dev_reset(self, tmpl, t_start):
+        """(Re)start every robot's schedule: stance until t_start [B], then template tmpl [B] (ids or names).  Clears the command timeline.  Synchronous."""
+        B = self.batch; tmpl = list(tmpl)
+        ids = self.gait_template_ids(tmpl) if any(isinstance(n, str) for n in tmpl) else _i32(tmpl, (B,))
+        ids, t_start = _i32(ids, (B,)), _f64(np.broadcast_to(np.asarray(t_start, dtype=np.float64), (B,)))
+        self._call("gait_dev_reset", _p(ids), _p(t_start))
+
+    def gait_dev_set_commands(self, t, tmpl, cmd_vel):
+        """The command timeline: t [B, C] (sorted per robot, +inf pads), tmpl [B, C] (ids, -1: none), cmd_vel [B, C, 4] (NaN rows: none).  Every cursor
+        goes back to 0.  Synchronous."""
+        B = self.batch; t = _f64(t); n = t.shape[1] if t.ndim == 2 else -1
+        t = _f64(t, (B, n)); tmpl = _i32(tmpl, (B, n)); cmd_vel = _f64(cmd_vel, (B, n, 4))
+        self._call("gait_dev_set_commands", n, _p(t), _p(tmpl), _p(cmd_vel))
+
+    def gait_dev_step(self, t_obs, prob, cmd):
+        """Host variant of gait_dev_step_dev: prob's n_events / event_times / modes and cmd [B, 7] are updated in place (numpy) → (tmpl [B], mode [B],
+        status [B])."""
+        B = self.batch; t_obs = _f64(t_obs, (B,)); tm = np.zeros(B, dtype=np.int32); md = np.zeros(B, dtype=np.int32); st = np.zeros(B, dtype=np.int32)
+        for k, a in (("n_events", (B,)), ("event_times", (B, EMAX)), ("modes", (B, EMAX + 1))):
+            prob[k] = (_i32 if k != "event_times" else _f64)(prob[k], a)
+        self._call("gait_dev_step", _p(t_obs), _p(prob["n_events"]), _p(prob["event_times"]), _p(prob["modes"]), _p(cmd), _p(tm), _p(md), _p(st))
+        return tm, md, st
+
+    def gait_dev_step_dev(self, t_obs, prob, cmd, tmpl, mode, status, stream=None):
+        """One step per robot at t_obs [B] on the device problem rows of prob (n_events, event_times, modes) and cmd [B, 7]; tmpl, mode (or None) and
+        status [B] int32 written; no synchronisation."""
+        self._call("gait_dev_step_dev", _p(t_obs), _p(prob["n_events"]), _p(prob["event_times"]), _p(prob["modes"]), _p(cmd), _p(tmpl), _p(mode), _p(status), stream)
+
+    def gait_dev_get(self):
+        """→ dict(n_events [B], event_times [B, GAIT_CAP], modes [B, GAIT_CAP + 1], tmpl [B], cursor [B]).  Synchronous."""
+        B, cap = self.batch, _lib.GAIT_CAP
+        n = np.zeros(B, dtype=np.int32); ev = np.zeros((B, cap)); md = np.zeros((B, cap + 1), dtype=np.int32); tm = np.zeros(B, dtype=np.int32); cur = np.zeros(B, dtype=np.int32)
+        self._call("gait_dev_get", _p(n), _p(ev), _p(md), _p(tm), _p(cur))
+        return dict(n_events=n, event_times=ev, modes=md, tmpl=tm, cursor=cur)
+
+    def gait_dev_stop(self):
+        """Release the schedules and the timeline (the template table stays)."""
+        self._call("gait_dev_stop")
+
     # ---------------- utilities ----------------
     def centroidal_state_from_rbd(self, rbd):
         rbd = _f64(rbd); n = rbd.shape[0]; x = np.empty((n, NX))
@@ -642,6 +700,16 @@ def gait_schedule(gait_name, t_start, lo, hi, gait_file=None):
     if n < 0:
         raise QmbError("qmb200_gait_schedule failed: " + lib.qmb200_last_error(None).decode())
     return ev, md, n
+
+
+def gait_template_names(gait_file=None):
+    """The template names of a gait.info file, in the order of its `list` block."""
+    import re
+    txt = open(gait_file or _lib.asset("qm_gait.info")).read()
+    m = re.search(r"(?m)^list\s*\{(.*?)^\}", txt, re.S)
+    if m is None:
+        raise ValueError("no list block in %s" % gait_file)
+    return [n for _, n in sorted((int(i), n) for i, n in re.findall(r"\[(\d+)\]\s+(\S+)", m.group(1)))]
 
 
 class GaitSchedule:

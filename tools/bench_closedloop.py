@@ -44,6 +44,12 @@ quality lines are then those of the chain with the detector.  The JSON line gain
 events, alternated with blocks of plant steps); the robots with any foot flagged; and, for the warm-up run (the timed run's twin) and for one more
 untimed run of the same sweep without the detector, the fallen robots, the xy drift of the estimate at the end (p50 / p95) and |v_hat - v| over the run
 from the error watch.  With --vary these come per friction bin as well.
+
+--gait-commands adds the device gait schedule (closed_loop.run(commands=...)).  The JSON line gains "gait_commands": the wall time per simulated second
+of the same run with a timeline that changes nothing (every robot re-sends its cmd_vel at 0.3 s), timed after the sweep below in the same process; the
+device time per call of the gait step and of the MPC solve in that run (CUDA events around each call); and a switch sweep of 4 s: every robot stands,
+trots at cmd_vel from 0.5 s and switches at 2 s to one of stance, standing_trot, flying_trot, pace, static_walk, dynamic_walk and amble (equally
+often), with the fallen robots and the OR of the status bits per pair.
 """
 import argparse
 import json
@@ -267,6 +273,41 @@ def slip_times(solver, xy_yaw, reps=7, calls=20):
             "spread": [float(min(times["slip"])), float(max(times["slip"]))]}
 
 
+def gait_commands(solver, closed_loop, B, sim_s, cmd, xy, kw, upright):
+    """The switch sweep (which also warms the commands path up), then the timed run with a timeline that changes nothing, its gait step and MPC solve
+    bracketed with CUDA events."""
+    import torch
+    targets = ("stance", "standing_trot", "flying_trot", "pace", "static_walk", "dynamic_walk", "amble"); pair = np.arange(B) % len(targets)
+    sweep = dict(t=np.tile([0.5, 2.0], (B, 1)), gait=np.array([["trot", targets[p]] for p in pair], dtype=object), cmd_vel=np.tile([cmd, [np.nan] * 4], (B, 1, 1)))
+    sw = closed_loop.run(solver, duration=4.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), xy_yaw=xy, commands=sweep, **kw)
+    up, bits = upright(sw), np.bitwise_or.reduce(sw["status"], axis=0)
+    pairs = [{"pair": "stance -> trot -> " + g, "robots": int(np.sum(pair == i)), "fallen": int(np.sum(~up[pair == i])),
+              "status_bits_or": int(np.bitwise_or.reduce(bits[pair == i]))} for i, g in enumerate(targets)]
+    ev = {"gait_dev_step_dev": [], "mpc_solve_dev": []}
+
+    def bracket(name):
+        orig = getattr(solver, name)
+
+        def call(*a, **k):
+            e = [torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)]; s = torch.cuda.ExternalStream(a[-1]) if isinstance(a[-1], int) else None
+            e[0].record(s); orig(*a, **k); e[1].record(s); ev[name].append(e)
+        setattr(solver, name, call)
+    for n in ev:
+        bracket(n)
+    try:
+        noop = dict(t=np.full((B, 1), 0.3), gait=np.full((B, 1), None, dtype=object), cmd_vel=np.tile(cmd, (B, 1, 1)))
+        torch.cuda.synchronize(); t0 = time.perf_counter()
+        closed_loop.run(solver, duration=sim_s, gait="trot", cmd_vel=cmd, xy_yaw=xy, commands=noop, **kw)
+        torch.cuda.synchronize(); wall = time.perf_counter() - t0
+    finally:
+        for n in ev:
+            delattr(solver, n)
+    ms = {n: float(np.median([a.elapsed_time(b) for a, b in e])) for n, e in ev.items()}
+    return {"label": "timed: the run with commands that change nothing, after the sweep; per-call device times are medians over that run's calls",
+            "wall_s_per_sim_s": wall / sim_s, "gait_step_ms_per_call": ms["gait_dev_step_dev"], "mpc_solve_ms_per_call": ms["mpc_solve_dev"],
+            "switch_sweep": {"label": "4 s: stance, trot at cmd_vel from 0.5 s, the target gait from 2 s (each command takes effect 1 s later)", "pairs": pairs}}
+
+
 def watch_state_est(solver):
     """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
     error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
@@ -301,6 +342,7 @@ def main():
     ap.add_argument("--sensor-noise", choices=["reference"], help="with --state-estimator: the IMU noise of qm_gazebo/config/default.yaml")
     ap.add_argument("--attitude-filter", action="store_true", help="with --state-estimator: filter the IMU orientation before the estimator reads it")
     ap.add_argument("--slip-detector", action="store_true", help="with --state-estimator: keep slipping stance feet out of the estimate")
+    ap.add_argument("--gait-commands", action="store_true", help="time the device gait schedule in the loop and run a gait switch sweep")
     args = ap.parse_args()
     if args.vary and args.terrain:
         ap.error("--vary and --terrain are separate sweeps")
@@ -451,6 +493,9 @@ def main():
             if args.vary:
                 extra["slip"]["mu_bins"] = [{"mu": float(val), **{tag: slip_arm(run, verr, idx["mu"] == i) for tag, (run, verr) in arms.items()}}
                                             for i, val in enumerate(bins["mu"])]
+    if args.gait_commands:
+        extra["gait_commands"] = {**gait_commands(solver, closed_loop, B, sim_s, cmd, xy, kw, upright), "gpu": name, "power_limit": limit,
+                                  "wall_s_per_sim_s_without_commands": wall / sim_s}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
