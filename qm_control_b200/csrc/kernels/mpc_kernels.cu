@@ -535,6 +535,9 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+// threadIdx.x read through volatile asm: what a loop body derives from it cannot be hoisted out of the loop (and then spilled across the sweep's
+// high-pressure phase 3); it is recomputed where it is used
+__device__ __forceinline__ int fresh_tid() { int t; asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t)); return t; }
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) { asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 // A "copy group": with QMB_TMA one elected thread arms the mbarrier and issues the bulk copies; without it every thread copies its share with cp.async and the
@@ -618,7 +621,7 @@ __global__ void __launch_bounds__(RIC_THREADS, 4) mpc_riccati_kernel(const DevMo
   // node k wait for it, and they have slack (the factorisation warp is the critical path of phase 3)
   auto issue_q = [&](int k) { gQ.begin(Q_PACKED * 8, tid); gQ.copy(sm.Bm, sgb + (size_t)k * STAGE_DBL + ST_Q, Q_PACKED * 8, tid); };
   // rebuild the structured part of A~ / B~ of the node whose tail sits in sm.tail (all threads; A~ rows 3:12 and B~ rows 3:12 arrive by copy)
-  auto expand = [&]() {
+  auto expand = [&]() { const int tid = fresh_tid();
     const double* tl = sm.tail; const int32_t* si = reinterpret_cast<const int32_t*>(tl + T_INT); const double dtw = tl[T_MISC];
     for (int e = tid; e < 144; e += RIC_THREADS) { const int j12 = e / 12, c = e - 12 * j12; const int col = sup_col(c, 3 * (j12 / 3));   // rows 12:24: I + dtw * Px on the leg's support columns
       sm.A[(12 + j12) * LDX + col] = ((col == 12 + j12) ? 1.0 : 0.0) + dtw * tl[T_PXJ + e]; }
@@ -777,11 +780,15 @@ __global__ void __launch_bounds__(RIC_THREADS, 4) mpc_riccati_kernel(const DevMo
   double armijo = 0.0, dxn2 = 0.0, dun2 = 0.0;
   if (!(st & MST_NOT_PD)) {
     // buffer set 0: {G, A[0:9 rows], Bm[0:9 rows], A + 9 rows} ; set 1: {W, P, PB, P + 9 rows}
+    // the copy group is bound at each call site, never through a run-time reference: a reference chosen at run time takes both groups' addresses and puts their
+    // mbarrier pointer and phase in local memory, one dependent local load per copy and wait
     auto issue_fwd = [&](int k) {
-      if (k >= N) return; const int o = k & 1; CopyGroup& cg = o ? gF1 : gAB; const double* sg = sgb + (size_t)k * STAGE_DBL; const bool ev = node_type(k) == 1;
-      cg.begin((ev ? 0 : (GAIN_DBL + 9 * LDX + 9 * LDB) * 8) + TAIL_DBL * 8, tid);
-      cg.copy((o ? sm.P : sm.A) + 9 * LDX, sg + ST_TAIL, TAIL_DBL * 8, tid);
-      if (!ev) { cg.copy(o ? sm.W : sm.G, gb + (size_t)k * GAIN_DBL, GAIN_DBL * 8, tid); cg.copy(o ? sm.P : sm.A, sg + ST_AR, 9 * LDX * 8, tid); cg.copy(o ? sm.PB : sm.Bm, sg + ST_BR, 9 * LDB * 8, tid); } };
+      if (k >= N) return; const double* sg = sgb + (size_t)k * STAGE_DBL; const bool ev = node_type(k) == 1;
+      auto issue = [&](CopyGroup& cg, double* kb, double* ab, double* bb) {
+        cg.begin((ev ? 0 : (GAIN_DBL + 9 * LDX + 9 * LDB) * 8) + TAIL_DBL * 8, tid);
+        cg.copy(ab + 9 * LDX, sg + ST_TAIL, TAIL_DBL * 8, tid);
+        if (!ev) { cg.copy(kb, gb + (size_t)k * GAIN_DBL, GAIN_DBL * 8, tid); cg.copy(ab, sg + ST_AR, 9 * LDX * 8, tid); cg.copy(bb, sg + ST_BR, 9 * LDB * 8, tid); } };
+      if (k & 1) issue(gF1, sm.W, sm.P, sm.PB); else issue(gAB, sm.G, sm.A, sm.Bm); };
     issue_fwd(0);
     for (int k = 0; k < N; ++k) {
       const int o = k & 1; const double* Kb = o ? sm.W : sm.G; const double* ARb = o ? sm.P : sm.A; const double* BRb = o ? sm.PB : sm.Bm; const double* tl = (o ? sm.P : sm.A) + 9 * LDX;
