@@ -237,6 +237,13 @@ int qmb200_gait_dev_reset(qmb200_handle* h, const int32_t* tmpl /*[B]*/, const d
  * n_cmd = 0 clears the timeline.  Rejects a NaN time, unsorted times, a template outside [-1, n_templates) and a cmd_vel row neither finite nor all
  * NaN.  Synchronous. */
 int qmb200_gait_dev_set_commands(qmb200_handle* h, int32_t n_cmd, const double* t /*[B][n_cmd]*/, const int32_t* tmpl /*[B][n_cmd]*/, const double* cmd_vel /*[B][n_cmd][4]*/);
+/* The same timeline with end-effector commands (DESIGN.md §4.8): command c of robot b may instead of a cmd_vel row carry ee_kind[b][c] =
+ * QMB200_TARGET_EE_CMD_VEL (ee_cmd[b][c][0:3] = vx, vy, vz of the end effector, world frame; [3:7] ignored) or QMB200_TARGET_EE_GOAL (ee_cmd[b][c] = goal
+ * position, quaternion xyzw, world frame); -1: none (the row is ignored).  Besides the checks above it rejects an ee_kind outside {-1, 1, 2}, a command
+ * with both a cmd_vel row and an end-effector command, a non-finite ee_cmd_vel or goal and a goal quaternion whose norm differs from 1 by more than
+ * 1e-9.  ee_kind and ee_cmd both NULL: qmb200_gait_dev_set_commands.  Synchronous. */
+int qmb200_gait_dev_set_commands_ee(qmb200_handle* h, int32_t n_cmd, const double* t /*[B][n_cmd]*/, const int32_t* tmpl /*[B][n_cmd]*/, const double* cmd_vel /*[B][n_cmd][4]*/,
+                                    const int32_t* ee_kind /*[B][n_cmd] or NULL*/, const double* ee_cmd /*[B][n_cmd][7] or NULL*/);
 /* One step per robot at t = t_obs[b], right before the MPC tick's target_trajectories: (1) every command of the robot due at t (time <= t) and not yet
  * applied, in order: a template is inserted with qmb200_gait_insert_template's arithmetic at (t + T, T) (GaitReceiver::preSolverRun: start = the
  * solve's final time, final = the time horizon), a cmd_vel row is written to cmd[b][0:4] (the target front-end's cmd[B][7]); (2) the window
@@ -250,6 +257,18 @@ int qmb200_gait_dev_step(qmb200_handle* h, const double* t_obs /*[B]*/, int32_t*
                          int32_t* status /*[B]*/);
 int qmb200_gait_dev_step_dev(qmb200_handle* h, const double* t_obs, int32_t* n_events, double* event_times, int32_t* mode_sequence, double* cmd, int32_t* tmpl,
                              int32_t* mode, int32_t* status, void* cuda_stream);
+/* The step with the publisher's target source (DESIGN.md §4.8).  Each robot's source is the cmd_vel stream after qmb200_gait_dev_reset.  Among the
+ * robot's commands applied by the step, the last target command (cmd_vel, ee_cmd_vel or goal) sets the source: a cmd_vel row writes cmd[b][0:4], an
+ * ee_cmd_vel row cmd[b][0:3], a goal row cmd[b][0:7].  target_kind [B] (or NULL) is the kind this tick's target call takes
+ * (qmb200_target_trajectories_per_robot): QMB200_TARGET_EE_GOAL when the step applied a goal as its last target command (the goal is published once),
+ * -1 while a published goal is held (the target call then leaves the robot's target and last_ee_target as they are), otherwise the source's stream,
+ * QMB200_TARGET_CMD_VEL or QMB200_TARGET_EE_CMD_VEL.  A failed step (QMB200_ST_NAN / QMB200_ST_OVERFLOW) leaves the source unchanged and reports that
+ * source's kind (-1 for a held goal).  target_kind is written for every robot. */
+int qmb200_gait_dev_step_ee(qmb200_handle* h, const double* t_obs /*[B]*/, int32_t* n_events /*[B] in-out*/, double* event_times /*[B][EMAX] in-out*/,
+                            int32_t* mode_sequence /*[B][EMAX+1] in-out*/, double* cmd /*[B][7] in-out*/, int32_t* tmpl /*[B] or NULL*/, int32_t* mode /*[B] or NULL*/,
+                            int32_t* status /*[B]*/, int32_t* target_kind /*[B] or NULL*/);
+int qmb200_gait_dev_step_ee_dev(qmb200_handle* h, const double* t_obs, int32_t* n_events, double* event_times, int32_t* mode_sequence, double* cmd, int32_t* tmpl,
+                                int32_t* mode, int32_t* status, int32_t* target_kind, void* cuda_stream);
 /* Synchronous: each robot's stored schedule (count, event times [B][GAIT_CAP] with 0 past the count, modes [B][GAIT_CAP+1] with stance past it), active
  * template and cursor.  Any output may be NULL. */
 int qmb200_gait_dev_get(qmb200_handle* h, int32_t* n_events /*[B]*/, double* event_times /*[B][QMB200_GAIT_CAP]*/, int32_t* mode_sequence /*[B][QMB200_GAIT_CAP+1]*/,
@@ -280,6 +299,17 @@ int qmb200_target_trajectories(qmb200_handle* h, int32_t kind, const double* cmd
                                double* last_ee_target /*[B][7] in-out*/, int32_t* n_target /*[B]*/, double* target_times /*[B][KMAX]*/, double* target_states /*[B][KMAX][37]*/);
 int qmb200_target_trajectories_dev(qmb200_handle* h, int32_t kind, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state, double* last_ee_target,
                                    int32_t* n_target, double* target_times, double* target_states, void* cuda_stream);
+/* The same with a kind per robot: kind[b] in {QMB200_TARGET_CMD_VEL, _EE_CMD_VEL, _EE_GOAL} as above, or -1: robot b is left untouched (a held goal: its
+ * n_target, target_times, target_states and last_ee_target keep the published 2-knot trajectory, which the MPC keeps tracking; past its final time
+ * the target holds the final knot).  The host variant rejects a kind outside [-1, 2] and stages the target rows in-out; the _dev variant leaves a
+ * robot whose kind lies outside [0, 2] untouched.  For QMB200_TARGET_EE_CMD_VEL and _EE_GOAL the base target is the end-effector target minus
+ * (0.52, 0.09) in the world frame, as QmTargetTrajectoriesPublisher_node.cpp:152-153, 184-185 compute it: right for a robot facing +x only (the base
+ * of a robot turned by yaw is asked to stand 0.52 m world-x behind the hand, not 0.52 m behind it along its own heading). */
+int qmb200_target_trajectories_per_robot(qmb200_handle* h, const int32_t* kind /*[B]*/, const double* cmd /*[B][7]*/, const double* t_obs /*[B]*/, const double* x_obs /*[B][30]*/,
+                                         const double* ee_state /*[B][7]*/, double* last_ee_target /*[B][7] in-out*/, int32_t* n_target /*[B] in-out*/,
+                                         double* target_times /*[B][KMAX] in-out*/, double* target_states /*[B][KMAX][37] in-out*/);
+int qmb200_target_trajectories_per_robot_dev(qmb200_handle* h, const int32_t* kind, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
+                                             double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, void* cuda_stream);
 void qmb200_initial_ee_target(double* last_ee_target7);
 
 /* SafetyChecker::check + QMController::updateControlLaw (QMController.cpp:159-165,177-190) or, for a handle created with

@@ -9,6 +9,7 @@ ASSETS = os.path.join(ROOT, "assets")
 
 NX, NU, RBD, CMD, TARGET, EMAX, KMAX = 30, 30, 55, 54, 37, 32, 4
 GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
+TARGET_CMD_VEL, TARGET_EE_CMD_VEL, TARGET_EE_GOAL = 0, 1, 2   # QMB200_TARGET_*: the target front-end's kinds (-1 in a per-robot kind: a held goal)
 
 dp = C.POINTER(C.c_double)
 ip = C.POINTER(C.c_int32)
@@ -130,14 +131,19 @@ PROTOTYPES = {
     "qmb200_gait_dev_set_templates": (I32, [P, S, P, I32]),
     "qmb200_gait_dev_reset": (I32, [P] * 3),
     "qmb200_gait_dev_set_commands": (I32, [P, I32] + [P] * 3),
+    "qmb200_gait_dev_set_commands_ee": (I32, [P, I32] + [P] * 5),
     "qmb200_gait_dev_step": (I32, [P] * 9),
     "qmb200_gait_dev_step_dev": (I32, [P] * 10),
+    "qmb200_gait_dev_step_ee": (I32, [P] * 10),
+    "qmb200_gait_dev_step_ee_dev": (I32, [P] * 11),
     "qmb200_gait_dev_get": (I32, [P] * 6),
     "qmb200_gait_dev_stop": (I32, [P]),
     "qmb200_observation_update": (I32, [P] * 5),
     "qmb200_observation_update_dev": (I32, [P] * 6),
     "qmb200_target_trajectories": (I32, [P, I32] + [P] * 8),
     "qmb200_target_trajectories_dev": (I32, [P, I32] + [P] * 9),
+    "qmb200_target_trajectories_per_robot": (I32, [P] * 10),
+    "qmb200_target_trajectories_per_robot_dev": (I32, [P] * 11),
     "qmb200_initial_ee_target": (None, [P]),
     "qmb200_control_law": (I32, [P] * 10),
     "qmb200_control_law_dev": (I32, [P] * 11),

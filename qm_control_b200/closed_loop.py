@@ -19,7 +19,9 @@ With attitude_filter set as well, an attitude filter (Solver.attitude_*) rewrite
 With slip_detector set as well, a slip detector (Solver.slip_*) removes the stance feet that slide from the contact mask the estimator reads.
 On terrain the estimator needs ground_map, its own map of the run's tile library (Solver.state_est_set_ground); the controller still sees no terrain.
 With commands set, the gait is rolled on the device (Solver.gait_dev_*): each robot follows its own timeline of gait and cmd_vel commands, and a gait
-step right before every target call writes the window GaitSchedule::getModeSchedule gives into the MPC problem's mode schedule rows.
+step right before every target call writes the window GaitSchedule::getModeSchedule gives into the MPC problem's mode schedule rows.  The
+timeline may also command the end effector (a goal pose published once and then held, or an ee_cmd_vel stream): the step then tells each robot's
+target call which kind to take (DESIGN.md §4.8).
 The start mirrors QMController::starting (QMController.cpp:98-126): the first observation from the measured state and one blocking solve before
 the loop.  The clock starts at t >= 10 s, so the legs are torque controlled from the first tick (QMController.cpp:177-190).  Without commands the
 mode schedule is tiled once on the host for the whole run.  No host synchronisation happens inside the loop; the per-MPC-tick record is the one host copy.
@@ -88,20 +90,28 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     (Solver.state_est_set_ground), on this run's tile library: True gives it the run's own terrain rows (a perfect map), a dict rows of its own (a
     wrong tile, a shifted origin).  Its foot-height rows then follow the mapped ground under each foot.  The controller still does not see the terrain.
     The previous map is restored when run returns.
-    commands: dict(t [B, C] in seconds after the start, gait [B, C] of template names or None, cmd_vel [B, C, 4] with NaN rows for none (optional)):
-    robot b's timeline, sorted per robot.  The run then loads every template of qm_gait.info (Solver.gait_dev_set_templates), starts each robot on
+    commands: dict(t [B, C] in seconds after the start, gait [B, C] of template names or None, and optionally cmd_vel [B, C, 4], ee_goal [B, C, 7]
+    (position, quaternion xyzw of unit norm, world frame) and ee_cmd_vel [B, C, 3] (end-effector velocity, world frame), each with NaN rows for none
+    and at most one of the three per command): robot b's timeline, sorted per robot.  The run then loads every template of qm_gait.info (Solver.gait_dev_set_templates), starts each robot on
     stance until t_start and then its gait (Solver.gait_dev_reset), and right before every target call (the first, blocking solve included) a gait
     step applies the robot's commands due at t_obs (a gait is inserted at t_obs + T after phaseTransitionStanceTime of stance, as GaitReceiver
     does; a cmd_vel row replaces the robot's cmd_vel) and writes the window [t_obs - T, t_obs + 2T] into the MPC's mode schedule rows.  The host
     tiling and its limit of QMB200_EMAX events over the whole run do not apply.  Its status is OR-ed into the record's; the device schedule is
-    stopped when run returns.
+    stopped when run returns.  Each robot's target source starts on the cmd_vel stream; the last target command a step applies sets it
+    (DESIGN.md §4.8): an ee_goal row is published once by that tick's target call (EEgoalPoseToTargetTrajectories, last_ee_target set) and then
+    held (the robot's target is left as published), an ee_cmd_vel row switches the robot to the ee_cmd_vel stream (EeCmdVelToTargetTrajectories
+    every tick), a cmd_vel row back to the cmd_vel stream.  For both end-effector commands the base target is the end-effector target minus
+    (0.52, 0.09) in the world frame, as upstream computes it: meant for robots facing +x.  With commands every target call takes each robot's kind
+    from its gait step (Solver.target_trajectories_dev with a per-robot kind).
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
     payload_est[ticks, B, 8] = the model payload rows committed at each record's MPC tick; with state_estimator also base_est[ticks, B, 6], the estimated base in
     the layout of base; with slip_detector also slip[ticks, B], the OR of the detector's slip masks over each record's 10 ms window; with commands also
     gait[ticks, B], the active template id after each record's gait step (an index of gait_templates), mode[ticks, B], the window's mode at that
-    step's t_obs, and gait_templates, the table's names)."""
+    step's t_obs, gait_templates, the table's names, target_kind[ticks, B], the kind each robot's target call took at that record's MPC tick (0
+    cmd_vel, 1 ee_cmd_vel, 2 goal published, -1 goal held), and ee_target[ticks, B, 7], the final-knot end-effector pose of the target in force after
+    that call)."""
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
     if state_estimator is not None and state_estimator is not True and not isinstance(state_estimator, dict):
@@ -151,14 +161,15 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
 
 
 def _gait_commands(B, gait, commands):
-    """closed_loop.run's gait and commands → dict(names, gait [B] ids, t [B, C], tmpl [B, C] ids or -1, cmd_vel [B, C, 4]); ValueError when malformed"""
+    """closed_loop.run's gait and commands → dict(names, gait [B] ids, t [B, C], tmpl [B, C] ids or -1, cmd_vel [B, C, 4], ee: {} or dict(ee_kind [B, C],
+    ee_cmd [B, C, 7]) when the timeline has ee_goal / ee_cmd_vel); ValueError when malformed"""
     names = gait_template_names()
     ids = {n: i for i, n in enumerate(names)}
     start = [gait] * B if isinstance(gait, str) else list(gait)
     if len(start) != B:
         raise ValueError("closed_loop.run: gait must be one name or a sequence of %d names, got %d" % (B, len(start)))
-    if not isinstance(commands, dict) or not {"t", "gait"} <= set(commands) or not set(commands) <= {"t", "gait", "cmd_vel"}:
-        raise ValueError("closed_loop.run: commands must be dict(t, gait[, cmd_vel]), got %r" % (commands,))
+    if not isinstance(commands, dict) or not {"t", "gait"} <= set(commands) or not set(commands) <= {"t", "gait", "cmd_vel", "ee_goal", "ee_cmd_vel"}:
+        raise ValueError("closed_loop.run: commands must be dict(t, gait[, cmd_vel][, ee_goal][, ee_cmd_vel]), got %r" % (commands,))
     t = np.asarray(commands["t"], dtype=np.float64)
     if t.ndim != 2 or t.shape[0] != B:
         raise ValueError("closed_loop.run: commands t must have shape (%d, C), got %s" % (B, t.shape))
@@ -175,7 +186,29 @@ def _gait_commands(B, gait, commands):
     if np.any(np.isnan(vel).any(-1) != np.isnan(vel).all(-1)) or np.any(np.isinf(vel)):
         raise ValueError("closed_loop.run: each commands cmd_vel row must be finite or all NaN")
     tmpl = np.array([[-1 if n is None else ids[n] for n in row] for row in g], dtype=np.int32).reshape(B, C)
-    return dict(names=names, gait=np.array([ids[n] for n in start], dtype=np.int32), t=t, tmpl=tmpl, cmd_vel=vel)
+    return dict(names=names, gait=np.array([ids[n] for n in start], dtype=np.int32), t=t, tmpl=tmpl, cmd_vel=vel, ee=_ee_commands(B, C, commands, vel))
+
+
+def _ee_commands(B, C, commands, vel):
+    """commands' ee_goal [B, C, 7] / ee_cmd_vel [B, C, 3] → {} when neither is given, else dict(ee_kind [B, C], ee_cmd [B, C, 7]) for
+    Solver.gait_dev_set_commands; ValueError when malformed"""
+    if commands.get("ee_goal") is None and commands.get("ee_cmd_vel") is None:
+        return {}
+    goal = np.full((B, C, 7), np.nan) if commands.get("ee_goal") is None else np.asarray(commands["ee_goal"], dtype=np.float64)
+    eev = np.full((B, C, 3), np.nan) if commands.get("ee_cmd_vel") is None else np.asarray(commands["ee_cmd_vel"], dtype=np.float64)
+    if goal.shape != (B, C, 7) or eev.shape != (B, C, 3):
+        raise ValueError("closed_loop.run: commands ee_goal must have shape (%d, %d, 7) and ee_cmd_vel (%d, %d, 3), got %s and %s" % (B, C, B, C, goal.shape, eev.shape))
+    for name, a in (("ee_goal", goal), ("ee_cmd_vel", eev)):
+        if np.any(np.isnan(a).any(-1) != np.isnan(a).all(-1)) or np.any(np.isinf(a)):
+            raise ValueError("closed_loop.run: each commands %s row must be finite or all NaN" % name)
+    has_goal, has_eev = ~np.isnan(goal[..., 0]), ~np.isnan(eev[..., 0])
+    if np.any(has_goal.astype(int) + has_eev + ~np.isnan(vel[..., 0]) > 1):
+        raise ValueError("closed_loop.run: a command carries at most one of cmd_vel, ee_goal and ee_cmd_vel")
+    if np.any(np.abs(np.linalg.norm(goal[has_goal][:, 3:7], axis=-1) - 1.0) > 1e-9):
+        raise ValueError("closed_loop.run: each commands ee_goal quaternion (xyzw) must have unit norm (within 1e-9)")
+    kind = np.where(has_goal, _lib.TARGET_EE_GOAL, np.where(has_eev, _lib.TARGET_EE_CMD_VEL, -1)).astype(np.int32)
+    cmd = np.where(has_goal[..., None], goal, 0.0); cmd[..., :3] = np.where(has_eev[..., None], eev, cmd[..., :3])
+    return dict(ee_kind=kind, ee_cmd=cmd)
 
 
 @contextlib.contextmanager
@@ -372,6 +405,7 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             rec_slip = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
         if gd is not None:
             gait_st = torch.zeros_like(contact); rec_gait = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_mode = torch.zeros_like(rec_gait)
+            rec_kind = torch.zeros_like(rec_gait); rec_ee_target = torch.zeros((ticks, B, 7), dtype=torch.float64, device=dev)
         push = None
         if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
             push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench), zero=torch.zeros((B, 12), dtype=torch.float64, device=dev),
@@ -379,17 +413,21 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     stream.synchronize()
     if gd is not None:
         solver.gait_dev_reset(gd["gait"], np.full(B, t_start))
-        solver.gait_dev_set_commands(t_start + gd["t"], gd["tmpl"], gd["cmd_vel"])
+        solver.gait_dev_set_commands(t_start + gd["t"], gd["tmpl"], gd["cmd_vel"], **gd["ee"])
     solver.hw_set_delay(HW_DELAY)
 
     def mpc_tick(i):
         if est:
             solver.payload_est_commit_dev(s); solver.get_model_payload_dev(rec_pl[i], s)
         ee_state.copy_(meas[:, 48:55])
-        if gd is not None:
-            solver.gait_dev_step_dev(t_obs, prob, cmd7, rec_gait[i], rec_mode[i], gait_st, s)
+        if gd is None:
+            solver.target_trajectories_dev(0, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
+        else:   # the step's target kinds go straight to the target call, and stay in the record
+            kind = rec_kind[i]
+            solver.gait_dev_step_dev(t_obs, prob, cmd7, rec_gait[i], rec_mode[i], gait_st, s, target_kind=kind)
             acc_st.bitwise_or_(gait_st)
-        solver.target_trajectories_dev(0, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
+            solver.target_trajectories_dev(kind, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
+            rec_ee_target[i] = prob["target_states"][:, 1, 30:37]
         solver.mpc_solve_dev(prob, s)
 
     with torch.cuda.stream(stream):
@@ -443,5 +481,6 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     if sl:
         out["slip"] = rec_slip.cpu().numpy()
     if gd is not None:
-        out.update(gait=rec_gait.cpu().numpy(), mode=rec_mode.cpu().numpy(), gait_templates=list(gd["names"]))
+        out.update(gait=rec_gait.cpu().numpy(), mode=rec_mode.cpu().numpy(), gait_templates=list(gd["names"]), target_kind=rec_kind.cpu().numpy(),
+                   ee_target=rec_ee_target.cpu().numpy())
     return out

@@ -25,8 +25,9 @@ struct ControlLawParams {
 };
 
 int launch_observation(const DevModel* mdl, int B, const double* rbd, const double* period, double* t_obs, double* x_obs, cudaStream_t s, const double* srbd /*[B][SRBD_DBL] or NULL*/);
-int launch_target(const TargetParams& prm, int kind, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state, double* last_ee_target,
-                  int32_t* n_target, double* target_times, double* target_states, cudaStream_t s);
+// kinds [B] (device, or NULL: every robot `kind`): per-robot kind; robots outside [0, 2] are left untouched
+int launch_target(const TargetParams& prm, int kind, const int32_t* kinds, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
+                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s);
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,
                        double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s);
 int launch_hw_write(int B, double delay, const double* time, const double* period, const double* joint_cmd, const double* joint_pos, const double* joint_vel,

@@ -1,5 +1,6 @@
 // Device gait schedule (gait_kernel.cu): per robot, ocs2::legged_robot::GaitSchedule as the host object qmb200_gait keeps it (capi_mpc.inc), on
-// fixed-capacity arrays, with a timeline of gait and cmd_vel commands, rolled once per MPC tick (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7).
+// fixed-capacity arrays, with a timeline of gait, cmd_vel and end-effector commands, rolled once per MPC tick (include/qmb200.h: qmb200_gait_dev_*;
+// DESIGN.md §4.7, §4.8).
 // The core (gs_*) is host + device: tests/gait_host.cpp compiles it with g++ and checks it against the host objects on the CPU.  Its arithmetic is
 // that of qmb200_gait_insert_template / qmb200_gait_get_mode_schedule: the event times come out bit for bit equal.
 #pragma once
@@ -16,10 +17,16 @@ constexpr int GS_STANCE = 15;
 struct GsTemplate { int32_t n; int32_t md[GS_MAXM]; double sw[GS_MAXM + 1]; };
 // one robot's schedule: event times ev[n] (strictly increasing) and the n + 1 modes md[0..n] before, between and after them
 struct GsSchedule { int32_t n; int32_t md[GS_CAP + 1]; double ev[GS_CAP]; };
-// one robot's device state: the stored schedule and the active template (its index in the handle's table)
-struct GsRobot { GsSchedule s; int32_t tmpl; };
-// one robot's commands (robot-major arrays [B][n_cmd]): time t (sorted per robot), template (-1: none), cmd_vel row [4] (NaN: none)
-struct GsCommands { int n; const double* t; const int32_t* tmpl; const double* vel; };
+// the target source of a robot's publisher (DESIGN.md §4.8): the cmd_vel stream (0, a zeroed robot's), the ee_cmd_vel stream, or a published goal
+// that is held
+constexpr int GS_SRC_CMD_VEL = QMB200_TARGET_CMD_VEL, GS_SRC_EE_CMD_VEL = QMB200_TARGET_EE_CMD_VEL, GS_SRC_EE_GOAL = QMB200_TARGET_EE_GOAL;
+constexpr int GS_KIND_HELD = -1;   // target kind of a robot whose goal is held: its target call writes nothing
+// one robot's device state: the stored schedule, the active template (its index in the handle's table) and the target source
+struct GsRobot { GsSchedule s; int32_t tmpl; int32_t src; };
+// one robot's commands (robot-major arrays [B][n_cmd]): time t (sorted per robot), template (-1: none), cmd_vel row [4] (NaN: none), and optionally
+// an end-effector command: kind (-1: none, QMB200_TARGET_EE_CMD_VEL, QMB200_TARGET_EE_GOAL) with its row [7] (ee_cmd_vel: vx, vy, vz; goal: pos,
+// quat xyzw).  NULL ee_kind: no end-effector rows.  A row carries at most one of cmd_vel and an end-effector command.
+struct GsCommands { int n; const double* t; const int32_t* tmpl; const double* vel; const int32_t* ee_kind = nullptr; const double* ee = nullptr; };
 
 QMB_HD int gs_lower_bound(const double* a, int n, double t) { int lo = 0, hi = n; while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < t) lo = mid + 1; else hi = mid; } return lo; }
 
@@ -63,29 +70,43 @@ QMB_HD int gs_get(GsSchedule& s, const GsTemplate& t, double lower, double upper
   return s.n > QMB200_EMAX ? -2 : s.n;
 }
 
+// the target kind of a robot's target call on a tick: a goal published by this tick's step (applied = QMB200_TARGET_EE_GOAL), else the source's
+// stream, GS_KIND_HELD for a held goal
+QMB_HD int gs_target_kind(int src, int applied) { return applied == GS_SRC_EE_GOAL ? GS_SRC_EE_GOAL : src == GS_SRC_EE_GOAL ? GS_KIND_HELD : src; }
+
 // One step of robot b at time t: the robot's commands due at t (time <= t, from *cursor on) in order: a template is inserted at t + horizon with
-// final horizon (GaitReceiver::preSolverRun), a cmd_vel row goes to cmd[0:4]; then the window [t - horizon, t + 2 horizon] is taken.  All or
-// nothing: status QMB200_ST_NAN (non-finite t) or QMB200_ST_OVERFLOW (a window above QMB200_EMAX events, or GS_CAP exceeded) leaves r, *cursor,
-// the MPC rows and cmd untouched.  Otherwise writes n_events, event_times[EMAX] (0 past the count), modes[EMAX + 1] (stance past the count) and cmd.
+// final horizon (GaitReceiver::preSolverRun), a cmd_vel row goes to cmd[0:4], an ee_cmd_vel row to cmd[0:3], a goal row to cmd[0:7]; the last of
+// these target commands sets the robot's source.  Then the window [t - horizon, t + 2 horizon] is taken.  All or nothing: status QMB200_ST_NAN
+// (non-finite t) or QMB200_ST_OVERFLOW (a window above QMB200_EMAX events, or GS_CAP exceeded) leaves r (its source included), *cursor, the MPC rows
+// and cmd untouched.  Otherwise writes n_events, event_times[EMAX] (0 past the count), modes[EMAX + 1] (stance past the count) and cmd.
+// target_kind (when non-NULL) is written on every path: gs_target_kind of the source after the step and the last target command it applied.
 // Returns the status.
 QMB_HD int gs_step(GsRobot& r, int32_t* cursor, const GsTemplate* table, const GsCommands& c, int b, double t, double horizon, double stance_time,
-                   int32_t* n_events, double* event_times, int32_t* modes, double* cmd) {
+                   int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* target_kind = nullptr) {
+  if (target_kind) *target_kind = gs_target_kind(r.src, -1);   // a failed step leaves the source as it was
   if (!isfinite(t)) return QMB200_ST_NAN;
-  GsRobot w = r; int cur = *cursor; double vel[4]; bool has_vel = false;
+  GsRobot w = r; int cur = *cursor; double row[7]; int wrote = 0, applied = -1;   // row[0:wrote]: the cmd slots written (every command writes a prefix)
   for (; cur < c.n && c.t[(size_t)b * c.n + cur] <= t; ++cur) {
     const size_t k = (size_t)b * c.n + cur;
     if (c.tmpl[k] >= 0) {
       if (gs_insert(w.s, table[c.tmpl[k]], t + horizon, horizon, stance_time)) return QMB200_ST_OVERFLOW;
       w.tmpl = c.tmpl[k];
     }
-    if (!isnan(c.vel[4 * k])) { for (int i = 0; i < 4; ++i) vel[i] = c.vel[4 * k + i]; has_vel = true; }
+    if (!isnan(c.vel[4 * k])) { for (int i = 0; i < 4; ++i) row[i] = c.vel[4 * k + i]; wrote = wrote > 4 ? wrote : 4; applied = GS_SRC_CMD_VEL; }
+    if (c.ee_kind && c.ee_kind[k] >= 0) {
+      const int m = c.ee_kind[k] == GS_SRC_EE_GOAL ? 7 : 3;
+      for (int i = 0; i < m; ++i) row[i] = c.ee[7 * k + i];
+      wrote = wrote > m ? wrote : m; applied = c.ee_kind[k];
+    }
   }
   const int n = gs_get(w.s, table[w.tmpl], t - horizon, t + 2.0 * horizon);
   if (n < 0) return QMB200_ST_OVERFLOW;
   *n_events = n;
   for (int i = 0; i < QMB200_EMAX; ++i) event_times[i] = i < n ? w.s.ev[i] : 0.0;
   for (int i = 0; i <= QMB200_EMAX; ++i) modes[i] = i <= n ? w.s.md[i] : GS_STANCE;
-  if (has_vel) for (int i = 0; i < 4; ++i) cmd[i] = vel[i];
+  for (int i = 0; i < wrote; ++i) cmd[i] = row[i];
+  if (applied >= 0) w.src = applied;
+  if (target_kind) *target_kind = gs_target_kind(w.src, applied);
   r = w; *cursor = cur;
   return 0;
 }
@@ -94,8 +115,9 @@ QMB_HD int gs_step(GsRobot& r, int32_t* cursor, const GsTemplate* table, const G
 QMB_HD int gs_mode_at(const GsSchedule& s, double t) { return s.md[gs_lower_bound(s.ev, s.n, t)]; }
 
 // one step per robot (gs_step) at t_obs [B] on the MPC problem rows n_events [B], event_times [B][EMAX], modes [B][EMAX + 1] and cmd [B][7];
-// writes status [B], and tmpl [B] (active template) and mode [B] (gs_mode_at t_obs of the stored schedule) when non-NULL
+// writes status [B], and tmpl [B] (active template), mode [B] (gs_mode_at t_obs of the stored schedule) and target_kind [B] when non-NULL
 int launch_gait_step(int B, const GsTemplate* table, GsRobot* robots, int32_t* cursor, GsCommands c, double horizon, double stance_time, const double* t_obs,
-                     int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, cudaStream_t s);
+                     int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, int32_t* target_kind,
+                     cudaStream_t s);
 
 }  // namespace qmb

@@ -11,12 +11,12 @@ __global__ void __launch_bounds__(GS_THREADS) gait_step_kernel(int B, const GsTe
                                                                 int32_t* __restrict__ cursor, GsCommands c, double horizon, double stance_time,
                                                                 const double* __restrict__ t_obs, int32_t* __restrict__ n_events, double* __restrict__ event_times,
                                                                 int32_t* __restrict__ modes, double* __restrict__ cmd, int32_t* __restrict__ tmpl,
-                                                                int32_t* __restrict__ mode, int32_t* __restrict__ status) {
+                                                                int32_t* __restrict__ mode, int32_t* __restrict__ status, int32_t* __restrict__ target_kind) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const double t = t_obs[b];
   status[b] = gs_step(robots[b], cursor + b, table, c, b, t, horizon, stance_time, n_events + b, event_times + (size_t)b * QMB200_EMAX,
-                      modes + (size_t)b * (QMB200_EMAX + 1), cmd + (size_t)b * 7);
+                      modes + (size_t)b * (QMB200_EMAX + 1), cmd + (size_t)b * 7, target_kind ? target_kind + b : nullptr);
   if (tmpl) tmpl[b] = robots[b].tmpl;
   if (mode) mode[b] = gs_mode_at(robots[b].s, t);
 }
@@ -24,9 +24,10 @@ __global__ void __launch_bounds__(GS_THREADS) gait_step_kernel(int B, const GsTe
 }  // namespace
 
 int launch_gait_step(int B, const GsTemplate* table, GsRobot* robots, int32_t* cursor, GsCommands c, double horizon, double stance_time, const double* t_obs,
-                     int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, cudaStream_t s) {
+                     int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, int32_t* target_kind,
+                     cudaStream_t s) {
   gait_step_kernel<<<(B + GS_THREADS - 1) / GS_THREADS, GS_THREADS, 0, s>>>(B, table, robots, cursor, c, horizon, stance_time, t_obs, n_events, event_times,
-                                                                           modes, cmd, tmpl, mode, status);
+                                                                           modes, cmd, tmpl, mode, status, target_kind);
   return 1;
 }
 

@@ -5,6 +5,7 @@ simulated second, the plant step's device time per call (CUDA events) and its sh
 deviation from the initial pose, as percentiles over the robots) of this project's compliant-contact plant.  Writes nothing to disk.
 
     python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter] [--slip-detector]]
+                                     [--gait-commands] [--ee-goals]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -50,6 +51,13 @@ of the same run with a timeline that changes nothing (every robot re-sends its c
 device time per call of the gait step and of the MPC solve in that run (CUDA events around each call); and a switch sweep of 4 s: every robot stands,
 trots at cmd_vel from 0.5 s and switches at 2 s to one of stance, standing_trot, flying_trot, pace, static_walk, dynamic_walk and amble (equally
 often), with the fallen robots and the OR of the status bits per pair.
+
+--ee-goals commands the end effector on the device command timeline (closed_loop.run(commands=dict(..., ee_goal=...))).  The JSON line gains "ee_goals":
+a reach sweep of 5 s in which every robot starts at yaw 0 on the grid, trots, is given one goal at 0.2 s (an offset from its start pose of dx -0.1..0.4 m,
+dz -0.1..0.1 m and a rotation of 0-20 deg about a fixed axis, every combination equally often) and is commanded to stance at 2.5 s, with per bin of each
+axis the end-effector position and orientation errors at the end (p50 / p95), the fallen robots and the OR of the status bits; the device time per call
+of the per-robot target call and of the scalar one on the same rows (CUDA events, alternated blocks); and the wall time per simulated second of a run
+of --duration with the goals, with a timeline that changes nothing, and without commands (the timed run above).
 """
 import argparse
 import json
@@ -308,6 +316,67 @@ def gait_commands(solver, closed_loop, B, sim_s, cmd, xy, kw, upright):
             "switch_sweep": {"label": "4 s: stance, trot at cmd_vel from 0.5 s, the target gait from 2 s (each command takes effect 1 s later)", "pairs": pairs}}
 
 
+def target_call_times(solver, reps=7, calls=50):
+    """Device time per target call of the whole batch: the scalar entry point (kind 0 for every robot) and the per-robot one with the same kinds and
+    with kinds 0 / 1 / 2 / -1 mixed, alternated `reps` times in blocks of `calls` on one set of rows (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev); rng = np.random.default_rng(0)
+    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+    cmd = np.zeros((B, 7)); cmd[:, :3] = [0.6, 0.1, 0.45]; cmd[:, 3:] = [0.5, -0.5, 0.5, -0.5]
+    x = np.zeros((B, 30)); x[:, 8] = 0.45; ee = np.tile([0.52, 0.09, 0.44, 0.5, -0.5, 0.5, -0.5], (B, 1))
+    rows = [f64(cmd), f64(np.full(B, 10.0)), f64(x), f64(ee), f64(ee), torch.zeros(B, dtype=torch.int32, device=dev), torch.zeros((B, 4), dtype=torch.float64, device=dev),
+            torch.zeros((B, 4, 37), dtype=torch.float64, device=dev)]
+    kinds = {"scalar": 0, "per_robot": torch.zeros(B, dtype=torch.int32, device=dev),
+             "per_robot_mixed": torch.as_tensor(rng.integers(-1, 3, B).astype(np.int32), device=dev)}
+    times = {k: [] for k in kinds}
+    for rep in range(reps + 1):   # the first round warms up
+        for name, kind in kinds.items():
+            torch.cuda.synchronize(dev)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+            for _ in range(calls):
+                solver.target_trajectories_dev(kind, *rows, s.cuda_stream)
+            b.record(s); torch.cuda.synchronize(dev)
+            if rep:
+                times[name].append(a.elapsed_time(b) / calls)
+    return {"label": "device time per target call of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            **{"ms_per_call_" + k: float(np.median(v)) for k, v in times.items()}, "spread_per_robot": [float(min(times["per_robot"])), float(max(times["per_robot"]))]}
+
+
+def ee_goals(solver, closed_loop, B, sim_s, xy, upright):
+    """The reach sweep, the target call times, then the runs of sim_s with the goals and with a timeline that changes nothing (wall time)."""
+    import torch
+    b = np.arange(B); bins = dict(dx_m=np.array([-0.1, 0.0, 0.1, 0.2, 0.3, 0.4]), dz_m=np.array([-0.1, 0.0, 0.1]), rot_deg=np.array([0.0, 10.0, 20.0]))
+    idx = dict(dx_m=b % 6, dz_m=(b // 6) % 3, rot_deg=(b // 18) % 3)
+    ee0 = closed_loop.run(solver, duration=0.01, gait="stance", xy_yaw=xy)["start_ee"]
+    goal = ee0.copy(); goal[:, 0] += bins["dx_m"][idx["dx_m"]]; goal[:, 2] += bins["dz_m"][idx["dz_m"]]
+    half = np.radians(bins["rot_deg"][idx["rot_deg"]]) / 2; axis = np.array([1.0, 1.0, 1.0]) / np.sqrt(3.0)
+    rq = np.c_[np.outer(np.sin(half), axis), np.cos(half)]; qx, qy, qz, qw = ee0[:, 3:].T; rx, ry, rz, rw = rq.T   # goal orientation: rq * start's
+    goal[:, 3:] = np.c_[rw * qx + rx * qw + ry * qz - rz * qy, rw * qy - rx * qz + ry * qw + rz * qx, rw * qz + rx * qy - ry * qx + rz * qw, rw * qw - rx * qx - ry * qy - rz * qz]
+    goal[:, 3:] /= np.linalg.norm(goal[:, 3:], axis=1, keepdims=True)
+    sweep = dict(t=np.tile([0.2, 2.5], (B, 1)), gait=np.tile(np.array([None, "stance"], dtype=object), (B, 1)), ee_goal=np.stack([goal, np.full((B, 7), np.nan)], 1))
+    solver.mpc_reset(); solver.wbc_set_input_last(None)
+    r = closed_loop.run(solver, duration=5.0, gait="trot", xy_yaw=xy, commands=sweep)
+    pe = np.linalg.norm(r["ee"][-1, :, :3] - goal[:, :3], axis=1)
+    oe = np.degrees(2.0 * np.arccos(np.clip(np.abs(np.sum(r["ee"][-1, :, 3:] * goal[:, 3:], axis=1)), 0.0, 1.0)))
+    up, bits = upright(r), np.bitwise_or.reduce(r["status"], axis=0)
+    pct = lambda a: [float(np.percentile(a, 50)), float(np.percentile(a, 95))]
+    sweep_bins = {axis: [{"value": float(val), "robots": int(np.sum(idx[axis] == i)), "fallen": int(np.sum(~up[idx[axis] == i])),
+                          "pos_err_m_p50_p95": pct(pe[idx[axis] == i]), "ori_err_deg_p50_p95": pct(oe[idx[axis] == i]),
+                          "status_bits_or": int(np.bitwise_or.reduce(bits[idx[axis] == i]))} for i, val in enumerate(bins[axis])] for axis in bins}
+    walls = {}
+    for name, cmds in (("with_goals", dict(t=np.full((B, 1), 0.2), gait=np.full((B, 1), None, dtype=object), ee_goal=goal[:, None])),
+                       ("timeline_that_changes_nothing", dict(t=np.full((B, 1), 0.2), gait=np.full((B, 1), None, dtype=object)))):
+        solver.mpc_reset(); solver.wbc_set_input_last(None)
+        torch.cuda.synchronize(); t0 = time.perf_counter()
+        closed_loop.run(solver, duration=sim_s, gait="stance", xy_yaw=xy, commands=cmds)
+        torch.cuda.synchronize(); walls[name] = (time.perf_counter() - t0) / sim_s
+    return {"reach_sweep": {"label": "5 s: trot from the start at yaw 0, one goal at 0.2 s (offset from the start pose), stance commanded at 2.5 s (in force from 3.5 s); "
+                                     "errors of the end effector against the goal at the end; fallen = min base z <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite",
+                            "bins": sweep_bins, "fallen": int(np.sum(~up)), "pos_err_m_p50_p95": pct(pe), "ori_err_deg_p50_p95": pct(oe)},
+            "target_call": target_call_times(solver),
+            "wall_s_per_sim_s": {"label": "stance runs of %.2f s from a cold MPC / WBC state" % sim_s, **walls}}
+
+
 def watch_state_est(solver):
     """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
     error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
@@ -343,6 +412,7 @@ def main():
     ap.add_argument("--attitude-filter", action="store_true", help="with --state-estimator: filter the IMU orientation before the estimator reads it")
     ap.add_argument("--slip-detector", action="store_true", help="with --state-estimator: keep slipping stance feet out of the estimate")
     ap.add_argument("--gait-commands", action="store_true", help="time the device gait schedule in the loop and run a gait switch sweep")
+    ap.add_argument("--ee-goals", action="store_true", help="end-effector goals on the device command timeline: a reach sweep and the target call's time")
     args = ap.parse_args()
     if args.vary and args.terrain:
         ap.error("--vary and --terrain are separate sweeps")
@@ -496,6 +566,8 @@ def main():
     if args.gait_commands:
         extra["gait_commands"] = {**gait_commands(solver, closed_loop, B, sim_s, cmd, xy, kw, upright), "gpu": name, "power_limit": limit,
                                   "wall_s_per_sim_s_without_commands": wall / sim_s}
+    if args.ee_goals:
+        extra["ee_goals"] = {**ee_goals(solver, closed_loop, B, sim_s, xy, upright), "gpu": name, "power_limit": limit, "wall_s_per_sim_s_without_commands": wall / sim_s}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
