@@ -80,6 +80,13 @@ PAYLOAD_LAYOUT = ("m_ee", "o_ee_x", "o_ee_y", "o_ee_z", "m_base", "o_base_x", "o
 # the controller's model payload (qmb200_set_model_payload) has PAYLOAD_LAYOUT too; per robot it yields SRBD_LAYOUT (qmb200_debug_srbd_constants)
 SRBD_LAYOUT = ("m",) + tuple("I_nom_%d%d" % (i, j) for i in range(3) for j in range(3)) + tuple("I_nom_inv_%d%d" % (i, j) for i in range(3) for j in range(3)) + \
               ("c_nom_x", "c_nom_y", "c_nom_z", "pad0", "pad1")
+# per-robot controller tuning (qmb200_set_robot_tuning): field -> (offset, width) in a row of TUNING doubles; the WBC gains in WbcGains order
+TUNING_LAYOUT = {}
+for _n, _w in [("friction_mu", 1), ("wbc_friction", 1), ("mu_ee_pos", 1), ("mu_ee_ori", 1), ("mu_final_ee_pos", 1), ("mu_final_ee_ori", 1)] + \
+              [(_f, getattr(_t, "_length_", 1)) for _f, _t in WbcGains._fields_] + [("kp_arm_wbc", 1), ("kd_arm_wbc", 1)]:
+    TUNING_LAYOUT[_n] = (sum(w for _, w in TUNING_LAYOUT.values()), _w)
+TUNING = sum(w for _, w in TUNING_LAYOUT.values())   # QMB200_TUNING
+del _n, _w
 WRENCH_LAYOUT = ("f_base_x", "f_base_y", "f_base_z", "n_base_x", "n_base_y", "n_base_z", "f_ee_x", "f_ee_y", "f_ee_z", "n_ee_x", "n_ee_y", "n_ee_z")
 
 
@@ -114,6 +121,9 @@ PROTOTYPES = {
     "qmb200_centroidal_state_from_rbd": (I32, [P, I32, P, P]),
     "qmb200_set_model_payload": (I32, [P] * 2),
     "qmb200_get_model_payload": (I32, [P] * 3),
+    "qmb200_set_robot_tuning": (I32, [P] * 2),
+    "qmb200_get_robot_tuning": (I32, [P] * 3),
+    "qmb200_get_handle_tuning": (I32, [P] * 2),
     "qmb200_payload_est_get_params": (I32, [P] * 2),
     "qmb200_payload_est_set_params": (I32, [P] * 2),
     "qmb200_payload_est_reset": (I32, [P] * 2),

@@ -55,7 +55,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None, ground_map=None, commands=None):
+        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -103,6 +103,9 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     every tick), a cmd_vel row back to the cmd_vel stream.  For both end-effector commands the base target is the end-effector target minus
     (0.52, 0.09) in the world frame, as upstream computes it: meant for robots facing +x.  With commands every target call takes each robot's kind
     from its gait step (Solver.target_trajectories_dev with a per-robot kind).
+    tuning: the controller's per-robot tuning rows for this run (Solver.set_robot_tuning): dict field of _lib.TUNING_LAYOUT -> scalar or [B] ([k] or [B, k]
+    for the vector gains), fields not named at the handle's own values; friction_mu="plant" / wbc_friction="plant" take this run's plant friction
+    (friction_mu's value, or the handle's robot params or plant params).  The previous rows are restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
@@ -135,6 +138,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     if slip_detector is not None and state_estimator is None:
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     gd = None if commands is None else _gait_commands(solver.batch, gait, commands)
+    tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
         if terrain is not None:
@@ -143,6 +147,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_ground_map(solver, terrain if ground_map is True else ground_map))
         if model_payload is not None:
             scope.enter_context(_model_payload(solver, model_payload, payload))
+        if tn is not None:
+            scope.enter_context(_robot_tuning(solver, tn, friction_mu))
         if payload_estimator is not None:
             scope.enter_context(_payload_estimator(solver, payload_estimator))
         if state_estimator is not None:
@@ -263,6 +269,41 @@ def _model_payload(solver, model_payload, payload):
         yield
     finally:
         solver.set_model_payload(prev_model)
+
+
+def _tuning_spec(B, tuning):
+    """closed_loop.run's tuning → dict field -> float array shaped as Solver.set_robot_tuning takes it, or "plant"; ValueError when malformed"""
+    if not isinstance(tuning, dict):
+        raise ValueError("closed_loop.run: tuning must be a dict of robot tuning fields, got %r" % (tuning,))
+    out = {}
+    for k, v in tuning.items():
+        if k not in _lib.TUNING_LAYOUT:
+            raise ValueError("closed_loop.run: unknown tuning field %r (one of %s)" % (k, ", ".join(_lib.TUNING_LAYOUT)))
+        if isinstance(v, str):
+            if v != "plant" or k not in ("friction_mu", "wbc_friction"):
+                raise ValueError("closed_loop.run: tuning %s must be numbers%s, got %r" % (k, " or \"plant\"" if k in ("friction_mu", "wbc_friction") else "", v))
+            out[k] = v; continue
+        w = _lib.TUNING_LAYOUT[k][1]; a = np.asarray(v, dtype=np.float64)
+        if a.shape not in ((), (B, w), (B,) if w == 1 else (w,)):
+            raise ValueError("closed_loop.run: tuning %s must be a scalar, %s, got shape %s" % (k, "[%d]" % B if w == 1 else "[%d] or [%d, %d]" % (w, B, w), a.shape))
+        if not np.all(np.isfinite(a)) or np.any(a <= 0.0 if k in ("friction_mu", "wbc_friction") else a < 0.0):
+            raise ValueError("closed_loop.run: tuning %s must be finite and %s" % (k, "> 0" if k in ("friction_mu", "wbc_friction") else ">= 0"))
+        out[k] = a
+    return out
+
+
+@contextlib.contextmanager
+def _robot_tuning(solver, spec, friction_mu):
+    prev = solver.get_robot_tuning()
+    try:
+        if any(isinstance(v, str) for v in spec.values()):
+            plant = friction_mu if friction_mu is not None else solver.sim_get_robot_params()["friction_mu"]
+            plant = solver.sim_get_params()["friction_mu"] if plant is None else plant
+            spec = {k: (np.broadcast_to(np.asarray(plant, dtype=np.float64), (solver.batch,)) if isinstance(v, str) else v) for k, v in spec.items()}
+        solver.set_robot_tuning(spec)
+        yield
+    finally:
+        solver.set_robot_tuning(prev)
 
 
 @contextlib.contextmanager

@@ -23,7 +23,8 @@
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
                        double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0 = 0, int b1 = -1, int32_t* diag = nullptr,
-                       const double* srbd = nullptr, const double* payload = nullptr);   // srbd [B][SRBD_DBL] / payload [B][8]: the model payload (NULL: none)
+                       const double* srbd = nullptr, const double* payload = nullptr,    // srbd [B][SRBD_DBL] / payload [B][8]: the model payload (NULL: none)
+                       const double* tuning = nullptr);                                  // tuning [B][TUNING_DBL]: the robot tuning rows (NULL: none)
 int wbc_configure_device();   // per-device kernel attributes (opt-in shared memory): wbc_kernel.cu / mpc_kernels.cu
 int mpc_configure_device();
 }
@@ -64,6 +65,7 @@ struct qmb200_handle {
   RobotArray terrain{3};          // per-robot [tile, origin_x, origin_y] on the tile library (qmb200_sim_set_robot_terrain)
   struct { std::vector<double> host; double* d = nullptr; int n_tiles = 0, nx = 0, ny = 0; double cell = 0.0; } tiles;   // heightfield library (qmb200_sim_set_terrain)
   RobotArray mpayload{8}, srbd{SRBD_DBL};   // the controller's model payload (qmb200_set_model_payload) and the robots' SRBD constants it gives
+  RobotArray tuning{TUNING_DBL};            // per-robot controller parameters (qmb200_set_robot_tuning): Tuning, then the control law's arm kp / kd
   qmb200_payload_est_params est_prm{}; double* d_est = nullptr;   // payload estimator (capi_est.inc): parameters and state [B][EST_DBL], NULL when not running
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
   qmb200_state_est_params se_prm{}; double* d_se = nullptr;        // base state estimator: parameters and state [B][SE_DBL], NULL when not running
@@ -161,10 +163,10 @@ class Staging {
   }
 };
 
-// WbcBase::update of robots [b0, b1) with the handle's model, WBC state (input_last, diagnostics) and model payload
+// WbcBase::update of robots [b0, b1) with the handle's model, WBC state (input_last, diagnostics), model payload and robot tuning rows
 void wbc_launch(qmb200_handle* h, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time, double* cmd,
                 int32_t* status, cudaStream_t s, int b0 = 0, int b1 = -1) {
-  launch_wbc_update(h->d_model, h->B, x_des, u_des, rbd, mode, period, time, h->d_input_last, h->variant, cmd, status, s, b0, b1, h->d_wbc_diag, h->srbd.dev(), h->mpayload.dev());
+  launch_wbc_update(h->d_model, h->B, x_des, u_des, rbd, mode, period, time, h->d_input_last, h->variant, cmd, status, s, b0, b1, h->d_wbc_diag, h->srbd.dev(), h->mpayload.dev(), h->tuning.dev());
   h->launches += 1;
 }
 }  // namespace
@@ -291,6 +293,50 @@ int qmb200_debug_srbd_constants(const qmb200_config* cfg, int32_t n, const doubl
   } catch (const std::exception& e) { g_create_error = e.what(); return -2; }
 }
 
+// ------------------------------------------------------------------ robot tuning
+static_assert(TUNING_DBL == QMB200_TUNING && TUNING_MODEL == 6 + sizeof(qmb200_wbc_gains) / 8, "tuning row of include/qmb200.h: Tuning, then the two arm gains");
+}  // extern "C"
+namespace {
+// Field names of a tuning row (include/qmb200.h), for the validation messages; the 32 WBC gains in qmb200_wbc_gains order
+const char* tuning_field(int i) {
+  static const char* const head[14] = {"friction_mu", "wbc_friction", "mu_ee_pos", "mu_ee_ori", "mu_final_ee_pos", "mu_final_ee_ori", "kp_swing", "kd_swing",
+                                       "base_height_kp", "base_height_kd", "kp_base_linear", "kd_base_linear", "kp_base_angular", "kd_base_angular"};
+  static const char* const vec[6] = {"kp_arm_joint", "kd_arm_joint", "kp_ee_linear", "kd_ee_linear", "kp_ee_angular", "kd_ee_angular"};
+  static const int start[7] = {14, 20, 26, 29, 32, 35, 38};
+  static thread_local std::string name;
+  if (i < 14) return head[i];
+  if (i == TUNING_ARM_KP) return "kp_arm_wbc";
+  if (i == TUNING_ARM_KD) return "kd_arm_wbc";
+  int v = 0; while (i >= start[v + 1]) ++v;
+  name = std::string(vec[v]) + "[" + std::to_string(i - start[v]) + "]"; return name.c_str();
+}
+// the handle's values as one tuning row: DevModel's tuned block and the control law's arm gains
+void handle_tuning(const qmb200_handle* h, double* row) {
+  std::memcpy(row, tuning_of(&h->hm.dev, nullptr, 0), sizeof(Tuning)); row[TUNING_ARM_KP] = h->law_prm.arm_kp; row[TUNING_ARM_KD] = h->law_prm.arm_kd;
+}
+}  // namespace
+extern "C" {
+
+int qmb200_set_robot_tuning(qmb200_handle* h, const double* rows) {
+  if (!h) return -1; const size_t B = (size_t)h->B;
+  if (rows) for (size_t b = 0; b < B; ++b) for (int i = 0; i < TUNING_DBL; ++i) {
+    const double v = rows[b * TUNING_DBL + i];
+    const char* why = !std::isfinite(v) ? "must be finite" : (i < 2 && !(v > 0.0)) ? "must be > 0" : (v < 0.0) ? "must be >= 0" : nullptr;
+    if (why) return fail(h, std::string("qmb200_set_robot_tuning: ") + tuning_field(i) + " of robot " + std::to_string(b) + " " + why);
+  }
+  return set_robot_arrays(h, {{&h->tuning, rows}});
+}
+int qmb200_get_robot_tuning(const qmb200_handle* h, double* rows, int32_t* is_set) {
+  if (!h) return -1; const size_t B = (size_t)h->B; const std::vector<double>& t = h->tuning.host;
+  if (rows) { if (t.empty()) for (size_t b = 0; b < B; ++b) handle_tuning(h, rows + b * TUNING_DBL); else std::memcpy(rows, t.data(), B * TUNING_DBL * 8); }
+  if (is_set) *is_set = t.empty() ? 0 : 1;
+  return 0;
+}
+int qmb200_get_handle_tuning(const qmb200_handle* h, double* row) {
+  if (!h) return -1; if (!row) return fail(const_cast<qmb200_handle*>(h), "qmb200_get_handle_tuning: null row");
+  handle_tuning(h, row); return 0;
+}
+
 int qmb200_get_dims(const qmb200_handle* h, int32_t* batch, int32_t* nmax, int32_t* emax, int32_t* kmax) {
   if (!h) return -1; if (batch) *batch = h->B; if (nmax) *nmax = h->nmax; if (emax) *emax = QMB200_EMAX; if (kmax) *kmax = QMB200_KMAX; return 0;
 }
@@ -341,6 +387,7 @@ int qmb200_wbc_get_gains(const qmb200_handle* h, qmb200_wbc_gains* g) {
   for (int i = 0; i < 3; ++i) { g->kp_ee_linear[i] = d.ee_linear_kp[i]; g->kd_ee_linear[i] = d.ee_linear_kd[i]; g->kp_ee_angular[i] = d.ee_angular_kp[i]; g->kd_ee_angular[i] = d.ee_angular_kd[i]; }
   return 0;
 }
+// the handle's gains: robots with a tuning row (qmb200_set_robot_tuning) use the row's instead until the rows are cleared
 int qmb200_wbc_set_gains(qmb200_handle* h, const qmb200_wbc_gains* g) {
   if (!h) return -1; if (!g) return fail(h, "qmb200_wbc_set_gains: null gains");
   QMB_CUDA(h, cudaSetDevice(h->device)); DevModel& d = h->hm.dev;

@@ -29,7 +29,8 @@ int launch_observation(const DevModel* mdl, int B, const double* rbd, const doub
 int launch_target(const TargetParams& prm, int kind, const int32_t* kinds, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
                   double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s);
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,
-                       double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s);
+                       double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s,
+                       const double* tuning /*[B][TUNING_DBL] or NULL: the robots' arm gains in place of prm's*/);
 int launch_hw_write(int B, double delay, const double* time, const double* period, const double* joint_cmd, const double* joint_pos, const double* joint_vel,
                     double* ring_cmd, double* ring_stamp, int32_t* ring_state, double* effort, int32_t* status, cudaStream_t s);
 

@@ -121,13 +121,14 @@ __global__ void __launch_bounds__(128) ctrl_target_kernel(TargetParams prm, int 
 // -----------------------------------------------------------------------------------------------------------------
 // Control law: one thread per (robot, joint).  joint_cmd[b][j] = (posDes, velDes, kp, kd, ff) as HybridJointHandle::setCommand receives them.
 // variant 0 (QMController): legs only once time > 10 (before that the handle keeps its previous command: the entry is left untouched);
-//   arm joints (posDes, 0, arm_kp, arm_kd, torque).
+//   arm joints (posDes, 0, arm_kp, arm_kd, torque), with the robot's own arm gains when it has a tuning row (tuning [B][TUNING_DBL], NULL: none).
 // variant 1 (QMMpcController): legs always; the arm is position controlled at 100 Hz: arm_pos_cmd[b][j] = state(24+j) + velDes(12+j)/100
 //   whenever time - last_time > 1/100 (last_time is then advanced); its hybrid entries are left untouched.
 // status: bit 0 = SafetyChecker orientation check failed (|roll| > pi/2 → the reference calls stopRequest).
 __global__ void __launch_bounds__(ControlLawParams::THREADS) ctrl_control_law_kernel(ControlLawParams prm, int B, const double* __restrict__ x_des, const double* __restrict__ u_des, const double* __restrict__ wbc_cmd,
                                                                                       const double* __restrict__ t_obs, const double* __restrict__ x_obs, double* __restrict__ joint_cmd /*[B][18][5]*/,
-                                                                                      double* __restrict__ arm_pos_cmd /*[B][6]*/, double* __restrict__ last_time /*[B]*/, int32_t* __restrict__ status) {
+                                                                                      double* __restrict__ arm_pos_cmd /*[B][6]*/, double* __restrict__ last_time /*[B]*/, int32_t* __restrict__ status,
+                                                                                      const double* __restrict__ tuning) {
   const int b = blockIdx.x * ControlLawParams::ROBOTS + threadIdx.x / NJ, j = threadIdx.x % NJ;
   const bool live = threadIdx.x < ControlLawParams::ROBOTS * NJ && b < B;
   double t = 0.0, lt = 0.0;
@@ -138,7 +139,9 @@ __global__ void __launch_bounds__(ControlLawParams::THREADS) ctrl_control_law_ke
     if (j < 12) {
       if (prm.variant == 1 || t > 10.0) { jc[0] = pos_des; jc[1] = vel_des; jc[2] = 0.0; jc[3] = 3.0; jc[4] = tau; }
     } else if (prm.variant == 0) {
-      jc[0] = pos_des; jc[1] = 0.0; jc[2] = prm.arm_kp; jc[3] = prm.arm_kd; jc[4] = tau;
+      double kp = prm.arm_kp, kd = prm.arm_kd;
+      if (tuning) { const double* tr = tuning + (size_t)b * TUNING_DBL; kp = tr[TUNING_ARM_KP]; kd = tr[TUNING_ARM_KD]; }
+      jc[0] = pos_des; jc[1] = 0.0; jc[2] = kp; jc[3] = kd; jc[4] = tau;
     } else {
       lt = last_time[b];
       if (t - lt > 1.0 / 100.0) arm_pos_cmd[(size_t)b * 6 + j - 12] = x_obs[(size_t)b * NX + 12 + j] + vel_des * 1.0 / 100.0;
@@ -189,8 +192,8 @@ int launch_target(const TargetParams& prm, int kind, const int32_t* kinds, int B
   ctrl_target_kernel<<<(B + 127) / 128, 128, 0, s>>>(prm, kind, kinds, B, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states); return 1;
 }
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,
-                       double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s) {
-  ctrl_control_law_kernel<<<(B + ControlLawParams::ROBOTS - 1) / ControlLawParams::ROBOTS, ControlLawParams::THREADS, 0, s>>>(prm, B, x_des, u_des, wbc_cmd, t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time, status); return 1;
+                       double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s, const double* tuning) {
+  ctrl_control_law_kernel<<<(B + ControlLawParams::ROBOTS - 1) / ControlLawParams::ROBOTS, ControlLawParams::THREADS, 0, s>>>(prm, B, x_des, u_des, wbc_cmd, t_obs, x_obs, joint_cmd, arm_pos_cmd, last_time, status, tuning); return 1;
 }
 int launch_hw_write(int B, double delay, const double* time, const double* period, const double* joint_cmd, const double* joint_pos, const double* joint_vel,
                     double* ring_cmd, double* ring_stamp, int32_t* ring_state, double* effort, int32_t* status, cudaStream_t s) {

@@ -50,18 +50,21 @@ struct DevModel {
   double I_nom[9], I_nom_inv[9], c_nom[3];   // SRBD centroidalInertiaNominal, its inverse, comToBasePositionNominal
   double effort[NJ];
   double arm_pos_lower[6], arm_pos_upper[6];
-  // WBC gains (wbcWigeht.cfg:7-47) and friction (task.info:346-349)
-  double kp_swing, kd_swing, base_height_kp, base_height_kd, base_linear_kp, base_linear_kd, base_angular_kp, base_angular_kd;
-  double arm_joint_kp[6], arm_joint_kd[6], ee_linear_kp[3], ee_linear_kd[3], ee_angular_kp[3], ee_angular_kd[3];
-  double wbc_friction;
   // MPC settings (task.info:75-92,138-147,192-343)
   double Q[NX * NX], R[NU * NU];
   double Qdiag[NX]; int q_is_diag;   // Q of task.info:192-233 is diagonal: fast path when the loaded matrix really is (checked at create), dense fallback otherwise
   double Rblk[8][9], Rarm[6];   // R is block diagonal (QMInterface.cpp:274-299): 3x3 blocks per foot force / per leg, diagonal for the arm; checked at create
-  double mu_ee_pos, mu_ee_ori, mu_final_ee_pos, mu_final_ee_ori;
-  double friction_mu, friction_barrier_mu, friction_barrier_delta, friction_reg, friction_hess_shift;
+  // what the projection kernel reads per node stays on adjacent cache lines, from Qdiag to the end-effector weights of the tuned block
   double pos_limit_mu, pos_limit_delta, vel_limit_mu, vel_limit_delta;
   double arm_vel_lower[6], arm_vel_upper[6];
+  double friction_barrier_mu, friction_barrier_delta, friction_reg, friction_hess_shift;
+  // The tuned block, in Tuning's order (a robot with a tuning row reads its own copy, qmb200_set_robot_tuning): the MPC friction-cone coefficient
+  // (task.info:290-292), the WBC friction pyramid (task.info:346-348), the end-effector soft-constraint weights (task.info:235-246) and the WBC gains
+  // (wbcWigeht.cfg:7-47)
+  double friction_mu, wbc_friction;
+  double mu_ee_pos, mu_ee_ori, mu_final_ee_pos, mu_final_ee_ori;
+  double kp_swing, kd_swing, base_height_kp, base_height_kd, base_linear_kp, base_linear_kd, base_angular_kp, base_angular_kd;
+  double arm_joint_kp[6], arm_joint_kd[6], ee_linear_kp[3], ee_linear_kd[3], ee_angular_kp[3], ee_angular_kd[3];
   double lift_off_velocity, touch_down_velocity, swing_height, swing_time_scale, position_error_gain;
   double dt, time_horizon, delta_tol, g_max, g_min, alpha_decay, alpha_min, gamma_c, armijo_factor;
   double rk_c, rk_w1, rk_w2;
@@ -82,6 +85,25 @@ static_assert(offsetof(DevModel, I_nom) == offsetof(DevModel, total_mass) + offs
               offsetof(DevModel, c_nom) == offsetof(DevModel, total_mass) + offsetof(SrbdConst, c_nom) && sizeof(SrbdConst) <= SRBD_DBL * 8, "DevModel's SRBD fields have SrbdConst's layout");
 QMB_HD const SrbdConst* srbd_of(const DevModel* mdl, const double* srbd, int b) {
   return srbd ? reinterpret_cast<const SrbdConst*>(srbd + (size_t)SRBD_DBL * b) : reinterpret_cast<const SrbdConst*>(&mdl->total_mass);
+}
+
+// The controller parameters one robot may override (qmb200_set_robot_tuning), in the order DevModel keeps the handle's: the first TUNING_MODEL doubles of a
+// tuning row.  The row's last two doubles are the control law's arm gains (ControlLawParams arm_kp / arm_kd), read by the control law alone.  As with
+// SrbdConst, every consumer reads through one pointer: tuning_of(mdl, rows, b) with rows = the per-robot rows, or NULL for the handle's values.
+struct Tuning {
+  double friction_mu, wbc_friction, mu_ee_pos, mu_ee_ori, mu_final_ee_pos, mu_final_ee_ori;
+  double kp_swing, kd_swing, base_height_kp, base_height_kd, base_linear_kp, base_linear_kd, base_angular_kp, base_angular_kd;
+  double arm_joint_kp[6], arm_joint_kd[6], ee_linear_kp[3], ee_linear_kd[3], ee_angular_kp[3], ee_angular_kd[3];
+};
+constexpr int TUNING_MODEL = 38, TUNING_DBL = 40, TUNING_ARM_KP = 38, TUNING_ARM_KD = 39;
+static_assert(sizeof(Tuning) == TUNING_MODEL * 8 && offsetof(DevModel, ee_angular_kd) + 3 * 8 - offsetof(DevModel, friction_mu) == sizeof(Tuning) &&
+              offsetof(DevModel, wbc_friction) == offsetof(DevModel, friction_mu) + offsetof(Tuning, wbc_friction) &&
+              offsetof(DevModel, mu_ee_pos) == offsetof(DevModel, friction_mu) + offsetof(Tuning, mu_ee_pos) &&
+              offsetof(DevModel, kp_swing) == offsetof(DevModel, friction_mu) + offsetof(Tuning, kp_swing) &&
+              offsetof(DevModel, arm_joint_kp) == offsetof(DevModel, friction_mu) + offsetof(Tuning, arm_joint_kp) &&
+              offsetof(DevModel, ee_angular_kd) == offsetof(DevModel, friction_mu) + offsetof(Tuning, ee_angular_kd), "DevModel's tuned fields have Tuning's layout");
+QMB_HD const Tuning* tuning_of(const DevModel* mdl, const double* rows, int b) {
+  return rows ? reinterpret_cast<const Tuning*>(rows + (size_t)TUNING_DBL * b) : reinterpret_cast<const Tuning*>(&mdl->friction_mu);
 }
 
 #ifdef __CUDACC__

@@ -57,9 +57,10 @@ struct MpcBuffers {
 bool mpc_alloc(MpcBuffers& m, int B, int nmax, std::string& err, std::vector<void*>& allocs, cudaStream_t stream);
 int mpc_configure_device();   // per-device opt-in shared memory of the MPC kernels (qmb200_create, after cudaSetDevice)
 
-// srbd: per-robot SRBD constants [B][SRBD_DBL] (qmb200_set_model_payload), indexed by the global robot index; NULL = the model's (DevModel) for every robot
+// srbd: per-robot SRBD constants [B][SRBD_DBL] (qmb200_set_model_payload), indexed by the global robot index; NULL = the model's (DevModel) for every robot.
+// tuning: per-robot tuning rows [B][TUNING_DBL] (qmb200_set_robot_tuning), indexed the same way; NULL = the handle's values (DevModel) for every robot.
 struct MpcProblemDev { const double* t0; const double* x0; const int32_t* n_events; const double* event_times; const int32_t* modes; const int32_t* n_target; const double* target_times; const double* target_states;
-                       const double* srbd; };
+                       const double* srbd; const double* tuning; };
 
 // One SQP iteration for robots [b0, b1) (4 kernels on `stream`): reads m.sol[m.cur], writes m.sol[1 - m.cur]; the caller
 // flips m.cur after queueing every range.  Returns the number of kernels launched.

@@ -19,9 +19,10 @@ __device__ __forceinline__ double target_xnom(const double* tt, const double* ts
 }
 
 // Intermediate (or terminal) cost value and its quadratic model in the compact form of QuadWs (NOT scaled by dt).  ws: {x[30], u[30]} of the node; cw: end-effector
-// error e[6] and its Jacobian Je[6][12] (flow kernel); sc: the robot's SRBD constants (srbd_of); xnom: this lane's state reference; `flagmask` = contact flags (bit i = foot i).  Returns the value (lane-uniform).
+// error e[6] and its Jacobian Je[6][12] (flow kernel); sc: the robot's SRBD constants (srbd_of); tn: the robot's end-effector weights and friction coefficient (tuning_of);
+// xnom: this lane's state reference; `flagmask` = contact flags (bit i = foot i).  Returns the value (lane-uniform).
 template <class WS, class CW>
-__device__ __forceinline__ double stage_cost_quad(const DevModel* __restrict__ mdl, const SrbdConst* sc, const WS* ws, const CW* cw, QuadWs* qw, double xnom, int flagmask, bool terminal, int lane) {
+__device__ __forceinline__ double stage_cost_quad(const DevModel* __restrict__ mdl, const SrbdConst* sc, const Tuning* tn, const WS* ws, const CW* cw, QuadWs* qw, double xnom, int flagmask, bool terminal, int lane) {
   double value = 0.0;
   for (int e = lane; e < 144; e += 32) qw->E[e] = 0.0; for (int e = lane; e < 36; e += 32) qw->fric[e] = 0.0; if (lane < NX) { qw->qdiag[lane] = 0.0; qw->rdiag[lane] = 0.0; qw->qf[lane] = 0.0; qw->rf[lane] = 0.0; } __syncwarp();
   int nst = 0; for (int i = 0; i < 4; ++i) nst += (flagmask >> i) & 1;
@@ -44,7 +45,7 @@ __device__ __forceinline__ double stage_cost_quad(const DevModel* __restrict__ m
   }
   // end-effector soft constraint (quadratic penalty, Gauss-Newton)
   {
-    const double mup = terminal ? mdl->mu_final_ee_pos : mdl->mu_ee_pos, muo = terminal ? mdl->mu_final_ee_ori : mdl->mu_ee_ori;
+    const double mup = terminal ? tn->mu_final_ee_pos : tn->mu_ee_pos, muo = terminal ? tn->mu_final_ee_ori : tn->mu_ee_ori;
     double v = 0.0; for (int r = 0; r < 6; ++r) v += 0.5 * (r < 3 ? mup : muo) * cw->e[r] * cw->e[r]; value += v;
     {
       for (int e = lane; e < 144; e += 32) { const int i = e / 12, j = e % 12; double s = 0.0; for (int r = 0; r < 6; ++r) s += (r < 3 ? mup : muo) * cw->Je[r * 12 + i] * cw->Je[r * 12 + j]; qw->E[e] = s; }
@@ -69,9 +70,9 @@ __device__ __forceinline__ double stage_cost_quad(const DevModel* __restrict__ m
       const int i = lane - 12;
       if ((flagmask >> i) & 1) {
         const double Fx = ws->u[3 * i], Fy = ws->u[3 * i + 1], Fz = ws->u[3 * i + 2]; const double n2 = Fx * Fx + Fy * Fy + mdl->friction_reg, n = sqrt(n2), in = 1.0 / n, in32 = in * in * in;
-        const double h = mdl->friction_mu * Fz - n; double p0, p1, p2; relaxed_barrier(mdl->friction_barrier_mu, mdl->friction_barrier_delta, h, p0, p1, p2); bv = p0;
+        const double h = tn->friction_mu * Fz - n; double p0, p1, p2; relaxed_barrier(mdl->friction_barrier_mu, mdl->friction_barrier_delta, h, p0, p1, p2); bv = p0;
         {
-          const double g[3] = {-Fx * in, -Fy * in, mdl->friction_mu}; const double H2[9] = {-(Fy * Fy + mdl->friction_reg) * in32, Fx * Fy * in32, 0, Fx * Fy * in32, -(Fx * Fx + mdl->friction_reg) * in32, 0, 0, 0, 0};
+          const double g[3] = {-Fx * in, -Fy * in, tn->friction_mu}; const double H2[9] = {-(Fy * Fy + mdl->friction_reg) * in32, Fx * Fy * in32, 0, Fx * Fy * in32, -(Fx * Fx + mdl->friction_reg) * in32, 0, 0, 0, 0};
           for (int a = 0; a < 3; ++a) { qw->rf[3 * i + a] += p1 * g[a]; for (int b = 0; b < 3; ++b) qw->fric[i * 9 + 3 * a + b] = p2 * g[a] * g[b] + p1 * H2[3 * a + b]; }
           shift = -p1 * mdl->friction_hess_shift;
         }

@@ -215,6 +215,8 @@ __device__ __forceinline__ double flow_inner(const ne::FlowBlk& fb, int r, int q
   if (q < 6) return 0.0;
   return r < 3 ? fb.hth[q - 6][r] : (r < 6 ? fb.vp[q - 6][r - 3] : fb.vt[q - 6][r - 6]);
 }
+// TUNED: the batch has robot tuning rows (p.tuning).  Without them the kernel reads the model's block at its fixed place in DevModel, as it did before rows existed.
+template <bool TUNED>
 __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(const DevModel* __restrict__ mdl, int b0, int B, int nmax, MpcProblemDev p, MpcSolutionDev sol, const double* __restrict__ rec, double* __restrict__ stage, int32_t* __restrict__ status) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31; const long long gid = (long long)blockIdx.x * LQ_WARPS + warp;
@@ -263,7 +265,7 @@ __global__ void __launch_bounds__(32 * LQ_WARPS, QMB_LQ_MINB) mpc_lq_kernel(cons
   {
   // ---- cost quadratic model at (x, u) (the end-effector error and its Jacobian come with the record) ----
   struct XU { double x[NX], u[NU]; }; static_assert(offsetof(LqSmem, u) == offsetof(LqSmem, x) + NX * 8, "x then u");
-  cost_val = stage_cost_quad(mdl, sc, reinterpret_cast<const XU*>(sm.x), &sm.rec.ee, &sm.quad, target_xnom(tt, ts, nk, t, lane), fm, terminal, lane);
+  cost_val = stage_cost_quad(mdl, sc, tuning_of(mdl, TUNED ? p.tuning : nullptr, b), reinterpret_cast<const XU*>(sm.x), &sm.rec.ee, &sm.quad, target_xnom(tt, ts, nk, t, lane), fm, terminal, lane);
   if (terminal) {   // setupTerminalNode: finalEndEffector soft constraint only (QMInterface.cpp:104)
     double* tl = sg + ST_TAIL; int32_t* si = reinterpret_cast<int32_t*>(tl + T_INT);
     for (int r = 0; r < NX; ++r) { const int a = ee_pos(r); if (lane < q_row_padded(r)) { const int cc = (lane <= r) ? ee_pos(lane) : -1; sg[ST_Q + q_row_offset(r) + lane] = (a >= 0 && cc >= 0) ? sm.quad.E[a * 12 + cc] : 0.0; } }   // final cost: packed lower triangle
@@ -899,7 +901,7 @@ __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_ker
       ne::flow_finish<false>(mdl, xa, bk, acc, f1, nullptr, srb);
       asm volatile("" ::: "memory");   // f1 is read back after the cost, not held in registers across it
       { const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, xa, bk, pref, qref, ee, nullptr);
-        cost += dt * ne::cost_value(mdl, xa, ua, sg, ee, fm, terminal, srb); }
+        cost += dt * ne::cost_value(mdl, xa, ua, sg, ee, fm, terminal, srb, tuning_of(mdl, p.tuning, b)); }
       if (terminal) continue;
       const double cdt = mdl->rk_c * dt;   // second stage in place (the trial state is re-read from L2 for the defect)
 #pragma unroll
@@ -979,7 +981,7 @@ __global__ void __launch_bounds__(32 * LS_WARPS, QMB_LS_MINB) mpc_linesearch_ker
 constexpr int RO_THREADS = 128, RO_MAXTRIALS = 32;
 // one RK2 step of the flow map from (x, u); with PERF also the node's cost (unscaled by dt) and equality SSE at (x, u).  x is replaced by the next state.
 template <bool PERF, class MT>
-__device__ __forceinline__ void rollout_step(const DevModel* __restrict__ mdl, const SrbdConst* sc, double* x, const double* u, double t, double dt, int fm, const double* ev, const MT* modes, int ne, const double* tt, const double* ts, int nk, double& cost, double& eq) {
+__device__ __forceinline__ void rollout_step(const DevModel* __restrict__ mdl, const SrbdConst* sc, const Tuning* tn, double* x, const double* u, double t, double dt, int fm, const double* ev, const MT* modes, int ne, const double* tt, const double* ts, int nk, double& cost, double& eq) {
   ne::BaseKin bk; ne::FlowAcc acc; double f1[12], x2[NX]; ne::base_eval<false>(mdl, x, bk, sc); ne::flow_acc_init(acc);
   if (PERF) { double es = 0.0; bool ok = true;
 #pragma unroll 1
@@ -987,7 +989,7 @@ __device__ __forceinline__ void rollout_step(const DevModel* __restrict__ mdl, c
       ne::equality_add(mdl, u, fe, pf, fm, ev, modes, ne, t, i, es, ok); }
     eq += dt * es;
     const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, x, bk, pref, qref, ee, nullptr);
-    cost += dt * ne::cost_value(mdl, x, u, sg, ee, fm, false, sc);
+    cost += dt * ne::cost_value(mdl, x, u, sg, ee, fm, false, sc, tn);
   } else {
 #pragma unroll 1
     for (int i = 0; i < 4; ++i) { double d[3]; ne::foot_eval<false>(mdl, x, u, bk, i, acc, d, nullptr, nullptr, nullptr, nullptr, sc); } }
@@ -1040,7 +1042,7 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_kernel(co
       if (ge[k] != 1) { const double t = interval_start(gt[k], ge[k]); const double dt = interval_end(gt[k + 1], ge[k + 1]) - t; double u[NU];
 #pragma unroll
         for (int i = 0; i < NU; ++i) u[i] = gu[(size_t)k * NU + i];
-        rollout_step<false>(mdl, srbd_of(mdl, p.srbd, b), xa, u, t, dt, 0, ev, modes, ne, tt, ts, nk, cost, eq); }
+        rollout_step<false>(mdl, srbd_of(mdl, p.srbd, b), tuning_of(mdl, p.tuning, b), xa, u, t, dt, 0, ev, modes, ne, tt, ts, nk, cost, eq); }
 #pragma unroll
       for (int i = 0; i < NX; ++i) gx[(size_t)(k + 1) * NX + i] = xa[i];
     }
@@ -1071,7 +1073,7 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_kernel(co
         rollout_input(tl, gb + (size_t)k * GAIN_DBL, gu + (size_t)k * NU, dxv, alpha, lfp, un);
         for (int i = 0; i < NU; ++i) gu[(size_t)k * NU + i] = un[i];
         const double t = interval_start(gt[k], ge[k]); const double dt = interval_end(gt[k + 1], ge[k + 1]) - t; const int fm = flag_mask(mode_at_time(ev, modes, ne, t));
-        rollout_step<false>(mdl, srbd_of(mdl, p.srbd, b), xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
+        rollout_step<false>(mdl, srbd_of(mdl, p.srbd, b), tuning_of(mdl, p.tuning, b), xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
       }
       // the nominal state of the next node is read before the new one replaces it (in-place commit)
 #pragma unroll
@@ -1122,7 +1124,7 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_trials_ke
         for (int i = 0; i < NX; ++i) dxv[i] = xa[i] - xnom[i];
         rollout_input(tl, sK + r * GAIN_DBL, gu + (size_t)k * NU, dxv, alpha, lfp, un);
         const double t = interval_start(gt[k], ge[k]); const double dt = interval_end(gt[k + 1], ge[k + 1]) - t; const int fm = flag_mask(mode_at_time(ev, modes, ne, t));
-        rollout_step<true>(mdl, srbd_of(mdl, p.srbd, (int)bb), xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
+        rollout_step<true>(mdl, srbd_of(mdl, p.srbd, (int)bb), tuning_of(mdl, p.tuning, (int)bb), xa, un, t, dt, fm, ev, modes, ne, tt, ts, nk, cost, eq);
       }
 #pragma unroll
       for (int i = 0; i < NX; ++i) xnom[i] = gx[(size_t)(k + 1) * NX + i];
@@ -1131,7 +1133,7 @@ __global__ void __launch_bounds__(RO_THREADS, QMB_RO_MINB) mpc_rollout_trials_ke
   if (active) {   // final cost at x_N
     const double t = interval_start(gt[N], ge[N]); ne::BaseKin bk; ne::base_eval<false>(mdl, xa, bk, srbd_of(mdl, p.srbd, b)); double u0[NU]; for (int i = 0; i < NU; ++i) u0[i] = 0.0;
     const ne::TargetSeg sg = ne::target_segment(tt, ts, nk, t); double pref[3], qref[4], ee[6]; ne::target_pose(sg, nk, pref, qref); ne::ee_eval<false>(mdl, xa, bk, pref, qref, ee, nullptr);
-    cost += ne::cost_value(mdl, xa, u0, sg, ee, 0, true, srbd_of(mdl, p.srbd, b));
+    cost += ne::cost_value(mdl, xa, u0, sg, ee, 0, true, srbd_of(mdl, p.srbd, b), tuning_of(mdl, p.tuning, b));
     double* tb = trial + (size_t)b * RO_MAXTRIALS * 2; tb[2 * tr] = cost; tb[2 * tr + 1] = eq; }
 }
 
@@ -1166,7 +1168,8 @@ int mpc_configure_device() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_flow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FL_SMEM);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_linesearch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LS_SMEM);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_rollout_trials_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RO_RPC_MAX * GAIN_DBL * 8);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_lq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LqSmem) * LQ_WARPS));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_lq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LqSmem) * LQ_WARPS));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_lq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LqSmem) * LQ_WARPS));
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_riccati_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RicSmem));
   return (int)e;
 }
@@ -1187,7 +1190,7 @@ int mpc_solve_launch(const DevModel* mdl, const DevModel& hm, MpcBuffers& m, con
   for (int it = 0; it < iters; ++it) {
     mpc_flow_kernel<<<(unsigned)((nodes + 32 * FL_WARPS - 1) / (32 * FL_WARPS)), 32 * FL_WARPS, FL_SMEM, stream>>>(mdl, b0, b1, nmax, p, next, m.node_rec, m.status);
     if (ev && it == iters - 1) cudaEventRecord(ev[7], stream);
-    mpc_lq_kernel<<<(unsigned)((nodes + LQ_WARPS - 1) / LQ_WARPS), 32 * LQ_WARPS, sizeof(LqSmem) * LQ_WARPS, stream>>>(mdl, b0, b1, nmax, p, next, m.node_rec, m.stage, m.status);
+    (p.tuning ? mpc_lq_kernel<true> : mpc_lq_kernel<false>)<<<(unsigned)((nodes + LQ_WARPS - 1) / LQ_WARPS), 32 * LQ_WARPS, sizeof(LqSmem) * LQ_WARPS, stream>>>(mdl, b0, b1, nmax, p, next, m.node_rec, m.stage, m.status);
     if (ev && it == iters - 1) cudaEventRecord(ev[2], stream);
     mpc_riccati_kernel<<<nb, RIC_THREADS, sizeof(RicSmem), stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.dx, m.du, m.robot, m.status);
     if (ev && it == iters - 1) cudaEventRecord(ev[3], stream);

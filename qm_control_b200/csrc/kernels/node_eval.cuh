@@ -204,8 +204,11 @@ QMB_HD void ee_eval(const DevModel* __restrict__ mdl, const double* x, const Bas
   }
 }
 
-// Intermediate (or terminal) cost VALUE at (x, u) given the end-effector error (stage_cost<false> of mpc_device.cuh; unscaled by dt)
-QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, const double* u, const TargetSeg& sg, const double* ee, int flagmask, bool terminal, const SrbdConst* sc = nullptr) {
+// Intermediate (or terminal) cost VALUE at (x, u) given the end-effector error (stage_cost<false> of mpc_device.cuh; unscaled by dt).  tn: the robot's tuning row
+// (tuning_of), NULL for the model's values.
+QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, const double* u, const TargetSeg& sg, const double* ee, int flagmask, bool terminal, const SrbdConst* sc = nullptr,
+                         const Tuning* tn = nullptr) {
+  if (!tn) tn = tuning_of(mdl, nullptr, 0);
   double value = 0.0;
   if (!terminal) {
     int nst = 0; for (int i = 0; i < 4; ++i) nst += (flagmask >> i) & 1;
@@ -222,7 +225,7 @@ QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, cons
     for (int i = 0; i < 6; ++i) acc = fma(u[24 + i] * mdl->Rarm[i], u[24 + i], acc);
     value += 0.5 * acc;
   }
-  { const double mup = terminal ? mdl->mu_final_ee_pos : mdl->mu_ee_pos, muo = terminal ? mdl->mu_final_ee_ori : mdl->mu_ee_ori;
+  { const double mup = terminal ? tn->mu_final_ee_pos : tn->mu_ee_pos, muo = terminal ? tn->mu_final_ee_ori : tn->mu_ee_ori;
     double v = 0.0; for (int r = 0; r < 6; ++r) v += 0.5 * (r < 3 ? mup : muo) * ee[r] * ee[r]; value += v; }
   if (!terminal) {
     // relaxed log barriers: sum_i -mu log(h_i) = -mu log(prod_i h_i) over the entries in the logarithmic branch (24 + 4 fp64 logarithms become 3); the
@@ -235,7 +238,7 @@ QMB_HD double cost_value(const DevModel* __restrict__ mdl, const double* x, cons
         for (int sd = 0; sd < 2; ++sd) { const double h = h2[sd]; if (h > de) prod *= h; else { const double tq = (h - 2.0 * de) / de; bv += mu * (-log(de) + 0.5 * tq * tq - 0.5); } } }
       bv -= mu * log(prod); }
     { double prod = 1.0; const double mu = mdl->friction_barrier_mu, de = mdl->friction_barrier_delta;   // friction cone soft constraints of the stance feet
-      for (int i = 0; i < 4; ++i) if ((flagmask >> i) & 1) { const double Fx = u[3 * i], Fy = u[3 * i + 1], Fz = u[3 * i + 2]; const double h = mdl->friction_mu * Fz - sqrt(Fx * Fx + Fy * Fy + mdl->friction_reg);
+      for (int i = 0; i < 4; ++i) if ((flagmask >> i) & 1) { const double Fx = u[3 * i], Fy = u[3 * i + 1], Fz = u[3 * i + 2]; const double h = tn->friction_mu * Fz - sqrt(Fx * Fx + Fy * Fy + mdl->friction_reg);
         if (h > de) prod *= h; else { const double tq = (h - 2.0 * de) / de; bv += mu * (-log(de) + 0.5 * tq * tq - 0.5); } }
       bv -= mu * log(prod); }
     value += bv;

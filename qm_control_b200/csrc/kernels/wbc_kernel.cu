@@ -66,6 +66,7 @@ struct WbcSmem {
   double Jc[12 * LJC], djv_f[12], fpos_m[12], fvel_m[12], fpos_d[12], fvel_d[12];
   double Tm[9], wdot_base[3], base_acc[6], fdes[12], lim[NJ], vstar[56];   // fdes: the MPC's contact forces (the rest of x_des / u_des is read from HBM once)
   QpWs qp;
+  Tuning tun;   // the robot's gains and friction pyramid (tuning_of), staged here so that no pointer to them stays live in registers
 };
 
 // ---------------------------------------------------------------------------------------------------------
@@ -149,7 +150,7 @@ __device__ int cod_lstsq(QpWs& qp, double* W, int n, int r, int ldw, const doubl
 //   level 1: HierarchicalWbc: height, base angular, EE linear, EE angular, 100*swing (t>=10) | arm joint tracking (t<10)
 //            HierarchicalMpcWbc: height, base angular, base linear, 100*swing
 //   level 2: contact force + base linear | contact force
-__device__ int build_level(WbcSmem& sm, const DevModel* __restrict__ mdl, int level, int mode, int variant, bool init_phase, int ffp, int lane) {
+__device__ int build_level(WbcSmem& sm, const Tuning* __restrict__ tn, int level, int mode, int variant, bool init_phase, int ffp, int lane) {
   QpWs& qp = sm.qp; double* Ap = qp.za.q.AR; const EeWs& ee = qp.ah.ee; int nc = 0; for (int f = 0; f < 4; ++f) nc += contact_flag(mode, f);
   int rows = 0;
   if (level == 0) rows = 18;
@@ -166,11 +167,11 @@ __device__ int build_level(WbcSmem& sm, const DevModel* __restrict__ mdl, int le
   } else if (level == 1) {
     int row = 0;
     if (variant == 0 && init_phase) {   // formulateArmJointNomalTrackingTask (WbcBase.cpp:439-465)
-      if (lane < 6) { const int k = NQ - 6 + lane; Ap[lane * LDZ + k] = 1.0; qp.bp[lane] = mdl->arm_joint_kp[lane] * (sm.qd[k] - sm.q[k]) + mdl->arm_joint_kd[lane] * (sm.vd[k] - sm.v[k]); }
+      if (lane < 6) { const int k = NQ - 6 + lane; Ap[lane * LDZ + k] = 1.0; qp.bp[lane] = tn->arm_joint_kp[lane] * (sm.qd[k] - sm.q[k]) + tn->arm_joint_kd[lane] * (sm.vd[k] - sm.v[k]); }
       row = 6;
     } else {
       // formulateBaseHeightMotionTask (WbcBase.cpp:296-308)
-      if (lane == 0) { Ap[2] = 1.0; qp.bp[0] = sm.base_acc[2] + mdl->base_height_kp * (sm.qd[2] - sm.q[2]) + mdl->base_height_kd * (sm.vd[2] - sm.v[2]); }
+      if (lane == 0) { Ap[2] = 1.0; qp.bp[0] = sm.base_acc[2] + tn->base_height_kp * (sm.qd[2] - sm.q[2]) + tn->base_height_kd * (sm.vd[2] - sm.v[2]); }
       // formulateBaseAngularMotionTask (WbcBase.cpp:258-293): base_j angular rows are [0 | T | 0]
       if (lane < 3) {
         const int r = lane; for (int k = 0; k < 3; ++k) Ap[(1 + r) * LDZ + 3 + k] = sm.Tm[3 * r + k];
@@ -178,33 +179,33 @@ __device__ int build_level(WbcSmem& sm, const DevModel* __restrict__ mdl, int le
         double Rm[9], Rr[9], err[3]; rot_zyx(sm.q[3], sm.q[4], sm.q[5], Rm); rot_zyx(sm.qd[3], sm.qd[4], sm.qd[5], Rr); rotation_error_world(Rr, Rm, err);
         // getGlobalAngularAccelerationFromEulerAnglesZyxDerivatives(eulerMeasured, eulerRatesDesired, eulerAccDesired) = T edd + Tdot(ed) ed
         double tdd[3], tde[3]; matvec3(sm.Tm, sm.base_acc + 3, tdd); euler_rate_map_dot_times(sm.q[3], sm.q[4], sm.vd + 3, tde);
-        qp.bp[1 + r] = tdd[r] + tde[r] + mdl->base_angular_kp * err[r] + mdl->base_angular_kd * (wD[r] - wM[r]) - sm.wdot_base[r];
+        qp.bp[1 + r] = tdd[r] + tde[r] + tn->base_angular_kp * err[r] + tn->base_angular_kd * (wD[r] - wM[r]) - sm.wdot_base[r];
       }
       row = 4;
       if (variant == 0) {
         // formulateEeLinearMotionTrackingTask (WbcBase.cpp:467-492) and formulateEeAngularMotionTrackingTask (:494-531)
         for (int e = lane; e < 6 * NQ; e += 32) { const int a = e / NQ, k = e % NQ; const bool zero = (a >= 3 && k >= 3 && k < 6); Ap[(row + a) * LDZ + k] = zero ? 0.0 : ee.Jee[a * LDM + k]; }
-        if (lane < 3) qp.bp[row + lane] = mdl->ee_linear_kp[lane] * (ee.ee_d_pos[lane] - ee.ee_m_pos[lane]) + mdl->ee_linear_kd[lane] * (ee.ee_d_vel[lane] - ee.ee_m_vel[lane]) - ee.djv_ee[lane];
+        if (lane < 3) qp.bp[row + lane] = tn->ee_linear_kp[lane] * (ee.ee_d_pos[lane] - ee.ee_m_pos[lane]) + tn->ee_linear_kd[lane] * (ee.ee_d_vel[lane] - ee.ee_m_vel[lane]) - ee.djv_ee[lane];
         if (lane == 3) { double err[3]; rotation_error_world(ee.ee_d_rot, ee.ee_m_rot, err);
           // arm_dj_tmp zeroes columns 3:6 of the angular rows: Jdot_w v minus the base euler part (= Tdot ed = base angular bias acc)
-          for (int a = 0; a < 3; ++a) qp.bp[row + 3 + a] = mdl->ee_angular_kp[a] * err[a] - mdl->ee_angular_kd[a] * ee.ee_m_w[a] - (ee.djv_ee[3 + a] - sm.wdot_base[a]); }
+          for (int a = 0; a < 3; ++a) qp.bp[row + 3 + a] = tn->ee_angular_kp[a] * err[a] - tn->ee_angular_kd[a] * ee.ee_m_w[a] - (ee.djv_ee[3 + a] - sm.wdot_base[a]); }
         row += 6;
       } else {
         // formulateBaseLinearMotionTask (WbcBase.cpp:228-240)
-        if (lane < 2) { Ap[(row + lane) * LDZ + lane] = 1.0; qp.bp[row + lane] = sm.base_acc[lane] + mdl->base_linear_kp * (sm.qd[lane] - sm.q[lane]) + mdl->base_linear_kd * (sm.vd[lane] - sm.v[lane]); }
+        if (lane < 2) { Ap[(row + lane) * LDZ + lane] = 1.0; qp.bp[row + lane] = sm.base_acc[lane] + tn->base_linear_kp * (sm.qd[lane] - sm.q[lane]) + tn->base_linear_kd * (sm.vd[lane] - sm.v[lane]); }
         row += 2;
       }
       // formulateSwingLegTask * 100 (WbcBase.cpp:311-334, HierarchicalWbc.cpp:29)
       for (int f = 0; f < 4; ++f) if (!contact_flag(mode, f)) {
         if (lane < 27) { const int a = lane / 9, c = lane - 9 * a; Ap[(row + a) * LDZ + (c < 6 ? c : foot_first(ffp, f) + c)] = 100.0 * sm.Jc[(3 * f + a) * LJC + c]; }
-        if (lane < 3) { const int i = 3 * f + lane; qp.bp[row + lane] = 100.0 * (mdl->kp_swing * (sm.fpos_d[i] - sm.fpos_m[i]) + mdl->kd_swing * (sm.fvel_d[i] - sm.fvel_m[i]) - sm.djv_f[i]); }
+        if (lane < 3) { const int i = 3 * f + lane; qp.bp[row + lane] = 100.0 * (tn->kp_swing * (sm.fpos_d[i] - sm.fpos_m[i]) + tn->kd_swing * (sm.fvel_d[i] - sm.fvel_m[i]) - sm.djv_f[i]); }
         row += 3;
       }
     }
   } else {
     // formulateContactForceTask (WbcBase.cpp:534-546)
     if (lane < 12) { Ap[lane * LDZ + NQ + lane] = 1.0; qp.bp[lane] = sm.fdes[lane]; }
-    if (variant == 0 && lane < 2) { Ap[(12 + lane) * LDZ + lane] = 1.0; qp.bp[12 + lane] = sm.base_acc[lane] + mdl->base_linear_kp * (sm.qd[lane] - sm.q[lane]) + mdl->base_linear_kd * (sm.vd[lane] - sm.v[lane]); }
+    if (variant == 0 && lane < 2) { Ap[(12 + lane) * LDZ + lane] = 1.0; qp.bp[12 + lane] = sm.base_acc[lane] + tn->base_linear_kp * (sm.qd[lane] - sm.q[lane]) + tn->base_linear_kd * (sm.vd[lane] - sm.v[lane]); }
   }
   __syncwarp();
   return rows;
@@ -304,13 +305,16 @@ __device__ int solve_level(WbcSmem& sm, const IneqCtx& ic, int rows, int off, in
   return status;
 }
 
+// TUNED: the batch has robot tuning rows.  Without them the kernel reads the gains at their fixed place in DevModel, as it did before rows existed.
+template <bool TUNED>
 __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevModel* __restrict__ mdl, int b0, int B, const double* __restrict__ x_des, const double* __restrict__ u_des,
                                                                    const double* __restrict__ rbd_meas, const int32_t* __restrict__ mode_in, const double* __restrict__ period_in,
                                                                    const double* __restrict__ time_in, double* __restrict__ input_last, int variant,
                                                                    double* __restrict__ cmd_out, int32_t* __restrict__ status_out, int32_t* __restrict__ diag_out,
-                                                                   const double* __restrict__ srbd, const double* __restrict__ payload) {
+                                                                   const double* __restrict__ srbd, const double* __restrict__ payload, const double* __restrict__ tuning) {
   // srbd [B][SRBD_DBL] / payload [B][8]: the robot's model payload (qmb200_set_model_payload) - its SRBD constants and the point masses the rigid-body passes add
-  // (payload.cuh); both NULL without one (the same for the whole grid)
+  // (payload.cuh); both NULL without one (the same for the whole grid).  tuning [B][TUNING_DBL]: the robot's gains and friction pyramid (qmb200_set_robot_tuning), NULL for the
+  // handle's (WbcBase::dynamicCallback, WbcBase.cpp:69-117; frictionConeTask.frictionCoefficient, task.info:346-348)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = b0 + blockIdx.x * (int)(blockDim.x >> 5) + warp;   // robots per CTA = warps per CTA, chosen at launch (the warps of a CTA never synchronise with each other)
@@ -400,7 +404,11 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   __syncwarp();
 
   // ---- hierarchy ----
-  QpWs& qp = sm.qp; IneqCtx ic{&sm, mode, nc, mdl->wbc_friction, lfp, ffp}; int status = 0;
+  // with rows, every level reads the robot's row staged in shared memory (visible after the __syncwarp below): a pointer to it held in registers across the
+  // hierarchy costs spills
+  if (TUNED) { const double* tr = tuning + (size_t)b * TUNING_DBL; for (int i = lane; i < TUNING_MODEL; i += 32) reinterpret_cast<double*>(&sm.tun)[i] = tr[i]; }
+  const Tuning* tn = TUNED ? &sm.tun : tuning_of(mdl, nullptr, 0);
+  QpWs& qp = sm.qp; IneqCtx ic{&sm, mode, nc, TUNED ? tuning[(size_t)b * TUNING_DBL + 1] : mdl->wbc_friction, lfp, ffp}; int status = 0;
   const bool init_phase = time < 10.0;   // HierarchicalWbc.cpp:32
   double* AR = qp.za.q.AR; double* Z = qp.za.q.Z;
   for (int i = lane; i < 36; i += 32) qp.xbar[i] = 0.0;
@@ -411,7 +419,7 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   unsigned vmask0 = 0, vmask1 = 0;   // violated set, bit per inequality (lane-uniform)
   int k0 = 0;
   for (int it = 0; it < cap0; ++it) {
-    int r = build_level(sm, mdl, 0, mode, variant, init_phase, ffp, lane); it0 = it + 1;
+    int r = build_level(sm, tn, 0, mode, variant, init_phase, ffp, lane); it0 = it + 1;
     // append violated rows
     for (int i = 0; i < nineq; ++i) { const bool in = (i < 32) ? ((vmask0 >> i) & 1u) : ((vmask1 >> (i - 32)) & 1u); if (in) { if (r >= MAXR) { status |= ST_TOO_MANY_ROWS; break; }
         for (int k = lane; k < 36; k += 32) AR[r * LDZ + k] = ineq_row_elem(ic, i, k); if (lane == 0) qp.bp[r] = ineq_rhs(ic, i); ++r; } }
@@ -433,7 +441,7 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   int off = 0, nzc = 0, nw = 0, it1 = 0, it2 = 0;
   {
     if (vmask0 | vmask1) {   // the last factorisation contains violated rows: factor A0 alone (otherwise the one in AR already is the QR of A0')
-      const int rows0 = build_level(sm, mdl, 0, mode, variant, init_phase, ffp, lane);
+      const int rows0 = build_level(sm, tn, 0, mode, variant, init_phase, ffp, lane);
       k0 = w_qrcp(AR, 36, rows0, LDZ, qp.tau, qp.perm, 1e-11, lane);
     }
     nzc = 36 - k0;
@@ -442,7 +450,7 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   }
   // levels 1 and 2
   for (int level = 1; level <= 2 && nzc > 0; ++level) {
-    const int rows = build_level(sm, mdl, level, mode, variant, init_phase, ffp, lane);
+    const int rows = build_level(sm, tn, level, mode, variant, init_phase, ffp, lane);
     const int nz = nzc - off;
     if (nz <= 0) break;                                   // trivial kernel (the reference keeps one zero column, HoQp.cpp:129)
     project_task(qp, rows, off, nz, lane);
@@ -468,17 +476,21 @@ static_assert(sizeof(WbcSmem) * WBC_WARPS <= 227 * 1024, "WBC shared-memory budg
 size_t wbc_smem_bytes() { return sizeof(WbcSmem) * WBC_WARPS; }
 
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
-                       double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0, int b1, int32_t* diag, const double* srbd, const double* payload) {
+                       double* input_last, int variant, double* cmd, int32_t* status, cudaStream_t stream, int b0, int b1, int32_t* diag, const double* srbd, const double* payload, const double* tuning) {
   if (b1 < 0) b1 = B; if (b1 <= b0) return;
   // Eight robots per CTA, one CTA per SM (8 x 28 KB of shared memory: the same 227 KB budget per block on H100).  Smaller CTAs would even out the per-CTA tail, but
   // the kernel is ~24 k SASS instructions (sm_90a build) and the warps of one CTA run in phase and share the instruction cache; a batch of one wave takes the time of its slowest
   // robot whatever the CTA shape.
   const int nb = b1 - b0; const int wpc = WBC_WARPS;
   const int grid = (nb + wpc - 1) / wpc;
-  wbc_update_kernel<<<grid, 32 * wpc, sizeof(WbcSmem) * wpc, stream>>>(mdl, b0, b1, x_des, u_des, rbd, mode, period, time, input_last, variant, cmd, status, diag, srbd, payload);
+  (tuning ? wbc_update_kernel<true> : wbc_update_kernel<false>)<<<grid, 32 * wpc, sizeof(WbcSmem) * wpc, stream>>>(mdl, b0, b1, x_des, u_des, rbd, mode, period, time, input_last, variant, cmd, status, diag, srbd, payload, tuning);
 }
 
 // cudaFuncSetAttribute is per device: called from qmb200_create after cudaSetDevice (one handle per GPU, several handles / devices per process allowed)
-int wbc_configure_device() { return (int)cudaFuncSetAttribute(wbc_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wbc_smem_bytes()); }
+int wbc_configure_device() {
+  cudaError_t e = cudaFuncSetAttribute(wbc_update_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wbc_smem_bytes());
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(wbc_update_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wbc_smem_bytes());
+  return (int)e;
+}
 
 }  // namespace qmb

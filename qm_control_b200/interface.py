@@ -378,6 +378,39 @@ class Solver:
         self._call("get_model_payload", _p(pl), C.byref(is_set))
         return pl if is_set.value else None
 
+    def set_robot_tuning(self, tuning=None):
+        """Per-robot controller parameters (_lib.TUNING_LAYOUT): the MPC friction cone, the WBC friction pyramid, the end-effector weights, the WBC gains and
+        the control law's arm gains.  tuning: dict field -> scalar or [B] ([k] or [B, k] for the vector gains); fields not named take the handle's current
+        values (get_handle_tuning).  While rows are set they replace the handle's values for every robot.  None clears them.  Synchronous."""
+        rows = None if tuning is None else self.robot_tuning_rows(tuning)   # held until the library has copied it
+        self._call("set_robot_tuning", _p(rows))
+
+    def robot_tuning_rows(self, tuning):
+        """The rows [B, TUNING] that set_robot_tuning(tuning) stores: the handle's current values with the named fields replaced.  Raises ValueError on an
+        unknown field or a value of the wrong shape; the values themselves are checked by the library."""
+        B = self.batch; rows = np.repeat(self.get_handle_tuning()[None, :], B, axis=0)
+        for k, v in tuning.items():
+            if k not in _lib.TUNING_LAYOUT:
+                raise ValueError("robot tuning: unknown field %r (one of %s)" % (k, ", ".join(_lib.TUNING_LAYOUT)))
+            off, w = _lib.TUNING_LAYOUT[k]; a = np.asarray(v, dtype=np.float64)
+            ok = a.shape in ((), (B, w)) or a.shape == ((B,) if w == 1 else (w,))
+            if not ok:
+                raise ValueError("robot tuning: %s must be a scalar, %s, got shape %s" % (k, "[%d]" % B if w == 1 else "[%d] or [%d, %d]" % (w, B, w), a.shape))
+            rows[:, off:off + w] = a.reshape(B, 1) if w == 1 and a.shape == (B,) else a   # a vector field's [k] is per axis, also when B == k
+        return rows
+
+    def get_handle_tuning(self):
+        """→ the handle's own values as one tuning row [TUNING]: what every robot uses while no rows are set."""
+        row = np.zeros(_lib.TUNING); self._call("get_handle_tuning", _p(row)); return row
+
+    def get_robot_tuning(self):
+        """→ dict field -> [B] ([B, k] for the vector gains) of the stored rows, or None when none are set."""
+        rows = np.zeros((self.batch, _lib.TUNING)); is_set = C.c_int32()
+        self._call("get_robot_tuning", _p(rows), C.byref(is_set))
+        if not is_set.value:
+            return None
+        return {k: rows[:, off] if w == 1 else rows[:, off:off + w] for k, (off, w) in _lib.TUNING_LAYOUT.items()}
+
     # ---------------- online payload estimate (include/qmb200.h: qmb200_payload_est_*; DESIGN.md §4.6) ----------------
     def payload_est_get_params(self):
         """→ dict of qmb200_payload_est_params."""

@@ -57,7 +57,12 @@ a reach sweep of 5 s in which every robot starts at yaw 0 on the grid, trots, is
 dz -0.1..0.1 m and a rotation of 0-20 deg about a fixed axis, every combination equally often) and is commanded to stance at 2.5 s, with per bin of each
 axis the end-effector position and orientation errors at the end (p50 / p95), the fallen robots and the OR of the status bits; the device time per call
 of the per-robot target call and of the scalar one on the same rows (CUDA events, alternated blocks); and the wall time per simulated second of a run
-of --duration with the goals, with a timeline that changes nothing, and without commands (the timed run above).
+of --duration with the goals, with a timeline that changes nothing, and without commands (the timed run above).  --ee-tuning adds "ee_tuning_sweep": the
+same reach sweep once more with per-robot tuning rows (closed_loop.run(tuning=...)) over the MPC's end-effector weights x 0.5 / 1 / 2 / 4, the WBC's
+end-effector gains x 0.5 / 1 / 2 and kd_arm_wbc 0.5 / 2, every goal bin in every tuning cell alike, with the errors per bin and per cell.
+
+--model-friction plant (with --vary) tells the MPC friction cone and the WBC friction pyramid each robot's floor friction (closed_loop.run(tuning=...)),
+and runs the same sweep untold as well; both arms start from a cold MPC and WBC state.
 """
 import argparse
 import json
@@ -69,6 +74,7 @@ import time
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from qm_control_b200 import _lib   # noqa: E402  (the tree's package, as above)
 
 
 def card():
@@ -342,8 +348,9 @@ def target_call_times(solver, reps=7, calls=50):
             **{"ms_per_call_" + k: float(np.median(v)) for k, v in times.items()}, "spread_per_robot": [float(min(times["per_robot"])), float(max(times["per_robot"]))]}
 
 
-def ee_goals(solver, closed_loop, B, sim_s, xy, upright):
-    """The reach sweep, the target call times, then the runs of sim_s with the goals and with a timeline that changes nothing (wall time)."""
+def ee_goals(solver, closed_loop, B, sim_s, xy, upright, tuning=False):
+    """The reach sweep, the target call times, then the runs of sim_s with the goals and with a timeline that changes nothing (wall time).  With tuning
+    also the reach sweep again under per-robot tuning rows (ee_tuning_sweep)."""
     import torch
     b = np.arange(B); bins = dict(dx_m=np.array([-0.1, 0.0, 0.1, 0.2, 0.3, 0.4]), dz_m=np.array([-0.1, 0.0, 0.1]), rot_deg=np.array([0.0, 10.0, 20.0]))
     idx = dict(dx_m=b % 6, dz_m=(b // 6) % 3, rot_deg=(b // 18) % 3)
@@ -373,8 +380,39 @@ def ee_goals(solver, closed_loop, B, sim_s, xy, upright):
     return {"reach_sweep": {"label": "5 s: trot from the start at yaw 0, one goal at 0.2 s (offset from the start pose), stance commanded at 2.5 s (in force from 3.5 s); "
                                      "errors of the end effector against the goal at the end; fallen = min base z <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite",
                             "bins": sweep_bins, "fallen": int(np.sum(~up)), "pos_err_m_p50_p95": pct(pe), "ori_err_deg_p50_p95": pct(oe)},
+            **({"ee_tuning_sweep": ee_tuning_sweep(solver, closed_loop, B, xy, upright, sweep, goal, idx["dz_m"], idx["rot_deg"])} if tuning else {}),
             "target_call": target_call_times(solver),
             "wall_s_per_sim_s": {"label": "stance runs of %.2f s from a cold MPC / WBC state" % sim_s, **walls}}
+
+
+def ee_tuning_sweep(solver, closed_loop, B, xy, upright, sweep, goal, dz_bin, rot_bin):
+    """The reach sweep of ee_goals again, each robot with its own tuning row: the MPC's end-effector weights (mu_ee_pos / ori and the final ones, scaled
+    together), the WBC's end-effector gains (kp / kd of ee_linear and ee_angular, scaled together) and the control law's kd_arm_wbc.  The tuning index is
+    b // 54, so every tuning bin holds every goal bin of ee_goals (period 54) alike.  Errors at the end per bin of each axis and per cell."""
+    b = np.arange(B); h = solver.get_handle_tuning(); L = _lib.TUNING_LAYOUT
+    bins = dict(mu_ee_scale=np.array([0.5, 1.0, 2.0, 4.0]), wbc_ee_gain_scale=np.array([0.5, 1.0, 2.0]), kd_arm_wbc=np.array([0.5, 2.0]))
+    cell = (b // 54) % 24; idx = dict(mu_ee_scale=cell % 4, wbc_ee_gain_scale=(cell // 4) % 3, kd_arm_wbc=cell // 12)
+    rows = np.repeat(h[None], B, axis=0)
+    for k in ("mu_ee_pos", "mu_ee_ori", "mu_final_ee_pos", "mu_final_ee_ori"):
+        rows[:, L[k][0]] *= bins["mu_ee_scale"][idx["mu_ee_scale"]]
+    for k in ("kp_ee_linear", "kd_ee_linear", "kp_ee_angular", "kd_ee_angular"):
+        off, w = L[k]; rows[:, off:off + w] *= bins["wbc_ee_gain_scale"][idx["wbc_ee_gain_scale"]][:, None]
+    rows[:, L["kd_arm_wbc"][0]] = bins["kd_arm_wbc"][idx["kd_arm_wbc"]]
+    solver.mpc_reset(); solver.wbc_set_input_last(None)
+    r = closed_loop.run(solver, duration=5.0, gait="trot", xy_yaw=xy, commands=sweep,
+                        tuning={k: rows[:, off] if w == 1 else rows[:, off:off + w] for k, (off, w) in L.items()})
+    pe = np.linalg.norm(r["ee"][-1, :, :3] - goal[:, :3], axis=1)
+    oe = np.degrees(2.0 * np.arccos(np.clip(np.abs(np.sum(r["ee"][-1, :, 3:] * goal[:, 3:], axis=1)), 0.0, 1.0)))
+    up = upright(r); pct = lambda a: [float(np.percentile(a, 50)), float(np.percentile(a, 95))]
+    def stats(m):
+        return {"robots": int(np.sum(m)), "fallen": int(np.sum(~up[m])), "pos_err_m_p50_p95": pct(pe[m]), "ori_err_deg_p50_p95": pct(oe[m])}
+    hard = (dz_bin == 2) | (rot_bin == 2)   # the goals the untuned sweep misses most: 10 cm up or turned 20 degrees
+    return {"label": "the reach sweep of ee_goals with per-robot tuning rows; scales multiply the handle's values (scale 1 and kd_arm_wbc 0.5 = the handle's own); "
+                     "hard_goals = dz +0.1 m or 20 degrees",
+            "bins": {axis: [{"value": float(v), **stats(idx[axis] == i), "hard_goals": stats((idx[axis] == i) & hard)} for i, v in enumerate(bins[axis])] for axis in bins},
+            "cells": [{"mu_ee_scale": float(bins["mu_ee_scale"][c % 4]), "wbc_ee_gain_scale": float(bins["wbc_ee_gain_scale"][(c // 4) % 3]),
+                       "kd_arm_wbc": float(bins["kd_arm_wbc"][c // 12]), **stats(cell == c), "hard_goals": stats((cell == c) & hard)} for c in range(24)],
+            "fallen": int(np.sum(~up))}
 
 
 def watch_state_est(solver):
@@ -406,6 +444,7 @@ def main():
     ap.add_argument("--vary", action="store_true", help="per-robot sweep of EE payload, floor friction and a lateral base push")
     ap.add_argument("--model-payload", choices=["plant", "estimate"],
                     help="plant: tell the controller the plant's payload (its model payload, Solver.set_model_payload); estimate: run the online payload estimator")
+    ap.add_argument("--model-friction", choices=["plant"], help="with --vary: tell the MPC friction cone and the WBC friction pyramid each robot's floor friction (robot tuning rows)")
     ap.add_argument("--terrain", action="store_true", help="per-robot sweep of ramp angle and step rise under the feet")
     ap.add_argument("--state-estimator", action="store_true", help="the controller reads the base state estimate from the IMU, encoders and contact flags")
     ap.add_argument("--sensor-noise", choices=["reference"], help="with --state-estimator: the IMU noise of qm_gazebo/config/default.yaml")
@@ -413,7 +452,12 @@ def main():
     ap.add_argument("--slip-detector", action="store_true", help="with --state-estimator: keep slipping stance feet out of the estimate")
     ap.add_argument("--gait-commands", action="store_true", help="time the device gait schedule in the loop and run a gait switch sweep")
     ap.add_argument("--ee-goals", action="store_true", help="end-effector goals on the device command timeline: a reach sweep and the target call's time")
+    ap.add_argument("--ee-tuning", action="store_true", help="with --ee-goals: the reach sweep again with per-robot end-effector weights, WBC end-effector gains and kd_arm_wbc")
     args = ap.parse_args()
+    if args.ee_tuning and not args.ee_goals:
+        ap.error("--ee-tuning needs --ee-goals")
+    if args.model_friction and not args.vary:
+        ap.error("--model-friction needs --vary")
     if args.vary and args.terrain:
         ap.error("--vary and --terrain are separate sweeps")
     if args.sensor_noise and not args.state_estimator:
@@ -445,11 +489,14 @@ def main():
         ter = dict(tiles=tiles, cell=T.CELL, tile=idx["ramp_deg"] * 4 + idx["step_rise_m"], origin=T.centred_origin(xy[:, :2]))
         kw = dict(terrain=ter)
     told = {"plant": dict(model_payload="plant"), "estimate": dict(payload_estimator=True), None: {}}[args.model_payload]
+    if args.model_friction:
+        told = dict(told, tuning=dict(friction_mu="plant", wbc_friction="plant"))
     se = dict(state_estimator=True, sensor_noise=args.sensor_noise, **({"attitude_filter": True} if args.attitude_filter else {}),
               **({"slip_detector": True} if args.slip_detector else {}), **({"ground_map": True} if args.terrain else {})) if args.state_estimator else {}
     def fresh():
-        """with --state-estimator every run starts from a cold MPC and WBC state: a run whose robots fell leaves warm starts the next run must not inherit"""
-        if args.state_estimator:
+        """with --state-estimator or --model-friction every run starts from a cold MPC and WBC state: a run whose robots fell leaves warm starts the next run
+        must not inherit"""
+        if args.state_estimator or args.model_friction:
             solver.mpc_reset(); solver.wbc_set_input_last(None)
     if args.state_estimator:
         box, unwrap = watch_state_est(solver)
@@ -505,6 +552,9 @@ def main():
             extra["vary"]["model_payload"] = {"plant": "the controller is told the plant's payload (bins)", "estimate": "the controller runs the online payload estimate (bins)"}[
                 args.model_payload] + "; payload_kg_not_told: the same sweep, controller not told"
             extra["vary"]["payload_kg_not_told"] = vary_bins(closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw), "payload_kg")
+        if args.model_friction:
+            extra["vary"]["model_friction"] = "the MPC cone and the WBC pyramid are told the plant's floor friction (bins); mu_not_told: the same sweep, controller not told; both arms from a cold MPC and WBC state"
+            fresh(); extra["vary"]["mu_not_told"] = vary_bins(closed_loop.run(solver, duration=sim_s, gait=args.gait, cmd_vel=cmd, xy_yaw=xy, **kw), "mu")
     if args.terrain:
         extra["terrain"] = {"label": "per-robot sweep, controller blind to the terrain; fallen = height above the ground under the base <= 0.3 m or |roll|, |pitch| >= 0.3 rad "
                                      "or non-finite", "tiles": "ground z = 0 up to 0.35 m ahead of the start, then a ramp (deg) with steps (rise m, run 0.3 m) on it",
@@ -567,7 +617,7 @@ def main():
         extra["gait_commands"] = {**gait_commands(solver, closed_loop, B, sim_s, cmd, xy, kw, upright), "gpu": name, "power_limit": limit,
                                   "wall_s_per_sim_s_without_commands": wall / sim_s}
     if args.ee_goals:
-        extra["ee_goals"] = {**ee_goals(solver, closed_loop, B, sim_s, xy, upright), "gpu": name, "power_limit": limit, "wall_s_per_sim_s_without_commands": wall / sim_s}
+        extra["ee_goals"] = {**ee_goals(solver, closed_loop, B, sim_s, xy, upright, tuning=args.ee_tuning), "gpu": name, "power_limit": limit, "wall_s_per_sim_s_without_commands": wall / sim_s}
     print(json.dumps({"metric": "robot_sim_seconds_per_s", "value": B * sim_s / wall, "unit": "robot-simulated-seconds per wall-clock second", "n_gpus": 1,
                       "wall_s_per_sim_s": wall / sim_s, "gpu": name, "power_limit": limit, "dtype": "f64", "data": "synthetic",
                       "plant": {"ms_per_call": per_call, "calls": len(pairs), "share_of_loop": sim_ms * 1e-3 / wall},
