@@ -555,6 +555,29 @@ int qmb200_slip_get(qmb200_handle* h, int32_t* mask /*[B]*/, int32_t* hold /*[B]
 /* Releases the detector state.  Step and get fail until the next reset.  Stopping a detector that is not running does nothing and returns 0. */
 int qmb200_slip_stop(qmb200_handle* h);
 
+/* ---- per-robot restart: QMController::starting (QMController.cpp:98-126) for single robots of a batch, inside a stream-ordered loop (DESIGN.md §4.10).
+ *      The start image holds, per robot, the rows of every component running when it is saved: the state estimator, attitude filter, slip detector and
+ *      payload estimator states, the model payload rows (qmb200_set_model_payload, as a commit may have left them) and the device gait schedule with
+ *      its timeline cursor.  Handle settings (parameters, tuning rows, plant robot params, terrain, ground map, gait templates, command timeline) are not
+ *      state and are never written.  Each reset, stop or re-allocation of an imaged component (and qmb200_gait_dev_set_commands, which resets the
+ *      cursors) makes the image stale for it. */
+/* Saves the image of the components running now, replacing any previous one.  Synchronous. */
+int qmb200_robot_image_save(qmb200_handle* h);
+/* Frees the image (qmb200_destroy does too).  Clearing when none is saved does nothing and returns 0. */
+int qmb200_robot_image_clear(qmb200_handle* h);
+/* One launch, no host work: for every robot with mask[b] != 0 the imaged rows return to the image, both MPC warm-start sides forget the robot's
+ * solution (n_nodes = 0, what qmb200_mpc_reset does for all), its WBC last input is zeroed and its hw_write FIFO emptied.  Robots with mask[b] == 0
+ * are not written.  Fails, naming the component and writing nothing, when no image is saved, an imaged component was stopped, reset or re-allocated
+ * since, or a component runs that was not imaged. */
+int qmb200_robot_image_restore(qmb200_handle* h, const int32_t* mask /*[B]*/);
+int qmb200_robot_image_restore_dev(qmb200_handle* h, const int32_t* mask /*[B] device*/, void* cuda_stream);
+/* The fall rule of the closed-loop sweeps, one thread per robot on the plant's rbd [B][55]: robot b is fallen when its base rows (zyx, p) hold a
+ * non-finite value, p_z - H(p_x, p_y) <= z_min with H the plant's ground under the base (its terrain tile, the plane ground_height otherwise), or
+ * |pitch| or |roll| >= tilt_max.  fallen [B] = 1 / 0; count [B] (in-out) grows by one on a fallen call and drops to 0 otherwise.  Rejects a non-finite
+ * z_min and tilt_max that is non-finite or <= 0. */
+int qmb200_fall_detect(qmb200_handle* h, const double* rbd /*[B][55]*/, double z_min, double tilt_max, int32_t* count /*[B] in-out*/, int32_t* fallen /*[B]*/);
+int qmb200_fall_detect_dev(qmb200_handle* h, const double* rbd, double z_min, double tilt_max, int32_t* count, int32_t* fallen, void* cuda_stream);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

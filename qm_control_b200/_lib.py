@@ -201,6 +201,12 @@ PROTOTYPES = {
     "qmb200_slip_step_dev": (I32, [P, D] + [P] * 6),
     "qmb200_slip_get": (I32, [P] * 4),
     "qmb200_slip_stop": (I32, [P]),
+    "qmb200_robot_image_save": (I32, [P]),
+    "qmb200_robot_image_clear": (I32, [P]),
+    "qmb200_robot_image_restore": (I32, [P] * 2),
+    "qmb200_robot_image_restore_dev": (I32, [P] * 3),
+    "qmb200_fall_detect": (I32, [P, P, D, D, P, P]),
+    "qmb200_fall_detect_dev": (I32, [P, P, D, D, P, P, P]),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

@@ -55,7 +55,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None):
+        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -106,6 +106,15 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     tuning: the controller's per-robot tuning rows for this run (Solver.set_robot_tuning): dict field of _lib.TUNING_LAYOUT -> scalar or [B] ([k] or [B, k]
     for the vector gains), fields not named at the handle's own values; friction_mu="plant" / wbc_friction="plant" take this run's plant friction
     (friction_mu's value, or the handle's robot params or plant params).  The previous rows are restored when run returns.
+    respawn: True or dict(on_fall=True, hold=0.1, z_min=0.3, tilt_max=0.3, every=None) restarts single robots inside the loop (DESIGN.md §4.10).
+    Right before the first solve the run saves its start image (Solver.robot_image_save and a device copy of the loop's own per-robot rows) and
+    restores it for every robot, so the first episode starts through the same cold path as every later one.  At the end of every 10 ms window the
+    fall detector (Solver.fall_detect_dev, z_min / tilt_max) runs on the plant's rbd; a robot respawns at the next window boundary, before the MPC
+    tick, when on_fall and it has been fallen at the last hold / 10 ms window ends, or when every is set and its episode has lasted every seconds
+    (hold and every: positive multiples of 10 ms).  A respawned robot returns to its start pose, its estimators' and gait schedule's start
+    rows and a cold MPC, WBC and command FIFO, and lives on its own episode clock: its hw_write time, pushes (t_on counts from the episode's start),
+    gait commands and mode schedule replay; only the sensor noise keeps the global sample index, so each episode draws new noise.  The image is freed
+    when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
@@ -114,7 +123,9 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     gait[ticks, B], the active template id after each record's gait step (an index of gait_templates), mode[ticks, B], the window's mode at that
     step's t_obs, gait_templates, the table's names, target_kind[ticks, B], the kind each robot's target call took at that record's MPC tick (0
     cmd_vel, 1 ee_cmd_vel, 2 goal published, -1 goal held), and ee_target[ticks, B, 7], the final-knot end-effector pose of the target in force after
-    that call)."""
+    that call); with respawn also episode[ticks, B], each robot's episode index in that record's window (0 for the first), and fallen[ticks, B], the
+    detector's flag at that window's end."""
+    rs = None if respawn is None else _respawn_spec(respawn)
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
     if state_estimator is not None and state_estimator is not True and not isinstance(state_estimator, dict):
@@ -161,9 +172,41 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_robot_params(solver, friction_mu, payload))
         if gd is not None:
             scope.enter_context(_gait_dev(solver, gd))
+        if rs is not None:
+            scope.callback(solver.robot_image_clear)
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd)
+                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs)
+
+
+def _respawn_spec(respawn):
+    """closed_loop.run's respawn → dict(on_fall, hold_windows, z_min, tilt_max, every_ms or None); ValueError when malformed"""
+    spec = dict(on_fall=True, hold=0.1, z_min=0.3, tilt_max=0.3, every=None)
+    if respawn is not True:
+        if not isinstance(respawn, dict) or not set(respawn) <= set(spec):
+            raise ValueError("closed_loop.run: respawn must be None, True or dict(on_fall, hold, z_min, tilt_max, every), got %r" % (respawn,))
+        spec.update(respawn)
+    if not isinstance(spec["on_fall"], (bool, np.bool_)):
+        raise ValueError("closed_loop.run: respawn on_fall must be True or False, got %r" % (spec["on_fall"],))
+
+    def ms(name, v):
+        try:
+            x = np.nan if isinstance(v, (str, bool)) else float(v) * 1e3
+        except (TypeError, ValueError):
+            x = np.nan
+        n = int(round(x)) if np.isfinite(x) else 0
+        if not (n > 0 and n % MPC_PERIOD_MS == 0 and abs(x - n) < 1e-6):
+            raise ValueError("closed_loop.run: respawn %s must be a positive multiple of %d ms, got %r" % (name, MPC_PERIOD_MS, v))
+        return n
+    hold = ms("hold", spec["hold"]); every = None if spec["every"] is None else ms("every", spec["every"])
+    for name in ("z_min", "tilt_max"):
+        if isinstance(spec[name], (bool, str)) or not np.isfinite(np.asarray(spec[name], dtype=np.float64)) or np.ndim(spec[name]) != 0:
+            raise ValueError("closed_loop.run: respawn %s must be a finite number, got %r" % (name, spec[name]))
+    if not float(spec["tilt_max"]) > 0.0:
+        raise ValueError("closed_loop.run: respawn tilt_max must be > 0, got %r" % (spec["tilt_max"],))
+    if not spec["on_fall"] and every is None:
+        raise ValueError("closed_loop.run: respawn needs on_fall or every (it would never restart a robot)")
+    return dict(on_fall=bool(spec["on_fall"]), hold_windows=hold // MPC_PERIOD_MS, z_min=float(spec["z_min"]), tilt_max=float(spec["tilt_max"]), every_ms=every)
 
 
 def _gait_commands(B, gait, commands):
@@ -369,7 +412,8 @@ def _robot_params(solver, friction_mu, payload):
         solver.sim_set_robot_params(**prev)
 
 
-def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None):
+def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
+         rs=None):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -471,22 +515,47 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             rec_ee_target[i] = prob["target_states"][:, 1, 30:37]
         solver.mpc_solve_dev(prob, s)
 
+    if rs is not None:   # the start image: the library's rows and the loop's own, then one restore of every robot through the cold path of every later one
+        own = [q, v, rbd, contact, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, cmd7, last_ee, prob["n_events"], prob["event_times"], prob["modes"],
+               prob["n_target"], prob["target_times"], prob["target_states"]] + ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
+        solver.robot_image_save()
+        with torch.cuda.stream(stream):
+            start = [a.clone() for a in own]
+            k0 = torch.zeros(B, dtype=torch.int64, device=dev); dk = torch.zeros_like(k0)   # each robot's episode start (plant step), and k - k0
+            episode = torch.zeros(B, dtype=torch.int32, device=dev); fall_count = torch.zeros_like(episode); fallen = torch.zeros_like(episode)
+            due = torch.ones_like(episode); rec_episode = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_fallen = torch.zeros_like(rec_episode)
+        solver.robot_image_restore_dev(due, s)
+
+    def respawn(k):   # the robots due restart at window boundary k: the library's rows, then the loop's
+        solver.robot_image_restore_dev(due, s)
+        m = due.bool()
+        for a, a0 in zip(own, start):
+            a.copy_(torch.where(m.view((B,) + (1,) * (a.dim() - 1)), a0, a))
+        k0.copy_(torch.where(m, k, k0)); episode.add_(due); fall_count.masked_fill_(m, 0)
+
     with torch.cuda.stream(stream):
         mpc_tick(0); stream.synchronize()          # QMController::starting: one blocking solve before the loop
         for k in range(n_ms):
             if k % MPC_PERIOD_MS == 0 and k > 0:
+                if rs is not None:
+                    respawn(k)
                 mpc_tick(k // MPC_PERIOD_MS)
             if k % wbc_period_ms == 0:
                 solver.update_dev(meas, period, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, ctl_st, s)
                 acc_st.bitwise_or_(ctl_st)
-            hw_time.fill_(t_start + k * 1e-3); jpos.copy_(q[:, 6:]); jvel.copy_(v[:, 6:])
+            if rs is None:
+                hw_time.fill_(t_start + k * 1e-3)
+            else:   # the robot's episode clock
+                torch.sub(k0, k, out=dk).neg_(); hw_time.copy_(dk).mul_(1e-3).add_(t_start)
+            jpos.copy_(q[:, 6:]); jvel.copy_(v[:, 6:])
             solver.hw_write_dev(hw_time, hw_period, joint_cmd, jpos, jvel, effort, hw_st, s)
             if se:
                 v_prev.copy_(v)
             if sim_timer:
                 sim_timer(True)
             if push is not None:
-                torch.where(((push["on"] <= k) & (push["off"] > k))[:, None], push["wrench"], push["zero"], out=push["now"])
+                kk = k if rs is None else dk   # plant steps since the episode's start
+                torch.where(((push["on"] <= kk) & (push["off"] > kk))[:, None], push["wrench"], push["zero"], out=push["now"])
             solver.sim_step_dev(1e-3, effort, q, v, rbd, contact, sim_st, s, wrench=None if push is None else push["now"])
             if sim_timer:
                 sim_timer(False)
@@ -511,6 +580,13 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                     rec_base_est[i, :, 0:3] = rbd_est[:, 3:6]; rec_base_est[i, :, 3:6] = rbd_est[:, 0:3]
                 if sl:
                     rec_slip[i] = slip_acc; slip_acc.zero_()
+                if rs is not None:
+                    solver.fall_detect_dev(rbd, fall_count, fallen, rs["z_min"], rs["tilt_max"], s)
+                    rec_episode[i] = episode; rec_fallen[i] = fallen
+                    d = fall_count >= rs["hold_windows"] if rs["on_fall"] else torch.zeros_like(fallen, dtype=torch.bool)
+                    if rs["every_ms"] is not None:
+                        d |= (k + 1 - k0) >= rs["every_ms"]
+                    due.copy_(d)
     stream.synchronize()
     t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
     out = dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
@@ -524,4 +600,6 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     if gd is not None:
         out.update(gait=rec_gait.cpu().numpy(), mode=rec_mode.cpu().numpy(), gait_templates=list(gd["names"]), target_kind=rec_kind.cpu().numpy(),
                    ee_target=rec_ee_target.cpu().numpy())
+    if rs is not None:
+        out.update(episode=rec_episode.cpu().numpy(), fallen=rec_fallen.cpu().numpy())
     return out

@@ -19,6 +19,7 @@
 #include "kernels/attitude_api.cuh"
 #include "kernels/slip_api.cuh"
 #include "kernels/gait_api.cuh"
+#include "kernels/respawn_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -38,6 +39,10 @@ struct RobotArray {
   int width; std::vector<double> host; double* d = nullptr;
   const double* dev() const { return host.empty() ? nullptr : d; }
 };
+
+// The components a start image covers (capi_respawn.inc).  Each has a generation that its reset, stop and re-allocation bump, so a restore can tell
+// that the rows it would write no longer belong to the state it imaged.
+enum ImageComponent { IMG_STATE_EST, IMG_ATTITUDE, IMG_SLIP, IMG_PAYLOAD_EST, IMG_MODEL_PAYLOAD, IMG_GAIT, IMG_N };
 
 struct qmb200_handle {
   HostModel hm;
@@ -78,6 +83,10 @@ struct qmb200_handle {
     int32_t* d_ee_kind = nullptr; double* d_ee = nullptr;   // the timeline's end-effector commands [B][n_cmd] and [B][n_cmd][7], NULL when it has none
   } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
+  uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
+  struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
+    bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
+  } image;
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
 
@@ -222,6 +231,7 @@ void qmb200_destroy(qmb200_handle* h) {
   if (h->d_sl) cudaFree(h->d_sl);
   cudaFree(h->gs.d_table); cudaFree(h->gs.d_robots); cudaFree(h->gs.d_cursor); cudaFree(h->gs.d_t); cudaFree(h->gs.d_tmpl); cudaFree(h->gs.d_vel);
   cudaFree(h->gs.d_ee_kind); cudaFree(h->gs.d_ee);
+  cudaFree(h->image.d);
   delete h;
 }
 
@@ -273,6 +283,7 @@ int qmb200_set_model_payload(qmb200_handle* h, const double* payload) {
   std::vector<double> srbd; if (payload) { srbd.resize(B * SRBD_DBL); srbd_rows(h->hm, payload, B, srbd.data()); }
   const int rc = set_robot_arrays(h, {{&h->mpayload, payload}, {&h->srbd, payload ? srbd.data() : nullptr}});
   if (!rc) h->model_on_device = false;   // set_robot_arrays waited for the device: the rows just written replace any committed ones
+  h->gen[IMG_MODEL_PAYLOAD] += 1;
   return rc;
 }
 int qmb200_get_model_payload(const qmb200_handle* h, double* payload, int32_t* is_set) {
@@ -422,3 +433,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_attitude.inc"
 #include "capi_slip.inc"
 #include "capi_gait.inc"
+#include "capi_respawn.inc"

@@ -674,6 +674,37 @@ class Solver:
         """Release the detector state."""
         self._call("slip_stop")
 
+    # ---------------- per-robot restart (include/qmb200.h: qmb200_robot_image_*, qmb200_fall_detect; DESIGN.md §4.10) ----------------
+    def robot_image_save(self):
+        """Save the start image: the per-robot rows of every component running now (state estimator, attitude filter, slip detector, payload
+        estimator, model payload rows, device gait schedule and its cursors).  Replaces any previous image.  Synchronous."""
+        self._call("robot_image_save")
+
+    def robot_image_restore(self, mask):
+        """Host variant of robot_image_restore_dev: mask [B] (nonzero: restart the robot)."""
+        mask = _i32(np.broadcast_to(np.asarray(mask), (self.batch,)), (self.batch,))
+        self._call("robot_image_restore", _p(mask))
+
+    def robot_image_restore_dev(self, mask, stream=None):
+        """For every robot with mask[b] != 0 (int32 [B] device tensor): its imaged rows return to the image, its MPC warm starts, WBC last input and
+        hw_write FIFO go back to the cold start; one launch, no synchronisation.  Fails when the image no longer matches the running components."""
+        self._call("robot_image_restore_dev", _p(mask), stream)
+
+    def robot_image_clear(self):
+        """Free the start image."""
+        self._call("robot_image_clear")
+
+    def fall_detect(self, rbd, count, z_min=0.3, tilt_max=0.3):
+        """Host variant of fall_detect_dev: rbd [B, 55], count [B] → (count [B] updated, fallen [B])."""
+        B = self.batch; rbd = _f64(rbd, (B, RBD)); count = _i32(count, (B,)).copy(); fallen = np.zeros(B, dtype=np.int32)
+        self._call("fall_detect", _p(rbd), float(z_min), float(tilt_max), _p(count), _p(fallen))
+        return count, fallen
+
+    def fall_detect_dev(self, rbd, count, fallen, z_min=0.3, tilt_max=0.3, stream=None):
+        """The sweeps' fall rule on the plant's rbd [B, 55]: fallen [B] int32 = non-finite base rows, height above the plant's ground under the base
+        <= z_min, or |pitch|, |roll| >= tilt_max; count [B] int32 grows by one per fallen call and drops to 0 otherwise.  No synchronisation."""
+        self._call("fall_detect_dev", _p(rbd), float(z_min), float(tilt_max), _p(count), _p(fallen), stream)
+
     # ---------------- device gait schedule (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7) ----------------
     def gait_dev_set_templates(self, names=None, gait_file=None):
         """Load the template table: names (default: every template of the gait file, in the order of its list) → the names, a template's id being its

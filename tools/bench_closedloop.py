@@ -6,6 +6,7 @@ deviation from the initial pose, as percentiles over the robots) of this project
 
     python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter] [--slip-detector]]
                                      [--gait-commands] [--ee-goals]
+    python tools/bench_closedloop.py --respawn [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -63,6 +64,13 @@ end-effector gains x 0.5 / 1 / 2 and kd_arm_wbc 0.5 / 2, every goal bin in every
 
 --model-friction plant (with --vary) tells the MPC friction cone and the WBC friction pyramid each robot's floor friction (closed_loop.run(tuning=...)),
 and runs the same sweep untold as well; both arms start from a cold MPC and WBC state.
+
+--respawn measures episode rates instead (closed_loop.run(respawn=...)): trot at --vx on the state estimate with the reference IMU noise and no attitude
+filter, robots restarted after 0.1 s fallen.  It prints one JSON line "respawn" with, from one 5 s run, the episodes per robot, the falls per
+robot-second and the fraction of episodes that fall within their first second, for first and later episodes apart, over the episodes that start at
+least 1 s before the run's end (with binomial standard deviations);
+the wall time per simulated second of --duration runs with and without respawn, alternated in one process; and the device time per call of the fall
+detector and the image restore against the plant step (CUDA events, alternated blocks).
 """
 import argparse
 import json
@@ -415,6 +423,93 @@ def ee_tuning_sweep(solver, closed_loop, B, xy, upright, sweep, goal, dz_bin, ro
             "fallen": int(np.sum(~up))}
 
 
+def respawn_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per fall detector call, per image restore (every robot masked, and none) and per 1 ms plant step of the whole batch, alternated
+    `reps` times in blocks of `calls` from one standing state, with the state estimator running and imaged (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact); count = torch.zeros_like(contact); fallen = torch.zeros_like(contact)
+    every, none = torch.ones_like(contact), torch.zeros_like(contact)
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream); torch.cuda.synchronize(dev)
+    solver.hw_set_delay(0.009); solver.state_est_reset(q0[:, 0:3]); solver.robot_image_save()
+    calls_of = {"fall_detect": lambda: solver.fall_detect_dev(rbd, count, fallen, 0.3, 0.3, s.cuda_stream),
+                "restore_all": lambda: solver.robot_image_restore_dev(every, s.cuda_stream), "restore_none": lambda: solver.robot_image_restore_dev(none, s.cuda_stream),
+                "plant": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    call()
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.robot_image_clear(); solver.state_est_stop()
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls; the image holds the state estimator's rows" % (B, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}, "spread_restore_all": [float(min(times["restore_all"])), float(max(times["restore_all"]))]}
+
+
+def respawn_rates(r, ep_s=1.0):
+    """Episode statistics of a closed_loop.run(respawn=...) result: episodes per robot, falls per robot-second and, for first and later episodes apart,
+    the fraction of episodes that fall within their first ep_s seconds.  Only episodes that start at least ep_s before the run's end count, fallen or
+    not: an episode that starts later is cut off by the run whatever its outcome, and counting it only when it falls would bias the later episodes'
+    fraction upwards (first episodes all start at 0)."""
+    ep, fl = r["episode"], r["fallen"].astype(bool); ticks, B = ep.shape; w = int(round(ep_s * 100))
+    falls = 0; first = [0, 0]; later = [0, 0]
+    for b in range(B):
+        for e in range(int(ep[-1, b]) + 1):
+            rows = np.flatnonzero(ep[:, b] == e); f = fl[rows, b]
+            falls += int(f.any())
+            if rows[0] + w <= ticks:   # its first ep_s seconds lie inside the run
+                box = first if e == 0 else later; box[0] += int(f[:w].any()); box[1] += 1
+    frac = lambda a: {"fell": a[0], "episodes": a[1], "fraction": a[0] / a[1] if a[1] else None,
+                      "binomial_sd": float(np.sqrt(a[0] / a[1] * (1 - a[0] / a[1]) / a[1])) if a[1] else None}
+    return {"episodes_per_robot": float(np.mean(ep[-1] + 1)), "falls_per_robot_s": falls / (B * ticks * 0.01), "falls": falls,
+            "fell_within_%gs_first_episodes" % ep_s: frac(first), "fell_within_%gs_later_episodes" % ep_s: frac(later)}
+
+
+def respawn_main(args, episode_run_s=5.0):
+    """--respawn: trot at --vx on the estimate from the reference IMU noise without the attitude filter, robots restarted after 0.1 s fallen.  One
+    run of episode_run_s for the rates; the wall time per simulated second of --duration runs with and without respawn, alternated twice after one
+    warm-up run of each; the per-call device times."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch; cmd = (args.vx, 0.0, 0.0, 0.0)
+    solver = q.Solver(batch=B, device=0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    kw = dict(gait=args.gait, cmd_vel=cmd, xy_yaw=xy, state_estimator=True, sensor_noise="reference")
+
+    def timed(respawn, duration):
+        solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+        r = closed_loop.run(solver, duration=duration, **kw, **({"respawn": dict(hold=0.1)} if respawn else {}))
+        torch.cuda.synchronize(dev)
+        return r, (time.perf_counter() - t0) / duration
+    wall = {False: [], True: []}
+    for rep in range(3):   # the first round warms up
+        for respawn in (False, True):
+            _, w = timed(respawn, args.duration)
+            if rep:
+                wall[respawn].append(w)
+    r, _ = timed(True, episode_run_s)
+    name, limit = card()
+    print(json.dumps({"metric": "respawn", "gpu": name, "power_limit": limit, "batch": B,
+                      "config": "%s at %.2f m/s on the state estimate, reference IMU noise, no attitude filter; respawn after 0.1 s fallen (min base height above "
+                                "the ground <= 0.3 m or |roll|, |pitch| >= 0.3 rad or non-finite)" % (args.gait, args.vx),
+                      "rates": {"simulated_s": episode_run_s, **respawn_rates(r)},
+                      "wall_s_per_sim_s": {"label": "runs of %.1f s, two alternated pairs after a warm-up pair" % args.duration,
+                                           "without_respawn": wall[False], "with_respawn": wall[True]},
+                      "per_call": respawn_times(solver, xy)}))
+
+
 def watch_state_est(solver):
     """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
     error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
@@ -453,7 +548,10 @@ def main():
     ap.add_argument("--gait-commands", action="store_true", help="time the device gait schedule in the loop and run a gait switch sweep")
     ap.add_argument("--ee-goals", action="store_true", help="end-effector goals on the device command timeline: a reach sweep and the target call's time")
     ap.add_argument("--ee-tuning", action="store_true", help="with --ee-goals: the reach sweep again with per-robot end-effector weights, WBC end-effector gains and kd_arm_wbc")
+    ap.add_argument("--respawn", action="store_true", help="restart robots that fell (hold 0.1 s) on the reference IMU noise without the attitude filter: episode rates")
     args = ap.parse_args()
+    if args.respawn:
+        return respawn_main(args)
     if args.ee_tuning and not args.ee_goals:
         ap.error("--ee-tuning needs --ee-goals")
     if args.model_friction and not args.vary:
