@@ -578,6 +578,37 @@ int qmb200_robot_image_restore_dev(qmb200_handle* h, const int32_t* mask /*[B] d
 int qmb200_fall_detect(qmb200_handle* h, const double* rbd /*[B][55]*/, double z_min, double tilt_max, int32_t* count /*[B] in-out*/, int32_t* fallen /*[B]*/);
 int qmb200_fall_detect_dev(qmb200_handle* h, const double* rbd, double z_min, double tilt_max, int32_t* count, int32_t* fallen, void* cuda_stream);
 
+/* ---- per-episode plant draws (DESIGN.md §4.11): each episode of each robot gets a new plant, drawn on the device right after its restart.
+ *   row[QMB200_EPISODE]  offset  0       friction_mu      the plant's Coulomb coefficient (qmb200_sim_set_robot_params)
+ *                                1-8     payload          the plant's payload row, qmb200_sim_set_robot_params' layout
+ *                                9-10    push_t_on, push_duration   s from the episode's start
+ *                                11-22   wrench           the push, qmb200_sim_step_ext's layout
+ *                                23-26   cmd_vel_x, cmd_vel_y, cmd_vel_z, cmd_yaw_rate   the base-frame velocity command
+ * Column c of robot b in episode e is fma(u, hi[b][c] - lo[b][c], lo[b][c]) with u = ((mix64(h) >> 11) + 0.5) 2^-53 in (0, 1), h the splitmix64 finaliser
+ * over (seed ^ a domain constant, global robot rank * B + b, e, c) in turn, as the sensor noise hashes its words: a pure function of those words and the
+ * ranges, identical on host and device; a column with lo == hi is lo itself, byte for byte. */
+#define QMB200_EPISODE 27
+#define QMB200_EPISODE_MODEL_PAYLOAD 1   /* link: the payload also goes to the controller's model payload and its SRBD rows (qmb200_set_model_payload) */
+#define QMB200_EPISODE_MPC_FRICTION 2    /* link: friction_mu also goes to the tuning rows' MPC friction coefficient (qmb200_set_robot_tuning) */
+#define QMB200_EPISODE_WBC_FRICTION 4    /* link: friction_mu also goes to the tuning rows' WBC friction coefficient */
+/* Per-robot ranges lo, hi [B][QMB200_EPISODE] and the seed (its 64 bits; the draw reads it as unsigned).  NULL lo and hi clear them.  Rejects a non-finite
+ * bound, lo > hi, a non-finite hi - lo, friction_mu lo <= 0 and a negative lo of a payload mass, push_t_on or push_duration, naming the field and the
+ * robot; on rejection the stored ranges stay unchanged.  Setting ranges makes sure the plant's robot params (qmb200_sim_set_robot_params) are set, at
+ * the values in force where they were not, so the sampler has rows to write.  Host arrays; synchronous. */
+int qmb200_episode_set_ranges(qmb200_handle* h, const double* lo /*[B][QMB200_EPISODE] or NULL*/, const double* hi /*[B][QMB200_EPISODE] or NULL*/, int64_t seed);
+/* The stored ranges and seed (zeros when none are set); is_set = 1 when ranges are set.  Any output may be NULL. */
+int qmb200_episode_get_ranges(const qmb200_handle* h, double* lo /*[B][QMB200_EPISODE]*/, double* hi /*[B][QMB200_EPISODE]*/, int64_t* seed, int32_t* is_set);
+/* One launch, no host work: every robot with mask[b] != 0 draws episode[b]'s row into rows[b] and the plant's robot params friction_mu[b] and payload[b];
+ * link (QMB200_EPISODE_* bits) also writes the model payload row with its SRBD row (srbd_payload_fold, as a payload estimator commit does) and the tuning
+ * rows' friction coefficients.  Robots with mask[b] == 0 are not written.  The getters (qmb200_sim_get_robot_params, qmb200_get_model_payload,
+ * qmb200_get_robot_tuning) wait for the device and report the rows written.  Fails, writing nothing, when no ranges are set, the plant's robot params
+ * were cleared since, a link's rows are not set, or the model payload link is asked while the payload estimator runs.  The start image
+ * (qmb200_robot_image_save) holds no plant or tuning rows: restore first, then sample. */
+int qmb200_episode_sample(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* episode /*[B]*/, int32_t link, double* rows /*[B][QMB200_EPISODE] in-out*/);
+int qmb200_episode_sample_dev(qmb200_handle* h, const int32_t* mask, const int32_t* episode, int32_t link, double* rows, void* cuda_stream);
+/* Host only: the rows [n][QMB200_EPISODE] of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the sampler draws. */
+int qmb200_episode_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][QMB200_EPISODE]*/);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

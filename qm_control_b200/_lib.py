@@ -88,6 +88,10 @@ for _n, _w in [("friction_mu", 1), ("wbc_friction", 1), ("mu_ee_pos", 1), ("mu_e
 TUNING = sum(w for _, w in TUNING_LAYOUT.values())   # QMB200_TUNING
 del _n, _w
 WRENCH_LAYOUT = ("f_base_x", "f_base_y", "f_base_z", "n_base_x", "n_base_y", "n_base_z", "f_ee_x", "f_ee_y", "f_ee_z", "n_ee_x", "n_ee_y", "n_ee_z")
+# one episode's plant draw (qmb200_episode_*): the columns of a row of EPISODE doubles, and the link bits of qmb200_episode_sample(_dev)
+EPISODE_LAYOUT = ("friction_mu",) + PAYLOAD_LAYOUT + ("push_t_on", "push_duration") + WRENCH_LAYOUT + ("cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate")
+EPISODE = len(EPISODE_LAYOUT)   # QMB200_EPISODE
+EPISODE_MODEL_PAYLOAD, EPISODE_MPC_FRICTION, EPISODE_WBC_FRICTION = 1, 2, 4   # QMB200_EPISODE_*
 
 
 # every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
@@ -207,6 +211,11 @@ PROTOTYPES = {
     "qmb200_robot_image_restore_dev": (I32, [P] * 3),
     "qmb200_fall_detect": (I32, [P, P, D, D, P, P]),
     "qmb200_fall_detect_dev": (I32, [P, P, D, D, P, P, P]),
+    "qmb200_episode_set_ranges": (I32, [P, P, P, I64]),
+    "qmb200_episode_get_ranges": (I32, [P] * 5),
+    "qmb200_episode_sample": (I32, [P, P, P, I32, P]),
+    "qmb200_episode_sample_dev": (I32, [P, P, P, I32, P, P]),
+    "qmb200_episode_draw": (I32, [P, I32, P, P, P]),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

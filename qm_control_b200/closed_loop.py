@@ -55,7 +55,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None):
+        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -115,6 +115,14 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     rows and a cold MPC, WBC and command FIFO, and lives on its own episode clock: its hw_write time, pushes (t_on counts from the episode's start),
     gait commands and mode schedule replay; only the sensor noise keeps the global sample index, so each episode draws new noise.  The image is freed
     when run returns.
+    randomize: dict(seed=0, <field>=(lo, hi), ...) draws a new plant for every episode (DESIGN.md §4.11): fields of _lib.EPISODE_LAYOUT (the plant's
+    friction_mu and payload columns, push_t_on and push_duration in s from the episode's start, the push wrench columns, cmd_vel_x / _y / _z and
+    cmd_yaw_rate), each bound a scalar or [B]; fields not named stay at this run's values (friction_mu, payload, pushes and cmd_vel, else the handle's
+    robot params or plant params, zero payload and no push).  The start state is read and the start image taken under those values; then every
+    episode, the first included, draws its row on the device (Solver.episode_sample_dev) right before its first solve: the plant's friction and
+    payload, its push rows and its cmd_vel.  Without respawn every robot draws episode 0 once.  model_payload="plant" also writes a drawn payload into
+    the model payload (not together with payload_estimator), tuning friction_mu="plant" / wbc_friction="plant" a drawn friction into the tuning rows.
+    The previous ranges, robot params, model payload and tuning rows are restored when run returns.
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
@@ -124,8 +132,10 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     step's t_obs, gait_templates, the table's names, target_kind[ticks, B], the kind each robot's target call took at that record's MPC tick (0
     cmd_vel, 1 ee_cmd_vel, 2 goal published, -1 goal held), and ee_target[ticks, B, 7], the final-knot end-effector pose of the target in force after
     that call); with respawn also episode[ticks, B], each robot's episode index in that record's window (0 for the first), and fallen[ticks, B], the
-    detector's flag at that window's end."""
+    detector's flag at that window's end; with randomize also episode_params[B, E, 27], the row each robot drew for each episode e < E (E: the most
+    episodes of any robot), NaN where a robot had no episode e."""
     rs = None if respawn is None else _respawn_spec(respawn)
+    rz = None if randomize is None else _randomize_spec(getattr(solver, "batch", None), randomize)
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
     if state_estimator is not None and state_estimator is not True and not isinstance(state_estimator, dict):
@@ -150,6 +160,13 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     gd = None if commands is None else _gait_commands(solver.batch, gait, commands)
     tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
+    if rz is not None:   # the links: a drawn payload / friction also goes where the run told the controller the plant's
+        if isinstance(model_payload, str) and model_payload == "plant" and set(rz["fields"]) & set(_lib.PAYLOAD_LAYOUT):
+            if payload_estimator is not None:
+                raise ValueError("closed_loop.run: model_payload=\"plant\" with a randomized payload cannot run with payload_estimator (its commits own the model payload)")
+            rz["link"] |= _lib.EPISODE_MODEL_PAYLOAD
+        if tn is not None and "friction_mu" in rz["fields"]:
+            rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
         if terrain is not None:
@@ -168,15 +185,17 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_attitude_filter(solver, attitude_filter))
         if slip_detector is not None:
             scope.enter_context(_slip_detector(solver, slip_detector))
-        if friction_mu is not None or payload is not None:
+        if friction_mu is not None or payload is not None or rz is not None:
             scope.enter_context(_robot_params(solver, friction_mu, payload))
+        if rz is not None:
+            scope.enter_context(_episode_ranges(solver))
         if gd is not None:
             scope.enter_context(_gait_dev(solver, gd))
         if rs is not None:
             scope.callback(solver.robot_image_clear)
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs)
+                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz)
 
 
 def _respawn_spec(respawn):
@@ -207,6 +226,51 @@ def _respawn_spec(respawn):
     if not spec["on_fall"] and every is None:
         raise ValueError("closed_loop.run: respawn needs on_fall or every (it would never restart a robot)")
     return dict(on_fall=bool(spec["on_fall"]), hold_windows=hold // MPC_PERIOD_MS, z_min=float(spec["z_min"]), tilt_max=float(spec["tilt_max"]), every_ms=every)
+
+
+def _randomize_spec(B, randomize):
+    """closed_loop.run's randomize → dict(seed, fields: name -> (lo, hi) float arrays, scalar or [B], link=0); ValueError when malformed.  B None: the
+    bounds' length is not checked."""
+    if not isinstance(randomize, dict):
+        raise ValueError("closed_loop.run: randomize must be None or dict(seed=..., <field>=(lo, hi), ...), got %r" % (randomize,))
+    seed = randomize.get("seed", 0)
+    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
+        raise ValueError("closed_loop.run: randomize seed must be an integer in [0, 2^64), got %r" % (seed,))
+    fields = {}
+    for k, v in randomize.items():
+        if k == "seed":
+            continue
+        if k not in _lib.EPISODE_LAYOUT:
+            raise ValueError("closed_loop.run: unknown randomize field %r (one of seed, %s)" % (k, ", ".join(_lib.EPISODE_LAYOUT)))
+        try:
+            if isinstance(v, str) or len(v) != 2 or any(isinstance(a, str) for a in v):
+                raise TypeError
+            lo, hi = (np.asarray(a, dtype=np.float64) for a in v)
+        except (TypeError, ValueError):
+            raise ValueError("closed_loop.run: randomize %s must be a pair (lo, hi) of numbers or [B] arrays, got %r" % (k, v)) from None
+        if any(a.ndim > 1 or (a.ndim == 1 and B is not None and a.shape != (B,)) for a in (lo, hi)) or (lo.ndim == hi.ndim == 1 and lo.shape != hi.shape):
+            raise ValueError("closed_loop.run: randomize %s bounds must be scalars or [%s], got shapes %s and %s" % (k, "B" if B is None else B, lo.shape, hi.shape))
+        with np.errstate(invalid="ignore", over="ignore"):
+            if not (np.all(np.isfinite(lo)) and np.all(np.isfinite(hi)) and np.all(lo <= hi) and np.all(np.isfinite(hi - lo))):
+                raise ValueError("closed_loop.run: randomize %s bounds must be finite with lo <= hi, got %r" % (k, v))
+        if k == "friction_mu" and not np.all(lo > 0.0):
+            raise ValueError("closed_loop.run: randomize friction_mu lo must be > 0")
+        if k in ("m_ee", "m_base", "push_t_on", "push_duration") and not np.all(lo >= 0.0):
+            raise ValueError("closed_loop.run: randomize %s lo must be >= 0" % k)
+        fields[k] = (lo, hi)
+    return dict(seed=int(seed), fields=fields, link=0)
+
+
+@contextlib.contextmanager
+def _episode_ranges(solver):
+    prev = solver.episode_get_ranges()
+    try:
+        yield   # _run sets this run's ranges once it has read its fixed values
+    finally:
+        if prev is None:
+            solver.episode_set_ranges(None)
+        else:
+            solver.episode_set_ranges(**prev)
 
 
 def _gait_commands(B, gait, commands):
@@ -413,7 +477,7 @@ def _robot_params(solver, friction_mu, payload):
 
 
 def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
-         rs=None):
+         rs=None, rz=None):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -425,6 +489,22 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         t_on, t_dur, wrench = (np.asarray(a, dtype=np.float64) for a in pushes)
         if t_on.shape != (B,) or t_dur.shape != (B,) or wrench.shape != (B, 12):
             raise ValueError("closed_loop.run: pushes must be (t_on[%d], duration[%d], wrench[%d, 12])" % (B, B, B))
+    if rz is not None:   # the ranges: this run's values (entered after _robot_params: the handle's robot params are this run's plant), the named fields' bounds
+        EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}
+        rp = solver.sim_get_robot_params()
+        lo = np.zeros((B, _lib.EPISODE))
+        lo[:, EP["friction_mu"]] = solver.sim_get_params()["friction_mu"] if rp["friction_mu"] is None else rp["friction_mu"]
+        if rp["payload"] is not None:
+            lo[:, EP["m_ee"]:EP["m_ee"] + 8] = rp["payload"]
+        if pushes is not None:
+            lo[:, EP["push_t_on"]] = t_on; lo[:, EP["push_duration"]] = t_dur; lo[:, EP["f_base_x"]:EP["f_base_x"] + 12] = wrench
+        lo[:, EP["cmd_vel_x"]:EP["cmd_vel_x"] + 4] = cmd_vel
+        hi = lo.copy()
+        for k, (l, h) in rz["fields"].items():
+            lo[:, EP[k]] = l; hi[:, EP[k]] = h
+        solver.episode_set_ranges(lo, hi, rz["seed"])
+        if pushes is None and np.any(hi[:, EP["push_duration"]] > 0.0):   # the draws overwrite these rows before the first solve
+            t_on, t_dur, wrench = np.zeros(B), np.zeros(B), np.zeros((B, 12)); pushes = (t_on, t_dur, wrench)
     stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
     f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
     i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
@@ -526,12 +606,31 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             due = torch.ones_like(episode); rec_episode = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_fallen = torch.zeros_like(rec_episode)
         solver.robot_image_restore_dev(due, s)
 
-    def respawn(k):   # the robots due restart at window boundary k: the library's rows, then the loop's
+    def respawn(k):   # the robots due restart at window boundary k: the library's rows, then the loop's, then their new plant
         solver.robot_image_restore_dev(due, s)
         m = due.bool()
         for a, a0 in zip(own, start):
             a.copy_(torch.where(m.view((B,) + (1,) * (a.dim() - 1)), a0, a))
         k0.copy_(torch.where(m, k, k0)); episode.add_(due); fall_count.masked_fill_(m, 0)
+        if rz is not None:
+            draw(due, episode)
+
+    def draw(mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
+        solver.episode_sample_dev(mask, idx, ep_rows, rz["link"], s)
+        m = mask.bool()
+        cmd7[:, :4] = torch.where(m[:, None], ep_rows[:, 23:27], cmd7[:, :4])
+        if push is not None:
+            on = ep_rows[:, 9] * 1e3 - 1e-6; off = (ep_rows[:, 9] + ep_rows[:, 10]) * 1e3 - 1e-6
+            push["on"].copy_(torch.where(m, on, push["on"])); push["off"].copy_(torch.where(m, off, push["off"]))
+            push["wrench"].copy_(torch.where(m[:, None], ep_rows[:, 11:23], push["wrench"]))
+
+    if rz is not None:   # every robot's first episode draws its row right before the first solve (after the restore of the start image)
+        with torch.cuda.stream(stream):
+            ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev)
+            if rs is None:
+                draw(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
+            else:
+                draw(due, episode)
 
     with torch.cuda.stream(stream):
         mpc_tick(0); stream.synchronize()          # QMController::starting: one blocking solve before the loop
@@ -602,4 +701,9 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                    ee_target=rec_ee_target.cpu().numpy())
     if rs is not None:
         out.update(episode=rec_episode.cpu().numpy(), fallen=rec_fallen.cpu().numpy())
+    if rz is not None:   # rebuilt on the host from the episode record: the sampler's rows are a pure function of (ranges, seed, robot, episode)
+        ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
+        had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
+        rb, re_ = np.nonzero(had)
+        out["episode_params"] = np.full(had.shape + (_lib.EPISODE,), np.nan); out["episode_params"][rb, re_] = solver.episode_draw(rb, re_)
     return out

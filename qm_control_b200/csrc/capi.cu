@@ -20,6 +20,7 @@
 #include "kernels/slip_api.cuh"
 #include "kernels/gait_api.cuh"
 #include "kernels/respawn_api.cuh"
+#include "kernels/episode_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -83,6 +84,10 @@ struct qmb200_handle {
     int32_t* d_ee_kind = nullptr; double* d_ee = nullptr;   // the timeline's end-effector commands [B][n_cmd] and [B][n_cmd][7], NULL when it has none
   } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
+  bool plant_on_device = false, tuning_on_device = false;   // an episode draw wrote mu / payload or tuning on the device: plant_ / tuning_rows_sync refresh them
+  struct {   // per-episode plant draws (capi_episode.inc): the robots' ranges [B][EP_DBL] (empty: none set), their device copies (dalloc: freed with allocs) and the seed
+    std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0;
+  } episode;
   uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
   struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
     bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
@@ -260,16 +265,17 @@ std::string payload_error(const double* payload, size_t n, const char* who) {
   }
   return "";
 }
-// After a payload estimator commit the device holds the model payload rows: wait for it and copy them into the host copies, which say what is set
-int model_rows_sync(const qmb200_handle* hc) {
-  qmb200_handle* h = const_cast<qmb200_handle*>(hc);
-  if (!h->model_on_device) return 0;
-  const size_t B = (size_t)h->B;
+// After a kernel wrote robot rows on the device (a payload estimator commit, a restore, an episode draw) the device holds them: when on_device says so,
+// wait for it and copy them into the host copies, which say what is set and what the getters report
+int rows_sync(qmb200_handle* h, bool& on_device, std::initializer_list<RobotArray*> arrays) {
+  if (!on_device) return 0;
   QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());
-  QMB_CUDA(h, cudaMemcpy(h->mpayload.host.data(), h->mpayload.d, B * 8 * 8, cudaMemcpyDeviceToHost));
-  QMB_CUDA(h, cudaMemcpy(h->srbd.host.data(), h->srbd.d, B * SRBD_DBL * 8, cudaMemcpyDeviceToHost));
-  h->model_on_device = false; return 0;
+  for (RobotArray* a : arrays) QMB_CUDA(h, cudaMemcpy(a->host.data(), a->d, a->host.size() * 8, cudaMemcpyDeviceToHost));
+  on_device = false; return 0;
 }
+int model_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->model_on_device, {&h->mpayload, &h->srbd}); }
+int plant_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->plant_on_device, {&h->mu, &h->payload}); }
+int tuning_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->tuning_on_device, {&h->tuning}); }
 // SRBD constants of n robots with payload rows [n][8] (NULL: none)
 void srbd_rows(const HostModel& hm, const double* payload, size_t n, double* out) {
   for (size_t b = 0; b < n; ++b) srbd_constants(hm.dev, payload ? payload + 8 * b : nullptr, out + SRBD_DBL * b);
@@ -335,10 +341,14 @@ int qmb200_set_robot_tuning(qmb200_handle* h, const double* rows) {
     const char* why = !std::isfinite(v) ? "must be finite" : (i < 2 && !(v > 0.0)) ? "must be > 0" : (v < 0.0) ? "must be >= 0" : nullptr;
     if (why) return fail(h, std::string("qmb200_set_robot_tuning: ") + tuning_field(i) + " of robot " + std::to_string(b) + " " + why);
   }
-  return set_robot_arrays(h, {{&h->tuning, rows}});
+  const int rc = set_robot_arrays(h, {{&h->tuning, rows}});
+  if (!rc) h->tuning_on_device = false;   // set_robot_arrays waited for the device: the rows just written replace any drawn ones
+  return rc;
 }
 int qmb200_get_robot_tuning(const qmb200_handle* h, double* rows, int32_t* is_set) {
-  if (!h) return -1; const size_t B = (size_t)h->B; const std::vector<double>& t = h->tuning.host;
+  if (!h) return -1; const size_t B = (size_t)h->B;
+  if (int rc = tuning_rows_sync(h)) return rc;
+  const std::vector<double>& t = h->tuning.host;
   if (rows) { if (t.empty()) for (size_t b = 0; b < B; ++b) handle_tuning(h, rows + b * TUNING_DBL); else std::memcpy(rows, t.data(), B * TUNING_DBL * 8); }
   if (is_set) *is_set = t.empty() ? 0 : 1;
   return 0;
@@ -434,3 +444,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_slip.inc"
 #include "capi_gait.inc"
 #include "capi_respawn.inc"
+#include "capi_episode.inc"

@@ -304,6 +304,12 @@ QMB_HD void srbd_payload_fold(const DevModel& d, const double* pl, double* out) 
   for (int i = 22; i < SRBD_DBL; ++i) o[i] = 0.0;
 }
 
+// splitmix64's finaliser: a bijection of 64-bit words whose output bits each depend on every input bit.  The counter-based draws hash their keys with
+// it: the sensor noise (state_est_api.cuh) and the per-episode plant rows (episode_api.cuh).
+QMB_HD uint64_t mix64(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull; z = (z ^ (z >> 27)) * 0x94d049bb133111ebull; return z ^ (z >> 31);
+}
+
 // modeNumber2StanceLeg: bit3 LF, bit2 RF, bit1 LH, bit0 RH (contact order LF,RF,LH,RH)
 QMB_HD bool contact_flag(int mode, int foot) { return (mode >> (3 - foot)) & 1; }
 

@@ -16,10 +16,6 @@ static_assert(SEN_JVEL + NJ == QMB200_SENSORS, "sensor layout of include/qmb200.
 // noise channels of one reading: orientation (3), gyro (3), accel (3), joint pos (18), joint vel (18)
 constexpr int CH_ORI = 0, CH_GYRO = 3, CH_ACCEL = 6, CH_JPOS = 9, CH_JVEL = 27;
 
-// splitmix64's finaliser: a bijection of 64-bit words whose output bits each depend on every input bit
-QMB_HD uint64_t mix64(uint64_t z) {
-  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull; z = (z ^ (z >> 27)) * 0x94d049bb133111ebull; return z ^ (z >> 31);
-}
 // One standard normal draw, a pure function of (seed, robot, sample, channel): the four words are hashed in turn, two 53-bit uniforms in (0, 1) are cut
 // from two more hashes, and Box-Muller's cosine branch turns them into N(0, 1).  No generator state, so a draw does not depend on the batch or the launch.
 QMB_HD double sensor_normal(uint64_t seed, uint64_t robot, uint64_t sample, int channel) {

@@ -705,6 +705,41 @@ class Solver:
         <= z_min, or |pitch|, |roll| >= tilt_max; count [B] int32 grows by one per fallen call and drops to 0 otherwise.  No synchronisation."""
         self._call("fall_detect_dev", _p(rbd), float(z_min), float(tilt_max), _p(count), _p(fallen), stream)
 
+    # ---------------- per-episode plant draws (include/qmb200.h: qmb200_episode_*; DESIGN.md §4.11) ----------------
+    def episode_set_ranges(self, lo=None, hi=None, seed=0):
+        """Per-robot ranges lo, hi [B, EPISODE] (columns _lib.EPISODE_LAYOUT) and a 64-bit seed of the per-episode draws; None clears them.  Makes sure
+        the plant's robot params are set (at the values in force where they were not).  Synchronous."""
+        if lo is None and hi is None:
+            self._call("episode_set_ranges", None, None, 0); return
+        shape = (self.batch, _lib.EPISODE); lo = _f64(lo, shape); hi = _f64(hi, shape)
+        s = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._call("episode_set_ranges", _p(lo), _p(hi), s - (1 << 64) if s >> 63 else s)
+
+    def episode_get_ranges(self):
+        """→ dict(lo [B, EPISODE], hi [B, EPISODE], seed) of the stored ranges, or None when none are set."""
+        lo = np.zeros((self.batch, _lib.EPISODE)); hi = np.zeros_like(lo); seed = C.c_int64(); is_set = C.c_int32()
+        self._call("episode_get_ranges", _p(lo), _p(hi), C.byref(seed), C.byref(is_set))
+        return dict(lo=lo, hi=hi, seed=seed.value & 0xFFFFFFFFFFFFFFFF) if is_set.value else None
+
+    def episode_sample(self, mask, episode, link=0, rows=None):
+        """Host variant of episode_sample_dev: mask [B], episode [B] → rows [B, EPISODE] (rows of unmasked robots as given, zeros by default)."""
+        B = self.batch; rows = np.zeros((B, _lib.EPISODE)) if rows is None else _f64(rows, (B, _lib.EPISODE)).copy()
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,)); episode = _i32(np.broadcast_to(np.asarray(episode), (B,)), (B,))
+        self._call("episode_sample", _p(mask), _p(episode), int(link), _p(rows))
+        return rows
+
+    def episode_sample_dev(self, mask, episode, rows, link=0, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) draws episode[b]'s row (int32 [B]) into rows [B, EPISODE] (float64 device tensor) and
+        the plant's robot params; link (_lib.EPISODE_* bits) also writes the model payload and the tuning rows' friction coefficients.  One launch, no
+        synchronisation."""
+        self._call("episode_sample_dev", _p(mask), _p(episode), int(link), _p(rows), stream)
+
+    def episode_draw(self, robot, episode):
+        """Host only: robot [n] (in [0, B)), episode [n] → the rows [n, EPISODE] the sampler draws for them on the stored ranges and seed."""
+        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); rows = np.zeros((len(robot), _lib.EPISODE))
+        self._call("episode_draw", len(robot), _p(robot), _p(episode), _p(rows))
+        return rows
+
     # ---------------- device gait schedule (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7) ----------------
     def gait_dev_set_templates(self, names=None, gait_file=None):
         """Load the template table: names (default: every template of the gait file, in the order of its list) → the names, a template's id being its

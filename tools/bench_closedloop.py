@@ -6,7 +6,7 @@ deviation from the initial pose, as percentiles over the robots) of this project
 
     python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter] [--slip-detector]]
                                      [--gait-commands] [--ee-goals]
-    python tools/bench_closedloop.py --respawn [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
+    python tools/bench_closedloop.py --respawn [--randomize] [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -71,6 +71,12 @@ robot-second and the fraction of episodes that fall within their first second, f
 least 1 s before the run's end (with binomial standard deviations);
 the wall time per simulated second of --duration runs with and without respawn, alternated in one process; and the device time per call of the fall
 detector and the image restore against the plant step (CUDA events, alternated blocks).
+
+--respawn --randomize draws a new plant for every episode (closed_loop.run(randomize=...)): floor friction in [0.15, 1.0], end-effector payload in
+[0, 2] kg and a base push of (f_x, f_y) in [-180, 180] N each for 0.1 s from t_on in [0.2, 0.5] s of the episode.  It prints one JSON line "randomize"
+with, from one 5 s run, the episodes per robot and the fraction of episodes that fall within their first second per friction bin x push-magnitude bin
+(episodes that start at least 1 s before the run's end); the wall time per simulated second of --duration runs with and without randomize (both with
+respawn), alternated in one process; and the device time per call of the sampler against the image restore (CUDA events, alternated blocks).
 """
 import argparse
 import json
@@ -474,6 +480,83 @@ def respawn_rates(r, ep_s=1.0):
             "fell_within_%gs_first_episodes" % ep_s: frac(first), "fell_within_%gs_later_episodes" % ep_s: frac(later)}
 
 
+RANDOMIZE = dict(seed=0, friction_mu=(0.15, 1.0), m_ee=(0.0, 2.0), push_t_on=(0.2, 0.5), push_duration=(0.1, 0.1), f_base_x=(-180.0, 180.0), f_base_y=(-180.0, 180.0))
+MU_BINS, PUSH_BINS = [0.15, 0.3, 0.45, 0.6, 0.8, 1.0], [0.0, 60.0, 120.0, 180.0, 255.0]
+
+
+def episode_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per sampler call (every robot masked, and none) and per image restore of every robot, alternated `reps` times in blocks of `calls`
+    (CUDA events), with RANDOMIZE's ranges and the state estimator running and imaged → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, _ = solver.sim_standing_state(xy_yaw)
+    EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}; lo = np.zeros((B, _lib.EPISODE)); lo[:, EP["friction_mu"]] = 0.6; hi = lo.copy()
+    for k, v in RANDOMIZE.items():
+        if k != "seed":
+            lo[:, EP[k]], hi[:, EP[k]] = v
+    every = torch.ones(B, dtype=torch.int32, device=dev); none = torch.zeros_like(every); ep = torch.zeros_like(every)
+    rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev)
+    prev = solver.sim_get_robot_params()
+    solver.hw_set_delay(0.009); solver.state_est_reset(q0[:, 0:3]); solver.robot_image_save(); solver.episode_set_ranges(lo, hi, 0)
+    calls_of = {"sample_all": lambda: solver.episode_sample_dev(every, ep, rows, 0, s.cuda_stream), "sample_none": lambda: solver.episode_sample_dev(none, ep, rows, 0, s.cuda_stream),
+                "restore_all": lambda: solver.robot_image_restore_dev(every, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    call()
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.episode_set_ranges(None); solver.sim_set_robot_params(**prev); solver.robot_image_clear(); solver.state_est_stop()
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls; the image holds the state estimator's rows" % (B, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}, "spread_sample_all": [float(min(times["sample_all"])), float(max(times["sample_all"]))]}
+
+
+def randomize_falls(r, ep_s=1.0):
+    """Per friction bin x push-magnitude bin of a closed_loop.run(respawn=..., randomize=RANDOMIZE) result: the episodes that start at least ep_s before
+    the run's end and how many of them fall within their first ep_s seconds"""
+    ep, fl, P = r["episode"], r["fallen"].astype(bool), r["episode_params"]; ticks, B = ep.shape; w = int(round(ep_s * 100))
+    EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}
+    fell = np.zeros((len(MU_BINS) - 1, len(PUSH_BINS) - 1), dtype=int); n = np.zeros_like(fell)
+    for b in range(B):
+        for e in range(int(ep[-1, b]) + 1):
+            rows = np.flatnonzero(ep[:, b] == e)
+            if rows[0] + w > ticks:
+                continue
+            mu = P[b, e, EP["friction_mu"]]; f = np.hypot(P[b, e, EP["f_base_x"]], P[b, e, EP["f_base_y"]])
+            i = min(np.searchsorted(MU_BINS, mu, side="right") - 1, len(MU_BINS) - 2); j = min(np.searchsorted(PUSH_BINS, f, side="right") - 1, len(PUSH_BINS) - 2)
+            n[i, j] += 1; fell[i, j] += int(fl[rows[:w], b].any())
+    return {"mu_bins": MU_BINS, "push_bins_N": PUSH_BINS, "episodes": n.tolist(), "fell": fell.tolist(),
+            "fraction": np.where(n > 0, fell / np.maximum(n, 1), np.nan).round(4).tolist(), "total_episodes": int(n.sum()), "total_fell": int(fell.sum())}
+
+
+def randomize_main(args, solver, kw, xy, timed, episode_run_s=5.0):
+    """--respawn --randomize: the same loop with RANDOMIZE drawn per episode.  One run of episode_run_s for the falls per bin; the wall time per
+    simulated second of --duration runs with and without randomize (both with respawn), alternated twice after one warm-up run of each; the sampler's
+    per-call device time."""
+    wall = {False: [], True: []}
+    for rep in range(3):   # the first round warms up
+        for rnd in (False, True):
+            _, w = timed(True, args.duration, randomize=RANDOMIZE if rnd else None)
+            if rep:
+                wall[rnd].append(w)
+    r, _ = timed(True, episode_run_s, randomize=RANDOMIZE)
+    name, limit = card()
+    print(json.dumps({"metric": "randomize", "gpu": name, "power_limit": limit, "batch": solver.batch,
+                      "config": "%s at %.2f m/s on the state estimate, reference IMU noise, no attitude filter; respawn after 0.1 s fallen; per episode: friction_mu "
+                                "U[0.15, 1.0], m_ee U[0, 2] kg, base push f_x, f_y U[-180, 180] N for 0.1 s from t_on U[0.2, 0.5] s" % (args.gait, args.vx),
+                      "simulated_s": episode_run_s, "episodes_per_robot": float(np.mean(r["episode"][-1] + 1)),
+                      "fell_within_1s": randomize_falls(r),
+                      "wall_s_per_sim_s": {"label": "runs of %.1f s with respawn, two alternated pairs after a warm-up pair" % args.duration,
+                                           "without_randomize": wall[False], "with_randomize": wall[True]},
+                      "per_call": episode_times(solver, xy)}))
+
+
 def respawn_main(args, episode_run_s=5.0):
     """--respawn: trot at --vx on the estimate from the reference IMU noise without the attitude filter, robots restarted after 0.1 s fallen.  One
     run of episode_run_s for the rates; the wall time per simulated second of --duration runs with and without respawn, alternated twice after one
@@ -488,11 +571,13 @@ def respawn_main(args, episode_run_s=5.0):
     xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
     kw = dict(gait=args.gait, cmd_vel=cmd, xy_yaw=xy, state_estimator=True, sensor_noise="reference")
 
-    def timed(respawn, duration):
+    def timed(respawn, duration, randomize=None):
         solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
-        r = closed_loop.run(solver, duration=duration, **kw, **({"respawn": dict(hold=0.1)} if respawn else {}))
+        r = closed_loop.run(solver, duration=duration, **kw, **({"respawn": dict(hold=0.1)} if respawn else {}), **({"randomize": randomize} if randomize else {}))
         torch.cuda.synchronize(dev)
         return r, (time.perf_counter() - t0) / duration
+    if args.randomize:
+        return randomize_main(args, solver, kw, xy, timed)
     wall = {False: [], True: []}
     for rep in range(3):   # the first round warms up
         for respawn in (False, True):
@@ -549,7 +634,10 @@ def main():
     ap.add_argument("--ee-goals", action="store_true", help="end-effector goals on the device command timeline: a reach sweep and the target call's time")
     ap.add_argument("--ee-tuning", action="store_true", help="with --ee-goals: the reach sweep again with per-robot end-effector weights, WBC end-effector gains and kd_arm_wbc")
     ap.add_argument("--respawn", action="store_true", help="restart robots that fell (hold 0.1 s) on the reference IMU noise without the attitude filter: episode rates")
+    ap.add_argument("--randomize", action="store_true", help="with --respawn: a new plant per episode (friction, payload, push): falls per friction x push bin")
     args = ap.parse_args()
+    if args.randomize and not args.respawn:
+        ap.error("--randomize needs --respawn")
     if args.respawn:
         return respawn_main(args)
     if args.ee_tuning and not args.ee_goals:
