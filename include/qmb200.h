@@ -609,6 +609,41 @@ int qmb200_episode_sample_dev(qmb200_handle* h, const int32_t* mask, const int32
 /* Host only: the rows [n][QMB200_EPISODE] of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the sampler draws. */
 int qmb200_episode_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][QMB200_EPISODE]*/);
 
+/* ---- per-episode spawns (DESIGN.md §4.12): each episode of each robot starts on new ground, drawn on the device right after its restart.
+ *   row[QMB200_SPAWN]  0  tile    the plant's tile for the episode, an integer in [-1, n_tiles) (-1: the plane)
+ *                      1  dx      the robot stands dx, dy m further along its tile, world axes: the tile's origin becomes the robot's origin at the set
+ *                      2  dy      minus (dx, dy).  The base's world x, y do not move; the ground moves under it.  Tiles are not rotated.
+ *                      3  yaw     the base yaw, in [-pi, pi]
+ * Column c of robot b in episode e: a uniform u in (0, 1) of (seed ^ a domain constant of its own, global robot rank * B + b, e, c) as the episode draw
+ * hashes them; dx, dy and yaw are fma(u, hi - lo, lo), the tile is lo + min(floor(u (hi - lo + 1)), hi - lo); a column with lo == hi is lo itself. */
+#define QMB200_SPAWN 4
+#define QMB200_SPAWN_GROUND_MAP 1   /* link: the drawn terrain row also goes to the state estimator's ground map (qmb200_state_est_set_ground) */
+/* Per-robot ranges lo, hi [B][QMB200_SPAWN] and the seed.  NULL lo and hi clear them.  Rejects a non-finite bound, lo > hi, a non-finite hi - lo, tile
+ * bounds that are not integers in [-1, n_tiles) of the library in force and yaw bounds outside [-pi, pi], naming the field and the robot; on rejection
+ * the stored ranges stay unchanged.  The set takes the robots' tile origins from the plant's robot terrain rows in force (zeros where none are set),
+ * and when any tile bound is >= 0 makes sure those rows exist (tile -1, origin 0 where they were not set).  Host arrays; synchronous. */
+int qmb200_spawn_set_ranges(qmb200_handle* h, const double* lo /*[B][QMB200_SPAWN] or NULL*/, const double* hi /*[B][QMB200_SPAWN] or NULL*/, int64_t seed);
+/* The stored ranges and seed (zeros when none are set); is_set = 1 when ranges are set.  Any output may be NULL. */
+int qmb200_spawn_get_ranges(const qmb200_handle* h, double* lo /*[B][QMB200_SPAWN]*/, double* hi /*[B][QMB200_SPAWN]*/, int64_t* seed, int32_t* is_set);
+/* One launch, no host work: every robot with mask[b] != 0 draws episode[b]'s spawn row into rows[b] and stands there.  It writes the plant's robot terrain
+ * row [tile, origin - (dx, dy)] (when the plant has robot terrain rows) and, with link QMB200_SPAWN_GROUND_MAP, the estimator's ground-map row to the same
+ * values; q[b]: x, y as given, the standing pose on that ground (qmb200_sim_standing_state's, on the plane bit for bit), the drawn yaw, defaultJointState;
+ * v[b] = 0; rbd[b] the measured state at (q, 0) with the end-effector pose; contact[b] the feet the plant's contact law presses into the ground there;
+ * x_obs[b] the observation of rbd[b] (qmb200_centroidal_state_from_rbd); last_ee[b] (the held end-effector target, position and quaternion xyzw) turned
+ * about the vertical through the base by the drawn yaw minus the given q[b]'s yaw; rbd_est[b] = rbd[b] when rbd_est is given; and the rows the resets
+ * write for every component that runs: the state estimator's as qmb200_state_est_reset at the new base position (its next call places the feet), the
+ * attitude filter's as qmb200_attitude_reset, the slip detector's zeroed.  Robots with mask[b] == 0 are not written.  The getters
+ * (qmb200_sim_get_robot_terrain, qmb200_state_est_get_ground, qmb200_sim_standing_state) wait for the device and report the rows written.  Fails,
+ * writing nothing, when no ranges are set, the library has fewer tiles than a stored bound, the ground-map link has no map, or the plant's robot terrain
+ * rows were cleared since the set. */
+int qmb200_spawn_sample(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* episode /*[B]*/, int32_t link, double* rows /*[B][QMB200_SPAWN] in-out*/,
+                        double* q /*[B][24] in-out*/, double* v /*[B][24] in-out*/, double* rbd /*[B][55] in-out*/, int32_t* contact /*[B] in-out*/,
+                        double* x_obs /*[B][30] in-out*/, double* last_ee /*[B][7] in-out*/, double* rbd_est /*[B][55] in-out or NULL*/);
+int qmb200_spawn_sample_dev(qmb200_handle* h, const int32_t* mask, const int32_t* episode, int32_t link, double* rows, double* q, double* v, double* rbd, int32_t* contact,
+                            double* x_obs, double* last_ee, double* rbd_est, void* cuda_stream);
+/* Host only: the rows [n][QMB200_SPAWN] of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the sampler draws. */
+int qmb200_spawn_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][QMB200_SPAWN]*/);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

@@ -92,6 +92,10 @@ WRENCH_LAYOUT = ("f_base_x", "f_base_y", "f_base_z", "n_base_x", "n_base_y", "n_
 EPISODE_LAYOUT = ("friction_mu",) + PAYLOAD_LAYOUT + ("push_t_on", "push_duration") + WRENCH_LAYOUT + ("cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate")
 EPISODE = len(EPISODE_LAYOUT)   # QMB200_EPISODE
 EPISODE_MODEL_PAYLOAD, EPISODE_MPC_FRICTION, EPISODE_WBC_FRICTION = 1, 2, 4   # QMB200_EPISODE_*
+# one episode's spawn (qmb200_spawn_*): the columns of a row of SPAWN doubles, and the link bit of qmb200_spawn_sample(_dev)
+SPAWN_LAYOUT = ("tile", "dx", "dy", "yaw")
+SPAWN = len(SPAWN_LAYOUT)   # QMB200_SPAWN
+SPAWN_GROUND_MAP = 1        # QMB200_SPAWN_GROUND_MAP
 
 
 # every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
@@ -216,6 +220,11 @@ PROTOTYPES = {
     "qmb200_episode_sample": (I32, [P, P, P, I32, P]),
     "qmb200_episode_sample_dev": (I32, [P, P, P, I32, P, P]),
     "qmb200_episode_draw": (I32, [P, I32, P, P, P]),
+    "qmb200_spawn_set_ranges": (I32, [P, P, P, I64]),
+    "qmb200_spawn_get_ranges": (I32, [P] * 5),
+    "qmb200_spawn_sample": (I32, [P, P, P, I32] + [P] * 8),
+    "qmb200_spawn_sample_dev": (I32, [P, P, P, I32] + [P] * 9),
+    "qmb200_spawn_draw": (I32, [P, I32, P, P, P]),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

@@ -55,7 +55,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None):
+        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -123,6 +123,16 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     payload, its push rows and its cmd_vel.  Without respawn every robot draws episode 0 once.  model_payload="plant" also writes a drawn payload into
     the model payload (not together with payload_estimator), tuning friction_mu="plant" / wbc_friction="plant" a drawn friction into the tuning rows.
     The previous ranges, robot params, model payload and tuning rows are restored when run returns.
+    spawn: dict(seed=0, tile=(lo, hi), dx=(lo, hi), dy=(lo, hi), yaw=(lo, hi)) starts every episode on new ground (DESIGN.md §4.12), each bound a scalar
+    or [B]: the plant's tile (an integer of the run's library, -1 the plane), the offset (dx, dy) in m the robot stands further along it (world axes:
+    the tile moves by -(dx, dy) under the robot, whose world x, y stay), and the base yaw in [-pi, pi].  Columns not named stay at this run's values
+    (the robot's terrain row, no offset, xy_yaw's yaw, wrapped into [-pi, pi] where it lies outside).  tile, dx and dy need terrain; with
+    ground_map=True the estimator's map follows the draw, and a ground_map dict cannot go with them; a yaw that is not fixed cannot go with ee_goal /
+    ee_cmd_vel commands (their world-frame goals assume +x).  The start image is taken under the run's own pose; then every episode, the first included, draws its spawn on the device (Solver.spawn_sample_dev)
+    right after its restore and its randomize draw and before its first solve: the plant's terrain row, the standing pose there, the measured state,
+    the observation, the held end-effector target turned with the base and the estimators' reset rows.  Without respawn every robot spawns episode 0
+    once.  The previous terrain rows and ground map are restored when run returns, and then the previous ranges, whose offsets count again from the
+    origins of the restored robot terrain rows (the origins are read when ranges are set, and are not part of what spawn_get_ranges reports).
     sim_timer: optional callable(start: bool) wrapped around every sim_step_dev (tools/bench_closedloop.py brackets them with CUDA events).
     Returns dict(t[ticks], base[ticks, B, 6] = (x, y, z, yaw, pitch, roll), ee[ticks, B, 7] = (pos, quat xyzw), status[ticks, B] = OR of the WBC /
     safety, hw_write and plant status words since the previous record, contact[B] at the end, q[B, 24], v[B, 24] at the end; with payload_estimator also
@@ -133,7 +143,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     cmd_vel, 1 ee_cmd_vel, 2 goal published, -1 goal held), and ee_target[ticks, B, 7], the final-knot end-effector pose of the target in force after
     that call); with respawn also episode[ticks, B], each robot's episode index in that record's window (0 for the first), and fallen[ticks, B], the
     detector's flag at that window's end; with randomize also episode_params[B, E, 27], the row each robot drew for each episode e < E (E: the most
-    episodes of any robot), NaN where a robot had no episode e."""
+    episodes of any robot), NaN where a robot had no episode e; with spawn also spawn_params[B, E, 4], the spawn row of each such episode."""
     rs = None if respawn is None else _respawn_spec(respawn)
     rz = None if randomize is None else _randomize_spec(getattr(solver, "batch", None), randomize)
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
@@ -160,6 +170,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     gd = None if commands is None else _gait_commands(solver.batch, gait, commands)
     tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
+    sp = None if spawn is None else _spawn_spec(getattr(solver, "batch", None), spawn, terrain, ground_map, gd)
     if rz is not None:   # the links: a drawn payload / friction also goes where the run told the controller the plant's
         if isinstance(model_payload, str) and model_payload == "plant" and set(rz["fields"]) & set(_lib.PAYLOAD_LAYOUT):
             if payload_estimator is not None:
@@ -169,6 +180,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
+        if sp is not None:   # restored last: the earlier ranges are set again on the earlier library and robot terrain rows, which give their origins
+            scope.enter_context(_spawn_ranges(solver))
         if terrain is not None:
             scope.enter_context(_terrain(solver, terrain))
         if ground_map is not None:
@@ -195,7 +208,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.callback(solver.robot_image_clear)
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz)
+                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp)
 
 
 def _respawn_spec(respawn):
@@ -259,6 +272,61 @@ def _randomize_spec(B, randomize):
             raise ValueError("closed_loop.run: randomize %s lo must be >= 0" % k)
         fields[k] = (lo, hi)
     return dict(seed=int(seed), fields=fields, link=0)
+
+
+def _spawn_spec(B, spawn, terrain, ground_map, gd):
+    """closed_loop.run's spawn (with its terrain, ground_map and parsed commands) → dict(seed, fields: name -> (lo, hi) float arrays, scalar or [B],
+    link); ValueError when malformed.  B None: the bounds' length is not checked."""
+    if not isinstance(spawn, dict):
+        raise ValueError("closed_loop.run: spawn must be None or dict(seed=..., tile=(lo, hi), dx=(lo, hi), dy=(lo, hi), yaw=(lo, hi)), got %r" % (spawn,))
+    seed = spawn.get("seed", 0)
+    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
+        raise ValueError("closed_loop.run: spawn seed must be an integer in [0, 2^64), got %r" % (seed,))
+    fields = {}
+    for k, v in spawn.items():
+        if k == "seed":
+            continue
+        if k not in _lib.SPAWN_LAYOUT:
+            raise ValueError("closed_loop.run: unknown spawn field %r (one of seed, %s)" % (k, ", ".join(_lib.SPAWN_LAYOUT)))
+        try:
+            if isinstance(v, str) or len(v) != 2 or any(isinstance(a, str) for a in v):
+                raise TypeError
+            lo, hi = (np.asarray(a, dtype=np.float64) for a in v)
+        except (TypeError, ValueError):
+            raise ValueError("closed_loop.run: spawn %s must be a pair (lo, hi) of numbers or [B] arrays, got %r" % (k, v)) from None
+        if any(a.ndim > 1 or (a.ndim == 1 and B is not None and a.shape != (B,)) for a in (lo, hi)) or (lo.ndim == hi.ndim == 1 and lo.shape != hi.shape):
+            raise ValueError("closed_loop.run: spawn %s bounds must be scalars or [%s], got shapes %s and %s" % (k, "B" if B is None else B, lo.shape, hi.shape))
+        with np.errstate(invalid="ignore", over="ignore"):
+            if not (np.all(np.isfinite(lo)) and np.all(np.isfinite(hi)) and np.all(lo <= hi) and np.all(np.isfinite(hi - lo))):
+                raise ValueError("closed_loop.run: spawn %s bounds must be finite with lo <= hi, got %r" % (k, v))
+        if k == "yaw" and not (np.all(lo >= -np.pi) and np.all(hi <= np.pi)):
+            raise ValueError("closed_loop.run: spawn yaw bounds must lie in [-pi, pi]")
+        fields[k] = (lo, hi)
+    ground = set(fields) & {"tile", "dx", "dy"}
+    if ground and terrain is None:
+        raise ValueError("closed_loop.run: spawn %s needs terrain (it moves the plant's tile under the robot)" % ", ".join(sorted(ground)))
+    if "tile" in fields:
+        lo, hi = fields["tile"]; n = len(terrain["tiles"])
+        if not (np.all(np.floor(lo) == lo) and np.all(np.floor(hi) == hi) and np.all(lo >= -1) and np.all(hi < n)):
+            raise ValueError("closed_loop.run: spawn tile bounds must be integers in [-1, %d), the run's tile library" % n)
+    if ground and isinstance(ground_map, dict):
+        raise ValueError("closed_loop.run: a ground_map dict cannot go with a spawn that draws %s (the map would not follow the ground; ground_map=True does)"
+                         % ", ".join(sorted(ground)))
+    if "yaw" in fields and gd is not None and gd["ee"] and np.any(fields["yaw"][0] != fields["yaw"][1]):
+        raise ValueError("closed_loop.run: a drawn spawn yaw cannot go with ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)")
+    return dict(seed=int(seed), fields=fields, link=_lib.SPAWN_GROUND_MAP if ground_map is True else 0)
+
+
+@contextlib.contextmanager
+def _spawn_ranges(solver):
+    prev = solver.spawn_get_ranges()
+    try:
+        yield   # _run sets this run's ranges once it has read its fixed values
+    finally:
+        if prev is None:
+            solver.spawn_set_ranges(None)
+        else:
+            solver.spawn_set_ranges(**prev)
 
 
 @contextlib.contextmanager
@@ -477,7 +545,7 @@ def _robot_params(solver, friction_mu, payload):
 
 
 def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
-         rs=None, rz=None):
+         rs=None, rz=None, sp=None):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -505,12 +573,21 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         solver.episode_set_ranges(lo, hi, rz["seed"])
         if pushes is None and np.any(hi[:, EP["push_duration"]] > 0.0):   # the draws overwrite these rows before the first solve
             t_on, t_dur, wrench = np.zeros(B), np.zeros(B), np.zeros((B, 12)); pushes = (t_on, t_dur, wrench)
+    xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
+    if sp is not None:   # the ranges: this run's values (entered after _terrain: the robot terrain rows are this run's), the named columns' bounds
+        SP = {n: i for i, n in enumerate(_lib.SPAWN_LAYOUT)}
+        rt = solver.sim_get_robot_terrain()
+        yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)   # the same heading within [-pi, pi]
+        lo = np.zeros((B, _lib.SPAWN)); lo[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; lo[:, SP["yaw"]] = yaw
+        hi = lo.copy()
+        for k, (l, h) in sp["fields"].items():
+            lo[:, SP[k]] = l; hi[:, SP[k]] = h
+        solver.spawn_set_ranges(lo, hi, sp["seed"])
     stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
     f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
     i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
 
     # ---- plant state, the first measurement, the controller's members (host → device once) ----
-    xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
     q0, v0 = solver.sim_standing_state(xy)
     t_obs0 = t_start - wbc_period_ms * 1e-3   # observation clock of `starting`; the first update brings it to t_start, the plant's clock
     if gd is None:
@@ -614,6 +691,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         k0.copy_(torch.where(m, k, k0)); episode.add_(due); fall_count.masked_fill_(m, 0)
         if rz is not None:
             draw(due, episode)
+        if sp is not None:
+            stand(due, episode)
 
     def draw(mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
         solver.episode_sample_dev(mask, idx, ep_rows, rz["link"], s)
@@ -631,6 +710,17 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                 draw(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
             else:
                 draw(due, episode)
+
+    def stand(mask, idx):   # the masked robots spawn episode idx: new ground under them, their start state there
+        solver.spawn_sample_dev(mask, idx, sp_rows, q, v, rbd, contact, x_obs, last_ee, rbd_est if se else None, sp["link"], s)
+
+    if sp is not None:   # every robot's first episode spawns right before the first solve (after the restore and the draw of its plant)
+        with torch.cuda.stream(stream):
+            sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev)
+            if rs is None:
+                stand(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
+            else:
+                stand(due, episode)
 
     with torch.cuda.stream(stream):
         mpc_tick(0); stream.synchronize()          # QMController::starting: one blocking solve before the loop
@@ -706,4 +796,9 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
         rb, re_ = np.nonzero(had)
         out["episode_params"] = np.full(had.shape + (_lib.EPISODE,), np.nan); out["episode_params"][rb, re_] = solver.episode_draw(rb, re_)
+    if sp is not None:   # as episode_params: the spawn rows are a pure function of (ranges, seed, robot, episode)
+        ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
+        had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
+        rb, re_ = np.nonzero(had)
+        out["spawn_params"] = np.full(had.shape + (_lib.SPAWN,), np.nan); out["spawn_params"][rb, re_] = solver.spawn_draw(rb, re_)
     return out

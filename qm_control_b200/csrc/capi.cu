@@ -21,6 +21,7 @@
 #include "kernels/gait_api.cuh"
 #include "kernels/respawn_api.cuh"
 #include "kernels/episode_api.cuh"
+#include "kernels/spawn_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -88,6 +89,11 @@ struct qmb200_handle {
   struct {   // per-episode plant draws (capi_episode.inc): the robots' ranges [B][EP_DBL] (empty: none set), their device copies (dalloc: freed with allocs) and the seed
     std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0;
   } episode;
+  bool terrain_on_device = false;   // a spawn wrote the plant's robot terrain / the ground map on the device: terrain_rows_sync refreshes them
+  struct {   // per-episode spawns (capi_spawn.inc): ranges [B][SP_DBL] (empty: none set), seed, and device copies (dalloc: freed with allocs) of the ranges,
+             // the robots' tile origins at the set [B][2] and the standing pose's joints [NJ]; terrain: the plant had robot terrain rows at the set
+    std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr, *d_origin = nullptr, *d_qj = nullptr; uint64_t seed = 0; bool terrain = false;
+  } spawn;
   uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
   struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
     bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
@@ -270,12 +276,13 @@ std::string payload_error(const double* payload, size_t n, const char* who) {
 int rows_sync(qmb200_handle* h, bool& on_device, std::initializer_list<RobotArray*> arrays) {
   if (!on_device) return 0;
   QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());
-  for (RobotArray* a : arrays) QMB_CUDA(h, cudaMemcpy(a->host.data(), a->d, a->host.size() * 8, cudaMemcpyDeviceToHost));
+  for (RobotArray* a : arrays) if (!a->host.empty()) QMB_CUDA(h, cudaMemcpy(a->host.data(), a->d, a->host.size() * 8, cudaMemcpyDeviceToHost));
   on_device = false; return 0;
 }
 int model_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->model_on_device, {&h->mpayload, &h->srbd}); }
 int plant_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->plant_on_device, {&h->mu, &h->payload}); }
 int tuning_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->tuning_on_device, {&h->tuning}); }
+int terrain_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->terrain_on_device, {&h->terrain, &h->se_ground}); }
 // SRBD constants of n robots with payload rows [n][8] (NULL: none)
 void srbd_rows(const HostModel& hm, const double* payload, size_t n, double* out) {
   for (size_t b = 0; b < n; ++b) srbd_constants(hm.dev, payload ? payload + 8 * b : nullptr, out + SRBD_DBL * b);
@@ -445,3 +452,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_gait.inc"
 #include "capi_respawn.inc"
 #include "capi_episode.inc"
+#include "capi_spawn.inc"

@@ -740,6 +740,46 @@ class Solver:
         self._call("episode_draw", len(robot), _p(robot), _p(episode), _p(rows))
         return rows
 
+    # ---------------- per-episode spawns (include/qmb200.h: qmb200_spawn_*; DESIGN.md §4.12) ----------------
+    def spawn_set_ranges(self, lo=None, hi=None, seed=0):
+        """Per-robot ranges lo, hi [B, SPAWN] (columns _lib.SPAWN_LAYOUT) and a 64-bit seed of the per-episode spawns; None clears them.  The offsets
+        count from the plant's robot terrain origins in force; with a tile bound >= 0 the robot terrain rows are made to exist.  Synchronous."""
+        if lo is None and hi is None:
+            self._call("spawn_set_ranges", None, None, 0); return
+        shape = (self.batch, _lib.SPAWN); lo = _f64(lo, shape); hi = _f64(hi, shape)
+        s = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._call("spawn_set_ranges", _p(lo), _p(hi), s - (1 << 64) if s >> 63 else s)
+
+    def spawn_get_ranges(self):
+        """→ dict(lo [B, SPAWN], hi [B, SPAWN], seed) of the stored ranges, or None when none are set."""
+        lo = np.zeros((self.batch, _lib.SPAWN)); hi = np.zeros_like(lo); seed = C.c_int64(); is_set = C.c_int32()
+        self._call("spawn_get_ranges", _p(lo), _p(hi), C.byref(seed), C.byref(is_set))
+        return dict(lo=lo, hi=hi, seed=seed.value & 0xFFFFFFFFFFFFFFFF) if is_set.value else None
+
+    def spawn_sample(self, mask, episode, q, v, rbd, contact, x_obs, last_ee, rbd_est=None, link=0, rows=None):
+        """Host variant of spawn_sample_dev on copies of the arrays → dict(rows [B, SPAWN], q, v, rbd, contact, x_obs, last_ee[, rbd_est]); unmasked
+        robots keep what was given (rows: zeros by default)."""
+        B = self.batch
+        out = dict(rows=np.zeros((B, _lib.SPAWN)) if rows is None else _f64(rows, (B, _lib.SPAWN)).copy(), q=_f64(q, (B, 24)).copy(), v=_f64(v, (B, 24)).copy(),
+                   rbd=_f64(rbd, (B, RBD)).copy(), contact=_i32(contact, (B,)).copy(), x_obs=_f64(x_obs, (B, NX)).copy(), last_ee=_f64(last_ee, (B, 7)).copy())
+        if rbd_est is not None:
+            out["rbd_est"] = _f64(rbd_est, (B, RBD)).copy()
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,)); episode = _i32(np.broadcast_to(np.asarray(episode), (B,)), (B,))
+        self._call("spawn_sample", _p(mask), _p(episode), int(link), *(_p(out[k]) for k in ("rows", "q", "v", "rbd", "contact", "x_obs", "last_ee")), _p(out.get("rbd_est")))
+        return out
+
+    def spawn_sample_dev(self, mask, episode, rows, q, v, rbd, contact, x_obs, last_ee, rbd_est=None, link=0, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) draws episode[b]'s spawn row (int32 [B]) into rows [B, SPAWN] and stands there: the
+        plant's robot terrain row (and with link _lib.SPAWN_GROUND_MAP the estimator's ground map), q, v, rbd, contact, x_obs, last_ee turned with the
+        base, rbd_est when given, and the reset rows of the running estimators (float64 / int32 device tensors).  One launch, no synchronisation."""
+        self._call("spawn_sample_dev", _p(mask), _p(episode), int(link), _p(rows), _p(q), _p(v), _p(rbd), _p(contact), _p(x_obs), _p(last_ee), _p(rbd_est), stream)
+
+    def spawn_draw(self, robot, episode):
+        """Host only: robot [n] (in [0, B)), episode [n] → the spawn rows [n, SPAWN] the sampler draws for them on the stored ranges and seed."""
+        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); rows = np.zeros((len(robot), _lib.SPAWN))
+        self._call("spawn_draw", len(robot), _p(robot), _p(episode), _p(rows))
+        return rows
+
     # ---------------- device gait schedule (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7) ----------------
     def gait_dev_set_templates(self, names=None, gait_file=None):
         """Load the template table: names (default: every template of the gait file, in the order of its list) → the names, a template's id being its

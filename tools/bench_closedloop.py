@@ -6,7 +6,7 @@ deviation from the initial pose, as percentiles over the robots) of this project
 
     python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter] [--slip-detector]]
                                      [--gait-commands] [--ee-goals]
-    python tools/bench_closedloop.py --respawn [--randomize] [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
+    python tools/bench_closedloop.py --respawn [--randomize | --spawn] [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -77,6 +77,15 @@ detector and the image restore against the plant step (CUDA events, alternated b
 with, from one 5 s run, the episodes per robot and the fraction of episodes that fall within their first second per friction bin x push-magnitude bin
 (episodes that start at least 1 s before the run's end); the wall time per simulated second of --duration runs with and without randomize (both with
 respawn), alternated in one process; and the device time per call of the sampler against the image restore (CUDA events, alternated blocks).
+
+--respawn --spawn starts every episode on new ground (closed_loop.run(spawn=...)) on a library of flat ground, a 10 deg ramp, 6 cm stairs and rough
+ground (2 cm), each flat within 0.35 m of its centre: the tile U{0..3}, dx U[-0.5, 0] m (the flat zone before the first edge, so the controller's
+absolute base-height target is met at the start), dy U[-0.2, 0.2] m and the yaw U[-pi, pi]; the estimator's ground map follows the draw.  It prints
+one JSON line "spawn" with, from one 5 s run, the fraction of episodes that fall within their first second per tile x 45 deg heading bin (episodes that
+start at least 1 s before the run's end); the same bins from a control run of 5 s without spawn, each robot's heading drawn once into xy_yaw on the
+flat tile; the wall time per simulated second of --duration runs without spawn, with spawn ranges fixed at the run's values and with the draws (all
+with respawn on the library), alternated in one process; and the device time per call of the spawn sampler against the plant step (CUDA events,
+alternated blocks).
 """
 import argparse
 import json
@@ -557,6 +566,106 @@ def randomize_main(args, solver, kw, xy, timed, episode_run_s=5.0):
                       "per_call": episode_times(solver, xy)}))
 
 
+SPAWN_TILES = ("flat", "ramp_10deg", "stairs_6cm", "rough_2cm")
+SPAWN = dict(seed=0, tile=(0, 3), dx=(-0.5, 0.0), dy=(-0.2, 0.2), yaw=(-np.pi, np.pi))
+
+
+def spawn_terrain(xy):
+    """the --spawn library and every robot's run row: tile 0 (flat) centred under its start"""
+    from qm_control_b200 import terrain as T
+    tiles = np.stack([T.flat(), T.ramp(10.0, start=0.35), T.stairs(0.06, 0.25, start=0.35), T.rough(0.02, seed=1, flat_radius=0.35)])
+    return dict(tiles=tiles, cell=T.CELL, tile=np.zeros(len(xy), dtype=np.int32), origin=T.centred_origin(xy[:, :2]))
+
+
+def spawn_times(solver, ter, xy_yaw, reps=7, calls=20):
+    """Device time per spawn call (every robot masked, and none) on SPAWN's ranges with the state estimator, attitude filter and slip detector running
+    and the ground-map link, against the plant step on the same library, alternated `reps` times in blocks of `calls` (CUDA events) → median ms per call"""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    solver.sim_set_terrain(ter["tiles"], ter["cell"]); solver.sim_set_robot_terrain(ter["tile"], ter["origin"]); solver.state_est_set_ground(ter["tile"], ter["origin"])
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    solver.state_est_reset(q0[:, 0:3]); solver.attitude_reset(); solver.slip_reset()
+    lo = np.zeros((B, _lib.SPAWN)); hi = np.zeros((B, _lib.SPAWN))
+    for i, k in enumerate(_lib.SPAWN_LAYOUT):
+        lo[:, i], hi[:, i] = SPAWN[k]
+    solver.spawn_set_ranges(lo, hi, 0)
+    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+    q0t = f64(q0); q = q0t.clone(); v = f64(v0); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev); x_obs = torch.zeros((B, 30), dtype=torch.float64, device=dev)
+    last_ee = f64(solver.initial_ee_target()); rbd_est = torch.zeros_like(rbd); rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact); eff = torch.zeros((B, 18), dtype=torch.float64, device=dev)
+    every = torch.ones(B, dtype=torch.int32, device=dev); none = torch.zeros_like(every); ep = torch.arange(B, dtype=torch.int32, device=dev)
+    spawn = lambda m: solver.spawn_sample_dev(m, ep, rows, q, v, rbd, contact, x_obs, last_ee, rbd_est, _lib.SPAWN_GROUND_MAP, s.cuda_stream)
+    calls_of = {"spawn_all": lambda: spawn(every), "spawn_none": lambda: spawn(none),
+                "plant_step": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                q.copy_(q0t); v.zero_(); torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    call()
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.spawn_set_ranges(None); solver.state_est_set_ground(None); solver.sim_set_robot_terrain(None); solver.sim_set_terrain(None)
+        solver.slip_stop(); solver.attitude_stop(); solver.state_est_stop()
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls; estimator, attitude filter, slip detector and ground-map "
+                     "link on, plant step on the same library" % (B, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}, "spread_spawn_all": [float(min(times["spawn_all"])), float(max(times["spawn_all"]))]}
+
+
+def spawn_falls(r, ep_s=1.0, P=None):
+    """Per tile x 45 deg heading bin of a closed_loop.run(respawn=..., spawn=SPAWN) result: the episodes that start at least ep_s before the run's end and
+    how many of them fall within their first ep_s seconds.  P [B, E, 4]: the spawn rows to bin by (default the run's spawn_params)"""
+    ep, fl = r["episode"], r["fallen"].astype(bool); P = r["spawn_params"] if P is None else P; ticks, B = ep.shape; w = int(round(ep_s * 100))
+    edges = np.linspace(-np.pi, np.pi, 9)
+    fell = np.zeros((len(SPAWN_TILES), 8), dtype=int); n = np.zeros_like(fell)
+    for b in range(B):
+        for e in range(int(ep[-1, b]) + 1):
+            rows = np.flatnonzero(ep[:, b] == e)
+            if rows[0] + w > ticks:
+                continue
+            i = int(P[b, e, 0]); j = min(np.searchsorted(edges, P[b, e, 3], side="right") - 1, 7)
+            n[i, j] += 1; fell[i, j] += int(fl[rows[:w], b].any())
+    return {"tiles": list(SPAWN_TILES), "heading_bins_deg": np.degrees(edges).round(1).tolist(), "episodes": n.tolist(), "fell": fell.tolist(),
+            "fraction": np.where(n > 0, fell / np.maximum(n, 1), np.nan).round(4).tolist(), "total_episodes": int(n.sum()), "total_fell": int(fell.sum())}
+
+
+def spawn_main(args, solver, kw, xy, timed, episode_run_s=5.0):
+    """--respawn --spawn: the same loop on the --spawn library with SPAWN drawn per episode.  One run of episode_run_s for the falls per bin; the wall
+    time per simulated second of --duration runs with and without spawns (both with respawn and the library), alternated twice after one warm-up run
+    of each; the spawn call's per-call device time against the plant step."""
+    ter = spawn_terrain(xy); kw.update(terrain=ter, ground_map=True)
+    arms = {"without_spawn": None, "spawn_fixed_at_the_runs_values": dict(seed=0), "with_spawn": SPAWN}
+    wall = {k: [] for k in arms}
+    for rep in range(3):   # the first round warms up
+        for name, sp in arms.items():
+            _, w = timed(True, args.duration, spawn=sp)
+            if rep:
+                wall[name].append(w)
+    r, _ = timed(True, episode_run_s, spawn=SPAWN)
+    # the control: no spawn, each robot's heading built by hand into xy_yaw (drawn once, kept by every respawn), on the flat tile
+    yaw = np.random.default_rng(0).uniform(-np.pi, np.pi, solver.batch); kw_xy = kw["xy_yaw"]; kw["xy_yaw"] = np.c_[xy[:, :2], yaw]
+    try:
+        rc, _ = timed(True, episode_run_s)
+    finally:
+        kw["xy_yaw"] = kw_xy
+    E = int(rc["episode"].max()) + 1; Pc = np.zeros((solver.batch, E, _lib.SPAWN)); Pc[:, :, 3] = yaw[:, None]
+    name, limit = card()
+    print(json.dumps({"metric": "spawn", "gpu": name, "power_limit": limit, "batch": solver.batch,
+                      "config": "%s at %.2f m/s on the state estimate with the ground map, reference IMU noise, no attitude filter; respawn after 0.1 s fallen; "
+                                "per episode: tile U{flat, 10 deg ramp, 6 cm stairs, 2 cm rough}, dx U[-0.5, 0] m, dy U[-0.2, 0.2] m, yaw U[-pi, pi]" % (args.gait, args.vx),
+                      "simulated_s": episode_run_s, "episodes_per_robot": float(np.mean(r["episode"][-1] + 1)),
+                      "fell_within_1s": spawn_falls(r),
+                      "control_fell_within_1s": {"label": "no spawn: the same run on the flat tile with each robot's heading drawn once into xy_yaw",
+                                                 "episodes_per_robot": float(np.mean(rc["episode"][-1] + 1)), **spawn_falls(rc, P=Pc)},
+                      "wall_s_per_sim_s": {"label": "runs of %.1f s with respawn on the library, the three arms alternated twice after a warm-up round; the fixed "
+                                                    "arm runs the spawn path at the run's own values (flat tile, yaw 0)" % args.duration, **wall},
+                      "per_call": spawn_times(solver, ter, xy)}))
+
+
 def respawn_main(args, episode_run_s=5.0):
     """--respawn: trot at --vx on the estimate from the reference IMU noise without the attitude filter, robots restarted after 0.1 s fallen.  One
     run of episode_run_s for the rates; the wall time per simulated second of --duration runs with and without respawn, alternated twice after one
@@ -571,13 +680,16 @@ def respawn_main(args, episode_run_s=5.0):
     xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
     kw = dict(gait=args.gait, cmd_vel=cmd, xy_yaw=xy, state_estimator=True, sensor_noise="reference")
 
-    def timed(respawn, duration, randomize=None):
+    def timed(respawn, duration, randomize=None, spawn=None):
         solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
-        r = closed_loop.run(solver, duration=duration, **kw, **({"respawn": dict(hold=0.1)} if respawn else {}), **({"randomize": randomize} if randomize else {}))
+        r = closed_loop.run(solver, duration=duration, **kw, **({"respawn": dict(hold=0.1)} if respawn else {}), **({"randomize": randomize} if randomize else {}),
+                            **({"spawn": spawn} if spawn else {}))
         torch.cuda.synchronize(dev)
         return r, (time.perf_counter() - t0) / duration
     if args.randomize:
         return randomize_main(args, solver, kw, xy, timed)
+    if args.spawn:
+        return spawn_main(args, solver, kw, xy, timed)
     wall = {False: [], True: []}
     for rep in range(3):   # the first round warms up
         for respawn in (False, True):
@@ -635,9 +747,12 @@ def main():
     ap.add_argument("--ee-tuning", action="store_true", help="with --ee-goals: the reach sweep again with per-robot end-effector weights, WBC end-effector gains and kd_arm_wbc")
     ap.add_argument("--respawn", action="store_true", help="restart robots that fell (hold 0.1 s) on the reference IMU noise without the attitude filter: episode rates")
     ap.add_argument("--randomize", action="store_true", help="with --respawn: a new plant per episode (friction, payload, push): falls per friction x push bin")
+    ap.add_argument("--spawn", action="store_true", help="with --respawn: new ground per episode (tile, offset, yaw): falls per tile x heading bin")
     args = ap.parse_args()
     if args.randomize and not args.respawn:
         ap.error("--randomize needs --respawn")
+    if args.spawn and not args.respawn:
+        ap.error("--spawn needs --respawn")
     if args.respawn:
         return respawn_main(args)
     if args.ee_tuning and not args.ee_goals:

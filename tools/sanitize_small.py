@@ -1,4 +1,6 @@
-"""Tiny end-to-end run for compute-sanitizer (memcheck / racecheck / initcheck): every kernel of the library once, 5 robots (mixed gaits)."""
+"""Tiny end-to-end run for compute-sanitizer (memcheck / racecheck / initcheck): every kernel of the library once, 5 robots (mixed gaits); then the
+per-episode spawn sampler inside a few respawned windows of closed_loop.run on terrain, with the ground-map link and the estimator, attitude filter and
+slip detector rows live."""
 import os
 import sys
 
@@ -25,4 +27,10 @@ for name in ("ipm", "ddp", "sqp"):
 dev = torch.device("cuda", 0); cmd_d = torch.from_numpy(cmd).to(dev); all_d = torch.zeros((B, 18), dtype=torch.float64, device=dev)
 perm = s.gait_bin_permutation(prob); s.allgather_torque(cmd_d, all_d, torch.from_numpy(perm).to(dev)); torch.cuda.synchronize()
 s1 = q.Solver(batch=B, dt=0.015, wbc_variant=1); c1, st1 = s1.tick(prob, prob["t0"] + 0.002, wbc["rbd"], wbc["period"])
-print("sanitize_small ok", status, status2, out["status"], st1)
+# per-episode spawns (DESIGN.md §4.12): 50 ms with a respawn every 20 ms, so the sampler runs at the start and at two window boundaries
+from qm_control_b200 import closed_loop, terrain as T  # noqa: E402
+s2 = q.Solver(batch=B); xy = np.c_[3.0 * np.arange(B), np.zeros(B), np.zeros(B)]
+ter = dict(tiles=np.stack([T.flat(), T.stairs(0.06, 0.25)]), cell=T.CELL, tile=np.arange(B) % 3 - 1, origin=T.centred_origin(xy[:, :2]))
+r = closed_loop.run(s2, duration=0.05, gait="trot", xy_yaw=xy, terrain=ter, state_estimator=True, attitude_filter=True, slip_detector=True, ground_map=True,
+                    respawn=dict(on_fall=False, every=0.02), spawn=dict(seed=1, tile=(-1, 1), dx=(-0.2, 0.0), dy=(-0.1, 0.1), yaw=(-np.pi, np.pi)))
+print("sanitize_small ok", status, status2, out["status"], st1, "spawn episodes", r["episode"][-1], "rows", r["spawn_params"].shape)
