@@ -181,7 +181,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
         if sp is not None:   # restored last: the earlier ranges are set again on the earlier library and robot terrain rows, which give their origins
-            scope.enter_context(_spawn_ranges(solver))
+            scope.enter_context(_ranges(solver, "spawn"))
         if terrain is not None:
             scope.enter_context(_terrain(solver, terrain))
         if ground_map is not None:
@@ -201,7 +201,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         if friction_mu is not None or payload is not None or rz is not None:
             scope.enter_context(_robot_params(solver, friction_mu, payload))
         if rz is not None:
-            scope.enter_context(_episode_ranges(solver))
+            scope.enter_context(_ranges(solver, "episode"))
         if gd is not None:
             scope.enter_context(_gait_dev(solver, gd))
         if rs is not None:
@@ -241,37 +241,45 @@ def _respawn_spec(respawn):
     return dict(on_fall=bool(spec["on_fall"]), hold_windows=hold // MPC_PERIOD_MS, z_min=float(spec["z_min"]), tilt_max=float(spec["tilt_max"]), every_ms=every)
 
 
-def _randomize_spec(B, randomize):
-    """closed_loop.run's randomize → dict(seed, fields: name -> (lo, hi) float arrays, scalar or [B], link=0); ValueError when malformed.  B None: the
-    bounds' length is not checked."""
-    if not isinstance(randomize, dict):
-        raise ValueError("closed_loop.run: randomize must be None or dict(seed=..., <field>=(lo, hi), ...), got %r" % (randomize,))
-    seed = randomize.get("seed", 0)
+def _ranges_spec(kind, layout, B, value):
+    """closed_loop.run's randomize or spawn dict (kind names it) → (seed, fields: name -> (lo, hi) float arrays, scalar or [B]) for the columns of
+    layout; ValueError when the seed or a field is malformed.  B None: the bounds' length is not checked."""
+    seed = value.get("seed", 0)
     if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
-        raise ValueError("closed_loop.run: randomize seed must be an integer in [0, 2^64), got %r" % (seed,))
+        raise ValueError("closed_loop.run: %s seed must be an integer in [0, 2^64), got %r" % (kind, seed))
     fields = {}
-    for k, v in randomize.items():
+    for k, v in value.items():
         if k == "seed":
             continue
-        if k not in _lib.EPISODE_LAYOUT:
-            raise ValueError("closed_loop.run: unknown randomize field %r (one of seed, %s)" % (k, ", ".join(_lib.EPISODE_LAYOUT)))
+        if k not in layout:
+            raise ValueError("closed_loop.run: unknown %s field %r (one of seed, %s)" % (kind, k, ", ".join(layout)))
         try:
             if isinstance(v, str) or len(v) != 2 or any(isinstance(a, str) for a in v):
                 raise TypeError
             lo, hi = (np.asarray(a, dtype=np.float64) for a in v)
         except (TypeError, ValueError):
-            raise ValueError("closed_loop.run: randomize %s must be a pair (lo, hi) of numbers or [B] arrays, got %r" % (k, v)) from None
+            raise ValueError("closed_loop.run: %s %s must be a pair (lo, hi) of numbers or [B] arrays, got %r" % (kind, k, v)) from None
         if any(a.ndim > 1 or (a.ndim == 1 and B is not None and a.shape != (B,)) for a in (lo, hi)) or (lo.ndim == hi.ndim == 1 and lo.shape != hi.shape):
-            raise ValueError("closed_loop.run: randomize %s bounds must be scalars or [%s], got shapes %s and %s" % (k, "B" if B is None else B, lo.shape, hi.shape))
+            raise ValueError("closed_loop.run: %s %s bounds must be scalars or [%s], got shapes %s and %s" % (kind, k, "B" if B is None else B, lo.shape, hi.shape))
         with np.errstate(invalid="ignore", over="ignore"):
             if not (np.all(np.isfinite(lo)) and np.all(np.isfinite(hi)) and np.all(lo <= hi) and np.all(np.isfinite(hi - lo))):
-                raise ValueError("closed_loop.run: randomize %s bounds must be finite with lo <= hi, got %r" % (k, v))
+                raise ValueError("closed_loop.run: %s %s bounds must be finite with lo <= hi, got %r" % (kind, k, v))
+        fields[k] = (lo, hi)
+    return int(seed), fields
+
+
+def _randomize_spec(B, randomize):
+    """closed_loop.run's randomize → dict(seed, fields: name -> (lo, hi) float arrays, scalar or [B], link=0); ValueError when malformed.  B None: the
+    bounds' length is not checked."""
+    if not isinstance(randomize, dict):
+        raise ValueError("closed_loop.run: randomize must be None or dict(seed=..., <field>=(lo, hi), ...), got %r" % (randomize,))
+    seed, fields = _ranges_spec("randomize", _lib.EPISODE_LAYOUT, B, randomize)
+    for k, (lo, hi) in fields.items():
         if k == "friction_mu" and not np.all(lo > 0.0):
             raise ValueError("closed_loop.run: randomize friction_mu lo must be > 0")
         if k in ("m_ee", "m_base", "push_t_on", "push_duration") and not np.all(lo >= 0.0):
             raise ValueError("closed_loop.run: randomize %s lo must be >= 0" % k)
-        fields[k] = (lo, hi)
-    return dict(seed=int(seed), fields=fields, link=0)
+    return dict(seed=seed, fields=fields, link=0)
 
 
 def _spawn_spec(B, spawn, terrain, ground_map, gd):
@@ -279,29 +287,9 @@ def _spawn_spec(B, spawn, terrain, ground_map, gd):
     link); ValueError when malformed.  B None: the bounds' length is not checked."""
     if not isinstance(spawn, dict):
         raise ValueError("closed_loop.run: spawn must be None or dict(seed=..., tile=(lo, hi), dx=(lo, hi), dy=(lo, hi), yaw=(lo, hi)), got %r" % (spawn,))
-    seed = spawn.get("seed", 0)
-    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 1 << 64:
-        raise ValueError("closed_loop.run: spawn seed must be an integer in [0, 2^64), got %r" % (seed,))
-    fields = {}
-    for k, v in spawn.items():
-        if k == "seed":
-            continue
-        if k not in _lib.SPAWN_LAYOUT:
-            raise ValueError("closed_loop.run: unknown spawn field %r (one of seed, %s)" % (k, ", ".join(_lib.SPAWN_LAYOUT)))
-        try:
-            if isinstance(v, str) or len(v) != 2 or any(isinstance(a, str) for a in v):
-                raise TypeError
-            lo, hi = (np.asarray(a, dtype=np.float64) for a in v)
-        except (TypeError, ValueError):
-            raise ValueError("closed_loop.run: spawn %s must be a pair (lo, hi) of numbers or [B] arrays, got %r" % (k, v)) from None
-        if any(a.ndim > 1 or (a.ndim == 1 and B is not None and a.shape != (B,)) for a in (lo, hi)) or (lo.ndim == hi.ndim == 1 and lo.shape != hi.shape):
-            raise ValueError("closed_loop.run: spawn %s bounds must be scalars or [%s], got shapes %s and %s" % (k, "B" if B is None else B, lo.shape, hi.shape))
-        with np.errstate(invalid="ignore", over="ignore"):
-            if not (np.all(np.isfinite(lo)) and np.all(np.isfinite(hi)) and np.all(lo <= hi) and np.all(np.isfinite(hi - lo))):
-                raise ValueError("closed_loop.run: spawn %s bounds must be finite with lo <= hi, got %r" % (k, v))
-        if k == "yaw" and not (np.all(lo >= -np.pi) and np.all(hi <= np.pi)):
-            raise ValueError("closed_loop.run: spawn yaw bounds must lie in [-pi, pi]")
-        fields[k] = (lo, hi)
+    seed, fields = _ranges_spec("spawn", _lib.SPAWN_LAYOUT, B, spawn)
+    if "yaw" in fields and not (np.all(fields["yaw"][0] >= -np.pi) and np.all(fields["yaw"][1] <= np.pi)):
+        raise ValueError("closed_loop.run: spawn yaw bounds must lie in [-pi, pi]")
     ground = set(fields) & {"tile", "dx", "dy"}
     if ground and terrain is None:
         raise ValueError("closed_loop.run: spawn %s needs terrain (it moves the plant's tile under the robot)" % ", ".join(sorted(ground)))
@@ -314,31 +302,31 @@ def _spawn_spec(B, spawn, terrain, ground_map, gd):
                          % ", ".join(sorted(ground)))
     if "yaw" in fields and gd is not None and gd["ee"] and np.any(fields["yaw"][0] != fields["yaw"][1]):
         raise ValueError("closed_loop.run: a drawn spawn yaw cannot go with ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)")
-    return dict(seed=int(seed), fields=fields, link=_lib.SPAWN_GROUND_MAP if ground_map is True else 0)
+    return dict(seed=seed, fields=fields, link=_lib.SPAWN_GROUND_MAP if ground_map is True else 0)
 
 
 @contextlib.contextmanager
-def _spawn_ranges(solver):
-    prev = solver.spawn_get_ranges()
+def _ranges(solver, kind):
+    """the ranges of solver's kind ("episode" or "spawn") draws in force, set again on exit"""
+    prev = getattr(solver, kind + "_get_ranges")()
     try:
         yield   # _run sets this run's ranges once it has read its fixed values
     finally:
         if prev is None:
-            solver.spawn_set_ranges(None)
+            getattr(solver, kind + "_set_ranges")(None)
         else:
-            solver.spawn_set_ranges(**prev)
+            getattr(solver, kind + "_set_ranges")(**prev)
 
 
-@contextlib.contextmanager
-def _episode_ranges(solver):
-    prev = solver.episode_get_ranges()
-    try:
-        yield   # _run sets this run's ranges once it has read its fixed values
-    finally:
-        if prev is None:
-            solver.episode_set_ranges(None)
-        else:
-            solver.episode_set_ranges(**prev)
+def _set_ranges(solver, kind, layout, row, spec):
+    """sets the run's ranges of solver's kind draws: every column fixed at the run's value, row [B, C], except the spec's fields, drawn within their
+    bounds → hi [B, C]"""
+    col = {n: i for i, n in enumerate(layout)}
+    lo = row.copy(); hi = row.copy()
+    for k, (l, h) in spec["fields"].items():
+        lo[:, col[k]] = l; hi[:, col[k]] = h
+    getattr(solver, kind + "_set_ranges")(lo, hi, spec["seed"])
+    return hi
 
 
 def _gait_commands(B, gait, commands):
@@ -560,17 +548,14 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     if rz is not None:   # the ranges: this run's values (entered after _robot_params: the handle's robot params are this run's plant), the named fields' bounds
         EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}
         rp = solver.sim_get_robot_params()
-        lo = np.zeros((B, _lib.EPISODE))
-        lo[:, EP["friction_mu"]] = solver.sim_get_params()["friction_mu"] if rp["friction_mu"] is None else rp["friction_mu"]
+        row = np.zeros((B, _lib.EPISODE))
+        row[:, EP["friction_mu"]] = solver.sim_get_params()["friction_mu"] if rp["friction_mu"] is None else rp["friction_mu"]
         if rp["payload"] is not None:
-            lo[:, EP["m_ee"]:EP["m_ee"] + 8] = rp["payload"]
+            row[:, EP["m_ee"]:EP["m_ee"] + 8] = rp["payload"]
         if pushes is not None:
-            lo[:, EP["push_t_on"]] = t_on; lo[:, EP["push_duration"]] = t_dur; lo[:, EP["f_base_x"]:EP["f_base_x"] + 12] = wrench
-        lo[:, EP["cmd_vel_x"]:EP["cmd_vel_x"] + 4] = cmd_vel
-        hi = lo.copy()
-        for k, (l, h) in rz["fields"].items():
-            lo[:, EP[k]] = l; hi[:, EP[k]] = h
-        solver.episode_set_ranges(lo, hi, rz["seed"])
+            row[:, EP["push_t_on"]] = t_on; row[:, EP["push_duration"]] = t_dur; row[:, EP["f_base_x"]:EP["f_base_x"] + 12] = wrench
+        row[:, EP["cmd_vel_x"]:EP["cmd_vel_x"] + 4] = cmd_vel
+        hi = _set_ranges(solver, "episode", _lib.EPISODE_LAYOUT, row, rz)
         if pushes is None and np.any(hi[:, EP["push_duration"]] > 0.0):   # the draws overwrite these rows before the first solve
             t_on, t_dur, wrench = np.zeros(B), np.zeros(B), np.zeros((B, 12)); pushes = (t_on, t_dur, wrench)
     xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
@@ -578,11 +563,8 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         SP = {n: i for i, n in enumerate(_lib.SPAWN_LAYOUT)}
         rt = solver.sim_get_robot_terrain()
         yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)   # the same heading within [-pi, pi]
-        lo = np.zeros((B, _lib.SPAWN)); lo[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; lo[:, SP["yaw"]] = yaw
-        hi = lo.copy()
-        for k, (l, h) in sp["fields"].items():
-            lo[:, SP[k]] = l; hi[:, SP[k]] = h
-        solver.spawn_set_ranges(lo, hi, sp["seed"])
+        row = np.zeros((B, _lib.SPAWN)); row[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; row[:, SP["yaw"]] = yaw
+        _set_ranges(solver, "spawn", _lib.SPAWN_LAYOUT, row, sp)
     stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
     f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
     i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
@@ -689,10 +671,13 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         for a, a0 in zip(own, start):
             a.copy_(torch.where(m.view((B,) + (1,) * (a.dim() - 1)), a0, a))
         k0.copy_(torch.where(m, k, k0)); episode.add_(due); fall_count.masked_fill_(m, 0)
+        begin(due, episode)
+
+    def begin(mask, idx):   # the masked robots begin episode idx: their plant's draw, then their spawn
         if rz is not None:
-            draw(due, episode)
+            draw(mask, idx)
         if sp is not None:
-            stand(due, episode)
+            stand(mask, idx)
 
     def draw(mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
         solver.episode_sample_dev(mask, idx, ep_rows, rz["link"], s)
@@ -703,24 +688,17 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             push["on"].copy_(torch.where(m, on, push["on"])); push["off"].copy_(torch.where(m, off, push["off"]))
             push["wrench"].copy_(torch.where(m[:, None], ep_rows[:, 11:23], push["wrench"]))
 
-    if rz is not None:   # every robot's first episode draws its row right before the first solve (after the restore of the start image)
-        with torch.cuda.stream(stream):
-            ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev)
-            if rs is None:
-                draw(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
-            else:
-                draw(due, episode)
-
     def stand(mask, idx):   # the masked robots spawn episode idx: new ground under them, their start state there
         solver.spawn_sample_dev(mask, idx, sp_rows, q, v, rbd, contact, x_obs, last_ee, rbd_est if se else None, sp["link"], s)
 
-    if sp is not None:   # every robot's first episode spawns right before the first solve (after the restore and the draw of its plant)
+    if rz is not None or sp is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
         with torch.cuda.stream(stream):
-            sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev)
+            ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev) if rz is not None else None
+            sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev) if sp is not None else None
             if rs is None:
-                stand(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
+                begin(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
             else:
-                stand(due, episode)
+                begin(due, episode)
 
     with torch.cuda.stream(stream):
         mpc_tick(0); stream.synchronize()          # QMController::starting: one blocking solve before the loop
@@ -791,14 +769,11 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                    ee_target=rec_ee_target.cpu().numpy())
     if rs is not None:
         out.update(episode=rec_episode.cpu().numpy(), fallen=rec_fallen.cpu().numpy())
-    if rz is not None:   # rebuilt on the host from the episode record: the sampler's rows are a pure function of (ranges, seed, robot, episode)
+    if rz is not None or sp is not None:   # rebuilt on the host from the episode record: the samplers' rows are pure functions of (ranges, seed, robot, episode)
         ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
         had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
         rb, re_ = np.nonzero(had)
-        out["episode_params"] = np.full(had.shape + (_lib.EPISODE,), np.nan); out["episode_params"][rb, re_] = solver.episode_draw(rb, re_)
-    if sp is not None:   # as episode_params: the spawn rows are a pure function of (ranges, seed, robot, episode)
-        ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
-        had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
-        rb, re_ = np.nonzero(had)
-        out["spawn_params"] = np.full(had.shape + (_lib.SPAWN,), np.nan); out["spawn_params"][rb, re_] = solver.spawn_draw(rb, re_)
+        for kind, spec, width in (("episode", rz, _lib.EPISODE), ("spawn", sp, _lib.SPAWN)):
+            if spec is not None:
+                out[kind + "_params"] = np.full(had.shape + (width,), np.nan); out[kind + "_params"][rb, re_] = getattr(solver, kind + "_draw")(rb, re_)
     return out

@@ -42,6 +42,12 @@ struct RobotArray {
   const double* dev() const { return host.empty() ? nullptr : d; }
 };
 
+// Per-robot ranges of a per-episode draw (capi_episode.inc, capi_spawn.inc): lo, hi [B][width] (empty: none set), their device copies (dalloc: freed
+// with allocs) and the seed
+struct DrawRanges {
+  int width; std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0;
+};
+
 // The components a start image covers (capi_respawn.inc).  Each has a generation that its reset, stop and re-allocation bump, so a restore can tell
 // that the rows it would write no longer belong to the state it imaged.
 enum ImageComponent { IMG_STATE_EST, IMG_ATTITUDE, IMG_SLIP, IMG_PAYLOAD_EST, IMG_MODEL_PAYLOAD, IMG_GAIT, IMG_N };
@@ -86,14 +92,12 @@ struct qmb200_handle {
   } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   bool plant_on_device = false, tuning_on_device = false;   // an episode draw wrote mu / payload or tuning on the device: plant_ / tuning_rows_sync refresh them
-  struct {   // per-episode plant draws (capi_episode.inc): the robots' ranges [B][EP_DBL] (empty: none set), their device copies (dalloc: freed with allocs) and the seed
-    std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0;
-  } episode;
+  DrawRanges episode{EP_DBL};       // per-episode plant draws (capi_episode.inc)
   bool terrain_on_device = false;   // a spawn wrote the plant's robot terrain / the ground map on the device: terrain_rows_sync refreshes them
-  struct {   // per-episode spawns (capi_spawn.inc): ranges [B][SP_DBL] (empty: none set), seed, and device copies (dalloc: freed with allocs) of the ranges,
-             // the robots' tile origins at the set [B][2] and the standing pose's joints [NJ]; terrain: the plant had robot terrain rows at the set
-    std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr, *d_origin = nullptr, *d_qj = nullptr; uint64_t seed = 0; bool terrain = false;
-  } spawn;
+  struct SpawnRanges : DrawRanges {   // per-episode spawns (capi_spawn.inc), and device copies of the robots' tile origins at the set [B][2] and the
+                                      // standing pose's joints [NJ]; terrain: the plant had robot terrain rows at the set
+    double *d_origin = nullptr, *d_qj = nullptr; bool terrain = false;
+  } spawn{{SP_DBL}};
   uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
   struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
     bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
@@ -283,6 +287,52 @@ int model_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb
 int plant_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->plant_on_device, {&h->mu, &h->payload}); }
 int tuning_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->tuning_on_device, {&h->tuning}); }
 int terrain_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->terrain_on_device, {&h->terrain, &h->se_ground}); }
+// The ranged draws' set / get / draw path (qmb200_<kind>_set_ranges, _get_ranges, _draw; kind: "episode" or "spawn").
+// Set: NULL lo and hi clear the ranges once no queued draw reads them; else error() checks them ("" when valid), the device copies are allocated, then
+// prepare() makes sure the rows the sampler writes exist (it may fail, leaving the ranges as they were), and the ranges are copied and stored.
+template <class Error, class Prepare>
+int ranges_set(qmb200_handle* h, DrawRanges& r, const char* kind, const double* lo, const double* hi, int64_t seed, Error error, Prepare prepare) {
+  const std::string who = std::string("qmb200_") + kind + "_set_ranges"; const size_t n = (size_t)h->B * r.width;
+  if (!lo != !hi) return fail(h, who + ": lo and hi must both be set or both be NULL");
+  if (!lo) {
+    QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());   // no queued draw still reads the ranges
+    r.lo.clear(); r.hi.clear(); r.seed = 0; return 0;
+  }
+  if (const std::string e = error(); !e.empty()) return fail(h, e);
+  QMB_CUDA(h, cudaSetDevice(h->device));
+  if (!r.d_lo && !dalloc(h, &r.d_lo, n)) return -4;
+  if (!r.d_hi && !dalloc(h, &r.d_hi, n)) return -4;
+  if (int rc = prepare()) return rc;
+  QMB_CUDA(h, cudaDeviceSynchronize());   // no queued draw still reads the ranges
+  QMB_CUDA(h, cudaMemcpy(r.d_lo, lo, n * 8, cudaMemcpyHostToDevice)); QMB_CUDA(h, cudaMemcpy(r.d_hi, hi, n * 8, cudaMemcpyHostToDevice));
+  r.lo.assign(lo, lo + n); r.hi.assign(hi, hi + n); r.seed = (uint64_t)seed;
+  return 0;
+}
+int ranges_get(const qmb200_handle* h, const DrawRanges& r, double* lo, double* hi, int64_t* seed, int32_t* is_set) {
+  const size_t n = (size_t)h->B * r.width; const bool set = !r.lo.empty();
+  if (lo) { if (set) std::memcpy(lo, r.lo.data(), n * 8); else std::memset(lo, 0, n * 8); }
+  if (hi) { if (set) std::memcpy(hi, r.hi.data(), n * 8); else std::memset(hi, 0, n * 8); }
+  if (seed) *seed = (int64_t)r.seed;
+  if (is_set) *is_set = set ? 1 : 0;
+  return 0;
+}
+int no_ranges(qmb200_handle* h, const char* who, const char* kind) {
+  return fail(h, std::string(who) + ": no ranges are set (qmb200_" + kind + "_set_ranges sets them)");
+}
+// The rows [n][width] robots robot [n] draw in episodes episode [n] on the stored ranges, each row(lo, hi, seed, global robot, episode, out) on the host
+int ranges_draw(qmb200_handle* h, const DrawRanges& r, const char* kind, int32_t n, const int32_t* robot, const int32_t* episode, double* rows,
+                void (*row)(const double*, const double*, uint64_t, uint64_t, uint64_t, double*)) {
+  const std::string who = std::string("qmb200_") + kind + "_draw";
+  if (n < 0 || (n > 0 && (!robot || !episode || !rows))) return fail(h, who + ": n must be >= 0 and the buffers non-null");
+  if (r.lo.empty()) return no_ranges(h, who.c_str(), kind);
+  for (int32_t i = 0; i < n; ++i) if (robot[i] < 0 || robot[i] >= h->B) return fail(h, who + ": robot must be in [0, B)");
+  const int64_t robot0 = (int64_t)h->comm_rank * h->B;
+  for (int32_t i = 0; i < n; ++i) {
+    const size_t b = (size_t)robot[i];
+    row(r.lo.data() + b * r.width, r.hi.data() + b * r.width, r.seed, (uint64_t)(robot0 + robot[i]), (uint64_t)(int64_t)episode[i], rows + (size_t)i * r.width);
+  }
+  return 0;
+}
 // SRBD constants of n robots with payload rows [n][8] (NULL: none)
 void srbd_rows(const HostModel& hm, const double* payload, size_t n, double* out) {
   for (size_t b = 0; b < n; ++b) srbd_constants(hm.dev, payload ? payload + 8 * b : nullptr, out + SRBD_DBL * b);

@@ -7,6 +7,9 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <cmath>
+#include <string>
+
 // Scalar helpers are host + device: tests/nodeeval_host.cpp compiles the one-thread-per-node evaluator (node_eval.cuh) with g++ and checks it against the
 // oracle on the CPU.  Everything that needs warp intrinsics stays inside #ifdef __CUDACC__.
 #ifdef __CUDACC__
@@ -305,9 +308,33 @@ QMB_HD void srbd_payload_fold(const DevModel& d, const double* pl, double* out) 
 }
 
 // splitmix64's finaliser: a bijection of 64-bit words whose output bits each depend on every input bit.  The counter-based draws hash their keys with
-// it: the sensor noise (state_est_api.cuh) and the per-episode plant rows (episode_api.cuh).
+// it: the sensor noise (state_est_api.cuh), the per-episode plant rows (episode_api.cuh) and spawns (spawn_api.cuh).
 QMB_HD uint64_t mix64(uint64_t z) {
   z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull; z = (z ^ (z >> 27)) * 0x94d049bb133111ebull; return z ^ (z >> 31);
+}
+// The key of one counter-based draw: (seed ^ domain, robot, index, column) hashed in turn.  Each consumer xors its own domain constant into the seed, so
+// that its draws and another's of the same words are unrelated.  No generator state, so a draw does not depend on the batch or the launch.
+QMB_HD uint64_t keyed_hash(uint64_t seed, uint64_t domain, uint64_t robot, uint64_t index, int column) {
+  return mix64(mix64(mix64(mix64(seed ^ domain) ^ robot) ^ index) ^ (uint64_t)column);
+}
+// u in (0, 1) of a key h: the 53 high bits of one more hash, plus a half
+QMB_HD double hash_uniform(uint64_t h) { return ((double)(mix64(h) >> 11) + 0.5) * 1.1102230246251565e-16; }
+QMB_HD double keyed_uniform(uint64_t seed, uint64_t domain, uint64_t robot, uint64_t index, int column) {
+  return hash_uniform(keyed_hash(seed, domain, robot, index, column));
+}
+
+// The check of a per-episode draw's ranges lo, hi [B][width] (qmb200_episode_set_ranges, qmb200_spawn_set_ranges; who names the entry point): "" when
+// valid, else the first offence naming the field and the robot.  Every column needs finite bounds, lo <= hi and a finite hi - lo; extra(c, lo, hi)
+// returns column c's own offence, or "".
+template <class Extra>
+std::string ranges_error(const char* who, const char* const* names, int width, const double* lo, const double* hi, size_t B, Extra extra) {
+  for (size_t b = 0; b < B; ++b) for (int c = 0; c < width; ++c) {
+    const double l = lo[b * width + c], u = hi[b * width + c];
+    const std::string why = !(std::isfinite(l) && std::isfinite(u)) ? "bounds must be finite" : !(l <= u) ? "lo must be <= hi"
+                          : !std::isfinite(u - l) ? "hi - lo must be finite" : extra(c, l, u);
+    if (!why.empty()) return std::string(who) + ": " + names[c] + " of robot " + std::to_string(b) + ": " + why;
+  }
+  return "";
 }
 
 // modeNumber2StanceLeg: bit3 LF, bit2 RF, bit1 LH, bit0 RH (contact order LF,RF,LH,RH)

@@ -76,18 +76,8 @@ __global__ void __launch_bounds__(SP_THREADS) spawn_sample_kernel(const DevModel
   }
 
   // the reset rows: the state estimator at the new base position with no call yet (its next call places the feet), the attitude filter, the detector
-  if (a.se) {
-    double* st = a.se + (size_t)b * SE_DBL;
-    for (int i = 0; i < SE_DBL; ++i) st[i] = 0.0;
-    st[SE_X] = x; st[SE_X + 1] = y; st[SE_X + 2] = z;
-    for (int i = 0; i < SE_NX; ++i) st[SE_P + i * (i + 1) / 2 + i] = i < 3 ? a.se_p0[0] : (i < 6 ? a.se_p0[1] : a.se_p0[2]);
-  }
-  if (a.at) {
-    double* st = a.at + (size_t)b * AT_DBL;
-    for (int i = 0; i < AT_DBL; ++i) st[i] = 0.0;
-    st[AT_Q + 3] = 1.0;
-    for (int i = 0; i < AT_NX; ++i) st[AT_P + i * (i + 1) / 2 + i] = i < 3 ? a.at_p0[0] : a.at_p0[1];
-  }
+  if (a.se) state_est_reset_row(a.se_prm, base, a.se + (size_t)b * SE_DBL);   // base[0..2]: the base position
+  if (a.at) attitude_reset_row(a.at_prm, a.at + (size_t)b * AT_DBL);
   if (a.sl) for (int i = 0; i < SL_DBL; ++i) a.sl[(size_t)b * SL_DBL + i] = 0.0;
 }
 }  // namespace

@@ -16,11 +16,11 @@ static_assert(SEN_JVEL + NJ == QMB200_SENSORS, "sensor layout of include/qmb200.
 // noise channels of one reading: orientation (3), gyro (3), accel (3), joint pos (18), joint vel (18)
 constexpr int CH_ORI = 0, CH_GYRO = 3, CH_ACCEL = 6, CH_JPOS = 9, CH_JVEL = 27;
 
-// One standard normal draw, a pure function of (seed, robot, sample, channel): the four words are hashed in turn, two 53-bit uniforms in (0, 1) are cut
-// from two more hashes, and Box-Muller's cosine branch turns them into N(0, 1).  No generator state, so a draw does not depend on the batch or the launch.
+// One standard normal draw, a pure function of (seed, robot, sample, channel): two 53-bit uniforms in (0, 1) are cut from the key (keyed_hash with the
+// sensor domain) and from the key xor-ed with a second constant, and Box-Muller's cosine branch turns them into N(0, 1).
 QMB_HD double sensor_normal(uint64_t seed, uint64_t robot, uint64_t sample, int channel) {
-  const uint64_t h = mix64(mix64(mix64(mix64(seed ^ 0x9e3779b97f4a7c15ull) ^ robot) ^ sample) ^ (uint64_t)channel);
-  const double u1 = ((double)(mix64(h) >> 11) + 0.5) * 1.1102230246251565e-16, u2 = ((double)(mix64(h ^ 0xd1b54a32d192ed03ull) >> 11) + 0.5) * 1.1102230246251565e-16;
+  const uint64_t h = keyed_hash(seed, 0x9e3779b97f4a7c15ull, robot, sample, channel);
+  const double u1 = hash_uniform(h), u2 = hash_uniform(h ^ 0xd1b54a32d192ed03ull);
   return sqrt(-2.0 * log(u1)) * cos(6.283185307179586 * u2);
 }
 
@@ -30,6 +30,13 @@ QMB_HD double sensor_normal(uint64_t seed, uint64_t robot, uint64_t sample, int 
 //   [189]       calls since the reset (0: the next call only places the feet)
 constexpr int SE_NX = 18, SE_TRI = SE_NX * (SE_NX + 1) / 2, SE_NY = 28;
 constexpr int SE_X = 0, SE_P = SE_X + SE_NX, SE_N = SE_P + SE_TRI, SE_DBL = SE_N + 1;
+// The reset row st [SE_DBL] of one robot at base position base_pos [3]: zero velocity and feet, P diagonal with p's p0 variances, no call yet (the next
+// call places the feet).  qmb200_state_est_reset and the spawn sampler both write it.
+QMB_HD void state_est_reset_row(const qmb200_state_est_params& p, const double* base_pos, double* st) {
+  for (int i = 0; i < SE_DBL; ++i) st[i] = 0.0;
+  for (int i = 0; i < 3; ++i) st[SE_X + i] = base_pos[i];
+  for (int i = 0; i < SE_NX; ++i) st[SE_P + i * (i + 1) / 2 + i] = i < 3 ? p.p0_base_pos : (i < 6 ? p.p0_base_vel : p.p0_foot);
+}
 
 // sensors of robots [0, B) at the plant state (q, v) after a step of dt seconds that started at velocity v_prev; robot b draws its noise as robot robot0 + b
 int launch_read_sensors(const qmb200_sensor_params& prm, int B, int64_t robot0, double dt, int64_t sample, const double* q, const double* v, const double* v_prev,

@@ -705,21 +705,33 @@ class Solver:
         <= z_min, or |pitch|, |roll| >= tilt_max; count [B] int32 grows by one per fallen call and drops to 0 otherwise.  No synchronisation."""
         self._call("fall_detect_dev", _p(rbd), float(z_min), float(tilt_max), _p(count), _p(fallen), stream)
 
+    # ---------------- per-episode draws: the ranges' set / get / draw path of qmb200_episode_* and qmb200_spawn_* (kind "episode" or "spawn") ----------------
+    def _ranges_set(self, kind, width, lo, hi, seed):
+        if lo is None and hi is None:
+            self._call(kind + "_set_ranges", None, None, 0); return
+        shape = (self.batch, width); lo = _f64(lo, shape); hi = _f64(hi, shape)
+        s = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._call(kind + "_set_ranges", _p(lo), _p(hi), s - (1 << 64) if s >> 63 else s)
+
+    def _ranges_get(self, kind, width):
+        lo = np.zeros((self.batch, width)); hi = np.zeros_like(lo); seed = C.c_int64(); is_set = C.c_int32()
+        self._call(kind + "_get_ranges", _p(lo), _p(hi), C.byref(seed), C.byref(is_set))
+        return dict(lo=lo, hi=hi, seed=seed.value & 0xFFFFFFFFFFFFFFFF) if is_set.value else None
+
+    def _ranges_draw(self, kind, width, robot, episode):
+        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); rows = np.zeros((len(robot), width))
+        self._call(kind + "_draw", len(robot), _p(robot), _p(episode), _p(rows))
+        return rows
+
     # ---------------- per-episode plant draws (include/qmb200.h: qmb200_episode_*; DESIGN.md §4.11) ----------------
     def episode_set_ranges(self, lo=None, hi=None, seed=0):
         """Per-robot ranges lo, hi [B, EPISODE] (columns _lib.EPISODE_LAYOUT) and a 64-bit seed of the per-episode draws; None clears them.  Makes sure
         the plant's robot params are set (at the values in force where they were not).  Synchronous."""
-        if lo is None and hi is None:
-            self._call("episode_set_ranges", None, None, 0); return
-        shape = (self.batch, _lib.EPISODE); lo = _f64(lo, shape); hi = _f64(hi, shape)
-        s = int(seed) & 0xFFFFFFFFFFFFFFFF
-        self._call("episode_set_ranges", _p(lo), _p(hi), s - (1 << 64) if s >> 63 else s)
+        self._ranges_set("episode", _lib.EPISODE, lo, hi, seed)
 
     def episode_get_ranges(self):
         """→ dict(lo [B, EPISODE], hi [B, EPISODE], seed) of the stored ranges, or None when none are set."""
-        lo = np.zeros((self.batch, _lib.EPISODE)); hi = np.zeros_like(lo); seed = C.c_int64(); is_set = C.c_int32()
-        self._call("episode_get_ranges", _p(lo), _p(hi), C.byref(seed), C.byref(is_set))
-        return dict(lo=lo, hi=hi, seed=seed.value & 0xFFFFFFFFFFFFFFFF) if is_set.value else None
+        return self._ranges_get("episode", _lib.EPISODE)
 
     def episode_sample(self, mask, episode, link=0, rows=None):
         """Host variant of episode_sample_dev: mask [B], episode [B] → rows [B, EPISODE] (rows of unmasked robots as given, zeros by default)."""
@@ -736,25 +748,17 @@ class Solver:
 
     def episode_draw(self, robot, episode):
         """Host only: robot [n] (in [0, B)), episode [n] → the rows [n, EPISODE] the sampler draws for them on the stored ranges and seed."""
-        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); rows = np.zeros((len(robot), _lib.EPISODE))
-        self._call("episode_draw", len(robot), _p(robot), _p(episode), _p(rows))
-        return rows
+        return self._ranges_draw("episode", _lib.EPISODE, robot, episode)
 
     # ---------------- per-episode spawns (include/qmb200.h: qmb200_spawn_*; DESIGN.md §4.12) ----------------
     def spawn_set_ranges(self, lo=None, hi=None, seed=0):
         """Per-robot ranges lo, hi [B, SPAWN] (columns _lib.SPAWN_LAYOUT) and a 64-bit seed of the per-episode spawns; None clears them.  The offsets
         count from the plant's robot terrain origins in force; with a tile bound >= 0 the robot terrain rows are made to exist.  Synchronous."""
-        if lo is None and hi is None:
-            self._call("spawn_set_ranges", None, None, 0); return
-        shape = (self.batch, _lib.SPAWN); lo = _f64(lo, shape); hi = _f64(hi, shape)
-        s = int(seed) & 0xFFFFFFFFFFFFFFFF
-        self._call("spawn_set_ranges", _p(lo), _p(hi), s - (1 << 64) if s >> 63 else s)
+        self._ranges_set("spawn", _lib.SPAWN, lo, hi, seed)
 
     def spawn_get_ranges(self):
         """→ dict(lo [B, SPAWN], hi [B, SPAWN], seed) of the stored ranges, or None when none are set."""
-        lo = np.zeros((self.batch, _lib.SPAWN)); hi = np.zeros_like(lo); seed = C.c_int64(); is_set = C.c_int32()
-        self._call("spawn_get_ranges", _p(lo), _p(hi), C.byref(seed), C.byref(is_set))
-        return dict(lo=lo, hi=hi, seed=seed.value & 0xFFFFFFFFFFFFFFFF) if is_set.value else None
+        return self._ranges_get("spawn", _lib.SPAWN)
 
     def spawn_sample(self, mask, episode, q, v, rbd, contact, x_obs, last_ee, rbd_est=None, link=0, rows=None):
         """Host variant of spawn_sample_dev on copies of the arrays → dict(rows [B, SPAWN], q, v, rbd, contact, x_obs, last_ee[, rbd_est]); unmasked
@@ -776,9 +780,7 @@ class Solver:
 
     def spawn_draw(self, robot, episode):
         """Host only: robot [n] (in [0, B)), episode [n] → the spawn rows [n, SPAWN] the sampler draws for them on the stored ranges and seed."""
-        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); rows = np.zeros((len(robot), _lib.SPAWN))
-        self._call("spawn_draw", len(robot), _p(robot), _p(episode), _p(rows))
-        return rows
+        return self._ranges_draw("spawn", _lib.SPAWN, robot, episode)
 
     # ---------------- device gait schedule (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7) ----------------
     def gait_dev_set_templates(self, names=None, gait_file=None):

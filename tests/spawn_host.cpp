@@ -1,18 +1,11 @@
-// TEST INFRASTRUCTURE: host build (g++) of the per-episode spawn core (qm_control_b200/csrc/kernels/spawn_api.cuh), the same functions the sampler
-// kernel and qmb200_spawn_draw compile, so that the CPU suite can check the draw against a numpy statement and the ported standing pose against the
-// host's standing_on_terrain (tests/test_spawn_cpu.py).  The suite compiles this file with -DHOST_STANDING naming a file that holds the host function's
-// text as capi_sim.inc has it, and links host/qm_config.cpp for the model and the host kinematics.
-#include <algorithm>
+// TEST INFRASTRUCTURE: host build (g++) of the per-episode spawn core (qm_control_b200/csrc/kernels/spawn_api.cuh) and the standing pose
+// (kernels/sim_api.cuh), the same functions the sampler kernel, qmb200_spawn_draw and qmb200_sim_standing_state compile, so that the CPU suite can check
+// the draw against a numpy statement, the standing pose against its recorded outputs and the chain kinematics against the host kinematics
+// (tests/test_spawn_cpu.py).  Links host/qm_config.cpp for the model and host_fk.
 #include <cstring>
 
 #include "host/qm_config.h"
 #include "kernels/spawn_api.cuh"
-
-namespace qmb {
-namespace host_twin {
-#include HOST_STANDING
-}  // namespace host_twin
-}  // namespace qmb
 
 using namespace qmb;
 
@@ -45,21 +38,16 @@ int sp_chains_serial(void* h) {
   }
   return 1;
 }
-// n robots at xy_yaw [n][3] on terrain rows [n][3] of the library tiles [n_tiles][ny][nx]: the port (standing_on_tile) into port [n][3] = (z, pitch,
-// roll) and the host's standing_on_terrain into host [n][3]; both at defaultJointState
-void sp_standing(void* hp, const double* tiles, int nx, int ny, double cell, int n, const double* rows, const double* xy_yaw, double radius, double delta0, double* port,
-                 double* host) {
+// n robots at xy_yaw [n][3] on terrain rows [n][3] of the library tiles [n_tiles][ny][nx] at defaultJointState: standing_on_tile into out [n][3] =
+// (z, pitch, roll)
+void sp_standing(void* hp, const double* tiles, int nx, int ny, double cell, int n, const double* rows, const double* xy_yaw, double radius, double delta0, double* out) {
   const HostModel& hm = *static_cast<HostModel*>(hp); const SimTerrain t{tiles, nullptr, nx, ny, cell};
   for (int i = 0; i < n; ++i) {
-    const double* r = rows + 3 * i; const double* p = xy_yaw + 3 * i;
-    double z, pitch, roll; standing_on_tile(hm.dev, t, r, radius, delta0, hm.default_joint_state, p[0], p[1], p[2], z, pitch, roll);
-    port[3 * i] = z; port[3 * i + 1] = pitch; port[3 * i + 2] = roll;
-    double q[NQ] = {0}; q[0] = p[0]; q[1] = p[1]; q[3] = p[2]; for (int j = 0; j < NJ; ++j) q[6 + j] = hm.default_joint_state[j];
-    host_twin::standing_on_terrain(hm.dev, t, r, radius, delta0, q);
-    host[3 * i] = q[2]; host[3 * i + 1] = q[4]; host[3 * i + 2] = q[5];
+    const double* p = xy_yaw + 3 * i;
+    standing_on_tile(hm.dev, t, rows + 3 * i, radius, delta0, hm.default_joint_state, p[0], p[1], p[2], out[3 * i], out[3 * i + 1], out[3 * i + 2]);
   }
 }
-// the end-effector pose and the four feet of the port's forward kinematics at the standing configuration (x, y, z, yaw, pitch, roll): ee [7] (position,
+// the end-effector pose and the four feet of the chain kinematics at the standing configuration (x, y, z, yaw, pitch, roll): ee [7] (position,
 // quaternion xyzw), feet [4][3]; and the host kinematics' (host_fk) into ee_host, feet_host
 void sp_kinematics(void* hp, const double* base, double* ee, double* feet, double* ee_host, double* feet_host) {
   const HostModel& hm = *static_cast<HostModel*>(hp); const DevModel& d = hm.dev; const double* qj = hm.default_joint_state;

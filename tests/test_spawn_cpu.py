@@ -1,6 +1,6 @@
 """Per-episode spawns on the host, no GPU (DESIGN.md §4.12): the draw core compiled with g++ (tests/spawn_host.cpp) against its numpy statement, its
-distribution and its keys, the range check, the ported standing pose against the host's standing_on_terrain, closed_loop.run(spawn=...) validation and
-its ranges on a fake Solver, the bindings and the kernel's resources."""
+distribution and its keys, the range check, the standing pose against its recorded outputs (tests/golden/standing_pose.npz), closed_loop.run(spawn=...)
+validation and its ranges on a fake Solver, the bindings and the kernel's resources."""
 import ctypes as C
 import os
 import re
@@ -15,7 +15,6 @@ from scipy import stats
 
 import _episode_twin as etw
 from _oracle import GAINS, REFERENCE, TASK, URDF
-from _state_est_twin import _mix
 from qm_control_b200 import _lib, closed_loop, terrain
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -25,33 +24,20 @@ NAMES = ("qmb200_spawn_set_ranges", "qmb200_spawn_get_ranges", "qmb200_spawn_sam
 DOMAIN = np.uint64(0xbb67ae8584caa73b)   # spawn_api.cuh's SPAWN_DOMAIN
 
 
-def twin_uniform(seed, robot, episode, column):
-    """u in (0, 1) of (seed, robot, episode, column): the four words hashed in turn (the spawn domain), the 53 high bits of one more hash, plus a half"""
-    u = etw._u64
-    h = _mix(_mix(_mix(_mix(u(seed) ^ DOMAIN) ^ u(robot)) ^ u(episode)) ^ u(column))
-    return ((_mix(h) >> np.uint64(11)).astype(np.float64) + 0.5) * 2.0 ** -53
-
-
 def twin_rows(lo, hi, seed, robot, episode):
-    """lo, hi [n, 4], keys [n] → rows [n, 4]: lo where hi == lo; the tile lo + min(floor(u (hi - lo + 1)), hi - lo); else fma(u, hi - lo, lo)"""
+    """lo, hi [n, 4], keys [n] → rows [n, 4]: the episode twin's rows on the spawn domain, with the tile lo + min(floor(u (hi - lo + 1)), hi - lo)"""
     lo = np.asarray(lo, dtype=np.float64); hi = np.asarray(hi, dtype=np.float64); d = hi - lo
-    u = twin_uniform(np.asarray(seed)[:, None], np.asarray(robot)[:, None], np.asarray(episode)[:, None], np.arange(_lib.SPAWN)[None, :])
-    out = etw.fma(u, d, lo)
-    out[:, 0] = lo[:, 0] + np.minimum(np.floor(u[:, 0] * (d[:, 0] + 1.0)), d[:, 0])
-    return np.where(hi == lo, lo, out)
+    out = etw.rows(lo, hi, seed, robot, episode, DOMAIN)
+    u = etw.uniform(seed, robot, episode, 0, DOMAIN)
+    out[:, 0] = np.where(hi[:, 0] == lo[:, 0], lo[:, 0], lo[:, 0] + np.minimum(np.floor(u * (d[:, 0] + 1.0)), d[:, 0]))
+    return out
 
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    d = tmp_path_factory.mktemp("spawn")
-    # the host's standing_on_terrain, its text as capi_sim.inc has it, compiled beside the port
-    src = open(os.path.join(CSRC, "capi_sim.inc")).read()
-    m = re.search(r"^void standing_on_terrain\(.*?^}\n", src, re.S | re.M); assert m, "capi_sim.inc has standing_on_terrain"
-    (d / "host_standing.inc").write_text(m.group(0))
-    lib_path = str(d / "libspawnhost.so")
+    lib_path = str(tmp_path_factory.mktemp("spawn") / "libspawnhost.so")
     subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-attributes", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-I" + CSRC,
-                           "-DHOST_STANDING=\"%s\"" % (d / "host_standing.inc"), "-o", lib_path, os.path.join(ROOT, "tests", "spawn_host.cpp"),
-                           os.path.join(CSRC, "host", "qm_config.cpp")])
+                           "-o", lib_path, os.path.join(ROOT, "tests", "spawn_host.cpp"), os.path.join(CSRC, "host", "qm_config.cpp")])
     lib = C.CDLL(lib_path); lib.sp_create.restype = C.c_void_p
     return lib
 
@@ -93,7 +79,7 @@ def test_core_equals_the_numpy_statement_bit_for_bit(core):
     rng = np.random.default_rng(21); n = 120_000
     seed, robot, episode = _keys(rng, n); col = rng.integers(0, _lib.SPAWN, n).astype(np.int32)
     u = np.zeros(n); core.sp_uniform(C.c_int(n), _ptr(seed), _ptr(robot), _ptr(episode), _ptr(col), _ptr(u))
-    np.testing.assert_array_equal(u, twin_uniform(seed, robot, episode, col))
+    np.testing.assert_array_equal(u, etw.uniform(seed, robot, episode, col, DOMAIN))
     assert np.all(u > 0.0) and np.all(u < 1.0)
     m = 30_000; seed, robot, episode = _keys(rng, m); lo, hi = _ranges(rng, m)   # 120000 values
     got = _rows(core, lo, hi, seed, robot, episode)
@@ -163,19 +149,17 @@ def test_every_chain_is_a_serial_chain_off_the_base(core, model):
     assert core.sp_chains_serial(model) == 1
 
 
-def test_port_equals_the_host_standing_on_terrain(core, model):
-    """ramp, stairs, rough and combined tiles, seeded offsets and yaws: z, pitch and roll within 1e-12 m / rad of the host's standing_on_terrain"""
-    tiles = _library(); ny, nx = tiles.shape[1:]; rng = np.random.default_rng(8); n = 400
-    tile = rng.integers(0, len(tiles), n); origin = terrain.centred_origin(np.zeros(2)) - rng.uniform(-1.2, 1.2, (n, 2))
-    rows = np.c_[tile, origin].astype(np.float64); xy_yaw = np.c_[rng.uniform(-0.3, 0.3, (n, 2)), rng.uniform(-np.pi, np.pi, n)]
-    radius, delta0 = 0.0265, 0.0
-    for delta0 in (0.0, 1e-4):
-        port = np.zeros((n, 3)); host = np.zeros((n, 3))
+def test_standing_pose_equals_the_recorded_poses(core, model):
+    """ramp, stairs, rough and combined tiles, seeded offsets and yaws: z, pitch and roll bit for bit as recorded (tests/golden/standing_pose.md)"""
+    g = np.load(os.path.join(ROOT, "tests", "golden", "standing_pose.npz"))
+    tiles = _library(); ny, nx = tiles.shape[1:]; rows = g["rows"]; xy_yaw = g["xy_yaw"]; n = len(rows)
+    for delta0, want in zip(g["delta0"], g["z_pitch_roll"]):
+        got = np.zeros((n, 3))
         core.sp_standing(model, _ptr(np.ascontiguousarray(tiles)), C.c_int(nx), C.c_int(ny), C.c_double(terrain.CELL), C.c_int(n), _ptr(rows), _ptr(xy_yaw),
-                         C.c_double(radius), C.c_double(delta0), _ptr(port), _ptr(host))
-        assert np.all(np.isfinite(port))
-        np.testing.assert_allclose(port, host, rtol=0, atol=1e-12)
-        assert np.ptp(port[:, 1]) > 0.1 and np.ptp(port[:, 0]) > 0.05   # the tiles tilt and lift the robots
+                         C.c_double(g["radius"]), C.c_double(delta0), _ptr(got))
+        assert np.all(np.isfinite(got))
+        assert got.tobytes() == want.tobytes()
+        assert np.ptp(got[:, 1]) > 0.1 and np.ptp(got[:, 0]) > 0.05   # the tiles tilt and lift the robots
 
 
 def test_port_kinematics_equal_the_host_kinematics(core, model):
@@ -184,7 +168,7 @@ def test_port_kinematics_equal_the_host_kinematics(core, model):
         base = np.r_[rng.uniform(-2, 2, 2), rng.uniform(0.3, 0.6), rng.uniform(-np.pi, np.pi), rng.uniform(-0.3, 0.3, 2)]
         ee, feet, eh, fh = np.zeros(7), np.zeros(12), np.zeros(7), np.zeros(12)
         core.sp_kinematics(model, _ptr(base), _ptr(ee), _ptr(feet), _ptr(eh), _ptr(fh))
-        np.testing.assert_allclose(ee, eh, rtol=0, atol=1e-12); np.testing.assert_allclose(feet, fh, rtol=0, atol=1e-12)
+        assert ee.tobytes() == eh.tobytes() and feet.tobytes() == fh.tobytes()
 
 
 # --------------------------------------------------------------------------------------------------------------------------- closed_loop.run(spawn=...)
