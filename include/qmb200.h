@@ -644,6 +644,60 @@ int qmb200_spawn_sample_dev(qmb200_handle* h, const int32_t* mask, const int32_t
 /* Host only: the rows [n][QMB200_SPAWN] of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the sampler draws. */
 int qmb200_spawn_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][QMB200_SPAWN]*/);
 
+/* ---- per-episode metrics (DESIGN.md §4.13): each robot's episode is scored on the device from the plant's truth, one sample per plant step.
+ * A sample is the plant's state after one step: its rbd, its contact mask and the effort held over the step.  The first sample of an episode opens it
+ * (the start xy, the foot positions, the contact mask); per-sample terms count from the first sample, displacement terms (path, slip, touchdowns)
+ * between consecutive samples from the second on.  A closed episode is one row of QMB200_METRICS doubles:
+ *   0  duration          sum of dt over the samples (samples x dt at a fixed step) (s)
+ *   1  end               why it closed: 0 run end (truncated), 1 respawn on a fall, 2 respawn at the episode length limit
+ *   2  status            bitwise OR of the status words passed with its samples, as a double
+ *   3  distance          planar distance between the base xy of the first and of the last sample (m)
+ *   4  path_length       sum of the planar base displacement between consecutive samples (m)
+ *   5  min_height        min of p_z - H(p_x, p_y), H the plant's ground under the base (its terrain row in force at the sample, as qmb200_fall_detect) (m)
+ *   6  max_tilt          max of max(|pitch|, |roll|) (rad)
+ *   7  vel_err_rms       RMS over the cmd_vel samples of |v_xy - v_ref,xy|, v_ref = target_states[b][0][0:2] (the cmd_vel target's world velocity) (m/s)
+ *   8  yaw_rate_err_rms  RMS over the same samples of omega_z - cmd[b][3] (rad/s)
+ *   9  ee_pos_err_rms    RMS of |p_ee - p_ref(t)|, p_ref the target trajectory's end-effector position at the sample's time, as the MPC interpolates it (m)
+ *  10  ee_pos_err_max    max of the same (m)
+ *  11  ee_ori_err_rms    RMS of the angle of q_ref^-1 q_ee, 2 atan2(|vec|, |w|) (rad)
+ *  12  energy            sum over the samples and the 18 joints of |tau_j qd_j| dt (J)
+ *  13  torque_rms        sqrt(mean over the samples of sum_j tau_j^2 / 18) (N m)
+ *  14  slip              sum over feet and consecutive sample pairs with the foot's contact bit set in both of its foot frame's planar displacement (m)
+ *  15  touchdowns        count of 0 -> 1 transitions of the four contact bits
+ *  16  est_pos_err_rms   RMS of |p_est - p| over the samples passed with an estimate rbd_est (m)
+ *  17  est_vel_err_rms   RMS of |v_est - v| over the same samples (m/s)
+ * A cmd_vel sample is one whose robot's target kind is QMB200_TARGET_CMD_VEL (kind [B], or every robot when kind is NULL).  An RMS, max, min or distance
+ * over no samples is NaN.
+ * The open episode of each robot is an accumulator row of QMB200_METRICS_ACC doubles, owned by the caller; all zeros is an open, empty episode:
+ *   0 samples  1 sum of dt  2 status OR  3-4 first base xy  5-6 last base xy  7-14 last foot xy [4][2] (contact order)  15 last contact mask  16 path
+ *   17 min height  18 max tilt  19 cmd_vel samples  20-21 their squared velocity and yaw-rate errors  22 squared EE position errors  23 max EE error
+ *   24 squared EE angles  25 energy  26 sum of sum_j tau_j^2 / 18  27 slip  28 touchdowns  29 samples with an estimate  30-31 their squared errors */
+#define QMB200_METRICS 18
+#define QMB200_METRICS_ACC 32
+/* One launch, no host work: one sample of every robot into acc [B][QMB200_METRICS_ACC] (in-out).  rbd [B][55], contact [B] and effort [B][18] are the
+ * plant's state after the step and the effort held over it; cmd [B][7] the target commands (cmd[b][3]: the commanded yaw rate); kind [B] or NULL the
+ * robots' target kinds; n_target [B] (clamped to [1, QMB200_KMAX] as the MPC does), target_times [B][QMB200_KMAX] and target_states
+ * [B][QMB200_KMAX][QMB200_TARGET] the target trajectories in force; time [B] the plant clock at the start of the step, so the sample lies at time + dt;
+ * status [B] the words to OR into the episode's; rbd_est [B][55] or NULL the estimate.  The foot frames come from the joints of rbd, the ground from the
+ * plant's terrain (qmb200_sim_set_terrain, qmb200_sim_set_robot_terrain).  Fails, writing nothing, on a null required buffer and a dt that is not finite
+ * and > 0. */
+int qmb200_metrics_step(qmb200_handle* h, double dt, const double* rbd /*[B][55]*/, const int32_t* contact /*[B]*/, const double* effort /*[B][18]*/,
+                        const double* cmd /*[B][7]*/, const int32_t* kind /*[B] or NULL*/, const int32_t* n_target /*[B]*/, const double* target_times,
+                        const double* target_states, const double* time /*[B]*/, const int32_t* status /*[B]*/, const double* rbd_est /*[B][55] or NULL*/,
+                        double* acc /*[B][QMB200_METRICS_ACC] in-out*/);
+int qmb200_metrics_step_dev(qmb200_handle* h, double dt, const double* rbd, const int32_t* contact, const double* effort, const double* cmd, const int32_t* kind,
+                            const int32_t* n_target, const double* target_times, const double* target_states, const double* time, const int32_t* status,
+                            const double* rbd_est, double* acc, void* cuda_stream);
+/* One launch, no host work: every robot with mask[b] != 0 closes its episode: its row, with end[b] as column 1, goes to out[b][episode[b]] (out
+ * [B][n_episodes][QMB200_METRICS], in-out) and its accumulator row is zeroed, which opens the next episode.  When episode[b] lies outside [0, n_episodes)
+ * no row is written, QMB200_ST_OVERFLOW is OR-ed into status[b] and the accumulator is still zeroed.  Robots with mask[b] == 0 are not written.  Fails,
+ * writing nothing, on a null buffer and n_episodes < 1; the host variant also on a masked end outside {0, 1, 2}, which the device variant, unable to read
+ * it on the host, refuses per robot by writing nothing of that robot. */
+int qmb200_metrics_close(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* end /*[B]*/, const int32_t* episode /*[B]*/, int32_t n_episodes,
+                         double* acc /*[B][QMB200_METRICS_ACC] in-out*/, double* out /*[B][n_episodes][QMB200_METRICS] in-out*/, int32_t* status /*[B] in-out*/);
+int qmb200_metrics_close_dev(qmb200_handle* h, const int32_t* mask, const int32_t* end, const int32_t* episode, int32_t n_episodes, double* acc, double* out,
+                             int32_t* status, void* cuda_stream);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

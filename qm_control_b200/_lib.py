@@ -96,6 +96,11 @@ EPISODE_MODEL_PAYLOAD, EPISODE_MPC_FRICTION, EPISODE_WBC_FRICTION = 1, 2, 4   # 
 SPAWN_LAYOUT = ("tile", "dx", "dy", "yaw")
 SPAWN = len(SPAWN_LAYOUT)   # QMB200_SPAWN
 SPAWN_GROUND_MAP = 1        # QMB200_SPAWN_GROUND_MAP
+# one closed episode's metrics (qmb200_metrics_*): the columns of a row of METRICS doubles, and the width of the accumulator row of an open episode
+METRICS_LAYOUT = ("duration", "end", "status", "distance", "path_length", "min_height", "max_tilt", "vel_err_rms", "yaw_rate_err_rms", "ee_pos_err_rms",
+                  "ee_pos_err_max", "ee_ori_err_rms", "energy", "torque_rms", "slip", "touchdowns", "est_pos_err_rms", "est_vel_err_rms")
+METRICS = len(METRICS_LAYOUT)   # QMB200_METRICS
+METRICS_ACC = 32                # QMB200_METRICS_ACC
 
 
 # every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
@@ -225,6 +230,10 @@ PROTOTYPES = {
     "qmb200_spawn_sample": (I32, [P, P, P, I32] + [P] * 8),
     "qmb200_spawn_sample_dev": (I32, [P, P, P, I32] + [P] * 9),
     "qmb200_spawn_draw": (I32, [P, I32, P, P, P]),
+    "qmb200_metrics_step": (I32, [P, D] + [P] * 12),
+    "qmb200_metrics_step_dev": (I32, [P, D] + [P] * 13),
+    "qmb200_metrics_close": (I32, [P] * 4 + [I32] + [P] * 3),
+    "qmb200_metrics_close_dev": (I32, [P] * 4 + [I32] + [P] * 4),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

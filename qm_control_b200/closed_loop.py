@@ -55,7 +55,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None):
+        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -143,7 +143,16 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     cmd_vel, 1 ee_cmd_vel, 2 goal published, -1 goal held), and ee_target[ticks, B, 7], the final-knot end-effector pose of the target in force after
     that call); with respawn also episode[ticks, B], each robot's episode index in that record's window (0 for the first), and fallen[ticks, B], the
     detector's flag at that window's end; with randomize also episode_params[B, E, 27], the row each robot drew for each episode e < E (E: the most
-    episodes of any robot), NaN where a robot had no episode e; with spawn also spawn_params[B, E, 4], the spawn row of each such episode."""
+    episodes of any robot), NaN where a robot had no episode e; with spawn also spawn_params[B, E, 4], the spawn row of each such episode.
+    metrics: True scores every episode on the device (DESIGN.md §4.13, Solver.metrics_step_dev / metrics_close_dev): after every plant step, once the
+    step's status words are in the record's and the estimators have stepped, one sample of the plant's truth (its rbd, contact mask and the effort held
+    over the step, the target in force, the robot's episode clock, the record's status word and, with state_estimator, the estimate) goes into each
+    robot's accumulator.  A respawning robot's episode closes right before its restore (end 1 when the fall rule restarted it, 2 when every did), and
+    every robot's open episode closes when the loop ends (end 0).  The samples only read the loop's tensors, so every other output is unchanged.
+    Returns also episode_metrics[B, E, METRICS] in the columns of metrics_layout (_lib.METRICS_LAYOUT), E as for episode_params, NaN rows where a
+    robot had no episode e."""
+    if metrics is not None and metrics is not True:
+        raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else _respawn_spec(respawn)
     rz = None if randomize is None else _randomize_spec(getattr(solver, "batch", None), randomize)
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
@@ -208,7 +217,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.callback(solver.robot_image_clear)
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp)
+                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp, mt=metrics is not None)
 
 
 def _respawn_spec(respawn):
@@ -532,8 +541,17 @@ def _robot_params(solver, friction_mu, payload):
         solver.sim_set_robot_params(**prev)
 
 
+def _metrics_episodes(ticks, rs):
+    """the most episodes a run of `ticks` 10 ms windows can hold under the respawn spec rs (None: one): a robot respawns only at a window boundary
+    after its episode has lasted at least hold windows (on the fall rule) or every (at the limit), whichever is shorter, and at least one window"""
+    if rs is None:
+        return 1
+    shortest = min([rs["hold_windows"]] * rs["on_fall"] + ([rs["every_ms"] // MPC_PERIOD_MS] if rs["every_ms"] is not None else []))
+    return (ticks - 1) // max(shortest, 1) + 1
+
+
 def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
-         rs=None, rz=None, sp=None):
+         rs=None, rz=None, sp=None, mt=False):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -663,9 +681,18 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             k0 = torch.zeros(B, dtype=torch.int64, device=dev); dk = torch.zeros_like(k0)   # each robot's episode start (plant step), and k - k0
             episode = torch.zeros(B, dtype=torch.int32, device=dev); fall_count = torch.zeros_like(episode); fallen = torch.zeros_like(episode)
             due = torch.ones_like(episode); rec_episode = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_fallen = torch.zeros_like(rec_episode)
+            if mt:   # the fall part of due: why a closed episode ended
+                due_fall = torch.zeros_like(episode); mt_end = torch.zeros_like(episode)
         solver.robot_image_restore_dev(due, s)
+    if mt:   # every robot's open episode (zeros: open and empty) and its closed rows
+        with torch.cuda.stream(stream):
+            mt_acc = torch.zeros((B, _lib.METRICS_ACC), dtype=torch.float64, device=dev)
+            mt_out = torch.full((B, _metrics_episodes(ticks, rs), _lib.METRICS), np.nan, dtype=torch.float64, device=dev)
 
-    def respawn(k):   # the robots due restart at window boundary k: the library's rows, then the loop's, then their new plant
+    def respawn(k):   # the robots due restart at window boundary k: their episode closes, then the library's rows, the loop's, their new plant
+        if mt:
+            mt_end.copy_(due_fall).neg_().add_(2)   # 1: the fall rule, 2: every
+            solver.metrics_close_dev(due, mt_end, episode, mt_acc, mt_out, acc_st, s)
         solver.robot_image_restore_dev(due, s)
         m = due.bool()
         for a, a0 in zip(own, start):
@@ -740,6 +767,9 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             if est:
                 solver.payload_est_step_dev(1e-3, effort, meas, est_st, s)
                 acc_st.bitwise_or_(est_st)
+            if mt:   # the plant's truth after the step, on the robot's episode clock, with the window's status so far
+                solver.metrics_step_dev(1e-3, rbd, contact, effort, cmd7, prob["n_target"], prob["target_times"], prob["target_states"], hw_time, acc_st, mt_acc,
+                                        kind=None if gd is None else rec_kind[k // MPC_PERIOD_MS], rbd_est=rbd_est if se else None, stream=s)
             if (k + 1) % MPC_PERIOD_MS == 0:
                 i = (k + 1) // MPC_PERIOD_MS - 1
                 rec_base[i, :, 0:3] = rbd[:, 3:6]; rec_base[i, :, 3:6] = rbd[:, 0:3]; rec_ee[i] = rbd[:, 48:55]; rec_st[i] = acc_st; acc_st.zero_()
@@ -751,9 +781,14 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                     solver.fall_detect_dev(rbd, fall_count, fallen, rs["z_min"], rs["tilt_max"], s)
                     rec_episode[i] = episode; rec_fallen[i] = fallen
                     d = fall_count >= rs["hold_windows"] if rs["on_fall"] else torch.zeros_like(fallen, dtype=torch.bool)
+                    if mt:
+                        due_fall.copy_(d)
                     if rs["every_ms"] is not None:
                         d |= (k + 1 - k0) >= rs["every_ms"]
                     due.copy_(d)
+        if mt:   # the run's end closes every robot's open episode
+            ones = torch.ones(B, dtype=torch.int32, device=dev)
+            solver.metrics_close_dev(ones, torch.zeros_like(ones), episode if rs is not None else torch.zeros_like(ones), mt_acc, mt_out, acc_st, s)
     stream.synchronize()
     t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
     out = dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
@@ -776,4 +811,7 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         for kind, spec, width in (("episode", rz, _lib.EPISODE), ("spawn", sp, _lib.SPAWN)):
             if spec is not None:
                 out[kind + "_params"] = np.full(had.shape + (width,), np.nan); out[kind + "_params"][rb, re_] = getattr(solver, kind + "_draw")(rb, re_)
+    if mt:   # trimmed to the most episodes of any robot
+        E = int(out["episode"].max()) + 1 if rs is not None else 1
+        out.update(episode_metrics=mt_out[:, :E].cpu().numpy(), metrics_layout=_lib.METRICS_LAYOUT)
     return out

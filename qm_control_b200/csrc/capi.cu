@@ -22,6 +22,7 @@
 #include "kernels/respawn_api.cuh"
 #include "kernels/episode_api.cuh"
 #include "kernels/spawn_api.cuh"
+#include "kernels/metrics_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -150,14 +151,20 @@ int set_robot_arrays(qmb200_handle* h, std::initializer_list<RobotRows> sets) {
 // Every array declared out must be written in full by the kernels, since the arena holds whatever the previous call left there.
 class Staging {
  public:
-  // The widest entry point, qmb200_control_law, stages 242 doubles and one int32 per robot (qmb200_update: 238 and one); each of its at most
-  // STAGE_SLICES slices starts on a 256-byte boundary, the alignment cudaMalloc gives.
+  // The widest fixed-size entry point, qmb200_control_law, stages 242 doubles and one int32 per robot (qmb200_update: 238 and one); each of its at most
+  // STAGE_SLICES slices starts on a 256-byte boundary, the alignment cudaMalloc gives.  A call that stages more (the metrics entry points, whose widths
+  // grow with their inputs) asks open() for its bytes, and the arena grows to them.
   static constexpr size_t ROBOT_BYTES = 243 * 8, ALIGN = 256, STAGE_SLICES = 10;
   explicit Staging(qmb200_handle* h) : h_(h) {}
-  int open() {
+  int open(size_t need = 0) {
     QMB_CUDA(h_, cudaSetDevice(h_->device));
+    const size_t bytes = std::max((size_t)h_->B * ROBOT_BYTES + STAGE_SLICES * ALIGN, need);
+    if (h_->stage && h_->stage_bytes < bytes) {   // no queued copy may still read the old arena: h->stream is the only stream that uses it
+      QMB_CUDA(h_, cudaStreamSynchronize(h_->stream));
+      h_->allocs.erase(std::find(h_->allocs.begin(), h_->allocs.end(), static_cast<void*>(h_->stage)));
+      QMB_CUDA(h_, cudaFree(h_->stage)); h_->stage = nullptr;
+    }
     if (!h_->stage) {
-      const size_t bytes = (size_t)h_->B * ROBOT_BYTES + STAGE_SLICES * ALIGN;
       if (!dalloc(h_, &h_->stage, bytes)) return -4;   // zeroed on h->stream, the only stream that uses the arena
       h_->stage_bytes = bytes;
     }
@@ -503,3 +510,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_respawn.inc"
 #include "capi_episode.inc"
 #include "capi_spawn.inc"
+#include "capi_metrics.inc"

@@ -165,13 +165,17 @@ struct TargetSeg { const double* l; const double* rr; double a; };
 QMB_HD TargetSeg target_segment(const double* tt, const double* ts /*[K][37]*/, int nk, double t) {
   int idx; double a; time_segment(tt, nk, t, idx, a); TargetSeg sg; sg.l = ts + (size_t)idx * 37; sg.rr = ts + (size_t)((nk > 1) ? idx + 1 : idx) * 37; sg.a = (nk <= 1) ? 1.0 : a; return sg;
 }
-QMB_HD void target_pose(const TargetSeg& sg, int nk, double* pref, double* qref) {
+// The slerp's sines take angles in [0, pi/2]; Sin lets a caller that must stay off the stack pass a sine without the huge-argument slow path
+// (metrics_api.cuh's BoundedSin).
+struct StdSin { QMB_HD double operator()(double x) const { return sin(x); } };
+template <class Sin = StdSin>
+QMB_HD void target_pose(const TargetSeg& sg, int nk, double* pref, double* qref, Sin sine = Sin()) {
   const double* l = sg.l; const double* rr = sg.rr; const double a = sg.a;
   for (int i = 0; i < 3; ++i) pref[i] = a * l[30 + i] + (1.0 - a) * rr[30 + i];
   if (nk > 1) {
     const double* ql = l + 33; const double* qr = rr + 33; const double tq = 1.0 - a; double d = 0.0; for (int i = 0; i < 4; ++i) d += ql[i] * qr[i];
     const double ad = fabs(d); double s0, s1;
-    if (ad >= 1.0 - 2.220446049250313e-16) { s0 = 1.0 - tq; s1 = tq; } else { const double th = acos(ad), st = sin(th); const double ist = 1.0 / st; s0 = sin((1.0 - tq) * th) * ist; s1 = sin(tq * th) * ist; }
+    if (ad >= 1.0 - 2.220446049250313e-16) { s0 = 1.0 - tq; s1 = tq; } else { const double th = acos(ad), st = sine(th); const double ist = 1.0 / st; s0 = sine((1.0 - tq) * th) * ist; s1 = sine(tq * th) * ist; }
     if (d < 0.0) s1 = -s1;
     for (int i = 0; i < 4; ++i) qref[i] = s0 * ql[i] + s1 * qr[i];
   } else { for (int i = 0; i < 4; ++i) qref[i] = l[33 + i]; }

@@ -782,6 +782,43 @@ class Solver:
         """Host only: robot [n] (in [0, B)), episode [n] → the spawn rows [n, SPAWN] the sampler draws for them on the stored ranges and seed."""
         return self._ranges_draw("spawn", _lib.SPAWN, robot, episode)
 
+    # ---------------- per-episode metrics (include/qmb200.h: qmb200_metrics_*; DESIGN.md §4.13) ----------------
+    def metrics_step(self, dt, rbd, contact, effort, cmd, n_target, target_times, target_states, time, status, acc, kind=None, rbd_est=None):
+        """Host variant of metrics_step_dev on a copy of acc [B, METRICS_ACC] → the accumulator rows after the sample."""
+        B = self.batch; acc = _f64(acc, (B, _lib.METRICS_ACC)).copy()
+        args = [_f64(rbd, (B, RBD)), _i32(contact, (B,)), _f64(effort, (B, 18)), _f64(cmd, (B, 7)), None if kind is None else _i32(kind, (B,)),
+                _i32(n_target, (B,)), _f64(target_times, (B, KMAX)), _f64(target_states, (B, KMAX, TARGET)), _f64(time, (B,)), _i32(status, (B,)),
+                None if rbd_est is None else _f64(rbd_est, (B, RBD)), acc]
+        self._call("metrics_step", float(dt), *(_p(a) for a in args))
+        return acc
+
+    def metrics_step_dev(self, dt, rbd, contact, effort, cmd, n_target, target_times, target_states, time, status, acc, kind=None, rbd_est=None, stream=None):
+        """One sample of every robot after a plant step of dt s into its accumulator row acc [B, METRICS_ACC] (float64 device tensor, in-out): the plant's
+        rbd [B, 55], contact [B] and the effort [B, 18] held over the step, the target commands cmd [B, 7] and kinds kind [B] (None: every robot on
+        cmd_vel), the target rows in force (n_target [B], target_times [B, KMAX], target_states [B, KMAX, TARGET]), the plant clock time [B] at the
+        step's start, the status words [B] to OR in, the estimate rbd_est [B, 55] or None.  One launch, no synchronisation."""
+        self._call("metrics_step_dev", float(dt), _p(rbd), _p(contact), _p(effort), _p(cmd), _p(kind), _p(n_target), _p(target_times), _p(target_states), _p(time),
+                   _p(status), _p(rbd_est), _p(acc), stream)
+
+    def metrics_close(self, mask, end, episode, acc, out, status):
+        """Host variant of metrics_close_dev on copies of acc, out [B, E, METRICS] and status [B] → dict(acc, out, status)."""
+        B = self.batch; out = _f64(out).copy()
+        if out.ndim != 3 or out.shape[0] != B or out.shape[2] != _lib.METRICS:
+            raise ValueError("expected out of shape (%d, E, %d), got %s" % (B, _lib.METRICS, out.shape))
+        acc = _f64(acc, (B, _lib.METRICS_ACC)).copy(); status = _i32(status, (B,)).copy()
+        mask, end, episode = (_i32(np.broadcast_to(np.asarray(a), (B,)), (B,)) for a in (mask, end, episode))
+        self._call("metrics_close", _p(mask), _p(end), _p(episode), out.shape[1], _p(acc), _p(out), _p(status))
+        return dict(acc=acc, out=out, status=status)
+
+    def metrics_close_dev(self, mask, end, episode, acc, out, status, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) closes its episode: the row of its accumulator acc [B, METRICS_ACC], with end[b] (0 run
+        end, 1 fall, 2 episode length limit) as column 1, goes to out[b, episode[b]] (out float64 [B, E, METRICS]) and the accumulator is zeroed.  An
+        episode index outside [0, E) writes no row and ORs QMB200_ST_OVERFLOW into status[b]; a masked end outside {0, 1, 2} leaves the robot unwritten.
+        One launch, no synchronisation."""
+        if out.dim() != 3 or out.shape[0] != self.batch or out.shape[2] != _lib.METRICS:
+            raise ValueError("expected out of shape (%d, E, %d), got %s" % (self.batch, _lib.METRICS, tuple(out.shape)))
+        self._call("metrics_close_dev", _p(mask), _p(end), _p(episode), int(out.shape[1]), _p(acc), _p(out), _p(status), stream)
+
     # ---------------- device gait schedule (include/qmb200.h: qmb200_gait_dev_*; DESIGN.md §4.7) ----------------
     def gait_dev_set_templates(self, names=None, gait_file=None):
         """Load the template table: names (default: every template of the gait file, in the order of its list) → the names, a template's id being its

@@ -707,6 +707,78 @@ def respawn_main(args, episode_run_s=5.0):
                       "per_call": respawn_times(solver, xy)}))
 
 
+def metrics_times(solver, xy_yaw, reps=7, calls=20):
+    """Device time per metrics sample (metrics_step_dev), per close of every robot (metrics_close_dev) and per 1 ms plant step of the whole batch,
+    alternated `reps` times in blocks of `calls` from one standing state with a cmd_vel target (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    q0, v0 = solver.sim_standing_state(xy_yaw)
+    q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream); torch.cuda.synchronize(dev)
+    x = torch.as_tensor(solver.centroidal_state_from_rbd(rbd.cpu().numpy()), device=dev); t_obs = torch.full((B,), 10.0, dtype=torch.float64, device=dev)
+    cmd = torch.zeros((B, 7), dtype=torch.float64, device=dev); cmd[:, 0] = 0.3; last_ee = torch.as_tensor(solver.initial_ee_target(), device=dev)
+    n_target = torch.zeros(B, dtype=torch.int32, device=dev); tt = torch.zeros((B, _lib.KMAX), dtype=torch.float64, device=dev)
+    ts = torch.zeros((B, _lib.KMAX, _lib.TARGET), dtype=torch.float64, device=dev)
+    solver.target_trajectories_dev(0, cmd, t_obs, x, rbd[:, 48:55].contiguous(), last_ee, n_target, tt, ts, s.cuda_stream)
+    acc = torch.zeros((B, _lib.METRICS_ACC), dtype=torch.float64, device=dev); out = torch.zeros((B, 1, _lib.METRICS), dtype=torch.float64, device=dev)
+    every, zero = torch.ones_like(contact), torch.zeros_like(contact)
+    calls_of = {"metrics_step": lambda: solver.metrics_step_dev(1e-3, rbd, contact, eff, cmd, n_target, tt, ts, t_obs, st, acc, stream=s.cuda_stream),
+                "metrics_close_all": lambda: solver.metrics_close_dev(every, zero, zero, acc, out, st, s.cuda_stream),
+                "plant": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    for rep in range(reps + 1):   # the first round warms up
+        for mode, call in calls_of.items():
+            torch.cuda.synchronize(dev)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+            for _ in range(calls):
+                call()
+            b.record(s); torch.cuda.synchronize(dev)
+            if rep:
+                times[mode].append(a.elapsed_time(b) / calls)
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}, "spread_metrics_step": [float(min(times["metrics_step"])), float(max(times["metrics_step"]))]}
+
+
+def metrics_main(args, episode_run_s=3.0):
+    """--metrics: the wall time per simulated second of --duration runs of --gait at --vx on the plant's truth with and without metrics, alternated three
+    times after one warm-up run of each; the per-call device times; and the medians of every column over the complete episodes (closed by a respawn) of
+    an episode_run_s run on the state estimate with the reference IMU noise, respawn (0.1 s fallen, or 1 s) and RANDOMIZE's plant per episode."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch
+    solver = q.Solver(batch=B, device=0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    kw = dict(gait=args.gait, cmd_vel=(args.vx, 0.0, 0.0, 0.0), xy_yaw=xy)
+
+    def timed(duration, **extra):
+        solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+        r = closed_loop.run(solver, duration=duration, **kw, **extra)
+        torch.cuda.synchronize(dev)
+        return r, (time.perf_counter() - t0) / duration
+    wall = {"without_metrics": [], "with_metrics": []}
+    for rep in range(4):   # the first round warms up
+        for name, extra in (("without_metrics", {}), ("with_metrics", dict(metrics=True))):
+            _, w = timed(args.duration, **extra)
+            if rep:
+                wall[name].append(w)
+    r, _ = timed(episode_run_s, metrics=True, state_estimator=True, sensor_noise="reference", respawn=dict(hold=0.1, every=1.0), randomize=RANDOMIZE)
+    M = r["episode_metrics"]; done = M[..., 1] > 0
+    name, limit = card()
+    print(json.dumps({"metric": "metrics", "gpu": name, "power_limit": limit, "batch": B,
+                      "wall_s_per_sim_s": {"label": "%s at %.2f m/s on the plant's truth, runs of %.1f s, three alternated pairs after a warm-up pair"
+                                                    % (args.gait, args.vx, args.duration), **wall},
+                      "per_call": metrics_times(solver, xy),
+                      "episodes": {"label": "%s at %.2f m/s on the state estimate, reference IMU noise; respawn after 0.1 s fallen or 1 s; RANDOMIZE per episode; "
+                                            "%.1f s; medians over the episodes a respawn closed" % (args.gait, args.vx, episode_run_s),
+                                   "complete": int(done.sum()), "fell": int(np.sum(M[..., 1] == 1)),
+                                   "median": {c: float(np.nanmedian(M[..., i][done])) for i, c in enumerate(r["metrics_layout"]) if c not in ("end", "status")}}}))
+
+
 def watch_state_est(solver):
     """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
     error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
@@ -748,7 +820,10 @@ def main():
     ap.add_argument("--respawn", action="store_true", help="restart robots that fell (hold 0.1 s) on the reference IMU noise without the attitude filter: episode rates")
     ap.add_argument("--randomize", action="store_true", help="with --respawn: a new plant per episode (friction, payload, push): falls per friction x push bin")
     ap.add_argument("--spawn", action="store_true", help="with --respawn: new ground per episode (tile, offset, yaw): falls per tile x heading bin")
+    ap.add_argument("--metrics", action="store_true", help="per-episode metrics: wall time with and without them, per-call times, column medians of a respawn run")
     args = ap.parse_args()
+    if args.metrics:
+        return metrics_main(args)
     if args.randomize and not args.respawn:
         ap.error("--randomize needs --respawn")
     if args.spawn and not args.respawn:
