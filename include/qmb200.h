@@ -294,6 +294,11 @@ int qmb200_gait_dev_step_ee_dev(qmb200_handle* h, const double* t_obs, int32_t* 
  * template and cursor.  Any output may be NULL. */
 int qmb200_gait_dev_get(qmb200_handle* h, int32_t* n_events /*[B]*/, double* event_times /*[B][QMB200_GAIT_CAP]*/, int32_t* mode_sequence /*[B][QMB200_GAIT_CAP+1]*/,
                         int32_t* tmpl /*[B]*/, int32_t* cursor /*[B]*/);
+/* Synchronous: the loaded command timeline (qmb200_gait_dev_set_commands(_ee), qmb200_timeline_sample_dev): n_cmd, and t [B][n_cmd], tmpl [B][n_cmd],
+ * cmd_vel [B][n_cmd][4], ee_kind [B][n_cmd] and ee_cmd [B][n_cmd][7] in the layouts qmb200_gait_dev_set_commands_ee takes (ee_kind -1 and ee_cmd zeros
+ * when the timeline has no end-effector rows).  Any output may be NULL: a call with n_cmd alone sizes the others.  Fails while the schedule is not running. */
+int qmb200_gait_dev_get_commands(qmb200_handle* h, int32_t* n_cmd, double* t /*[B][n_cmd]*/, int32_t* tmpl /*[B][n_cmd]*/, double* cmd_vel /*[B][n_cmd][4]*/,
+                                 int32_t* ee_kind /*[B][n_cmd]*/, double* ee_cmd /*[B][n_cmd][7]*/);
 /* Releases the schedules and the timeline; the template table stays.  Step and get fail until the next reset.  Stopping a schedule that is not
  * running does nothing and returns 0. */
 int qmb200_gait_dev_stop(qmb200_handle* h);
@@ -697,6 +702,46 @@ int qmb200_metrics_close(qmb200_handle* h, const int32_t* mask /*[B]*/, const in
                          double* acc /*[B][QMB200_METRICS_ACC] in-out*/, double* out /*[B][n_episodes][QMB200_METRICS] in-out*/, int32_t* status /*[B] in-out*/);
 int qmb200_metrics_close_dev(qmb200_handle* h, const int32_t* mask, const int32_t* end, const int32_t* episode, int32_t n_episodes, double* acc, double* out,
                              int32_t* status, void* cuda_stream);
+
+/* ---- per-episode command timelines (DESIGN.md §4.14): each episode of each robot gets a new command timeline, drawn on the device right after its
+ *      restart into the device gait schedule's timeline, which the gait step then consumes as it consumes a loaded one.
+ *   ranges row[QMB200_TIMELINE]  0      t_first      slot 0's time on the robot's observation clock (s)
+ *                                1      gap          time from slot j - 1 to slot j (s), lo >= 0
+ *                                2      p_gait       probability that a slot inserts a gait; fixed (lo == hi), in [0, 1]
+ *                                3      gait_set     bitmask of the templates a gait slot picks among; fixed, an integer in [0, 2^32), non-zero when p_gait > 0
+ *                                4-7    w_none, w_cmd_vel, w_ee_cmd_vel, w_ee_goal   weights of the slot's target command; fixed, >= 0, positive sum
+ *                                8-11   cmd_vel_x, cmd_vel_y, cmd_vel_z, cmd_yaw_rate   base frame
+ *                                12-14  ee_vx, ee_vy, ee_vz   end-effector velocity, world frame
+ *                                15-17  ee_x, ee_y, ee_z      goal position, world frame
+ *                                18-21  ee_qx, ee_qy, ee_qz, ee_qw   goal orientation; fixed, unit norm within 1e-9
+ *   drawn slot[QMB200_TIMELINE_CMD]  t, tmpl (-1 or a template id), cmd_vel[4] (the quiet NaN 0x7FF8000000000000 unless the kind is cmd_vel), ee_kind (-1,
+ *                                QMB200_TARGET_EE_CMD_VEL or QMB200_TARGET_EE_GOAL), ee[7] (zeros; (v, 0, 0, 0, 0) for ee_cmd_vel; position and quaternion for a goal):
+ *                                one command of qmb200_gait_dev_set_commands_ee.
+ * Every draw of slot j is u = the keyed uniform of the episode draws on a domain constant of its own over (seed, global robot rank * B + b, e, 16 j + c); a box
+ * column is fma(u, hi - lo, lo), a fixed column lo itself, byte for byte.  t_0 = draw(t_first) on channel 0, t_j = t_{j-1} + draw(gap) on channel 16 j;
+ * c = 1: a gait is inserted when u < p_gait; c = 2: the template is the k-th set bit of gait_set in increasing bit order, k = min(floor(u popcount),
+ * popcount - 1); c = 3: the kind is the first of (none, cmd_vel, ee_cmd_vel, ee_goal) whose running sum of weights exceeds u W, W their sum in that order
+ * (else the last with a positive weight); c = 4-7 cmd_vel; c = 8-10 the end-effector velocity; c = 11-13 the goal position. */
+#define QMB200_TIMELINE 22
+#define QMB200_TIMELINE_CMD 14
+/* Per-robot ranges lo, hi [B][QMB200_TIMELINE], n_cmd (>= 1) slots per episode and the seed.  NULL lo and hi clear them.  Rejects a non-finite bound,
+ * lo > hi, a non-finite hi - lo and the column rules above, naming the field and the robot; on rejection the stored ranges stay unchanged.  Host arrays;
+ * synchronous. */
+int qmb200_timeline_set_ranges(qmb200_handle* h, int32_t n_cmd, const double* lo /*[B][QMB200_TIMELINE] or NULL*/, const double* hi /*[B][QMB200_TIMELINE] or NULL*/,
+                               int64_t seed);
+/* The stored n_cmd, ranges and seed (zeros when none are set); is_set = 1 when ranges are set.  Any output may be NULL. */
+int qmb200_timeline_get_ranges(const qmb200_handle* h, int32_t* n_cmd, double* lo /*[B][QMB200_TIMELINE]*/, double* hi /*[B][QMB200_TIMELINE]*/, int64_t* seed,
+                               int32_t* is_set);
+/* One launch, no host work: every robot with mask[b] != 0 draws episode[b]'s n_cmd slots into rows[b] and into the device gait schedule's timeline that
+ * qmb200_gait_dev_set_commands(_ee) loaded (its time, template, cmd_vel and, when it has them, end-effector rows), and its cursor goes back to 0.  Robots
+ * with mask[b] == 0 are not written.  Fails, writing nothing, when no ranges are set, the device gait schedule is not running, the loaded timeline's width
+ * differs from n_cmd, a robot weighs an end-effector kind and the timeline has no end-effector rows, or a gait_set bit lies at or above the template
+ * table's size. */
+int qmb200_timeline_sample(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* episode /*[B]*/, double* rows /*[B][n_cmd][QMB200_TIMELINE_CMD] in-out*/);
+int qmb200_timeline_sample_dev(qmb200_handle* h, const int32_t* mask, const int32_t* episode, double* rows, void* cuda_stream);
+/* Host only: the slots [n][n_cmd][QMB200_TIMELINE_CMD] of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the
+ * sampler draws. */
+int qmb200_timeline_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][n_cmd][QMB200_TIMELINE_CMD]*/);
 
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */

@@ -101,6 +101,12 @@ METRICS_LAYOUT = ("duration", "end", "status", "distance", "path_length", "min_h
                   "ee_pos_err_max", "ee_ori_err_rms", "energy", "torque_rms", "slip", "touchdowns", "est_pos_err_rms", "est_vel_err_rms")
 METRICS = len(METRICS_LAYOUT)   # QMB200_METRICS
 METRICS_ACC = 32                # QMB200_METRICS_ACC
+# one episode's command timeline (qmb200_timeline_*): the columns of a ranges row of TIMELINE doubles, and of a drawn slot of TIMELINE_CMD doubles
+TIMELINE_LAYOUT = ("t_first", "gap", "p_gait", "gait_set", "w_none", "w_cmd_vel", "w_ee_cmd_vel", "w_ee_goal", "cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate",
+                   "ee_vx", "ee_vy", "ee_vz", "ee_x", "ee_y", "ee_z", "ee_qx", "ee_qy", "ee_qz", "ee_qw")
+TIMELINE = len(TIMELINE_LAYOUT)   # QMB200_TIMELINE
+TIMELINE_CMD_LAYOUT = ("t", "tmpl", "cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate", "ee_kind") + tuple("ee_%d" % i for i in range(7))
+TIMELINE_CMD = len(TIMELINE_CMD_LAYOUT)   # QMB200_TIMELINE_CMD
 
 
 # every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
@@ -160,6 +166,7 @@ PROTOTYPES = {
     "qmb200_gait_dev_step_ee": (I32, [P] * 10),
     "qmb200_gait_dev_step_ee_dev": (I32, [P] * 11),
     "qmb200_gait_dev_get": (I32, [P] * 6),
+    "qmb200_gait_dev_get_commands": (I32, [P] * 7),
     "qmb200_gait_dev_stop": (I32, [P]),
     "qmb200_observation_update": (I32, [P] * 5),
     "qmb200_observation_update_dev": (I32, [P] * 6),
@@ -234,6 +241,11 @@ PROTOTYPES = {
     "qmb200_metrics_step_dev": (I32, [P, D] + [P] * 13),
     "qmb200_metrics_close": (I32, [P] * 4 + [I32] + [P] * 3),
     "qmb200_metrics_close_dev": (I32, [P] * 4 + [I32] + [P] * 4),
+    "qmb200_timeline_set_ranges": (I32, [P, I32, P, P, I64]),
+    "qmb200_timeline_get_ranges": (I32, [P] * 6),
+    "qmb200_timeline_sample": (I32, [P] * 4),
+    "qmb200_timeline_sample_dev": (I32, [P] * 5),
+    "qmb200_timeline_draw": (I32, [P, I32, P, P, P]),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

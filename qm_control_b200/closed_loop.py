@@ -55,7 +55,8 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
-        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None):
+        attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None,
+        timeline=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -150,7 +151,19 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     robot's accumulator.  A respawning robot's episode closes right before its restore (end 1 when the fall rule restarted it, 2 when every did), and
     every robot's open episode closes when the loop ends (end 0).  The samples only read the loop's tensors, so every other output is unchanged.
     Returns also episode_metrics[B, E, METRICS] in the columns of metrics_layout (_lib.METRICS_LAYOUT), E as for episode_params, NaN rows where a
-    robot had no episode e."""
+    robot had no episode e.
+    timeline: dict(seed=0, n, t_first=(lo, hi), gap=(lo, hi), p_gait=0, gaits=[names], weights=dict(none, cmd_vel, ee_cmd_vel, ee_goal), <box>=(lo, hi),
+    ee_quat) draws a new command timeline of n slots for every episode (DESIGN.md §4.14), in place of commands: slot 0 at t_first s after the start, each
+    later one gap s after the one before; each slot inserts a gait with probability p_gait, picked uniformly among gaits (qm_gait.info names: one list, or
+    B lists), and carries one target command, none, cmd_vel, ee_cmd_vel or ee_goal, with probability proportional to its weight (missing weights are 0;
+    default none=1).  The box columns are cmd_vel_x, cmd_vel_y, cmd_vel_z, cmd_yaw_rate (a column not named stays at the run's cmd_vel), ee_vx, ee_vy,
+    ee_vz and ee_x, ee_y, ee_z (world frame; named when their kind's weight is positive), ee_quat the goal's quaternion xyzw [4] or [B, 4] (with ee_goal).
+    Every bound, p_gait and weight is a scalar or [B].  The run rolls the gait on the device as with commands (gait is the start gait, the same record
+    and outputs): it loads a placeholder timeline of width n and every episode, the first included, draws its slots on the device
+    (Solver.timeline_sample_dev) right after its restore, its randomize draw and its spawn, before its first solve.  With randomize cmd_vel fields the
+    episode's drawn cmd_vel applies from its start, and the timeline's cmd_vel slots replace it as they fall due.  ee_goal / ee_cmd_vel weights cannot
+    go with a drawn spawn yaw.  The previous ranges are restored when run returns.  Returns also timeline_params[B, E, n, TIMELINE_CMD], the slots of
+    each episode (_lib.TIMELINE_CMD_LAYOUT, t in s after the episode's start), E and the NaN rows as for episode_params."""
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else _respawn_spec(respawn)
@@ -178,6 +191,9 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     if slip_detector is not None and state_estimator is None:
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     gd = None if commands is None else _gait_commands(solver.batch, gait, commands)
+    tl = None if timeline is None else _timeline_spec(getattr(solver, "batch", None), gait, timeline, commands)
+    if tl is not None:
+        gd = tl["gd"]
     tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
     sp = None if spawn is None else _spawn_spec(getattr(solver, "batch", None), spawn, terrain, ground_map, gd)
     if rz is not None:   # the links: a drawn payload / friction also goes where the run told the controller the plant's
@@ -211,13 +227,15 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_robot_params(solver, friction_mu, payload))
         if rz is not None:
             scope.enter_context(_ranges(solver, "episode"))
+        if tl is not None:
+            scope.enter_context(_ranges(solver, "timeline"))
         if gd is not None:
             scope.enter_context(_gait_dev(solver, gd))
         if rs is not None:
             scope.callback(solver.robot_image_clear)
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp, mt=metrics is not None)
+                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp, mt=metrics is not None, tl=tl)
 
 
 def _respawn_spec(respawn):
@@ -316,7 +334,7 @@ def _spawn_spec(B, spawn, terrain, ground_map, gd):
 
 @contextlib.contextmanager
 def _ranges(solver, kind):
-    """the ranges of solver's kind ("episode" or "spawn") draws in force, set again on exit"""
+    """the ranges of solver's kind ("episode", "spawn" or "timeline") draws in force, set again on exit"""
     prev = getattr(solver, kind + "_get_ranges")()
     try:
         yield   # _run sets this run's ranges once it has read its fixed values
@@ -387,6 +405,76 @@ def _ee_commands(B, C, commands, vel):
     kind = np.where(has_goal, _lib.TARGET_EE_GOAL, np.where(has_eev, _lib.TARGET_EE_CMD_VEL, -1)).astype(np.int32)
     cmd = np.where(has_goal[..., None], goal, 0.0); cmd[..., :3] = np.where(has_eev[..., None], eev, cmd[..., :3])
     return dict(ee_kind=kind, ee_cmd=cmd)
+
+
+TIMELINE_BOX = ("t_first", "gap", "cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate", "ee_vx", "ee_vy", "ee_vz", "ee_x", "ee_y", "ee_z")
+TIMELINE_KINDS = ("none", "cmd_vel", "ee_cmd_vel", "ee_goal")
+
+
+def _timeline_spec(B, gait, timeline, commands):
+    """closed_loop.run's gait and timeline → dict(seed, n, fields: name -> (lo, hi) float arrays, scalar or [B], p_gait, gait_set, weights [4] or [B, 4],
+    quat [4] or [B, 4], gd: the placeholder timeline as _gait_commands gives it); ValueError when malformed.  B None: the lengths are not checked."""
+    if commands is not None:
+        raise ValueError("closed_loop.run: timeline and commands cannot go together (both set the device gait schedule's timeline)")
+    if not isinstance(timeline, dict):
+        raise ValueError("closed_loop.run: timeline must be None or dict(seed, n, t_first, gap, p_gait, gaits, weights, <field>=(lo, hi), ee_quat), got %r" % (timeline,))
+    n = timeline.get("n")
+    if isinstance(n, (bool, np.bool_)) or not isinstance(n, (int, np.integer)) or n < 1:
+        raise ValueError("closed_loop.run: timeline n must be an integer >= 1, got %r" % (n,))
+    seed, fields = _ranges_spec("timeline", TIMELINE_BOX, B, {k: v for k, v in timeline.items() if k not in ("n", "p_gait", "gaits", "weights", "ee_quat")})
+    for k in ("t_first", "gap"):
+        if k not in fields:
+            raise ValueError("closed_loop.run: timeline needs %s=(lo, hi)" % k)
+    if not np.all(fields["gap"][0] >= 0.0):
+        raise ValueError("closed_loop.run: timeline gap lo must be >= 0")
+
+    def per_robot(name, v, width=None):
+        a = np.asarray(v, dtype=np.float64) if not isinstance(v, (str, bool, np.bool_)) else np.array(np.nan)
+        ok = ((width,),) if width else ((),)
+        if a.shape not in ok and not (a.ndim == (2 if width else 1) and (B is None or a.shape[0] == B) and (not width or a.shape[1] == width)):
+            raise ValueError("closed_loop.run: timeline %s must be %s or [%s%s], got shape %s" % (name, "[%d]" % width if width else "a scalar", "B" if B is None else B,
+                                                                                           ", %d" % width if width else "", a.shape))
+        if not np.all(np.isfinite(a)):
+            raise ValueError("closed_loop.run: timeline %s must be finite, got %r" % (name, v))
+        return a
+    p_gait = per_robot("p_gait", timeline.get("p_gait", 0.0))
+    if not np.all((p_gait >= 0.0) & (p_gait <= 1.0)):
+        raise ValueError("closed_loop.run: timeline p_gait must lie in [0, 1]")
+    names = gait_template_names(); ids = {nm: i for i, nm in enumerate(names)}
+    start = [gait] * (1 if B is None else B) if isinstance(gait, str) else list(gait)
+    if B is not None and len(start) != B:
+        raise ValueError("closed_loop.run: gait must be one name or a sequence of %d names, got %d" % (B, len(start)))
+    gaits = timeline.get("gaits", [])
+    sets = [gaits] if all(isinstance(g, str) for g in gaits) else list(gaits)
+    if any(isinstance(g, str) or not all(isinstance(x, str) for x in g) for g in sets) or (len(sets) != 1 and B is not None and len(sets) != B):
+        raise ValueError("closed_loop.run: timeline gaits must be one list of gait names or %s such lists, got %r" % ("B" if B is None else B, gaits))
+    unknown = sorted({str(x) for x in start + [x for g in sets for x in g] if x not in ids})
+    if unknown:
+        raise ValueError("closed_loop.run: unknown gait name(s) %s (qm_gait.info has %s)" % (", ".join(unknown), ", ".join(names)))
+    gait_set = np.array([float(sum(1 << ids[x] for x in set(g))) for g in sets]); gait_set = gait_set[0] if len(sets) == 1 else gait_set
+    if np.any((p_gait > 0.0) & (gait_set == 0.0)):
+        raise ValueError("closed_loop.run: timeline gaits must name at least one gait where p_gait > 0")
+    w = timeline.get("weights", dict(none=1.0))
+    if not isinstance(w, dict) or not set(w) <= set(TIMELINE_KINDS):
+        raise ValueError("closed_loop.run: timeline weights must be dict(%s), got %r" % (", ".join(TIMELINE_KINDS), w))
+    weights = np.stack(np.broadcast_arrays(*(per_robot("weight " + k, w.get(k, 0.0)) for k in TIMELINE_KINDS)), axis=-1)
+    if np.any(weights < 0.0) or not np.all(weights.sum(-1) > 0.0):
+        raise ValueError("closed_loop.run: timeline weights must be >= 0 with a positive sum")
+    need = [(k, c) for k, cols in (("ee_cmd_vel", ("ee_vx", "ee_vy", "ee_vz")), ("ee_goal", ("ee_x", "ee_y", "ee_z"))) for c in cols
+            if np.any(weights[..., TIMELINE_KINDS.index(k)] > 0.0) and c not in fields]
+    if need:
+        raise ValueError("closed_loop.run: timeline %s needs %s=(lo, hi) (its weight is positive)" % (need[0][0], need[0][1]))
+    goal = np.any(weights[..., 3] > 0.0)
+    if goal and timeline.get("ee_quat") is None:
+        raise ValueError("closed_loop.run: timeline ee_goal needs ee_quat (its weight is positive)")
+    quat = per_robot("ee_quat", timeline.get("ee_quat", (0.0, 0.0, 0.0, 1.0)), 4)
+    if np.any(np.abs(np.linalg.norm(quat, axis=-1) - 1.0) > 1e-9):
+        raise ValueError("closed_loop.run: timeline ee_quat (xyzw) must have unit norm (within 1e-9)")
+    Bn = len(start)   # the placeholder timeline the sampler writes into: +inf times, no command
+    ee = {} if not np.any(weights[..., 2:] > 0.0) else dict(ee_kind=np.full((Bn, n), -1, dtype=np.int32), ee_cmd=np.zeros((Bn, n, 7)))
+    gd = dict(names=names, gait=np.array([ids[x] for x in start], dtype=np.int32), t=np.full((Bn, n), np.inf), tmpl=np.full((Bn, n), -1, dtype=np.int32),
+              cmd_vel=np.full((Bn, n, 4), np.nan), ee=ee)
+    return dict(seed=seed, n=int(n), fields=fields, p_gait=p_gait, gait_set=gait_set, weights=weights, quat=quat, gd=gd)
 
 
 @contextlib.contextmanager
@@ -551,7 +639,7 @@ def _metrics_episodes(ticks, rs):
 
 
 def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
-         rs=None, rz=None, sp=None, mt=False):
+         rs=None, rz=None, sp=None, mt=False, tl=None):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -583,6 +671,15 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)   # the same heading within [-pi, pi]
         row = np.zeros((B, _lib.SPAWN)); row[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; row[:, SP["yaw"]] = yaw
         _set_ranges(solver, "spawn", _lib.SPAWN_LAYOUT, row, sp)
+    if tl is not None:   # the ranges: the fixed columns, the run's cmd_vel where not named, the named columns' bounds; times on the observation clock
+        TL = {n: i for i, n in enumerate(_lib.TIMELINE_LAYOUT)}
+        row = np.zeros((B, _lib.TIMELINE)); row[:, TL["p_gait"]] = tl["p_gait"]; row[:, TL["gait_set"]] = tl["gait_set"]
+        row[:, TL["w_none"]:TL["w_none"] + 4] = tl["weights"]; row[:, TL["cmd_vel_x"]:TL["cmd_vel_x"] + 4] = cmd_vel; row[:, TL["ee_qx"]:TL["ee_qx"] + 4] = tl["quat"]
+        lo = row.copy(); hi = row.copy()
+        for k, (l, h) in tl["fields"].items():
+            lo[:, TL[k]] = l; hi[:, TL[k]] = h
+        lo[:, TL["t_first"]] += t_start; hi[:, TL["t_first"]] += t_start
+        solver.timeline_set_ranges(tl["n"], lo, hi, tl["seed"])
     stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
     f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
     i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
@@ -700,11 +797,13 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         k0.copy_(torch.where(m, k, k0)); episode.add_(due); fall_count.masked_fill_(m, 0)
         begin(due, episode)
 
-    def begin(mask, idx):   # the masked robots begin episode idx: their plant's draw, then their spawn
+    def begin(mask, idx):   # the masked robots begin episode idx: their plant's draw, then their spawn, then their command timeline
         if rz is not None:
             draw(mask, idx)
         if sp is not None:
             stand(mask, idx)
+        if tl is not None:
+            solver.timeline_sample_dev(mask, idx, tl_rows, s)
 
     def draw(mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
         solver.episode_sample_dev(mask, idx, ep_rows, rz["link"], s)
@@ -718,10 +817,11 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
     def stand(mask, idx):   # the masked robots spawn episode idx: new ground under them, their start state there
         solver.spawn_sample_dev(mask, idx, sp_rows, q, v, rbd, contact, x_obs, last_ee, rbd_est if se else None, sp["link"], s)
 
-    if rz is not None or sp is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
+    if rz is not None or sp is not None or tl is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
         with torch.cuda.stream(stream):
             ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev) if rz is not None else None
             sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev) if sp is not None else None
+            tl_rows = torch.zeros((B, tl["n"], _lib.TIMELINE_CMD), dtype=torch.float64, device=dev) if tl is not None else None
             if rs is None:
                 begin(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
             else:
@@ -804,13 +904,15 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                    ee_target=rec_ee_target.cpu().numpy())
     if rs is not None:
         out.update(episode=rec_episode.cpu().numpy(), fallen=rec_fallen.cpu().numpy())
-    if rz is not None or sp is not None:   # rebuilt on the host from the episode record: the samplers' rows are pure functions of (ranges, seed, robot, episode)
+    if rz is not None or sp is not None or tl is not None:   # rebuilt on the host from the episode record: the samplers' rows are pure functions of (ranges, seed, robot, episode)
         ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
         had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
         rb, re_ = np.nonzero(had)
-        for kind, spec, width in (("episode", rz, _lib.EPISODE), ("spawn", sp, _lib.SPAWN)):
+        for kind, spec, shape in (("episode", rz, (_lib.EPISODE,)), ("spawn", sp, (_lib.SPAWN,)), ("timeline", tl, (0 if tl is None else tl["n"], _lib.TIMELINE_CMD))):
             if spec is not None:
-                out[kind + "_params"] = np.full(had.shape + (width,), np.nan); out[kind + "_params"][rb, re_] = getattr(solver, kind + "_draw")(rb, re_)
+                out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = getattr(solver, kind + "_draw")(rb, re_)
+        if tl is not None:   # on the episode's clock: exact for drawn times in [t_start / 2, 2 t_start]
+            out["timeline_params"][..., 0] -= t_start
     if mt:   # trimmed to the most episodes of any robot
         E = int(out["episode"].max()) + 1 if rs is not None else 1
         out.update(episode_metrics=mt_out[:, :E].cpu().numpy(), metrics_layout=_lib.METRICS_LAYOUT)

@@ -23,6 +23,7 @@
 #include "kernels/episode_api.cuh"
 #include "kernels/spawn_api.cuh"
 #include "kernels/metrics_api.cuh"
+#include "kernels/timeline_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -43,7 +44,7 @@ struct RobotArray {
   const double* dev() const { return host.empty() ? nullptr : d; }
 };
 
-// Per-robot ranges of a per-episode draw (capi_episode.inc, capi_spawn.inc): lo, hi [B][width] (empty: none set), their device copies (dalloc: freed
+// Per-robot ranges of a per-episode draw (capi_episode.inc, capi_spawn.inc, capi_timeline.inc): lo, hi [B][width] (empty: none set), their device copies (dalloc: freed
 // with allocs) and the seed
 struct DrawRanges {
   int width; std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0;
@@ -99,6 +100,10 @@ struct qmb200_handle {
                                       // standing pose's joints [NJ]; terrain: the plant had robot terrain rows at the set
     double *d_origin = nullptr, *d_qj = nullptr; bool terrain = false;
   } spawn{{SP_DBL}};
+  struct TimelineRanges : DrawRanges {   // per-episode command timelines (capi_timeline.inc): slots per episode, and what the sampler's checks read of the
+                                         // ranges: whether any robot weighs an end-effector kind, one past the highest gait_set bit
+    int n_cmd = 0; bool ee = false; int gait_bits = 0;
+  } timeline{{TL_DBL}};
   uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
   struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
     bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
@@ -294,7 +299,7 @@ int model_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb
 int plant_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->plant_on_device, {&h->mu, &h->payload}); }
 int tuning_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->tuning_on_device, {&h->tuning}); }
 int terrain_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->terrain_on_device, {&h->terrain, &h->se_ground}); }
-// The ranged draws' set / get / draw path (qmb200_<kind>_set_ranges, _get_ranges, _draw; kind: "episode" or "spawn").
+// The ranged draws' set / get / draw path (qmb200_<kind>_set_ranges, _get_ranges, _draw; kind: "episode", "spawn" or "timeline").
 // Set: NULL lo and hi clear the ranges once no queued draw reads them; else error() checks them ("" when valid), the device copies are allocated, then
 // prepare() makes sure the rows the sampler writes exist (it may fail, leaving the ranges as they were), and the ranges are copied and stored.
 template <class Error, class Prepare>
@@ -326,9 +331,9 @@ int ranges_get(const qmb200_handle* h, const DrawRanges& r, double* lo, double* 
 int no_ranges(qmb200_handle* h, const char* who, const char* kind) {
   return fail(h, std::string(who) + ": no ranges are set (qmb200_" + kind + "_set_ranges sets them)");
 }
-// The rows [n][width] robots robot [n] draw in episodes episode [n] on the stored ranges, each row(lo, hi, seed, global robot, episode, out) on the host
-int ranges_draw(qmb200_handle* h, const DrawRanges& r, const char* kind, int32_t n, const int32_t* robot, const int32_t* episode, double* rows,
-                void (*row)(const double*, const double*, uint64_t, uint64_t, uint64_t, double*)) {
+// The rows [n][out_width] robots robot [n] draw in episodes episode [n] on the stored ranges, each row(lo, hi, seed, global robot, episode, out) on the host
+template <class Row>
+int ranges_draw(qmb200_handle* h, const DrawRanges& r, const char* kind, int32_t n, const int32_t* robot, const int32_t* episode, double* rows, size_t out_width, Row row) {
   const std::string who = std::string("qmb200_") + kind + "_draw";
   if (n < 0 || (n > 0 && (!robot || !episode || !rows))) return fail(h, who + ": n must be >= 0 and the buffers non-null");
   if (r.lo.empty()) return no_ranges(h, who.c_str(), kind);
@@ -336,7 +341,7 @@ int ranges_draw(qmb200_handle* h, const DrawRanges& r, const char* kind, int32_t
   const int64_t robot0 = (int64_t)h->comm_rank * h->B;
   for (int32_t i = 0; i < n; ++i) {
     const size_t b = (size_t)robot[i];
-    row(r.lo.data() + b * r.width, r.hi.data() + b * r.width, r.seed, (uint64_t)(robot0 + robot[i]), (uint64_t)(int64_t)episode[i], rows + (size_t)i * r.width);
+    row(r.lo.data() + b * r.width, r.hi.data() + b * r.width, r.seed, (uint64_t)(robot0 + robot[i]), (uint64_t)(int64_t)episode[i], rows + (size_t)i * out_width);
   }
   return 0;
 }
@@ -511,3 +516,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_episode.inc"
 #include "capi_spawn.inc"
 #include "capi_metrics.inc"
+#include "capi_timeline.inc"

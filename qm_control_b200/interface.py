@@ -782,6 +782,45 @@ class Solver:
         """Host only: robot [n] (in [0, B)), episode [n] → the spawn rows [n, SPAWN] the sampler draws for them on the stored ranges and seed."""
         return self._ranges_draw("spawn", _lib.SPAWN, robot, episode)
 
+    # ---------------- per-episode command timelines (include/qmb200.h: qmb200_timeline_*; DESIGN.md §4.14) ----------------
+    def timeline_set_ranges(self, n=None, lo=None, hi=None, seed=0):
+        """Per-robot ranges lo, hi [B, TIMELINE] (columns _lib.TIMELINE_LAYOUT) of n slots per episode and a 64-bit seed of the per-episode timelines;
+        None clears them.  Synchronous."""
+        if lo is None and hi is None:
+            self._call("timeline_set_ranges", 0, None, None, 0); return
+        shape = (self.batch, _lib.TIMELINE); lo = _f64(lo, shape); hi = _f64(hi, shape)
+        s = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._call("timeline_set_ranges", int(n), _p(lo), _p(hi), s - (1 << 64) if s >> 63 else s)
+
+    def timeline_get_ranges(self):
+        """→ dict(n, lo [B, TIMELINE], hi [B, TIMELINE], seed) of the stored ranges, or None when none are set."""
+        lo = np.zeros((self.batch, _lib.TIMELINE)); hi = np.zeros_like(lo); n = C.c_int32(); seed = C.c_int64(); is_set = C.c_int32()
+        self._call("timeline_get_ranges", C.byref(n), _p(lo), _p(hi), C.byref(seed), C.byref(is_set))
+        return dict(n=n.value, lo=lo, hi=hi, seed=seed.value & 0xFFFFFFFFFFFFFFFF) if is_set.value else None
+
+    def _timeline_n(self):
+        n = C.c_int32(); self._call("timeline_get_ranges", C.byref(n), None, None, None, None)
+        return n.value
+
+    def timeline_sample(self, mask, episode, rows=None):
+        """Host variant of timeline_sample_dev: mask [B], episode [B] → rows [B, n, TIMELINE_CMD] (rows of unmasked robots as given, zeros by default)."""
+        B = self.batch; shape = (B, self._timeline_n(), _lib.TIMELINE_CMD)
+        rows = np.zeros(shape) if rows is None else _f64(rows, shape).copy()
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,)); episode = _i32(np.broadcast_to(np.asarray(episode), (B,)), (B,))
+        self._call("timeline_sample", _p(mask), _p(episode), _p(rows))
+        return rows
+
+    def timeline_sample_dev(self, mask, episode, rows, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) draws episode[b]'s n slots (int32 [B]) into rows [B, n, TIMELINE_CMD] (float64 device
+        tensor) and into the device gait schedule's loaded timeline, and its cursor goes back to 0.  One launch, no synchronisation."""
+        self._call("timeline_sample_dev", _p(mask), _p(episode), _p(rows), stream)
+
+    def timeline_draw(self, robot, episode):
+        """Host only: robot [n] (in [0, B)), episode [n] → the slots [n, n_cmd, TIMELINE_CMD] the sampler draws for them on the stored ranges and seed."""
+        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); rows = np.zeros((len(robot), self._timeline_n(), _lib.TIMELINE_CMD))
+        self._call("timeline_draw", len(robot), _p(robot), _p(episode), _p(rows))
+        return rows
+
     # ---------------- per-episode metrics (include/qmb200.h: qmb200_metrics_*; DESIGN.md §4.13) ----------------
     def metrics_step(self, dt, rbd, contact, effort, cmd, n_target, target_times, target_states, time, status, acc, kind=None, rbd_est=None):
         """Host variant of metrics_step_dev on a copy of acc [B, METRICS_ACC] → the accumulator rows after the sample."""
@@ -889,6 +928,15 @@ class Solver:
         n = np.zeros(B, dtype=np.int32); ev = np.zeros((B, cap)); md = np.zeros((B, cap + 1), dtype=np.int32); tm = np.zeros(B, dtype=np.int32); cur = np.zeros(B, dtype=np.int32)
         self._call("gait_dev_get", _p(n), _p(ev), _p(md), _p(tm), _p(cur))
         return dict(n_events=n, event_times=ev, modes=md, tmpl=tm, cursor=cur)
+
+    def gait_dev_get_commands(self):
+        """→ dict(t [B, C], tmpl [B, C], cmd_vel [B, C, 4], ee_kind [B, C], ee_cmd [B, C, 7]) of the loaded command timeline (ee_kind -1 and ee_cmd
+        zeros when it has no end-effector rows).  Synchronous."""
+        n = C.c_int32(); self._call("gait_dev_get_commands", C.byref(n), None, None, None, None, None)
+        B, c = self.batch, n.value
+        out = dict(t=np.zeros((B, c)), tmpl=np.zeros((B, c), dtype=np.int32), cmd_vel=np.zeros((B, c, 4)), ee_kind=np.zeros((B, c), dtype=np.int32), ee_cmd=np.zeros((B, c, 7)))
+        self._call("gait_dev_get_commands", None, *(_p(out[k]) for k in ("t", "tmpl", "cmd_vel", "ee_kind", "ee_cmd")))
+        return out
 
     def gait_dev_stop(self):
         """Release the schedules and the timeline (the template table stays)."""

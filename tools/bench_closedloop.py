@@ -779,6 +779,123 @@ def metrics_main(args, episode_run_s=3.0):
                                    "median": {c: float(np.nanmedian(M[..., i][done])) for i, c in enumerate(r["metrics_layout"]) if c not in ("end", "status")}}}))
 
 
+# A gait slot due at t takes effect at the first MPC tick at or after t, plus the time horizon (GaitReceiver's insertion time) and the transition stance:
+# with the 1 s horizon the first switch starts 1.0-1.4 s into an episode, so the episodes of the per-transition run last TIMELINE_EPISODE_S
+TIMELINE = dict(seed=1, n=3, t_first=(0.0, 0.3), gap=(0.8, 1.2), p_gait=0.5, gaits=["trot", "pace", "static_walk", "standing_trot"],
+                weights=dict(none=1.0, cmd_vel=1.0), cmd_vel_x=(-0.2, 0.6), cmd_yaw_rate=(-0.3, 0.3))
+TIMELINE_EPISODE_S = 3.0
+
+
+def timeline_times(solver, reps=7, calls=20):
+    """Device time per timeline draw of every robot (timeline_sample_dev, TIMELINE's ranges on a loaded placeholder timeline) and per 1 ms plant step of
+    the whole batch, alternated `reps` times in blocks of `calls` (CUDA events) → median ms per call of each."""
+    import torch
+    from qm_control_b200 import closed_loop
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev); n = TIMELINE["n"]
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    q0, v0 = solver.sim_standing_state(xy); q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    tl = closed_loop._timeline_spec(B, "trot", TIMELINE, None); gd = tl["gd"]
+    solver.gait_dev_set_templates(gd["names"]); solver.gait_dev_reset(gd["gait"], np.full(B, 10.0)); solver.gait_dev_set_commands(gd["t"], gd["tmpl"], gd["cmd_vel"])
+    TL = {c: i for i, c in enumerate(_lib.TIMELINE_LAYOUT)}
+    lo = np.zeros((B, _lib.TIMELINE)); lo[:, TL["p_gait"]] = tl["p_gait"]; lo[:, TL["gait_set"]] = tl["gait_set"]; lo[:, 4:8] = tl["weights"]; lo[:, TL["ee_qw"]] = 1.0
+    hi = lo.copy()
+    for c, (l, h) in tl["fields"].items():
+        lo[:, TL[c]] = l; hi[:, TL[c]] = h
+    solver.timeline_set_ranges(n, lo, hi, 1)
+    every = torch.ones_like(contact); episode = torch.zeros_like(contact); rows = torch.zeros((B, n, _lib.TIMELINE_CMD), dtype=torch.float64, device=dev)
+    calls_of = {"timeline_sample": lambda: (episode.add_(1), solver.timeline_sample_dev(every, episode, rows, s.cuda_stream)),
+                "plant": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    with torch.cuda.stream(s):
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    call()
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    solver.timeline_set_ranges(None); solver.gait_dev_stop()
+    return {"label": "device time per call on %d robots (every robot drawing %d slots), median of %d alternated blocks of %d calls" % (B, n, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()},
+            "spread_timeline_sample": [float(min(times["timeline_sample"])), float(max(times["timeline_sample"]))]}
+
+
+def stance_time(solver):
+    """phaseTransitionStanceTime of the solver's task file, the stance a gait insertion puts before the new gait (0.4 s where the file has none)"""
+    import re
+    m = re.search(r"phaseTransitionStanceTime\s+([-+0-9.eE]+)", open(solver.interface.taskFile).read())
+    return float(m.group(1)) if m else 0.4
+
+
+def timeline_bins(r, start_gait, cmd_vel, horizon, stance, wbc_period=0.002):
+    """Each episode scored by metrics, classed by its first gait switch that takes effect inside it (start gait → drawn gait) and by |delta cmd_vel|
+    (planar) of its first cmd_vel slot that takes effect inside it → per class: episodes, fall rate, median vel_err_rms (over the whole episode) and the
+    median time the episode ran after the switch or step.  A slot due at t (s after the episode's start) is applied by the first MPC tick at or after t
+    (ticks at -wbc_period + 10 ms k); a cmd_vel row takes effect there, a gait at that tick + horizon + the transition stance (an upper bound: no stance
+    is inserted where the schedule already stands there)."""
+    M, P, names = r["episode_metrics"], r["timeline_params"], r["gait_templates"]
+    ok = ~np.isnan(M[..., 0]); by_gait, by_dv = {}, {}
+    for b, e in zip(*np.nonzero(ok)):
+        dur = M[b, e, 0]; tick = np.ceil(np.round((P[b, e, :, 0] + wbc_period) / 0.01, 9)) * 0.01 - wbc_period
+        g = P[b, e, :, 1]; v = P[b, e, :, 2:4]; t_gait = tick + horizon + stance
+        gi = np.nonzero((g >= 0) & (t_gait < dur))[0]; vi = np.nonzero(~np.isnan(v[:, 0]) & (tick < dur))[0]
+        key_g = "%s -> %s" % (start_gait, names[int(g[gi[0]])]) if len(gi) else "no switch in the episode"
+        dv = np.hypot(*(v[vi[0]] - cmd_vel[:2])) if len(vi) else None
+        key_v = "no step in the episode" if dv is None else "[%.1f, %.1f)" % (np.floor(dv / 0.2) * 0.2, np.floor(dv / 0.2) * 0.2 + 0.2)
+        for d, k, t0 in ((by_gait, key_g, t_gait[gi[0]] if len(gi) else np.nan), (by_dv, key_v, tick[vi[0]] if len(vi) else np.nan)):
+            d.setdefault(k, []).append((M[b, e, 1] == 1, M[b, e, 7], dur - t0))
+
+    def stats(d):
+        return {k: {"episodes": len(x), "fall_rate": float(np.mean([f for f, _, _ in x])), "median_vel_err_rms": float(np.nanmedian([m for _, m, _ in x])),
+                    "median_s_after": None if np.all(np.isnan([a for _, _, a in x])) else float(np.nanmedian([a for _, _, a in x]))}
+                for k, x in sorted(d.items())}
+    return {"transition": stats(by_gait), "abs_dcmd_vel": stats(by_dv)}
+
+
+def timeline_main(args, episode_run_s=6.0):
+    """--respawn --timeline: the sampler's per-call device time; the wall time per simulated second of --duration respawning runs of --gait at --vx on the
+    plant's truth with and without TIMELINE, alternated twice after one warm-up pair; and episodes, fall rate and median velocity error per gait
+    transition and per |delta cmd_vel| bin (timeline_bins) of an episode_run_s run with respawn (0.1 s fallen, or TIMELINE_EPISODE_S), TIMELINE and
+    metrics."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch
+    solver = q.Solver(batch=B, device=0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    cmd = np.array([args.vx, 0.0, 0.0, 0.0]); kw = dict(gait=args.gait, cmd_vel=cmd, xy_yaw=xy)
+
+    def timed(duration, respawn=dict(hold=0.1, every=1.0), **extra):
+        solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+        r = closed_loop.run(solver, duration=duration, respawn=respawn, **kw, **extra)
+        torch.cuda.synchronize(dev)
+        return r, (time.perf_counter() - t0) / duration
+    per_call = timeline_times(solver)
+    wall = {"without_timeline": [], "with_timeline": []}
+    for rep in range(3):   # the first round warms up
+        for name, extra in (("without_timeline", {}), ("with_timeline", dict(timeline=TIMELINE))):
+            _, w = timed(args.duration, **extra)
+            if rep:
+                wall[name].append(w)
+    r, _ = timed(episode_run_s, metrics=True, timeline=TIMELINE, respawn=dict(hold=0.1, every=TIMELINE_EPISODE_S))
+    name, limit = card()
+    print(json.dumps({"metric": "timeline", "gpu": name, "power_limit": limit, "batch": B,
+                      "per_call": per_call,
+                      "wall_s_per_sim_s": {"label": "%s at %.2f m/s on the plant's truth, respawn after 0.1 s fallen or 1 s, runs of %.1f s, two alternated pairs "
+                                                    "after a warm-up pair" % (args.gait, args.vx, args.duration), **wall},
+                      "episodes": {"label": "%.1f s, respawn after 0.1 s fallen or %.1f s, TIMELINE per episode, metrics; classed by the first gait switch and the "
+                                            "first cmd_vel step that take effect inside the episode (horizon %.2f s, transition stance %.2f s)"
+                                            % (episode_run_s, TIMELINE_EPISODE_S, solver.time_horizon, stance_time(solver)),
+                                   "count": int(np.sum(~np.isnan(r["episode_metrics"][..., 0]))),
+                                   **timeline_bins(r, args.gait, cmd, solver.time_horizon, stance_time(solver))}}))
+
+
 def watch_state_est(solver):
     """Wrap the solver's plant and estimator steps so that each estimator call updates per-robot maxima of |z_hat - z|, |v_hat - v| and the wrapped zyx
     error (the largest of the three angles) on the device (no synchronisation) → (box, unwrap); box["max"] [B, 3], box["last"] [B, 3] after the run."""
@@ -821,9 +938,15 @@ def main():
     ap.add_argument("--randomize", action="store_true", help="with --respawn: a new plant per episode (friction, payload, push): falls per friction x push bin")
     ap.add_argument("--spawn", action="store_true", help="with --respawn: new ground per episode (tile, offset, yaw): falls per tile x heading bin")
     ap.add_argument("--metrics", action="store_true", help="per-episode metrics: wall time with and without them, per-call times, column medians of a respawn run")
+    ap.add_argument("--timeline", action="store_true", help="with --respawn: a new command timeline per episode (gait switches, cmd_vel steps): sampler time, "
+                                                            "wall time, falls and velocity error per transition")
     args = ap.parse_args()
     if args.metrics:
         return metrics_main(args)
+    if args.timeline and not args.respawn:
+        ap.error("--timeline needs --respawn")
+    if args.timeline:
+        return timeline_main(args)
     if args.randomize and not args.respawn:
         ap.error("--randomize needs --respawn")
     if args.spawn and not args.respawn:
