@@ -743,6 +743,60 @@ int qmb200_timeline_sample_dev(qmb200_handle* h, const int32_t* mask, const int3
  * sampler draws. */
 int qmb200_timeline_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][n_cmd][QMB200_TIMELINE_CMD]*/);
 
+/* ---- per-robot curricula (DESIGN.md §4.15): each robot has a level in [0, n_levels) that places the ranges of every attached draw kind (episode,
+ *      spawn, timeline) on the line from an easy box (level 0, the kind's ranges when attached) to a hard box (level n_levels - 1).  When a robot's
+ *      episode closes, a device update steps its level from the episode's end code and, optionally, its metrics row, and writes the box of the new level
+ *      into the kinds' device ranges, which the unchanged samplers then draw the next episode from.
+ *   box at level l, f = l / (n_levels - 1), per column of lo and of hi: base at l = 0, top at l = n_levels - 1, base where base == top, else
+ *                                fma(f, top - base, base); the spawn's tile column then floor(x + 0.5).  The timeline's gait_set and ee_q* must be equal at both ends.
+ *   row[QMB200_CURRICULUM]        0 start_level (an integer in [0, n_levels)), 1 up_after, 2 down_after (integers >= 1), 3-6 threshold[4] (finite)
+ *   state[QMB200_CURRICULUM_STATE]  int32: level, pass_run, fail_run, n_updates
+ *   rule: n_levels >= 2 and n_cond <= QMB200_CURRICULUM_MAX_COND conditions; condition i compares the closed episode's metrics column column[i]
+ *   (QMB200_METRICS) with the robot's threshold[i] by op[i] (QMB200_CURRICULUM_GE: >=, _LE: <=; false when either side is NaN).
+ * An update with end 1 or 2 adds one to n_updates; the episode fails when end == 1 or a QMB200_CURRICULUM_FAIL condition holds, else passes when end == 2
+ * and every QMB200_CURRICULUM_PASS condition holds, else is neutral.  A pass zeroes fail_run and adds one to pass_run; at up_after the level goes up by
+ * one (at most n_levels - 1) and pass_run goes back to 0.  A fail does the same with fail_run, down_after and one level down (at least 0).  End 0 (the
+ * run's end) updates nothing.  The start image (qmb200_robot_image_save) does not hold the state: a restore leaves it. */
+#define QMB200_CURRICULUM 7
+#define QMB200_CURRICULUM_STATE 4
+#define QMB200_CURRICULUM_MAX_COND 4
+#define QMB200_CURRICULUM_EPISODE 0    /* kinds: the ranges of qmb200_episode_set_ranges, qmb200_spawn_set_ranges, qmb200_timeline_set_ranges */
+#define QMB200_CURRICULUM_SPAWN 1
+#define QMB200_CURRICULUM_TIMELINE 2
+#define QMB200_CURRICULUM_GE 0
+#define QMB200_CURRICULUM_LE 1
+#define QMB200_CURRICULUM_PASS 0
+#define QMB200_CURRICULUM_FAIL 1
+typedef struct qmb200_curriculum_rule {
+  int32_t n_levels, n_cond;
+  int32_t column[QMB200_CURRICULUM_MAX_COND], op[QMB200_CURRICULUM_MAX_COND], role[QMB200_CURRICULUM_MAX_COND];
+} qmb200_curriculum_rule;
+/* The rule and the rows [B][QMB200_CURRICULUM]; every robot's state starts at (start_level, 0, 0, 0).  Rejects an invalid rule or row, naming the field and
+ * the robot, and refuses while a kind is attached.  NULL rule and rows clear the curriculum: each attached kind's ranges go back to its base box and
+ * the kind is detached.  Host arrays; synchronous. */
+int qmb200_curriculum_set(qmb200_handle* h, const qmb200_curriculum_rule* rule, const double* rows /*[B][QMB200_CURRICULUM] or NULL*/);
+/* Attaches kind (QMB200_CURRICULUM_*): its ranges in force become level 0, lo_top / hi_top [B][width] level n_levels - 1.  Every level's box must pass the
+ * kind's own range check (the spawn's against the tile library in force); the first failure is named with its level, field and robot, and nothing is
+ * written.  Then each robot's box at its level is written into the kind's ranges.  While attached, the kind's *_set_ranges refuses.  Synchronous. */
+int qmb200_curriculum_attach(qmb200_handle* h, int32_t kind, const double* lo_top /*[B][width]*/, const double* hi_top /*[B][width]*/);
+/* One launch, no host work: every robot with mask[b] != 0 and end[b] in {1, 2} updates its state from end[b] and, when the rule has conditions, the closed
+ * row rows[b][episode[b]] (rows [B][n_episodes][QMB200_METRICS], qmb200_metrics_close's out), writes its level to level[b] and the box at that level into
+ * every attached kind's ranges.  When the rule has conditions and episode[b] lies outside [0, n_episodes), QMB200_ST_OVERFLOW is OR-ed into status[b]
+ * and nothing else is written.  A masked end outside {1, 2} and unmasked robots are not written.  Fails, writing nothing, when no curriculum is set, no
+ * kind is attached, the rule has conditions and rows is NULL, or n_episodes < 1. */
+int qmb200_curriculum_update(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* end /*[B]*/, const int32_t* episode /*[B]*/,
+                             const double* rows /*[B][n_episodes][QMB200_METRICS] or NULL*/, int32_t n_episodes, int32_t* level /*[B] in-out*/,
+                             int32_t* status /*[B] in-out*/);
+int qmb200_curriculum_update_dev(qmb200_handle* h, const int32_t* mask, const int32_t* end, const int32_t* episode, const double* rows, int32_t n_episodes,
+                                 int32_t* level, int32_t* status, void* cuda_stream);
+/* Synchronous: the state [B][QMB200_CURRICULUM_STATE] (zeros when none is set) after every queued update; is_set = 1 when a curriculum is set.  Any output
+ * may be NULL. */
+int qmb200_curriculum_get(const qmb200_handle* h, int32_t* state /*[B][QMB200_CURRICULUM_STATE]*/, int32_t* is_set);
+/* Host only: the rows of attached kind that its sampler draws for robots robot[n] in episodes episode[n] at levels level[n] (in [0, n_levels)): the
+ * kind's *_draw on the box at that level, [n][QMB200_EPISODE], [n][QMB200_SPAWN] or [n][n_cmd][QMB200_TIMELINE_CMD]. */
+int qmb200_curriculum_draw(const qmb200_handle* h, int32_t kind, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/,
+                           const int32_t* level /*[n]*/, double* rows);
+
 /* The whole QMController::update (QMController.cpp:128-175) on the stored policy: observation update → evaluatePolicy(t_obs) → WbcBase::update
  * (period, t_obs) → safety check + control law.  cmd = the WBC 54-vector, status = WBC status | QMB200_ST_SAFETY. */
 int qmb200_update(qmb200_handle* h, const double* rbd /*[B][55]*/, const double* period /*[B]*/, double* t_obs /*[B] in-out*/, double* x_obs /*[B][30] in-out*/, double* joint_cmd /*[B][18][5] in-out*/,

@@ -107,6 +107,21 @@ TIMELINE_LAYOUT = ("t_first", "gap", "p_gait", "gait_set", "w_none", "w_cmd_vel"
 TIMELINE = len(TIMELINE_LAYOUT)   # QMB200_TIMELINE
 TIMELINE_CMD_LAYOUT = ("t", "tmpl", "cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate", "ee_kind") + tuple("ee_%d" % i for i in range(7))
 TIMELINE_CMD = len(TIMELINE_CMD_LAYOUT)   # QMB200_TIMELINE_CMD
+# a robot's curriculum (qmb200_curriculum_*): the columns of its row of CURRICULUM doubles and of its state of CURRICULUM_STATE int32, the kinds a
+# curriculum attaches to, and a rule's condition ops and roles by their codes
+CURRICULUM_LAYOUT = ("start_level", "up_after", "down_after", "threshold_0", "threshold_1", "threshold_2", "threshold_3")
+CURRICULUM = len(CURRICULUM_LAYOUT)   # QMB200_CURRICULUM
+CURRICULUM_STATE_LAYOUT = ("level", "pass_run", "fail_run", "n_updates")
+CURRICULUM_STATE = len(CURRICULUM_STATE_LAYOUT)   # QMB200_CURRICULUM_STATE
+CURRICULUM_MAX_COND = 4   # QMB200_CURRICULUM_MAX_COND
+CURRICULUM_KINDS = ("episode", "spawn", "timeline")   # QMB200_CURRICULUM_EPISODE, _SPAWN, _TIMELINE
+CURRICULUM_OPS = (">=", "<=")         # QMB200_CURRICULUM_GE, _LE
+CURRICULUM_ROLES = ("pass", "fail")   # QMB200_CURRICULUM_PASS, _FAIL
+
+
+class CurriculumRule(C.Structure):
+    """qmb200_curriculum_rule: the level count and up to CURRICULUM_MAX_COND conditions on a closed episode's metrics row (include/qmb200.h)."""
+    _fields_ = [("n_levels", C.c_int32), ("n_cond", C.c_int32), ("column", C.c_int32 * 4), ("op", C.c_int32 * 4), ("role", C.c_int32 * 4)]
 
 
 # every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
@@ -246,6 +261,12 @@ PROTOTYPES = {
     "qmb200_timeline_sample": (I32, [P] * 4),
     "qmb200_timeline_sample_dev": (I32, [P] * 5),
     "qmb200_timeline_draw": (I32, [P, I32, P, P, P]),
+    "qmb200_curriculum_set": (I32, [P] * 3),
+    "qmb200_curriculum_attach": (I32, [P, I32, P, P]),
+    "qmb200_curriculum_update": (I32, [P] * 5 + [I32] + [P] * 2),
+    "qmb200_curriculum_update_dev": (I32, [P] * 5 + [I32] + [P] * 3),
+    "qmb200_curriculum_get": (I32, [P] * 3),
+    "qmb200_curriculum_draw": (I32, [P, I32, I32] + [P] * 4),
     "qmb200_update": (I32, [P] * 10),
     "qmb200_update_dev": (I32, [P] * 11),
     "qmb200_set_pipeline": (I32, [P, I32]),

@@ -56,7 +56,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
         attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None,
-        timeline=None):
+        timeline=None, curriculum=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -163,7 +163,18 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     (Solver.timeline_sample_dev) right after its restore, its randomize draw and its spawn, before its first solve.  With randomize cmd_vel fields the
     episode's drawn cmd_vel applies from its start, and the timeline's cmd_vel slots replace it as they fall due.  ee_goal / ee_cmd_vel weights cannot
     go with a drawn spawn yaw.  The previous ranges are restored when run returns.  Returns also timeline_params[B, E, n, TIMELINE_CMD], the slots of
-    each episode (_lib.TIMELINE_CMD_LAYOUT, t in s after the episode's start), E and the NaN rows as for episode_params."""
+    each episode (_lib.TIMELINE_CMD_LAYOUT, t in s after the episode's start), E and the NaN rows as for episode_params.
+    curriculum: dict(levels=L, start=0, up_after=1, down_after=1, when=[(column, op, threshold, role), ...], randomize=dict(<field>=(lo, hi)),
+    spawn=dict(...), timeline=dict(<box>=(lo, hi), p_gait=..., weights=...)) gives every robot a level in [0, L) that moves with the outcomes of its
+    episodes (DESIGN.md §4.15; needs respawn with every).  The run's own randomize / spawn / timeline specs are level 0; curriculum[kind] names the hard
+    box of the last level (the columns it does not name are equal at both ends; a timeline's gaits and ee_quat must stay), and level l draws from the
+    box fma(l / (L - 1), top - base, base) (Solver.curriculum_attach).  An episode fails when the fall rule ended it or a "fail" condition holds, and
+    passes when every ended it and every "pass" condition holds (column of _lib.METRICS_LAYOUT, op ">=" or "<=", threshold a scalar or [B]; conditions
+    need metrics=True); up_after passes in a row move a robot one level up, down_after fails one down.  At every respawn the update runs on the device
+    after the metrics close and before the restore, so the next episode draws at the new level.  start, up_after and down_after are integers or [B]
+    integers, every bound a scalar or [B].  The curriculum is cleared before the previous ranges are restored.  Returns also curriculum_level[ticks, B]
+    (each robot's level in that record's window), episode_level[B, E] (-1 where a robot had no episode e), curriculum_state[B, CURRICULUM_STATE] at
+    the end (_lib.CURRICULUM_STATE_LAYOUT), and each attached kind's *_params drawn at its episode's level."""
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else _respawn_spec(respawn)
@@ -196,12 +207,19 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
         gd = tl["gd"]
     tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
     sp = None if spawn is None else _spawn_spec(getattr(solver, "batch", None), spawn, terrain, ground_map, gd)
+    cu = None
+    if curriculum is not None:
+        cu = _curriculum_spec(getattr(solver, "batch", None), curriculum, rs, metrics is not None, gait, dict(episode=randomize, spawn=spawn, timeline=timeline),
+                              terrain, ground_map, gd)
+        if cu["gd"] is not None:   # a top box that weighs end-effector commands needs the placeholder timeline's end-effector rows
+            gd = tl["gd"] = cu["gd"]
     if rz is not None:   # the links: a drawn payload / friction also goes where the run told the controller the plant's
-        if isinstance(model_payload, str) and model_payload == "plant" and set(rz["fields"]) & set(_lib.PAYLOAD_LAYOUT):
+        drawn = set(rz["fields"]) | set(cu["tops"]["episode"]["fields"] if cu is not None and "episode" in cu["tops"] else ())
+        if isinstance(model_payload, str) and model_payload == "plant" and drawn & set(_lib.PAYLOAD_LAYOUT):
             if payload_estimator is not None:
                 raise ValueError("closed_loop.run: model_payload=\"plant\" with a randomized payload cannot run with payload_estimator (its commits own the model payload)")
             rz["link"] |= _lib.EPISODE_MODEL_PAYLOAD
-        if tn is not None and "friction_mu" in rz["fields"]:
+        if tn is not None and "friction_mu" in drawn:
             rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
     # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
     with contextlib.ExitStack() as scope:
@@ -229,13 +247,15 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             scope.enter_context(_ranges(solver, "episode"))
         if tl is not None:
             scope.enter_context(_ranges(solver, "timeline"))
+        if cu is not None:   # cleared first: the ranges go back to their base boxes, then the scopes above restore what they found
+            scope.callback(solver.curriculum_set)
         if gd is not None:
             scope.enter_context(_gait_dev(solver, gd))
         if rs is not None:
             scope.callback(solver.robot_image_clear)
         return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
                     torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp, mt=metrics is not None, tl=tl)
+                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp, mt=metrics is not None, tl=tl, cu=cu)
 
 
 def _respawn_spec(respawn):
@@ -345,15 +365,23 @@ def _ranges(solver, kind):
             getattr(solver, kind + "_set_ranges")(**prev)
 
 
-def _set_ranges(solver, kind, layout, row, spec):
-    """sets the run's ranges of solver's kind draws: every column fixed at the run's value, row [B, C], except the spec's fields, drawn within their
-    bounds → hi [B, C]"""
+def _box(layout, row, spec):
+    """a box of ranges: every column fixed at the run's value, row [B, C], except the spec's fields, drawn within their bounds → lo, hi [B, C]"""
     col = {n: i for i, n in enumerate(layout)}
     lo = row.copy(); hi = row.copy()
     for k, (l, h) in spec["fields"].items():
         lo[:, col[k]] = l; hi[:, col[k]] = h
-    getattr(solver, kind + "_set_ranges")(lo, hi, spec["seed"])
-    return hi
+    return lo, hi
+
+
+def _timeline_box(tl, cmd_vel, t_start):
+    """the box of a parsed timeline spec: the fixed columns, the run's cmd_vel where not named, the named columns' bounds; times on the observation clock"""
+    TL = {n: i for i, n in enumerate(_lib.TIMELINE_LAYOUT)}
+    row = np.zeros((len(cmd_vel), _lib.TIMELINE)); row[:, TL["p_gait"]] = tl["p_gait"]; row[:, TL["gait_set"]] = tl["gait_set"]
+    row[:, TL["w_none"]:TL["w_none"] + 4] = tl["weights"]; row[:, TL["cmd_vel_x"]:TL["cmd_vel_x"] + 4] = cmd_vel; row[:, TL["ee_qx"]:TL["ee_qx"] + 4] = tl["quat"]
+    lo, hi = _box(_lib.TIMELINE_LAYOUT, row, tl)
+    lo[:, TL["t_first"]] += t_start; hi[:, TL["t_first"]] += t_start
+    return lo, hi
 
 
 def _gait_commands(B, gait, commands):
@@ -475,6 +503,82 @@ def _timeline_spec(B, gait, timeline, commands):
     gd = dict(names=names, gait=np.array([ids[x] for x in start], dtype=np.int32), t=np.full((Bn, n), np.inf), tmpl=np.full((Bn, n), -1, dtype=np.int32),
               cmd_vel=np.full((Bn, n, 4), np.nan), ee=ee)
     return dict(seed=seed, n=int(n), fields=fields, p_gait=p_gait, gait_set=gait_set, weights=weights, quat=quat, gd=gd)
+
+
+CURRICULUM_KINDS = dict(randomize="episode", spawn="spawn", timeline="timeline")   # a curriculum spec's key → the draw kind it attaches to
+
+
+def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map, gd):
+    """closed_loop.run's curriculum (with the run's respawn spec rs, whether metrics is on, its gait, base: the run's own randomize / spawn / timeline
+    specs by kind, terrain, ground_map and parsed commands) → dict(levels, start, up_after, down_after (int arrays, scalar or [B]), conditions [(column,
+    op, role)], thresholds [float arrays, scalar or [B]], tops: kind -> the parsed spec of its top box, gd: the placeholder timeline when the top box
+    weighs end-effector commands and the base does not, else None); ValueError when malformed.  B None: the lengths are not checked."""
+    keys = ("levels", "start", "up_after", "down_after", "when") + tuple(CURRICULUM_KINDS)
+    if not isinstance(curriculum, dict) or not set(curriculum) <= set(keys):
+        raise ValueError("closed_loop.run: curriculum must be None or dict(%s), got %r" % (", ".join(keys), curriculum))
+    if rs is None:
+        raise ValueError("closed_loop.run: curriculum needs respawn (a level moves when an episode closes)")
+    if rs["every_ms"] is None:
+        raise ValueError("closed_loop.run: curriculum needs respawn every (without it no episode can pass)")
+
+    def ints(name, v, lo, hi=None):
+        a = np.asarray(v) if not isinstance(v, (str, bool, np.bool_)) else np.array(np.nan)
+        if a.ndim > 1 or (a.ndim == 1 and B is not None and a.shape != (B,)) or a.dtype.kind not in "iuf" or not np.all(np.isfinite(a)) or np.any(np.floor(a) != a) \
+                or np.any(a < lo) or (hi is not None and np.any(a >= hi)):
+            raise ValueError("closed_loop.run: curriculum %s must be an integer in [%d, %s) or [%s] such integers, got %r"
+                             % (name, lo, "inf" if hi is None else hi, "B" if B is None else B, v))
+        return a.astype(np.int64)
+    levels = curriculum.get("levels")
+    if isinstance(levels, (bool, np.bool_)) or not isinstance(levels, (int, np.integer)) or levels < 2:
+        raise ValueError("closed_loop.run: curriculum levels must be an integer >= 2, got %r" % (levels,))
+    start = ints("start", curriculum.get("start", 0), 0, int(levels))
+    up, down = (ints(k, curriculum.get(k, 1), 1, 1 << 31) for k in ("up_after", "down_after"))
+    when = list(curriculum.get("when", []))
+    if when and not metrics:
+        raise ValueError("closed_loop.run: curriculum when needs metrics=True (its conditions read the closed episode's metrics row)")
+    if len(when) > _lib.CURRICULUM_MAX_COND:
+        raise ValueError("closed_loop.run: curriculum when takes at most %d conditions, got %d" % (_lib.CURRICULUM_MAX_COND, len(when)))
+    conditions, thresholds = [], []
+    for c in when:
+        if isinstance(c, str) or len(c) != 4:
+            raise ValueError("closed_loop.run: a curriculum condition must be (column, op, threshold, role), got %r" % (c,))
+        col, op, thr, role = c
+        if col not in _lib.METRICS_LAYOUT:
+            raise ValueError("closed_loop.run: unknown curriculum column %r (one of %s)" % (col, ", ".join(_lib.METRICS_LAYOUT)))
+        if op not in _lib.CURRICULUM_OPS or role not in _lib.CURRICULUM_ROLES:
+            raise ValueError("closed_loop.run: a curriculum condition's op must be one of %s and its role one of %s, got %r and %r"
+                             % (", ".join(_lib.CURRICULUM_OPS), ", ".join(_lib.CURRICULUM_ROLES), op, role))
+        t = np.asarray(thr, dtype=np.float64) if not isinstance(thr, (str, bool, np.bool_)) else np.array(np.nan)
+        if t.ndim > 1 or (t.ndim == 1 and B is not None and t.shape != (B,)) or not np.all(np.isfinite(t)):
+            raise ValueError("closed_loop.run: curriculum threshold of %s must be a finite scalar or [%s], got %r" % (col, "B" if B is None else B, thr))
+        conditions.append((col, op, role)); thresholds.append(t)
+    tops, top_gd = {}, None
+    for key in ("timeline", "randomize", "spawn"):   # the timeline first: its end-effector weights decide what a drawn spawn yaw may go with
+        if key not in curriculum:
+            continue
+        kind = CURRICULUM_KINDS[key]; top = curriculum[key]
+        if base[kind] is None:
+            raise ValueError("closed_loop.run: curriculum %s needs the run's own %s (its level 0)" % (key, key))
+        if not isinstance(top, dict) or {"seed", "n"} & set(top):
+            raise ValueError("closed_loop.run: curriculum %s must be a dict of the top box's fields (the run's %s gives the seed%s), got %r"
+                             % (key, key, " and n" if key == "timeline" else "", top))
+        spec = dict(base[kind], **top)
+        if key == "randomize":
+            tops[kind] = _randomize_spec(B, spec)
+        elif key == "spawn":
+            tops[kind] = _spawn_spec(B, spec, terrain, ground_map, top_gd or gd)
+        else:
+            b, t = _timeline_spec(B, gait, base[kind], None), _timeline_spec(B, gait, spec, None)
+            for name, k in (("gaits (gait_set)", "gait_set"), ("ee_quat", "quat")):
+                if not np.array_equal(np.broadcast_to(b[k], np.broadcast_shapes(np.shape(b[k]), np.shape(t[k]))), np.broadcast_to(t[k], np.broadcast_shapes(np.shape(b[k]), np.shape(t[k])))):
+                    raise ValueError("closed_loop.run: curriculum timeline %s must equal the run's (only the boxes, p_gait and weights move with the level)" % name)
+            tops[kind] = t
+            top_gd = t["gd"] if t["gd"]["ee"] and not b["gd"]["ee"] else None
+    if not tops:
+        raise ValueError("closed_loop.run: curriculum needs at least one of %s (the boxes its level moves)" % ", ".join(CURRICULUM_KINDS))
+    if top_gd is not None and base["spawn"] is not None:   # the run's own spawn, checked against the timeline its top box needs
+        _spawn_spec(B, base["spawn"], terrain, ground_map, top_gd)
+    return dict(levels=int(levels), start=start, up_after=up, down_after=down, conditions=conditions, thresholds=thresholds, tops=tops, gd=top_gd)
 
 
 @contextlib.contextmanager
@@ -639,7 +743,7 @@ def _metrics_episodes(ticks, rs):
 
 
 def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
-         rs=None, rz=None, sp=None, mt=False, tl=None):
+         rs=None, rz=None, sp=None, mt=False, tl=None, cu=None):
     import torch
     B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
     n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
@@ -651,6 +755,7 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         t_on, t_dur, wrench = (np.asarray(a, dtype=np.float64) for a in pushes)
         if t_on.shape != (B,) or t_dur.shape != (B,) or wrench.shape != (B, 12):
             raise ValueError("closed_loop.run: pushes must be (t_on[%d], duration[%d], wrench[%d, 12])" % (B, B, B))
+    tops = {} if cu is None else dict(cu["tops"])   # each attached kind's top box, built from this run's values as its base box is
     if rz is not None:   # the ranges: this run's values (entered after _robot_params: the handle's robot params are this run's plant), the named fields' bounds
         EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}
         rp = solver.sim_get_robot_params()
@@ -661,7 +766,9 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         if pushes is not None:
             row[:, EP["push_t_on"]] = t_on; row[:, EP["push_duration"]] = t_dur; row[:, EP["f_base_x"]:EP["f_base_x"] + 12] = wrench
         row[:, EP["cmd_vel_x"]:EP["cmd_vel_x"] + 4] = cmd_vel
-        hi = _set_ranges(solver, "episode", _lib.EPISODE_LAYOUT, row, rz)
+        lo, hi = _box(_lib.EPISODE_LAYOUT, row, rz); solver.episode_set_ranges(lo, hi, rz["seed"])
+        if "episode" in tops:
+            tops["episode"] = _box(_lib.EPISODE_LAYOUT, row, tops["episode"]); hi = np.maximum(hi, tops["episode"][1])
         if pushes is None and np.any(hi[:, EP["push_duration"]] > 0.0):   # the draws overwrite these rows before the first solve
             t_on, t_dur, wrench = np.zeros(B), np.zeros(B), np.zeros((B, 12)); pushes = (t_on, t_dur, wrench)
     xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
@@ -670,16 +777,22 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
         rt = solver.sim_get_robot_terrain()
         yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)   # the same heading within [-pi, pi]
         row = np.zeros((B, _lib.SPAWN)); row[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; row[:, SP["yaw"]] = yaw
-        _set_ranges(solver, "spawn", _lib.SPAWN_LAYOUT, row, sp)
-    if tl is not None:   # the ranges: the fixed columns, the run's cmd_vel where not named, the named columns' bounds; times on the observation clock
-        TL = {n: i for i, n in enumerate(_lib.TIMELINE_LAYOUT)}
-        row = np.zeros((B, _lib.TIMELINE)); row[:, TL["p_gait"]] = tl["p_gait"]; row[:, TL["gait_set"]] = tl["gait_set"]
-        row[:, TL["w_none"]:TL["w_none"] + 4] = tl["weights"]; row[:, TL["cmd_vel_x"]:TL["cmd_vel_x"] + 4] = cmd_vel; row[:, TL["ee_qx"]:TL["ee_qx"] + 4] = tl["quat"]
-        lo = row.copy(); hi = row.copy()
-        for k, (l, h) in tl["fields"].items():
-            lo[:, TL[k]] = l; hi[:, TL[k]] = h
-        lo[:, TL["t_first"]] += t_start; hi[:, TL["t_first"]] += t_start
-        solver.timeline_set_ranges(tl["n"], lo, hi, tl["seed"])
+        solver.spawn_set_ranges(*_box(_lib.SPAWN_LAYOUT, row, sp), sp["seed"])
+        if "spawn" in tops:
+            tops["spawn"] = _box(_lib.SPAWN_LAYOUT, row, tops["spawn"])
+    if tl is not None:
+        cmd_b = np.broadcast_to(cmd_vel, (B, 4))
+        solver.timeline_set_ranges(tl["n"], *_timeline_box(tl, cmd_b, t_start), tl["seed"])
+        if "timeline" in tops:
+            tops["timeline"] = _timeline_box(tops["timeline"], cmd_b, t_start)
+    if cu is not None:   # the levels start at the run's start levels; each kind's ranges set above are its level 0
+        rows = np.zeros((B, _lib.CURRICULUM))
+        rows[:, 0] = cu["start"]; rows[:, 1] = cu["up_after"]; rows[:, 2] = cu["down_after"]
+        for i, thr in enumerate(cu["thresholds"]):
+            rows[:, 3 + i] = thr
+        solver.curriculum_set(cu["levels"], rows, cu["conditions"])
+        for kind, (lo, hi) in tops.items():
+            solver.curriculum_attach(kind, lo, hi)
     stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
     f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
     i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
@@ -778,18 +891,23 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
             k0 = torch.zeros(B, dtype=torch.int64, device=dev); dk = torch.zeros_like(k0)   # each robot's episode start (plant step), and k - k0
             episode = torch.zeros(B, dtype=torch.int32, device=dev); fall_count = torch.zeros_like(episode); fallen = torch.zeros_like(episode)
             due = torch.ones_like(episode); rec_episode = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_fallen = torch.zeros_like(rec_episode)
-            if mt:   # the fall part of due: why a closed episode ended
+            if mt or cu is not None:   # the fall part of due: why a closed episode ended
                 due_fall = torch.zeros_like(episode); mt_end = torch.zeros_like(episode)
+            if cu is not None:   # each robot's level, recorded beside its episode
+                cu_level = i32(np.broadcast_to(cu["start"], (B,))); rec_level = torch.zeros_like(rec_episode)
         solver.robot_image_restore_dev(due, s)
     if mt:   # every robot's open episode (zeros: open and empty) and its closed rows
         with torch.cuda.stream(stream):
             mt_acc = torch.zeros((B, _lib.METRICS_ACC), dtype=torch.float64, device=dev)
             mt_out = torch.full((B, _metrics_episodes(ticks, rs), _lib.METRICS), np.nan, dtype=torch.float64, device=dev)
 
-    def respawn(k):   # the robots due restart at window boundary k: their episode closes, then the library's rows, the loop's, their new plant
-        if mt:
+    def respawn(k):   # the robots due restart at window boundary k: their episode closes, their level moves, then the library's rows, the loop's, their new plant
+        if mt or cu is not None:
             mt_end.copy_(due_fall).neg_().add_(2)   # 1: the fall rule, 2: every
+        if mt:
             solver.metrics_close_dev(due, mt_end, episode, mt_acc, mt_out, acc_st, s)
+        if cu is not None:   # reads the row the close just wrote; writes the ranges the draws of begin() read
+            solver.curriculum_update_dev(due, mt_end, episode, mt_out if mt else None, cu_level, acc_st, s)
         solver.robot_image_restore_dev(due, s)
         m = due.bool()
         for a, a0 in zip(own, start):
@@ -880,8 +998,10 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                 if rs is not None:
                     solver.fall_detect_dev(rbd, fall_count, fallen, rs["z_min"], rs["tilt_max"], s)
                     rec_episode[i] = episode; rec_fallen[i] = fallen
+                    if cu is not None:
+                        rec_level[i] = cu_level
                     d = fall_count >= rs["hold_windows"] if rs["on_fall"] else torch.zeros_like(fallen, dtype=torch.bool)
-                    if mt:
+                    if mt or cu is not None:
                         due_fall.copy_(d)
                     if rs["every_ms"] is not None:
                         d |= (k + 1 - k0) >= rs["every_ms"]
@@ -904,13 +1024,18 @@ def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_
                    ee_target=rec_ee_target.cpu().numpy())
     if rs is not None:
         out.update(episode=rec_episode.cpu().numpy(), fallen=rec_fallen.cpu().numpy())
-    if rz is not None or sp is not None or tl is not None:   # rebuilt on the host from the episode record: the samplers' rows are pure functions of (ranges, seed, robot, episode)
+    if cu is not None:   # a robot's level is constant over an episode: it moves at the respawn that starts the next
+        ep = out["episode"]; lv = rec_level.cpu().numpy()
+        el = np.full((B, int(ep.max()) + 1), -1, dtype=np.int32); el[np.broadcast_to(np.arange(B), ep.shape), ep] = lv
+        out.update(curriculum_level=lv, episode_level=el, curriculum_state=solver.curriculum_get())
+    if rz is not None or sp is not None or tl is not None:   # rebuilt on the host from the episode record: the samplers' rows are pure functions of (ranges, seed, robot, episode[, level])
         ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
         had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
         rb, re_ = np.nonzero(had)
         for kind, spec, shape in (("episode", rz, (_lib.EPISODE,)), ("spawn", sp, (_lib.SPAWN,)), ("timeline", tl, (0 if tl is None else tl["n"], _lib.TIMELINE_CMD))):
             if spec is not None:
-                out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = getattr(solver, kind + "_draw")(rb, re_)
+                rows = solver.curriculum_draw(kind, rb, re_, el[rb, re_]) if kind in tops else getattr(solver, kind + "_draw")(rb, re_)
+                out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = rows
         if tl is not None:   # on the episode's clock: exact for drawn times in [t_start / 2, 2 t_start]
             out["timeline_params"][..., 0] -= t_start
     if mt:   # trimmed to the most episodes of any robot

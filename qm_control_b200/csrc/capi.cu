@@ -24,6 +24,7 @@
 #include "kernels/spawn_api.cuh"
 #include "kernels/metrics_api.cuh"
 #include "kernels/timeline_api.cuh"
+#include "kernels/curriculum_api.cuh"
 
 namespace qmb {
 void launch_wbc_update(const DevModel* mdl, int B, const double* x_des, const double* u_des, const double* rbd, const int32_t* mode, const double* period, const double* time,
@@ -45,9 +46,9 @@ struct RobotArray {
 };
 
 // Per-robot ranges of a per-episode draw (capi_episode.inc, capi_spawn.inc, capi_timeline.inc): lo, hi [B][width] (empty: none set), their device copies (dalloc: freed
-// with allocs) and the seed
+// with allocs) and the seed; attached: a curriculum owns them (capi_curriculum.inc), on_device: its update wrote the device copies, ranges_sync refreshes lo, hi
 struct DrawRanges {
-  int width; std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0;
+  int width; std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0; bool attached = false, on_device = false;
 };
 
 // The components a start image covers (capi_respawn.inc).  Each has a generation that its reset, stop and re-allocation bump, so a restore can tell
@@ -104,6 +105,12 @@ struct qmb200_handle {
                                          // ranges: whether any robot weighs an end-effector kind, one past the highest gait_set bit
     int n_cmd = 0; bool ee = false; int gait_bits = 0;
   } timeline{{TL_DBL}};
+  struct {   // per-robot curriculum (capi_curriculum.inc): the rule, the rows [B][CU_DBL] and the state [B][CUS_INT] (host copies, empty: none set; on_device:
+             // an update wrote the device state) with their device copies, and each kind's base and top boxes (host copies, empty: not attached) with
+             // their device copy d [4][B][width] (base lo, base hi, top lo, top hi)
+    qmb200_curriculum_rule rule{}; std::vector<double> rows; std::vector<int32_t> state; double* d_rows = nullptr; int32_t* d_state = nullptr; bool on_device = false;
+    struct Kind { std::vector<double> base_lo, base_hi, top_lo, top_hi; double* d = nullptr; } kind[CU_KINDS];
+  } cur;
   uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
   struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
     bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
@@ -302,9 +309,11 @@ int terrain_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<q
 // The ranged draws' set / get / draw path (qmb200_<kind>_set_ranges, _get_ranges, _draw; kind: "episode", "spawn" or "timeline").
 // Set: NULL lo and hi clear the ranges once no queued draw reads them; else error() checks them ("" when valid), the device copies are allocated, then
 // prepare() makes sure the rows the sampler writes exist (it may fail, leaving the ranges as they were), and the ranges are copied and stored.
+// Refused while a curriculum is attached to the ranges (qmb200_curriculum_attach), whose update writes them.
 template <class Error, class Prepare>
 int ranges_set(qmb200_handle* h, DrawRanges& r, const char* kind, const double* lo, const double* hi, int64_t seed, Error error, Prepare prepare) {
   const std::string who = std::string("qmb200_") + kind + "_set_ranges"; const size_t n = (size_t)h->B * r.width;
+  if (r.attached) return fail(h, who + ": a curriculum is attached to these ranges (qmb200_curriculum_set with NULL clears it)");
   if (!lo != !hi) return fail(h, who + ": lo and hi must both be set or both be NULL");
   if (!lo) {
     QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());   // no queued draw still reads the ranges
@@ -320,7 +329,16 @@ int ranges_set(qmb200_handle* h, DrawRanges& r, const char* kind, const double* 
   r.lo.assign(lo, lo + n); r.hi.assign(hi, hi + n); r.seed = (uint64_t)seed;
   return 0;
 }
+// After a curriculum update wrote the ranges on the device: wait for it and copy them into the host copies, which the getters and the host draws read
+int ranges_sync(const qmb200_handle* hc, const DrawRanges& rc) {
+  qmb200_handle* h = const_cast<qmb200_handle*>(hc); DrawRanges& r = const_cast<DrawRanges&>(rc);
+  if (!r.on_device) return 0;
+  QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());
+  QMB_CUDA(h, cudaMemcpy(r.lo.data(), r.d_lo, r.lo.size() * 8, cudaMemcpyDeviceToHost)); QMB_CUDA(h, cudaMemcpy(r.hi.data(), r.d_hi, r.hi.size() * 8, cudaMemcpyDeviceToHost));
+  r.on_device = false; return 0;
+}
 int ranges_get(const qmb200_handle* h, const DrawRanges& r, double* lo, double* hi, int64_t* seed, int32_t* is_set) {
+  if (int rc = ranges_sync(h, r)) return rc;
   const size_t n = (size_t)h->B * r.width; const bool set = !r.lo.empty();
   if (lo) { if (set) std::memcpy(lo, r.lo.data(), n * 8); else std::memset(lo, 0, n * 8); }
   if (hi) { if (set) std::memcpy(hi, r.hi.data(), n * 8); else std::memset(hi, 0, n * 8); }
@@ -338,6 +356,7 @@ int ranges_draw(qmb200_handle* h, const DrawRanges& r, const char* kind, int32_t
   if (n < 0 || (n > 0 && (!robot || !episode || !rows))) return fail(h, who + ": n must be >= 0 and the buffers non-null");
   if (r.lo.empty()) return no_ranges(h, who.c_str(), kind);
   for (int32_t i = 0; i < n; ++i) if (robot[i] < 0 || robot[i] >= h->B) return fail(h, who + ": robot must be in [0, B)");
+  if (int rc = ranges_sync(h, r)) return rc;
   const int64_t robot0 = (int64_t)h->comm_rank * h->B;
   for (int32_t i = 0; i < n; ++i) {
     const size_t b = (size_t)robot[i];
@@ -517,3 +536,4 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_spawn.inc"
 #include "capi_metrics.inc"
 #include "capi_timeline.inc"
+#include "capi_curriculum.inc"

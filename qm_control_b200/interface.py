@@ -821,6 +821,64 @@ class Solver:
         self._call("timeline_draw", len(robot), _p(robot), _p(episode), _p(rows))
         return rows
 
+    # ---------------- per-robot curricula (include/qmb200.h: qmb200_curriculum_*; DESIGN.md §4.15) ----------------
+    def curriculum_set(self, n_levels=None, rows=None, conditions=()):
+        """A curriculum of n_levels levels: per-robot rows [B, CURRICULUM] (_lib.CURRICULUM_LAYOUT) and up to CURRICULUM_MAX_COND conditions (column, op,
+        role): column a name of _lib.METRICS_LAYOUT or its index, op ">=" or "<=", role "pass" or "fail" (or their codes); condition i compares the closed
+        episode's column with each robot's threshold_i.  Every robot's state starts at its start_level.  None clears the curriculum, and every attached
+        kind's ranges go back to their base box.  Synchronous."""
+        if n_levels is None and rows is None:
+            self._call("curriculum_set", None, None); return
+        if len(conditions) > _lib.CURRICULUM_MAX_COND:
+            raise ValueError("at most %d curriculum conditions, got %d" % (_lib.CURRICULUM_MAX_COND, len(conditions)))
+        rule = _lib.CurriculumRule(); rule.n_levels = int(n_levels); rule.n_cond = len(conditions)
+        code = lambda names, v: names.index(v) if isinstance(v, str) and v in names else int(v) if not isinstance(v, str) else -1
+        for i, (col, op, role) in enumerate(conditions):
+            rule.column[i] = code(_lib.METRICS_LAYOUT, col); rule.op[i] = code(_lib.CURRICULUM_OPS, op); rule.role[i] = code(_lib.CURRICULUM_ROLES, role)
+        self._call("curriculum_set", C.byref(rule), _p(_f64(rows, (self.batch, _lib.CURRICULUM))))
+
+    def curriculum_attach(self, kind, lo_top, hi_top):
+        """Attach kind ("episode", "spawn" or "timeline"): its ranges in force become level 0, lo_top / hi_top [B, width] the last level, and each robot's
+        box at its level is written into the kind's ranges.  Synchronous."""
+        width = dict(episode=_lib.EPISODE, spawn=_lib.SPAWN, timeline=_lib.TIMELINE)[kind]
+        shape = (self.batch, width)
+        self._call("curriculum_attach", _lib.CURRICULUM_KINDS.index(kind), _p(_f64(lo_top, shape)), _p(_f64(hi_top, shape)))
+
+    def curriculum_get(self):
+        """→ the state [B, CURRICULUM_STATE] (_lib.CURRICULUM_STATE_LAYOUT) after every queued update, or None when no curriculum is set."""
+        state = np.zeros((self.batch, _lib.CURRICULUM_STATE), dtype=np.int32); is_set = C.c_int32()
+        self._call("curriculum_get", _p(state), C.byref(is_set))
+        return state if is_set.value else None
+
+    def curriculum_update(self, mask, end, episode, level, status, rows=None):
+        """Host variant of curriculum_update_dev on copies of level [B] and status [B] → dict(level, status)."""
+        B = self.batch; level = _i32(level, (B,)).copy(); status = _i32(status, (B,)).copy()
+        mask, end, episode = (_i32(np.broadcast_to(np.asarray(a), (B,)), (B,)) for a in (mask, end, episode))
+        if rows is not None:
+            rows = _f64(rows)
+            if rows.ndim != 3 or rows.shape[0] != B or rows.shape[2] != _lib.METRICS:
+                raise ValueError("expected rows of shape (%d, E, %d), got %s" % (B, _lib.METRICS, rows.shape))
+        self._call("curriculum_update", _p(mask), _p(end), _p(episode), _p(rows), 1 if rows is None else rows.shape[1], _p(level), _p(status))
+        return dict(level=level, status=status)
+
+    def curriculum_update_dev(self, mask, end, episode, rows, level, status, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) whose episode closed with end[b] 1 (fall) or 2 (length limit) updates its curriculum
+        state, from the closed row rows[b, episode[b]] (rows float64 [B, E, METRICS], metrics_close_dev's out; None when the rule has no conditions), and
+        writes its level to level[b] (int32 [B]) and its box into every attached kind's ranges.  With conditions, an episode index outside [0, E) ORs
+        QMB200_ST_OVERFLOW into status[b] and writes nothing else.  One launch, no synchronisation."""
+        if rows is not None and (rows.dim() != 3 or rows.shape[0] != self.batch or rows.shape[2] != _lib.METRICS):
+            raise ValueError("expected rows of shape (%d, E, %d), got %s" % (self.batch, _lib.METRICS, tuple(rows.shape)))
+        self._call("curriculum_update_dev", _p(mask), _p(end), _p(episode), _p(rows), 1 if rows is None else int(rows.shape[1]), _p(level), _p(status), stream)
+
+    def curriculum_draw(self, kind, robot, episode, level):
+        """Host only: robot [n], episode [n], level [n] → the rows attached kind's sampler draws for them at those levels ([n, EPISODE], [n, SPAWN] or
+        [n, n_cmd, TIMELINE_CMD])."""
+        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); level = _i32(np.ravel(level), robot.shape)
+        shape = dict(episode=(_lib.EPISODE,), spawn=(_lib.SPAWN,), timeline=(self._timeline_n(), _lib.TIMELINE_CMD))[kind]
+        rows = np.zeros((len(robot),) + shape)
+        self._call("curriculum_draw", _lib.CURRICULUM_KINDS.index(kind), len(robot), _p(robot), _p(episode), _p(level), _p(rows))
+        return rows
+
     # ---------------- per-episode metrics (include/qmb200.h: qmb200_metrics_*; DESIGN.md §4.13) ----------------
     def metrics_step(self, dt, rbd, contact, effort, cmd, n_target, target_times, target_states, time, status, acc, kind=None, rbd_est=None):
         """Host variant of metrics_step_dev on a copy of acc [B, METRICS_ACC] → the accumulator rows after the sample."""

@@ -6,7 +6,7 @@ deviation from the initial pose, as percentiles over the robots) of this project
 
     python tools/bench_closedloop.py [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3] [--vary | --terrain] [--state-estimator [--sensor-noise reference] [--attitude-filter] [--slip-detector]]
                                      [--gait-commands] [--ee-goals]
-    python tools/bench_closedloop.py --respawn [--randomize | --spawn] [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
+    python tools/bench_closedloop.py --respawn [--randomize | --spawn | --timeline | --curriculum] [--batch 8192] [--duration 1.0] [--gait trot] [--vx 0.3]
 
 --vary runs a per-robot robustness sweep on the same loop: robot b carries an end-effector payload of 0-2 kg (5 bins), stands on a floor with
 mu 0.15-1.0 (5 bins) and takes a lateral (+y) base push of 0-180 N for 0.1 s from 0.4 s (4 bins), every combination equally often.  The JSON line
@@ -77,6 +77,12 @@ detector and the image restore against the plant step (CUDA events, alternated b
 with, from one 5 s run, the episodes per robot and the fraction of episodes that fall within their first second per friction bin x push-magnitude bin
 (episodes that start at least 1 s before the run's end); the wall time per simulated second of --duration runs with and without randomize (both with
 respawn), alternated in one process; and the device time per call of the sampler against the image restore (CUDA events, alternated blocks).
+
+--respawn --curriculum gives every robot a level stepped from its episodes' outcomes (closed_loop.run(curriculum=...)).  It prints one JSON line
+"curriculum" with the update's device time against the plant step (CUDA events, alternated blocks); the wall time per simulated second of --duration
+runs with respawn and --randomize's plant in both arms, without and with a curriculum on the push bounds, alternated in one process; and an up-down
+staircase on the base push (12 levels from 0 to 255 N, one up after an episode that lasted 1 s, one down after a fall) per friction bin on the state
+estimate, beside the 50 % crossing of the fall fraction of a run with the push drawn uniformly over the same range, the same robots and duration.
 
 --respawn --spawn starts every episode on new ground (closed_loop.run(spawn=...)) on a library of flat ground, a 10 deg ramp, 6 cm stairs and rough
 ground (2 cm), each flat within 0.35 m of its centre: the tile U{0..3}, dx U[-0.5, 0] m (the flat zone before the first edge, so the controller's
@@ -918,6 +924,116 @@ def watch_state_est(solver):
     return box, unwrap
 
 
+# --respawn --curriculum: an up-down staircase (one level up after an episode that lasted `every`, one down after a fall) on the base push along +x, from
+# 0 N at level 0 to 255 N at level CURRICULUM_LEVELS - 1, starting half way, each robot on a fixed friction of one MU_BINS bin (the bins of
+# --randomize's sweep, on the same state estimate); pushes for 0.1 s from 0.2-0.5 s
+CURRICULUM_LEVELS, CURRICULUM_PUSH, CURRICULUM_MU_BINS = 12, 255.0, MU_BINS
+CURRICULUM_RUN_S, CURRICULUM_EVERY_S = 12.0, 1.0
+
+
+def curriculum_times(solver, reps=7, calls=20):
+    """Device time per curriculum update of every robot (curriculum_update_dev, one pass condition on a metrics row, the episode ranges attached) and per
+    1 ms plant step of the whole batch, alternated `reps` times in blocks of `calls` (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    q0, v0 = solver.sim_standing_state(xy); q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    lo = np.zeros((B, _lib.EPISODE)); lo[:, 0] = 0.7; hi = lo.copy(); hi[:, 11:13] = 180.0; lo[:, 11:13] = -180.0
+    solver.episode_set_ranges(lo, hi, 1)
+    rows = np.zeros((B, _lib.CURRICULUM)); rows[:, 1:3] = 1.0; rows[:, 3] = 0.2
+    solver.curriculum_set(CURRICULUM_LEVELS, rows, [("distance", ">=", "pass")]); solver.curriculum_attach("episode", lo * 1.4, hi * 1.4)
+    every = torch.ones_like(contact); end = torch.full_like(contact, 2); ep = torch.zeros_like(contact); level = torch.zeros_like(contact)
+    out = torch.rand((B, 1, _lib.METRICS), dtype=torch.float64, device=dev)
+    calls_of = {"curriculum_update": lambda: solver.curriculum_update_dev(every, end, ep, out, level, st, s.cuda_stream),
+                "plant": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    for rep in range(reps + 1):   # the first round warms up
+        for mode, call in calls_of.items():
+            torch.cuda.synchronize(dev)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+            for _ in range(calls):
+                call()
+            b.record(s); torch.cuda.synchronize(dev)
+            if rep:
+                times[mode].append(a.elapsed_time(b) / calls)
+    solver.curriculum_set(None); solver.episode_set_ranges(None)
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()},
+            "spread_curriculum_update": [float(min(times["curriculum_update"])), float(max(times["curriculum_update"]))]}
+
+
+def curriculum_main(args):
+    """--respawn --curriculum: the update's per-call device time; the wall time per simulated second of --duration runs of --gait at --vx on the plant's
+    truth with respawn and RANDOMIZE in both arms, without and with a curriculum on RANDOMIZE's push bounds, alternated twice after a warm-up pair; and
+    the push each friction bin survives, estimated two ways from runs of CURRICULUM_RUN_S with respawn (0.1 s fallen, or CURRICULUM_EVERY_S): the
+    staircase's threshold (each robot's mean level over the second half of its episodes) against the 50 % crossing of the fall fraction over the push
+    of a run with the push drawn uniformly from the staircase's range, the same robots and episode budget."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch
+    solver = q.Solver(batch=B, device=0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    kw = dict(gait=args.gait, cmd_vel=(args.vx, 0.0, 0.0, 0.0), xy_yaw=xy)
+
+    def timed(duration, **extra):
+        solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+        r = closed_loop.run(solver, duration=duration, **kw, **extra)
+        torch.cuda.synchronize(dev)
+        return r, (time.perf_counter() - t0) / duration
+    per_call = curriculum_times(solver)
+    respawn = dict(hold=0.1, every=CURRICULUM_EVERY_S)
+    wall = {"without_curriculum": [], "with_curriculum": []}
+    arms = (("without_curriculum", {}), ("with_curriculum", dict(curriculum=dict(levels=CURRICULUM_LEVELS, randomize=dict(f_base_x=(-255.0, 255.0), f_base_y=(-255.0, 255.0))))))
+    for rep in range(3):   # the first round warms up
+        for name, extra in arms:
+            _, w = timed(args.duration, respawn=respawn, randomize=RANDOMIZE, **extra)
+            if rep:
+                wall[name].append(w)
+    # runs of CURRICULUM_RUN_S roll the gait on the device (a command timeline that changes nothing): the host-tiled schedule holds about 5 s of trot
+    kw["commands"] = dict(t=np.full((B, 1), 0.2), gait=np.full((B, 1), None, dtype=object))
+    bins = np.array(CURRICULUM_MU_BINS); mu_bin = np.arange(B) % (len(bins) - 1)
+    mu = bins[mu_bin] + (bins[mu_bin + 1] - bins[mu_bin]) * ((np.arange(B) // (len(bins) - 1)) % 16 + 0.5) / 16.0
+    base = dict(seed=0, friction_mu=(mu, mu), push_t_on=(0.2, 0.5), push_duration=(0.1, 0.1))
+    est = dict(state_estimator=True, sensor_noise="reference")
+    stair, _ = timed(CURRICULUM_RUN_S, respawn=respawn, randomize=base, **est,
+                     curriculum=dict(levels=CURRICULUM_LEVELS, start=CURRICULUM_LEVELS // 2, randomize=dict(f_base_x=(CURRICULUM_PUSH, CURRICULUM_PUSH))))
+    flat, _ = timed(CURRICULUM_RUN_S, respawn=respawn, randomize=dict(base, f_base_x=(0.0, CURRICULUM_PUSH)), metrics=True, **est)
+    el = stair["episode_level"]; n_ep = (el >= 0).sum(1)
+    second = np.array([el[b, n_ep[b] // 2:n_ep[b]].mean() for b in range(B)])
+    thr = second * CURRICULUM_PUSH / (CURRICULUM_LEVELS - 1)
+    push_bins = np.linspace(0.0, CURRICULUM_PUSH, 9)
+    P, M = flat["episode_params"], flat["episode_metrics"]; ok = M[..., 1] > 0; fell = M[..., 1] == 1   # the episodes a respawn closed; those the fall rule did
+    out = {}
+    for i in range(len(bins) - 1):
+        rob = mu_bin == i; sel = ok & rob[:, None]; f = P[..., 11][sel]; y = fell[sel]
+        frac = [float(np.mean(y[(f >= a) & (f < c)])) if np.any((f >= a) & (f < c)) else None for a, c in zip(push_bins[:-1], push_bins[1:])]
+        centres = (push_bins[:-1] + push_bins[1:]) / 2; crossing = None
+        for j in range(len(frac) - 1):
+            if frac[j] is not None and frac[j + 1] is not None and frac[j] < 0.5 <= frac[j + 1]:
+                crossing = float(centres[j] + (0.5 - frac[j]) / (frac[j + 1] - frac[j]) * (centres[j + 1] - centres[j])); break
+        out["mu_%.2f-%.2f" % (bins[i], bins[i + 1])] = {
+            "staircase_threshold_N": {"mean": float(thr[rob].mean()), "median": float(np.median(thr[rob])), "robots": int(rob.sum())},
+            "saturated": {"bottom": float(np.mean(second[rob] == 0)), "top": float(np.mean(second[rob] == CURRICULUM_LEVELS - 1))},
+            "uniform_50pct_crossing_N": crossing, "uniform_fall_fraction_per_push_bin": frac, "uniform_episodes": int(sel.sum())}
+    name, limit = card()
+    print(json.dumps({"metric": "curriculum", "gpu": name, "power_limit": limit, "batch": B,
+                      "per_call": per_call,
+                      "wall_s_per_sim_s": {"label": "%s at %.2f m/s on the plant's truth, respawn after 0.1 s fallen or %.1f s, RANDOMIZE per episode; runs of %.1f s, "
+                                                    "two alternated pairs after a warm-up pair; the curriculum arm moves RANDOMIZE's push bounds to +-255 N over %d levels"
+                                                    % (args.gait, args.vx, CURRICULUM_EVERY_S, args.duration, CURRICULUM_LEVELS), **wall},
+                      "staircase": {"label": "%s at %.2f m/s on the state estimate with the reference IMU noise, the gait rolled on the device, %.1f s, respawn after 0.1 s fallen or %.1f s; push f_base_x for 0.1 s from "
+                                             "0.2-0.5 s; staircase 0-%.0f N over %d levels, up after an episode that lasted, down after a fall, from level 6; "
+                                             "uniform: f_base_x U[0, %.0f] N, fall fraction per push bin of %.0f N over the episodes a respawn closed"
+                                             % (args.gait, args.vx, CURRICULUM_RUN_S, CURRICULUM_EVERY_S, CURRICULUM_PUSH, CURRICULUM_LEVELS, CURRICULUM_PUSH,
+                                                push_bins[1]),
+                                    "episodes": {"staircase": int(n_ep.sum()), "uniform": int(ok.sum())}, "per_mu_bin": out}}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
@@ -940,7 +1056,13 @@ def main():
     ap.add_argument("--metrics", action="store_true", help="per-episode metrics: wall time with and without them, per-call times, column medians of a respawn run")
     ap.add_argument("--timeline", action="store_true", help="with --respawn: a new command timeline per episode (gait switches, cmd_vel steps): sampler time, "
                                                             "wall time, falls and velocity error per transition")
+    ap.add_argument("--curriculum", action="store_true", help="with --respawn: per-robot levels stepped from each episode's outcome: update time, wall time, "
+                                                              "an up-down staircase on the push against a uniform sweep")
     args = ap.parse_args()
+    if args.curriculum and not args.respawn:
+        ap.error("--curriculum needs --respawn")
+    if args.curriculum:
+        return curriculum_main(args)
     if args.metrics:
         return metrics_main(args)
     if args.timeline and not args.respawn:
