@@ -65,7 +65,9 @@ typedef struct {
   int32_t device;               /* CUDA device ordinal */
   double time_horizon;          /* <= 0 → mpc.timeHorizon (task.info:140) */
   double dt;                    /* <= 0 → sqp.dt (task.info:78) */
-  int32_t max_nodes;            /* <= 0 → ceil(horizon/dt) + 1 + 2*10 (room for 10 events inside the horizon) */
+  int32_t max_nodes;            /* <= 0 → ceil(horizon/dt) + 1 + 2*10 (room for 10 events inside the horizon).  At most 1060, given or by default: the
+                                   setup kernel stages 48 B per node + 320 B per warp, four warps per CTA, in at most 200 KB of shared memory; a larger value
+                                   fails qmb200_create ("max_nodes too large") */
   int32_t wbc_variant;          /* QMB200_WBC_* */
 } qmb200_config;
 
