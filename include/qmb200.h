@@ -39,6 +39,7 @@ extern "C" {
  *                           bits 8..15  MPC flags shifted left by 8 — only in the merged word qmb200_tick / qmb200_tick_dev return
  *                                       (qmb200_mpc_solve / qmb200_mpc_get_solution report the MPC flags unshifted in their own status array)
  *                           bit 16      QMB200_ST_SAFETY — qmb200_update / qmb200_control_law
+ *                           bit 17      QMB200_ST_COMMAND — qmb200_gait_dev_command(_dev), a rejected command row
  * Nothing else is ever OR-ed into a status word: the WBC's iteration counts live in qmb200_wbc_get_diagnostics. */
 #define QMB200_ST_ITER_CAP 1
 #define QMB200_ST_OVERFLOW 2      /* WBC: more rows than the working-set / level-0 buffers hold; MPC: node count > NMAX, event / target count out of range, swing phase not enclosed */
@@ -301,8 +302,23 @@ int qmb200_gait_dev_get(qmb200_handle* h, int32_t* n_events /*[B]*/, double* eve
  * when the timeline has no end-effector rows).  Any output may be NULL: a call with n_cmd alone sizes the others.  Fails while the schedule is not running. */
 int qmb200_gait_dev_get_commands(qmb200_handle* h, int32_t* n_cmd, double* t /*[B][n_cmd]*/, int32_t* tmpl /*[B][n_cmd]*/, double* cmd_vel /*[B][n_cmd][4]*/,
                                  int32_t* ee_kind /*[B][n_cmd]*/, double* ee_cmd /*[B][n_cmd][7]*/);
-/* Releases the schedules and the timeline; the template table stays.  Step and get fail until the next reset.  Stopping a schedule that is not
- * running does nothing and returns 0. */
+/* One command per robot from device buffers, applied by the robot's next step (DESIGN.md §4.16): each robot has one pending slot beside its schedule,
+ * empty after qmb200_gait_dev_reset.  For every robot with mask[b] != 0 the row tmpl[b] (-1: none), cmd_vel[b][4] (a NaN row: none), ee_kind[b] (-1,
+ * QMB200_TARGET_EE_CMD_VEL or QMB200_TARGET_EE_GOAL) and ee[b][7] (as ee_cmd of qmb200_gait_dev_set_commands_ee) is checked on the device with the rules
+ * of qmb200_gait_dev_set_commands_ee; an accepted row overwrites the slot (a later command before the step replaces an earlier one), a rejected row
+ * leaves it and gets status[b] = QMB200_ST_COMMAND.  status [B] is written, not OR-ed: 0 for accepted rows and for robots with mask[b] == 0, whose
+ * slots are not written.  The next step applies a set slot after the robot's timeline rows due at t, as one more row due at t, and clears it when it
+ * succeeds; a failed step leaves it set.  A restore (qmb200_robot_image_restore) clears the restored robots' slots.  Fails, writing nothing, while the
+ * schedule is not running or when a buffer is NULL.  One launch, no synchronisation. */
+int qmb200_gait_dev_command(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* tmpl /*[B]*/, const double* cmd_vel /*[B][4]*/, const int32_t* ee_kind /*[B]*/,
+                            const double* ee /*[B][7]*/, int32_t* status /*[B]*/);
+int qmb200_gait_dev_command_dev(qmb200_handle* h, const int32_t* mask, const int32_t* tmpl, const double* cmd_vel, const int32_t* ee_kind, const double* ee,
+                                int32_t* status, void* cuda_stream);
+/* Synchronous: each robot's pending slot, set [B] (1: a command waits for the next step), and the row last written to it: tmpl [B], cmd_vel [B][4],
+ * ee_kind [B], ee [B][7] (zeros after a reset or restore).  Any output may be NULL.  Fails while the schedule is not running. */
+int qmb200_gait_dev_get_pending(qmb200_handle* h, int32_t* set /*[B]*/, int32_t* tmpl /*[B]*/, double* cmd_vel /*[B][4]*/, int32_t* ee_kind /*[B]*/, double* ee /*[B][7]*/);
+/* Releases the schedules, the pending slots and the timeline; the template table stays.  Step and get fail until the next reset.  Stopping a schedule
+ * that is not running does nothing and returns 0. */
 int qmb200_gait_dev_stop(qmb200_handle* h);
 
 /* ---- controller side of the path (SURVEY.md section 8f): the steps of QMController::update around evaluatePolicy / WbcBase::update and the
@@ -313,6 +329,7 @@ int qmb200_gait_dev_stop(qmb200_handle* h);
 #define QMB200_TARGET_EE_GOAL 2      /* EEgoalPoseToTargetTrajectories  (:172-208) + processFeedback (QmTargetTrajectoriesPublisher.cpp:94-109): cmd = pos(3), quat xyzw(4) */
 #define QMB200_JOINT_CMD 5           /* HybridJointHandle::setCommand(posDes, velDes, kp, kd, ff) (HybridJointInterface.h:55-61) */
 #define QMB200_ST_SAFETY 0x10000     /* SafetyChecker::check failed (SafetyChecker.h:22-35): the reference stops the controller */
+#define QMB200_ST_COMMAND 0x20000    /* qmb200_gait_dev_command(_dev): the robot's command row was rejected (no other status word uses this bit) */
 #define QMB200_ST_HW_RING_FULL 2     /* qmb200_hw_write: more than 32 commands inside the delay window (the oldest was dropped) */
 
 /* QMController::updateStateEstimation tail (QMController.cpp:236-243): t_obs += period; x_obs = computeCentroidalStateFromRbdModel(rbd) with
@@ -566,14 +583,15 @@ int qmb200_slip_stop(qmb200_handle* h);
  *      The start image holds, per robot, the rows of every component running when it is saved: the state estimator, attitude filter, slip detector and
  *      payload estimator states, the model payload rows (qmb200_set_model_payload, as a commit may have left them) and the device gait schedule with
  *      its timeline cursor.  Handle settings (parameters, tuning rows, plant robot params, terrain, ground map, gait templates, command timeline) are not
- *      state and are never written.  Each reset, stop or re-allocation of an imaged component (and qmb200_gait_dev_set_commands, which resets the
- *      cursors) makes the image stale for it. */
+ *      state and are never written.  The gait schedule's pending command slots (qmb200_gait_dev_command) are cleared, not imaged.  Each reset, stop
+ *      or re-allocation of an imaged component (and qmb200_gait_dev_set_commands, which resets the cursors) makes the image stale for it. */
 /* Saves the image of the components running now, replacing any previous one.  Synchronous. */
 int qmb200_robot_image_save(qmb200_handle* h);
 /* Frees the image (qmb200_destroy does too).  Clearing when none is saved does nothing and returns 0. */
 int qmb200_robot_image_clear(qmb200_handle* h);
 /* One launch, no host work: for every robot with mask[b] != 0 the imaged rows return to the image, both MPC warm-start sides forget the robot's
- * solution (n_nodes = 0, what qmb200_mpc_reset does for all), its WBC last input is zeroed and its hw_write FIFO emptied.  Robots with mask[b] == 0
+ * solution (n_nodes = 0, what qmb200_mpc_reset does for all), its WBC last input is zeroed, its hw_write FIFO emptied and, while the device gait
+ * schedule runs, its pending command dropped (a command decided on the old episode's state never reaches the new one).  Robots with mask[b] == 0
  * are not written.  Fails, naming the component and writing nothing, when no image is saved, an imaged component was stopped, reset or re-allocated
  * since, or a component runs that was not imaged. */
 int qmb200_robot_image_restore(qmb200_handle* h, const int32_t* mask /*[B]*/);

@@ -10,6 +10,7 @@ ASSETS = os.path.join(ROOT, "assets")
 NX, NU, RBD, CMD, TARGET, EMAX, KMAX = 30, 30, 55, 54, 37, 32, 4
 GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
 TARGET_CMD_VEL, TARGET_EE_CMD_VEL, TARGET_EE_GOAL = 0, 1, 2   # QMB200_TARGET_*: the target front-end's kinds (-1 in a per-robot kind: a held goal)
+ST_COMMAND = 0x20000   # QMB200_ST_COMMAND: a rejected qmb200_gait_dev_command row
 
 dp = C.POINTER(C.c_double)
 ip = C.POINTER(C.c_int32)
@@ -182,6 +183,9 @@ PROTOTYPES = {
     "qmb200_gait_dev_step_ee_dev": (I32, [P] * 11),
     "qmb200_gait_dev_get": (I32, [P] * 6),
     "qmb200_gait_dev_get_commands": (I32, [P] * 7),
+    "qmb200_gait_dev_command": (I32, [P] * 7),
+    "qmb200_gait_dev_command_dev": (I32, [P] * 8),
+    "qmb200_gait_dev_get_pending": (I32, [P] * 6),
     "qmb200_gait_dev_stop": (I32, [P]),
     "qmb200_observation_update": (I32, [P] * 5),
     "qmb200_observation_update_dev": (I32, [P] * 6),

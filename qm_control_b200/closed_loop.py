@@ -175,6 +175,29 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     integers, every bound a scalar or [B].  The curriculum is cleared before the previous ranges are restored.  Returns also curriculum_level[ticks, B]
     (each robot's level in that record's window), episode_level[B, E] (-1 where a robot had no episode e), curriculum_state[B, CURRICULUM_STATE] at
     the end (_lib.CURRICULUM_STATE_LAYOUT), and each attached kind's *_params drawn at its episode's level."""
+    with Session(solver, duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start, torch_device=torch_device,
+                 sim_timer=sim_timer, friction_mu=friction_mu, payload=payload, pushes=pushes, model_payload=model_payload, terrain=terrain,
+                 payload_estimator=payload_estimator, state_estimator=state_estimator, sensor_noise=sensor_noise, attitude_filter=attitude_filter,
+                 slip_detector=slip_detector, ground_map=ground_map, commands=commands, tuning=tuning, respawn=respawn, randomize=randomize, spawn=spawn,
+                 metrics=metrics, timeline=timeline, curriculum=curriculum) as s:
+        rec = s.step(s.windows)
+        end = s.finish()   # synchronises the session's stream
+        out = {k: v if isinstance(v, np.ndarray) else v.cpu().numpy() for k, v in rec.items()}
+        out.update(end)
+        return out
+
+
+RUN_DEFAULTS = dict(gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None, friction_mu=None,
+                    payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None, attitude_filter=None,
+                    slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None, timeline=None, curriculum=None)
+
+
+def _run_specs(solver, steer, o):
+    """run's keywords o (RUN_DEFAULTS filled in) → the parsed specs; ValueError, before any solver call, when one is malformed.  steer: a run without
+    commands or timeline still rolls the device gait schedule, on an empty timeline."""
+    metrics, respawn, randomize, gait, commands, timeline, spawn, curriculum = (o[k] for k in ("metrics", "respawn", "randomize", "gait", "commands", "timeline", "spawn", "curriculum"))
+    payload_estimator, state_estimator, sensor_noise, ground_map, terrain = (o[k] for k in ("payload_estimator", "state_estimator", "sensor_noise", "ground_map", "terrain"))
+    attitude_filter, slip_detector, model_payload, tuning = (o[k] for k in ("attitude_filter", "slip_detector", "model_payload", "tuning"))
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else _respawn_spec(respawn)
@@ -202,6 +225,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     if slip_detector is not None and state_estimator is None:
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     gd = None if commands is None else _gait_commands(solver.batch, gait, commands)
+    if steer and commands is None and timeline is None:   # an empty timeline: the session's commands are the schedule's only input
+        gd = _gait_commands(solver.batch, gait, dict(t=np.zeros((solver.batch, 0)), gait=np.empty((solver.batch, 0), dtype=object)))
     tl = None if timeline is None else _timeline_spec(getattr(solver, "batch", None), gait, timeline, commands)
     if tl is not None:
         gd = tl["gd"]
@@ -221,41 +246,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
             rz["link"] |= _lib.EPISODE_MODEL_PAYLOAD
         if tn is not None and "friction_mu" in drawn:
             rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
-    # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
-    with contextlib.ExitStack() as scope:
-        if sp is not None:   # restored last: the earlier ranges are set again on the earlier library and robot terrain rows, which give their origins
-            scope.enter_context(_ranges(solver, "spawn"))
-        if terrain is not None:
-            scope.enter_context(_terrain(solver, terrain))
-        if ground_map is not None:
-            scope.enter_context(_ground_map(solver, terrain if ground_map is True else ground_map))
-        if model_payload is not None:
-            scope.enter_context(_model_payload(solver, model_payload, payload))
-        if tn is not None:
-            scope.enter_context(_robot_tuning(solver, tn, friction_mu))
-        if payload_estimator is not None:
-            scope.enter_context(_payload_estimator(solver, payload_estimator))
-        if state_estimator is not None:
-            scope.enter_context(_state_estimator(solver, state_estimator, sensor_noise))
-        if attitude_filter is not None:
-            scope.enter_context(_attitude_filter(solver, attitude_filter))
-        if slip_detector is not None:
-            scope.enter_context(_slip_detector(solver, slip_detector))
-        if friction_mu is not None or payload is not None or rz is not None:
-            scope.enter_context(_robot_params(solver, friction_mu, payload))
-        if rz is not None:
-            scope.enter_context(_ranges(solver, "episode"))
-        if tl is not None:
-            scope.enter_context(_ranges(solver, "timeline"))
-        if cu is not None:   # cleared first: the ranges go back to their base boxes, then the scopes above restore what they found
-            scope.callback(solver.curriculum_set)
-        if gd is not None:
-            scope.enter_context(_gait_dev(solver, gd))
-        if rs is not None:
-            scope.callback(solver.robot_image_clear)
-        return _run(solver, duration=duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start,
-                    torch_device=torch_device, sim_timer=sim_timer, pushes=pushes, est=payload_estimator is not None, se=state_estimator is not None,
-                    att=attitude_filter is not None, sl=slip_detector is not None, gd=gd, rs=rs, rz=rz, sp=sp, mt=metrics is not None, tl=tl, cu=cu)
+    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu)
 
 
 def _respawn_spec(respawn):
@@ -357,7 +348,7 @@ def _ranges(solver, kind):
     """the ranges of solver's kind ("episode", "spawn" or "timeline") draws in force, set again on exit"""
     prev = getattr(solver, kind + "_get_ranges")()
     try:
-        yield   # _run sets this run's ranges once it has read its fixed values
+        yield   # the session's start sets this run's ranges once it has read its fixed values
     finally:
         if prev is None:
             getattr(solver, kind + "_set_ranges")(None)
@@ -585,7 +576,7 @@ def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map
 def _gait_dev(solver, gd):
     solver.gait_dev_set_templates(gd["names"])
     try:
-        yield   # _run resets the schedule and loads the timeline once it knows the start time
+        yield   # the session's start resets the schedule and loads the timeline once it knows the start time
     finally:
         solver.gait_dev_stop()
 
@@ -692,7 +683,7 @@ def _state_estimator(solver, params, noise):
             solver.state_est_set_params(**params)
         if noise is not None:
             solver.sim_set_sensor_params(**(_lib.SENSOR_NOISE_REFERENCE if noise == "reference" else noise))
-        yield   # _run resets the estimator once it knows the start position
+        yield   # the session's start resets the estimator once it knows the start position
     finally:
         solver.state_est_stop()
         solver.sim_set_sensor_params(**prev_noise)
@@ -705,7 +696,7 @@ def _attitude_filter(solver, params):
     try:
         if isinstance(params, dict):
             solver.attitude_set_params(**params)
-        yield   # _run resets the filter right before its first reading
+        yield   # the session's start resets the filter right before its first reading
     finally:
         solver.attitude_stop()
         solver.attitude_set_params(**prev_params)
@@ -717,7 +708,7 @@ def _slip_detector(solver, params):
     try:
         if isinstance(params, dict):
             solver.slip_set_params(**params)
-        yield   # _run resets the detector with the estimator
+        yield   # the session's start resets the detector with the estimator
     finally:
         solver.slip_stop()
         solver.slip_set_params(**prev_params)
@@ -742,303 +733,507 @@ def _metrics_episodes(ticks, rs):
     return (ticks - 1) // max(shortest, 1) + 1
 
 
-def _run(solver, duration, gait, cmd_vel, wbc_period_ms, xy_yaw, t_start, torch_device, sim_timer, pushes, est=False, se=False, att=False, sl=False, gd=None,
-         rs=None, rz=None, sp=None, mt=False, tl=None, cu=None):
-    import torch
-    B = solver.batch; dev = torch.device(torch_device or "cuda:%d" % solver._cfg.device)
-    n_ms = int(round(duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
-    assert MPC_PERIOD_MS % wbc_period_ms == 0, "the WBC period must divide the MPC period"
-    cmd_vel = np.asarray(cmd_vel, dtype=np.float64)
-    if cmd_vel.shape not in ((4,), (B, 4)):
-        raise ValueError("closed_loop.run: cmd_vel must have shape (4,) or (%d, 4), got %s" % (B, cmd_vel.shape))
-    if pushes is not None:
-        t_on, t_dur, wrench = (np.asarray(a, dtype=np.float64) for a in pushes)
-        if t_on.shape != (B,) or t_dur.shape != (B,) or wrench.shape != (B, 12):
-            raise ValueError("closed_loop.run: pushes must be (t_on[%d], duration[%d], wrench[%d, 12])" % (B, B, B))
-    tops = {} if cu is None else dict(cu["tops"])   # each attached kind's top box, built from this run's values as its base box is
-    if rz is not None:   # the ranges: this run's values (entered after _robot_params: the handle's robot params are this run's plant), the named fields' bounds
-        EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}
-        rp = solver.sim_get_robot_params()
-        row = np.zeros((B, _lib.EPISODE))
-        row[:, EP["friction_mu"]] = solver.sim_get_params()["friction_mu"] if rp["friction_mu"] is None else rp["friction_mu"]
-        if rp["payload"] is not None:
-            row[:, EP["m_ee"]:EP["m_ee"] + 8] = rp["payload"]
+class Session:
+    """A closed loop stepped window by window: run's loop, with its live state on the device between windows and per-robot commands from device tensors.
+
+    Session(solver, duration, steer=False, **kw) takes run's keywords; duration fixes the capacities run computes from it (the host-tiled mode schedule's
+    horizon, the metrics rows' episodes) and the most windows step may take.  steer=True rolls the device gait schedule on an empty timeline when neither
+    commands nor timeline is given, so that command() can steer every robot.  Spec errors raise ValueError here, before any solver call.
+    with Session(...) as s: entering sets run's per-run overrides in run's order, reads the start state, saves the start image, begins episode 0 and
+    makes the blocking first solve (window 0's MPC tick); leaving restores the overrides in reverse.
+    s.step(windows=1) advances that many 10 ms windows and returns their per-window records (run's per-window keys; t a numpy array, the rest device
+    tensors [windows, B, ...]), enqueued on s.stream without a synchronisation: wait for s.stream before reading them on another stream.  The session
+    keeps no record of earlier chunks.
+    s.command(mask, gait=None, cmd_vel=None, ee_goal=None, ee_cmd_vel=None): one command for each masked robot, applied by its first MPC tick after the
+    call (Solver.gait_dev_command_dev; DESIGN.md §4.16).
+    s.state: the live device tensors (read-only: the loop writes them).  s.finish() closes the open episodes and returns run's end-of-run keys.
+    run(solver, duration, **kw) is Session + one step(windows) + finish()."""
+
+    def __init__(self, solver, duration=1.0, steer=False, **kw):
+        unknown = sorted(set(kw) - set(RUN_DEFAULTS))
+        if unknown:
+            raise TypeError("closed_loop.Session: unknown keyword argument(s) %s" % ", ".join(unknown))
+        self.solver, self.duration = solver, duration
+        self._o = dict(RUN_DEFAULTS, **kw)
+        self._spec = _run_specs(solver, steer, self._o)
+        sp, cu = self._spec["sp"], self._spec["cu"]
+        spawns = [x for x in (sp, cu["tops"].get("spawn") if cu is not None else None) if x is not None]
+        self._yaw_drawn = any("yaw" in x["fields"] and np.any(x["fields"]["yaw"][0] != x["fields"]["yaw"][1]) for x in spawns)
+        self._scope = None; self._open = False; self._finished = False
+
+    # ------------------------------------------------------------------------------------------------------------------------------------ scopes
+    def __enter__(self):
+        solver, o, p = self.solver, self._o, self._spec
+        sp, tn, rz, tl, cu, gd, rs = p["sp"], p["tn"], p["rz"], p["tl"], p["cu"], p["gd"], p["rs"]
+        # set in this order, restored in reverse: the estimator starts from the model payload in force, and "plant" reads this run's payload or the handle's
+        scope = self._scope = contextlib.ExitStack()
+        try:
+            if sp is not None:   # restored last: the earlier ranges are set again on the earlier library and robot terrain rows, which give their origins
+                scope.enter_context(_ranges(solver, "spawn"))
+            if o["terrain"] is not None:
+                scope.enter_context(_terrain(solver, o["terrain"]))
+            if o["ground_map"] is not None:
+                scope.enter_context(_ground_map(solver, o["terrain"] if o["ground_map"] is True else o["ground_map"]))
+            if o["model_payload"] is not None:
+                scope.enter_context(_model_payload(solver, o["model_payload"], o["payload"]))
+            if tn is not None:
+                scope.enter_context(_robot_tuning(solver, tn, o["friction_mu"]))
+            if o["payload_estimator"] is not None:
+                scope.enter_context(_payload_estimator(solver, o["payload_estimator"]))
+            if o["state_estimator"] is not None:
+                scope.enter_context(_state_estimator(solver, o["state_estimator"], o["sensor_noise"]))
+            if o["attitude_filter"] is not None:
+                scope.enter_context(_attitude_filter(solver, o["attitude_filter"]))
+            if o["slip_detector"] is not None:
+                scope.enter_context(_slip_detector(solver, o["slip_detector"]))
+            if o["friction_mu"] is not None or o["payload"] is not None or rz is not None:
+                scope.enter_context(_robot_params(solver, o["friction_mu"], o["payload"]))
+            if rz is not None:
+                scope.enter_context(_ranges(solver, "episode"))
+            if tl is not None:
+                scope.enter_context(_ranges(solver, "timeline"))
+            if cu is not None:   # cleared first: the ranges go back to their base boxes, then the scopes above restore what they found
+                scope.callback(solver.curriculum_set)
+            if gd is not None:
+                scope.enter_context(_gait_dev(solver, gd))
+            if rs is not None:
+                scope.callback(solver.robot_image_clear)
+            self._start()
+        except BaseException:
+            scope.__exit__(None, None, None)   # a failed start restores what it had set, as run's scope did
+            raise
+        self._open = True
+        return self
+
+    def __exit__(self, *exc):
+        self._open = False
+        return self._scope.__exit__(*exc)
+
+    # ------------------------------------------------------------------------------------------------------------------------------------ start
+    def _start(self):
+        """everything run does before its loop: the fixed values, the ranges, the start state, the start image, episode 0 and the blocking first solve"""
+        import torch
+        solver, o, p = self.solver, self._o, self._spec
+        rs, rz, sp, tl, cu, gd = p["rs"], p["rz"], p["sp"], p["tl"], p["cu"], p["gd"]
+        est, se, att, sl, mt = (o[k] is not None for k in ("payload_estimator", "state_estimator", "attitude_filter", "slip_detector", "metrics"))
+        gait, cmd_vel, wbc_period_ms, t_start, pushes = o["gait"], o["cmd_vel"], o["wbc_period_ms"], o["t_start"], o["pushes"]
+        B = solver.batch; dev = self.device = torch.device(o["torch_device"] or "cuda:%d" % solver._cfg.device)
+        n_ms = int(round(self.duration * 1e3)); assert n_ms > 0 and n_ms % MPC_PERIOD_MS == 0, "duration must be a multiple of 10 ms"
+        assert MPC_PERIOD_MS % wbc_period_ms == 0, "the WBC period must divide the MPC period"
+        cmd_vel = np.asarray(cmd_vel, dtype=np.float64)
+        if cmd_vel.shape not in ((4,), (B, 4)):
+            raise ValueError("closed_loop.run: cmd_vel must have shape (4,) or (%d, 4), got %s" % (B, cmd_vel.shape))
         if pushes is not None:
-            row[:, EP["push_t_on"]] = t_on; row[:, EP["push_duration"]] = t_dur; row[:, EP["f_base_x"]:EP["f_base_x"] + 12] = wrench
-        row[:, EP["cmd_vel_x"]:EP["cmd_vel_x"] + 4] = cmd_vel
-        lo, hi = _box(_lib.EPISODE_LAYOUT, row, rz); solver.episode_set_ranges(lo, hi, rz["seed"])
-        if "episode" in tops:
-            tops["episode"] = _box(_lib.EPISODE_LAYOUT, row, tops["episode"]); hi = np.maximum(hi, tops["episode"][1])
-        if pushes is None and np.any(hi[:, EP["push_duration"]] > 0.0):   # the draws overwrite these rows before the first solve
-            t_on, t_dur, wrench = np.zeros(B), np.zeros(B), np.zeros((B, 12)); pushes = (t_on, t_dur, wrench)
-    xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
-    if sp is not None:   # the ranges: this run's values (entered after _terrain: the robot terrain rows are this run's), the named columns' bounds
-        SP = {n: i for i, n in enumerate(_lib.SPAWN_LAYOUT)}
-        rt = solver.sim_get_robot_terrain()
-        yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)   # the same heading within [-pi, pi]
-        row = np.zeros((B, _lib.SPAWN)); row[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; row[:, SP["yaw"]] = yaw
-        solver.spawn_set_ranges(*_box(_lib.SPAWN_LAYOUT, row, sp), sp["seed"])
-        if "spawn" in tops:
-            tops["spawn"] = _box(_lib.SPAWN_LAYOUT, row, tops["spawn"])
-    if tl is not None:
-        cmd_b = np.broadcast_to(cmd_vel, (B, 4))
-        solver.timeline_set_ranges(tl["n"], *_timeline_box(tl, cmd_b, t_start), tl["seed"])
-        if "timeline" in tops:
-            tops["timeline"] = _timeline_box(tops["timeline"], cmd_b, t_start)
-    if cu is not None:   # the levels start at the run's start levels; each kind's ranges set above are its level 0
-        rows = np.zeros((B, _lib.CURRICULUM))
-        rows[:, 0] = cu["start"]; rows[:, 1] = cu["up_after"]; rows[:, 2] = cu["down_after"]
-        for i, thr in enumerate(cu["thresholds"]):
-            rows[:, 3 + i] = thr
-        solver.curriculum_set(cu["levels"], rows, cu["conditions"])
-        for kind, (lo, hi) in tops.items():
-            solver.curriculum_attach(kind, lo, hi)
-    stream = torch.cuda.Stream(device=dev); s = stream.cuda_stream
-    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
-    i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
+            t_on, t_dur, wrench = (np.asarray(a, dtype=np.float64) for a in pushes)
+            if t_on.shape != (B,) or t_dur.shape != (B,) or wrench.shape != (B, 12):
+                raise ValueError("closed_loop.run: pushes must be (t_on[%d], duration[%d], wrench[%d, 12])" % (B, B, B))
+        tops = {} if cu is None else dict(cu["tops"])   # each attached kind's top box, built from this run's values as its base box is
+        if rz is not None:   # the ranges: this run's values (entered after _robot_params: the handle's robot params are this run's plant), the named fields' bounds
+            EP = {n: i for i, n in enumerate(_lib.EPISODE_LAYOUT)}
+            rp = solver.sim_get_robot_params()
+            row = np.zeros((B, _lib.EPISODE))
+            row[:, EP["friction_mu"]] = solver.sim_get_params()["friction_mu"] if rp["friction_mu"] is None else rp["friction_mu"]
+            if rp["payload"] is not None:
+                row[:, EP["m_ee"]:EP["m_ee"] + 8] = rp["payload"]
+            if pushes is not None:
+                row[:, EP["push_t_on"]] = t_on; row[:, EP["push_duration"]] = t_dur; row[:, EP["f_base_x"]:EP["f_base_x"] + 12] = wrench
+            row[:, EP["cmd_vel_x"]:EP["cmd_vel_x"] + 4] = cmd_vel
+            lo, hi = _box(_lib.EPISODE_LAYOUT, row, rz); solver.episode_set_ranges(lo, hi, rz["seed"])
+            if "episode" in tops:
+                tops["episode"] = _box(_lib.EPISODE_LAYOUT, row, tops["episode"]); hi = np.maximum(hi, tops["episode"][1])
+            if pushes is None and np.any(hi[:, EP["push_duration"]] > 0.0):   # the draws overwrite these rows before the first solve
+                t_on, t_dur, wrench = np.zeros(B), np.zeros(B), np.zeros((B, 12)); pushes = (t_on, t_dur, wrench)
+        xy_yaw = o["xy_yaw"]
+        xy = np.zeros((B, 3)) if xy_yaw is None else np.asarray(xy_yaw, dtype=np.float64).reshape(B, 3)
+        if sp is not None:   # the ranges: this run's values (entered after _terrain: the robot terrain rows are this run's), the named columns' bounds
+            SP = {n: i for i, n in enumerate(_lib.SPAWN_LAYOUT)}
+            rt = solver.sim_get_robot_terrain()
+            yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)   # the same heading within [-pi, pi]
+            row = np.zeros((B, _lib.SPAWN)); row[:, SP["tile"]] = -1.0 if rt is None else rt["tile"]; row[:, SP["yaw"]] = yaw
+            solver.spawn_set_ranges(*_box(_lib.SPAWN_LAYOUT, row, sp), sp["seed"])
+            if "spawn" in tops:
+                tops["spawn"] = _box(_lib.SPAWN_LAYOUT, row, tops["spawn"])
+        if tl is not None:
+            cmd_b = np.broadcast_to(cmd_vel, (B, 4))
+            solver.timeline_set_ranges(tl["n"], *_timeline_box(tl, cmd_b, t_start), tl["seed"])
+            if "timeline" in tops:
+                tops["timeline"] = _timeline_box(tops["timeline"], cmd_b, t_start)
+        if cu is not None:   # the levels start at the run's start levels; each kind's ranges set above are its level 0
+            rows = np.zeros((B, _lib.CURRICULUM))
+            rows[:, 0] = cu["start"]; rows[:, 1] = cu["up_after"]; rows[:, 2] = cu["down_after"]
+            for i, thr in enumerate(cu["thresholds"]):
+                rows[:, 3 + i] = thr
+            solver.curriculum_set(cu["levels"], rows, cu["conditions"])
+            for kind, (lo, hi) in tops.items():
+                solver.curriculum_attach(kind, lo, hi)
+        stream = self.stream = torch.cuda.Stream(device=dev); s = self._s = stream.cuda_stream
+        f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+        i32 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.int32), device=dev)
+        self.B, self.windows, self.t_start, self._wbc, self._n_ms, self._k = B, n_ms // MPC_PERIOD_MS, t_start, wbc_period_ms, n_ms, 0
+        self._est, self._se, self._att, self._sl, self._mt, self._tops = est, se, att, sl, mt, tops
 
-    # ---- plant state, the first measurement, the controller's members (host → device once) ----
-    q0, v0 = solver.sim_standing_state(xy)
-    t_obs0 = t_start - wbc_period_ms * 1e-3   # observation clock of `starting`; the first update brings it to t_start, the plant's clock
-    if gd is None:
-        ev, md, ne = _schedules(gait, B, t_start, t_obs0, t_start + duration + solver.time_horizon + 1.0)
-    else:   # the first gait step writes the rows
-        ev, md, ne = np.zeros((B, EMAX)), np.full((B, EMAX + 1), 15, dtype=np.int32), np.zeros(B, dtype=np.int32)
-    with torch.cuda.stream(stream):
-        q = f64(q0); v = f64(v0); rbd = torch.zeros((B, RBD), dtype=torch.float64, device=dev)
-        contact = torch.zeros(B, dtype=torch.int32, device=dev); sim_st = torch.zeros_like(contact); hw_st = torch.zeros_like(contact); ctl_st = torch.zeros_like(contact)
-        acc_st = torch.zeros_like(contact)
-        effort = torch.zeros((B, 18), dtype=torch.float64, device=dev); jpos = torch.zeros_like(effort); jvel = torch.zeros_like(effort)
-        if se:   # the controller's measurement: the estimator's rbd_est in place of the plant's rbd
-            v_prev = torch.zeros_like(v); sensors = torch.zeros((B, SENSORS), dtype=torch.float64, device=dev); rbd_est = torch.zeros_like(rbd)
-            se_st = torch.zeros_like(contact); v_prev.copy_(v)
-            if att:
-                at_st = torch.zeros_like(contact)
-            if sl:   # the estimator reads the trusted stance mask in place of the plant's contact mask
-                stance = torch.zeros_like(contact); slip = torch.zeros_like(contact); sl_st = torch.zeros_like(contact); slip_acc = torch.zeros_like(contact)
-    stream.synchronize()
-    solver.sim_step_dev(1e-6, effort, q, v, rbd, contact, sim_st, s)   # a 1 us physics step with zero effort reads the first measured state
-    meas = rbd
-    if se:
-        solver.sim_read_sensors_dev(1e-6, -1, q, v, v_prev, sensors, s)
-        stream.synchronize()
-        solver.state_est_reset(q0[:, 0:3])
-        if att:
-            solver.attitude_reset()
-            solver.attitude_step_dev(1e-6, sensors, at_st, s)   # the first call after the reset takes the reading
-        se_contact = contact
-        if sl:
-            solver.slip_reset()
-            solver.slip_step_dev(1e-6, sensors, contact, stance, slip, sl_st, s)   # passes the contact mask through: the estimator has had no call yet
-            se_contact = stance
-        solver.state_est_step_dev(1e-6, sensors, se_contact, rbd_est, se_st, s)   # the first call after the reset places the feet
-        meas = rbd_est
-    stream.synchronize()
-    rbd_h = rbd.cpu().numpy()
-    x_obs0 = solver.centroidal_state_from_rbd(meas.cpu().numpy())
-    with torch.cuda.stream(stream):
-        t_obs = f64(np.full(B, t_obs0)); x_obs = f64(x_obs0)
-        joint_cmd = torch.zeros((B, 18, 5), dtype=torch.float64, device=dev); arm_pos = torch.zeros((B, 6), dtype=torch.float64, device=dev); last_time = f64(np.full(B, t_obs0))
-        cmd54 = torch.zeros((B, 54), dtype=torch.float64, device=dev)
-        cmd7 = torch.zeros((B, 7), dtype=torch.float64, device=dev); cmd7[:, :4] = f64(cmd_vel[None, :4] if cmd_vel.ndim == 1 else cmd_vel)
-        last_ee = f64(solver.initial_ee_target()); ee_state = torch.zeros((B, 7), dtype=torch.float64, device=dev)
-        prob = dict(t0=t_obs, x0=x_obs, n_events=i32(ne), event_times=f64(ev), modes=i32(md),
-                    n_target=torch.zeros(B, dtype=torch.int32, device=dev), target_times=torch.zeros((B, KMAX), dtype=torch.float64, device=dev),
-                    target_states=torch.zeros((B, KMAX, TARGET), dtype=torch.float64, device=dev))
-        period = f64(np.full(B, wbc_period_ms * 1e-3)); hw_period = f64(np.full(B, 1e-3)); hw_time = torch.zeros(B, dtype=torch.float64, device=dev)
-        ticks = n_ms // MPC_PERIOD_MS
-        rec_base = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev); rec_ee = torch.zeros((ticks, B, 7), dtype=torch.float64, device=dev)
-        rec_st = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
-        if est:
-            est_st = torch.zeros_like(contact); rec_pl = torch.zeros((ticks, B, 8), dtype=torch.float64, device=dev)   # row i: the rows of window i's MPC tick
-        if se:
-            rec_base_est = torch.zeros((ticks, B, 6), dtype=torch.float64, device=dev)
-        if sl:
-            rec_slip = torch.zeros((ticks, B), dtype=torch.int32, device=dev)
-        if gd is not None:
-            gait_st = torch.zeros_like(contact); rec_gait = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_mode = torch.zeros_like(rec_gait)
-            rec_kind = torch.zeros_like(rec_gait); rec_ee_target = torch.zeros((ticks, B, 7), dtype=torch.float64, device=dev)
-        push = None
-        if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
-            push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench), zero=torch.zeros((B, 12), dtype=torch.float64, device=dev),
-                        now=torch.zeros((B, 12), dtype=torch.float64, device=dev))
-    stream.synchronize()
-    if gd is not None:
-        solver.gait_dev_reset(gd["gait"], np.full(B, t_start))
-        solver.gait_dev_set_commands(t_start + gd["t"], gd["tmpl"], gd["cmd_vel"], **gd["ee"])
-    solver.hw_set_delay(HW_DELAY)
-
-    def mpc_tick(i):
-        if est:
-            solver.payload_est_commit_dev(s); solver.get_model_payload_dev(rec_pl[i], s)
-        ee_state.copy_(meas[:, 48:55])
+        # ---- plant state, the first measurement, the controller's members (host → device once) ----
+        q0, v0 = solver.sim_standing_state(xy)
+        t_obs0 = t_start - wbc_period_ms * 1e-3   # observation clock of `starting`; the first update brings it to t_start, the plant's clock
         if gd is None:
-            solver.target_trajectories_dev(0, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
+            ev, md, ne = _schedules(gait, B, t_start, t_obs0, t_start + self.duration + solver.time_horizon + 1.0)
+        else:   # the first gait step writes the rows
+            ev, md, ne = np.zeros((B, EMAX)), np.full((B, EMAX + 1), 15, dtype=np.int32), np.zeros(B, dtype=np.int32)
+        with torch.cuda.stream(stream):
+            q = self.q = f64(q0); v = self.v = f64(v0); rbd = self.rbd = torch.zeros((B, RBD), dtype=torch.float64, device=dev)
+            contact = self.contact = torch.zeros(B, dtype=torch.int32, device=dev)
+            self.sim_st = torch.zeros_like(contact); self.hw_st = torch.zeros_like(contact); self.ctl_st = torch.zeros_like(contact)
+            self.acc_st = torch.zeros_like(contact)
+            self.effort = torch.zeros((B, 18), dtype=torch.float64, device=dev); self.jpos = torch.zeros_like(self.effort); self.jvel = torch.zeros_like(self.effort)
+            if se:   # the controller's measurement: the estimator's rbd_est in place of the plant's rbd
+                v_prev = self.v_prev = torch.zeros_like(v); sensors = self.sensors = torch.zeros((B, SENSORS), dtype=torch.float64, device=dev)
+                rbd_est = self.rbd_est = torch.zeros_like(rbd)
+                self.se_st = torch.zeros_like(contact); v_prev.copy_(v)
+                if att:
+                    self.at_st = torch.zeros_like(contact)
+                if sl:   # the estimator reads the trusted stance mask in place of the plant's contact mask
+                    stance = self.stance = torch.zeros_like(contact); self.slip = torch.zeros_like(contact); self.sl_st = torch.zeros_like(contact)
+                    self.slip_acc = torch.zeros_like(contact)
+        stream.synchronize()
+        solver.sim_step_dev(1e-6, self.effort, q, v, rbd, contact, self.sim_st, s)   # a 1 us physics step with zero effort reads the first measured state
+        meas = rbd
+        if se:
+            solver.sim_read_sensors_dev(1e-6, -1, q, v, v_prev, sensors, s)
+            stream.synchronize()
+            solver.state_est_reset(q0[:, 0:3])
+            if att:
+                solver.attitude_reset()
+                solver.attitude_step_dev(1e-6, sensors, self.at_st, s)   # the first call after the reset takes the reading
+            self.se_contact = contact
+            if sl:
+                solver.slip_reset()
+                solver.slip_step_dev(1e-6, sensors, contact, stance, self.slip, self.sl_st, s)   # passes the contact mask through: the estimator has had no call yet
+                self.se_contact = stance
+            solver.state_est_step_dev(1e-6, sensors, self.se_contact, rbd_est, self.se_st, s)   # the first call after the reset places the feet
+            meas = rbd_est
+        self.meas = meas
+        stream.synchronize()
+        rbd_h = rbd.cpu().numpy()
+        x_obs0 = solver.centroidal_state_from_rbd(meas.cpu().numpy())
+        self._start_out = dict(start_base=np.c_[q0[:, 0:3], q0[:, 3:6]], start_ee=rbd_h[:, 48:55])
+        with torch.cuda.stream(stream):
+            t_obs = self.t_obs = f64(np.full(B, t_obs0)); x_obs = self.x_obs = f64(x_obs0)
+            self.joint_cmd = torch.zeros((B, 18, 5), dtype=torch.float64, device=dev); self.arm_pos = torch.zeros((B, 6), dtype=torch.float64, device=dev)
+            self.last_time = f64(np.full(B, t_obs0))
+            self.cmd54 = torch.zeros((B, 54), dtype=torch.float64, device=dev)
+            cmd7 = self.cmd7 = torch.zeros((B, 7), dtype=torch.float64, device=dev); cmd7[:, :4] = f64(cmd_vel[None, :4] if cmd_vel.ndim == 1 else cmd_vel)
+            self.last_ee = f64(solver.initial_ee_target()); self.ee_state = torch.zeros((B, 7), dtype=torch.float64, device=dev)
+            prob = self.prob = dict(t0=t_obs, x0=x_obs, n_events=i32(ne), event_times=f64(ev), modes=i32(md),
+                                    n_target=torch.zeros(B, dtype=torch.int32, device=dev), target_times=torch.zeros((B, KMAX), dtype=torch.float64, device=dev),
+                                    target_states=torch.zeros((B, KMAX, TARGET), dtype=torch.float64, device=dev))
+            self.period = f64(np.full(B, wbc_period_ms * 1e-3)); self.hw_period = f64(np.full(B, 1e-3)); self.hw_time = torch.zeros(B, dtype=torch.float64, device=dev)
+            ticks = self.windows
+            if est:   # the model payload rows committed at the current window's MPC tick
+                self.est_st = torch.zeros_like(contact); self.tick_pl = torch.zeros((B, 8), dtype=torch.float64, device=dev)
+            if gd is not None:   # the current window's gait step: active template, mode, target kind
+                self.gait_st = torch.zeros_like(contact); self.tick_gait = torch.zeros_like(contact); self.tick_mode = torch.zeros_like(contact)
+                self.tick_kind = torch.zeros_like(contact)
+                self.cmd_st = torch.zeros_like(contact); self.cmd_acc = torch.zeros_like(contact); self._commanded = False
+            push = self.push = None
+            if pushes is not None:   # robot b is pushed in plant step k (start k ms after the start) when t_on <= k ms < t_on + duration
+                push = self.push = dict(on=f64(t_on * 1e3 - 1e-6), off=f64((t_on + t_dur) * 1e3 - 1e-6), wrench=f64(wrench),
+                                        zero=torch.zeros((B, 12), dtype=torch.float64, device=dev), now=torch.zeros((B, 12), dtype=torch.float64, device=dev))
+        stream.synchronize()
+        if gd is not None:
+            solver.gait_dev_reset(gd["gait"], np.full(B, t_start))
+            solver.gait_dev_set_commands(t_start + gd["t"], gd["tmpl"], gd["cmd_vel"], **gd["ee"])
+        solver.hw_set_delay(HW_DELAY)
+
+        if rs is not None:   # the start image: the library's rows and the loop's own, then one restore of every robot through the cold path of every later one
+            self.own = [q, v, rbd, contact, t_obs, x_obs, self.joint_cmd, self.arm_pos, self.last_time, self.cmd54, cmd7, self.last_ee, prob["n_events"],
+                        prob["event_times"], prob["modes"], prob["n_target"], prob["target_times"], prob["target_states"]] + \
+                       ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
+            solver.robot_image_save()
+            with torch.cuda.stream(stream):
+                self.start = [a.clone() for a in self.own]
+                self.k0 = torch.zeros(B, dtype=torch.int64, device=dev); self.dk = torch.zeros_like(self.k0)   # each robot's episode start (plant step), and k - k0
+                episode = self.episode = torch.zeros(B, dtype=torch.int32, device=dev); self.fall_count = torch.zeros_like(episode)
+                self.fallen = torch.zeros_like(episode); self.due = torch.ones_like(episode)
+                if mt or cu is not None:   # the fall part of due: why a closed episode ended
+                    self.due_fall = torch.zeros_like(episode); self.mt_end = torch.zeros_like(episode)
+                if cu is not None:   # each robot's level, and the level of each episode it began
+                    self.cu_level = i32(np.broadcast_to(cu["start"], (B,)))
+                    self.ep_level = torch.full((B, _metrics_episodes(ticks, rs)), -1, dtype=torch.int32, device=dev); self._level_begun(self.due)
+            solver.robot_image_restore_dev(self.due, s)
+        if mt:   # every robot's open episode (zeros: open and empty) and its closed rows
+            with torch.cuda.stream(stream):
+                self.mt_acc = torch.zeros((B, _lib.METRICS_ACC), dtype=torch.float64, device=dev)
+                self.mt_out = torch.full((B, _metrics_episodes(ticks, rs), _lib.METRICS), np.nan, dtype=torch.float64, device=dev)
+
+        if rz is not None or sp is not None or tl is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
+            with torch.cuda.stream(stream):
+                self.ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev) if rz is not None else None
+                self.sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev) if sp is not None else None
+                self.tl_rows = torch.zeros((B, tl["n"], _lib.TIMELINE_CMD), dtype=torch.float64, device=dev) if tl is not None else None
+                if rs is None:
+                    self._begin(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
+                else:
+                    self._begin(self.due, self.episode)
+
+        with torch.cuda.stream(stream):
+            self._mpc_tick(); stream.synchronize()          # QMController::starting: one blocking solve before the loop
+
+    # ------------------------------------------------------------------------------------------------------------------------------------ the loop's parts
+    def _mpc_tick(self):
+        solver, s, gd, prob = self.solver, self._s, self._spec["gd"], self.prob
+        if self._est:
+            solver.payload_est_commit_dev(s); solver.get_model_payload_dev(self.tick_pl, s)
+        self.ee_state.copy_(self.meas[:, 48:55])
+        if gd is None:
+            solver.target_trajectories_dev(0, self.cmd7, self.t_obs, self.x_obs, self.ee_state, self.last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
         else:   # the step's target kinds go straight to the target call, and stay in the record
-            kind = rec_kind[i]
-            solver.gait_dev_step_dev(t_obs, prob, cmd7, rec_gait[i], rec_mode[i], gait_st, s, target_kind=kind)
-            acc_st.bitwise_or_(gait_st)
-            solver.target_trajectories_dev(kind, cmd7, t_obs, x_obs, ee_state, last_ee, prob["n_target"], prob["target_times"], prob["target_states"], s)
-            rec_ee_target[i] = prob["target_states"][:, 1, 30:37]
+            solver.gait_dev_step_dev(self.t_obs, prob, self.cmd7, self.tick_gait, self.tick_mode, self.gait_st, s, target_kind=self.tick_kind)
+            self.acc_st.bitwise_or_(self.gait_st)
+            if self._commanded:   # the status of the commands this step applied goes into the window it opens
+                self.acc_st.bitwise_or_(self.cmd_acc); self.cmd_acc.zero_(); self._commanded = False
+            solver.target_trajectories_dev(self.tick_kind, self.cmd7, self.t_obs, self.x_obs, self.ee_state, self.last_ee, prob["n_target"], prob["target_times"],
+                                           prob["target_states"], s)
         solver.mpc_solve_dev(prob, s)
 
-    if rs is not None:   # the start image: the library's rows and the loop's own, then one restore of every robot through the cold path of every later one
-        own = [q, v, rbd, contact, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, cmd7, last_ee, prob["n_events"], prob["event_times"], prob["modes"],
-               prob["n_target"], prob["target_times"], prob["target_states"]] + ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
-        solver.robot_image_save()
-        with torch.cuda.stream(stream):
-            start = [a.clone() for a in own]
-            k0 = torch.zeros(B, dtype=torch.int64, device=dev); dk = torch.zeros_like(k0)   # each robot's episode start (plant step), and k - k0
-            episode = torch.zeros(B, dtype=torch.int32, device=dev); fall_count = torch.zeros_like(episode); fallen = torch.zeros_like(episode)
-            due = torch.ones_like(episode); rec_episode = torch.zeros((ticks, B), dtype=torch.int32, device=dev); rec_fallen = torch.zeros_like(rec_episode)
-            if mt or cu is not None:   # the fall part of due: why a closed episode ended
-                due_fall = torch.zeros_like(episode); mt_end = torch.zeros_like(episode)
-            if cu is not None:   # each robot's level, recorded beside its episode
-                cu_level = i32(np.broadcast_to(cu["start"], (B,))); rec_level = torch.zeros_like(rec_episode)
-        solver.robot_image_restore_dev(due, s)
-    if mt:   # every robot's open episode (zeros: open and empty) and its closed rows
-        with torch.cuda.stream(stream):
-            mt_acc = torch.zeros((B, _lib.METRICS_ACC), dtype=torch.float64, device=dev)
-            mt_out = torch.full((B, _metrics_episodes(ticks, rs), _lib.METRICS), np.nan, dtype=torch.float64, device=dev)
-
-    def respawn(k):   # the robots due restart at window boundary k: their episode closes, their level moves, then the library's rows, the loop's, their new plant
-        if mt or cu is not None:
-            mt_end.copy_(due_fall).neg_().add_(2)   # 1: the fall rule, 2: every
-        if mt:
-            solver.metrics_close_dev(due, mt_end, episode, mt_acc, mt_out, acc_st, s)
-        if cu is not None:   # reads the row the close just wrote; writes the ranges the draws of begin() read
-            solver.curriculum_update_dev(due, mt_end, episode, mt_out if mt else None, cu_level, acc_st, s)
+    def _respawn(self, k):   # the robots due restart at window boundary k: their episode closes, their level moves, then the library's rows, the loop's, their new plant
+        import torch
+        solver, s, cu, due = self.solver, self._s, self._spec["cu"], self.due
+        if self._mt or cu is not None:
+            self.mt_end.copy_(self.due_fall).neg_().add_(2)   # 1: the fall rule, 2: every
+        if self._mt:
+            solver.metrics_close_dev(due, self.mt_end, self.episode, self.mt_acc, self.mt_out, self.acc_st, s)
+        if cu is not None:   # reads the row the close just wrote; writes the ranges the draws of _begin() read
+            solver.curriculum_update_dev(due, self.mt_end, self.episode, self.mt_out if self._mt else None, self.cu_level, self.acc_st, s)
         solver.robot_image_restore_dev(due, s)
         m = due.bool()
-        for a, a0 in zip(own, start):
-            a.copy_(torch.where(m.view((B,) + (1,) * (a.dim() - 1)), a0, a))
-        k0.copy_(torch.where(m, k, k0)); episode.add_(due); fall_count.masked_fill_(m, 0)
-        begin(due, episode)
+        for a, a0 in zip(self.own, self.start):
+            a.copy_(torch.where(m.view((self.B,) + (1,) * (a.dim() - 1)), a0, a))
+        self.k0.copy_(torch.where(m, k, self.k0)); self.episode.add_(due); self.fall_count.masked_fill_(m, 0)
+        if cu is not None:
+            self._level_begun(due)
+        self._begin(due, self.episode)
 
-    def begin(mask, idx):   # the masked robots begin episode idx: their plant's draw, then their spawn, then their command timeline
-        if rz is not None:
-            draw(mask, idx)
-        if sp is not None:
-            stand(mask, idx)
-        if tl is not None:
-            solver.timeline_sample_dev(mask, idx, tl_rows, s)
+    def _level_begun(self, mask):   # the masked robots begin their episode at their current level
+        import torch
+        rows = torch.arange(self.B, device=self.device); e = self.episode.long()
+        self.ep_level[rows, e] = torch.where(mask.bool(), self.cu_level, self.ep_level[rows, e])
 
-    def draw(mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
-        solver.episode_sample_dev(mask, idx, ep_rows, rz["link"], s)
+    def _begin(self, mask, idx):   # the masked robots begin episode idx: their plant's draw, then their spawn, then their command timeline
+        p, solver, s = self._spec, self.solver, self._s
+        if p["rz"] is not None:
+            self._draw(mask, idx)
+        if p["sp"] is not None:   # new ground under them, their start state there
+            solver.spawn_sample_dev(mask, idx, self.sp_rows, self.q, self.v, self.rbd, self.contact, self.x_obs, self.last_ee, self.rbd_est if self._se else None,
+                                    p["sp"]["link"], s)
+        if p["tl"] is not None:
+            solver.timeline_sample_dev(mask, idx, self.tl_rows, s)
+
+    def _draw(self, mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
+        import torch
+        ep_rows, push = self.ep_rows, self.push
+        self.solver.episode_sample_dev(mask, idx, ep_rows, self._spec["rz"]["link"], self._s)
         m = mask.bool()
-        cmd7[:, :4] = torch.where(m[:, None], ep_rows[:, 23:27], cmd7[:, :4])
+        self.cmd7[:, :4] = torch.where(m[:, None], ep_rows[:, 23:27], self.cmd7[:, :4])
         if push is not None:
             on = ep_rows[:, 9] * 1e3 - 1e-6; off = (ep_rows[:, 9] + ep_rows[:, 10]) * 1e3 - 1e-6
             push["on"].copy_(torch.where(m, on, push["on"])); push["off"].copy_(torch.where(m, off, push["off"]))
             push["wrench"].copy_(torch.where(m[:, None], ep_rows[:, 11:23], push["wrench"]))
 
-    def stand(mask, idx):   # the masked robots spawn episode idx: new ground under them, their start state there
-        solver.spawn_sample_dev(mask, idx, sp_rows, q, v, rbd, contact, x_obs, last_ee, rbd_est if se else None, sp["link"], s)
-
-    if rz is not None or sp is not None or tl is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
-        with torch.cuda.stream(stream):
-            ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev) if rz is not None else None
-            sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev) if sp is not None else None
-            tl_rows = torch.zeros((B, tl["n"], _lib.TIMELINE_CMD), dtype=torch.float64, device=dev) if tl is not None else None
-            if rs is None:
-                begin(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
-            else:
-                begin(due, episode)
-
-    with torch.cuda.stream(stream):
-        mpc_tick(0); stream.synchronize()          # QMController::starting: one blocking solve before the loop
-        for k in range(n_ms):
-            if k % MPC_PERIOD_MS == 0 and k > 0:
-                if rs is not None:
-                    respawn(k)
-                mpc_tick(k // MPC_PERIOD_MS)
-            if k % wbc_period_ms == 0:
-                solver.update_dev(meas, period, t_obs, x_obs, joint_cmd, arm_pos, last_time, cmd54, ctl_st, s)
-                acc_st.bitwise_or_(ctl_st)
-            if rs is None:
-                hw_time.fill_(t_start + k * 1e-3)
-            else:   # the robot's episode clock
-                torch.sub(k0, k, out=dk).neg_(); hw_time.copy_(dk).mul_(1e-3).add_(t_start)
-            jpos.copy_(q[:, 6:]); jvel.copy_(v[:, 6:])
-            solver.hw_write_dev(hw_time, hw_period, joint_cmd, jpos, jvel, effort, hw_st, s)
+    # ------------------------------------------------------------------------------------------------------------------------------------ public
+    def step(self, windows=1):
+        """Advance `windows` 10 ms windows → their records: t [windows] (numpy, the window ends), and device tensors base [windows, B, 6], ee, status
+        and the optional records of run, row i for the session's window (done + i).  Enqueued on self.stream; no synchronisation."""
+        import torch
+        if not self._open or self._finished:
+            raise ValueError("closed_loop.Session.step: the session is not open (enter it with `with`; finish() ends it)")
+        if isinstance(windows, (bool, np.bool_)) or not isinstance(windows, (int, np.integer)) or windows < 1:
+            raise ValueError("closed_loop.Session.step: windows must be an integer >= 1, got %r" % (windows,))
+        i0 = self._k // MPC_PERIOD_MS
+        if i0 + windows > self.windows:
+            raise ValueError("closed_loop.Session.step: %d windows past window %d exceed the session's %d (its duration, %g s)" % (windows, i0, self.windows, self.duration))
+        solver, s, p, B, dev = self.solver, self._s, self._spec, self.B, self.device
+        rs, cu, gd, se, sl, est, mt, att = p["rs"], p["cu"], p["gd"], self._se, self._sl, self._est, self._mt, self._att
+        q, v, rbd, contact, acc_st, push, sim_timer = self.q, self.v, self.rbd, self.contact, self.acc_st, self.push, self._o["sim_timer"]
+        n = windows
+        with torch.cuda.stream(self.stream):
+            rec = dict(t=self.t_start + np.arange(i0 + 1, i0 + n + 1) * MPC_PERIOD_MS * 1e-3, base=torch.zeros((n, B, 6), dtype=torch.float64, device=dev),
+                       ee=torch.zeros((n, B, 7), dtype=torch.float64, device=dev), status=torch.zeros((n, B), dtype=torch.int32, device=dev))
+            if est:   # row i: the rows of window i's MPC tick
+                rec["payload_est"] = torch.zeros((n, B, 8), dtype=torch.float64, device=dev)
             if se:
-                v_prev.copy_(v)
-            if sim_timer:
-                sim_timer(True)
-            if push is not None:
-                kk = k if rs is None else dk   # plant steps since the episode's start
-                torch.where(((push["on"] <= kk) & (push["off"] > kk))[:, None], push["wrench"], push["zero"], out=push["now"])
-            solver.sim_step_dev(1e-3, effort, q, v, rbd, contact, sim_st, s, wrench=None if push is None else push["now"])
-            if sim_timer:
-                sim_timer(False)
-            acc_st.bitwise_or_(hw_st).bitwise_or_(sim_st)
-            if se:
-                solver.sim_read_sensors_dev(1e-3, k, q, v, v_prev, sensors, s)
-                if att:
-                    solver.attitude_step_dev(1e-3, sensors, at_st, s)
-                    acc_st.bitwise_or_(at_st)
-                if sl:
-                    solver.slip_step_dev(1e-3, sensors, contact, stance, slip, sl_st, s)
-                    acc_st.bitwise_or_(sl_st); slip_acc.bitwise_or_(slip)
-                solver.state_est_step_dev(1e-3, sensors, se_contact, rbd_est, se_st, s)
-                acc_st.bitwise_or_(se_st)
-            if est:
-                solver.payload_est_step_dev(1e-3, effort, meas, est_st, s)
-                acc_st.bitwise_or_(est_st)
-            if mt:   # the plant's truth after the step, on the robot's episode clock, with the window's status so far
-                solver.metrics_step_dev(1e-3, rbd, contact, effort, cmd7, prob["n_target"], prob["target_times"], prob["target_states"], hw_time, acc_st, mt_acc,
-                                        kind=None if gd is None else rec_kind[k // MPC_PERIOD_MS], rbd_est=rbd_est if se else None, stream=s)
-            if (k + 1) % MPC_PERIOD_MS == 0:
-                i = (k + 1) // MPC_PERIOD_MS - 1
-                rec_base[i, :, 0:3] = rbd[:, 3:6]; rec_base[i, :, 3:6] = rbd[:, 0:3]; rec_ee[i] = rbd[:, 48:55]; rec_st[i] = acc_st; acc_st.zero_()
+                rec["base_est"] = torch.zeros((n, B, 6), dtype=torch.float64, device=dev)
+            if sl:
+                rec["slip"] = torch.zeros((n, B), dtype=torch.int32, device=dev)
+            if gd is not None:
+                for key in ("gait", "mode", "target_kind"):
+                    rec[key] = torch.zeros((n, B), dtype=torch.int32, device=dev)
+                rec["ee_target"] = torch.zeros((n, B, 7), dtype=torch.float64, device=dev)
+            if rs is not None:
+                rec["episode"] = torch.zeros((n, B), dtype=torch.int32, device=dev); rec["fallen"] = torch.zeros_like(rec["episode"])
+                if cu is not None:
+                    rec["curriculum_level"] = torch.zeros_like(rec["episode"])
+            for k in range(self._k, self._k + n * MPC_PERIOD_MS):
+                if k % MPC_PERIOD_MS == 0 and k > 0:
+                    if rs is not None:
+                        self._respawn(k)
+                    self._mpc_tick()
+                if k % self._wbc == 0:
+                    solver.update_dev(self.meas, self.period, self.t_obs, self.x_obs, self.joint_cmd, self.arm_pos, self.last_time, self.cmd54, self.ctl_st, s)
+                    acc_st.bitwise_or_(self.ctl_st)
+                if rs is None:
+                    self.hw_time.fill_(self.t_start + k * 1e-3)
+                else:   # the robot's episode clock
+                    torch.sub(self.k0, k, out=self.dk).neg_(); self.hw_time.copy_(self.dk).mul_(1e-3).add_(self.t_start)
+                self.jpos.copy_(q[:, 6:]); self.jvel.copy_(v[:, 6:])
+                solver.hw_write_dev(self.hw_time, self.hw_period, self.joint_cmd, self.jpos, self.jvel, self.effort, self.hw_st, s)
                 if se:
-                    rec_base_est[i, :, 0:3] = rbd_est[:, 3:6]; rec_base_est[i, :, 3:6] = rbd_est[:, 0:3]
-                if sl:
-                    rec_slip[i] = slip_acc; slip_acc.zero_()
-                if rs is not None:
-                    solver.fall_detect_dev(rbd, fall_count, fallen, rs["z_min"], rs["tilt_max"], s)
-                    rec_episode[i] = episode; rec_fallen[i] = fallen
-                    if cu is not None:
-                        rec_level[i] = cu_level
-                    d = fall_count >= rs["hold_windows"] if rs["on_fall"] else torch.zeros_like(fallen, dtype=torch.bool)
-                    if mt or cu is not None:
-                        due_fall.copy_(d)
-                    if rs["every_ms"] is not None:
-                        d |= (k + 1 - k0) >= rs["every_ms"]
-                    due.copy_(d)
-        if mt:   # the run's end closes every robot's open episode
-            ones = torch.ones(B, dtype=torch.int32, device=dev)
-            solver.metrics_close_dev(ones, torch.zeros_like(ones), episode if rs is not None else torch.zeros_like(ones), mt_acc, mt_out, acc_st, s)
-    stream.synchronize()
-    t = t_start + np.arange(1, ticks + 1) * MPC_PERIOD_MS * 1e-3
-    out = dict(t=t, base=rec_base.cpu().numpy(), ee=rec_ee.cpu().numpy(), status=rec_st.cpu().numpy(), contact=contact.cpu().numpy(), q=q.cpu().numpy(), v=v.cpu().numpy(),
-               start_base=np.c_[q0[:, 0:3], q0[:, 3:6]], start_ee=rbd_h[:, 48:55])
-    if est:
-        out["payload_est"] = rec_pl.cpu().numpy()
-    if se:
-        out["base_est"] = rec_base_est.cpu().numpy()
-    if sl:
-        out["slip"] = rec_slip.cpu().numpy()
-    if gd is not None:
-        out.update(gait=rec_gait.cpu().numpy(), mode=rec_mode.cpu().numpy(), gait_templates=list(gd["names"]), target_kind=rec_kind.cpu().numpy(),
-                   ee_target=rec_ee_target.cpu().numpy())
-    if rs is not None:
-        out.update(episode=rec_episode.cpu().numpy(), fallen=rec_fallen.cpu().numpy())
-    if cu is not None:   # a robot's level is constant over an episode: it moves at the respawn that starts the next
-        ep = out["episode"]; lv = rec_level.cpu().numpy()
-        el = np.full((B, int(ep.max()) + 1), -1, dtype=np.int32); el[np.broadcast_to(np.arange(B), ep.shape), ep] = lv
-        out.update(curriculum_level=lv, episode_level=el, curriculum_state=solver.curriculum_get())
-    if rz is not None or sp is not None or tl is not None:   # rebuilt on the host from the episode record: the samplers' rows are pure functions of (ranges, seed, robot, episode[, level])
-        ep = out["episode"] if rs is not None else np.zeros((ticks, B), dtype=np.int32)
-        had = np.zeros((B, int(ep.max()) + 1), dtype=bool); had[np.broadcast_to(np.arange(B), ep.shape), ep] = True
-        rb, re_ = np.nonzero(had)
-        for kind, spec, shape in (("episode", rz, (_lib.EPISODE,)), ("spawn", sp, (_lib.SPAWN,)), ("timeline", tl, (0 if tl is None else tl["n"], _lib.TIMELINE_CMD))):
-            if spec is not None:
-                rows = solver.curriculum_draw(kind, rb, re_, el[rb, re_]) if kind in tops else getattr(solver, kind + "_draw")(rb, re_)
-                out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = rows
-        if tl is not None:   # on the episode's clock: exact for drawn times in [t_start / 2, 2 t_start]
-            out["timeline_params"][..., 0] -= t_start
-    if mt:   # trimmed to the most episodes of any robot
-        E = int(out["episode"].max()) + 1 if rs is not None else 1
-        out.update(episode_metrics=mt_out[:, :E].cpu().numpy(), metrics_layout=_lib.METRICS_LAYOUT)
-    return out
+                    self.v_prev.copy_(v)
+                if sim_timer:
+                    sim_timer(True)
+                if push is not None:
+                    kk = k if rs is None else self.dk   # plant steps since the episode's start
+                    torch.where(((push["on"] <= kk) & (push["off"] > kk))[:, None], push["wrench"], push["zero"], out=push["now"])
+                solver.sim_step_dev(1e-3, self.effort, q, v, rbd, contact, self.sim_st, s, wrench=None if push is None else push["now"])
+                if sim_timer:
+                    sim_timer(False)
+                acc_st.bitwise_or_(self.hw_st).bitwise_or_(self.sim_st)
+                if se:
+                    solver.sim_read_sensors_dev(1e-3, k, q, v, self.v_prev, self.sensors, s)
+                    if att:
+                        solver.attitude_step_dev(1e-3, self.sensors, self.at_st, s)
+                        acc_st.bitwise_or_(self.at_st)
+                    if sl:
+                        solver.slip_step_dev(1e-3, self.sensors, contact, self.stance, self.slip, self.sl_st, s)
+                        acc_st.bitwise_or_(self.sl_st); self.slip_acc.bitwise_or_(self.slip)
+                    solver.state_est_step_dev(1e-3, self.sensors, self.se_contact, self.rbd_est, self.se_st, s)
+                    acc_st.bitwise_or_(self.se_st)
+                if est:
+                    solver.payload_est_step_dev(1e-3, self.effort, self.meas, self.est_st, s)
+                    acc_st.bitwise_or_(self.est_st)
+                if mt:   # the plant's truth after the step, on the robot's episode clock, with the window's status so far
+                    solver.metrics_step_dev(1e-3, rbd, contact, self.effort, self.cmd7, self.prob["n_target"], self.prob["target_times"], self.prob["target_states"],
+                                            self.hw_time, acc_st, self.mt_acc, kind=None if gd is None else self.tick_kind, rbd_est=self.rbd_est if se else None, stream=s)
+                if (k + 1) % MPC_PERIOD_MS == 0:
+                    i = (k + 1) // MPC_PERIOD_MS - 1 - i0
+                    rec["base"][i, :, 0:3] = rbd[:, 3:6]; rec["base"][i, :, 3:6] = rbd[:, 0:3]; rec["ee"][i] = rbd[:, 48:55]; rec["status"][i] = acc_st; acc_st.zero_()
+                    if est:
+                        rec["payload_est"][i] = self.tick_pl
+                    if se:
+                        rec["base_est"][i, :, 0:3] = self.rbd_est[:, 3:6]; rec["base_est"][i, :, 3:6] = self.rbd_est[:, 0:3]
+                    if sl:
+                        rec["slip"][i] = self.slip_acc; self.slip_acc.zero_()
+                    if gd is not None:   # the window's gait step and the target in force after its target call
+                        rec["gait"][i] = self.tick_gait; rec["mode"][i] = self.tick_mode; rec["target_kind"][i] = self.tick_kind
+                        rec["ee_target"][i] = self.prob["target_states"][:, 1, 30:37]
+                    if rs is not None:
+                        solver.fall_detect_dev(rbd, self.fall_count, self.fallen, rs["z_min"], rs["tilt_max"], s)
+                        rec["episode"][i] = self.episode; rec["fallen"][i] = self.fallen
+                        if cu is not None:
+                            rec["curriculum_level"][i] = self.cu_level
+                        d = self.fall_count >= rs["hold_windows"] if rs["on_fall"] else torch.zeros_like(self.fallen, dtype=torch.bool)
+                        if mt or cu is not None:
+                            self.due_fall.copy_(d)
+                        if rs["every_ms"] is not None:
+                            d |= (k + 1 - self.k0) >= rs["every_ms"]
+                        self.due.copy_(d)
+        self._k += n * MPC_PERIOD_MS
+        return rec
+
+    def command(self, mask, gait=None, cmd_vel=None, ee_goal=None, ee_cmd_vel=None):
+        """One command for each robot with mask [B] set, from device tensors (host arrays are copied): gait [B] template ids (an index of
+        self.gait_templates, -1: none), cmd_vel [B, 4], ee_goal [B, 7] (position, quaternion xyzw of unit norm, world frame) and ee_cmd_vel [B, 3], NaN
+        rows meaning none; a row carries at most one of cmd_vel, ee_goal and ee_cmd_vel.  The rows take the semantics of a commands timeline row due at
+        the robot's first MPC tick after this call: the tick at the start of the next step (before the first step, the one that opens window 1).  A
+        later command before that tick replaces an earlier one; a robot that respawns at that boundary drops it.  A rejected row (checked on the device
+        with the timeline's rules) is not applied and sets _lib.ST_COMMAND in that window's record status.  Enqueued on self.stream after the work
+        the caller's current stream holds (the tensors may come from it), no synchronisation.  ValueError without the device gait schedule (steer, commands or timeline), on wrong shapes, and for end-effector commands in
+        a session that draws spawn yaws."""
+        import torch
+        if self._spec["gd"] is None:
+            raise ValueError("closed_loop.Session.command: needs the device gait schedule (steer=True, commands or timeline)")
+        if self._yaw_drawn and (ee_goal is not None or ee_cmd_vel is not None):
+            raise ValueError("closed_loop.Session.command: ee_goal / ee_cmd_vel cannot go with a drawn spawn yaw (their world-frame goals assume the robot faces +x)")
+        B = getattr(self.solver, "batch", None)
+        for name, a, shape in (("mask", mask, (B,)), ("gait", gait, (B,)), ("cmd_vel", cmd_vel, (B, 4)), ("ee_goal", ee_goal, (B, 7)), ("ee_cmd_vel", ee_cmd_vel, (B, 3))):
+            if a is not None and tuple(np.shape(a)) != shape:
+                raise ValueError("closed_loop.Session.command: %s must have shape %s, got %s" % (name, shape, tuple(np.shape(a))))
+        if not self._open or self._finished:
+            raise ValueError("closed_loop.Session.command: the session is not open (enter it with `with`; finish() ends it)")
+        dev = self.device
+        if dev.type == "cuda":   # rows the caller wrote on its own stream are complete before the session's stream reads them
+            self.stream.wait_stream(torch.cuda.current_stream(dev))
+
+        def put(a, dtype, shape, fill):
+            if a is None:
+                return torch.full(shape, fill, dtype=dtype, device=dev)
+            if isinstance(a, torch.Tensor):
+                t = a.to(device=dev, dtype=dtype).contiguous()
+                if t.is_cuda:   # the caller may free it before the session's stream has read it: its memory waits for that stream
+                    t.record_stream(self.stream)
+                return t
+            return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64 if dtype == torch.float64 else np.int32), device=dev)
+        with torch.cuda.stream(self.stream):
+            m = put(mask, torch.int32, (B,), 0); tmpl = put(gait, torch.int32, (B,), -1); vel = put(cmd_vel, torch.float64, (B, 4), np.nan)
+            goal = put(ee_goal, torch.float64, (B, 7), np.nan); eev = put(ee_cmd_vel, torch.float64, (B, 3), np.nan)
+            has_goal, has_eev = ~torch.isnan(goal).all(-1), ~torch.isnan(eev).all(-1)   # a partly NaN row is a command the check rejects
+            kind = torch.where(has_goal, _lib.TARGET_EE_GOAL, torch.where(has_eev, _lib.TARGET_EE_CMD_VEL, -1))
+            kind = torch.where(has_goal & has_eev, 3, kind).to(torch.int32)   # both: a kind the check rejects
+            ee = torch.where(has_goal[:, None], goal, 0.0); ee[:, :3] = torch.where(has_eev[:, None], eev, ee[:, :3])
+            self.solver.gait_dev_command_dev(m, tmpl, vel, kind, ee, self.cmd_st, self._s)
+            self.cmd_acc.bitwise_or_(self.cmd_st)
+        self._commanded = True
+
+    @property
+    def gait_templates(self):
+        """the device gait schedule's template names (a template id is its index), or None without it"""
+        gd = self._spec["gd"]
+        return None if gd is None else list(gd["names"])
+
+    @property
+    def state(self):
+        """The live device tensors at the current window boundary (the loop writes them: read, do not write): q, v [B, 24] and rbd [B, 55] (the plant's
+        truth), meas (what the controller reads: rbd, or the estimator's rbd_est), x_obs, t_obs, contact, cmd [B, 7] (the target front-end's command),
+        and with respawn episode, fallen and due (the robots that respawn at the next boundary), with curriculum level; None where not running.  clock
+        [B]: each robot's episode time in s, computed on self.stream at this call."""
+        import torch
+        rs, cu = self._spec["rs"], self._spec["cu"]
+        with torch.cuda.stream(self.stream):
+            clock = (self._k - self.k0).to(torch.float64) * 1e-3 if rs is not None else torch.full((self.B,), self._k * 1e-3, dtype=torch.float64, device=self.device)
+        return dict(q=self.q, v=self.v, rbd=self.rbd, meas=self.meas, x_obs=self.x_obs, t_obs=self.t_obs, contact=self.contact, cmd=self.cmd7,
+                    episode=self.episode if rs is not None else None, fallen=self.fallen if rs is not None else None, due=self.due if rs is not None else None,
+                    level=self.cu_level if cu is not None else None, clock=clock)
+
+    def finish(self):
+        """Close every robot's open episode (end 0) and return run's end-of-run keys as numpy arrays, from the device state: contact, q, v, start_base,
+        start_ee, and as run gives them gait_templates, episode_level, curriculum_state, episode_params, spawn_params, timeline_params, episode_metrics
+        and metrics_layout.  Synchronises self.stream; the session takes no more steps."""
+        import torch
+        if not self._open or self._finished:
+            raise ValueError("closed_loop.Session.finish: the session is not open (enter it with `with`; finish() ends it)")
+        self._finished = True
+        solver, p, B = self.solver, self._spec, self.B
+        rs, rz, sp, tl, cu, gd = p["rs"], p["rz"], p["sp"], p["tl"], p["cu"], p["gd"]
+        if self._mt:   # the run's end closes every robot's open episode
+            with torch.cuda.stream(self.stream):
+                ones = torch.ones(B, dtype=torch.int32, device=self.device)
+                solver.metrics_close_dev(ones, torch.zeros_like(ones), self.episode if rs is not None else torch.zeros_like(ones), self.mt_acc, self.mt_out, self.acc_st, self._s)
+        self.stream.synchronize()
+        out = dict(contact=self.contact.cpu().numpy(), q=self.q.cpu().numpy(), v=self.v.cpu().numpy(), **self._start_out)
+        if gd is not None:
+            out["gait_templates"] = list(gd["names"])
+        last = self.episode.cpu().numpy() if rs is not None else np.zeros(B, dtype=np.int32)   # a robot's episodes are 0 .. last[b]
+        had = np.arange(int(last.max()) + 1)[None, :] <= last[:, None]
+        if cu is not None:   # a robot's level is constant over an episode: it moves at the respawn that starts the next
+            el = self.ep_level[:, :had.shape[1]].cpu().numpy()
+            out.update(episode_level=el, curriculum_state=solver.curriculum_get())
+        if rz is not None or sp is not None or tl is not None:   # rebuilt on the host: the samplers' rows are pure functions of (ranges, seed, robot, episode[, level])
+            rb, re_ = np.nonzero(had)
+            for kind, spec, shape in (("episode", rz, (_lib.EPISODE,)), ("spawn", sp, (_lib.SPAWN,)), ("timeline", tl, (0 if tl is None else tl["n"], _lib.TIMELINE_CMD))):
+                if spec is not None:
+                    rows = solver.curriculum_draw(kind, rb, re_, el[rb, re_]) if kind in self._tops else getattr(solver, kind + "_draw")(rb, re_)
+                    out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = rows
+            if tl is not None:   # on the episode's clock: exact for drawn times in [t_start / 2, 2 t_start]
+                out["timeline_params"][..., 0] -= self.t_start
+        if self._mt:   # trimmed to the most episodes of any robot
+            out.update(episode_metrics=self.mt_out[:, :had.shape[1]].cpu().numpy(), metrics_layout=_lib.METRICS_LAYOUT)
+        return out

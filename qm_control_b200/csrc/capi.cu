@@ -92,6 +92,7 @@ struct qmb200_handle {
     std::vector<GsTemplate> table; GsTemplate* d_table = nullptr; GsRobot* d_robots = nullptr; int32_t* d_cursor = nullptr;
     double* d_t = nullptr; int32_t* d_tmpl = nullptr; double* d_vel = nullptr; int n_cmd = 0; double stance_time = 0.0;
     int32_t* d_ee_kind = nullptr; double* d_ee = nullptr;   // the timeline's end-effector commands [B][n_cmd] and [B][n_cmd][7], NULL when it has none
+    GsPending* d_pending = nullptr;                          // each robot's pending command (qmb200_gait_dev_command) [B], allocated with d_robots
   } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   bool plant_on_device = false, tuning_on_device = false;   // an episode draw wrote mu / payload or tuning on the device: plant_ / tuning_rows_sync refresh them
@@ -264,7 +265,7 @@ void qmb200_destroy(qmb200_handle* h) {
   if (h->d_at) cudaFree(h->d_at);
   if (h->d_sl) cudaFree(h->d_sl);
   cudaFree(h->gs.d_table); cudaFree(h->gs.d_robots); cudaFree(h->gs.d_cursor); cudaFree(h->gs.d_t); cudaFree(h->gs.d_tmpl); cudaFree(h->gs.d_vel);
-  cudaFree(h->gs.d_ee_kind); cudaFree(h->gs.d_ee);
+  cudaFree(h->gs.d_ee_kind); cudaFree(h->gs.d_ee); cudaFree(h->gs.d_pending);
   cudaFree(h->image.d);
   delete h;
 }

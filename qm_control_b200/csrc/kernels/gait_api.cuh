@@ -27,6 +27,9 @@ struct GsRobot { GsSchedule s; int32_t tmpl; int32_t src; };
 // an end-effector command: kind (-1: none, QMB200_TARGET_EE_CMD_VEL, QMB200_TARGET_EE_GOAL) with its row [7] (ee_cmd_vel: vx, vy, vz; goal: pos,
 // quat xyzw).  NULL ee_kind: no end-effector rows.  A row carries at most one of cmd_vel and an end-effector command.
 struct GsCommands { int n; const double* t; const int32_t* tmpl; const double* vel; const int32_t* ee_kind = nullptr; const double* ee = nullptr; };
+// one robot's pending command (qmb200_gait_dev_command): one row of GsCommands without its time, applied by the robot's next step.  set 0: none.
+// Zeroed words are an empty slot, so the restore clears it with one zero segment.
+struct GsPending { int32_t set; int32_t tmpl; double vel[4]; int32_t ee_kind; int32_t pad; double ee[7]; };
 
 QMB_HD int gs_lower_bound(const double* a, int n, double t) { int lo = 0, hi = n; while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < t) lo = mid + 1; else hi = mid; } return lo; }
 
@@ -74,31 +77,62 @@ QMB_HD int gs_get(GsSchedule& s, const GsTemplate& t, double lower, double upper
 // stream, GS_KIND_HELD for a held goal
 QMB_HD int gs_target_kind(int src, int applied) { return applied == GS_SRC_EE_GOAL ? GS_SRC_EE_GOAL : src == GS_SRC_EE_GOAL ? GS_KIND_HELD : src; }
 
+// the rules qmb200_gait_dev_set_commands_ee checks on the host, for one command row: QMB200_ST_COMMAND when the template lies outside [-1, n_templates),
+// the cmd_vel row is neither all finite nor all NaN, the kind is not -1, QMB200_TARGET_EE_CMD_VEL or QMB200_TARGET_EE_GOAL, an end-effector value
+// (ee[0:3] of ee_cmd_vel, ee[0:7] of a goal) is not finite, a goal quaternion's norm differs from 1 by more than 1e-9, or the row carries both a cmd_vel
+// and an end-effector command; else 0
+QMB_HD int gs_command_check(int tmpl, const double* vel, int ee_kind, const double* ee, int n_templates) {
+  if (tmpl < -1 || tmpl >= n_templates) return QMB200_ST_COMMAND;
+  const bool none = isnan(vel[0]);
+  for (int i = 0; i < 4; ++i) if (none ? !isnan(vel[i]) : !isfinite(vel[i])) return QMB200_ST_COMMAND;
+  if (ee_kind == -1) return 0;
+  if (ee_kind != GS_SRC_EE_CMD_VEL && ee_kind != GS_SRC_EE_GOAL) return QMB200_ST_COMMAND;
+  if (!none) return QMB200_ST_COMMAND;
+  const bool goal = ee_kind == GS_SRC_EE_GOAL;
+  for (int i = 0; i < (goal ? 7 : 3); ++i) if (!isfinite(ee[i])) return QMB200_ST_COMMAND;
+  const double qn = sqrt(ee[3] * ee[3] + ee[4] * ee[4] + ee[5] * ee[5] + ee[6] * ee[6]);
+  return goal && !(fabs(qn - 1.0) <= 1e-9) ? QMB200_ST_COMMAND : 0;
+}
+
+// one command row due at t applied to w: a template is inserted at t + horizon with final horizon, a cmd_vel row fills row[0:4], an ee_cmd_vel row
+// row[0:3], a goal row row[0:7]; wrote grows to the longest prefix written, applied becomes the row's target command.  QMB200_ST_OVERFLOW (w partly
+// written) or 0.
+QMB_HD int gs_apply(GsRobot& w, const GsTemplate* table, int tmpl, const double* vel, int ee_kind, const double* ee, double t, double horizon, double stance_time,
+                    double* row, int& wrote, int& applied) {
+  if (tmpl >= 0) {
+    if (gs_insert(w.s, table[tmpl], t + horizon, horizon, stance_time)) return QMB200_ST_OVERFLOW;
+    w.tmpl = tmpl;
+  }
+  if (!isnan(vel[0])) { for (int i = 0; i < 4; ++i) row[i] = vel[i]; wrote = wrote > 4 ? wrote : 4; applied = GS_SRC_CMD_VEL; }
+  if (ee_kind >= 0) {
+    const int m = ee_kind == GS_SRC_EE_GOAL ? 7 : 3;
+    for (int i = 0; i < m; ++i) row[i] = ee[i];
+    wrote = wrote > m ? wrote : m; applied = ee_kind;
+  }
+  return 0;
+}
+
 // One step of robot b at time t: the robot's commands due at t (time <= t, from *cursor on) in order: a template is inserted at t + horizon with
 // final horizon (GaitReceiver::preSolverRun), a cmd_vel row goes to cmd[0:4], an ee_cmd_vel row to cmd[0:3], a goal row to cmd[0:7]; the last of
-// these target commands sets the robot's source.  Then the window [t - horizon, t + 2 horizon] is taken.  All or nothing: status QMB200_ST_NAN
-// (non-finite t) or QMB200_ST_OVERFLOW (a window above QMB200_EMAX events, or GS_CAP exceeded) leaves r (its source included), *cursor, the MPC rows
-// and cmd untouched.  Otherwise writes n_events, event_times[EMAX] (0 past the count), modes[EMAX + 1] (stance past the count) and cmd.
+// these target commands sets the robot's source.  A set pending command (non-NULL pending) is applied after them as one more row due at t, and its
+// slot is cleared (set = 0) when the step succeeds.  Then the window [t - horizon, t + 2 horizon] is taken.  All or nothing: status QMB200_ST_NAN
+// (non-finite t) or QMB200_ST_OVERFLOW (a window above QMB200_EMAX events, or GS_CAP exceeded) leaves r (its source included), *cursor, the pending
+// slot, the MPC rows and cmd untouched.  Otherwise writes n_events, event_times[EMAX] (0 past the count), modes[EMAX + 1] (stance past the count) and cmd.
 // target_kind (when non-NULL) is written on every path: gs_target_kind of the source after the step and the last target command it applied.
 // Returns the status.
 QMB_HD int gs_step(GsRobot& r, int32_t* cursor, const GsTemplate* table, const GsCommands& c, int b, double t, double horizon, double stance_time,
-                   int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* target_kind = nullptr) {
+                   int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* target_kind = nullptr, GsPending* pending = nullptr) {
   if (target_kind) *target_kind = gs_target_kind(r.src, -1);   // a failed step leaves the source as it was
   if (!isfinite(t)) return QMB200_ST_NAN;
   GsRobot w = r; int cur = *cursor; double row[7]; int wrote = 0, applied = -1;   // row[0:wrote]: the cmd slots written (every command writes a prefix)
   for (; cur < c.n && c.t[(size_t)b * c.n + cur] <= t; ++cur) {
     const size_t k = (size_t)b * c.n + cur;
-    if (c.tmpl[k] >= 0) {
-      if (gs_insert(w.s, table[c.tmpl[k]], t + horizon, horizon, stance_time)) return QMB200_ST_OVERFLOW;
-      w.tmpl = c.tmpl[k];
-    }
-    if (!isnan(c.vel[4 * k])) { for (int i = 0; i < 4; ++i) row[i] = c.vel[4 * k + i]; wrote = wrote > 4 ? wrote : 4; applied = GS_SRC_CMD_VEL; }
-    if (c.ee_kind && c.ee_kind[k] >= 0) {
-      const int m = c.ee_kind[k] == GS_SRC_EE_GOAL ? 7 : 3;
-      for (int i = 0; i < m; ++i) row[i] = c.ee[7 * k + i];
-      wrote = wrote > m ? wrote : m; applied = c.ee_kind[k];
-    }
+    if (gs_apply(w, table, c.tmpl[k], c.vel + 4 * k, c.ee_kind ? c.ee_kind[k] : -1, c.ee ? c.ee + 7 * k : nullptr, t, horizon, stance_time, row, wrote, applied))
+      return QMB200_ST_OVERFLOW;
   }
+  const bool pend = pending && pending->set;   // the pending command: one more row due at t, after the timeline's
+  if (pend && gs_apply(w, table, pending->tmpl, pending->vel, pending->ee_kind, pending->ee, t, horizon, stance_time, row, wrote, applied))
+    return QMB200_ST_OVERFLOW;
   const int n = gs_get(w.s, table[w.tmpl], t - horizon, t + 2.0 * horizon);
   if (n < 0) return QMB200_ST_OVERFLOW;
   *n_events = n;
@@ -108,6 +142,7 @@ QMB_HD int gs_step(GsRobot& r, int32_t* cursor, const GsTemplate* table, const G
   if (applied >= 0) w.src = applied;
   if (target_kind) *target_kind = gs_target_kind(w.src, applied);
   r = w; *cursor = cur;
+  if (pend) pending->set = 0;
   return 0;
 }
 
@@ -115,9 +150,15 @@ QMB_HD int gs_step(GsRobot& r, int32_t* cursor, const GsTemplate* table, const G
 QMB_HD int gs_mode_at(const GsSchedule& s, double t) { return s.md[gs_lower_bound(s.ev, s.n, t)]; }
 
 // one step per robot (gs_step) at t_obs [B] on the MPC problem rows n_events [B], event_times [B][EMAX], modes [B][EMAX + 1] and cmd [B][7];
-// writes status [B], and tmpl [B] (active template), mode [B] (gs_mode_at t_obs of the stored schedule) and target_kind [B] when non-NULL
+// writes status [B], and tmpl [B] (active template), mode [B] (gs_mode_at t_obs of the stored schedule) and target_kind [B] when non-NULL; consumes the
+// pending slots [B]
 int launch_gait_step(int B, const GsTemplate* table, GsRobot* robots, int32_t* cursor, GsCommands c, double horizon, double stance_time, const double* t_obs,
                      int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, int32_t* target_kind,
-                     cudaStream_t s);
+                     GsPending* pending, cudaStream_t s);
+
+// one thread per robot: a masked robot's row (tmpl [B], vel [B][4], ee_kind [B], ee [B][7]) that passes gs_command_check overwrites its pending slot;
+// status [B] = that check's word for masked robots, 0 for the others, whose slots are not written
+int launch_gait_command(int B, int n_templates, GsPending* pending, const int32_t* mask, const int32_t* tmpl, const double* vel, const int32_t* ee_kind,
+                        const double* ee, int32_t* status, cudaStream_t s);
 
 }  // namespace qmb

@@ -9,7 +9,7 @@ namespace qmb {
 
 // One block of per-robot rows [B][words] of 4-byte words, written for every masked robot: from src [B][words] (the image), or zeros when src is NULL.
 struct RestoreSeg { uint32_t* dst; const uint32_t* src; int32_t words; };
-constexpr int RESTORE_MAX_SEGS = 12;
+constexpr int RESTORE_MAX_SEGS = 16;   // 8 imaged blocks when every component runs, 5 cold-start blocks
 struct RestoreTable { RestoreSeg seg[RESTORE_MAX_SEGS]; int n; };
 
 // one launch over every segment of the table: robot b's rows are written when mask[b] != 0, and left alone otherwise

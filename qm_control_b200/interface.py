@@ -996,8 +996,29 @@ class Solver:
         self._call("gait_dev_get_commands", None, *(_p(out[k]) for k in ("t", "tmpl", "cmd_vel", "ee_kind", "ee_cmd")))
         return out
 
+    def gait_dev_command(self, mask, tmpl, cmd_vel, ee_kind, ee):
+        """Host variant of gait_dev_command_dev: numpy rows mask [B], tmpl [B], cmd_vel [B, 4], ee_kind [B], ee [B, 7] → status [B].  Synchronous."""
+        B = self.batch; st = np.zeros(B, dtype=np.int32)
+        rows = (_i32(mask, (B,)), _i32(tmpl, (B,)), _f64(cmd_vel, (B, 4)), _i32(ee_kind, (B,)), _f64(ee, (B, 7)))   # held until the call returns
+        self._call("gait_dev_command", *(_p(a) for a in rows), _p(st))
+        return st
+
+    def gait_dev_command_dev(self, mask, tmpl, cmd_vel, ee_kind, ee, status, stream=None):
+        """One command per masked robot, applied by its next gait step (qmb200_gait_dev_command_dev; DESIGN.md §4.16): device int32 mask [B], tmpl [B]
+        (ids, -1: none), float64 cmd_vel [B, 4] (NaN rows: none), int32 ee_kind [B] (-1, 1: ee_cmd_vel, 2: goal), float64 ee [B, 7] (as ee_cmd of
+        gait_dev_set_commands); status [B] int32 receives _lib.ST_COMMAND for a rejected row, else 0.  An accepted row replaces the robot's pending one.
+        No synchronisation."""
+        self._call("gait_dev_command_dev", _p(mask), _p(tmpl), _p(cmd_vel), _p(ee_kind), _p(ee), _p(status), stream)
+
+    def gait_dev_get_pending(self):
+        """→ dict(set [B], tmpl [B], cmd_vel [B, 4], ee_kind [B], ee [B, 7]): each robot's pending command slot.  Synchronous."""
+        B = self.batch
+        out = dict(set=np.zeros(B, dtype=np.int32), tmpl=np.zeros(B, dtype=np.int32), cmd_vel=np.zeros((B, 4)), ee_kind=np.zeros(B, dtype=np.int32), ee=np.zeros((B, 7)))
+        self._call("gait_dev_get_pending", *(_p(out[k]) for k in ("set", "tmpl", "cmd_vel", "ee_kind", "ee")))
+        return out
+
     def gait_dev_stop(self):
-        """Release the schedules and the timeline (the template table stays)."""
+        """Release the schedules, the pending commands and the timeline (the template table stays)."""
         self._call("gait_dev_stop")
 
     # ---------------- utilities ----------------

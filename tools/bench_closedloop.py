@@ -1034,6 +1034,84 @@ def curriculum_main(args):
                                     "episodes": {"staircase": int(n_ep.sum()), "uniform": int(ok.sum())}, "per_mu_bin": out}}))
 
 
+def heading_controller(state, goal, vx=0.25, gain=2.0, rate_max=0.6):
+    """a torch heading controller on a session's live tensors: cmd_vel = (vx, 0, 0, clamp(gain * wrap(goal - yaw))) from the plant's yaw q[:, 3]"""
+    import torch
+    err = torch.remainder(goal - state["q"][:, 3] + np.pi, 2.0 * np.pi) - np.pi
+    vel = torch.zeros((len(goal), 4), dtype=torch.float64, device=goal.device)
+    vel[:, 0] = vx; vel[:, 3] = torch.clamp(gain * err, -rate_max, rate_max)
+    return vel
+
+
+def command_times(solver, reps=7, calls=50):
+    """Device time per qmb200_gait_dev_command_dev on every robot (a cmd_vel row each) and per 1 ms plant step of the whole batch, alternated `reps`
+    times in blocks of `calls` (CUDA events) → median ms per call of each."""
+    import torch
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    solver.gait_dev_set_templates(); solver.gait_dev_reset(np.zeros(B, dtype=np.int32), np.full(B, 10.0))
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    q0, v0 = solver.sim_standing_state(xy); q = torch.as_tensor(q0, device=dev); v = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact)
+    ones = torch.ones_like(contact); tmpl = torch.full_like(contact, -1); kind = torch.full_like(contact, -1)
+    vel = torch.full((B, 4), 0.2, dtype=torch.float64, device=dev); ee = torch.zeros((B, 7), dtype=torch.float64, device=dev)
+    calls_of = {"command": lambda: solver.gait_dev_command_dev(ones, tmpl, vel, kind, ee, st, s.cuda_stream),
+                "plant": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    for rep in range(reps + 1):   # the first round warms up
+        for mode, call in calls_of.items():
+            torch.cuda.synchronize(dev)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+            for _ in range(calls):
+                call()
+            b.record(s); torch.cuda.synchronize(dev)
+            if rep:
+                times[mode].append(a.elapsed_time(b) / calls)
+    solver.gait_dev_stop()
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+            **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()},
+            "spread_command": [float(min(times["command"])), float(max(times["command"]))]}
+
+
+def session_main(args, reps=2):
+    """Wall time per simulated second of closed_loop.run against a Session stepped one 10 ms window at a time, without commands and with one heading
+    command per window from a torch controller on the session's stream (alternated, best of reps), and the command kernel's time."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    B = args.batch; sim_s = args.duration; solver = q.Solver(batch=B, device=0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    kw = dict(gait=args.gait, cmd_vel=(args.vx, 0.0, 0.0, 0.0), xy_yaw=xy)
+    goal_h = np.random.default_rng(0).uniform(-1.0, 1.0, B)
+
+    def stepped(commanded, duration):
+        with closed_loop.Session(solver, duration, steer=commanded, **kw) as ss:
+            with torch.cuda.stream(ss.stream):
+                goal = torch.as_tensor(goal_h, device=ss.device); ones = torch.ones(B, dtype=torch.int32, device=ss.device)
+            for _ in range(ss.windows):
+                if commanded:
+                    with torch.cuda.stream(ss.stream):
+                        ss.command(ones, cmd_vel=heading_controller(ss.state, goal))
+                ss.step(1)
+            return ss.finish()
+    modes = {"run": lambda d: closed_loop.run(solver, duration=d, **kw), "session": lambda d: stepped(False, d), "session_commands": lambda d: stepped(True, d)}
+    for f in modes.values():   # warm-up: every shape of the timed runs
+        f(0.05)
+    wall = {k: [] for k in modes}; end = None
+    for _ in range(reps):
+        for k, f in modes.items():
+            torch.cuda.synchronize(); t0 = time.perf_counter(); r = f(sim_s); torch.cuda.synchronize(); wall[k].append((time.perf_counter() - t0) / sim_s)
+            end = r if k == "session_commands" else end
+    err = np.abs(np.remainder(goal_h - end["q"][:, 3] + np.pi, 2 * np.pi) - np.pi)
+    name, limit = card()
+    print(json.dumps({"metric": "session", "gpu": name, "power_limit": limit, "batch": B, "gait": args.gait, "sim_s": sim_s,
+                      "wall_s_per_sim_s": {k: float(min(v)) for k, v in wall.items()}, "wall_s_per_sim_s_all": wall,
+                      "heading_error_rad": dict(max=float(err.max()), mean=float(err.mean()), start_max=float(np.abs(goal_h).max())),
+                      "times": command_times(solver)}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
@@ -1058,7 +1136,11 @@ def main():
                                                             "wall time, falls and velocity error per transition")
     ap.add_argument("--curriculum", action="store_true", help="with --respawn: per-robot levels stepped from each episode's outcome: update time, wall time, "
                                                               "an up-down staircase on the push against a uniform sweep")
+    ap.add_argument("--session", action="store_true", help="closed_loop.run against a Session stepped one window at a time, without commands and with a "
+                                                           "torch heading controller's command every window: wall time per simulated second, the command kernel's time")
     args = ap.parse_args()
+    if args.session:
+        return session_main(args)
     if args.curriculum and not args.respawn:
         ap.error("--curriculum needs --respawn")
     if args.curriculum:
