@@ -40,6 +40,7 @@ extern "C" {
  *                                       (qmb200_mpc_solve / qmb200_mpc_get_solution report the MPC flags unshifted in their own status array)
  *                           bit 16      QMB200_ST_SAFETY — qmb200_update / qmb200_control_law
  *                           bit 17      QMB200_ST_COMMAND — qmb200_gait_dev_command(_dev), a rejected command row
+ *                           bit 18      QMB200_ST_RESTORE — qmb200_robot_state_load(_dev), a source robot outside [0, B)
  * Nothing else is ever OR-ed into a status word: the WBC's iteration counts live in qmb200_wbc_get_diagnostics. */
 #define QMB200_ST_ITER_CAP 1
 #define QMB200_ST_OVERFLOW 2      /* WBC: more rows than the working-set / level-0 buffers hold; MPC: node count > NMAX, event / target count out of range, swing phase not enclosed */
@@ -330,6 +331,8 @@ int qmb200_gait_dev_stop(qmb200_handle* h);
 #define QMB200_JOINT_CMD 5           /* HybridJointHandle::setCommand(posDes, velDes, kp, kd, ff) (HybridJointInterface.h:55-61) */
 #define QMB200_ST_SAFETY 0x10000     /* SafetyChecker::check failed (SafetyChecker.h:22-35): the reference stops the controller */
 #define QMB200_ST_COMMAND 0x20000    /* qmb200_gait_dev_command(_dev): the robot's command row was rejected (no other status word uses this bit) */
+#define QMB200_ST_RESTORE (QMB200_ST_COMMAND << 1)   /* qmb200_robot_state_load(_dev): the robot's source row lies outside [0, B), the robot was not written
+                                                        (bit 18; no other status word uses it) */
 #define QMB200_ST_HW_RING_FULL 2     /* qmb200_hw_write: more than 32 commands inside the delay window (the oldest was dropped) */
 
 /* QMController::updateStateEstimation tail (QMController.cpp:236-243): t_obs += period; x_obs = computeCentroidalStateFromRbdModel(rbd) with
@@ -596,6 +599,45 @@ int qmb200_robot_image_clear(qmb200_handle* h);
  * since, or a component runs that was not imaged. */
 int qmb200_robot_image_restore(qmb200_handle* h, const int32_t* mask /*[B]*/);
 int qmb200_robot_image_restore_dev(qmb200_handle* h, const int32_t* mask /*[B] device*/, void* cuda_stream);
+
+/* ---- robot-state snapshots: the start image generalised to any window boundary, with the warm state, restored onto any robot (DESIGN.md §4.17).
+ *      A snapshot holds, per robot, every [B][...] block of the handle that a later solve, update, plant step or estimator step reads before it writes,
+ *      in this order (block i is bit i of qmb200_robot_state_desc.blocks; a block is held when it exists now):
+ *        0 state estimator  1 attitude filter  2 slip detector  3 payload estimator  4 model payload rows  5 their SRBD constants
+ *        6 device gait schedule  7 its timeline cursor  8-12 the current MPC solution side (n_nodes, node times, events, x, u: the warm start)
+ *        13 the WBC's last input  14-16 the hw_write FIFO (commands, stamps, head / count)  17 the pending gait command
+ *        18 plant friction  19 plant payload  20 plant robot terrain  21 state estimator ground map  22 tuning rows
+ *        23-27 the gait schedule's command timeline (t, template, cmd_vel, end-effector kind, end-effector row)
+ *        28-31 the MPC's copy of the last solve's mode schedule (event count, event times, modes), which every policy evaluation (qmb200_update,
+ *              qmb200_policy_eval) reads until the next solve, and that solve's status
+ *      A load may therefore sit anywhere in a loop: before a solve, or between a solve and the updates that evaluate its policy.
+ *      It holds no shared settings (tiles, templates, parameters, gains), no draw ranges, curriculum or start image, and no per-call intermediates.  The
+ *      buffer is caller-owned device memory of B * qmb200_robot_state_bytes bytes, one block [B][bytes] after the other.  Each block carries the
+ *      generation of what owns it, bumped when that is reset, stopped, allocated, re-allocated or cleared: a load refuses a snapshot whose rows no
+ *      longer belong to the handle's state. */
+#define QMB200_STATE_BLOCKS 32
+typedef struct qmb200_robot_state_desc {
+  int32_t batch;                        /* B of the handle that saved it */
+  int32_t n_blocks;                     /* blocks held (set bits of blocks) */
+  int64_t bytes;                        /* bytes per robot: the sum of the held blocks' row widths */
+  uint64_t blocks;                      /* bit i: block i is held */
+  uint64_t gen[QMB200_STATE_BLOCKS];    /* generation of each held block's owner at the save (0 where not held) */
+} qmb200_robot_state_desc;
+/* Bytes per robot of a snapshot of the blocks that exist now (> 0: the MPC solution side and the WBC input always do); -1 for a NULL handle. */
+int64_t qmb200_robot_state_bytes(const qmb200_handle* h);
+/* One launch on the stream, no host synchronisation: copies every robot's held blocks into buf (device, at least bytes = B * qmb200_robot_state_bytes)
+ * in the handle's current state in stream order, and fills desc.  Fails before any launch, writing nothing, on a NULL or short buffer. */
+int qmb200_robot_state_save_dev(qmb200_handle* h, void* buf /*device*/, int64_t bytes, qmb200_robot_state_desc* desc, void* cuda_stream);
+/* One launch, no host synchronisation: every robot b with mask[b] != 0 takes robot source[b]'s rows of the snapshot (NULL source: its own, b), the MPC
+ * solution into the side current at this call.  A source outside [0, B) leaves the robot untouched and sets status[b] = QMB200_ST_RESTORE; status [B]
+ * (NULL: none) is written, not OR-ed, 0 for restored and unmasked robots.  The getters of the plant, model payload, tuning and terrain rows report the
+ * loaded rows.  Fails before any launch, writing nothing and naming the block, when buf is NULL, the snapshot is of another batch, its block set differs
+ * from the blocks that exist now or a block's generation moved since the save. */
+int qmb200_robot_state_load_dev(qmb200_handle* h, const void* buf /*device*/, const qmb200_robot_state_desc* desc, const int32_t* mask /*[B] device*/,
+                                const int32_t* source /*[B] device, NULL: b*/, int32_t* status /*[B] device, NULL: none*/, void* cuda_stream);
+/* Host mask, source and status (staged on the handle's stream, synchronous); buf is device memory as for qmb200_robot_state_load_dev. */
+int qmb200_robot_state_load(qmb200_handle* h, const void* buf, const qmb200_robot_state_desc* desc, const int32_t* mask /*[B]*/, const int32_t* source /*[B] or NULL*/,
+                            int32_t* status /*[B] or NULL*/);
 /* The fall rule of the closed-loop sweeps, one thread per robot on the plant's rbd [B][55]: robot b is fallen when its base rows (zyx, p) hold a
  * non-finite value, p_z - H(p_x, p_y) <= z_min with H the plant's ground under the base (its terrain tile, the plane ground_height otherwise), or
  * |pitch| or |roll| >= tilt_max.  fallen [B] = 1 / 0; count [B] (in-out) grows by one on a fallen call and drops to 0 otherwise.  Rejects a non-finite

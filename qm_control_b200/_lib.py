@@ -11,6 +11,7 @@ NX, NU, RBD, CMD, TARGET, EMAX, KMAX = 30, 30, 55, 54, 37, 32, 4
 GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
 TARGET_CMD_VEL, TARGET_EE_CMD_VEL, TARGET_EE_GOAL = 0, 1, 2   # QMB200_TARGET_*: the target front-end's kinds (-1 in a per-robot kind: a held goal)
 ST_COMMAND = 0x20000   # QMB200_ST_COMMAND: a rejected qmb200_gait_dev_command row
+ST_RESTORE = 0x40000   # QMB200_ST_RESTORE: a qmb200_robot_state_load source row outside [0, B)
 
 dp = C.POINTER(C.c_double)
 ip = C.POINTER(C.c_int32)
@@ -123,6 +124,18 @@ CURRICULUM_ROLES = ("pass", "fail")   # QMB200_CURRICULUM_PASS, _FAIL
 class CurriculumRule(C.Structure):
     """qmb200_curriculum_rule: the level count and up to CURRICULUM_MAX_COND conditions on a closed episode's metrics row (include/qmb200.h)."""
     _fields_ = [("n_levels", C.c_int32), ("n_cond", C.c_int32), ("column", C.c_int32 * 4), ("op", C.c_int32 * 4), ("role", C.c_int32 * 4)]
+
+
+# the blocks of a robot-state snapshot (qmb200_robot_state_*), block i being bit i of RobotStateDesc.blocks
+ROBOT_STATE_BLOCKS = ("state_est", "attitude", "slip", "payload_est", "model_payload", "model_srbd", "gait", "gait_cursor", "mpc_n_nodes", "mpc_t", "mpc_event",
+                      "mpc_x", "mpc_u", "wbc_input_last", "hw_ring_cmd", "hw_ring_stamp", "hw_ring_state", "gait_pending", "plant_mu", "plant_payload",
+                      "robot_terrain", "ground_map", "tuning", "timeline_t", "timeline_tmpl", "timeline_vel", "timeline_ee_kind", "timeline_ee",
+                      "mpc_n_events", "mpc_event_times", "mpc_modes", "mpc_status")
+
+
+class RobotStateDesc(C.Structure):
+    """qmb200_robot_state_desc: what a robot-state snapshot holds (include/qmb200.h, DESIGN.md §4.17)."""
+    _fields_ = [("batch", C.c_int32), ("n_blocks", C.c_int32), ("bytes", C.c_int64), ("blocks", C.c_uint64), ("gen", C.c_uint64 * len(ROBOT_STATE_BLOCKS))]
 
 
 # every function include/qmb200.h declares, in header order: name -> (restype, argtypes).  Every pointer is c_void_p (numpy / torch addresses, byref,
@@ -244,6 +257,10 @@ PROTOTYPES = {
     "qmb200_robot_image_clear": (I32, [P]),
     "qmb200_robot_image_restore": (I32, [P] * 2),
     "qmb200_robot_image_restore_dev": (I32, [P] * 3),
+    "qmb200_robot_state_bytes": (I64, [P]),
+    "qmb200_robot_state_save_dev": (I32, [P, P, I64, P, P]),
+    "qmb200_robot_state_load_dev": (I32, [P] * 7),
+    "qmb200_robot_state_load": (I32, [P] * 6),
     "qmb200_fall_detect": (I32, [P, P, D, D, P, P]),
     "qmb200_fall_detect_dev": (I32, [P, P, D, D, P, P, P]),
     "qmb200_episode_set_ranges": (I32, [P, P, P, I64]),

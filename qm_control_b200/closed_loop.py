@@ -733,6 +733,24 @@ def _metrics_episodes(ticks, rs):
     return (ticks - 1) // max(shortest, 1) + 1
 
 
+class Snapshot:
+    """Every robot of a Session at one window boundary (Session.snapshot; DESIGN.md §4.17): buf, the library's rows (uint8 device tensor), desc, what
+    they hold (_lib.RobotStateDesc), rows, device clones of the loop's per-robot rows (Session.rows), k0 [B], each robot's clock origin then, and k, the
+    plant step of the boundary (window = k / 10)."""
+
+    def __init__(self, session, buf, desc, rows, k0, k):
+        self.session, self.buf, self.desc, self.rows, self.k0, self.k = session, buf, desc, rows, k0, k
+
+    @property
+    def window(self):
+        return self.k // MPC_PERIOD_MS
+
+    @property
+    def nbytes(self):
+        """device bytes the snapshot holds: the library's rows and the loop's"""
+        return self.buf.numel() + sum(a.numel() * a.element_size() for a in self.rows) + self.k0.numel() * 8
+
+
 class Session:
     """A closed loop stepped window by window: run's loop, with its live state on the device between windows and per-robot commands from device tensors.
 
@@ -747,6 +765,9 @@ class Session:
     s.command(mask, gait=None, cmd_vel=None, ee_goal=None, ee_cmd_vel=None): one command for each masked robot, applied by its first MPC tick after the
     call (Solver.gait_dev_command_dev; DESIGN.md §4.16).
     s.state: the live device tensors (read-only: the loop writes them).  s.finish() closes the open episodes and returns run's end-of-run keys.
+    snap = s.snapshot() and s.restore(snap, mask=None, source=None) rewind robots to a window boundary, or branch one robot's state onto others
+    (DESIGN.md §4.17); not with respawn, randomize, spawn, timeline or curriculum.  Sensor noise is a pure function of (seed, robot, plant step k,
+    channel): a rewound or branched robot draws fresh noise, so exact replay needs the noise off.
     run(solver, duration, **kw) is Session + one step(windows) + finish()."""
 
     def __init__(self, solver, duration=1.0, steer=False, **kw):
@@ -944,10 +965,14 @@ class Session:
             solver.gait_dev_set_commands(t_start + gd["t"], gd["tmpl"], gd["cmd_vel"], **gd["ee"])
         solver.hw_set_delay(HW_DELAY)
 
+        # the loop's per-robot rows: own, the rows a respawn returns to the start image, then the rows a snapshot holds as well (self.rows, completed once
+        # the accumulator exists): the push rows, the metrics accumulator, the pending commands' status, the current window's MPC tick rows and its
+        # status accumulators (a snapshot of window 0 is taken after that window's tick)
+        self.own = [q, v, rbd, contact, t_obs, x_obs, self.joint_cmd, self.arm_pos, self.last_time, self.cmd54, cmd7, self.last_ee, prob["n_events"],
+                    prob["event_times"], prob["modes"], prob["n_target"], prob["target_times"], prob["target_states"]] + \
+                   ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
+        self.k0 = None   # each robot's clock origin (plant step): with respawn, or once a restore has happened; the global k otherwise
         if rs is not None:   # the start image: the library's rows and the loop's own, then one restore of every robot through the cold path of every later one
-            self.own = [q, v, rbd, contact, t_obs, x_obs, self.joint_cmd, self.arm_pos, self.last_time, self.cmd54, cmd7, self.last_ee, prob["n_events"],
-                        prob["event_times"], prob["modes"], prob["n_target"], prob["target_times"], prob["target_states"]] + \
-                       ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
             solver.robot_image_save()
             with torch.cuda.stream(stream):
                 self.start = [a.clone() for a in self.own]
@@ -964,6 +989,11 @@ class Session:
             with torch.cuda.stream(stream):
                 self.mt_acc = torch.zeros((B, _lib.METRICS_ACC), dtype=torch.float64, device=dev)
                 self.mt_out = torch.full((B, _metrics_episodes(ticks, rs), _lib.METRICS), np.nan, dtype=torch.float64, device=dev)
+        self.rows = self.own + ([push["on"], push["off"], push["wrench"]] if push is not None else []) + ([self.mt_acc] if mt else []) + \
+            ([self.cmd_acc, self.tick_gait, self.tick_mode, self.tick_kind] if gd is not None else []) + ([self.tick_pl] if est else []) + \
+            [self.acc_st] + ([self.slip_acc] if sl else [])
+        with torch.cuda.stream(stream):
+            self.restore_st = torch.zeros(B, dtype=torch.int32, device=dev)   # a restore's status (ST_RESTORE for an invalid source)
 
         if rz is not None or sp is not None or tl is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
             with torch.cuda.stream(stream):
@@ -1080,7 +1110,7 @@ class Session:
                 if k % self._wbc == 0:
                     solver.update_dev(self.meas, self.period, self.t_obs, self.x_obs, self.joint_cmd, self.arm_pos, self.last_time, self.cmd54, self.ctl_st, s)
                     acc_st.bitwise_or_(self.ctl_st)
-                if rs is None:
+                if self.k0 is None:
                     self.hw_time.fill_(self.t_start + k * 1e-3)
                 else:   # the robot's episode clock
                     torch.sub(self.k0, k, out=self.dk).neg_(); self.hw_time.copy_(self.dk).mul_(1e-3).add_(self.t_start)
@@ -1091,7 +1121,7 @@ class Session:
                 if sim_timer:
                     sim_timer(True)
                 if push is not None:
-                    kk = k if rs is None else self.dk   # plant steps since the episode's start
+                    kk = k if self.k0 is None else self.dk   # plant steps since the episode's start
                     torch.where(((push["on"] <= kk) & (push["off"] > kk))[:, None], push["wrench"], push["zero"], out=push["now"])
                 solver.sim_step_dev(1e-3, self.effort, q, v, rbd, contact, self.sim_st, s, wrench=None if push is None else push["now"])
                 if sim_timer:
@@ -1159,19 +1189,8 @@ class Session:
                 raise ValueError("closed_loop.Session.command: %s must have shape %s, got %s" % (name, shape, tuple(np.shape(a))))
         if not self._open or self._finished:
             raise ValueError("closed_loop.Session.command: the session is not open (enter it with `with`; finish() ends it)")
-        dev = self.device
-        if dev.type == "cuda":   # rows the caller wrote on its own stream are complete before the session's stream reads them
-            self.stream.wait_stream(torch.cuda.current_stream(dev))
-
-        def put(a, dtype, shape, fill):
-            if a is None:
-                return torch.full(shape, fill, dtype=dtype, device=dev)
-            if isinstance(a, torch.Tensor):
-                t = a.to(device=dev, dtype=dtype).contiguous()
-                if t.is_cuda:   # the caller may free it before the session's stream has read it: its memory waits for that stream
-                    t.record_stream(self.stream)
-                return t
-            return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64 if dtype == torch.float64 else np.int32), device=dev)
+        self._wait_caller()
+        put = self._put
         with torch.cuda.stream(self.stream):
             m = put(mask, torch.int32, (B,), 0); tmpl = put(gait, torch.int32, (B,), -1); vel = put(cmd_vel, torch.float64, (B, 4), np.nan)
             goal = put(ee_goal, torch.float64, (B, 7), np.nan); eev = put(ee_cmd_vel, torch.float64, (B, 3), np.nan)
@@ -1182,6 +1201,80 @@ class Session:
             self.solver.gait_dev_command_dev(m, tmpl, vel, kind, ee, self.cmd_st, self._s)
             self.cmd_acc.bitwise_or_(self.cmd_st)
         self._commanded = True
+
+    def _wait_caller(self):   # rows the caller wrote on its own stream are complete before the session's stream reads them
+        import torch
+        if self.device.type == "cuda":
+            self.stream.wait_stream(torch.cuda.current_stream(self.device))
+
+    def _put(self, a, dtype, shape, fill):   # a caller's rows (device tensor, host array or None: fill) as a tensor the session's stream may read
+        import torch
+        dev = self.device
+        if a is None:
+            return torch.full(shape, fill, dtype=dtype, device=dev)
+        if isinstance(a, torch.Tensor):
+            t = a.to(device=dev, dtype=dtype).contiguous()
+            if t.is_cuda:   # the caller may free it before the session's stream has read it: its memory waits for that stream
+                t.record_stream(self.stream)
+            return t
+        return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64 if dtype == torch.float64 else np.int32), device=dev)
+
+    def _branchable(self, who):   # ValueError where snapshots do not apply: finish() rebuilds per-episode rows from (robot, episode)
+        used = [k for k, key in (("respawn", "rs"), ("randomize", "rz"), ("spawn", "sp"), ("timeline", "tl"), ("curriculum", "cu")) if self._spec[key] is not None]
+        if used:
+            raise ValueError("closed_loop.Session.%s: snapshots cannot go with %s (a branched robot would break the per-episode rows finish() rebuilds "
+                             "from robot and episode)" % (who, ", ".join(used)))
+        if not self._open or self._finished:
+            raise ValueError("closed_loop.Session.%s: the session is not open (enter it with `with`; finish() ends it)" % who)
+
+    def snapshot(self):
+        """A Snapshot of every robot at the current window boundary: the library's rows (Solver.robot_state_save_dev) and device clones of the loop's
+        per-robot rows.  Enqueued on self.stream, no synchronisation.  ValueError with respawn, randomize, spawn, timeline or curriculum."""
+        import torch
+        self._branchable("snapshot")
+        with torch.cuda.stream(self.stream):
+            buf = torch.empty(self.B * self.solver.robot_state_bytes(), dtype=torch.uint8, device=self.device)
+            desc = self.solver.robot_state_save_dev(buf, self._s)
+            rows = [a.clone() for a in self.rows]
+            k0 = self.k0.clone() if self.k0 is not None else torch.zeros(self.B, dtype=torch.int64, device=self.device)
+        return Snapshot(self, buf, desc, rows, k0, self._k)
+
+    def restore(self, snap, mask=None, source=None):
+        """Each robot b with mask[b] set (device tensor [B], as command takes; None: every robot) takes robot source[b]'s rows of snap (int32 [B]; None:
+        its own): the library's and the loop's, and its clock, so that it resumes where the source was when snap was taken.  Applied in stream order at
+        the current window boundary, before the next MPC tick.  A source outside [0, B) leaves the robot untouched and OR-s _lib.ST_RESTORE into the
+        record of the window that tick opens.  Enqueued on self.stream after the caller's current stream, no synchronisation.  ValueError, before any
+        write, for a snapshot of another or a finished session, one the library refuses (a component reset, stopped or re-allocated since, a settings
+        array set or cleared since), one taken at window 0 (after the first MPC tick) restored at a later boundary or the reverse, and as snapshot()."""
+        import torch
+        from ._lib import QmbError
+        self._branchable("restore")
+        B = self.B
+        if not isinstance(snap, Snapshot) or snap.session is not self:
+            raise ValueError("closed_loop.Session.restore: the snapshot belongs to another session")
+        if (snap.k == 0) != (self._k == 0):
+            raise ValueError("closed_loop.Session.restore: a snapshot of window 0 (taken after the first MPC tick) restores only at window 0, and a later one "
+                             "only at a later boundary (before its MPC tick)")
+        for name, a in (("mask", mask), ("source", source)):
+            if a is not None and tuple(np.shape(a)) != (B,):
+                raise ValueError("closed_loop.Session.restore: %s must have shape (%d,), got %s" % (name, B, tuple(np.shape(a))))
+        self._wait_caller()
+        with torch.cuda.stream(self.stream):
+            m = self._put(mask, torch.int32, (B,), 1); src = None if source is None else self._put(source, torch.int32, (B,), 0)
+            try:
+                self.solver.robot_state_load_dev(snap.buf, snap.desc, m, src, self.restore_st, self._s)
+            except QmbError as e:
+                raise ValueError("closed_loop.Session.restore: the library refuses the snapshot: %s" % e) from None
+            ok = m.bool() if src is None else m.bool() & (src >= 0) & (src < B)
+            idx = torch.arange(B, device=self.device) if src is None else src.long().clamp(0, B - 1)
+            for a, a0 in zip(self.rows, snap.rows):
+                a.copy_(torch.where(ok.view((B,) + (1,) * (a.dim() - 1)), a0[idx], a))
+            if self.k0 is None:   # from now on every robot runs on its own clock; k0 = 0 gives the global one
+                self.k0 = torch.zeros(B, dtype=torch.int64, device=self.device); self.dk = torch.zeros_like(self.k0)
+            self.k0.copy_(torch.where(ok, self._k - (snap.k - snap.k0[idx]), self.k0))
+            self.acc_st.bitwise_or_(self.restore_st)
+        if self._spec["gd"] is not None:   # the restored robots' pending commands' status goes into the window the tick opens
+            self._commanded = True
 
     @property
     def gait_templates(self):
@@ -1198,7 +1291,7 @@ class Session:
         import torch
         rs, cu = self._spec["rs"], self._spec["cu"]
         with torch.cuda.stream(self.stream):
-            clock = (self._k - self.k0).to(torch.float64) * 1e-3 if rs is not None else torch.full((self.B,), self._k * 1e-3, dtype=torch.float64, device=self.device)
+            clock = (self._k - self.k0).to(torch.float64) * 1e-3 if self.k0 is not None else torch.full((self.B,), self._k * 1e-3, dtype=torch.float64, device=self.device)
         return dict(q=self.q, v=self.v, rbd=self.rbd, meas=self.meas, x_obs=self.x_obs, t_obs=self.t_obs, contact=self.contact, cmd=self.cmd7,
                     episode=self.episode if rs is not None else None, fallen=self.fallen if rs is not None else None, due=self.due if rs is not None else None,
                     level=self.cu_level if cu is not None else None, clock=clock)

@@ -39,9 +39,10 @@ using namespace qmb;
 
 static thread_local std::string g_create_error;
 
-// A per-robot array the kernels read, `width` doubles per robot: the host copy (empty = not set) and its device copy, allocated on the first set.
+// A per-robot array the kernels read, `width` doubles per robot: the host copy (empty = not set) and its device copy, allocated on the first set; gen
+// moves whenever the array is set after being clear or cleared after being set, so that a robot-state snapshot can tell its rows no longer apply.
 struct RobotArray {
-  int width; std::vector<double> host; double* d = nullptr;
+  int width; std::vector<double> host; double* d = nullptr; uint64_t gen = 0;
   const double* dev() const { return host.empty() ? nullptr : d; }
 };
 
@@ -75,6 +76,7 @@ struct qmb200_handle {
   static constexpr int MAX_CHUNKS = 8;
   TargetParams target_prm{}; ControlLawParams law_prm{0, 0.0, 0.5};   // controller-side constants (capi_ctrl.inc)
   double hw_delay = 0.0; double *hw_ring_cmd = nullptr, *hw_ring_stamp = nullptr; int32_t* hw_ring_state = nullptr;   // QMHWSim command-delay FIFO
+  uint64_t hw_gen = 0;   // generation of the FIFO: qmb200_hw_set_delay empties it
   void* comm = nullptr; int comm_ranks = 0, comm_rank = 0; double* d_send = nullptr;   // NCCL communicator of this handle (capi_comm.inc) and the packed torque rows
   SimParams sim_prm{};   // plant step (capi_sim.inc)
   RobotArray mu{1}, payload{8};   // per-robot plant variation (qmb200_sim_set_robot_params)
@@ -93,6 +95,7 @@ struct qmb200_handle {
     double* d_t = nullptr; int32_t* d_tmpl = nullptr; double* d_vel = nullptr; int n_cmd = 0; double stance_time = 0.0;
     int32_t* d_ee_kind = nullptr; double* d_ee = nullptr;   // the timeline's end-effector commands [B][n_cmd] and [B][n_cmd][7], NULL when it has none
     GsPending* d_pending = nullptr;                          // each robot's pending command (qmb200_gait_dev_command) [B], allocated with d_robots
+    uint64_t tl_gen = 0;                                     // generation of the command timeline: moves whenever it is freed or replaced
   } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   bool plant_on_device = false, tuning_on_device = false;   // an episode draw wrote mu / payload or tuning on the device: plant_ / tuning_rows_sync refresh them
@@ -154,7 +157,10 @@ int set_robot_arrays(qmb200_handle* h, std::initializer_list<RobotRows> sets) {
   for (const RobotRows& s : sets) if (s.rows && !s.a->d && !dalloc(h, &s.a->d, B * s.a->width)) return -4;
   QMB_CUDA(h, cudaDeviceSynchronize());
   for (const RobotRows& s : sets) if (s.rows) QMB_CUDA(h, cudaMemcpy(s.a->d, s.rows, B * s.a->width * 8, cudaMemcpyHostToDevice));
-  for (const RobotRows& s : sets) { if (s.rows) s.a->host.assign(s.rows, s.rows + B * s.a->width); else s.a->host.clear(); }
+  for (const RobotRows& s : sets) {
+    if (!s.rows != s.a->host.empty()) s.a->gen += 1;
+    if (s.rows) s.a->host.assign(s.rows, s.rows + B * s.a->width); else s.a->host.clear();
+  }
   return 0;
 }
 

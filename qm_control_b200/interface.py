@@ -694,6 +694,40 @@ class Solver:
         """Free the start image."""
         self._call("robot_image_clear")
 
+    # ---------------- robot-state snapshots (qmb200_robot_state_*; DESIGN.md §4.17) ----------------
+    def robot_state_bytes(self):
+        """Bytes per robot of a snapshot of the blocks that exist now (_lib.ROBOT_STATE_BLOCKS)."""
+        n = int(self.lib.qmb200_robot_state_bytes(self.h))
+        if n < 0:
+            raise QmbError("qmb200_robot_state_bytes failed (%d)" % n)
+        return n
+
+    def robot_state_save_dev(self, buf, stream=None):
+        """Copy every robot's live rows into buf (a device tensor of at least batch * robot_state_bytes() bytes) in stream order → the descriptor
+        (_lib.RobotStateDesc) a load needs.  One launch, no synchronisation."""
+        desc = _lib.RobotStateDesc()
+        self._call("robot_state_save_dev", _p(buf), buf.numel() * buf.element_size(), C.byref(desc), stream)
+        return desc
+
+    def _state_buf(self, buf, desc):
+        if buf is None or buf.numel() * buf.element_size() < self.batch * desc.bytes:
+            raise QmbError("qmb200_robot_state_load: the buffer holds %d bytes, the snapshot %d" % (0 if buf is None else buf.numel() * buf.element_size(), self.batch * desc.bytes))
+        return _p(buf)
+
+    def robot_state_load_dev(self, buf, desc, mask, source=None, status=None, stream=None):
+        """Every robot b with mask[b] != 0 (int32 [B] device tensor) takes robot source[b]'s rows of the snapshot in buf (int32 [B] device tensor, None:
+        its own); a source outside [0, B) leaves the robot untouched and writes _lib.ST_RESTORE into status[b] (int32 [B] device tensor or None;
+        written, not OR-ed).  One launch, no synchronisation.  Raises, writing nothing, on a short buffer or a snapshot whose blocks no longer match
+        the handle's."""
+        self._call("robot_state_load_dev", self._state_buf(buf, desc), C.byref(desc), _p(mask), _p(source), _p(status), stream)
+
+    def robot_state_load(self, buf, desc, mask, source=None):
+        """Host variant of robot_state_load_dev: numpy mask [B] and source [B] (None: b) → status [B].  Synchronous; buf is a device tensor."""
+        B = self.batch; st = np.zeros(B, dtype=np.int32)
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,)); source = None if source is None else _i32(source, (B,))
+        self._call("robot_state_load", self._state_buf(buf, desc), C.byref(desc), _p(mask), _p(source), _p(st))
+        return st
+
     def fall_detect(self, rbd, count, z_min=0.3, tilt_max=0.3):
         """Host variant of fall_detect_dev: rbd [B, 55], count [B] → (count [B] updated, fallen [B])."""
         B = self.batch; rbd = _f64(rbd, (B, RBD)); count = _i32(count, (B,)).copy(); fallen = np.zeros(B, dtype=np.int32)

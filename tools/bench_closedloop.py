@@ -92,6 +92,13 @@ start at least 1 s before the run's end); the same bins from a control run of 5 
 flat tile; the wall time per simulated second of --duration runs without spawn, with spawn ranges fixed at the run's values and with the draws (all
 with respawn on the library), alternated in one process; and the device time per call of the spawn sampler against the plant step (CUDA events,
 alternated blocks).
+
+--snapshot times robot-state snapshots (closed_loop.Session.snapshot / restore) with every component running (payload and state estimators, attitude
+filter, slip detector, terrain with a ground map, per-robot friction, payload, model payload and tuning rows, a commands timeline with a gait switch and
+an end-effector goal, metrics).  It prints one JSON line "snapshot" with the held blocks, the library's and the session's bytes per robot, the device
+time per save and per load of every robot from a permuted source (CUDA events, alternated blocks) with the copy bandwidth they reach (bytes read and
+written) beside the H100's 3.35 TB/s, and the wall time per simulated second of a session stepped one window at a time without a restore and with a
+snapshot and a branch of every robot every window, alternated; the card's name and power limit are read in the same process.
 """
 import argparse
 import json
@@ -1112,6 +1119,70 @@ def session_main(args, reps=2):
                       "times": command_times(solver)}))
 
 
+
+def snapshot_main(args, reps=7, calls=10, sim_reps=2):
+    """Robot-state snapshots (DESIGN.md §4.17) with every component running and a commands timeline: bytes per robot, device time per save and per
+    load of every robot from a permuted source (CUDA events, alternated blocks of `calls`, median of reps) with the copy bandwidth (bytes read +
+    written) against the H100's 3.35 TB/s, and wall time per simulated second of a Session stepped one window at a time without a restore and with a
+    snapshot and a branch of every robot every window (alternated, best of sim_reps)."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    from qm_control_b200 import terrain as TR
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    B = args.batch; sim_s = args.duration; solver = q.Solver(batch=B, device=0); rng = np.random.default_rng(0)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    ter = dict(tiles=np.stack([TR.ramp(5.0), TR.rough(0.01, seed=3)]), cell=TR.CELL, tile=(np.arange(B) % 3 - 1).astype(np.int32), origin=TR.centred_origin(xy[:, :2]))
+    t = np.tile([0.2, 0.5], (B, 1)); goal = np.full((B, 2, 7), np.nan); goal[:, 1] = [0.55, 0.0, 0.45, 0.0, 0.0, 0.0, 1.0]
+    commands = dict(t=t, gait=[["pace", None]] * B, cmd_vel=np.full((B, 2, 4), np.nan), ee_goal=goal)
+    kw = dict(gait=args.gait, cmd_vel=(args.vx, 0.0, 0.0, 0.0), xy_yaw=xy, terrain=ter, friction_mu=rng.uniform(0.5, 0.9, B), payload=np.c_[rng.uniform(0, 0.5, B), np.zeros((B, 7))],
+              model_payload="plant", tuning=dict(kp_swing=rng.uniform(300.0, 400.0, B)), payload_estimator=True, state_estimator=True, attitude_filter=True,
+              slip_detector=True, ground_map=True, commands=commands, metrics=True)
+    perm = torch.as_tensor(rng.permutation(B).astype(np.int32), device="cuda:0")
+
+    def stepped(branch, duration):
+        with closed_loop.Session(solver, duration, **kw) as ss:
+            for _ in range(ss.windows):
+                if branch:
+                    ss.restore(ss.snapshot(), source=perm)
+                ss.step(1)
+            return ss.finish()
+
+    with closed_loop.Session(solver, 0.05, **kw) as ss:
+        ss.step(2); st = ss._s; per_robot = solver.robot_state_bytes()
+        snap = ss.snapshot(); loop_bytes = snap.nbytes - B * per_robot
+        blocks = [n for i, n in enumerate(_lib.ROBOT_STATE_BLOCKS) if (snap.desc.blocks >> i) & 1]
+        buf = torch.empty(B * per_robot, dtype=torch.uint8, device=ss.device); ones = torch.ones(B, dtype=torch.int32, device=ss.device)
+        calls_of = {"save": lambda: solver.robot_state_save_dev(buf, st), "load": lambda: solver.robot_state_load_dev(snap.buf, snap.desc, ones, perm, None, st)}
+        times = {k: [] for k in calls_of}
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                torch.cuda.synchronize()
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(ss.stream)
+                for _ in range(calls):
+                    call()
+                b.record(ss.stream); torch.cuda.synchronize()
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+        ss.finish()
+    name, limit = card()   # read in the same call as the timings
+    modes = {"no_restore": lambda d: stepped(False, d), "branch_every_window": lambda d: stepped(True, d)}
+    for f in modes.values():   # warm-up: every shape of the timed runs
+        f(0.03)
+    wall = {k: [] for k in modes}
+    for _ in range(sim_reps):
+        for k, f in modes.items():
+            torch.cuda.synchronize(); t0 = time.perf_counter(); f(sim_s); torch.cuda.synchronize(); wall[k].append((time.perf_counter() - t0) / sim_s)
+    moved = 2.0 * B * per_robot   # every robot's rows read once and written once
+    print(json.dumps({"metric": "snapshot", "gpu": name, "power_limit": limit, "batch": B, "gait": args.gait, "sim_s": sim_s, "blocks": blocks,
+                      "library_bytes_per_robot": per_robot, "loop_bytes_per_robot": loop_bytes / B, "snapshot_bytes": snap.nbytes,
+                      "label": "device time per call on %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+                      **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}, "ms_all": times,
+                      **{"tb_per_s_%s" % k: moved / (float(np.median(v)) * 1e-3) / 1e12 for k, v in times.items()}, "hbm_tb_per_s_datasheet": 3.35,
+                      "wall_s_per_sim_s": {k: float(min(v)) for k, v in wall.items()}, "wall_s_per_sim_s_all": wall}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8192); ap.add_argument("--duration", type=float, default=1.0)
@@ -1136,11 +1207,15 @@ def main():
                                                             "wall time, falls and velocity error per transition")
     ap.add_argument("--curriculum", action="store_true", help="with --respawn: per-robot levels stepped from each episode's outcome: update time, wall time, "
                                                               "an up-down staircase on the push against a uniform sweep")
+    ap.add_argument("--snapshot", action="store_true", help="robot-state snapshots with every component running: bytes per robot, save and load times, and a "
+                    "session branching every robot every window against one without restores")
     ap.add_argument("--session", action="store_true", help="closed_loop.run against a Session stepped one window at a time, without commands and with a "
                                                            "torch heading controller's command every window: wall time per simulated second, the command kernel's time")
     args = ap.parse_args()
     if args.session:
         return session_main(args)
+    if args.snapshot:
+        return snapshot_main(args)
     if args.curriculum and not args.respawn:
         ap.error("--curriculum needs --respawn")
     if args.curriculum:
