@@ -586,8 +586,9 @@ int qmb200_slip_stop(qmb200_handle* h);
  *      The start image holds, per robot, the rows of every component running when it is saved: the state estimator, attitude filter, slip detector and
  *      payload estimator states, the model payload rows (qmb200_set_model_payload, as a commit may have left them) and the device gait schedule with
  *      its timeline cursor.  Handle settings (parameters, tuning rows, plant robot params, terrain, ground map, gait templates, command timeline) are not
- *      state and are never written.  The gait schedule's pending command slots (qmb200_gait_dev_command) are cleared, not imaged.  Each reset, stop
- *      or re-allocation of an imaged component (and qmb200_gait_dev_set_commands, which resets the cursors) makes the image stale for it. */
+ *      state and are never written.  The gait schedule's pending command slots (qmb200_gait_dev_command) are cleared, not imaged.  The image is the
+ *      handle's own robot-state snapshot (below) of blocks 0-7, with their generations: each reset, stop or re-allocation of an imaged component (and
+ *      qmb200_gait_dev_set_commands, which resets the cursors) makes the image stale for it. */
 /* Saves the image of the components running now, replacing any previous one.  Synchronous. */
 int qmb200_robot_image_save(qmb200_handle* h);
 /* Frees the image (qmb200_destroy does too).  Clearing when none is saved does nothing and returns 0. */
@@ -595,8 +596,8 @@ int qmb200_robot_image_clear(qmb200_handle* h);
 /* One launch, no host work: for every robot with mask[b] != 0 the imaged rows return to the image, both MPC warm-start sides forget the robot's
  * solution (n_nodes = 0, what qmb200_mpc_reset does for all), its WBC last input is zeroed, its hw_write FIFO emptied and, while the device gait
  * schedule runs, its pending command dropped (a command decided on the old episode's state never reaches the new one).  Robots with mask[b] == 0
- * are not written.  Fails, naming the component and writing nothing, when no image is saved, an imaged component was stopped, reset or re-allocated
- * since, or a component runs that was not imaged. */
+ * are not written.  Fails, naming the block and writing nothing, when no image is saved or, as qmb200_robot_state_load_dev does for blocks 0-7, an
+ * imaged block was reset, stopped or re-allocated since or no longer exists, or one of those blocks exists now that was not imaged. */
 int qmb200_robot_image_restore(qmb200_handle* h, const int32_t* mask /*[B]*/);
 int qmb200_robot_image_restore_dev(qmb200_handle* h, const int32_t* mask /*[B] device*/, void* cuda_stream);
 

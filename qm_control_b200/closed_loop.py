@@ -733,6 +733,12 @@ def _metrics_episodes(ticks, rs):
     return (ticks - 1) // max(shortest, 1) + 1
 
 
+def _gather(rows, src_rows, ok, idx=None):   # every robot b with ok[b] (bool [B]) takes row idx[b] (None: b) of each src_rows tensor into rows
+    import torch
+    for a, a0 in zip(rows, src_rows):
+        a.copy_(torch.where(ok.view((ok.shape[0],) + (1,) * (a.dim() - 1)), a0 if idx is None else a0[idx], a))
+
+
 class Snapshot:
     """Every robot of a Session at one window boundary (Session.snapshot; DESIGN.md §4.17): buf, the library's rows (uint8 device tensor), desc, what
     they hold (_lib.RobotStateDesc), rows, device clones of the loop's per-robot rows (Session.rows), k0 [B], each robot's clock origin then, and k, the
@@ -1026,7 +1032,6 @@ class Session:
         solver.mpc_solve_dev(prob, s)
 
     def _respawn(self, k):   # the robots due restart at window boundary k: their episode closes, their level moves, then the library's rows, the loop's, their new plant
-        import torch
         solver, s, cu, due = self.solver, self._s, self._spec["cu"], self.due
         if self._mt or cu is not None:
             self.mt_end.copy_(self.due_fall).neg_().add_(2)   # 1: the fall rule, 2: every
@@ -1036,9 +1041,8 @@ class Session:
             solver.curriculum_update_dev(due, self.mt_end, self.episode, self.mt_out if self._mt else None, self.cu_level, self.acc_st, s)
         solver.robot_image_restore_dev(due, s)
         m = due.bool()
-        for a, a0 in zip(self.own, self.start):
-            a.copy_(torch.where(m.view((self.B,) + (1,) * (a.dim() - 1)), a0, a))
-        self.k0.copy_(torch.where(m, k, self.k0)); self.episode.add_(due); self.fall_count.masked_fill_(m, 0)
+        _gather(self.own + [self.k0], self.start + [k], m)   # their rows return to the start, their clock origin to k
+        self.episode.add_(due); self.fall_count.masked_fill_(m, 0)
         if cu is not None:
             self._level_begun(due)
         self._begin(due, self.episode)
@@ -1059,15 +1063,13 @@ class Session:
             solver.timeline_sample_dev(mask, idx, self.tl_rows, s)
 
     def _draw(self, mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
-        import torch
         ep_rows, push = self.ep_rows, self.push
         self.solver.episode_sample_dev(mask, idx, ep_rows, self._spec["rz"]["link"], self._s)
         m = mask.bool()
-        self.cmd7[:, :4] = torch.where(m[:, None], ep_rows[:, 23:27], self.cmd7[:, :4])
+        _gather([self.cmd7[:, :4]], [ep_rows[:, 23:27]], m)
         if push is not None:
             on = ep_rows[:, 9] * 1e3 - 1e-6; off = (ep_rows[:, 9] + ep_rows[:, 10]) * 1e3 - 1e-6
-            push["on"].copy_(torch.where(m, on, push["on"])); push["off"].copy_(torch.where(m, off, push["off"]))
-            push["wrench"].copy_(torch.where(m[:, None], ep_rows[:, 11:23], push["wrench"]))
+            _gather([push["on"], push["off"], push["wrench"]], [on, off, ep_rows[:, 11:23]], m)
 
     # ------------------------------------------------------------------------------------------------------------------------------------ public
     def step(self, windows=1):
@@ -1266,12 +1268,10 @@ class Session:
             except QmbError as e:
                 raise ValueError("closed_loop.Session.restore: the library refuses the snapshot: %s" % e) from None
             ok = m.bool() if src is None else m.bool() & (src >= 0) & (src < B)
-            idx = torch.arange(B, device=self.device) if src is None else src.long().clamp(0, B - 1)
-            for a, a0 in zip(self.rows, snap.rows):
-                a.copy_(torch.where(ok.view((B,) + (1,) * (a.dim() - 1)), a0[idx], a))
             if self.k0 is None:   # from now on every robot runs on its own clock; k0 = 0 gives the global one
                 self.k0 = torch.zeros(B, dtype=torch.int64, device=self.device); self.dk = torch.zeros_like(self.k0)
-            self.k0.copy_(torch.where(ok, self._k - (snap.k - snap.k0[idx]), self.k0))
+            idx = None if src is None else src.long().clamp(0, B - 1)
+            _gather(self.rows + [self.k0], snap.rows + [self._k - (snap.k - snap.k0)], ok, idx)   # the rows, and the source's clock shifted to now
             self.acc_st.bitwise_or_(self.restore_st)
         if self._spec["gd"] is not None:   # the restored robots' pending commands' status goes into the window the tick opens
             self._commanded = True

@@ -52,9 +52,10 @@ struct DrawRanges {
   int width; std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0; bool attached = false, on_device = false;
 };
 
-// The components a start image covers (capi_respawn.inc).  Each has a generation that its reset, stop and re-allocation bump, so a restore can tell
-// that the rows it would write no longer belong to the state it imaged.
-enum ImageComponent { IMG_STATE_EST, IMG_ATTITUDE, IMG_SLIP, IMG_PAYLOAD_EST, IMG_MODEL_PAYLOAD, IMG_GAIT, IMG_N };
+// The per-robot state of a filter, `width` doubles per robot on the device (d NULL: not running), and what names it in errors: the filter and the entry
+// point that starts it.  gen moves on every start and stop (filter_start, filter_stop), so that a start image or a robot-state snapshot can tell its rows
+// no longer belong to the state.
+struct FilterState { int width; const char *name, *starter; double* d = nullptr; uint64_t gen = 0; };
 
 struct qmb200_handle {
   HostModel hm;
@@ -84,18 +85,20 @@ struct qmb200_handle {
   struct { std::vector<double> host; double* d = nullptr; int n_tiles = 0, nx = 0, ny = 0; double cell = 0.0; } tiles;   // heightfield library (qmb200_sim_set_terrain)
   RobotArray mpayload{8}, srbd{SRBD_DBL};   // the controller's model payload (qmb200_set_model_payload) and the robots' SRBD constants it gives
   RobotArray tuning{TUNING_DBL};            // per-robot controller parameters (qmb200_set_robot_tuning): Tuning, then the control law's arm kp / kd
-  qmb200_payload_est_params est_prm{}; double* d_est = nullptr;   // payload estimator (capi_est.inc): parameters and state [B][EST_DBL], NULL when not running
+  qmb200_payload_est_params est_prm{}; FilterState est{EST_DBL, "payload estimator", "qmb200_payload_est_reset"};   // payload estimator (capi_est.inc)
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
-  qmb200_state_est_params se_prm{}; double* d_se = nullptr;        // base state estimator: parameters and state [B][SE_DBL], NULL when not running
+  qmb200_state_est_params se_prm{}; FilterState se{SE_DBL, "state estimator", "qmb200_state_est_reset"};   // base state estimator
   RobotArray se_ground{3};        // the estimator's ground map: per-robot [tile, origin_x, origin_y] on the tile library (qmb200_state_est_set_ground)
-  qmb200_attitude_params at_prm{}; double* d_at = nullptr;         // attitude filter (capi_attitude.inc): parameters and state [B][AT_DBL], NULL when not running
-  qmb200_slip_params sl_prm{}; double* d_sl = nullptr;             // slip detector (capi_slip.inc): parameters and state [B][SL_DBL], NULL when not running
+  qmb200_attitude_params at_prm{}; FilterState at{AT_DBL, "attitude filter", "qmb200_attitude_reset"};   // attitude filter (capi_attitude.inc)
+  qmb200_slip_params sl_prm{}; FilterState sl{SL_DBL, "slip detector", "qmb200_slip_reset"};             // slip detector (capi_slip.inc)
+  uint64_t model_gen = 0;   // generation of the model payload rows mpayload / srbd: every qmb200_set_model_payload moves it
   struct {   // device gait schedule (capi_gait.inc): template table, per-robot state (NULL when not running) and command timeline [B][n_cmd]
     std::vector<GsTemplate> table; GsTemplate* d_table = nullptr; GsRobot* d_robots = nullptr; int32_t* d_cursor = nullptr;
     double* d_t = nullptr; int32_t* d_tmpl = nullptr; double* d_vel = nullptr; int n_cmd = 0; double stance_time = 0.0;
     int32_t* d_ee_kind = nullptr; double* d_ee = nullptr;   // the timeline's end-effector commands [B][n_cmd] and [B][n_cmd][7], NULL when it has none
     GsPending* d_pending = nullptr;                          // each robot's pending command (qmb200_gait_dev_command) [B], allocated with d_robots
     uint64_t tl_gen = 0;                                     // generation of the command timeline: moves whenever it is freed or replaced
+    uint64_t gen = 0;                                        // generation of the per-robot state and cursors: reset, set_commands and stop move it
   } gs;
   bool model_on_device = false;   // a commit wrote mpayload / srbd on the device: model_rows_sync refreshes the host copies before they are read
   bool plant_on_device = false, tuning_on_device = false;   // an episode draw wrote mu / payload or tuning on the device: plant_ / tuning_rows_sync refresh them
@@ -115,9 +118,8 @@ struct qmb200_handle {
     qmb200_curriculum_rule rule{}; std::vector<double> rows; std::vector<int32_t> state; double* d_rows = nullptr; int32_t* d_state = nullptr; bool on_device = false;
     struct Kind { std::vector<double> base_lo, base_hi, top_lo, top_hi; double* d = nullptr; } kind[CU_KINDS];
   } cur;
-  uint64_t gen[IMG_N] = {};       // generation of each imaged component (ImageComponent)
-  struct {                        // start image (qmb200_robot_image_save): the running components' rows, one block after the other in d
-    bool saved = false; char* d = nullptr; bool on[IMG_N] = {}; uint64_t gen[IMG_N] = {};
+  struct {   // start image (qmb200_robot_image_save): a robot-state snapshot of the blocks of its components (capi_respawn.inc) in d, described by desc
+    bool saved = false; char* d = nullptr; qmb200_robot_state_desc desc{};
   } image;
   int chunks = 1; cudaStream_t cs[MAX_CHUNKS] = {nullptr}; cudaEvent_t fork_ev = nullptr, join_ev[MAX_CHUNKS] = {nullptr};
 };
@@ -161,6 +163,37 @@ int set_robot_arrays(qmb200_handle* h, std::initializer_list<RobotRows> sets) {
     if (!s.rows != s.a->host.empty()) s.a->gen += 1;
     if (s.rows) s.a->host.assign(s.rows, s.rows + B * s.a->width); else s.a->host.clear();
   }
+  return 0;
+}
+
+// The lifecycle of a filter state (FilterState).  Every entry point that reads the state fails, as `who`, while the filter is not running.
+int filter_required(qmb200_handle* h, const FilterState& f, const char* who) {
+  if (!f.d) return fail(h, std::string(who) + ": the " + f.name + " is not running (" + f.starter + " starts it)");
+  return 0;
+}
+// (Re)starts the filter with rows [B][width] (NULL: zeros).  No queued step may still read the state, and a copy from pageable memory may return before
+// its DMA lands while a step on a non-blocking stream would not wait for it: wait for the device before and after.
+int filter_start(qmb200_handle* h, FilterState& f, const double* rows) {
+  const size_t bytes = (size_t)h->B * f.width * 8;
+  QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());
+  f.gen += 1;
+  if (!f.d) QMB_CUDA(h, cudaMalloc(&f.d, bytes));
+  if (rows) QMB_CUDA(h, cudaMemcpy(f.d, rows, bytes, cudaMemcpyHostToDevice)); else QMB_CUDA(h, cudaMemset(f.d, 0, bytes));
+  QMB_CUDA(h, cudaDeviceSynchronize());
+  return 0;
+}
+// The rows [B][width] of a running filter, once every queued step has written them
+int filter_read(qmb200_handle* h, const FilterState& f, std::vector<double>& rows) {
+  rows.resize((size_t)h->B * f.width);
+  QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());
+  QMB_CUDA(h, cudaMemcpy(rows.data(), f.d, rows.size() * 8, cudaMemcpyDeviceToHost));
+  return 0;
+}
+// Releases the state; stopping a filter that is not running does nothing
+int filter_stop(qmb200_handle* h, FilterState& f) {
+  if (!f.d) return 0;
+  QMB_CUDA(h, cudaSetDevice(h->device)); QMB_CUDA(h, cudaDeviceSynchronize());   // no queued step still reads the state
+  QMB_CUDA(h, cudaFree(f.d)); f.d = nullptr; f.gen += 1;
   return 0;
 }
 
@@ -266,10 +299,7 @@ void qmb200_destroy(qmb200_handle* h) {
   if (h->fork_ev) cudaEventDestroy(h->fork_ev);
   for (void* p : h->allocs) cudaFree(p);
   if (h->tiles.d) cudaFree(h->tiles.d);
-  if (h->d_est) cudaFree(h->d_est);
-  if (h->d_se) cudaFree(h->d_se);
-  if (h->d_at) cudaFree(h->d_at);
-  if (h->d_sl) cudaFree(h->d_sl);
+  cudaFree(h->est.d); cudaFree(h->se.d); cudaFree(h->at.d); cudaFree(h->sl.d);
   cudaFree(h->gs.d_table); cudaFree(h->gs.d_robots); cudaFree(h->gs.d_cursor); cudaFree(h->gs.d_t); cudaFree(h->gs.d_tmpl); cudaFree(h->gs.d_vel);
   cudaFree(h->gs.d_ee_kind); cudaFree(h->gs.d_ee); cudaFree(h->gs.d_pending);
   cudaFree(h->image.d);
@@ -384,7 +414,7 @@ int qmb200_set_model_payload(qmb200_handle* h, const double* payload) {
   std::vector<double> srbd; if (payload) { srbd.resize(B * SRBD_DBL); srbd_rows(h->hm, payload, B, srbd.data()); }
   const int rc = set_robot_arrays(h, {{&h->mpayload, payload}, {&h->srbd, payload ? srbd.data() : nullptr}});
   if (!rc) h->model_on_device = false;   // set_robot_arrays waited for the device: the rows just written replace any committed ones
-  h->gen[IMG_MODEL_PAYLOAD] += 1;
+  h->model_gen += 1;
   return rc;
 }
 int qmb200_get_model_payload(const qmb200_handle* h, double* payload, int32_t* is_set) {
