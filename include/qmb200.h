@@ -41,6 +41,7 @@ extern "C" {
  *                           bit 16      QMB200_ST_SAFETY — qmb200_update / qmb200_control_law
  *                           bit 17      QMB200_ST_COMMAND — qmb200_gait_dev_command(_dev), a rejected command row
  *                           bit 18      QMB200_ST_RESTORE — qmb200_robot_state_load(_dev), a source robot outside [0, B)
+ *                           bit 19      QMB200_ST_SPAWN — qmb200_spawn_place(_dev), a rejected spawn row
  * Nothing else is ever OR-ed into a status word: the WBC's iteration counts live in qmb200_wbc_get_diagnostics. */
 #define QMB200_ST_ITER_CAP 1
 #define QMB200_ST_OVERFLOW 2      /* WBC: more rows than the working-set / level-0 buffers hold; MPC: node count > NMAX, event / target count out of range, swing phase not enclosed */
@@ -333,6 +334,8 @@ int qmb200_gait_dev_stop(qmb200_handle* h);
 #define QMB200_ST_COMMAND 0x20000    /* qmb200_gait_dev_command(_dev): the robot's command row was rejected (no other status word uses this bit) */
 #define QMB200_ST_RESTORE (QMB200_ST_COMMAND << 1)   /* qmb200_robot_state_load(_dev): the robot's source row lies outside [0, B), the robot was not written
                                                         (bit 18; no other status word uses it) */
+#define QMB200_ST_SPAWN (QMB200_ST_RESTORE << 1)     /* qmb200_spawn_place(_dev): the robot's spawn row was rejected, the robot was not written (bit 19; no
+                                                        other status word uses it) */
 #define QMB200_ST_HW_RING_FULL 2     /* qmb200_hw_write: more than 32 commands inside the delay window (the oldest was dropped) */
 
 /* QMController::updateStateEstimation tail (QMController.cpp:236-243): t_obs += period; x_obs = computeCentroidalStateFromRbdModel(rbd) with
@@ -709,6 +712,25 @@ int qmb200_spawn_sample(qmb200_handle* h, const int32_t* mask /*[B]*/, const int
                         double* x_obs /*[B][30] in-out*/, double* last_ee /*[B][7] in-out*/, double* rbd_est /*[B][55] in-out or NULL*/);
 int qmb200_spawn_sample_dev(qmb200_handle* h, const int32_t* mask, const int32_t* episode, int32_t link, double* rows, double* q, double* v, double* rbd, int32_t* contact,
                             double* x_obs, double* last_ee, double* rbd_est, void* cuda_stream);
+/* One launch, no host work (DESIGN.md §4.18): every robot with mask[b] != 0 stands on the given row rows[b] exactly as qmb200_spawn_sample_dev stands a
+ * robot on a drawn row, writing the same buffers and rows; its offsets count from origin[b] (the tile's origin becomes origin[b] - (dx, dy)).  No ranges
+ * are needed.  The row is checked on the device: the tile an integer in [-1, n_tiles) of the library in force, a tile >= 0 only where the plant has
+ * robot terrain rows, dx and dy finite, the yaw in [-pi, pi].  A rejected robot is not written and gets status[b] = QMB200_ST_SPAWN; status [B] is
+ * written, not OR-ed: 0 for accepted robots and for robots with mask[b] == 0, which are not written.  Fails, writing nothing, on a NULL buffer (rbd_est
+ * may be NULL), unknown link bits, or the ground-map link without a map. */
+int qmb200_spawn_place(qmb200_handle* h, const int32_t* mask /*[B]*/, const double* rows /*[B][QMB200_SPAWN]*/, const double* origin /*[B][2]*/, int32_t link,
+                       double* q /*[B][24] in-out*/, double* v /*[B][24] in-out*/, double* rbd /*[B][55] in-out*/, int32_t* contact /*[B] in-out*/,
+                       double* x_obs /*[B][30] in-out*/, double* last_ee /*[B][7] in-out*/, double* rbd_est /*[B][55] in-out or NULL*/, int32_t* status /*[B]*/);
+int qmb200_spawn_place_dev(qmb200_handle* h, const int32_t* mask, const double* rows, const double* origin, int32_t link, double* q, double* v, double* rbd,
+                           int32_t* contact, double* x_obs, double* last_ee, double* rbd_est, int32_t* status, void* cuda_stream);
+/* One launch, no host work (DESIGN.md §4.18): every robot with mask[b] != 0 writes into rows[b] the spawn row that, once the robot is back at its start
+ * pose q_start[b] and placed with qmb200_spawn_place(_dev) and the same origin, stands it on the ground point under its base now (rbd[b]) with its
+ * heading now: tile = the plant's robot terrain tile (-1 without robot terrain rows), (dx, dy) = (x - x_start, y - y_start) + (origin - the robot
+ * terrain origin now) (origin itself without rows), yaw = rbd[b]'s yaw wrapped into [-pi, pi].  On the plane only the heading carries over: a spawn
+ * keeps the base's world x, y.  Rows of robots with mask[b] == 0 are not written.  Fails, writing nothing, on a NULL buffer. */
+int qmb200_spawn_here(qmb200_handle* h, const int32_t* mask /*[B]*/, const double* rbd /*[B][55]*/, const double* q_start /*[B][24]*/, const double* origin /*[B][2]*/,
+                      double* rows /*[B][QMB200_SPAWN] in-out*/);
+int qmb200_spawn_here_dev(qmb200_handle* h, const int32_t* mask, const double* rbd, const double* q_start, const double* origin, double* rows, void* cuda_stream);
 /* Host only: the rows [n][QMB200_SPAWN] of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the sampler draws. */
 int qmb200_spawn_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][QMB200_SPAWN]*/);
 

@@ -12,6 +12,7 @@ GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
 TARGET_CMD_VEL, TARGET_EE_CMD_VEL, TARGET_EE_GOAL = 0, 1, 2   # QMB200_TARGET_*: the target front-end's kinds (-1 in a per-robot kind: a held goal)
 ST_COMMAND = 0x20000   # QMB200_ST_COMMAND: a rejected qmb200_gait_dev_command row
 ST_RESTORE = 0x40000   # QMB200_ST_RESTORE: a qmb200_robot_state_load source row outside [0, B)
+ST_SPAWN = 0x80000     # QMB200_ST_SPAWN: a rejected qmb200_spawn_place row
 
 dp = C.POINTER(C.c_double)
 ip = C.POINTER(C.c_int32)
@@ -272,6 +273,10 @@ PROTOTYPES = {
     "qmb200_spawn_get_ranges": (I32, [P] * 5),
     "qmb200_spawn_sample": (I32, [P, P, P, I32] + [P] * 8),
     "qmb200_spawn_sample_dev": (I32, [P, P, P, I32] + [P] * 9),
+    "qmb200_spawn_place": (I32, [P, P, P, P, I32] + [P] * 8),
+    "qmb200_spawn_place_dev": (I32, [P, P, P, P, I32] + [P] * 9),
+    "qmb200_spawn_here": (I32, [P] * 6),
+    "qmb200_spawn_here_dev": (I32, [P] * 7),
     "qmb200_spawn_draw": (I32, [P, I32, P, P, P]),
     "qmb200_metrics_step": (I32, [P, D] + [P] * 12),
     "qmb200_metrics_step_dev": (I32, [P, D] + [P] * 13),

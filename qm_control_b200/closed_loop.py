@@ -115,7 +115,11 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     (hold and every: positive multiples of 10 ms).  A respawned robot returns to its start pose, its estimators' and gait schedule's start
     rows and a cold MPC, WBC and command FIFO, and lives on its own episode clock: its hw_write time, pushes (t_on counts from the episode's start),
     gait commands and mode schedule replay; only the sensor noise keeps the global sample index, so each episode draws new noise.  The image is freed
-    when run returns.
+    when run returns.  at="here" (default "start") restarts a robot where it is (DESIGN.md §4.18): right before its restore the row that stands it on the
+    ground point under its base with its heading (Solver.spawn_here_dev, on the plant's rbd), then the restore, then that row placed
+    (Solver.spawn_place_dev) with the run's start origins in place of a spawn draw; with spawn episode 0 still draws.  Not with a curriculum spawn, a
+    drawn spawn yaw, ee_goal / ee_cmd_vel commands or a ground_map dict.  on_request=True (a Session only; it may stand without on_fall and every) lets
+    Session.respawn end robots' episodes.
     randomize: dict(seed=0, <field>=(lo, hi), ...) draws a new plant for every episode (DESIGN.md §4.11): fields of _lib.EPISODE_LAYOUT (the plant's
     friction_mu and payload columns, push_t_on and push_duration in s from the episode's start, the push wrench columns, cmd_vel_x / _y / _z and
     cmd_yaw_rate), each bound a scalar or [B]; fields not named stay at this run's values (friction_mu, payload, pushes and cmd_vel, else the handle's
@@ -144,7 +148,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     cmd_vel, 1 ee_cmd_vel, 2 goal published, -1 goal held), and ee_target[ticks, B, 7], the final-knot end-effector pose of the target in force after
     that call); with respawn also episode[ticks, B], each robot's episode index in that record's window (0 for the first), and fallen[ticks, B], the
     detector's flag at that window's end; with randomize also episode_params[B, E, 27], the row each robot drew for each episode e < E (E: the most
-    episodes of any robot), NaN where a robot had no episode e; with spawn also spawn_params[B, E, 4], the spawn row of each such episode.
+    episodes of any robot), NaN where a robot had no episode e; with spawn also spawn_params[B, E, 4], the spawn row of each such episode (once any
+    restart placed a robot, with or without spawn, the device's record of every episode's row: drawn, placed, or the start's; NaN for a rejected place).
     metrics: True scores every episode on the device (DESIGN.md §4.13, Solver.metrics_step_dev / metrics_close_dev): after every plant step, once the
     step's status words are in the record's and the estimators have stepped, one sample of the plant's truth (its rbd, contact mask and the effort held
     over the step, the target in force, the robot's episode clock, the record's status word and, with state_estimator, the estimate) goes into each
@@ -175,6 +180,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     integers, every bound a scalar or [B].  The curriculum is cleared before the previous ranges are restored.  Returns also curriculum_level[ticks, B]
     (each robot's level in that record's window), episode_level[B, E] (-1 where a robot had no episode e), curriculum_state[B, CURRICULUM_STATE] at
     the end (_lib.CURRICULUM_STATE_LAYOUT), and each attached kind's *_params drawn at its episode's level."""
+    if isinstance(respawn, dict) and _place_spec(respawn)["on_request"]:
+        raise ValueError("closed_loop.run: respawn on_request needs a Session (nothing can request a restart inside run; Session.respawn does)")
     with Session(solver, duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start, torch_device=torch_device,
                  sim_timer=sim_timer, friction_mu=friction_mu, payload=payload, pushes=pushes, model_payload=model_payload, terrain=terrain,
                  payload_estimator=payload_estimator, state_estimator=state_estimator, sensor_noise=sensor_noise, attitude_filter=attitude_filter,
@@ -200,7 +207,7 @@ def _run_specs(solver, steer, o):
     attitude_filter, slip_detector, model_payload, tuning = (o[k] for k in ("attitude_filter", "slip_detector", "model_payload", "tuning"))
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
-    rs = None if respawn is None else _respawn_spec(respawn)
+    rs = None if respawn is None else dict(_respawn_spec(respawn), **_place_spec(respawn))
     rz = None if randomize is None else _randomize_spec(getattr(solver, "batch", None), randomize)
     if payload_estimator is not None and payload_estimator is not True and not isinstance(payload_estimator, dict):
         raise ValueError("closed_loop.run: payload_estimator must be None, True or a dict of estimator parameters, got %r" % (payload_estimator,))
@@ -238,6 +245,11 @@ def _run_specs(solver, steer, o):
                               terrain, ground_map, gd)
         if cu["gd"] is not None:   # a top box that weighs end-effector commands needs the placeholder timeline's end-effector rows
             gd = tl["gd"] = cu["gd"]
+    if rs is not None and rs["at"] == "here":
+        yaw_drawn = sp is not None and "yaw" in sp["fields"] and np.any(sp["fields"]["yaw"][0] != sp["fields"]["yaw"][1])
+        why = _here_refusal(yaw_drawn, gd, curriculum, ground_map)
+        if why is not None:
+            raise ValueError("closed_loop.run: respawn at=\"here\" cannot go with %s" % why)
     if rz is not None:   # the links: a drawn payload / friction also goes where the run told the controller the plant's
         drawn = set(rz["fields"]) | set(cu["tops"]["episode"]["fields"] if cu is not None and "episode" in cu["tops"] else ())
         if isinstance(model_payload, str) and model_payload == "plant" and drawn & set(_lib.PAYLOAD_LAYOUT):
@@ -250,12 +262,14 @@ def _run_specs(solver, steer, o):
 
 
 def _respawn_spec(respawn):
-    """closed_loop.run's respawn → dict(on_fall, hold_windows, z_min, tilt_max, every_ms or None); ValueError when malformed"""
+    """closed_loop.run's respawn → dict(on_fall, hold_windows, z_min, tilt_max, every_ms or None); ValueError when malformed (_place_spec reads at and
+    on_request)"""
     spec = dict(on_fall=True, hold=0.1, z_min=0.3, tilt_max=0.3, every=None)
+    place = _place_spec(respawn)
     if respawn is not True:
-        if not isinstance(respawn, dict) or not set(respawn) <= set(spec):
-            raise ValueError("closed_loop.run: respawn must be None, True or dict(on_fall, hold, z_min, tilt_max, every), got %r" % (respawn,))
-        spec.update(respawn)
+        if not isinstance(respawn, dict) or not set(respawn) <= set(spec) | set(place):
+            raise ValueError("closed_loop.run: respawn must be None, True or dict(on_fall, hold, z_min, tilt_max, every, at, on_request), got %r" % (respawn,))
+        spec.update({k: v for k, v in respawn.items() if k not in place})
     if not isinstance(spec["on_fall"], (bool, np.bool_)):
         raise ValueError("closed_loop.run: respawn on_fall must be True or False, got %r" % (spec["on_fall"],))
 
@@ -274,9 +288,37 @@ def _respawn_spec(respawn):
             raise ValueError("closed_loop.run: respawn %s must be a finite number, got %r" % (name, spec[name]))
     if not float(spec["tilt_max"]) > 0.0:
         raise ValueError("closed_loop.run: respawn tilt_max must be > 0, got %r" % (spec["tilt_max"],))
-    if not spec["on_fall"] and every is None:
-        raise ValueError("closed_loop.run: respawn needs on_fall or every (it would never restart a robot)")
+    if not spec["on_fall"] and every is None and not place["on_request"]:
+        raise ValueError("closed_loop.run: respawn needs on_fall, every or on_request (it would never restart a robot)")
     return dict(on_fall=bool(spec["on_fall"]), hold_windows=hold // MPC_PERIOD_MS, z_min=float(spec["z_min"]), tilt_max=float(spec["tilt_max"]), every_ms=every)
+
+
+RESPAWN_AT = ("start", "here")   # respawn at: a restart returns to the start pose (or draws the spawn), or stands the robot where it is (DESIGN.md §4.18)
+
+
+def _place_spec(respawn):
+    """closed_loop.run's respawn → dict(at, on_request): where its restarts stand robots and whether a Session may request them; ValueError when malformed"""
+    spec = dict(at="start", on_request=False)
+    if isinstance(respawn, dict):
+        spec.update({k: respawn[k] for k in spec if k in respawn})
+    if not isinstance(spec["on_request"], (bool, np.bool_)):
+        raise ValueError("closed_loop.run: respawn on_request must be True or False, got %r" % (spec["on_request"],))
+    if not isinstance(spec["at"], str) or spec["at"] not in RESPAWN_AT:
+        raise ValueError("closed_loop.run: respawn at must be \"start\" or \"here\", got %r" % (spec["at"],))
+    return dict(at=spec["at"], on_request=bool(spec["on_request"]))
+
+
+def _here_refusal(sp_yaw_drawn, gd, curriculum, ground_map):
+    """why a restart "here" (or on given spawn rows) cannot go with this run's specs, or None: the heading it keeps varies per robot"""
+    if curriculum is not None and "spawn" in curriculum:
+        return "a curriculum attached to the spawn (its levels draw every spawn)"
+    if sp_yaw_drawn:
+        return "a drawn spawn yaw (the heading a restart keeps would not be the draw's)"
+    if gd is not None and gd["ee"]:
+        return "ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)"
+    if isinstance(ground_map, dict):
+        return "a ground_map dict (the map would not follow the ground; ground_map=True does)"
+    return None
 
 
 def _ranges_spec(kind, layout, B, value):
@@ -729,6 +771,8 @@ def _metrics_episodes(ticks, rs):
     after its episode has lasted at least hold windows (on the fall rule) or every (at the limit), whichever is shorter, and at least one window"""
     if rs is None:
         return 1
+    if rs.get("on_request"):   # a request may restart a robot at every boundary
+        return ticks
     shortest = min([rs["hold_windows"]] * rs["on_fall"] + ([rs["every_ms"] // MPC_PERIOD_MS] if rs["every_ms"] is not None else []))
     return (ticks - 1) // max(shortest, 1) + 1
 
@@ -772,7 +816,8 @@ class Session:
     call (Solver.gait_dev_command_dev; DESIGN.md §4.16).
     s.state: the live device tensors (read-only: the loop writes them).  s.finish() closes the open episodes and returns run's end-of-run keys.
     snap = s.snapshot() and s.restore(snap, mask=None, source=None) rewind robots to a window boundary, or branch one robot's state onto others
-    (DESIGN.md §4.17); not with respawn, randomize, spawn, timeline or curriculum.  Sensor noise is a pure function of (seed, robot, plant step k,
+    (DESIGN.md §4.17); not with respawn, randomize, spawn, timeline or curriculum.
+    s.respawn(mask, end=2, at=None) restarts robots at the next boundary (respawn=dict(..., on_request=True); DESIGN.md §4.18).  Sensor noise is a pure function of (seed, robot, plant step k,
     channel): a rewound or branched robot draws fresh noise, so exact replay needs the noise off.
     run(solver, duration, **kw) is Session + one step(windows) + finish()."""
 
@@ -786,6 +831,11 @@ class Session:
         sp, cu = self._spec["sp"], self._spec["cu"]
         spawns = [x for x in (sp, cu["tops"].get("spawn") if cu is not None else None) if x is not None]
         self._yaw_drawn = any("yaw" in x["fields"] and np.any(x["fields"]["yaw"][0] != x["fields"]["yaw"][1]) for x in spawns)
+        rs = self._spec["rs"]
+        # restarts may place robots on rows of their own: "here", or a request's (DESIGN.md §4.18); the heading then varies as with a drawn yaw
+        self._placing = rs is not None and (rs["at"] == "here" or rs["on_request"])
+        self._heading_varies = self._yaw_drawn or (rs is not None and rs["at"] == "here")
+        self._ee_commanded = False; self._place_due = rs is not None and rs["at"] == "here"   # whether the next boundary places robots
         self._scope = None; self._open = False; self._finished = False
 
     # ------------------------------------------------------------------------------------------------------------------------------------ scopes
@@ -1001,6 +1051,21 @@ class Session:
         with torch.cuda.stream(stream):
             self.restore_st = torch.zeros(B, dtype=torch.int32, device=dev)   # a restore's status (ST_RESTORE for an invalid source)
 
+        if self._placing:   # the rows restarts place robots on, counted from the run's start origins, and every episode's spawn row on the device
+            rt = solver.sim_get_robot_terrain(); self.sp_rows = None
+            yaw = xy[:, 2]; yaw = np.where(np.abs(yaw) <= np.pi, yaw, np.remainder(yaw + np.pi, 2.0 * np.pi) - np.pi)
+            start_row = np.zeros((B, _lib.SPAWN)); start_row[:, 0] = -1.0 if rt is None else rt["tile"]; start_row[:, 3] = yaw
+            with torch.cuda.stream(stream):
+                self.sp_origin = f64(np.zeros((B, 2)) if rt is None else rt["origin"]); self.start_row = f64(start_row)
+                self.pl_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev); self.pl_st = torch.zeros_like(contact)
+                self.sp_rec = torch.full((B, _metrics_episodes(ticks, rs), _lib.SPAWN), np.nan, dtype=torch.float64, device=dev)
+                self.pl_any = torch.zeros(1, dtype=torch.int32, device=dev)
+                self._at_default = 1 if rs["at"] == "here" else 0   # each robot's next restart: 0 start (or the spawn's draw), 1 here, 2 a request's row
+                self.at_mode = torch.full((B,), self._at_default, dtype=torch.int32, device=dev)
+                if rs["on_request"]:
+                    self.req = torch.zeros_like(contact); self.req_end = torch.full_like(contact, 2); self.req_rows = torch.zeros_like(self.pl_rows)
+            self._place_link = p["sp"]["link"] if sp is not None else (_lib.SPAWN_GROUND_MAP if o["ground_map"] is True else 0)
+
         if rz is not None or sp is not None or tl is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
             with torch.cuda.stream(stream):
                 self.ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev) if rz is not None else None
@@ -1010,6 +1075,11 @@ class Session:
                     self._begin(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
                 else:
                     self._begin(self.due, self.episode)
+        if self._placing:
+            with torch.cuda.stream(stream):
+                self._record_spawn(self.due, None)
+                if rs["on_request"]:   # the start restored every robot; from here on due holds the robots that restart at the next boundary
+                    self.due.zero_()
 
         with torch.cuda.stream(stream):
             self._mpc_tick(); stream.synchronize()          # QMController::starting: one blocking solve before the loop
@@ -1032,35 +1102,65 @@ class Session:
         solver.mpc_solve_dev(prob, s)
 
     def _respawn(self, k):   # the robots due restart at window boundary k: their episode closes, their level moves, then the library's rows, the loop's, their new plant
-        solver, s, cu, due = self.solver, self._s, self._spec["cu"], self.due
+        solver, s, cu, due, rs = self.solver, self._s, self._spec["cu"], self.due, self._spec["rs"]
         if self._mt or cu is not None:
             self.mt_end.copy_(self.due_fall).neg_().add_(2)   # 1: the fall rule, 2: every
+            if rs["on_request"]:   # a request's end, where the fall rule did not end the episode
+                self.mt_end.copy_(self.mt_end.where(self.due_fall.bool() | ~self.req.bool(), self.req_end))
         if self._mt:
             solver.metrics_close_dev(due, self.mt_end, self.episode, self.mt_acc, self.mt_out, self.acc_st, s)
         if cu is not None:   # reads the row the close just wrote; writes the ranges the draws of _begin() read
             solver.curriculum_update_dev(due, self.mt_end, self.episode, self.mt_out if self._mt else None, self.cu_level, self.acc_st, s)
+        placed = None
+        if self._place_due:   # the rows of the robots placed here, read from the plant before the restore: here, then a request's own rows
+            m = due.bool()
+            here = (m & (self.at_mode == 1)).to(due.dtype); placed = (m & (self.at_mode >= 1)).to(due.dtype)
+            solver.spawn_here_dev(here, self.rbd, self.start[0], self.sp_origin, self.pl_rows, s)
+            if rs["on_request"]:
+                _gather([self.pl_rows], [self.req_rows], m & (self.at_mode == 2))
         solver.robot_image_restore_dev(due, s)
         m = due.bool()
         _gather(self.own + [self.k0], self.start + [k], m)   # their rows return to the start, their clock origin to k
         self.episode.add_(due); self.fall_count.masked_fill_(m, 0)
         if cu is not None:
             self._level_begun(due)
-        self._begin(due, self.episode)
+        self._begin(due, self.episode, placed)
+        if self._placing:
+            self._record_spawn(due, placed)
+            self.at_mode.fill_(self._at_default)
+            self._place_due = rs["at"] == "here"
+            if rs["on_request"]:
+                self.req.zero_()
 
     def _level_begun(self, mask):   # the masked robots begin their episode at their current level
         import torch
         rows = torch.arange(self.B, device=self.device); e = self.episode.long()
         self.ep_level[rows, e] = torch.where(mask.bool(), self.cu_level, self.ep_level[rows, e])
 
-    def _begin(self, mask, idx):   # the masked robots begin episode idx: their plant's draw, then their spawn, then their command timeline
+    def _begin(self, mask, idx, placed=None):   # the masked robots begin episode idx: their plant's draw, then their spawn or place, then their command timeline
         p, solver, s = self._spec, self.solver, self._s
         if p["rz"] is not None:
             self._draw(mask, idx)
         if p["sp"] is not None:   # new ground under them, their start state there
-            solver.spawn_sample_dev(mask, idx, self.sp_rows, self.q, self.v, self.rbd, self.contact, self.x_obs, self.last_ee, self.rbd_est if self._se else None,
+            drawn = mask if placed is None else (mask.bool() & ~placed.bool()).to(mask.dtype)
+            solver.spawn_sample_dev(drawn, idx, self.sp_rows, self.q, self.v, self.rbd, self.contact, self.x_obs, self.last_ee, self.rbd_est if self._se else None,
                                     p["sp"]["link"], s)
+        if placed is not None:   # the placed robots stand on their rows; a rejected row leaves the robot at its restored start and goes into the window's status
+            solver.spawn_place_dev(placed, self.pl_rows, self.sp_origin, self.q, self.v, self.rbd, self.contact, self.x_obs, self.last_ee,
+                                   self.rbd_est if self._se else None, self.pl_st, self._place_link, s)
+            self.acc_st.bitwise_or_(self.pl_st)
         if p["tl"] is not None:
             solver.timeline_sample_dev(mask, idx, self.tl_rows, s)
+
+    def _record_spawn(self, mask, placed):   # the masked robots' new episode's spawn row: placed, drawn, or the start's; NaN where a place was rejected
+        import torch
+        row = self.start_row if self.sp_rows is None else self.sp_rows
+        if placed is not None:
+            ok = placed.bool() & (self.pl_st == 0)
+            row = torch.where(ok[:, None], self.pl_rows, torch.where(placed.bool()[:, None], torch.full_like(row, np.nan), row))
+            self.pl_any.bitwise_or_(ok.any().to(torch.int32))
+        b = torch.arange(self.B, device=self.device); e = self.episode.long()
+        self.sp_rec[b, e] = torch.where(mask.bool()[:, None], row, self.sp_rec[b, e])
 
     def _draw(self, mask, idx):   # the masked robots draw episode idx: the plant rows on the device, then the loop's cmd_vel and push rows from the drawn row
         ep_rows, push = self.ep_rows, self.push
@@ -1167,6 +1267,8 @@ class Session:
                             self.due_fall.copy_(d)
                         if rs["every_ms"] is not None:
                             d |= (k + 1 - self.k0) >= rs["every_ms"]
+                        if rs["on_request"]:
+                            d |= self.req.bool()
                         self.due.copy_(d)
         self._k += n * MPC_PERIOD_MS
         return rec
@@ -1183,8 +1285,9 @@ class Session:
         import torch
         if self._spec["gd"] is None:
             raise ValueError("closed_loop.Session.command: needs the device gait schedule (steer=True, commands or timeline)")
-        if self._yaw_drawn and (ee_goal is not None or ee_cmd_vel is not None):
-            raise ValueError("closed_loop.Session.command: ee_goal / ee_cmd_vel cannot go with a drawn spawn yaw (their world-frame goals assume the robot faces +x)")
+        if self._heading_varies and (ee_goal is not None or ee_cmd_vel is not None):
+            raise ValueError("closed_loop.Session.command: ee_goal / ee_cmd_vel cannot go with a drawn spawn yaw or a restart \"here\" (their world-frame goals "
+                             "assume the robot faces +x)")
         B = getattr(self.solver, "batch", None)
         for name, a, shape in (("mask", mask, (B,)), ("gait", gait, (B,)), ("cmd_vel", cmd_vel, (B, 4)), ("ee_goal", ee_goal, (B, 7)), ("ee_cmd_vel", ee_cmd_vel, (B, 3))):
             if a is not None and tuple(np.shape(a)) != shape:
@@ -1203,6 +1306,57 @@ class Session:
             self.solver.gait_dev_command_dev(m, tmpl, vel, kind, ee, self.cmd_st, self._s)
             self.cmd_acc.bitwise_or_(self.cmd_st)
         self._commanded = True
+        self._ee_commanded |= ee_goal is not None or ee_cmd_vel is not None
+
+    def respawn(self, mask, end=2, at=None):
+        """Restart each robot with mask [B] set at the next window boundary, before its MPC tick, through run's respawn path (DESIGN.md §4.18); needs
+        respawn=dict(..., on_request=True).  end: why its episode ended, 1 (failure) or 2 (ended alive), a scalar or [B]: the metrics row's end and the
+        curriculum's fail / pass (the fall rule's 1 wins where it also restarts the robot).  at: None (the respawn spec's at), "start", "here", or [B, 4]
+        spawn rows (_lib.SPAWN_LAYOUT) counted from the run's start origins; a row the device rejects leaves the robot at its restored start pose and
+        sets _lib.ST_SPAWN in the record of the window the next tick opens.  A later request before the boundary replaces an earlier one; state["due"]
+        shows the merged mask.  mask and rows as command takes them (device tensors, enqueued on self.stream after the caller's current stream, no
+        synchronisation); an end tensor's values are checked on the host.  ValueError, before any write, on wrong shapes or values, without on_request,
+        and for "here" or rows where run refuses at="here"."""
+        import torch
+        rs, B = self._spec["rs"], getattr(self.solver, "batch", None)
+        if rs is None or not rs["on_request"]:
+            raise ValueError("closed_loop.Session.respawn: needs respawn=dict(..., on_request=True)")
+        if tuple(np.shape(mask)) != (B,):
+            raise ValueError("closed_loop.Session.respawn: mask must have shape (%s,), got %s" % (B, tuple(np.shape(mask))))
+        if isinstance(end, (bool, np.bool_)) or tuple(np.shape(end)) not in ((), (B,)):
+            raise ValueError("closed_loop.Session.respawn: end must be 1 or 2, a scalar or [%s], got %r" % (B, end))
+        e = end.detach().cpu().numpy() if isinstance(end, torch.Tensor) else np.asarray(end)
+        if e.dtype.kind not in "iuf" or not np.all(np.isin(e, (1, 2))):
+            raise ValueError("closed_loop.Session.respawn: end must be 1 (failure) or 2 (ended alive), got %r" % (end,))
+        rows = None
+        if at is None:
+            code = 1 if rs["at"] == "here" else 0
+        elif isinstance(at, str):
+            if at not in RESPAWN_AT:
+                raise ValueError("closed_loop.Session.respawn: at must be None, \"start\", \"here\" or [%s, 4] spawn rows, got %r" % (B, at))
+            code = RESPAWN_AT.index(at)
+        else:
+            if tuple(np.shape(at)) != (B, _lib.SPAWN):
+                raise ValueError("closed_loop.Session.respawn: at rows must have shape (%s, %d), got %s" % (B, _lib.SPAWN, tuple(np.shape(at))))
+            code, rows = 2, at
+        if code:
+            why = _here_refusal(False, self._spec["gd"], self._o["curriculum"], self._o["ground_map"])
+            if why is None and self._ee_commanded:
+                why = "ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)"
+            if why is not None:
+                raise ValueError("closed_loop.Session.respawn: a restart \"here\" or on given rows cannot go with %s" % why)
+        if not self._open or self._finished:
+            raise ValueError("closed_loop.Session.respawn: the session is not open (enter it with `with`; finish() ends it)")
+        self._wait_caller()
+        with torch.cuda.stream(self.stream):
+            m = self._put(mask, torch.int32, (B,), 0).bool()
+            self.due.bitwise_or_(m.to(self.due.dtype)); self.req.bitwise_or_(m.to(self.req.dtype))
+            self.req_end.copy_(torch.where(m, torch.as_tensor(np.broadcast_to(e, (B,)).astype(np.int32), device=self.device), self.req_end))
+            self.at_mode.masked_fill_(m, code)
+            if rows is not None:
+                _gather([self.req_rows], [self._put(rows, torch.float64, (B, _lib.SPAWN), 0.0)], m)
+        if code:
+            self._place_due = True; self._heading_varies = True
 
     def _wait_caller(self):   # rows the caller wrote on its own stream are complete before the session's stream reads them
         import torch
@@ -1286,7 +1440,7 @@ class Session:
     def state(self):
         """The live device tensors at the current window boundary (the loop writes them: read, do not write): q, v [B, 24] and rbd [B, 55] (the plant's
         truth), meas (what the controller reads: rbd, or the estimator's rbd_est), x_obs, t_obs, contact, cmd [B, 7] (the target front-end's command),
-        and with respawn episode, fallen and due (the robots that respawn at the next boundary), with curriculum level; None where not running.  clock
+        and with respawn episode, fallen and due (the robots that respawn at the next boundary, requests merged), with curriculum level; None where not running.  clock
         [B]: each robot's episode time in s, computed on self.stream at this call."""
         import torch
         rs, cu = self._spec["rs"], self._spec["cu"]
@@ -1327,6 +1481,8 @@ class Session:
                     out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = rows
             if tl is not None:   # on the episode's clock: exact for drawn times in [t_start / 2, 2 t_start]
                 out["timeline_params"][..., 0] -= self.t_start
+        if self._placing and int(self.pl_any.item()):   # placed rows are not draws: the device record holds every episode's row
+            out["spawn_params"] = self.sp_rec[:, :had.shape[1]].cpu().numpy()
         if self._mt:   # trimmed to the most episodes of any robot
             out.update(episode_metrics=self.mt_out[:, :had.shape[1]].cpu().numpy(), metrics_layout=_lib.METRICS_LAYOUT)
         return out

@@ -1,7 +1,8 @@
 // Per-episode spawns (spawn_kernel.cu; include/qmb200.h: qmb200_spawn_*; DESIGN.md §4.12): the spawn row of one episode of one robot (its tile, its
 // offset along the tile and its yaw), a pure function of (seed, global robot, episode, column) and the robot's ranges.  Host + device: the sampler
 // kernel, qmb200_spawn_draw and tests/spawn_host.cpp compile the same core, so host and device agree bit for bit.  The robot stands on the drawn ground
-// with standing_on_tile (sim_api.cuh), the pose qmb200_sim_standing_state gives.
+// with standing_on_tile (sim_api.cuh), the pose qmb200_sim_standing_state gives.  A restart "here" (DESIGN.md §4.18) writes its row with spawn_here_row
+// and places it after the device check spawn_place_ok; both are host + device too (tests/spawn_place_host.cpp).
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -46,11 +47,46 @@ inline std::string spawn_ranges_error(const double* lo, const double* hi, size_t
   });
 }
 
+// A yaw in [-pi, pi] with the same heading: y itself there; else y - 2 pi floor((y + pi) / (2 pi)), held inside [-pi, pi] against the rounding.  The
+// product is rounded on its own (no fma contraction), so that the kernel and a host build agree bit for bit.  A non-finite y is returned as it is.
+QMB_HD double spawn_wrap_yaw(double y) {
+  const double pi = 3.141592653589793, two_pi = 6.283185307179586;
+  if (fabs(y) <= pi || !isfinite(y)) return y;
+  const double k = floor((y + pi) / two_pi);
+#ifdef __CUDA_ARCH__
+  const double m = __dmul_rn(two_pi, k);
+#else
+  const double m = two_pi * k;
+#endif
+  return fmin(fmax(y - m, -pi), pi);
+}
+
+// The "here" row (qmb200_spawn_here): the spawn row that, once the robot is back at its start pose q_start [NQ], stands it on the ground point under its
+// base now (rbd [QMB200_RBD]) with its heading now.  ter: the plant's robot terrain row now [tile, origin] (NULL: none, the plane); origin [2]: the
+// origin the row's offsets count from (the run's).  The tile stays; the ground moves by the base's travel plus the origin's shift, so the base's
+// point in tile coordinates, x - ter origin, is the same after the place; the yaw is the base's, wrapped.  Without terrain rows only the heading
+// matters to the place; dx, dy then hold the base's travel from its start.
+QMB_HD void spawn_here_row(const double* rbd, const double* q_start, const double* origin, const double* ter, double* row) {
+  const double ox = ter ? ter[1] : origin[0], oy = ter ? ter[2] : origin[1];
+  row[SP_TILE] = ter ? ter[0] : -1.0;
+  row[SP_DX] = (rbd[RBD_POS] - q_start[0]) + (origin[0] - ox);
+  row[SP_DY] = (rbd[RBD_POS + 1] - q_start[1]) + (origin[1] - oy);
+  row[SP_YAW] = spawn_wrap_yaw(rbd[RBD_ZYX]);
+}
+
+// The device check of a row given to qmb200_spawn_place on a library of n_tiles tiles: the tile an integer in [-1, n_tiles), a tile >= 0 only where the
+// plant has robot terrain rows (rows: whether it has), finite dx and dy, the yaw in [-pi, pi].  NaN fails every comparison.
+QMB_HD bool spawn_place_ok(const double* row, int n_tiles, bool rows) {
+  const double pi = 3.141592653589793, t = row[SP_TILE];
+  return floor(t) == t && t >= -1.0 && t < (double)n_tiles && (t < 0.0 || rows) && isfinite(row[SP_DX]) && isfinite(row[SP_DY]) && row[SP_YAW] >= -pi &&
+         row[SP_YAW] <= pi;
+}
+
 #ifdef __CUDACC__
-// What qmb200_spawn_sample_dev reads and writes besides its per-call buffers.  NULL pointers: not written.
+// What qmb200_spawn_sample_dev and qmb200_spawn_place_dev read and write besides their per-call buffers.  NULL pointers: not written.
 struct SpawnArgs {
-  const double *lo, *hi; uint64_t seed; int64_t robot0;   // ranges [B][SP_DBL], seed, global rank of robot 0
-  const double* origin;     // [B][2] the robots' tile origins at the set (the run's), from which the drawn offsets count
+  const double *lo, *hi; uint64_t seed; int64_t robot0;   // the sampler's ranges [B][SP_DBL], seed, global rank of robot 0
+  const double* origin;     // [B][2] the robots' tile origins at the set (the run's), from which the drawn or given offsets count
   const double* qj;         // [NJ] the standing pose's joints (defaultJointState)
   double z_plane, radius, delta0, ground_height;   // the plane pose's base height and delta0 (plane_pose), the contact law's r, the plane
   SimTerrain ter;           // the tile library; ter.robot: the plant's robot terrain rows [B][3] the sampler writes (NULL: none, every robot on the plane)
@@ -62,6 +98,12 @@ struct SpawnArgs {
 // one thread per robot: robots with mask[b] != 0 draw episode[b] as global robot robot0 + b and stand there
 int launch_spawn_sample(const DevModel* mdl, int B, const SpawnArgs& a, const int32_t* mask, const int32_t* episode, double* rows, double* q, double* v, double* rbd,
                         int32_t* contact, double* x_obs, double* last_ee, double* rbd_est, cudaStream_t s);
+// one thread per robot: robots with mask[b] != 0 whose row rows[b] passes spawn_place_ok stand there; status[b] (written) QMB200_ST_SPAWN for a
+// rejected row, else 0
+int launch_spawn_place(const DevModel* mdl, int B, int n_tiles, const SpawnArgs& a, const int32_t* mask, const double* rows, double* q, double* v, double* rbd,
+                       int32_t* contact, double* x_obs, double* last_ee, double* rbd_est, int32_t* status, cudaStream_t s);
+// one thread per robot: robots with mask[b] != 0 write spawn_here_row into rows[b]; ter: the plant's robot terrain rows [B][3] or NULL
+int launch_spawn_here(int B, const int32_t* mask, const double* rbd, const double* q_start, const double* origin, const double* ter, double* rows, cudaStream_t s);
 #endif
 
 }  // namespace qmb

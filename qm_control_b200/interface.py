@@ -812,6 +812,41 @@ class Solver:
         base, rbd_est when given, and the reset rows of the running estimators (float64 / int32 device tensors).  One launch, no synchronisation."""
         self._call("spawn_sample_dev", _p(mask), _p(episode), int(link), _p(rows), _p(q), _p(v), _p(rbd), _p(contact), _p(x_obs), _p(last_ee), _p(rbd_est), stream)
 
+    def spawn_place(self, mask, rows, origin, q, v, rbd, contact, x_obs, last_ee, rbd_est=None, link=0):
+        """Host variant of spawn_place_dev on copies of the arrays → dict(q, v, rbd, contact, x_obs, last_ee[, rbd_est], status [B]); unmasked and rejected
+        robots keep what was given."""
+        B = self.batch
+        out = dict(q=_f64(q, (B, 24)).copy(), v=_f64(v, (B, 24)).copy(), rbd=_f64(rbd, (B, RBD)).copy(), contact=_i32(contact, (B,)).copy(),
+                   x_obs=_f64(x_obs, (B, NX)).copy(), last_ee=_f64(last_ee, (B, 7)).copy())
+        if rbd_est is not None:
+            out["rbd_est"] = _f64(rbd_est, (B, RBD)).copy()
+        out["status"] = np.zeros(B, dtype=np.int32)
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,)); rows = _f64(rows, (B, _lib.SPAWN)); origin = _f64(origin, (B, 2))
+        self._call("spawn_place", _p(mask), _p(rows), _p(origin), int(link), *(_p(out[k]) for k in ("q", "v", "rbd", "contact", "x_obs", "last_ee")),
+                   _p(out.get("rbd_est")), _p(out["status"]))
+        return out
+
+    def spawn_place_dev(self, mask, rows, origin, q, v, rbd, contact, x_obs, last_ee, rbd_est=None, status=None, link=0, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) stands on the given spawn row rows[b] ([B, SPAWN] float64), its offsets counted from
+        origin[b] ([B, 2]), exactly as spawn_sample_dev stands it on a drawn row (same buffers, link and reset rows).  The row is checked on the device;
+        a rejected robot is not written and gets status[b] = _lib.ST_SPAWN (int32 [B] device tensor, written, not OR-ed; 0 elsewhere).  One launch, no
+        synchronisation."""
+        self._call("spawn_place_dev", _p(mask), _p(rows), _p(origin), int(link), _p(q), _p(v), _p(rbd), _p(contact), _p(x_obs), _p(last_ee), _p(rbd_est),
+                   _p(status), stream)
+
+    def spawn_here(self, mask, rbd, q_start, origin, rows=None):
+        """Host variant of spawn_here_dev → rows [B, SPAWN] (rows of unmasked robots as given, zeros by default)."""
+        B = self.batch; rows = np.zeros((B, _lib.SPAWN)) if rows is None else _f64(rows, (B, _lib.SPAWN)).copy()
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,))
+        self._call("spawn_here", _p(mask), _p(_f64(rbd, (B, RBD))), _p(_f64(q_start, (B, 24))), _p(_f64(origin, (B, 2))), _p(rows))
+        return rows
+
+    def spawn_here_dev(self, mask, rbd, q_start, origin, rows, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) writes into rows[b] ([B, SPAWN] float64 device tensor) the spawn row that, once it is
+        back at its start pose q_start[b] ([B, 24]) and placed (spawn_place_dev, same origin [B, 2]), stands it on the ground point under its base in
+        rbd[b] ([B, 55]) with that heading: the plant's robot terrain tile, the offsets, the yaw wrapped into [-pi, pi].  One launch, no synchronisation."""
+        self._call("spawn_here_dev", _p(mask), _p(rbd), _p(q_start), _p(origin), _p(rows), stream)
+
     def spawn_draw(self, robot, episode):
         """Host only: robot [n] (in [0, B)), episode [n] → the spawn rows [n, SPAWN] the sampler draws for them on the stored ranges and seed."""
         return self._ranges_draw("spawn", _lib.SPAWN, robot, episode)

@@ -720,6 +720,84 @@ def respawn_main(args, episode_run_s=5.0):
                       "per_call": respawn_times(solver, xy)}))
 
 
+def place_times(solver, reps=7, calls=20):
+    """Device time per spawn_here_dev + spawn_place_dev of every robot (the rows of a restart "here") and per 1 ms plant step of the whole batch, on
+    robot terrain rows of a stairs tile, alternated `reps` times in blocks of `calls` (CUDA events) → median ms per call of each."""
+    import torch
+    from qm_control_b200 import terrain as T
+    B = solver.batch; dev = torch.device("cuda", 0); s = torch.cuda.Stream(device=dev)
+    solver.sim_set_terrain(np.stack([T.stairs(0.05, 0.3)]), T.CELL); origin = T.centred_origin(np.zeros((B, 2))); solver.sim_set_robot_terrain(np.zeros(B), origin)
+    q0, v0 = solver.sim_standing_state(np.zeros((B, 3)))
+    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+    q, v, q_start, o = f64(q0), f64(v0), f64(q0), f64(origin)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); st = torch.zeros_like(contact); every = torch.ones_like(contact); pst = torch.zeros_like(contact)
+    x_obs = torch.zeros((B, 30), dtype=torch.float64, device=dev); last_ee = f64(solver.initial_ee_target()); rows = torch.zeros((B, 4), dtype=torch.float64, device=dev)
+    solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream); torch.cuda.synchronize(dev)
+
+    def here_place():
+        solver.spawn_here_dev(every, rbd, q_start, o, rows, s.cuda_stream)
+        solver.spawn_place_dev(every, rows, o, q, v, rbd, contact, x_obs, last_ee, None, pst, 0, s.cuda_stream)
+    calls_of = {"here_place_all": here_place, "plant": lambda: solver.sim_step_dev(1e-3, eff, q, v, rbd, contact, st, s.cuda_stream)}
+    times = {k: [] for k in calls_of}
+    try:
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(s)
+                for _ in range(calls):
+                    call()
+                b.record(s); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    finally:
+        solver.sim_set_robot_terrain(None); solver.sim_set_terrain(None)
+    return {"label": "device time per call on %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls), **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}}
+
+
+def at_here_main(args, course_s=6.0):
+    """--respawn --at-here: trot at --vx over a stairs tile with the fall rule (0.1 s fallen), restarts at the start against restarts "here".  The wall
+    time per simulated second of --duration runs of each, alternated twice after one warm-up run of each; a course run of course_s each, the farthest
+    point along the tile (tile x) each robot's base reached; the device time of here + place against a plant step."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop, terrain as T
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch
+    solver = q.Solver(batch=B, device=0)
+    origin = T.centred_origin(np.zeros((B, 2)))
+    ter = dict(tiles=np.stack([T.stairs(0.05, 0.3)]), cell=T.CELL, tile=np.zeros(B), origin=origin)
+    kw = dict(gait=args.gait, cmd_vel=(args.vx, 0.0, 0.0, 0.0), terrain=ter)
+
+    def timed(at, duration):
+        solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+        r = closed_loop.run(solver, duration=duration, **kw, respawn=dict(hold=0.1, at=at))
+        torch.cuda.synchronize(dev)
+        return r, (time.perf_counter() - t0) / duration
+    wall = {"start": [], "here": []}
+    for rep in range(3):   # the first round warms up
+        for at in wall:
+            _, w = timed(at, args.duration)
+            if rep:
+                wall[at].append(w)
+    course = {}
+    for at in wall:
+        r, _ = timed(at, course_s)
+        ep = r["episode"]; sp = r.get("spawn_params")
+        dx = np.zeros(ep.shape) if sp is None else np.take_along_axis(np.nan_to_num(sp[:, :, 1]), ep.T.astype(np.int64), axis=1).T
+        tile_x = r["base"][:, :, 0] - (origin[None, :, 0] - dx)   # the base's x in its tile's frame, window by window
+        reach = tile_x.max(axis=0)
+        course[at] = {"median_m": float(np.median(reach)), "p90_m": float(np.percentile(reach, 90)), "max_m": float(reach.max()),
+                      "restarts_per_robot": float(ep[-1].mean())}
+    name, limit = card()
+    print(json.dumps({"metric": "respawn_at_here", "gpu": name, "power_limit": limit, "batch": B,
+                      "config": "%s at %.2f m/s over a stairs tile (rise 0.05 m, run 0.3 m from 0.35 m), respawn after 0.1 s fallen" % (args.gait, args.vx),
+                      "wall_s_per_sim_s": {"label": "runs of %.1f s, two alternated pairs after a warm-up pair" % args.duration, **wall},
+                      "course": {"simulated_s": course_s, "label": "farthest tile x of the base per robot (m), over the run", **course},
+                      "per_call": place_times(solver)}))
+
+
 def metrics_times(solver, xy_yaw, reps=7, calls=20):
     """Device time per metrics sample (metrics_step_dev), per close of every robot (metrics_close_dev) and per 1 ms plant step of the whole batch,
     alternated `reps` times in blocks of `calls` from one standing state with a cmd_vel target (CUDA events) → median ms per call of each."""
@@ -1202,6 +1280,8 @@ def main():
     ap.add_argument("--respawn", action="store_true", help="restart robots that fell (hold 0.1 s) on the reference IMU noise without the attitude filter: episode rates")
     ap.add_argument("--randomize", action="store_true", help="with --respawn: a new plant per episode (friction, payload, push): falls per friction x push bin")
     ap.add_argument("--spawn", action="store_true", help="with --respawn: new ground per episode (tile, offset, yaw): falls per tile x heading bin")
+    ap.add_argument("--at-here", action="store_true", help="with --respawn: restarts where robots fell against restarts at the start on a stairs tile: "
+                                                            "wall time, distance along the tile, here + place device time")
     ap.add_argument("--metrics", action="store_true", help="per-episode metrics: wall time with and without them, per-call times, column medians of a respawn run")
     ap.add_argument("--timeline", action="store_true", help="with --respawn: a new command timeline per episode (gait switches, cmd_vel steps): sampler time, "
                                                             "wall time, falls and velocity error per transition")
@@ -1230,6 +1310,10 @@ def main():
         ap.error("--randomize needs --respawn")
     if args.spawn and not args.respawn:
         ap.error("--spawn needs --respawn")
+    if args.at_here and not args.respawn:
+        ap.error("--at-here needs --respawn")
+    if args.at_here:
+        return at_here_main(args)
     if args.respawn:
         return respawn_main(args)
     if args.ee_tuning and not args.ee_goals:
