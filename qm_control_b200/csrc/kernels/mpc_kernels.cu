@@ -516,7 +516,7 @@ struct RicSmem {
   double Bm[NX * LDB], PB[NX * LDB];        // B~ ; P'B~, later Y = L^{-1}[G | h] (18 x LDX)
   double G[MU * LDG];                       // G = S~ + B~'W (column 30: h = r~ + B~'(p + P b~))
   double H[MU * LDH];                       // H = R~ + B~'P B~
-  double Lt[MU * MU];                       // Cholesky factor of H, transposed: Lt[c][a] = L[a][c] (strict lower part; pivots live as reciprocals in dut)
+  alignas(16) double Lt[MU * MU];           // Cholesky factor of H, transposed: Lt[c][a] = L[a][c] (strict lower part; pivots live as reciprocals in dut); rows read as 16-byte pairs
   alignas(16) double tail[TAIL_DBL];        // backward sweep: the node's small pieces (Px rows, b~, q~, r~, R~ / S~ entries, index lists)
   double dx[32], dut[32], tmp[32];
   double red[RIC_THREADS / 32][4];
@@ -526,6 +526,15 @@ struct RicSmem {
   unsigned char ntype[RIC_NTYPE];           // node types of the whole horizon, loaded once: the sweep's control flow never waits on a global load
 };
 static_assert(sizeof(RicSmem) <= 57344 - 64, "Riccati kernel must keep four CTAs per SM");
+// QMB_RIC_CTAS (1-4): an occupancy experiment. The launch asks for enough dynamic shared memory that at most that many CTAs fit on an SM (228 KB of shared
+// memory per SM, 1 KB reserved per CTA); the kernel uses sizeof(RicSmem) of it either way.  The default, 4, asks for exactly sizeof(RicSmem).
+#ifndef QMB_RIC_CTAS
+#define QMB_RIC_CTAS 4
+#endif
+static_assert(QMB_RIC_CTAS >= 1 && QMB_RIC_CTAS <= 4, "QMB_RIC_CTAS: 1-4 CTAs per SM");
+constexpr int RIC_SMEM_SM = 233472, RIC_SMEM_MAX = 232448;
+constexpr int RIC_SMEM_LAUNCH = QMB_RIC_CTAS == 4 ? (int)sizeof(RicSmem) : (RIC_SMEM_SM / QMB_RIC_CTAS - 1024 < RIC_SMEM_MAX ? RIC_SMEM_SM / QMB_RIC_CTAS - 1024 : RIC_SMEM_MAX);
+static_assert(RIC_SMEM_LAUNCH >= (int)sizeof(RicSmem) && (QMB_RIC_CTAS + 1) * (RIC_SMEM_LAUNCH + 1024) > RIC_SMEM_SM, "QMB_RIC_CTAS + 1 CTAs must not fit");
 
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(b)), "r"(count) : "memory"); }
@@ -727,9 +736,11 @@ __global__ void __launch_bounds__(RIC_THREADS, 4) mpc_riccati_kernel(const DevMo
     if (warp == sw) {
       if (QMB_TMA) gQ.skip();
       // (a) Cholesky of H with the factor in registers (lane = row, read from the upper triangle: column access is bank-conflict free;
-      //     pivot and column broadcasts by shuffle) fused with the forward substitution Y = L^{-1}[G | h] (lane = column of [G | h]):
+      //     the pivot broadcast by shuffle) fused with the forward substitution Y = L^{-1}[G | h] (lane = column of [G | h]):
       //     the broadcast L[c][j] that updates row c of the factor is exactly the multiplier of the right-looking substitution step,
-      //     so Y costs one more FMA per shuffle and no extra dependent chain.  Lanes >= MU carry zeros in the factor role.
+      //     so Y costs one more FMA per broadcast and no extra dependent chain.  Lanes >= MU carry zeros in the factor role.
+      //     The column broadcast reads row j of Lt, stored in the same step: one 16-byte broadcast load serves two rows c, where a 64-bit
+      //     shuffle costs two SHFL per row plus the moves that pair the halves again.
       double hr[MU], y[MU]; double dinv = 0.0; bool ok = true; double* Yb = sm.PB;   // PB is free after phase 2; Y uses leading dimension LDX
 #pragma unroll
       for (int c = 0; c < MU; ++c) { hr[c] = (lane < MU) ? sm.H[c * LDH + lane] : 0.0; y[c] = sm.G[c * LDG + lane]; }
@@ -740,8 +751,12 @@ __global__ void __launch_bounds__(RIC_THREADS, 4) mpc_riccati_kernel(const DevMo
         if (lane == j) dinv = inv;
         if (lane < MU) sm.Lt[j * MU + lane] = lij;
         y[j] *= inv; Yb[j * LDX + lane] = y[j];
+        __syncwarp();
+        const double* ltj = sm.Lt + j * MU;   // ltj[c] = L[c][j]; row pitch 144 B, so even c is 16-byte aligned
 #pragma unroll
-        for (int c = j + 1; c < MU; ++c) { const double lcj = __shfl_sync(FULL, lij, c); hr[c] = fma(-lij, lcj, hr[c]); y[c] = fma(-lcj, y[j], y[c]); }
+        for (int c = (j + 1) & ~1; c < MU; c += 2) { const double2 l2 = *reinterpret_cast<const double2*>(ltj + c);
+          if (c > j) { hr[c] = fma(-lij, l2.x, hr[c]); y[c] = fma(-l2.x, y[j], y[c]); }
+          hr[c + 1] = fma(-lij, l2.y, hr[c + 1]); y[c + 1] = fma(-l2.y, y[j], y[c + 1]); }
       }
       if (lane < MU) sm.dut[lane] = dinv;
       if (!ok && lane == 0) sm.flag = 1;
@@ -1170,7 +1185,7 @@ int mpc_configure_device() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_rollout_trials_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RO_RPC_MAX * GAIN_DBL * 8);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_lq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LqSmem) * LQ_WARPS));
   if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_lq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(LqSmem) * LQ_WARPS));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_riccati_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RicSmem));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(mpc_riccati_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RIC_SMEM_LAUNCH);
   return (int)e;
 }
 
@@ -1192,7 +1207,7 @@ int mpc_solve_launch(const DevModel* mdl, const DevModel& hm, MpcBuffers& m, con
     if (ev && it == iters - 1) cudaEventRecord(ev[7], stream);
     (p.tuning ? mpc_lq_kernel<true> : mpc_lq_kernel<false>)<<<(unsigned)((nodes + LQ_WARPS - 1) / LQ_WARPS), 32 * LQ_WARPS, sizeof(LqSmem) * LQ_WARPS, stream>>>(mdl, b0, b1, nmax, p, next, m.node_rec, m.stage, m.status);
     if (ev && it == iters - 1) cudaEventRecord(ev[2], stream);
-    mpc_riccati_kernel<<<nb, RIC_THREADS, sizeof(RicSmem), stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.dx, m.du, m.robot, m.status);
+    mpc_riccati_kernel<<<nb, RIC_THREADS, RIC_SMEM_LAUNCH, stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.dx, m.du, m.robot, m.status);
     if (ev && it == iters - 1) cudaEventRecord(ev[3], stream);
     if (ddp) { mpc_rollout_trials_kernel<<<(nb + ro_rpc - 1) / ro_rpc, ro_rpc * tr_pitch, (size_t)ro_rpc * GAIN_DBL * 8, stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.ddp_trial, m.robot, m.status, n_trials, tr_pitch, ro_rpc);   // all step lengths side by side
       mpc_rollout_kernel<<<ro_grid, RO_THREADS, 0, stream>>>(mdl, b0, b1, nmax, p, next, m.stage, m.gains, m.ddp_trial, m.robot, m.status, m.step_info, 2, n_trials, tr_pitch, it); ++launched; }   // decision + in-place rollout of the accepted step
