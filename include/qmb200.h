@@ -355,13 +355,26 @@ int qmb200_target_trajectories_dev(qmb200_handle* h, int32_t kind, const double*
  * the target holds the final knot).  The host variant rejects a kind outside [-1, 2] and stages the target rows in-out; the _dev variant leaves a
  * robot whose kind lies outside [0, 2] untouched.  For QMB200_TARGET_EE_CMD_VEL and _EE_GOAL the base target is the end-effector target minus
  * (0.52, 0.09) in the world frame, as QmTargetTrajectoriesPublisher_node.cpp:152-153, 184-185 compute it: right for a robot facing +x only (the base
- * of a robot turned by yaw is asked to stand 0.52 m world-x behind the hand, not 0.52 m behind it along its own heading). */
+ * of a robot turned by yaw is asked to stand 0.52 m world-x behind the hand, not 0.52 m behind it along its own heading).  A robot whose end-effector
+ * frame is QMB200_EE_FRAME_HEADING (qmb200_set_ee_frame) takes its targets in its heading frame instead; every target call reads the rows. */
 int qmb200_target_trajectories_per_robot(qmb200_handle* h, const int32_t* kind /*[B]*/, const double* cmd /*[B][7]*/, const double* t_obs /*[B]*/, const double* x_obs /*[B][30]*/,
                                          const double* ee_state /*[B][7]*/, double* last_ee_target /*[B][7] in-out*/, int32_t* n_target /*[B] in-out*/,
                                          double* target_times /*[B][KMAX] in-out*/, double* target_states /*[B][KMAX][37] in-out*/);
 int qmb200_target_trajectories_per_robot_dev(qmb200_handle* h, const int32_t* kind, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
                                              double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, void* cuda_stream);
 void qmb200_initial_ee_target(double* last_ee_target7);
+/* Per-robot end-effector frames (DESIGN.md §4.19), read by every target call and by qmb200_spawn_sample(_dev) / qmb200_spawn_place(_dev).
+ * QMB200_EE_FRAME_WORLD: upstream's arithmetic, bit for bit.  QMB200_EE_FRAME_HEADING: the robot's heading frame H of its observed base (x_obs[6:8],
+ * the unwrapped yaw x_obs[9]; origin (x, y, 0), rotation Rz(yaw), z the world's) states its end-effector targets: last_ee_target is the hold in H
+ * (qmb200_initial_ee_target is then the nominal hold at any start pose), a goal (QMB200_TARGET_EE_GOAL) is a pose in H at the publishing call, the
+ * base offset (0.52, 0.09) of the end-effector kinds turns with the yaw, and a spawn leaves the hold as it is.  frame [B] of 0 / 1, or NULL to clear
+ * (every robot in the world frame).  The setter rejects any other value, naming the robot, and writes nothing; it waits for the device.  A per-robot
+ * setting like the tuning rows: robot-state snapshots hold the rows while they are set (block 32). */
+#define QMB200_EE_FRAME_WORLD 0
+#define QMB200_EE_FRAME_HEADING 1
+int qmb200_set_ee_frame(qmb200_handle* h, const int32_t* frame /*[B] or NULL to clear*/);
+/* frame [B] (zeros when none are set, may be NULL), is_set (may be NULL): whether rows are set */
+int qmb200_get_ee_frame(const qmb200_handle* h, int32_t* frame /*[B]*/, int32_t* is_set);
 
 /* SafetyChecker::check + QMController::updateControlLaw (QMController.cpp:159-165,177-190) or, for a handle created with
  * QMB200_WBC_HIERARCHICAL_MPC, QMMpcController::updateControlLaw (:427-445).  joint_cmd entries the reference does not write in a given call
@@ -614,12 +627,13 @@ int qmb200_robot_image_restore_dev(qmb200_handle* h, const int32_t* mask /*[B] d
  *        23-27 the gait schedule's command timeline (t, template, cmd_vel, end-effector kind, end-effector row)
  *        28-31 the MPC's copy of the last solve's mode schedule (event count, event times, modes), which every policy evaluation (qmb200_update,
  *              qmb200_policy_eval) reads until the next solve, and that solve's status
+ *        32 end-effector frame rows (qmb200_set_ee_frame; held while they are set): a robot branched from another takes its frame with its hold
  *      A load may therefore sit anywhere in a loop: before a solve, or between a solve and the updates that evaluate its policy.
  *      It holds no shared settings (tiles, templates, parameters, gains), no draw ranges, curriculum or start image, and no per-call intermediates.  The
  *      buffer is caller-owned device memory of B * qmb200_robot_state_bytes bytes, one block [B][bytes] after the other.  Each block carries the
  *      generation of what owns it, bumped when that is reset, stopped, allocated, re-allocated or cleared: a load refuses a snapshot whose rows no
  *      longer belong to the handle's state. */
-#define QMB200_STATE_BLOCKS 32
+#define QMB200_STATE_BLOCKS 33
 typedef struct qmb200_robot_state_desc {
   int32_t batch;                        /* B of the handle that saved it */
   int32_t n_blocks;                     /* blocks held (set bits of blocks) */

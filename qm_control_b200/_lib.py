@@ -10,6 +10,8 @@ ASSETS = os.path.join(ROOT, "assets")
 NX, NU, RBD, CMD, TARGET, EMAX, KMAX = 30, 30, 55, 54, 37, 32, 4
 GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
 TARGET_CMD_VEL, TARGET_EE_CMD_VEL, TARGET_EE_GOAL = 0, 1, 2   # QMB200_TARGET_*: the target front-end's kinds (-1 in a per-robot kind: a held goal)
+EE_FRAME_WORLD, EE_FRAME_HEADING = 0, 1   # QMB200_EE_FRAME_*: the frame a robot's end-effector targets are stated in (DESIGN.md §4.19)
+ST_OVERFLOW = 0x2      # QMB200_ST_OVERFLOW: a WBC overflow
 ST_COMMAND = 0x20000   # QMB200_ST_COMMAND: a rejected qmb200_gait_dev_command row
 ST_RESTORE = 0x40000   # QMB200_ST_RESTORE: a qmb200_robot_state_load source row outside [0, B)
 ST_SPAWN = 0x80000     # QMB200_ST_SPAWN: a rejected qmb200_spawn_place row
@@ -131,7 +133,7 @@ class CurriculumRule(C.Structure):
 ROBOT_STATE_BLOCKS = ("state_est", "attitude", "slip", "payload_est", "model_payload", "model_srbd", "gait", "gait_cursor", "mpc_n_nodes", "mpc_t", "mpc_event",
                       "mpc_x", "mpc_u", "wbc_input_last", "hw_ring_cmd", "hw_ring_stamp", "hw_ring_state", "gait_pending", "plant_mu", "plant_payload",
                       "robot_terrain", "ground_map", "tuning", "timeline_t", "timeline_tmpl", "timeline_vel", "timeline_ee_kind", "timeline_ee",
-                      "mpc_n_events", "mpc_event_times", "mpc_modes", "mpc_status")
+                      "mpc_n_events", "mpc_event_times", "mpc_modes", "mpc_status", "ee_frame")
 
 
 class RobotStateDesc(C.Structure):
@@ -208,6 +210,8 @@ PROTOTYPES = {
     "qmb200_target_trajectories_per_robot": (I32, [P] * 10),
     "qmb200_target_trajectories_per_robot_dev": (I32, [P] * 11),
     "qmb200_initial_ee_target": (None, [P]),
+    "qmb200_set_ee_frame": (I32, [P] * 2),
+    "qmb200_get_ee_frame": (I32, [P] * 3),
     "qmb200_control_law": (I32, [P] * 10),
     "qmb200_control_law_dev": (I32, [P] * 11),
     "qmb200_set_arm_gains": (I32, [P, D, D]),

@@ -56,7 +56,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
         attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None,
-        timeline=None, curriculum=None):
+        timeline=None, curriculum=None, ee_frame=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -179,14 +179,20 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     after the metrics close and before the restore, so the next episode draws at the new level.  start, up_after and down_after are integers or [B]
     integers, every bound a scalar or [B].  The curriculum is cleared before the previous ranges are restored.  Returns also curriculum_level[ticks, B]
     (each robot's level in that record's window), episode_level[B, E] (-1 where a robot had no episode e), curriculum_state[B, CURRICULUM_STATE] at
-    the end (_lib.CURRICULUM_STATE_LAYOUT), and each attached kind's *_params drawn at its episode's level."""
+    the end (_lib.CURRICULUM_STATE_LAYOUT), and each attached kind's *_params drawn at its episode's level.
+    ee_frame: the frame each robot's end-effector targets are stated in for this run (Solver.set_ee_frame; DESIGN.md §4.19): "world" (the default; no
+    rows are set, upstream's arithmetic), "heading" (every robot) or [B] of 0 (world) / 1 (heading).  A heading-frame robot holds its hand where it is
+    relative to its body while it walks and turns, its ee_goal rows (commands, timeline, Session.command) are poses in its heading frame at the
+    publishing tick (the timeline's ee_x / ee_y / ee_z box is in heading coordinates), and the base offset of its end-effector targets turns with its
+    yaw.  The refusals of end-effector commands beside varying headings (a drawn spawn yaw, a restart "here" or on given rows) then apply to
+    world-frame robots only.  The previous rows are restored when run returns."""
     if isinstance(respawn, dict) and _place_spec(respawn)["on_request"]:
         raise ValueError("closed_loop.run: respawn on_request needs a Session (nothing can request a restart inside run; Session.respawn does)")
     with Session(solver, duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start, torch_device=torch_device,
                  sim_timer=sim_timer, friction_mu=friction_mu, payload=payload, pushes=pushes, model_payload=model_payload, terrain=terrain,
                  payload_estimator=payload_estimator, state_estimator=state_estimator, sensor_noise=sensor_noise, attitude_filter=attitude_filter,
                  slip_detector=slip_detector, ground_map=ground_map, commands=commands, tuning=tuning, respawn=respawn, randomize=randomize, spawn=spawn,
-                 metrics=metrics, timeline=timeline, curriculum=curriculum) as s:
+                 metrics=metrics, timeline=timeline, curriculum=curriculum, ee_frame=ee_frame) as s:
         rec = s.step(s.windows)
         end = s.finish()   # synchronises the session's stream
         out = {k: v if isinstance(v, np.ndarray) else v.cpu().numpy() for k, v in rec.items()}
@@ -196,7 +202,8 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
 
 RUN_DEFAULTS = dict(gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None, friction_mu=None,
                     payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None, attitude_filter=None,
-                    slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None, timeline=None, curriculum=None)
+                    slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None, timeline=None, curriculum=None,
+                    ee_frame=None)
 
 
 def _run_specs(solver, steer, o):
@@ -205,6 +212,8 @@ def _run_specs(solver, steer, o):
     metrics, respawn, randomize, gait, commands, timeline, spawn, curriculum = (o[k] for k in ("metrics", "respawn", "randomize", "gait", "commands", "timeline", "spawn", "curriculum"))
     payload_estimator, state_estimator, sensor_noise, ground_map, terrain = (o[k] for k in ("payload_estimator", "state_estimator", "sensor_noise", "ground_map", "terrain"))
     attitude_filter, slip_detector, model_payload, tuning = (o[k] for k in ("attitude_filter", "slip_detector", "model_payload", "tuning"))
+    ef = _ee_frame_spec(getattr(solver, "batch", None), o["ee_frame"])
+    world = True if ef is None else ef == _lib.EE_FRAME_WORLD   # the robots whose end-effector targets assume they face +x
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else dict(_respawn_spec(respawn), **_place_spec(respawn))
@@ -238,16 +247,16 @@ def _run_specs(solver, steer, o):
     if tl is not None:
         gd = tl["gd"]
     tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
-    sp = None if spawn is None else _spawn_spec(getattr(solver, "batch", None), spawn, terrain, ground_map, gd)
+    sp = None if spawn is None else _spawn_spec(getattr(solver, "batch", None), spawn, terrain, ground_map, gd, world)
     cu = None
     if curriculum is not None:
         cu = _curriculum_spec(getattr(solver, "batch", None), curriculum, rs, metrics is not None, gait, dict(episode=randomize, spawn=spawn, timeline=timeline),
-                              terrain, ground_map, gd)
+                              terrain, ground_map, gd, world)
         if cu["gd"] is not None:   # a top box that weighs end-effector commands needs the placeholder timeline's end-effector rows
             gd = tl["gd"] = cu["gd"]
     if rs is not None and rs["at"] == "here":
         yaw_drawn = sp is not None and "yaw" in sp["fields"] and np.any(sp["fields"]["yaw"][0] != sp["fields"]["yaw"][1])
-        why = _here_refusal(yaw_drawn, gd, curriculum, ground_map)
+        why = _here_refusal(yaw_drawn, gd, curriculum, ground_map, world)
         if why is not None:
             raise ValueError("closed_loop.run: respawn at=\"here\" cannot go with %s" % why)
     if rz is not None:   # the links: a drawn payload / friction also goes where the run told the controller the plant's
@@ -258,7 +267,7 @@ def _run_specs(solver, steer, o):
             rz["link"] |= _lib.EPISODE_MODEL_PAYLOAD
         if tn is not None and "friction_mu" in drawn:
             rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
-    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu)
+    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu, ef=ef, world=world)
 
 
 def _respawn_spec(respawn):
@@ -308,14 +317,15 @@ def _place_spec(respawn):
     return dict(at=spec["at"], on_request=bool(spec["on_request"]))
 
 
-def _here_refusal(sp_yaw_drawn, gd, curriculum, ground_map):
-    """why a restart "here" (or on given spawn rows) cannot go with this run's specs, or None: the heading it keeps varies per robot"""
+def _here_refusal(sp_yaw_drawn, gd, curriculum, ground_map, world=True):
+    """why a restart "here" (or on given spawn rows) cannot go with this run's specs, or None: the heading it keeps varies per robot.  world: True or
+    bool [B], the world-frame robots (end-effector commands to heading-frame robots follow their heading)."""
     if curriculum is not None and "spawn" in curriculum:
         return "a curriculum attached to the spawn (its levels draw every spawn)"
     if sp_yaw_drawn:
         return "a drawn spawn yaw (the heading a restart keeps would not be the draw's)"
-    if gd is not None and gd["ee"]:
-        return "ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)"
+    if gd is not None and np.any(gd["ee_robots"] & world):
+        return "ee_goal / ee_cmd_vel commands to world-frame robots (their world-frame goals assume the robot faces +x)"
     if isinstance(ground_map, dict):
         return "a ground_map dict (the map would not follow the ground; ground_map=True does)"
     return None
@@ -362,9 +372,9 @@ def _randomize_spec(B, randomize):
     return dict(seed=seed, fields=fields, link=0)
 
 
-def _spawn_spec(B, spawn, terrain, ground_map, gd):
+def _spawn_spec(B, spawn, terrain, ground_map, gd, world=True):
     """closed_loop.run's spawn (with its terrain, ground_map and parsed commands) → dict(seed, fields: name -> (lo, hi) float arrays, scalar or [B],
-    link); ValueError when malformed.  B None: the bounds' length is not checked."""
+    link); ValueError when malformed.  B None: the bounds' length is not checked.  world: True or bool [B], the world-frame robots."""
     if not isinstance(spawn, dict):
         raise ValueError("closed_loop.run: spawn must be None or dict(seed=..., tile=(lo, hi), dx=(lo, hi), dy=(lo, hi), yaw=(lo, hi)), got %r" % (spawn,))
     seed, fields = _ranges_spec("spawn", _lib.SPAWN_LAYOUT, B, spawn)
@@ -380,8 +390,9 @@ def _spawn_spec(B, spawn, terrain, ground_map, gd):
     if ground and isinstance(ground_map, dict):
         raise ValueError("closed_loop.run: a ground_map dict cannot go with a spawn that draws %s (the map would not follow the ground; ground_map=True does)"
                          % ", ".join(sorted(ground)))
-    if "yaw" in fields and gd is not None and gd["ee"] and np.any(fields["yaw"][0] != fields["yaw"][1]):
-        raise ValueError("closed_loop.run: a drawn spawn yaw cannot go with ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)")
+    if "yaw" in fields and gd is not None and np.any((fields["yaw"][0] != fields["yaw"][1]) & gd["ee_robots"] & world):
+        raise ValueError("closed_loop.run: a drawn spawn yaw cannot go with ee_goal / ee_cmd_vel commands to world-frame robots (their world-frame goals "
+                         "assume the robot faces +x)")
     return dict(seed=seed, fields=fields, link=_lib.SPAWN_GROUND_MAP if ground_map is True else 0)
 
 
@@ -443,7 +454,9 @@ def _gait_commands(B, gait, commands):
     if np.any(np.isnan(vel).any(-1) != np.isnan(vel).all(-1)) or np.any(np.isinf(vel)):
         raise ValueError("closed_loop.run: each commands cmd_vel row must be finite or all NaN")
     tmpl = np.array([[-1 if n is None else ids[n] for n in row] for row in g], dtype=np.int32).reshape(B, C)
-    return dict(names=names, gait=np.array([ids[n] for n in start], dtype=np.int32), t=t, tmpl=tmpl, cmd_vel=vel, ee=_ee_commands(B, C, commands, vel))
+    ee = _ee_commands(B, C, commands, vel)
+    return dict(names=names, gait=np.array([ids[n] for n in start], dtype=np.int32), t=t, tmpl=tmpl, cmd_vel=vel, ee=ee,
+                ee_robots=(ee["ee_kind"] >= 0).any(-1) if ee else np.zeros(B, dtype=bool))
 
 
 def _ee_commands(B, C, commands, vel):
@@ -534,14 +547,14 @@ def _timeline_spec(B, gait, timeline, commands):
     Bn = len(start)   # the placeholder timeline the sampler writes into: +inf times, no command
     ee = {} if not np.any(weights[..., 2:] > 0.0) else dict(ee_kind=np.full((Bn, n), -1, dtype=np.int32), ee_cmd=np.zeros((Bn, n, 7)))
     gd = dict(names=names, gait=np.array([ids[x] for x in start], dtype=np.int32), t=np.full((Bn, n), np.inf), tmpl=np.full((Bn, n), -1, dtype=np.int32),
-              cmd_vel=np.full((Bn, n, 4), np.nan), ee=ee)
+              cmd_vel=np.full((Bn, n, 4), np.nan), ee=ee, ee_robots=np.any(weights[..., 2:] > 0.0, axis=-1))
     return dict(seed=seed, n=int(n), fields=fields, p_gait=p_gait, gait_set=gait_set, weights=weights, quat=quat, gd=gd)
 
 
 CURRICULUM_KINDS = dict(randomize="episode", spawn="spawn", timeline="timeline")   # a curriculum spec's key → the draw kind it attaches to
 
 
-def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map, gd):
+def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map, gd, world=True):
     """closed_loop.run's curriculum (with the run's respawn spec rs, whether metrics is on, its gait, base: the run's own randomize / spawn / timeline
     specs by kind, terrain, ground_map and parsed commands) → dict(levels, start, up_after, down_after (int arrays, scalar or [B]), conditions [(column,
     op, role)], thresholds [float arrays, scalar or [B]], tops: kind -> the parsed spec of its top box, gd: the placeholder timeline when the top box
@@ -599,7 +612,7 @@ def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map
         if key == "randomize":
             tops[kind] = _randomize_spec(B, spec)
         elif key == "spawn":
-            tops[kind] = _spawn_spec(B, spec, terrain, ground_map, top_gd or gd)
+            tops[kind] = _spawn_spec(B, spec, terrain, ground_map, top_gd or gd, world)
         else:
             b, t = _timeline_spec(B, gait, base[kind], None), _timeline_spec(B, gait, spec, None)
             for name, k in (("gaits (gait_set)", "gait_set"), ("ee_quat", "quat")):
@@ -610,7 +623,7 @@ def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map
     if not tops:
         raise ValueError("closed_loop.run: curriculum needs at least one of %s (the boxes its level moves)" % ", ".join(CURRICULUM_KINDS))
     if top_gd is not None and base["spawn"] is not None:   # the run's own spawn, checked against the timeline its top box needs
-        _spawn_spec(B, base["spawn"], terrain, ground_map, top_gd)
+        _spawn_spec(B, base["spawn"], terrain, ground_map, top_gd, world)
     return dict(levels=int(levels), start=start, up_after=up, down_after=down, conditions=conditions, thresholds=thresholds, tops=tops, gd=top_gd)
 
 
@@ -701,6 +714,34 @@ def _robot_tuning(solver, spec, friction_mu):
         yield
     finally:
         solver.set_robot_tuning(prev)
+
+
+EE_FRAMES = ("world", "heading")   # closed_loop.run's ee_frame names, in _lib.EE_FRAME_* order
+
+
+def _ee_frame_spec(B, ee_frame):
+    """closed_loop.run's ee_frame → None ("world", the default: no rows are set) or int32 [B] rows for Solver.set_ee_frame; ValueError when malformed.
+    B None: the rows' length is not checked."""
+    if ee_frame is None or (isinstance(ee_frame, str) and ee_frame == "world"):
+        return None
+    if isinstance(ee_frame, str):
+        if ee_frame not in EE_FRAMES:
+            raise ValueError("closed_loop.run: ee_frame must be \"world\", \"heading\" or [B] of 0 (world) / 1 (heading), got %r" % (ee_frame,))
+        return np.full(1 if B is None else B, _lib.EE_FRAME_HEADING, dtype=np.int32)
+    a = np.asarray(ee_frame)
+    if a.ndim != 1 or (B is not None and a.shape != (B,)) or a.dtype.kind not in "iub" or not np.all((a == 0) | (a == 1)):
+        raise ValueError("closed_loop.run: ee_frame must be \"world\", \"heading\" or [%s] of 0 (world) / 1 (heading), got %r" % ("B" if B is None else B, ee_frame))
+    return a.astype(np.int32)
+
+
+@contextlib.contextmanager
+def _ee_frame(solver, rows):
+    prev = solver.get_ee_frame()
+    try:
+        solver.set_ee_frame(rows)
+        yield
+    finally:
+        solver.set_ee_frame(prev)
 
 
 @contextlib.contextmanager
@@ -855,6 +896,8 @@ class Session:
                 scope.enter_context(_model_payload(solver, o["model_payload"], o["payload"]))
             if tn is not None:
                 scope.enter_context(_robot_tuning(solver, tn, o["friction_mu"]))
+            if p["ef"] is not None:
+                scope.enter_context(_ee_frame(solver, p["ef"]))
             if o["payload_estimator"] is not None:
                 scope.enter_context(_payload_estimator(solver, o["payload_estimator"]))
             if o["state_estimator"] is not None:
@@ -1285,13 +1328,14 @@ class Session:
         import torch
         if self._spec["gd"] is None:
             raise ValueError("closed_loop.Session.command: needs the device gait schedule (steer=True, commands or timeline)")
-        if self._heading_varies and (ee_goal is not None or ee_cmd_vel is not None):
-            raise ValueError("closed_loop.Session.command: ee_goal / ee_cmd_vel cannot go with a drawn spawn yaw or a restart \"here\" (their world-frame goals "
-                             "assume the robot faces +x)")
         B = getattr(self.solver, "batch", None)
         for name, a, shape in (("mask", mask, (B,)), ("gait", gait, (B,)), ("cmd_vel", cmd_vel, (B, 4)), ("ee_goal", ee_goal, (B, 7)), ("ee_cmd_vel", ee_cmd_vel, (B, 3))):
             if a is not None and tuple(np.shape(a)) != shape:
                 raise ValueError("closed_loop.Session.command: %s must have shape %s, got %s" % (name, shape, tuple(np.shape(a))))
+        ee_world = self._ee_to_world(mask, ee_goal is not None or ee_cmd_vel is not None)
+        if self._heading_varies and ee_world:
+            raise ValueError("closed_loop.Session.command: ee_goal / ee_cmd_vel to world-frame robots cannot go with a drawn spawn yaw or a restart \"here\" "
+                             "(their world-frame goals assume the robot faces +x)")
         if not self._open or self._finished:
             raise ValueError("closed_loop.Session.command: the session is not open (enter it with `with`; finish() ends it)")
         self._wait_caller()
@@ -1306,7 +1350,7 @@ class Session:
             self.solver.gait_dev_command_dev(m, tmpl, vel, kind, ee, self.cmd_st, self._s)
             self.cmd_acc.bitwise_or_(self.cmd_st)
         self._commanded = True
-        self._ee_commanded |= ee_goal is not None or ee_cmd_vel is not None
+        self._ee_commanded |= ee_world
 
     def respawn(self, mask, end=2, at=None):
         """Restart each robot with mask [B] set at the next window boundary, before its MPC tick, through run's respawn path (DESIGN.md §4.18); needs
@@ -1340,9 +1384,9 @@ class Session:
                 raise ValueError("closed_loop.Session.respawn: at rows must have shape (%s, %d), got %s" % (B, _lib.SPAWN, tuple(np.shape(at))))
             code, rows = 2, at
         if code:
-            why = _here_refusal(False, self._spec["gd"], self._o["curriculum"], self._o["ground_map"])
+            why = _here_refusal(False, self._spec["gd"], self._o["curriculum"], self._o["ground_map"], self._spec["world"])
             if why is None and self._ee_commanded:
-                why = "ee_goal / ee_cmd_vel commands (their world-frame goals assume the robot faces +x)"
+                why = "ee_goal / ee_cmd_vel commands to world-frame robots (their world-frame goals assume the robot faces +x)"
             if why is not None:
                 raise ValueError("closed_loop.Session.respawn: a restart \"here\" or on given rows cannot go with %s" % why)
         if not self._open or self._finished:
@@ -1357,6 +1401,15 @@ class Session:
                 _gather([self.req_rows], [self._put(rows, torch.float64, (B, _lib.SPAWN), 0.0)], m)
         if code:
             self._place_due = True; self._heading_varies = True
+
+    def _ee_to_world(self, mask, ee):
+        """whether a command with end-effector rows (ee) to the robots of mask [B] reaches a world-frame robot: any masked one (read on the host)
+        when the session sets frame rows, every command with end-effector rows when it does not"""
+        world = self._spec["world"]
+        if not ee or world is True:
+            return ee
+        m = mask.detach().cpu().numpy() if hasattr(mask, "detach") else np.asarray(mask)
+        return bool(np.any((m != 0) & world))
 
     def _wait_caller(self):   # rows the caller wrote on its own stream are complete before the session's stream reads them
         import torch

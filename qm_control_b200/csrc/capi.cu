@@ -85,6 +85,11 @@ struct qmb200_handle {
   struct { std::vector<double> host; double* d = nullptr; int n_tiles = 0, nx = 0, ny = 0; double cell = 0.0; } tiles;   // heightfield library (qmb200_sim_set_terrain)
   RobotArray mpayload{8}, srbd{SRBD_DBL};   // the controller's model payload (qmb200_set_model_payload) and the robots' SRBD constants it gives
   RobotArray tuning{TUNING_DBL};            // per-robot controller parameters (qmb200_set_robot_tuning): Tuning, then the control law's arm kp / kd
+  struct {   // per-robot end-effector frames (qmb200_set_ee_frame): host copy (empty = not set), device copy, generation as RobotArray's; on_device: a
+             // restore wrote the device rows, the getter refreshes the host copy
+    std::vector<int32_t> host; int32_t* d = nullptr; uint64_t gen = 0; bool on_device = false;
+    const int32_t* dev() const { return host.empty() ? nullptr : d; }
+  } ee_frame;
   qmb200_payload_est_params est_prm{}; FilterState est{EST_DBL, "payload estimator", "qmb200_payload_est_reset"};   // payload estimator (capi_est.inc)
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
   qmb200_state_est_params se_prm{}; FilterState se{SE_DBL, "state estimator", "qmb200_state_est_reset"};   // base state estimator

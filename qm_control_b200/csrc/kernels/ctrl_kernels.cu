@@ -34,13 +34,6 @@ __device__ __forceinline__ double shortest_angular_distance(double from, double 
   return a;
 }
 
-// Eigen::Quaterniond(w, x, y, z).toRotationMatrix()
-__device__ __forceinline__ void quat_to_rot(double w, double x, double y, double z, double* R) {
-  const double tx = 2.0 * x, ty = 2.0 * y, tz = 2.0 * z, twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
-  R[0] = 1.0 - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
-  R[3] = txy + twz; R[4] = 1.0 - (txx + tzz); R[5] = tyz - twx;
-  R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1.0 - (txx + tyy);
-}
 }  // namespace
 
 // -----------------------------------------------------------------------------------------------------------------
@@ -67,55 +60,16 @@ __global__ void __launch_bounds__(OBS_ROBOTS) ctrl_observation_kernel(const DevM
 // -----------------------------------------------------------------------------------------------------------------
 // Target front-end.  kind 0: /cmd_vel (cmd = vx, vy, vz, yaw rate), 1: /ee_cmd_vel (cmd = vx, vy, vz), 2: goal pose (cmd = pos(3), quat xyzw(4)).
 // kinds [B] (or NULL: every robot `kind`): robot b's kind; a robot whose kind lies outside [0, 2] (-1: its goal is held) is left untouched.
+// frame [B] (or NULL: every robot in the world frame): robot b's end-effector frame, EE_FRAME_WORLD or EE_FRAME_HEADING (target_robot).
 // Output: the 2-knot TargetTrajectories [time; 37-dim state = (0_6 | v, base pose, defaultJointState, EE pose)] in the solver's layout.
 __global__ void __launch_bounds__(128) ctrl_target_kernel(TargetParams prm, int kind_all, const int32_t* __restrict__ kinds, int B, const double* __restrict__ cmd /*[B][7]*/,
                                                            const double* __restrict__ t_obs, const double* __restrict__ x_obs, const double* __restrict__ ee_state /*[B][7]*/,
                                                            double* __restrict__ last_ee_target /*[B][7]*/, int32_t* __restrict__ n_target, double* __restrict__ target_times /*[B][KMAX]*/,
-                                                           double* __restrict__ target_states /*[B][KMAX][37]*/) {
+                                                           double* __restrict__ target_states /*[B][KMAX][37]*/, const int32_t* __restrict__ frame) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x; if (b >= B) return;
   const int kind = kinds ? kinds[b] : kind_all; if (kind < 0 || kind > 2) return;
-  const double* c = cmd + (size_t)b * 7; const double* x = x_obs + (size_t)b * NX; const double* ee = ee_state + (size_t)b * 7; double* le = last_ee_target + (size_t)b * 7;
-  const double t = t_obs[b];
-  double base_cur[6]; for (int i = 0; i < 6; ++i) base_cur[i] = x[6 + i];
-  double base_tgt[6], ee_cur[7], ee_tgt[7], vel[3] = {0.0, 0.0, 0.0}, t_reach;
-  if (kind == 0) {            // cmdVelToTargetTrajectories (:73-113)
-    double R[9]; rot_zyx(base_cur[3], base_cur[4], base_cur[5], R); matvec3(R, c, vel);
-    base_tgt[0] = base_cur[0] + vel[0] * prm.time_to_target; base_tgt[1] = base_cur[1] + vel[1] * prm.time_to_target; base_tgt[2] = prm.com_height;
-    base_tgt[3] = base_cur[3] + c[3] * prm.time_to_target; base_tgt[4] = 0.0; base_tgt[5] = 0.0;
-    const double d0 = le[0] - ee[0], d1 = le[1] - ee[1], d2 = le[2] - ee[2];
-    if (sqrt(d0 * d0 + d1 * d1 + d2 * d2) > 0.1) { le[0] = ee[0]; le[1] = ee[1]; le[2] = ee[2]; }
-    for (int i = 0; i < 7; ++i) { ee_tgt[i] = le[i]; ee_cur[i] = le[i]; }   // eeStateLast.state = EeTargetPose (:104-105)
-    t_reach = t + prm.time_to_target;
-  } else if (kind == 1) {     // EeCmdVelToTargetTrajectories (:118-165)
-    double Rq[9], Ri[9], M[9]; quat_to_rot(ee[6], ee[3], ee[4], ee[5], Rq); quat_to_rot(-0.5, 0.5, -0.5, 0.5, Ri); matmul3_nt(Rq, Ri, M);
-    double v[3]; matvec3(M, c, v);
-    for (int i = 0; i < 7; ++i) ee_cur[i] = ee[i];
-    ee_tgt[0] = ee[0] + v[0] * prm.time_to_target; ee_tgt[1] = ee[1] + v[1] * prm.time_to_target; for (int i = 2; i < 7; ++i) ee_tgt[i] = le[i];
-    for (int i = 0; i < 6; ++i) base_tgt[i] = base_cur[i];
-    base_tgt[0] = ee_tgt[0] - 0.52; base_tgt[1] = ee_tgt[1] - 0.09; base_tgt[2] = prm.com_height; base_tgt[4] = 0.0; base_tgt[5] = 0.0;
-    t_reach = t + prm.time_to_target;
-  } else {                    // EEgoalPoseToTargetTrajectories (:172-208) + processFeedback's lastEeTarget_ update
-    for (int i = 0; i < 7; ++i) { ee_cur[i] = ee[i]; ee_tgt[i] = c[i]; }
-    for (int i = 0; i < 6; ++i) base_tgt[i] = base_cur[i];
-    base_tgt[0] = c[0] - 0.52; base_tgt[1] = c[1] - 0.09; base_tgt[2] = prm.com_height; base_tgt[4] = 0.0; base_tgt[5] = 0.0;
-    // quaternionDistance(q_current, q_target) = w_c v_t - w_t v_c + v_c x v_t [upstream ocs2_robotic_tools, recalled]
-    const double wc = ee[6], wt = c[6]; const double vc[3] = {ee[3], ee[4], ee[5]}, vt[3] = {c[3], c[4], c[5]}; double cr[3]; cross3(vc, vt, cr);
-    double dl = 0.0, dr = 0.0;
-    for (int i = 0; i < 3; ++i) { const double dp = c[i] - ee[i], dq = wc * vt[i] - wt * vc[i] + cr[i]; dl += dp * dp; dr += dq * dq; }
-    t_reach = t + fmax(sqrt(dr) / prm.target_rotation_velocity, sqrt(dl) / prm.target_displacement_velocity);   // estimateTimeToTarget (:24-41)
-    for (int i = 0; i < 7; ++i) le[i] = c[i];
-  }
-  base_cur[2] = prm.com_height; base_cur[4] = 0.0; base_cur[5] = 0.0;   // targetPoseToTargetTrajectories (:44-68)
-  double* tt = target_times + (size_t)b * KMAX; double* ts = target_states + (size_t)b * KMAX * TARGET_DIM;
-  n_target[b] = 2; tt[0] = t; tt[1] = t_reach; for (int k = 2; k < KMAX; ++k) tt[k] = 0.0;
-  for (int k = 0; k < 2; ++k) {
-    double* s = ts + k * TARGET_DIM;
-    for (int i = 0; i < 3; ++i) { s[i] = vel[i]; s[3 + i] = 0.0; }
-    for (int i = 0; i < 6; ++i) s[6 + i] = k == 0 ? base_cur[i] : base_tgt[i];
-    for (int j = 0; j < NJ; ++j) s[12 + j] = prm.default_joint_state[j];
-    for (int i = 0; i < 7; ++i) s[30 + i] = k == 0 ? ee_cur[i] : ee_tgt[i];
-  }
-  for (int i = 2 * TARGET_DIM; i < KMAX * TARGET_DIM; ++i) ts[i] = 0.0;
+  target_robot(prm, kind, frame && frame[b] == EE_FRAME_HEADING, cmd + (size_t)b * 7, t_obs[b], x_obs + (size_t)b * NX, ee_state + (size_t)b * 7,
+               last_ee_target + (size_t)b * 7, n_target + b, target_times + (size_t)b * KMAX, target_states + (size_t)b * KMAX * TARGET_DIM);
 }
 
 // -----------------------------------------------------------------------------------------------------------------
@@ -188,8 +142,8 @@ int launch_observation(const DevModel* mdl, int B, const double* rbd, const doub
   ctrl_observation_kernel<<<(B + OBS_ROBOTS - 1) / OBS_ROBOTS, OBS_ROBOTS, 0, s>>>(mdl, B, rbd, period, t_obs, x_obs, srbd); return 1;
 }
 int launch_target(const TargetParams& prm, int kind, const int32_t* kinds, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
-                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s) {
-  ctrl_target_kernel<<<(B + 127) / 128, 128, 0, s>>>(prm, kind, kinds, B, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states); return 1;
+                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s, const int32_t* frame) {
+  ctrl_target_kernel<<<(B + 127) / 128, 128, 0, s>>>(prm, kind, kinds, B, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, frame); return 1;
 }
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,
                        double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s, const double* tuning) {

@@ -12,7 +12,7 @@ namespace qmb {
 // One block of per-robot rows [B][words] of 4-byte words, written for every masked robot: from src [B][words] (an image or a snapshot), or zeros when
 // src is NULL.
 struct RestoreSeg { uint32_t* dst; const uint32_t* src; int32_t words; };
-constexpr int RESTORE_MAX_SEGS = 32;   // a snapshot with every component running holds 32 blocks; the start image 8 imaged and 5 cold-start blocks
+constexpr int RESTORE_MAX_SEGS = 40;   // a snapshot with every component running holds 33 blocks; the start image 8 imaged and 5 cold-start blocks
 struct RestoreTable { RestoreSeg seg[RESTORE_MAX_SEGS]; int n; };
 
 // The gather rule, one word at a time (the kernel's body; tests/restore_host.cpp builds it with g++).  Robot b is written when mask[b] != 0 (NULL mask:

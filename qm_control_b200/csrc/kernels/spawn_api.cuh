@@ -82,6 +82,16 @@ QMB_HD bool spawn_place_ok(const double* row, int n_tiles, bool rows) {
          row[SP_YAW] <= pi;
 }
 
+// The held end-effector target e [7] of a robot the spawn turns from yaw0 to yaw about the vertical through its base (x, y): a world-frame hold turns
+// with the base; a heading-frame hold (heading: qmb200_set_ee_frame, DESIGN.md §4.19) is stated in the base's frame already and stays as it is.
+QMB_HD void spawn_turn_hold(double* e, double x, double y, double yaw0, double yaw, bool heading) {
+  if (yaw == yaw0 || heading) return;
+  const double dyaw = yaw - yaw0; double sn, c, sh, ch; spawn_sincos(dyaw, sn, c); spawn_sincos(0.5 * dyaw, sh, ch);
+  const double ex = e[0] - x, ey = e[1] - y, qx = e[3], qy = e[4], qz = e[5], qw = e[6];
+  e[0] = x + (c * ex - sn * ey); e[1] = y + (sn * ex + c * ey);
+  e[3] = ch * qx - sh * qy; e[4] = ch * qy + sh * qx; e[5] = ch * qz + sh * qw; e[6] = ch * qw - sh * qz;   // Rz(dyaw) quaternion times e's
+}
+
 #ifdef __CUDACC__
 // What qmb200_spawn_sample_dev and qmb200_spawn_place_dev read and write besides their per-call buffers.  NULL pointers: not written.
 struct SpawnArgs {
@@ -94,6 +104,7 @@ struct SpawnArgs {
   double* se; qmb200_state_est_params se_prm;   // state estimator [B][SE_DBL] and the parameters of its reset row
   double* at; qmb200_attitude_params at_prm;    // attitude filter [B][AT_DBL] and the parameters of its reset row
   double* sl;                    // slip detector [B][SL_DBL]
+  const int32_t* frame;          // [B] the robots' end-effector frames (qmb200_set_ee_frame), NULL: every robot in the world frame
 };
 // one thread per robot: robots with mask[b] != 0 draw episode[b] as global robot robot0 + b and stand there
 int launch_spawn_sample(const DevModel* mdl, int B, const SpawnArgs& a, const int32_t* mask, const int32_t* episode, double* rows, double* q, double* v, double* rbd,

@@ -5,9 +5,11 @@
 //   spawn_here_kernel     one thread per robot: a masked robot writes the row that stands it, from its start pose, where it is now (spawn_here_row).
 //   spawn_stand           moves the robot's tile under it (the plant's robot terrain row and, linked, the estimator's ground map), stands it on that ground
 //                         (standing_on_tile, or the plane pose), and writes the state every consumer starts from: q, v = 0, the measured state rbd with
-//                         the end-effector pose, the contact flags, the controller's observation, its held end-effector target turned with the base, and
-//                         the reset rows of the estimators that run.  Unmasked robots are not written by any of the kernels.
+//                         the end-effector pose, the contact flags, the controller's observation, its held end-effector target turned with the base (a
+//                         world-frame hold; a heading-frame hold turns with the base as it is), and the reset rows of the estimators that run.  Unmasked
+//                         robots are not written by any of the kernels.
 #include "spawn_api.cuh"
+#include "ctrl_api.cuh"
 #include "state_est_api.cuh"
 #include "attitude_api.cuh"
 #include "slip_api.cuh"
@@ -62,13 +64,7 @@ __device__ __forceinline__ void spawn_stand(const DevModel& d, const SpawnArgs& 
   for (int j = 0; j < NJ; ++j) xo[12 + j] = a.qj[j];
   if (rbd_est) for (int i = 0; i < QMB200_RBD; ++i) rbd_est[(size_t)b * QMB200_RBD + i] = s[i];
 
-  // the held end-effector target turns with the base about the vertical through it
-  if (yaw != yaw0) {
-    double* e = last_ee + (size_t)b * 7; const double dyaw = yaw - yaw0; double sn, c, sh, ch; spawn_sincos(dyaw, sn, c); spawn_sincos(0.5 * dyaw, sh, ch);
-    const double ex = e[0] - x, ey = e[1] - y, qx = e[3], qy = e[4], qz = e[5], qw = e[6];
-    e[0] = x + (c * ex - sn * ey); e[1] = y + (sn * ex + c * ey);
-    e[3] = ch * qx - sh * qy; e[4] = ch * qy + sh * qx; e[5] = ch * qz + sh * qw; e[6] = ch * qw - sh * qz;   // Rz(dyaw) quaternion times e's
-  }
+  spawn_turn_hold(last_ee + (size_t)b * 7, x, y, yaw0, yaw, a.frame && a.frame[b] == EE_FRAME_HEADING);
 
   // the reset rows: the state estimator at the new base position with no call yet (its next call places the feet), the attitude filter, the detector
   if (a.se) state_est_reset_row(a.se_prm, base, a.se + (size_t)b * SE_DBL);   // base[0..2]: the base position

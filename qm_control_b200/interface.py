@@ -274,6 +274,19 @@ class Solver:
     def initial_ee_target(self):
         v = np.zeros(7); self.lib.qmb200_initial_ee_target(_p(v)); return np.tile(v, (self.batch, 1))
 
+    def set_ee_frame(self, frame=None):
+        """Per-robot end-effector frames (DESIGN.md §4.19): frame [B] of _lib.EE_FRAME_WORLD (0) / _lib.EE_FRAME_HEADING (1), or a scalar for every robot;
+        None clears them (every robot in the world frame).  A heading-frame robot's held end-effector target, goals and base offset are stated in its
+        heading frame.  The library rejects other values.  Synchronous."""
+        rows = None if frame is None else _i32(np.broadcast_to(np.asarray(frame), (self.batch,)), (self.batch,))
+        self._call("set_ee_frame", _p(rows))
+
+    def get_ee_frame(self):
+        """→ the frame rows [B] (int32), or None when none are set."""
+        rows = np.zeros(self.batch, dtype=np.int32); is_set = C.c_int32()
+        self._call("get_ee_frame", _p(rows), C.byref(is_set))
+        return rows if is_set.value else None
+
     def set_arm_gains(self, kp, kd):
         self._call("set_arm_gains", float(kp), float(kd))
 

@@ -384,6 +384,49 @@ def target_call_times(solver, reps=7, calls=50):
             **{"ms_per_call_" + k: float(np.median(v)) for k, v in times.items()}, "spread_per_robot": [float(min(times["per_robot"])), float(max(times["per_robot"]))]}
 
 
+def ee_frame_main(args, sweep_s=4.0):
+    """End-effector targets in the heading frame (DESIGN.md §4.19): the target call of the whole batch (kinds 0 / 1 / 2 / -1 mixed) with no frame rows,
+    all-world rows and all-heading rows, alternated blocks of CUDA events, medians; then the turning sweep (start yaws over [-pi, pi], yaw rates
+    +-0.5 / +-1 rad/s, trot 0.3 m/s, sweep_s s) in both frames: fallen robots and QMB200_ST_OVERFLOW per frame and yaw rate."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: this benchmark measures the GPU and has no CPU fallback")
+    B = args.batch; solver = q.Solver(batch=B, device=0); dev = torch.device("cuda", 0); st = torch.cuda.Stream(device=dev); rng = np.random.default_rng(0)
+    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+    cmd = np.zeros((B, 7)); cmd[:, :3] = [0.6, 0.1, 0.45]; cmd[:, 3:] = [0.5, -0.5, 0.5, -0.5]
+    x = np.zeros((B, 30)); x[:, 8] = 0.45; x[:, 9] = rng.uniform(-np.pi, np.pi, B); ee = np.tile([0.52, 0.09, 0.44, 0.5, -0.5, 0.5, -0.5], (B, 1))
+    rows = [f64(cmd), f64(np.full(B, 10.0)), f64(x), f64(ee), f64(ee), torch.zeros(B, dtype=torch.int32, device=dev), torch.zeros((B, 4), dtype=torch.float64, device=dev),
+            torch.zeros((B, 4, 37), dtype=torch.float64, device=dev)]
+    kind = torch.as_tensor(rng.integers(-1, 3, B).astype(np.int32), device=dev)
+    settings = {"no_rows": None, "world_rows": np.zeros(B, dtype=np.int32), "heading_rows": np.ones(B, dtype=np.int32)}
+    times = {k: [] for k in settings}; reps, calls = 7, 50
+    for rep in range(reps + 1):   # the first round warms up
+        for name, frame in settings.items():
+            solver.set_ee_frame(frame); torch.cuda.synchronize(dev)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(st)
+            for _ in range(calls):
+                solver.target_trajectories_dev(kind, *rows, st.cuda_stream)
+            b.record(st); torch.cuda.synchronize(dev)
+            if rep:
+                times[name].append(a.elapsed_time(b) / calls)
+    solver.set_ee_frame(None)
+    out = {"card": card(), "target_call": {"label": "device ms per target call of %d robots (kinds mixed), median of %d alternated blocks of %d calls" % (B, reps, calls),
+                                           **{k: float(np.median(v)) for k, v in times.items()}}}
+    rates = np.array([-1.0, -0.5, 0.5, 1.0])[np.arange(B) % 4]
+    xy = np.c_[np.arange(B) * 3.0, np.zeros(B), -np.pi + 2 * np.pi * np.arange(B) / B]
+    cmd_vel = np.c_[np.full(B, 0.3), np.zeros(B), np.zeros(B), rates]
+    for frame in ("world", "heading"):
+        solver.mpc_reset(); solver.wbc_set_input_last(None)
+        r = closed_loop.run(solver, duration=sweep_s, gait="trot", cmd_vel=cmd_vel, xy_yaw=xy, ee_frame=frame)
+        base = r["base"]; up = np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3)
+        stw = np.bitwise_or.reduce(r["status"], axis=0); ovf = (stw & _lib.ST_OVERFLOW) != 0
+        out["turning_" + frame] = {str(w): {"robots": int(np.sum(rates == w)), "fallen": int(np.sum(~up & (rates == w))), "overflow": int(np.sum(ovf & (rates == w)))}
+                                   for w in (-1.0, -0.5, 0.5, 1.0)}
+    print(json.dumps(out))
+
+
 def ee_goals(solver, closed_loop, B, sim_s, xy, upright, tuning=False):
     """The reach sweep, the target call times, then the runs of sim_s with the goals and with a timeline that changes nothing (wall time).  With tuning
     also the reach sweep again under per-robot tuning rows (ee_tuning_sweep)."""
@@ -667,7 +710,7 @@ def spawn_main(args, solver, kw, xy, timed, episode_run_s=5.0):
         kw["xy_yaw"] = kw_xy
     E = int(rc["episode"].max()) + 1; Pc = np.zeros((solver.batch, E, _lib.SPAWN)); Pc[:, :, 3] = yaw[:, None]
     name, limit = card()
-    print(json.dumps({"metric": "spawn", "gpu": name, "power_limit": limit, "batch": solver.batch,
+    print(json.dumps({"metric": "spawn", "gpu": name, "power_limit": limit, "batch": solver.batch, "ee_frame": kw.get("ee_frame", "world"),
                       "config": "%s at %.2f m/s on the state estimate with the ground map, reference IMU noise, no attitude filter; respawn after 0.1 s fallen; "
                                 "per episode: tile U{flat, 10 deg ramp, 6 cm stairs, 2 cm rough}, dx U[-0.5, 0] m, dy U[-0.2, 0.2] m, yaw U[-pi, pi]" % (args.gait, args.vx),
                       "simulated_s": episode_run_s, "episodes_per_robot": float(np.mean(r["episode"][-1] + 1)),
@@ -692,6 +735,8 @@ def respawn_main(args, episode_run_s=5.0):
     solver = q.Solver(batch=B, device=0)
     xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
     kw = dict(gait=args.gait, cmd_vel=cmd, xy_yaw=xy, state_estimator=True, sensor_noise="reference")
+    if args.ee_frame:   # every robot's end-effector target in its heading frame (DESIGN.md §4.19)
+        kw["ee_frame"] = "heading"
 
     def timed(respawn, duration, randomize=None, spawn=None):
         solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
@@ -1291,7 +1336,12 @@ def main():
                     "session branching every robot every window against one without restores")
     ap.add_argument("--session", action="store_true", help="closed_loop.run against a Session stepped one window at a time, without commands and with a "
                                                            "torch heading controller's command every window: wall time per simulated second, the command kernel's time")
+    ap.add_argument("--ee-frame", action="store_true", help="end-effector targets in the heading frame: the target call's time with no, all-world and all-heading "
+                                                            "frame rows, and a turning sweep over start yaws and yaw rates in both frames; with --respawn: "
+                                                            "that run with every robot's targets in its heading frame")
     args = ap.parse_args()
+    if args.ee_frame and not args.respawn:
+        return ee_frame_main(args)
     if args.session:
         return session_main(args)
     if args.snapshot:
