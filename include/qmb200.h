@@ -267,7 +267,8 @@ int qmb200_gait_dev_set_commands(qmb200_handle* h, int32_t n_cmd, const double* 
  * QMB200_TARGET_EE_CMD_VEL (ee_cmd[b][c][0:3] = vx, vy, vz of the end effector, world frame; [3:7] ignored) or QMB200_TARGET_EE_GOAL (ee_cmd[b][c] = goal
  * position, quaternion xyzw, world frame); -1: none (the row is ignored).  Besides the checks above it rejects an ee_kind outside {-1, 1, 2}, a command
  * with both a cmd_vel row and an end-effector command, a non-finite ee_cmd_vel or goal and a goal quaternion whose norm differs from 1 by more than
- * 1e-9.  ee_kind and ee_cmd both NULL: qmb200_gait_dev_set_commands.  Synchronous. */
+ * 1e-9.  ee_kind and ee_cmd both NULL: qmb200_gait_dev_set_commands.  ee_kind QMB200_TARGET_EE_PATH starts the path ee_cmd[b][c][0] (an integer index
+ * of the path table in force, qmb200_set_ee_paths; [1:7] ignored).  Synchronous. */
 int qmb200_gait_dev_set_commands_ee(qmb200_handle* h, int32_t n_cmd, const double* t /*[B][n_cmd]*/, const int32_t* tmpl /*[B][n_cmd]*/, const double* cmd_vel /*[B][n_cmd][4]*/,
                                     const int32_t* ee_kind /*[B][n_cmd] or NULL*/, const double* ee_cmd /*[B][n_cmd][7] or NULL*/);
 /* One step per robot at t = t_obs[b], right before the MPC tick's target_trajectories: (1) every command of the robot due at t (time <= t) and not yet
@@ -289,7 +290,9 @@ int qmb200_gait_dev_step_dev(qmb200_handle* h, const double* t_obs, int32_t* n_e
  * (qmb200_target_trajectories_per_robot): QMB200_TARGET_EE_GOAL when the step applied a goal as its last target command (the goal is published once),
  * -1 while a published goal is held (the target call then leaves the robot's target and last_ee_target as they are), otherwise the source's stream,
  * QMB200_TARGET_CMD_VEL or QMB200_TARGET_EE_CMD_VEL.  A failed step (QMB200_ST_NAN / QMB200_ST_OVERFLOW) leaves the source unchanged and reports that
- * source's kind (-1 for a held goal).  target_kind is written for every robot. */
+ * source's kind (-1 for a held goal).  target_kind is written for every robot.  A path row (ee_kind QMB200_TARGET_EE_PATH, ee[0] the path index) writes
+ * cmd[b][0] and makes the path the source: QMB200_TARGET_EE_PATH on the tick that applied it, QMB200_TARGET_EE_PATH_FOLLOW after it (and from a
+ * failed step) while the source is the path (qmb200_target_trajectories_path). */
 int qmb200_gait_dev_step_ee(qmb200_handle* h, const double* t_obs /*[B]*/, int32_t* n_events /*[B] in-out*/, double* event_times /*[B][EMAX] in-out*/,
                             int32_t* mode_sequence /*[B][EMAX+1] in-out*/, double* cmd /*[B][7] in-out*/, int32_t* tmpl /*[B] or NULL*/, int32_t* mode /*[B] or NULL*/,
                             int32_t* status /*[B]*/, int32_t* target_kind /*[B] or NULL*/);
@@ -306,7 +309,8 @@ int qmb200_gait_dev_get_commands(qmb200_handle* h, int32_t* n_cmd, double* t /*[
                                  int32_t* ee_kind /*[B][n_cmd]*/, double* ee_cmd /*[B][n_cmd][7]*/);
 /* One command per robot from device buffers, applied by the robot's next step (DESIGN.md §4.16): each robot has one pending slot beside its schedule,
  * empty after qmb200_gait_dev_reset.  For every robot with mask[b] != 0 the row tmpl[b] (-1: none), cmd_vel[b][4] (a NaN row: none), ee_kind[b] (-1,
- * QMB200_TARGET_EE_CMD_VEL or QMB200_TARGET_EE_GOAL) and ee[b][7] (as ee_cmd of qmb200_gait_dev_set_commands_ee) is checked on the device with the rules
+ * QMB200_TARGET_EE_CMD_VEL, QMB200_TARGET_EE_GOAL or QMB200_TARGET_EE_PATH, whose index is checked against the path table in force) and ee[b][7] (as
+ * ee_cmd of qmb200_gait_dev_set_commands_ee) is checked on the device with the rules
  * of qmb200_gait_dev_set_commands_ee; an accepted row overwrites the slot (a later command before the step replaces an earlier one), a rejected row
  * leaves it and gets status[b] = QMB200_ST_COMMAND.  status [B] is written, not OR-ed: 0 for accepted rows and for robots with mask[b] == 0, whose
  * slots are not written.  The next step applies a set slot after the robot's timeline rows due at t, as one more row due at t, and clears it when it
@@ -329,6 +333,8 @@ int qmb200_gait_dev_stop(qmb200_handle* h);
 #define QMB200_TARGET_CMD_VEL 0      /* cmdVelToTargetTrajectories      (QmTargetTrajectoriesPublisher_node.cpp:73-113): cmd = vx, vy, vz, yaw rate */
 #define QMB200_TARGET_EE_CMD_VEL 1   /* EeCmdVelToTargetTrajectories    (:118-165): cmd = vx, vy, vz of the end effector */
 #define QMB200_TARGET_EE_GOAL 2      /* EEgoalPoseToTargetTrajectories  (:172-208) + processFeedback (QmTargetTrajectoriesPublisher.cpp:94-109): cmd = pos(3), quat xyzw(4) */
+#define QMB200_TARGET_EE_PATH 3      /* start of an end-effector path (qmb200_target_trajectories_path; DESIGN.md §4.20): cmd[0] = path index of the table */
+#define QMB200_TARGET_EE_PATH_FOLLOW 4   /* the path in force (path_state) at the call's time */
 #define QMB200_JOINT_CMD 5           /* HybridJointHandle::setCommand(posDes, velDes, kp, kd, ff) (HybridJointInterface.h:55-61) */
 #define QMB200_ST_SAFETY 0x10000     /* SafetyChecker::check failed (SafetyChecker.h:22-35): the reference stops the controller */
 #define QMB200_ST_COMMAND 0x20000    /* qmb200_gait_dev_command(_dev): the robot's command row was rejected (no other status word uses this bit) */
@@ -375,6 +381,36 @@ void qmb200_initial_ee_target(double* last_ee_target7);
 int qmb200_set_ee_frame(qmb200_handle* h, const int32_t* frame /*[B] or NULL to clear*/);
 /* frame [B] (zeros when none are set, may be NULL), is_set (may be NULL): whether rows are set */
 int qmb200_get_ee_frame(const qmb200_handle* h, int32_t* frame /*[B]*/, int32_t* is_set);
+
+/* End-effector paths (DESIGN.md §4.20): a handle-wide table of timed hand paths, shared by every robot as the gait templates are.  Path p has
+ * n_way[p] waypoints way[p][i] = (tau, position(3), quaternion xyzw(4)), tau in seconds after the path starts.  A robot that starts path p at time t0
+ * from the measured hand pose S follows the piecewise pose p(t) through (t0, S), (t0 + tau_1, w_1), ..., each segment a position lerp and an
+ * Eigen-semantics slerp (the MPC's own target interpolation); a heading-frame robot (qmb200_set_ee_frame) states the waypoints in its heading frame at
+ * the start, fixed for the rest of the path.  The setter rejects, naming the path and the waypoint, and writes nothing for: a non-finite value,
+ * n_way outside [1, QMB200_EE_PATH_MAX], tau_1 <= 0, times that are not strictly increasing, a gap between consecutive waypoints under T/2 (T the
+ * handle's MPC time horizon, qmb200_get_model_info's time_horizon: task.info's mpc.timeHorizon unless qmb200_create overrides it; every target then
+ * sees the path to t + T within QMB200_KMAX knots), a quaternion norm more than 1e-9 from 1.
+ * n_paths 0 or way NULL clears the table.  It waits for the device. */
+#define QMB200_EE_PATH_MAX 32
+int qmb200_set_ee_paths(qmb200_handle* h, int32_t n_paths, const int32_t* n_way /*[n_paths]*/, const double* way /*[n_paths][QMB200_EE_PATH_MAX][8]*/);
+/* n_paths (may be NULL): the table's size; n_way [n_paths] and way [n_paths][QMB200_EE_PATH_MAX][8] (zeros past n_way) may be NULL: a call with
+ * n_paths alone sizes the others */
+int qmb200_get_ee_paths(const qmb200_handle* h, int32_t* n_paths, int32_t* n_way, double* way);
+/* The per-robot target call with paths: kind[b] as qmb200_target_trajectories_per_robot takes it, or QMB200_TARGET_EE_PATH (start path cmd[b][0] now)
+ * or QMB200_TARGET_EE_PATH_FOLLOW (the path of path_state[b]).  path_state [B][QMB200_EE_PATH_STATE] is caller-owned and in-out: path index, start
+ * time t0, start heading (x0, y0, yaw0 = x_obs[6], [7], [9] at the start) and the hand's start pose [7] (world).  A start writes the row and
+ * last_ee_target (as a goal of the final waypoint published now leaves it), then follows.  Following at t writes the knot p(t) at t and the next
+ * (up to three) waypoints after t at t0 + tau: n_target = 2..4.  The base of knot 0 is the observed base at comHeight, level; a waypoint knot's base
+ * is the hand minus the (0.52, 0.09) offset (turned with the current yaw for a heading robot), at comHeight, level, at the current yaw.  With no
+ * waypoint after t the call writes nothing: the robot holds the last waypoint as a held goal.  A path index outside the current table leaves the
+ * robot untouched.  Robots of the other kinds get exactly what qmb200_target_trajectories_per_robot writes.  The host variant rejects kinds outside
+ * [-1, 4] and stages the rows in-out. */
+#define QMB200_EE_PATH_STATE 12
+int qmb200_target_trajectories_path(qmb200_handle* h, const int32_t* kind /*[B]*/, const double* cmd /*[B][7]*/, const double* t_obs /*[B]*/, const double* x_obs /*[B][30]*/,
+                                    const double* ee_state /*[B][7]*/, double* last_ee_target /*[B][7] in-out*/, double* path_state /*[B][EE_PATH_STATE] in-out*/,
+                                    int32_t* n_target /*[B] in-out*/, double* target_times /*[B][KMAX] in-out*/, double* target_states /*[B][KMAX][37] in-out*/);
+int qmb200_target_trajectories_path_dev(qmb200_handle* h, const int32_t* kind, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
+                                        double* last_ee_target, double* path_state, int32_t* n_target, double* target_times, double* target_states, void* cuda_stream);
 
 /* SafetyChecker::check + QMController::updateControlLaw (QMController.cpp:159-165,177-190) or, for a handle created with
  * QMB200_WBC_HIERARCHICAL_MPC, QMMpcController::updateControlLaw (:427-445).  joint_cmd entries the reference does not write in a given call

@@ -11,6 +11,8 @@ NX, NU, RBD, CMD, TARGET, EMAX, KMAX = 30, 30, 55, 54, 37, 32, 4
 GAIT_CAP, GAIT_MAXM = 64, 16   # QMB200_GAIT_CAP, QMB200_GAIT_MAXM
 TARGET_CMD_VEL, TARGET_EE_CMD_VEL, TARGET_EE_GOAL = 0, 1, 2   # QMB200_TARGET_*: the target front-end's kinds (-1 in a per-robot kind: a held goal)
 EE_FRAME_WORLD, EE_FRAME_HEADING = 0, 1   # QMB200_EE_FRAME_*: the frame a robot's end-effector targets are stated in (DESIGN.md §4.19)
+TARGET_EE_PATH, TARGET_EE_PATH_FOLLOW = 3, 4   # QMB200_TARGET_EE_PATH(_FOLLOW): start / follow an end-effector path (DESIGN.md §4.20)
+EE_PATH_MAX, EE_PATH_STATE = 32, 12   # QMB200_EE_PATH_MAX waypoints per path; QMB200_EE_PATH_STATE doubles of a robot's path state row
 ST_OVERFLOW = 0x2      # QMB200_ST_OVERFLOW: a WBC overflow
 ST_COMMAND = 0x20000   # QMB200_ST_COMMAND: a rejected qmb200_gait_dev_command row
 ST_RESTORE = 0x40000   # QMB200_ST_RESTORE: a qmb200_robot_state_load source row outside [0, B)
@@ -212,6 +214,10 @@ PROTOTYPES = {
     "qmb200_initial_ee_target": (None, [P]),
     "qmb200_set_ee_frame": (I32, [P] * 2),
     "qmb200_get_ee_frame": (I32, [P] * 3),
+    "qmb200_set_ee_paths": (I32, [P, I32, P, P]),
+    "qmb200_get_ee_paths": (I32, [P] * 4),
+    "qmb200_target_trajectories_path": (I32, [P] * 11),
+    "qmb200_target_trajectories_path_dev": (I32, [P] * 12),
     "qmb200_control_law": (I32, [P] * 10),
     "qmb200_control_law_dev": (I32, [P] * 11),
     "qmb200_set_arm_gains": (I32, [P, D, D]),

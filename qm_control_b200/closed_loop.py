@@ -56,7 +56,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
         attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None,
-        timeline=None, curriculum=None, ee_frame=None):
+        timeline=None, curriculum=None, ee_frame=None, ee_paths=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -185,14 +185,20 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     relative to its body while it walks and turns, its ee_goal rows (commands, timeline, Session.command) are poses in its heading frame at the
     publishing tick (the timeline's ee_x / ee_y / ee_z box is in heading coordinates), and the base offset of its end-effector targets turns with its
     yaw.  The refusals of end-effector commands beside varying headings (a drawn spawn yaw, a restart "here" or on given rows) then apply to
-    world-frame robots only.  The previous rows are restored when run returns."""
+    world-frame robots only.  The previous rows are restored when run returns.
+    ee_paths: the end-effector path table for this run (Solver.set_ee_paths; DESIGN.md §4.20), a list of (t [n], pose [n, 7]): waypoint times in
+    seconds after a path starts (t[0] > 0, strictly increasing, gaps >= time_horizon / 2, 1 <= n <= _lib.EE_PATH_MAX) and waypoint poses (position,
+    quaternion xyzw of unit norm; in the heading frame at the path's start for a heading-frame robot).  commands ee_path [B, C] (path ids, -1: none) and
+    Session.command(ee_path=[B]) start a path: the hand then follows the piecewise lerp / slerp from its pose at the start through the waypoints on
+    their schedule, and holds the last one.  Path commands to world-frame robots share the refusals of ee_goal / ee_cmd_vel.  The previous table is
+    restored when run returns; without ee_paths the loop makes exactly the calls it made before."""
     if isinstance(respawn, dict) and _place_spec(respawn)["on_request"]:
         raise ValueError("closed_loop.run: respawn on_request needs a Session (nothing can request a restart inside run; Session.respawn does)")
     with Session(solver, duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start, torch_device=torch_device,
                  sim_timer=sim_timer, friction_mu=friction_mu, payload=payload, pushes=pushes, model_payload=model_payload, terrain=terrain,
                  payload_estimator=payload_estimator, state_estimator=state_estimator, sensor_noise=sensor_noise, attitude_filter=attitude_filter,
                  slip_detector=slip_detector, ground_map=ground_map, commands=commands, tuning=tuning, respawn=respawn, randomize=randomize, spawn=spawn,
-                 metrics=metrics, timeline=timeline, curriculum=curriculum, ee_frame=ee_frame) as s:
+                 metrics=metrics, timeline=timeline, curriculum=curriculum, ee_frame=ee_frame, ee_paths=ee_paths) as s:
         rec = s.step(s.windows)
         end = s.finish()   # synchronises the session's stream
         out = {k: v if isinstance(v, np.ndarray) else v.cpu().numpy() for k, v in rec.items()}
@@ -203,7 +209,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
 RUN_DEFAULTS = dict(gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None, friction_mu=None,
                     payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None, attitude_filter=None,
                     slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None, timeline=None, curriculum=None,
-                    ee_frame=None)
+                    ee_frame=None, ee_paths=None)
 
 
 def _run_specs(solver, steer, o):
@@ -214,6 +220,7 @@ def _run_specs(solver, steer, o):
     attitude_filter, slip_detector, model_payload, tuning = (o[k] for k in ("attitude_filter", "slip_detector", "model_payload", "tuning"))
     ef = _ee_frame_spec(getattr(solver, "batch", None), o["ee_frame"])
     world = True if ef is None else ef == _lib.EE_FRAME_WORLD   # the robots whose end-effector targets assume they face +x
+    ep = _ee_paths_spec(getattr(solver, "time_horizon", None), o["ee_paths"])
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else dict(_respawn_spec(respawn), **_place_spec(respawn))
@@ -240,7 +247,7 @@ def _run_specs(solver, steer, o):
         raise ValueError("closed_loop.run: slip_detector must be None, True or a dict of slip detector parameters, got %r" % (slip_detector,))
     if slip_detector is not None and state_estimator is None:
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
-    gd = None if commands is None else _gait_commands(solver.batch, gait, commands)
+    gd = None if commands is None else _gait_commands(solver.batch, gait, commands, 0 if ep is None else len(ep))
     if steer and commands is None and timeline is None:   # an empty timeline: the session's commands are the schedule's only input
         gd = _gait_commands(solver.batch, gait, dict(t=np.zeros((solver.batch, 0)), gait=np.empty((solver.batch, 0), dtype=object)))
     tl = None if timeline is None else _timeline_spec(getattr(solver, "batch", None), gait, timeline, commands)
@@ -267,7 +274,7 @@ def _run_specs(solver, steer, o):
             rz["link"] |= _lib.EPISODE_MODEL_PAYLOAD
         if tn is not None and "friction_mu" in drawn:
             rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
-    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu, ef=ef, world=world)
+    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu, ef=ef, world=world, ep=ep)
 
 
 def _respawn_spec(respawn):
@@ -317,6 +324,21 @@ def _place_spec(respawn):
     return dict(at=spec["at"], on_request=bool(spec["on_request"]))
 
 
+def _ee_names(goal_or_vel, path):
+    """the end-effector commands a refusal names: "ee_goal / ee_cmd_vel", "ee_path" or both, or None for none"""
+    names = (["ee_goal / ee_cmd_vel"] if goal_or_vel else []) + (["ee_path"] if path else [])
+    return " / ".join(names) or None
+
+
+def _ee_refused(gd, world, robots=True):
+    """the end-effector commands of the parsed commands gd that go to world-frame robots (world: True or bool [B]) among robots (True or bool [B]),
+    named for a refusal (_ee_names), or None"""
+    if gd is None:
+        return None
+    m = gd["ee_robots"] & world & robots; path = gd.get("path_robots", False)
+    return _ee_names(np.any(m & gd.get("goal_robots", gd["ee_robots"])), np.any(m & path))
+
+
 def _here_refusal(sp_yaw_drawn, gd, curriculum, ground_map, world=True):
     """why a restart "here" (or on given spawn rows) cannot go with this run's specs, or None: the heading it keeps varies per robot.  world: True or
     bool [B], the world-frame robots (end-effector commands to heading-frame robots follow their heading)."""
@@ -324,8 +346,9 @@ def _here_refusal(sp_yaw_drawn, gd, curriculum, ground_map, world=True):
         return "a curriculum attached to the spawn (its levels draw every spawn)"
     if sp_yaw_drawn:
         return "a drawn spawn yaw (the heading a restart keeps would not be the draw's)"
-    if gd is not None and np.any(gd["ee_robots"] & world):
-        return "ee_goal / ee_cmd_vel commands to world-frame robots (their world-frame goals assume the robot faces +x)"
+    names = _ee_refused(gd, world)
+    if names is not None:
+        return "%s commands to world-frame robots (their world-frame goals assume the robot faces +x)" % names
     if isinstance(ground_map, dict):
         return "a ground_map dict (the map would not follow the ground; ground_map=True does)"
     return None
@@ -390,9 +413,10 @@ def _spawn_spec(B, spawn, terrain, ground_map, gd, world=True):
     if ground and isinstance(ground_map, dict):
         raise ValueError("closed_loop.run: a ground_map dict cannot go with a spawn that draws %s (the map would not follow the ground; ground_map=True does)"
                          % ", ".join(sorted(ground)))
-    if "yaw" in fields and gd is not None and np.any((fields["yaw"][0] != fields["yaw"][1]) & gd["ee_robots"] & world):
-        raise ValueError("closed_loop.run: a drawn spawn yaw cannot go with ee_goal / ee_cmd_vel commands to world-frame robots (their world-frame goals "
-                         "assume the robot faces +x)")
+    names = _ee_refused(gd, world, fields["yaw"][0] != fields["yaw"][1]) if "yaw" in fields else None
+    if names is not None:
+        raise ValueError("closed_loop.run: a drawn spawn yaw cannot go with %s commands to world-frame robots (their world-frame goals assume the robot "
+                         "faces +x)" % names)
     return dict(seed=seed, fields=fields, link=_lib.SPAWN_GROUND_MAP if ground_map is True else 0)
 
 
@@ -428,16 +452,16 @@ def _timeline_box(tl, cmd_vel, t_start):
     return lo, hi
 
 
-def _gait_commands(B, gait, commands):
+def _gait_commands(B, gait, commands, n_paths=0):
     """closed_loop.run's gait and commands → dict(names, gait [B] ids, t [B, C], tmpl [B, C] ids or -1, cmd_vel [B, C, 4], ee: {} or dict(ee_kind [B, C],
-    ee_cmd [B, C, 7]) when the timeline has ee_goal / ee_cmd_vel); ValueError when malformed"""
+    ee_cmd [B, C, 7]) when the timeline has ee_goal / ee_cmd_vel / ee_path); ValueError when malformed.  n_paths: the run's ee_paths table size"""
     names = gait_template_names()
     ids = {n: i for i, n in enumerate(names)}
     start = [gait] * B if isinstance(gait, str) else list(gait)
     if len(start) != B:
         raise ValueError("closed_loop.run: gait must be one name or a sequence of %d names, got %d" % (B, len(start)))
-    if not isinstance(commands, dict) or not {"t", "gait"} <= set(commands) or not set(commands) <= {"t", "gait", "cmd_vel", "ee_goal", "ee_cmd_vel"}:
-        raise ValueError("closed_loop.run: commands must be dict(t, gait[, cmd_vel][, ee_goal][, ee_cmd_vel]), got %r" % (commands,))
+    if not isinstance(commands, dict) or not {"t", "gait"} <= set(commands) or not set(commands) <= {"t", "gait", "cmd_vel", "ee_goal", "ee_cmd_vel", "ee_path"}:
+        raise ValueError("closed_loop.run: commands must be dict(t, gait[, cmd_vel][, ee_goal][, ee_cmd_vel][, ee_path]), got %r" % (commands,))
     t = np.asarray(commands["t"], dtype=np.float64)
     if t.ndim != 2 or t.shape[0] != B:
         raise ValueError("closed_loop.run: commands t must have shape (%d, C), got %s" % (B, t.shape))
@@ -454,16 +478,23 @@ def _gait_commands(B, gait, commands):
     if np.any(np.isnan(vel).any(-1) != np.isnan(vel).all(-1)) or np.any(np.isinf(vel)):
         raise ValueError("closed_loop.run: each commands cmd_vel row must be finite or all NaN")
     tmpl = np.array([[-1 if n is None else ids[n] for n in row] for row in g], dtype=np.int32).reshape(B, C)
-    ee = _ee_commands(B, C, commands, vel)
+    ee = _ee_commands(B, C, commands, vel, n_paths)
     return dict(names=names, gait=np.array([ids[n] for n in start], dtype=np.int32), t=t, tmpl=tmpl, cmd_vel=vel, ee=ee,
-                ee_robots=(ee["ee_kind"] >= 0).any(-1) if ee else np.zeros(B, dtype=bool))
+                ee_robots=(ee["ee_kind"] >= 0).any(-1) if ee else np.zeros(B, dtype=bool),
+                goal_robots=np.isin(ee["ee_kind"], (_lib.TARGET_EE_CMD_VEL, _lib.TARGET_EE_GOAL)).any(-1) if ee else np.zeros(B, dtype=bool),
+                path_robots=(ee["ee_kind"] == _lib.TARGET_EE_PATH).any(-1) if ee else np.zeros(B, dtype=bool))
 
 
-def _ee_commands(B, C, commands, vel):
-    """commands' ee_goal [B, C, 7] / ee_cmd_vel [B, C, 3] → {} when neither is given, else dict(ee_kind [B, C], ee_cmd [B, C, 7]) for
-    Solver.gait_dev_set_commands; ValueError when malformed"""
-    if commands.get("ee_goal") is None and commands.get("ee_cmd_vel") is None:
+def _ee_commands(B, C, commands, vel, n_paths=0):
+    """commands' ee_goal [B, C, 7] / ee_cmd_vel [B, C, 3] / ee_path [B, C] → {} when none is given, else dict(ee_kind [B, C], ee_cmd [B, C, 7]) for
+    Solver.gait_dev_set_commands; ValueError when malformed.  n_paths: the run's ee_paths table size (ee_path ids lie in [-1, n_paths))"""
+    if commands.get("ee_goal") is None and commands.get("ee_cmd_vel") is None and commands.get("ee_path") is None:
         return {}
+    path = np.full((B, C), -1) if commands.get("ee_path") is None else np.asarray(commands["ee_path"])
+    if path.shape != (B, C) or path.dtype.kind not in "iu" or np.any(path < -1):
+        raise ValueError("closed_loop.run: commands ee_path must be integer path ids (-1: none) of shape (%d, %d), got %r" % (B, C, commands.get("ee_path")))
+    if np.any(path >= n_paths):
+        raise ValueError("closed_loop.run: commands ee_path ids must lie in [-1, %d), the run's ee_paths (ee_paths=[(t, pose), ...] sets them)" % n_paths)
     goal = np.full((B, C, 7), np.nan) if commands.get("ee_goal") is None else np.asarray(commands["ee_goal"], dtype=np.float64)
     eev = np.full((B, C, 3), np.nan) if commands.get("ee_cmd_vel") is None else np.asarray(commands["ee_cmd_vel"], dtype=np.float64)
     if goal.shape != (B, C, 7) or eev.shape != (B, C, 3):
@@ -471,13 +502,14 @@ def _ee_commands(B, C, commands, vel):
     for name, a in (("ee_goal", goal), ("ee_cmd_vel", eev)):
         if np.any(np.isnan(a).any(-1) != np.isnan(a).all(-1)) or np.any(np.isinf(a)):
             raise ValueError("closed_loop.run: each commands %s row must be finite or all NaN" % name)
-    has_goal, has_eev = ~np.isnan(goal[..., 0]), ~np.isnan(eev[..., 0])
-    if np.any(has_goal.astype(int) + has_eev + ~np.isnan(vel[..., 0]) > 1):
-        raise ValueError("closed_loop.run: a command carries at most one of cmd_vel, ee_goal and ee_cmd_vel")
+    has_goal, has_eev, has_path = ~np.isnan(goal[..., 0]), ~np.isnan(eev[..., 0]), path >= 0
+    if np.any(has_goal.astype(int) + has_eev + has_path + ~np.isnan(vel[..., 0]) > 1):
+        raise ValueError("closed_loop.run: a command carries at most one of cmd_vel, ee_goal, ee_cmd_vel and ee_path")
     if np.any(np.abs(np.linalg.norm(goal[has_goal][:, 3:7], axis=-1) - 1.0) > 1e-9):
         raise ValueError("closed_loop.run: each commands ee_goal quaternion (xyzw) must have unit norm (within 1e-9)")
-    kind = np.where(has_goal, _lib.TARGET_EE_GOAL, np.where(has_eev, _lib.TARGET_EE_CMD_VEL, -1)).astype(np.int32)
+    kind = np.where(has_goal, _lib.TARGET_EE_GOAL, np.where(has_eev, _lib.TARGET_EE_CMD_VEL, np.where(has_path, _lib.TARGET_EE_PATH, -1))).astype(np.int32)
     cmd = np.where(has_goal[..., None], goal, 0.0); cmd[..., :3] = np.where(has_eev[..., None], eev, cmd[..., :3])
+    cmd[..., 0] = np.where(has_path, path, cmd[..., 0])
     return dict(ee_kind=kind, ee_cmd=cmd)
 
 
@@ -734,6 +766,44 @@ def _ee_frame_spec(B, ee_frame):
     return a.astype(np.int32)
 
 
+def _ee_paths_spec(T, ee_paths):
+    """closed_loop.run's ee_paths → None or a list of (t [n], pose [n, 7]) float arrays for Solver.set_ee_paths; ValueError when malformed (the
+    library's rules: DESIGN.md §4.20).  T: the handle's time horizon (None: the T/2 gap rule is left to the library)."""
+    if ee_paths is None:
+        return None
+    if isinstance(ee_paths, (str, dict)) or not hasattr(ee_paths, "__len__") or len(ee_paths) == 0:
+        raise ValueError("closed_loop.run: ee_paths must be a non-empty list of (t [n], pose [n, 7]), got %r" % (ee_paths,))
+    out = []
+    for p, item in enumerate(ee_paths):
+        try:
+            t, pose = item
+            t, pose = np.asarray(t, dtype=np.float64), np.asarray(pose, dtype=np.float64)
+        except (TypeError, ValueError):
+            raise ValueError("closed_loop.run: ee_paths[%d] must be a pair (t [n], pose [n, 7]) of numbers" % p) from None
+        if t.ndim != 1 or pose.shape != (len(t), 7) or not 1 <= len(t) <= _lib.EE_PATH_MAX:
+            raise ValueError("closed_loop.run: ee_paths[%d] must be (t [n], pose [n, 7]) with 1 <= n <= %d, got shapes %s and %s" % (p, _lib.EE_PATH_MAX, t.shape, pose.shape))
+        if not (np.all(np.isfinite(t)) and np.all(np.isfinite(pose))):
+            raise ValueError("closed_loop.run: ee_paths[%d] must be finite" % p)
+        if not (t[0] > 0.0 and np.all(np.diff(t) > 0.0)):
+            raise ValueError("closed_loop.run: ee_paths[%d] times must be > 0 and strictly increasing" % p)
+        if T is not None and np.any(np.diff(t) < 0.5 * T):
+            raise ValueError("closed_loop.run: ee_paths[%d] waypoints must lie at least time_horizon / 2 = %g s apart" % (p, 0.5 * T))
+        if np.any(np.abs(np.linalg.norm(pose[:, 3:7], axis=-1) - 1.0) > 1e-9):
+            raise ValueError("closed_loop.run: ee_paths[%d] quaternions (xyzw) must have unit norm (within 1e-9)" % p)
+        out.append((t, pose))
+    return out
+
+
+@contextlib.contextmanager
+def _ee_paths(solver, paths):
+    prev = solver.get_ee_paths()
+    try:
+        solver.set_ee_paths(paths)
+        yield
+    finally:
+        solver.set_ee_paths(prev)
+
+
 @contextlib.contextmanager
 def _ee_frame(solver, rows):
     prev = solver.get_ee_frame()
@@ -876,7 +946,7 @@ class Session:
         # restarts may place robots on rows of their own: "here", or a request's (DESIGN.md §4.18); the heading then varies as with a drawn yaw
         self._placing = rs is not None and (rs["at"] == "here" or rs["on_request"])
         self._heading_varies = self._yaw_drawn or (rs is not None and rs["at"] == "here")
-        self._ee_commanded = False; self._place_due = rs is not None and rs["at"] == "here"   # whether the next boundary places robots
+        self._ee_commanded = set(); self._place_due = rs is not None and rs["at"] == "here"   # whether the next boundary places robots
         self._scope = None; self._open = False; self._finished = False
 
     # ------------------------------------------------------------------------------------------------------------------------------------ scopes
@@ -898,6 +968,8 @@ class Session:
                 scope.enter_context(_robot_tuning(solver, tn, o["friction_mu"]))
             if p["ef"] is not None:
                 scope.enter_context(_ee_frame(solver, p["ef"]))
+            if p["ep"] is not None:
+                scope.enter_context(_ee_paths(solver, p["ep"]))
             if o["payload_estimator"] is not None:
                 scope.enter_context(_payload_estimator(solver, o["payload_estimator"]))
             if o["state_estimator"] is not None:
@@ -1070,6 +1142,11 @@ class Session:
         self.own = [q, v, rbd, contact, t_obs, x_obs, self.joint_cmd, self.arm_pos, self.last_time, self.cmd54, cmd7, self.last_ee, prob["n_events"],
                     prob["event_times"], prob["modes"], prob["n_target"], prob["target_times"], prob["target_states"]] + \
                    ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
+        self.path_state = None
+        if p["ep"] is not None:   # each robot's end-effector path row (index -1: none), the target call's in-out row beside last_ee
+            with torch.cuda.stream(stream):
+                self.path_state = torch.zeros((B, _lib.EE_PATH_STATE), dtype=torch.float64, device=dev); self.path_state[:, 0] = -1.0
+            self.own.append(self.path_state)
         self.k0 = None   # each robot's clock origin (plant step): with respawn, or once a restore has happened; the global k otherwise
         if rs is not None:   # the start image: the library's rows and the loop's own, then one restore of every robot through the cold path of every later one
             solver.robot_image_save()
@@ -1141,7 +1218,7 @@ class Session:
             if self._commanded:   # the status of the commands this step applied goes into the window it opens
                 self.acc_st.bitwise_or_(self.cmd_acc); self.cmd_acc.zero_(); self._commanded = False
             solver.target_trajectories_dev(self.tick_kind, self.cmd7, self.t_obs, self.x_obs, self.ee_state, self.last_ee, prob["n_target"], prob["target_times"],
-                                           prob["target_states"], s)
+                                           prob["target_states"], s, **({} if self.path_state is None else dict(path_state=self.path_state)))
         solver.mpc_solve_dev(prob, s)
 
     def _respawn(self, k):   # the robots due restart at window boundary k: their episode closes, their level moves, then the library's rows, the loop's, their new plant
@@ -1316,7 +1393,7 @@ class Session:
         self._k += n * MPC_PERIOD_MS
         return rec
 
-    def command(self, mask, gait=None, cmd_vel=None, ee_goal=None, ee_cmd_vel=None):
+    def command(self, mask, gait=None, cmd_vel=None, ee_goal=None, ee_cmd_vel=None, ee_path=None):
         """One command for each robot with mask [B] set, from device tensors (host arrays are copied): gait [B] template ids (an index of
         self.gait_templates, -1: none), cmd_vel [B, 4], ee_goal [B, 7] (position, quaternion xyzw of unit norm, world frame) and ee_cmd_vel [B, 3], NaN
         rows meaning none; a row carries at most one of cmd_vel, ee_goal and ee_cmd_vel.  The rows take the semantics of a commands timeline row due at
@@ -1324,18 +1401,25 @@ class Session:
         later command before that tick replaces an earlier one; a robot that respawns at that boundary drops it.  A rejected row (checked on the device
         with the timeline's rules) is not applied and sets _lib.ST_COMMAND in that window's record status.  Enqueued on self.stream after the work
         the caller's current stream holds (the tensors may come from it), no synchronisation.  ValueError without the device gait schedule (steer, commands or timeline), on wrong shapes, and for end-effector commands in
-        a session that draws spawn yaws."""
+        a session that draws spawn yaws.  ee_path [B]: integer path ids of the session's ee_paths (-1: none), which start that path (DESIGN.md §4.20);
+        ValueError without ee_paths."""
         import torch
         if self._spec["gd"] is None:
             raise ValueError("closed_loop.Session.command: needs the device gait schedule (steer=True, commands or timeline)")
         B = getattr(self.solver, "batch", None)
-        for name, a, shape in (("mask", mask, (B,)), ("gait", gait, (B,)), ("cmd_vel", cmd_vel, (B, 4)), ("ee_goal", ee_goal, (B, 7)), ("ee_cmd_vel", ee_cmd_vel, (B, 3))):
+        for name, a, shape in (("mask", mask, (B,)), ("gait", gait, (B,)), ("cmd_vel", cmd_vel, (B, 4)), ("ee_goal", ee_goal, (B, 7)), ("ee_cmd_vel", ee_cmd_vel, (B, 3)),
+                               ("ee_path", ee_path, (B,))):
             if a is not None and tuple(np.shape(a)) != shape:
                 raise ValueError("closed_loop.Session.command: %s must have shape %s, got %s" % (name, shape, tuple(np.shape(a))))
-        ee_world = self._ee_to_world(mask, ee_goal is not None or ee_cmd_vel is not None)
+        if ee_path is not None and self._spec["ep"] is None:
+            raise ValueError("closed_loop.Session.command: ee_path needs the session's ee_paths")
+        if ee_path is not None and (ee_path.dtype.is_floating_point or ee_path.dtype == torch.bool if isinstance(ee_path, torch.Tensor) else np.asarray(ee_path).dtype.kind not in "iu"):
+            raise ValueError("closed_loop.Session.command: ee_path must hold integer path ids (-1: none), got %r" % (ee_path,))
+        names = _ee_names(ee_goal is not None or ee_cmd_vel is not None, ee_path is not None)
+        ee_world = self._ee_to_world(mask, names is not None)
         if self._heading_varies and ee_world:
-            raise ValueError("closed_loop.Session.command: ee_goal / ee_cmd_vel to world-frame robots cannot go with a drawn spawn yaw or a restart \"here\" "
-                             "(their world-frame goals assume the robot faces +x)")
+            raise ValueError("closed_loop.Session.command: %s to world-frame robots cannot go with a drawn spawn yaw or a restart \"here\" "
+                             "(their world-frame goals assume the robot faces +x)" % names)
         if not self._open or self._finished:
             raise ValueError("closed_loop.Session.command: the session is not open (enter it with `with`; finish() ends it)")
         self._wait_caller()
@@ -1345,12 +1429,17 @@ class Session:
             goal = put(ee_goal, torch.float64, (B, 7), np.nan); eev = put(ee_cmd_vel, torch.float64, (B, 3), np.nan)
             has_goal, has_eev = ~torch.isnan(goal).all(-1), ~torch.isnan(eev).all(-1)   # a partly NaN row is a command the check rejects
             kind = torch.where(has_goal, _lib.TARGET_EE_GOAL, torch.where(has_eev, _lib.TARGET_EE_CMD_VEL, -1))
-            kind = torch.where(has_goal & has_eev, 3, kind).to(torch.int32)   # both: a kind the check rejects
             ee = torch.where(has_goal[:, None], goal, 0.0); ee[:, :3] = torch.where(has_eev[:, None], eev, ee[:, :3])
+            n_ee = has_goal.int() + has_eev.int()
+            if ee_path is not None:   # a path id below -1 is a path index the check rejects
+                path = put(ee_path, torch.float64, (B,), -1.0); has_path = path != -1.0
+                kind = torch.where(has_path, _lib.TARGET_EE_PATH, kind); ee[:, 0] = torch.where(has_path, path, ee[:, 0]); n_ee = n_ee + has_path.int()
+            kind = torch.where(n_ee > 1, -2, kind).to(torch.int32)   # more than one: a kind the check rejects
             self.solver.gait_dev_command_dev(m, tmpl, vel, kind, ee, self.cmd_st, self._s)
             self.cmd_acc.bitwise_or_(self.cmd_st)
         self._commanded = True
-        self._ee_commanded |= ee_world
+        if ee_world:
+            self._ee_commanded.add(names)
 
     def respawn(self, mask, end=2, at=None):
         """Restart each robot with mask [B] set at the next window boundary, before its MPC tick, through run's respawn path (DESIGN.md §4.18); needs
@@ -1386,7 +1475,8 @@ class Session:
         if code:
             why = _here_refusal(False, self._spec["gd"], self._o["curriculum"], self._o["ground_map"], self._spec["world"])
             if why is None and self._ee_commanded:
-                why = "ee_goal / ee_cmd_vel commands to world-frame robots (their world-frame goals assume the robot faces +x)"
+                names = _ee_names(any("ee_goal" in n for n in self._ee_commanded), any("ee_path" in n for n in self._ee_commanded))
+                why = "%s commands to world-frame robots (their world-frame goals assume the robot faces +x)" % names
             if why is not None:
                 raise ValueError("closed_loop.Session.respawn: a restart \"here\" or on given rows cannot go with %s" % why)
         if not self._open or self._finished:

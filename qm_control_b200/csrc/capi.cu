@@ -90,6 +90,9 @@ struct qmb200_handle {
     std::vector<int32_t> host; int32_t* d = nullptr; uint64_t gen = 0; bool on_device = false;
     const int32_t* dev() const { return host.empty() ? nullptr : d; }
   } ee_frame;
+  struct {   // the end-effector path table (qmb200_set_ee_paths): host copies (n_way empty = none) and device copies of n_way [n] and way [n][EE_PATH_MAX][8]
+    std::vector<int32_t> n_way; std::vector<double> way; int32_t* d_n_way = nullptr; double* d_way = nullptr;
+  } ee_path;
   qmb200_payload_est_params est_prm{}; FilterState est{EST_DBL, "payload estimator", "qmb200_payload_est_reset"};   // payload estimator (capi_est.inc)
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
   qmb200_state_est_params se_prm{}; FilterState se{SE_DBL, "state estimator", "qmb200_state_est_reset"};   // base state estimator
@@ -307,7 +310,7 @@ void qmb200_destroy(qmb200_handle* h) {
   cudaFree(h->est.d); cudaFree(h->se.d); cudaFree(h->at.d); cudaFree(h->sl.d);
   cudaFree(h->gs.d_table); cudaFree(h->gs.d_robots); cudaFree(h->gs.d_cursor); cudaFree(h->gs.d_t); cudaFree(h->gs.d_tmpl); cudaFree(h->gs.d_vel);
   cudaFree(h->gs.d_ee_kind); cudaFree(h->gs.d_ee); cudaFree(h->gs.d_pending);
-  cudaFree(h->image.d);
+  cudaFree(h->image.d); cudaFree(h->ee_path.d_n_way); cudaFree(h->ee_path.d_way);
   delete h;
 }
 

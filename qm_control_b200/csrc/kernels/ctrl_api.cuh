@@ -130,6 +130,89 @@ QMB_HD void target_robot(const TargetParams& prm, int kind, bool heading, const 
   for (int i = 2 * TARGET_DIM; i < KMAX * TARGET_DIM; ++i) ts[i] = 0.0;
 }
 
+// End-effector paths (qmb200_set_ee_paths, qmb200_target_trajectories_path; DESIGN.md §4.20).  A waypoint is (tau, position 3, quaternion xyzw 4); a
+// path row of the table is EE_PATH_MAX waypoints.  A robot's path state row: index, t0, the heading at the start (x0, y0, yaw0), the hand's start pose [7].
+constexpr int TARGET_EE_PATH = 3, TARGET_EE_PATH_FOLLOW = 4;
+constexpr int EE_PATH_MAX = 32, EE_PATH_WAY = 8, EE_PATH_STATE = 12;
+// The check of qmb200_set_ee_paths on n_paths paths (n_way [n_paths], way [n_paths][EE_PATH_MAX][EE_PATH_WAY]) for a handle of time horizon T: "" when
+// accepted, else the message naming the path and the waypoint
+inline std::string ee_paths_error(int n_paths, const int32_t* n_way, const double* way, double T) {
+  const std::string who = "qmb200_set_ee_paths: ";
+  if (n_paths < 0) return who + "n_paths must be >= 0";
+  for (int p = 0; p < n_paths; ++p) {
+    const std::string path = "path " + std::to_string(p);
+    if (n_way[p] < 1 || n_way[p] > EE_PATH_MAX) return who + path + " has " + std::to_string(n_way[p]) + " waypoints, not 1 to QMB200_EE_PATH_MAX (32)";
+    for (int i = 0; i < n_way[p]; ++i) {
+      const double* w = way + ((size_t)p * EE_PATH_MAX + i) * EE_PATH_WAY; const std::string at = who + path + ", waypoint " + std::to_string(i) + ": ";
+      for (int k = 0; k < EE_PATH_WAY; ++k) if (!std::isfinite(w[k])) return at + "value " + std::to_string(k) + " is not finite";
+      if (i == 0 && !(w[0] > 0.0)) return at + "its time must be > 0 (seconds after the path starts)";
+      if (i > 0 && !(w[0] > w[-EE_PATH_WAY])) return at + "its time is not after waypoint " + std::to_string(i - 1) + "'s";
+      if (i > 0 && w[0] - w[-EE_PATH_WAY] < 0.5 * T) return at + "its gap to waypoint " + std::to_string(i - 1) + " is under T/2 = " + std::to_string(0.5 * T) + " s";
+      const double qn = std::sqrt(w[4] * w[4] + w[5] * w[5] + w[6] * w[6] + w[7] * w[7]);
+      if (!(std::fabs(qn - 1.0) <= 1e-9)) return at + "its quaternion must have unit norm (within 1e-9)";
+    }
+  }
+  return "";
+}
+
+// o [7] = the pose at weight a between poses l and r [7] as target_pose interpolates two knots (a l + (1 - a) r, Eigen slerp semantics); a == 1 gives l
+// itself.  The slerp's sines take angles in [0, pi/2]: spawn_sincos, whose device path needs no stack.
+QMB_HD void path_pose(const double* l, const double* r, double a, double* o) {
+  if (a == 1.0) { for (int i = 0; i < 7; ++i) o[i] = l[i]; return; }
+  for (int i = 0; i < 3; ++i) o[i] = a * l[i] + (1.0 - a) * r[i];
+  const double* ql = l + 3; const double* qr = r + 3; const double tq = 1.0 - a; double d = 0.0; for (int i = 0; i < 4; ++i) d += ql[i] * qr[i];
+  const double ad = fabs(d); double s0, s1, cs;
+  if (ad >= 1.0 - 2.220446049250313e-16) { s0 = 1.0 - tq; s1 = tq; }
+  else { const double th = acos(ad); double st; spawn_sincos(th, st, cs); const double ist = 1.0 / st; spawn_sincos((1.0 - tq) * th, s0, cs); spawn_sincos(tq * th, s1, cs); s0 *= ist; s1 *= ist; }
+  if (d < 0.0) s1 = -s1;
+  for (int i = 0; i < 4; ++i) o[3 + i] = s0 * ql[i] + s1 * qr[i];
+}
+
+// waypoint w [EE_PATH_WAY] of a path → its pose o [7] in the world: itself, or h0 (the heading frame at the path's start) applied to it
+QMB_HD void path_way_world(const Heading& h0, bool heading, const double* w, double* o) {
+  if (!heading) for (int i = 0; i < 7; ++i) o[i] = w[1 + i];
+  else heading_to_world(h0, w + 1, o);
+}
+
+// One robot of the target front-end on a path (DESIGN.md §4.20): start (kind TARGET_EE_PATH: path index c[0]) or follow (TARGET_EE_PATH_FOLLOW) with
+// the path state row ps [EE_PATH_STATE] (in-out) on the table (n_paths paths, n_way [n_paths], way [n_paths][EE_PATH_MAX][EE_PATH_WAY]).  Arguments
+// otherwise as target_robot's.  A path index outside [0, n_paths) leaves everything untouched; so does a path with no waypoint after t, after a start's
+// writes.  Knot 0 is the path's own pose p(t) (not the measured hand), so that between knots the MPC's reference is the path itself.
+QMB_HD void target_path(const TargetParams& prm, bool start, bool heading, const double* c, double t, const double* x, const double* ee, double* le, double* ps,
+                        int n_paths, const int32_t* n_way, const double* way, int32_t* n_target, double* tt, double* ts) {
+  const double fi = start ? c[0] : ps[0];
+  if (!(fi >= 0.0 && fi < (double)n_paths && floor(fi) == fi)) return;
+  const int p = (int)fi, n = n_way[p]; const double* wp = way + (size_t)p * EE_PATH_MAX * EE_PATH_WAY;
+  const Heading hc = heading ? heading_at(x[6], x[7], x[9]) : Heading{0.0, 0.0, 0.0, 1.0, 0.0, 1.0};
+  const double ox = heading ? hc.c * 0.52 - hc.s * 0.09 : 0.52, oy = heading ? hc.s * 0.52 + hc.c * 0.09 : 0.09;   // the base offset, as the goal's
+  if (start) {
+    ps[0] = fi; ps[1] = t; ps[2] = x[6]; ps[3] = x[7]; ps[4] = x[9]; for (int i = 0; i < 7; ++i) ps[5 + i] = ee[i];
+    double g[7]; path_way_world(hc, heading, wp + (size_t)(n - 1) * EE_PATH_WAY, g);   // H(start) is H(cur) on the start tick
+    if (!heading) for (int i = 0; i < 7; ++i) le[i] = g[i];   // the final waypoint as a goal published now leaves the hold
+    else { const Heading ht{g[0] - ox, g[1] - oy, hc.s, hc.c, hc.sh, hc.ch}; heading_pos_from_world(ht, g, le); heading_quat_from_world(ht, g + 3, le + 3); }
+  }
+  const double t0 = ps[1];
+  int j = 0; while (j < n && !(t0 + wp[(size_t)j * EE_PATH_WAY] > t)) ++j;   // the first waypoint after t (n <= EE_PATH_MAX)
+  if (j == n) return;
+  const Heading h0 = heading ? heading_at(ps[2], ps[3], ps[4]) : hc;
+  double e[7], r[7];
+  path_way_world(h0, heading, wp + (size_t)j * EE_PATH_WAY, r);
+  const double tr = t0 + wp[(size_t)j * EE_PATH_WAY];
+  if (j == 0) path_pose(ps + 5, r, fmin((tr - t) / (tr - t0), 1.0), e);   // before its start the path is its start pose
+  else { double l[7]; path_way_world(h0, heading, wp + (size_t)(j - 1) * EE_PATH_WAY, l); const double tl = t0 + wp[(size_t)(j - 1) * EE_PATH_WAY]; path_pose(l, r, (tr - t) / (tr - tl), e); }
+  const int m = n - j < KMAX - 1 ? n - j : KMAX - 1;   // waypoint knots
+  *n_target = 1 + m; tt[0] = t;
+  for (int k = 0; k < KMAX; ++k) {
+    double* s = ts + k * TARGET_DIM;
+    if (k > m) { tt[k] = 0.0; for (int i = 0; i < TARGET_DIM; ++i) s[i] = 0.0; continue; }
+    if (k > 0) { const double* w = wp + (size_t)(j + k - 1) * EE_PATH_WAY; tt[k] = t0 + w[0]; path_way_world(h0, heading, w, e); }
+    for (int i = 0; i < 6; ++i) s[i] = 0.0;
+    s[6] = k == 0 ? x[6] : e[0] - ox; s[7] = k == 0 ? x[7] : e[1] - oy; s[8] = prm.com_height; s[9] = x[9]; s[10] = 0.0; s[11] = 0.0;
+    for (int jj = 0; jj < NJ; ++jj) s[12 + jj] = prm.default_joint_state[jj];
+    for (int i = 0; i < 7; ++i) s[30 + i] = e[i];
+  }
+}
+
 struct ControlLawParams {
   static constexpr int ROBOTS = 7, THREADS = 128;   // 7 robots x 18 joints = 126 threads of a 128-thread CTA
   int variant;                // 0 QMController, 1 QMMpcController
@@ -137,10 +220,13 @@ struct ControlLawParams {
 };
 
 int launch_observation(const DevModel* mdl, int B, const double* rbd, const double* period, double* t_obs, double* x_obs, cudaStream_t s, const double* srbd /*[B][SRBD_DBL] or NULL*/);
-// kinds [B] (device, or NULL: every robot `kind`): per-robot kind; robots outside [0, 2] are left untouched.  frame [B] (device, or NULL: every robot
-// EE_FRAME_WORLD): per-robot end-effector frame
+// kinds [B] (device, or NULL: every robot `kind`): per-robot kind; robots outside [0, 2] (and the path kinds when paths.state is set) are left
+// untouched.  frame [B] (device, or NULL: every robot EE_FRAME_WORLD): per-robot end-effector frame
+// paths: the path rows of qmb200_target_trajectories_path (state NULL: none; robots of the path kinds are then left untouched)
+struct TargetPaths { double* state; int n; const int32_t* n_way; const double* way; };
 int launch_target(const TargetParams& prm, int kind, const int32_t* kinds, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
-                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s, const int32_t* frame);
+                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s, const int32_t* frame,
+                  const TargetPaths& paths = TargetPaths{nullptr, 0, nullptr, nullptr});
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,
                        double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s,
                        const double* tuning /*[B][TUNING_DBL] or NULL: the robots' arm gains in place of prm's*/);

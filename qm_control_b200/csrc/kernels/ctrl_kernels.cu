@@ -61,15 +61,21 @@ __global__ void __launch_bounds__(OBS_ROBOTS) ctrl_observation_kernel(const DevM
 // Target front-end.  kind 0: /cmd_vel (cmd = vx, vy, vz, yaw rate), 1: /ee_cmd_vel (cmd = vx, vy, vz), 2: goal pose (cmd = pos(3), quat xyzw(4)).
 // kinds [B] (or NULL: every robot `kind`): robot b's kind; a robot whose kind lies outside [0, 2] (-1: its goal is held) is left untouched.
 // frame [B] (or NULL: every robot in the world frame): robot b's end-effector frame, EE_FRAME_WORLD or EE_FRAME_HEADING (target_robot).
+// paths.state set: robots of kind TARGET_EE_PATH / _FOLLOW run target_path on their path state row and the path table (2 to KMAX knots).
 // Output: the 2-knot TargetTrajectories [time; 37-dim state = (0_6 | v, base pose, defaultJointState, EE pose)] in the solver's layout.
 __global__ void __launch_bounds__(128) ctrl_target_kernel(TargetParams prm, int kind_all, const int32_t* __restrict__ kinds, int B, const double* __restrict__ cmd /*[B][7]*/,
                                                            const double* __restrict__ t_obs, const double* __restrict__ x_obs, const double* __restrict__ ee_state /*[B][7]*/,
                                                            double* __restrict__ last_ee_target /*[B][7]*/, int32_t* __restrict__ n_target, double* __restrict__ target_times /*[B][KMAX]*/,
-                                                           double* __restrict__ target_states /*[B][KMAX][37]*/, const int32_t* __restrict__ frame) {
+                                                           double* __restrict__ target_states /*[B][KMAX][37]*/, const int32_t* __restrict__ frame, TargetPaths paths) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x; if (b >= B) return;
-  const int kind = kinds ? kinds[b] : kind_all; if (kind < 0 || kind > 2) return;
-  target_robot(prm, kind, frame && frame[b] == EE_FRAME_HEADING, cmd + (size_t)b * 7, t_obs[b], x_obs + (size_t)b * NX, ee_state + (size_t)b * 7,
-               last_ee_target + (size_t)b * 7, n_target + b, target_times + (size_t)b * KMAX, target_states + (size_t)b * KMAX * TARGET_DIM);
+  const int kind = kinds ? kinds[b] : kind_all;
+  if (kind >= 0 && kind <= 2)
+    target_robot(prm, kind, frame && frame[b] == EE_FRAME_HEADING, cmd + (size_t)b * 7, t_obs[b], x_obs + (size_t)b * NX, ee_state + (size_t)b * 7,
+                 last_ee_target + (size_t)b * 7, n_target + b, target_times + (size_t)b * KMAX, target_states + (size_t)b * KMAX * TARGET_DIM);
+  else if (paths.state && (kind == TARGET_EE_PATH || kind == TARGET_EE_PATH_FOLLOW))
+    target_path(prm, kind == TARGET_EE_PATH, frame && frame[b] == EE_FRAME_HEADING, cmd + (size_t)b * 7, t_obs[b], x_obs + (size_t)b * NX, ee_state + (size_t)b * 7,
+                last_ee_target + (size_t)b * 7, paths.state + (size_t)b * EE_PATH_STATE, paths.n, paths.n_way, paths.way, n_target + b,
+                target_times + (size_t)b * KMAX, target_states + (size_t)b * KMAX * TARGET_DIM);
 }
 
 // -----------------------------------------------------------------------------------------------------------------
@@ -142,8 +148,10 @@ int launch_observation(const DevModel* mdl, int B, const double* rbd, const doub
   ctrl_observation_kernel<<<(B + OBS_ROBOTS - 1) / OBS_ROBOTS, OBS_ROBOTS, 0, s>>>(mdl, B, rbd, period, t_obs, x_obs, srbd); return 1;
 }
 int launch_target(const TargetParams& prm, int kind, const int32_t* kinds, int B, const double* cmd, const double* t_obs, const double* x_obs, const double* ee_state,
-                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s, const int32_t* frame) {
-  ctrl_target_kernel<<<(B + 127) / 128, 128, 0, s>>>(prm, kind, kinds, B, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, frame); return 1;
+                  double* last_ee_target, int32_t* n_target, double* target_times, double* target_states, cudaStream_t s, const int32_t* frame,
+                  const TargetPaths& paths) {
+  ctrl_target_kernel<<<(B + 127) / 128, 128, 0, s>>>(prm, kind, kinds, B, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, frame,
+                                                     paths); return 1;
 }
 int launch_control_law(const ControlLawParams& prm, int B, const double* x_des, const double* u_des, const double* wbc_cmd, const double* t_obs, const double* x_obs,
                        double* joint_cmd, double* arm_pos_cmd, double* last_time, int32_t* status, cudaStream_t s, const double* tuning) {

@@ -17,15 +17,17 @@ constexpr int GS_STANCE = 15;
 struct GsTemplate { int32_t n; int32_t md[GS_MAXM]; double sw[GS_MAXM + 1]; };
 // one robot's schedule: event times ev[n] (strictly increasing) and the n + 1 modes md[0..n] before, between and after them
 struct GsSchedule { int32_t n; int32_t md[GS_CAP + 1]; double ev[GS_CAP]; };
-// the target source of a robot's publisher (DESIGN.md §4.8): the cmd_vel stream (0, a zeroed robot's), the ee_cmd_vel stream, or a published goal
-// that is held
+// the target source of a robot's publisher (DESIGN.md §4.8): the cmd_vel stream (0, a zeroed robot's), the ee_cmd_vel stream, a published goal
+// that is held, or an end-effector path that is followed (DESIGN.md §4.20)
 constexpr int GS_SRC_CMD_VEL = QMB200_TARGET_CMD_VEL, GS_SRC_EE_CMD_VEL = QMB200_TARGET_EE_CMD_VEL, GS_SRC_EE_GOAL = QMB200_TARGET_EE_GOAL;
+constexpr int GS_SRC_EE_PATH = QMB200_TARGET_EE_PATH;
 constexpr int GS_KIND_HELD = -1;   // target kind of a robot whose goal is held: its target call writes nothing
+constexpr int GS_KIND_FOLLOW = QMB200_TARGET_EE_PATH_FOLLOW;   // target kind of a robot that follows its path
 // one robot's device state: the stored schedule, the active template (its index in the handle's table) and the target source
 struct GsRobot { GsSchedule s; int32_t tmpl; int32_t src; };
 // one robot's commands (robot-major arrays [B][n_cmd]): time t (sorted per robot), template (-1: none), cmd_vel row [4] (NaN: none), and optionally
-// an end-effector command: kind (-1: none, QMB200_TARGET_EE_CMD_VEL, QMB200_TARGET_EE_GOAL) with its row [7] (ee_cmd_vel: vx, vy, vz; goal: pos,
-// quat xyzw).  NULL ee_kind: no end-effector rows.  A row carries at most one of cmd_vel and an end-effector command.
+// an end-effector command: kind (-1: none, QMB200_TARGET_EE_CMD_VEL, QMB200_TARGET_EE_GOAL, QMB200_TARGET_EE_PATH) with its row [7] (ee_cmd_vel:
+// vx, vy, vz; goal: pos, quat xyzw; path: the path index).  NULL ee_kind: no end-effector rows.  A row carries at most one of cmd_vel and an end-effector command.
 struct GsCommands { int n; const double* t; const int32_t* tmpl; const double* vel; const int32_t* ee_kind = nullptr; const double* ee = nullptr; };
 // one robot's pending command (qmb200_gait_dev_command): one row of GsCommands without its time, applied by the robot's next step.  set 0: none.
 // Zeroed words are an empty slot, so the restore clears it with one zero segment.
@@ -73,21 +75,24 @@ QMB_HD int gs_get(GsSchedule& s, const GsTemplate& t, double lower, double upper
   return s.n > QMB200_EMAX ? -2 : s.n;
 }
 
-// the target kind of a robot's target call on a tick: a goal published by this tick's step (applied = QMB200_TARGET_EE_GOAL), else the source's
-// stream, GS_KIND_HELD for a held goal
-QMB_HD int gs_target_kind(int src, int applied) { return applied == GS_SRC_EE_GOAL ? GS_SRC_EE_GOAL : src == GS_SRC_EE_GOAL ? GS_KIND_HELD : src; }
+// the target kind of a robot's target call on a tick: a goal or path started by this tick's step (applied = QMB200_TARGET_EE_GOAL or _EE_PATH), else
+// the source's stream, GS_KIND_HELD for a held goal, GS_KIND_FOLLOW for a path
+QMB_HD int gs_target_kind(int src, int applied) {
+  return applied == GS_SRC_EE_GOAL || applied == GS_SRC_EE_PATH ? applied : src == GS_SRC_EE_GOAL ? GS_KIND_HELD : src == GS_SRC_EE_PATH ? GS_KIND_FOLLOW : src;
+}
 
 // the rules qmb200_gait_dev_set_commands_ee checks on the host, for one command row: QMB200_ST_COMMAND when the template lies outside [-1, n_templates),
-// the cmd_vel row is neither all finite nor all NaN, the kind is not -1, QMB200_TARGET_EE_CMD_VEL or QMB200_TARGET_EE_GOAL, an end-effector value
-// (ee[0:3] of ee_cmd_vel, ee[0:7] of a goal) is not finite, a goal quaternion's norm differs from 1 by more than 1e-9, or the row carries both a cmd_vel
-// and an end-effector command; else 0
-QMB_HD int gs_command_check(int tmpl, const double* vel, int ee_kind, const double* ee, int n_templates) {
+// the cmd_vel row is neither all finite nor all NaN, the kind is not -1, QMB200_TARGET_EE_CMD_VEL, QMB200_TARGET_EE_GOAL or QMB200_TARGET_EE_PATH, an
+// end-effector value (ee[0:3] of ee_cmd_vel, ee[0:7] of a goal) is not finite, a goal quaternion's norm differs from 1 by more than 1e-9, a path index
+// ee[0] is not an integer in [0, n_paths), or the row carries both a cmd_vel and an end-effector command; else 0
+QMB_HD int gs_command_check(int tmpl, const double* vel, int ee_kind, const double* ee, int n_templates, int n_paths = 0) {
   if (tmpl < -1 || tmpl >= n_templates) return QMB200_ST_COMMAND;
   const bool none = isnan(vel[0]);
   for (int i = 0; i < 4; ++i) if (none ? !isnan(vel[i]) : !isfinite(vel[i])) return QMB200_ST_COMMAND;
   if (ee_kind == -1) return 0;
-  if (ee_kind != GS_SRC_EE_CMD_VEL && ee_kind != GS_SRC_EE_GOAL) return QMB200_ST_COMMAND;
+  if (ee_kind != GS_SRC_EE_CMD_VEL && ee_kind != GS_SRC_EE_GOAL && ee_kind != GS_SRC_EE_PATH) return QMB200_ST_COMMAND;
   if (!none) return QMB200_ST_COMMAND;
+  if (ee_kind == GS_SRC_EE_PATH) return ee[0] >= 0.0 && ee[0] < (double)n_paths && floor(ee[0]) == ee[0] ? 0 : QMB200_ST_COMMAND;
   const bool goal = ee_kind == GS_SRC_EE_GOAL;
   for (int i = 0; i < (goal ? 7 : 3); ++i) if (!isfinite(ee[i])) return QMB200_ST_COMMAND;
   const double qn = sqrt(ee[3] * ee[3] + ee[4] * ee[4] + ee[5] * ee[5] + ee[6] * ee[6]);
@@ -95,7 +100,7 @@ QMB_HD int gs_command_check(int tmpl, const double* vel, int ee_kind, const doub
 }
 
 // one command row due at t applied to w: a template is inserted at t + horizon with final horizon, a cmd_vel row fills row[0:4], an ee_cmd_vel row
-// row[0:3], a goal row row[0:7]; wrote grows to the longest prefix written, applied becomes the row's target command.  QMB200_ST_OVERFLOW (w partly
+// row[0:3], a goal row row[0:7], a path row row[0:1]; wrote grows to the longest prefix written, applied becomes the row's target command.  QMB200_ST_OVERFLOW (w partly
 // written) or 0.
 QMB_HD int gs_apply(GsRobot& w, const GsTemplate* table, int tmpl, const double* vel, int ee_kind, const double* ee, double t, double horizon, double stance_time,
                     double* row, int& wrote, int& applied) {
@@ -105,7 +110,7 @@ QMB_HD int gs_apply(GsRobot& w, const GsTemplate* table, int tmpl, const double*
   }
   if (!isnan(vel[0])) { for (int i = 0; i < 4; ++i) row[i] = vel[i]; wrote = wrote > 4 ? wrote : 4; applied = GS_SRC_CMD_VEL; }
   if (ee_kind >= 0) {
-    const int m = ee_kind == GS_SRC_EE_GOAL ? 7 : 3;
+    const int m = ee_kind == GS_SRC_EE_GOAL ? 7 : ee_kind == GS_SRC_EE_PATH ? 1 : 3;
     for (int i = 0; i < m; ++i) row[i] = ee[i];
     wrote = wrote > m ? wrote : m; applied = ee_kind;
   }
@@ -156,9 +161,10 @@ int launch_gait_step(int B, const GsTemplate* table, GsRobot* robots, int32_t* c
                      int32_t* n_events, double* event_times, int32_t* modes, double* cmd, int32_t* tmpl, int32_t* mode, int32_t* status, int32_t* target_kind,
                      GsPending* pending, cudaStream_t s);
 
-// one thread per robot: a masked robot's row (tmpl [B], vel [B][4], ee_kind [B], ee [B][7]) that passes gs_command_check overwrites its pending slot;
-// status [B] = that check's word for masked robots, 0 for the others, whose slots are not written
-int launch_gait_command(int B, int n_templates, GsPending* pending, const int32_t* mask, const int32_t* tmpl, const double* vel, const int32_t* ee_kind,
+// one thread per robot: a masked robot's row (tmpl [B], vel [B][4], ee_kind [B], ee [B][7]) that passes gs_command_check (on n_templates templates
+// and n_paths end-effector paths) overwrites its pending slot; status [B] = that check's word for masked robots, 0 for the others, whose slots are not
+// written
+int launch_gait_command(int B, int n_templates, int n_paths, GsPending* pending, const int32_t* mask, const int32_t* tmpl, const double* vel, const int32_t* ee_kind,
                         const double* ee, int32_t* status, cudaStream_t s);
 
 }  // namespace qmb

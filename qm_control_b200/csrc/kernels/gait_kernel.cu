@@ -23,7 +23,7 @@ __global__ void __launch_bounds__(GS_THREADS) gait_step_kernel(int B, const GsTe
   if (mode) mode[b] = gs_mode_at(robots[b].s, t);
 }
 
-__global__ void __launch_bounds__(GS_THREADS) gait_command_kernel(int B, int n_templates, GsPending* __restrict__ pending, const int32_t* __restrict__ mask,
+__global__ void __launch_bounds__(GS_THREADS) gait_command_kernel(int B, int n_templates, int n_paths, GsPending* __restrict__ pending, const int32_t* __restrict__ mask,
                                                                    const int32_t* __restrict__ tmpl, const double* __restrict__ vel,
                                                                    const int32_t* __restrict__ ee_kind, const double* __restrict__ ee, int32_t* __restrict__ status) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -35,7 +35,7 @@ __global__ void __launch_bounds__(GS_THREADS) gait_command_kernel(int B, int n_t
 #pragma unroll
   for (int i = 0; i < 7; ++i) e[i] = ee[(size_t)b * 7 + i];
   const int tm = tmpl[b], kind = ee_kind[b];
-  const int st = gs_command_check(tm, v, kind, e, n_templates);
+  const int st = gs_command_check(tm, v, kind, e, n_templates, n_paths);
   status[b] = st;
   if (st) return;
   GsPending& p = pending[b];
@@ -56,9 +56,9 @@ int launch_gait_step(int B, const GsTemplate* table, GsRobot* robots, int32_t* c
   return 1;
 }
 
-int launch_gait_command(int B, int n_templates, GsPending* pending, const int32_t* mask, const int32_t* tmpl, const double* vel, const int32_t* ee_kind,
+int launch_gait_command(int B, int n_templates, int n_paths, GsPending* pending, const int32_t* mask, const int32_t* tmpl, const double* vel, const int32_t* ee_kind,
                         const double* ee, int32_t* status, cudaStream_t s) {
-  gait_command_kernel<<<(B + GS_THREADS - 1) / GS_THREADS, GS_THREADS, 0, s>>>(B, n_templates, pending, mask, tmpl, vel, ee_kind, ee, status);
+  gait_command_kernel<<<(B + GS_THREADS - 1) / GS_THREADS, GS_THREADS, 0, s>>>(B, n_templates, n_paths, pending, mask, tmpl, vel, ee_kind, ee, status);
   return 1;
 }
 

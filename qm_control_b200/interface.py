@@ -287,6 +287,41 @@ class Solver:
         self._call("get_ee_frame", _p(rows), C.byref(is_set))
         return rows if is_set.value else None
 
+    def set_ee_paths(self, paths=None):
+        """The end-effector path table (DESIGN.md §4.20): paths, a list of (t [n], pose [n, 7]) with t the waypoint times in seconds after the path
+        starts (t[0] > 0, gaps >= time_horizon / 2) and pose the waypoints (position, quaternion xyzw of unit norm), 1 <= n <= _lib.EE_PATH_MAX; None
+        or [] clears it.  The library rejects a malformed table, naming the path and the waypoint, and writes nothing.  Synchronous."""
+        if not paths:
+            self._call("set_ee_paths", 0, None, None); return
+        n_way = np.zeros(len(paths), dtype=np.int32); way = np.zeros((len(paths), _lib.EE_PATH_MAX, 8))
+        for p, (t, pose) in enumerate(paths):
+            t = np.asarray(t, dtype=np.float64).reshape(-1); pose = np.asarray(pose, dtype=np.float64)
+            if pose.shape != (len(t), 7) or not 1 <= len(t) <= _lib.EE_PATH_MAX:
+                raise ValueError("set_ee_paths: path %d must be (t [n], pose [n, 7]) with 1 <= n <= %d, got shapes %s and %s" % (p, _lib.EE_PATH_MAX, t.shape, pose.shape))
+            n_way[p] = len(t); way[p, :len(t), 0] = t; way[p, :len(t), 1:] = pose
+        self._call("set_ee_paths", len(paths), _p(n_way), _p(way))
+
+    def get_ee_paths(self):
+        """→ the path table as set_ee_paths takes it (a list of (t [n], pose [n, 7])), or None when none is set."""
+        n = C.c_int32(); self._call("get_ee_paths", C.byref(n), None, None)
+        if n.value == 0:
+            return None
+        n_way = np.zeros(n.value, dtype=np.int32); way = np.zeros((n.value, _lib.EE_PATH_MAX, 8))
+        self._call("get_ee_paths", None, _p(n_way), _p(way))
+        return [(way[p, :k, 0].copy(), way[p, :k, 1:].copy()) for p, k in enumerate(n_way)]
+
+    def target_trajectories_path(self, kind, cmd, t_obs, x_obs, ee_state, last_ee_target, path_state, target=None):
+        """qmb200_target_trajectories_path: target_trajectories with per-robot kinds [B] that may also be _lib.TARGET_EE_PATH (cmd[b, 0] the path index)
+        or _lib.TARGET_EE_PATH_FOLLOW, on path_state [B, EE_PATH_STATE] → (n_target, target_times, target_states, last_ee_target, path_state)."""
+        B = self.batch; c = np.zeros((B, 7)); cmd = np.asarray(cmd, dtype=np.float64).reshape(B, -1); c[:, :cmd.shape[1]] = cmd
+        le = _f64(last_ee_target, (B, 7)).copy(); ps = _f64(path_state, (B, _lib.EE_PATH_STATE)).copy()
+        nt, tt, ts = np.zeros(B, dtype=np.int32), np.zeros((B, KMAX)), np.zeros((B, KMAX, TARGET))
+        if target is not None:
+            nt, tt, ts = _i32(target[0], (B,)).copy(), _f64(target[1], (B, KMAX)).copy(), _f64(target[2], (B, KMAX, TARGET)).copy()
+        self._call("target_trajectories_path", _p(_i32(kind, (B,))), _p(c), _p(_f64(t_obs, (B,))), _p(_f64(x_obs, (B, NX))), _p(_f64(ee_state, (B, 7))), _p(le), _p(ps),
+                   _p(nt), _p(tt), _p(ts))
+        return nt, tt, ts, le, ps
+
     def set_arm_gains(self, kp, kd):
         self._call("set_arm_gains", float(kp), float(kd))
 
@@ -313,10 +348,16 @@ class Solver:
         return t, x, jc, ap, lt, cmd, st
 
     # device-pointer variants of the controller side (torch-cuda tensors, no synchronisation)
-    def target_trajectories_dev(self, kind, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, stream=None):
+    def target_trajectories_dev(self, kind, cmd, t_obs, x_obs, ee_state, last_ee_target, n_target, target_times, target_states, stream=None, path_state=None):
         """kind: one kind for every robot, or an int32 [B] device tensor of per-robot kinds (qmb200_target_trajectories_per_robot_dev; a robot whose
-        kind lies outside [0, 2], -1 for a held goal, is left untouched)."""
-        if not hasattr(kind, "data_ptr"):
+        kind lies outside [0, 2], -1 for a held goal, is left untouched).  path_state: a [B, EE_PATH_STATE] float64 device tensor (in-out) with per-robot
+        kinds: qmb200_target_trajectories_path_dev, where the kinds may also start or follow an end-effector path (DESIGN.md §4.20)."""
+        if path_state is not None:
+            if not hasattr(kind, "data_ptr"):
+                raise ValueError("target_trajectories_dev: path_state needs per-robot kinds (an int32 [B] device tensor), got kind=%r" % (kind,))
+            self._call("target_trajectories_path_dev", _p(kind), _p(cmd), _p(t_obs), _p(x_obs), _p(ee_state), _p(last_ee_target), _p(path_state), _p(n_target),
+                       _p(target_times), _p(target_states), stream)
+        elif not hasattr(kind, "data_ptr"):
             self._call("target_trajectories_dev", int(kind), _p(cmd), _p(t_obs), _p(x_obs), _p(ee_state), _p(last_ee_target), _p(n_target), _p(target_times), _p(target_states), stream)
         else:
             self._call("target_trajectories_per_robot_dev", _p(kind), _p(cmd), _p(t_obs), _p(x_obs), _p(ee_state), _p(last_ee_target), _p(n_target), _p(target_times),
@@ -1026,8 +1067,9 @@ class Solver:
 
     def gait_dev_set_commands(self, t, tmpl, cmd_vel, ee_kind=None, ee_cmd=None):
         """The command timeline: t [B, C] (sorted per robot, +inf pads), tmpl [B, C] (ids, -1: none), cmd_vel [B, C, 4] (NaN rows: none), and optionally
-        end-effector commands (DESIGN.md §4.8): ee_kind [B, C] (-1: none, 1: ee_cmd_vel, 2: goal) with ee_cmd [B, C, 7] (ee_cmd_vel: vx, vy, vz, the rest
-        ignored; goal: position, quaternion xyzw; world frame).  Every cursor goes back to 0.  Synchronous."""
+        end-effector commands (DESIGN.md §4.8): ee_kind [B, C] (-1: none, 1: ee_cmd_vel, 2: goal, 3: path) with ee_cmd [B, C, 7] (ee_cmd_vel: vx, vy, vz,
+        the rest ignored; goal: position, quaternion xyzw; world frame; path: ee_cmd[..., 0] an index of the path table, set_ee_paths).  Every cursor goes
+        back to 0.  Synchronous."""
         B = self.batch; t = _f64(t); n = t.shape[1] if t.ndim == 2 else -1
         t = _f64(t, (B, n)); tmpl = _i32(tmpl, (B, n)); cmd_vel = _f64(cmd_vel, (B, n, 4))
         if ee_kind is None and ee_cmd is None:

@@ -384,6 +384,71 @@ def target_call_times(solver, reps=7, calls=50):
             **{"ms_per_call_" + k: float(np.median(v)) for k, v in times.items()}, "spread_per_robot": [float(min(times["per_robot"])), float(max(times["per_robot"]))]}
 
 
+def ee_paths_main(args, duration=4.0, t_first=0.5, gap=0.75):
+    """End-effector paths (DESIGN.md §4.20): the target call of the whole batch without path robots (kinds 0 / 1 / 2 / -1 mixed, the per-robot call)
+    and with every robot following a path (the path call), alternated blocks of CUDA events, medians; then every robot standing in the heading frame
+    traces a 10 cm square (4 waypoints gap s apart from t_first, from the standing hand's pose at t_first, read from a first run of t_first s): the
+    hand's position error against p(t) between the first and the last waypoint and at the end (the final waypoint held), p50 / p95, and the wall
+    seconds per simulated second of the same loop with and without the path."""
+    import time
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("no CUDA device: this benchmark measures the GPU and has no CPU fallback")
+    B = args.batch; solver = q.Solver(batch=B, device=0); dev = torch.device("cuda", 0); st = torch.cuda.Stream(device=dev); rng = np.random.default_rng(0)
+    f64 = lambda a: torch.as_tensor(np.ascontiguousarray(a, dtype=np.float64), device=dev)
+    xy = np.c_[np.arange(B) * 2.0, np.zeros(B), np.zeros(B)]
+    r = closed_loop.run(solver, duration=t_first, gait="stance", xy_yaw=xy, ee_frame="heading")
+    hand = np.r_[r["ee"][-1, 0, :2] - r["base"][-1, 0, :2], r["ee"][-1, 0, 2:7]]   # robot 0's standing hand relative to its base (yaw 0)
+    corners = hand[:3] + np.array([[0.1, 0, 0], [0.1, 0.1, 0], [0, 0.1, 0], [0, 0, 0]])
+    tau = gap * np.arange(1, 5); paths = [(tau, np.c_[corners, np.tile(hand[3:7], (4, 1))])]
+    solver.set_ee_paths(paths)
+    cmd = np.zeros((B, 7)); cmd[:, :3] = [0.6, 0.1, 0.45]; cmd[:, 3:] = [0.5, -0.5, 0.5, -0.5]
+    x = np.zeros((B, 30)); x[:, 8] = 0.45; x[:, 9] = rng.uniform(-np.pi, np.pi, B); ee = np.tile([0.52, 0.09, 0.44, 0.5, -0.5, 0.5, -0.5], (B, 1))
+    ps = np.zeros((B, _lib.EE_PATH_STATE)); ps[:, 1] = 10.0 - rng.uniform(0.0, 3.0, B); ps[:, 4] = x[:, 9]; ps[:, 5:] = ee
+    rows = [f64(cmd), f64(np.full(B, 10.0)), f64(x), f64(ee), f64(ee), torch.zeros(B, dtype=torch.int32, device=dev), torch.zeros((B, 4), dtype=torch.float64, device=dev),
+            torch.zeros((B, 4, 37), dtype=torch.float64, device=dev)]
+    settings = {"no_path_robots": (torch.as_tensor(rng.integers(-1, 3, B).astype(np.int32), device=dev), None),
+                "every_robot_following": (torch.full((B,), _lib.TARGET_EE_PATH_FOLLOW, dtype=torch.int32, device=dev), f64(ps))}
+    times = {k: [] for k in settings}; reps, calls = 7, 50
+    for rep in range(reps + 1):   # the first round warms up
+        for name, (kind, path_state) in settings.items():
+            kw = {} if path_state is None else dict(path_state=path_state)
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(st)
+            for _ in range(calls):
+                solver.target_trajectories_dev(kind, *rows, st.cuda_stream, **kw)
+            b.record(st); torch.cuda.synchronize(dev)
+            if rep:
+                times[name].append(a.elapsed_time(b) / calls)
+    solver.set_ee_paths(None)
+    out = {"card": card(), "target_call": {"label": "device ms per target call of %d robots, median of %d alternated blocks of %d calls" % (B, reps, calls),
+                                           **{k: float(np.median(v)) for k, v in times.items()}}}
+    wall = {}
+    for name, kw in (("without_path", dict(steer=True)),
+                     ("with_path", dict(ee_paths=paths, commands=dict(t=np.full((B, 1), t_first), gait=[[None]] * B, ee_path=np.zeros((B, 1), dtype=np.int64))))):
+        solver.mpc_reset(); solver.wbc_set_input_last(None)
+        with closed_loop.Session(solver, duration, gait="stance", xy_yaw=xy, ee_frame="heading", **kw) as ss:
+            torch.cuda.synchronize(dev); t0 = time.perf_counter()
+            rec = ss.step(ss.windows); ss.stream.synchronize(); wall[name] = (time.perf_counter() - t0) / duration
+            rec = {k: (v if isinstance(v, np.ndarray) else v.cpu().numpy()) for k, v in rec.items()}
+            p = ss.path_state.cpu().numpy() if ss.path_state is not None else None
+            ss.finish()
+    t = rec["t"]; ref = np.zeros((len(t), B, 3))
+    for c in range(3):
+        ref[..., c] = np.interp(t[:, None] - p[None, :, 1], tau, paths[0][1][:, c])
+    cs, sn = np.cos(p[:, 4]), np.sin(p[:, 4])
+    world = np.stack([cs * ref[..., 0] - sn * ref[..., 1] + p[:, 2], sn * ref[..., 0] + cs * ref[..., 1] + p[:, 3], ref[..., 2]], -1)
+    err = np.linalg.norm(rec["ee"][..., :3] - world, axis=-1) * 1e3
+    along = (t[:, None] >= p[None, :, 1] + tau[0]) & (t[:, None] <= p[None, :, 1] + tau[-1])
+    base = rec["base"]; up = np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3)
+    out["square"] = {"robots": B, "frame": "heading", "side_m": 0.1, "gap_s": gap, "fallen": int(np.sum(~up)), "status_robots": int(np.sum(np.any(rec["status"] != 0, axis=0))),
+                     "along_path_mm_p50_p95": [float(v) for v in np.percentile(err[along], [50, 95])],
+                     "final_waypoint_mm_p50_p95": [float(v) for v in np.percentile(err[-1], [50, 95])],
+                     "wall_s_per_sim_s": wall}
+    print(json.dumps(out))
+
+
 def ee_frame_main(args, sweep_s=4.0):
     """End-effector targets in the heading frame (DESIGN.md §4.19): the target call of the whole batch (kinds 0 / 1 / 2 / -1 mixed) with no frame rows,
     all-world rows and all-heading rows, alternated blocks of CUDA events, medians; then the turning sweep (start yaws over [-pi, pi], yaw rates
@@ -1336,12 +1401,16 @@ def main():
                     "session branching every robot every window against one without restores")
     ap.add_argument("--session", action="store_true", help="closed_loop.run against a Session stepped one window at a time, without commands and with a "
                                                            "torch heading controller's command every window: wall time per simulated second, the command kernel's time")
+    ap.add_argument("--ee-paths", action="store_true", help="end-effector paths: the target call's time with and without path robots, and a 10 cm square "
+                    "traced by every robot standing: hand error along the path and at the final waypoint, wall time with and without the path")
     ap.add_argument("--ee-frame", action="store_true", help="end-effector targets in the heading frame: the target call's time with no, all-world and all-heading "
                                                             "frame rows, and a turning sweep over start yaws and yaw rates in both frames; with --respawn: "
                                                             "that run with every robot's targets in its heading frame")
     args = ap.parse_args()
     if args.ee_frame and not args.respawn:
         return ee_frame_main(args)
+    if args.ee_paths:
+        return ee_paths_main(args)
     if args.session:
         return session_main(args)
     if args.snapshot:
