@@ -878,12 +878,53 @@ int qmb200_timeline_sample_dev(qmb200_handle* h, const int32_t* mask, const int3
  * sampler draws. */
 int qmb200_timeline_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, double* rows /*[n][n_cmd][QMB200_TIMELINE_CMD]*/);
 
+/* ---- per-episode end-effector paths (DESIGN.md §4.21): each episode of each robot gets a new end-effector path, drawn on the device right after its
+ *      restart into a row of the path table that belongs to the robot, and a pending start of that row (qmb200_gait_dev_command's slot), so that the
+ *      path starts on the episode's first MPC tick, after any timeline command due on that tick.
+ *   ranges row[QMB200_EE_PATH_RANGES]  0      n_way        waypoint count; fixed (lo == hi), an integer in [1, QMB200_EE_PATH_MAX]
+ *                                      1      tau_first    waypoint 0's time after the path starts (s), lo > 0
+ *                                      2      gap          time from waypoint i - 1 to waypoint i (s), lo >= T/2 (T the MPC time horizon, as the table's);
+ *                                                          tau_first hi + (n_way - 1) gap hi <= 1e300, so that every drawn time is finite
+ *                                      3-5    x, y, z      waypoint position in the path's frame (the heading frame at the start for a heading-frame
+ *                                                          robot, the world frame otherwise: a table path's frame)
+ *                                      6      yaw          turn of the hand about that frame's z axis, bounds in [-pi, pi]
+ *                                      7-10   qx, qy, qz, qw   the quaternion it turns; fixed, unit norm within 1e-9
+ *   drawn waypoint i  (tau, x, y, z, quaternion xyzw): a row of the path table (qmb200_set_ee_paths' layout).  tau_0 = draw(tau_first), tau_i =
+ *                     tau_{i-1} + draw(gap), rounded up where the nearest rounding would leave tau_i - tau_{i-1} under the gap; the position the box drawn per waypoint; the quaternion Rz(draw(yaw)) quat, its half-angle sine and cosine
+ *                     from Taylor polynomials in single roundings, so that host and device agree bit for bit.
+ * Every draw of waypoint i is u = the keyed uniform of the episode draws on a domain constant of its own over (seed, global robot rank * B + b, e, 8 i + c):
+ * c = 0 the time, 1-3 the position, 4 the yaw.  A box column is fma(u, hi - lo, lo), a fixed column lo itself, byte for byte.  Every drawn row passes
+ * qmb200_set_ee_paths' check.
+ * While ranges are set the device path table holds the P paths of qmb200_set_ee_paths followed by B drawn rows: robot b's is row P + b, an ordinary table
+ * index of qmb200_target_trajectories_path.  qmb200_get_ee_paths reports the P paths only, qmb200_set_ee_paths refuses, and commands
+ * (qmb200_gait_dev_command, timelines) may still start the P paths only. */
+#define QMB200_EE_PATH_RANGES 11
+/* Per-robot ranges lo, hi [B][QMB200_EE_PATH_RANGES] and the seed; allocates the B drawn rows of the path table.  NULL lo and hi clear them (the table
+ * is the P paths again).  Rejects a non-finite bound, lo > hi, a non-finite hi - lo and the column rules above, naming the field and the robot; on
+ * rejection the stored ranges stay unchanged.  Refused while a curriculum is attached to them.  Host arrays; synchronous. */
+int qmb200_ee_path_set_ranges(qmb200_handle* h, const double* lo /*[B][QMB200_EE_PATH_RANGES] or NULL*/, const double* hi /*[B][QMB200_EE_PATH_RANGES] or NULL*/,
+                              int64_t seed);
+/* The stored ranges and seed (zeros when none are set); is_set = 1 when ranges are set.  Any output may be NULL. */
+int qmb200_ee_path_get_ranges(const qmb200_handle* h, double* lo /*[B][QMB200_EE_PATH_RANGES]*/, double* hi /*[B][QMB200_EE_PATH_RANGES]*/, int64_t* seed,
+                              int32_t* is_set);
+/* One launch, no host work: every robot with mask[b] != 0 draws episode[b]'s path into rows[b][0:n_way] and into table row P + b (the waypoints past
+ * n_way are not written: no target call reads them), and sets its pending slot to the row qmb200_gait_dev_command writes for (tmpl -1, cmd_vel the quiet NaN, ee_kind QMB200_TARGET_EE_PATH, ee (P + b, 0, ..., 0)).
+ * Robots with mask[b] == 0 are not written.  Fails, writing nothing, when no ranges are set or the device gait schedule is not running (its pending
+ * slots exist exactly while it runs). */
+int qmb200_ee_path_sample(qmb200_handle* h, const int32_t* mask /*[B]*/, const int32_t* episode /*[B]*/, double* rows /*[B][QMB200_EE_PATH_MAX][8] in-out*/);
+int qmb200_ee_path_sample_dev(qmb200_handle* h, const int32_t* mask, const int32_t* episode, double* rows, void* cuda_stream);
+/* Host only: the paths of robots robot[n] (in [0, B)) in episodes episode[n] on the stored ranges and seed, what the sampler draws: n_way [n] and way
+ * [n][QMB200_EE_PATH_MAX][8] (zeros past n_way). */
+int qmb200_ee_path_draw(const qmb200_handle* h, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/, int32_t* n_way /*[n]*/,
+                        double* way /*[n][QMB200_EE_PATH_MAX][8]*/);
+
 /* ---- per-robot curricula (DESIGN.md §4.15): each robot has a level in [0, n_levels) that places the ranges of every attached draw kind (episode,
- *      spawn, timeline) on the line from an easy box (level 0, the kind's ranges when attached) to a hard box (level n_levels - 1).  When a robot's
+ *      spawn, timeline, ee path) on the line from an easy box (level 0, the kind's ranges when attached) to a hard box (level n_levels - 1).  When a robot's
  *      episode closes, a device update steps its level from the episode's end code and, optionally, its metrics row, and writes the box of the new level
  *      into the kinds' device ranges, which the unchanged samplers then draw the next episode from.
  *   box at level l, f = l / (n_levels - 1), per column of lo and of hi: base at l = 0, top at l = n_levels - 1, base where base == top, else
- *                                fma(f, top - base, base); the spawn's tile column then floor(x + 0.5).  The timeline's gait_set and ee_q* must be equal at both ends.
+ *                                fma(f, top - base, base); the spawn's tile column then floor(x + 0.5).  The timeline's gait_set and ee_q* and the ee path's n_way and
+ *                                q* must be equal at both ends.
  *   row[QMB200_CURRICULUM]        0 start_level (an integer in [0, n_levels)), 1 up_after, 2 down_after (integers >= 1), 3-6 threshold[4] (finite)
  *   state[QMB200_CURRICULUM_STATE]  int32: level, pass_run, fail_run, n_updates
  *   rule: n_levels >= 2 and n_cond <= QMB200_CURRICULUM_MAX_COND conditions; condition i compares the closed episode's metrics column column[i]
@@ -895,9 +936,10 @@ int qmb200_timeline_draw(const qmb200_handle* h, int32_t n, const int32_t* robot
 #define QMB200_CURRICULUM 7
 #define QMB200_CURRICULUM_STATE 4
 #define QMB200_CURRICULUM_MAX_COND 4
-#define QMB200_CURRICULUM_EPISODE 0    /* kinds: the ranges of qmb200_episode_set_ranges, qmb200_spawn_set_ranges, qmb200_timeline_set_ranges */
-#define QMB200_CURRICULUM_SPAWN 1
+#define QMB200_CURRICULUM_EPISODE 0    /* kinds: the ranges of qmb200_episode_set_ranges, qmb200_spawn_set_ranges, qmb200_timeline_set_ranges, */
+#define QMB200_CURRICULUM_SPAWN 1      /* qmb200_ee_path_set_ranges */
 #define QMB200_CURRICULUM_TIMELINE 2
+#define QMB200_CURRICULUM_EE_PATH 3
 #define QMB200_CURRICULUM_GE 0
 #define QMB200_CURRICULUM_LE 1
 #define QMB200_CURRICULUM_PASS 0
@@ -911,7 +953,7 @@ typedef struct qmb200_curriculum_rule {
  * the kind is detached.  Host arrays; synchronous. */
 int qmb200_curriculum_set(qmb200_handle* h, const qmb200_curriculum_rule* rule, const double* rows /*[B][QMB200_CURRICULUM] or NULL*/);
 /* Attaches kind (QMB200_CURRICULUM_*): its ranges in force become level 0, lo_top / hi_top [B][width] level n_levels - 1.  Every level's box must pass the
- * kind's own range check (the spawn's against the tile library in force); the first failure is named with its level, field and robot, and nothing is
+ * kind's own range check (the spawn's against the tile library in force, the ee path's at the handle's T); the first failure is named with its level, field and robot, and nothing is
  * written.  Then each robot's box at its level is written into the kind's ranges.  While attached, the kind's *_set_ranges refuses.  Synchronous. */
 int qmb200_curriculum_attach(qmb200_handle* h, int32_t kind, const double* lo_top /*[B][width]*/, const double* hi_top /*[B][width]*/);
 /* One launch, no host work: every robot with mask[b] != 0 and end[b] in {1, 2} updates its state from end[b] and, when the rule has conditions, the closed
@@ -928,7 +970,8 @@ int qmb200_curriculum_update_dev(qmb200_handle* h, const int32_t* mask, const in
  * may be NULL. */
 int qmb200_curriculum_get(const qmb200_handle* h, int32_t* state /*[B][QMB200_CURRICULUM_STATE]*/, int32_t* is_set);
 /* Host only: the rows of attached kind that its sampler draws for robots robot[n] in episodes episode[n] at levels level[n] (in [0, n_levels)): the
- * kind's *_draw on the box at that level, [n][QMB200_EPISODE], [n][QMB200_SPAWN] or [n][n_cmd][QMB200_TIMELINE_CMD]. */
+ * kind's *_draw on the box at that level, [n][QMB200_EPISODE], [n][QMB200_SPAWN], [n][n_cmd][QMB200_TIMELINE_CMD] or, for the ee path,
+ * [n][1 + QMB200_EE_PATH_MAX * 8]: n_way (as a double), then the waypoints (zeros past n_way). */
 int qmb200_curriculum_draw(const qmb200_handle* h, int32_t kind, int32_t n, const int32_t* robot /*[n]*/, const int32_t* episode /*[n]*/,
                            const int32_t* level /*[n]*/, double* rows);
 

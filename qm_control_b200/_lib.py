@@ -114,6 +114,10 @@ TIMELINE_LAYOUT = ("t_first", "gap", "p_gait", "gait_set", "w_none", "w_cmd_vel"
 TIMELINE = len(TIMELINE_LAYOUT)   # QMB200_TIMELINE
 TIMELINE_CMD_LAYOUT = ("t", "tmpl", "cmd_vel_x", "cmd_vel_y", "cmd_vel_z", "cmd_yaw_rate", "ee_kind") + tuple("ee_%d" % i for i in range(7))
 TIMELINE_CMD = len(TIMELINE_CMD_LAYOUT)   # QMB200_TIMELINE_CMD
+# one episode's end-effector path (qmb200_ee_path_*): the columns of a ranges row of EE_PATH_RANGES doubles; a drawn path is a row of the path table
+# (qmb200_set_ee_paths): EE_PATH_MAX waypoints of (tau, x, y, z, qx, qy, qz, qw), zeros past its n_way
+EE_PATH_RANGES_LAYOUT = ("n_way", "tau_first", "gap", "x", "y", "z", "yaw", "qx", "qy", "qz", "qw")
+EE_PATH_RANGES = len(EE_PATH_RANGES_LAYOUT)   # QMB200_EE_PATH_RANGES
 # a robot's curriculum (qmb200_curriculum_*): the columns of its row of CURRICULUM doubles and of its state of CURRICULUM_STATE int32, the kinds a
 # curriculum attaches to, and a rule's condition ops and roles by their codes
 CURRICULUM_LAYOUT = ("start_level", "up_after", "down_after", "threshold_0", "threshold_1", "threshold_2", "threshold_3")
@@ -121,7 +125,7 @@ CURRICULUM = len(CURRICULUM_LAYOUT)   # QMB200_CURRICULUM
 CURRICULUM_STATE_LAYOUT = ("level", "pass_run", "fail_run", "n_updates")
 CURRICULUM_STATE = len(CURRICULUM_STATE_LAYOUT)   # QMB200_CURRICULUM_STATE
 CURRICULUM_MAX_COND = 4   # QMB200_CURRICULUM_MAX_COND
-CURRICULUM_KINDS = ("episode", "spawn", "timeline")   # QMB200_CURRICULUM_EPISODE, _SPAWN, _TIMELINE
+CURRICULUM_KINDS = ("episode", "spawn", "timeline", "ee_path")   # QMB200_CURRICULUM_EPISODE, _SPAWN, _TIMELINE, _EE_PATH
 CURRICULUM_OPS = (">=", "<=")         # QMB200_CURRICULUM_GE, _LE
 CURRICULUM_ROLES = ("pass", "fail")   # QMB200_CURRICULUM_PASS, _FAIL
 
@@ -297,6 +301,11 @@ PROTOTYPES = {
     "qmb200_timeline_sample": (I32, [P] * 4),
     "qmb200_timeline_sample_dev": (I32, [P] * 5),
     "qmb200_timeline_draw": (I32, [P, I32, P, P, P]),
+    "qmb200_ee_path_set_ranges": (I32, [P, P, P, I64]),
+    "qmb200_ee_path_get_ranges": (I32, [P] * 5),
+    "qmb200_ee_path_sample": (I32, [P] * 4),
+    "qmb200_ee_path_sample_dev": (I32, [P] * 5),
+    "qmb200_ee_path_draw": (I32, [P, I32] + [P] * 4),
     "qmb200_curriculum_set": (I32, [P] * 3),
     "qmb200_curriculum_attach": (I32, [P, I32, P, P]),
     "qmb200_curriculum_update": (I32, [P] * 5 + [I32] + [P] * 2),

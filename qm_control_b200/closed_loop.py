@@ -56,7 +56,7 @@ def _schedules(gait, B, t_start, t_obs0, t_end):
 def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None,
         friction_mu=None, payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None,
         attitude_filter=None, slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None,
-        timeline=None, curriculum=None, ee_frame=None, ee_paths=None):
+        timeline=None, curriculum=None, ee_frame=None, ee_paths=None, ee_path_draw=None):
     """Run `duration` s of closed loop for all solver.batch robots.
 
     gait: a gait.info template name ("stance", "trot", ...), or a sequence of B names, started at t_start; cmd_vel: (vx, vy, vz, yaw rate) in the
@@ -191,14 +191,25 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
     quaternion xyzw of unit norm; in the heading frame at the path's start for a heading-frame robot).  commands ee_path [B, C] (path ids, -1: none) and
     Session.command(ee_path=[B]) start a path: the hand then follows the piecewise lerp / slerp from its pose at the start through the waypoints on
     their schedule, and holds the last one.  Path commands to world-frame robots share the refusals of ee_goal / ee_cmd_vel.  The previous table is
-    restored when run returns; without ee_paths the loop makes exactly the calls it made before."""
+    restored when run returns; without ee_paths the loop makes exactly the calls it made before.
+    ee_path_draw: dict(seed=0, n, tau_first=(lo, hi), gap=(lo, hi), x=(lo, hi), y=(lo, hi), z=(lo, hi), yaw=(lo, hi), quat) draws a new end-effector path
+    of n waypoints for every episode (DESIGN.md §4.21): waypoint 0 at tau_first s after the episode's first MPC tick, each next one gap later (gap lo >=
+    time_horizon / 2), each at a position drawn in the box x, y, z and oriented Rz(draw(yaw)) quat (yaw in [-pi, pi], quat xyzw of unit norm), stated in
+    the path's frame as ee_paths' waypoints are.  Every bound is a scalar or [B].  It rolls the device gait schedule (as commands and timeline do, with
+    or without them and with or without ee_paths): every episode, the first included, draws its path on the device last in its beginning, after its
+    restore, its randomize draw, its spawn and its timeline draw (Solver.ee_path_sample_dev), into its own row of the path table, and the path starts on
+    the episode's first MPC tick.  World-frame robots cannot go with a drawn spawn yaw or restarts "here".  The previous ranges are cleared when run
+    returns, before the ee_paths table is restored.  Returns also ee_path_params[B, E, n, 8], the waypoints (tau in s after the episode's start,
+    position, quaternion xyzw) of every episode's path (NaN where a robot had no episode e): each robot's own draw, so a robot a Session branched
+    from robot s (restore with source) shows its draw while it follows s's path, row P + s; a curriculum may attach it as ee_path_draw=dict(<box>=(lo,
+    hi)).  Without ee_path_draw the loop makes exactly the calls it made before."""
     if isinstance(respawn, dict) and _place_spec(respawn)["on_request"]:
         raise ValueError("closed_loop.run: respawn on_request needs a Session (nothing can request a restart inside run; Session.respawn does)")
     with Session(solver, duration, gait=gait, cmd_vel=cmd_vel, wbc_period_ms=wbc_period_ms, xy_yaw=xy_yaw, t_start=t_start, torch_device=torch_device,
                  sim_timer=sim_timer, friction_mu=friction_mu, payload=payload, pushes=pushes, model_payload=model_payload, terrain=terrain,
                  payload_estimator=payload_estimator, state_estimator=state_estimator, sensor_noise=sensor_noise, attitude_filter=attitude_filter,
                  slip_detector=slip_detector, ground_map=ground_map, commands=commands, tuning=tuning, respawn=respawn, randomize=randomize, spawn=spawn,
-                 metrics=metrics, timeline=timeline, curriculum=curriculum, ee_frame=ee_frame, ee_paths=ee_paths) as s:
+                 metrics=metrics, timeline=timeline, curriculum=curriculum, ee_frame=ee_frame, ee_paths=ee_paths, ee_path_draw=ee_path_draw) as s:
         rec = s.step(s.windows)
         end = s.finish()   # synchronises the session's stream
         out = {k: v if isinstance(v, np.ndarray) else v.cpu().numpy() for k, v in rec.items()}
@@ -209,7 +220,7 @@ def run(solver, duration=1.0, gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_p
 RUN_DEFAULTS = dict(gait="stance", cmd_vel=(0.0, 0.0, 0.0, 0.0), wbc_period_ms=2, xy_yaw=None, t_start=T_START, torch_device=None, sim_timer=None, friction_mu=None,
                     payload=None, pushes=None, model_payload=None, terrain=None, payload_estimator=None, state_estimator=None, sensor_noise=None, attitude_filter=None,
                     slip_detector=None, ground_map=None, commands=None, tuning=None, respawn=None, randomize=None, spawn=None, metrics=None, timeline=None, curriculum=None,
-                    ee_frame=None, ee_paths=None)
+                    ee_frame=None, ee_paths=None, ee_path_draw=None)
 
 
 def _run_specs(solver, steer, o):
@@ -221,6 +232,7 @@ def _run_specs(solver, steer, o):
     ef = _ee_frame_spec(getattr(solver, "batch", None), o["ee_frame"])
     world = True if ef is None else ef == _lib.EE_FRAME_WORLD   # the robots whose end-effector targets assume they face +x
     ep = _ee_paths_spec(getattr(solver, "time_horizon", None), o["ee_paths"])
+    pd = None if o["ee_path_draw"] is None else _ee_path_draw_spec(getattr(solver, "batch", None), getattr(solver, "time_horizon", None), o["ee_path_draw"])
     if metrics is not None and metrics is not True:
         raise ValueError("closed_loop.run: metrics must be None or True, got %r" % (metrics,))
     rs = None if respawn is None else dict(_respawn_spec(respawn), **_place_spec(respawn))
@@ -248,19 +260,22 @@ def _run_specs(solver, steer, o):
     if slip_detector is not None and state_estimator is None:
         raise ValueError("closed_loop.run: slip_detector needs state_estimator (it chooses the stance feet the estimator trusts)")
     gd = None if commands is None else _gait_commands(solver.batch, gait, commands, 0 if ep is None else len(ep))
-    if steer and commands is None and timeline is None:   # an empty timeline: the session's commands are the schedule's only input
+    if (steer or pd is not None) and commands is None and timeline is None:   # an empty timeline: the session's commands are the schedule's only input
         gd = _gait_commands(solver.batch, gait, dict(t=np.zeros((solver.batch, 0)), gait=np.empty((solver.batch, 0), dtype=object)))
     tl = None if timeline is None else _timeline_spec(getattr(solver, "batch", None), gait, timeline, commands)
     if tl is not None:
         gd = tl["gd"]
+    if pd is not None:
+        gd = _with_paths(gd)
     tn = None if tuning is None else _tuning_spec(solver.batch, tuning)
     sp = None if spawn is None else _spawn_spec(getattr(solver, "batch", None), spawn, terrain, ground_map, gd, world)
     cu = None
     if curriculum is not None:
-        cu = _curriculum_spec(getattr(solver, "batch", None), curriculum, rs, metrics is not None, gait, dict(episode=randomize, spawn=spawn, timeline=timeline),
-                              terrain, ground_map, gd, world)
+        cu = _curriculum_spec(getattr(solver, "batch", None), curriculum, rs, metrics is not None, gait,
+                              dict(episode=randomize, spawn=spawn, timeline=timeline, ee_path=o["ee_path_draw"]), terrain, ground_map, gd, world,
+                              getattr(solver, "time_horizon", None))
         if cu["gd"] is not None:   # a top box that weighs end-effector commands needs the placeholder timeline's end-effector rows
-            gd = tl["gd"] = cu["gd"]
+            gd = tl["gd"] = cu["gd"] if pd is None else _with_paths(cu["gd"])
     if rs is not None and rs["at"] == "here":
         yaw_drawn = sp is not None and "yaw" in sp["fields"] and np.any(sp["fields"]["yaw"][0] != sp["fields"]["yaw"][1])
         why = _here_refusal(yaw_drawn, gd, curriculum, ground_map, world)
@@ -274,7 +289,7 @@ def _run_specs(solver, steer, o):
             rz["link"] |= _lib.EPISODE_MODEL_PAYLOAD
         if tn is not None and "friction_mu" in drawn:
             rz["link"] |= (_lib.EPISODE_MPC_FRICTION if isinstance(tn.get("friction_mu"), str) else 0) | (_lib.EPISODE_WBC_FRICTION if isinstance(tn.get("wbc_friction"), str) else 0)
-    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu, ef=ef, world=world, ep=ep)
+    return dict(rs=rs, rz=rz, gd=gd, tl=tl, tn=tn, sp=sp, cu=cu, ef=ef, world=world, ep=ep, pd=pd)
 
 
 def _respawn_spec(respawn):
@@ -422,7 +437,7 @@ def _spawn_spec(B, spawn, terrain, ground_map, gd, world=True):
 
 @contextlib.contextmanager
 def _ranges(solver, kind):
-    """the ranges of solver's kind ("episode", "spawn" or "timeline") draws in force, set again on exit"""
+    """the ranges of solver's kind ("episode", "spawn", "timeline" or "ee_path") draws in force, set again on exit"""
     prev = getattr(solver, kind + "_get_ranges")()
     try:
         yield   # the session's start sets this run's ranges once it has read its fixed values
@@ -583,14 +598,62 @@ def _timeline_spec(B, gait, timeline, commands):
     return dict(seed=seed, n=int(n), fields=fields, p_gait=p_gait, gait_set=gait_set, weights=weights, quat=quat, gd=gd)
 
 
-CURRICULUM_KINDS = dict(randomize="episode", spawn="spawn", timeline="timeline")   # a curriculum spec's key → the draw kind it attaches to
+EE_PATH_BOX = ("tau_first", "gap", "x", "y", "z", "yaw")
 
 
-def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map, gd, world=True):
+def _ee_path_draw_spec(B, T, spec):
+    """closed_loop.run's ee_path_draw → dict(seed, n, fields: name -> (lo, hi) float arrays, scalar or [B], quat [4] or [B, 4]); ValueError when malformed
+    (the library's rules: DESIGN.md §4.21).  B None: the lengths are not checked; T (the handle's time horizon) None: the T/2 gap rule is left to the
+    library."""
+    keys = ("seed", "n", "quat") + EE_PATH_BOX
+    if not isinstance(spec, dict) or not set(spec) <= set(keys):
+        raise ValueError("closed_loop.run: ee_path_draw must be None or dict(%s), got %r" % (", ".join(keys), spec))
+    n = spec.get("n")
+    if isinstance(n, (bool, np.bool_)) or not isinstance(n, (int, np.integer)) or not 1 <= n <= _lib.EE_PATH_MAX:
+        raise ValueError("closed_loop.run: ee_path_draw n must be an integer in [1, %d], got %r" % (_lib.EE_PATH_MAX, n))
+    seed, fields = _ranges_spec("ee_path_draw", EE_PATH_BOX, B, {k: v for k, v in spec.items() if k not in ("n", "quat")})
+    missing = [k for k in EE_PATH_BOX if k not in fields and k != "yaw"]
+    if missing:
+        raise ValueError("closed_loop.run: ee_path_draw needs %s=(lo, hi)" % missing[0])
+    if not np.all(fields["tau_first"][0] > 0.0):
+        raise ValueError("closed_loop.run: ee_path_draw tau_first lo must be > 0 (seconds after the path starts)")
+    if T is not None and not np.all(fields["gap"][0] >= 0.5 * T):
+        raise ValueError("closed_loop.run: ee_path_draw gap lo must be >= time_horizon / 2 = %g s" % (0.5 * T))
+    if "yaw" in fields and not (np.all(fields["yaw"][0] >= -np.pi) and np.all(fields["yaw"][1] <= np.pi)):
+        raise ValueError("closed_loop.run: ee_path_draw yaw bounds must lie in [-pi, pi]")
+    with np.errstate(over="ignore"):
+        if not np.all(fields["tau_first"][1] + (n - 1) * fields["gap"][1] <= 1e300):
+            raise ValueError("closed_loop.run: ee_path_draw tau_first hi + (n - 1) gap hi must be <= 1e300 s (every drawn time finite)")
+    q = spec.get("quat")
+    quat = np.array(np.nan) if q is None or isinstance(q, (str, bool, np.bool_)) else np.asarray(q, dtype=np.float64)
+    if quat.shape != (4,) and not (quat.ndim == 2 and quat.shape[1] == 4 and (B is None or quat.shape[0] == B)):
+        raise ValueError("closed_loop.run: ee_path_draw quat must be [4] or [%s, 4] (xyzw), got %r" % ("B" if B is None else B, q))
+    if not np.all(np.isfinite(quat)) or np.any(np.abs(np.linalg.norm(quat, axis=-1) - 1.0) > 1e-9):
+        raise ValueError("closed_loop.run: ee_path_draw quat (xyzw) must be finite with unit norm (within 1e-9)")
+    return dict(seed=seed, n=int(n), fields=fields, quat=quat)
+
+
+def _ee_path_box(pd, B):
+    """the ranges lo, hi [B, EE_PATH_RANGES] of a parsed ee_path_draw spec: n_way and the quaternion fixed, the named columns' bounds (yaw 0 unless named)"""
+    row = np.zeros((B, _lib.EE_PATH_RANGES)); row[:, 0] = pd["n"]; row[:, 7:11] = pd["quat"]
+    return _box(_lib.EE_PATH_RANGES_LAYOUT, row, pd)
+
+
+def _with_paths(gd):
+    """the parsed commands gd with every robot commanded an end-effector path (a drawn path starts every episode), for the refusals"""
+    B = len(gd["gait"])
+    return dict(gd, ee_robots=np.ones(B, dtype=bool), goal_robots=gd.get("goal_robots", gd["ee_robots"]), path_robots=np.ones(B, dtype=bool))
+
+
+CURRICULUM_KINDS = dict(randomize="episode", spawn="spawn", timeline="timeline", ee_path_draw="ee_path")   # a curriculum spec's key → the draw kind it attaches to
+
+
+def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map, gd, world=True, T=None):
     """closed_loop.run's curriculum (with the run's respawn spec rs, whether metrics is on, its gait, base: the run's own randomize / spawn / timeline
     specs by kind, terrain, ground_map and parsed commands) → dict(levels, start, up_after, down_after (int arrays, scalar or [B]), conditions [(column,
     op, role)], thresholds [float arrays, scalar or [B]], tops: kind -> the parsed spec of its top box, gd: the placeholder timeline when the top box
-    weighs end-effector commands and the base does not, else None); ValueError when malformed.  B None: the lengths are not checked."""
+    weighs end-effector commands and the base does not, else None); ValueError when malformed.  B None: the lengths are not checked; T: the handle's
+    time horizon, for an ee_path_draw top box."""
     keys = ("levels", "start", "up_after", "down_after", "when") + tuple(CURRICULUM_KINDS)
     if not isinstance(curriculum, dict) or not set(curriculum) <= set(keys):
         raise ValueError("closed_loop.run: curriculum must be None or dict(%s), got %r" % (", ".join(keys), curriculum))
@@ -631,7 +694,7 @@ def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map
             raise ValueError("closed_loop.run: curriculum threshold of %s must be a finite scalar or [%s], got %r" % (col, "B" if B is None else B, thr))
         conditions.append((col, op, role)); thresholds.append(t)
     tops, top_gd = {}, None
-    for key in ("timeline", "randomize", "spawn"):   # the timeline first: its end-effector weights decide what a drawn spawn yaw may go with
+    for key in ("timeline", "randomize", "spawn", "ee_path_draw"):   # the timeline first: its end-effector weights decide what a drawn spawn yaw may go with
         if key not in curriculum:
             continue
         kind = CURRICULUM_KINDS[key]; top = curriculum[key]
@@ -639,12 +702,17 @@ def _curriculum_spec(B, curriculum, rs, metrics, gait, base, terrain, ground_map
             raise ValueError("closed_loop.run: curriculum %s needs the run's own %s (its level 0)" % (key, key))
         if not isinstance(top, dict) or {"seed", "n"} & set(top):
             raise ValueError("closed_loop.run: curriculum %s must be a dict of the top box's fields (the run's %s gives the seed%s), got %r"
-                             % (key, key, " and n" if key == "timeline" else "", top))
+                             % (key, key, " and n" if key in ("timeline", "ee_path_draw") else "", top))
         spec = dict(base[kind], **top)
         if key == "randomize":
             tops[kind] = _randomize_spec(B, spec)
         elif key == "spawn":
             tops[kind] = _spawn_spec(B, spec, terrain, ground_map, top_gd or gd, world)
+        elif key == "ee_path_draw":
+            b, t = _ee_path_draw_spec(B, T, base[kind]), _ee_path_draw_spec(B, T, spec)
+            if not np.array_equal(*np.broadcast_arrays(b["quat"], t["quat"])):
+                raise ValueError("closed_loop.run: curriculum ee_path_draw quat must equal the run's (only the boxes move with the level)")
+            tops[kind] = t
         else:
             b, t = _timeline_spec(B, gait, base[kind], None), _timeline_spec(B, gait, spec, None)
             for name, k in (("gaits (gait_set)", "gait_set"), ("ee_quat", "quat")):
@@ -984,6 +1052,8 @@ class Session:
                 scope.enter_context(_ranges(solver, "episode"))
             if tl is not None:
                 scope.enter_context(_ranges(solver, "timeline"))
+            if p["pd"] is not None:   # cleared before the ee_paths scope restores the table, which the library refuses while ranges are set
+                scope.enter_context(_ranges(solver, "ee_path"))
             if cu is not None:   # cleared first: the ranges go back to their base boxes, then the scopes above restore what they found
                 scope.callback(solver.curriculum_set)
             if gd is not None:
@@ -1050,6 +1120,10 @@ class Session:
             solver.timeline_set_ranges(tl["n"], *_timeline_box(tl, cmd_b, t_start), tl["seed"])
             if "timeline" in tops:
                 tops["timeline"] = _timeline_box(tops["timeline"], cmd_b, t_start)
+        if p["pd"] is not None:
+            solver.ee_path_set_ranges(*_ee_path_box(p["pd"], B), p["pd"]["seed"])
+            if "ee_path" in tops:
+                tops["ee_path"] = _ee_path_box(tops["ee_path"], B)
         if cu is not None:   # the levels start at the run's start levels; each kind's ranges set above are its level 0
             rows = np.zeros((B, _lib.CURRICULUM))
             rows[:, 0] = cu["start"]; rows[:, 1] = cu["up_after"]; rows[:, 2] = cu["down_after"]
@@ -1143,7 +1217,7 @@ class Session:
                     prob["event_times"], prob["modes"], prob["n_target"], prob["target_times"], prob["target_states"]] + \
                    ([v_prev, sensors, rbd_est] if se else []) + ([stance] if sl else [])
         self.path_state = None
-        if p["ep"] is not None:   # each robot's end-effector path row (index -1: none), the target call's in-out row beside last_ee
+        if p["ep"] is not None or p["pd"] is not None:   # each robot's end-effector path row (index -1: none), the target call's in-out row beside last_ee
             with torch.cuda.stream(stream):
                 self.path_state = torch.zeros((B, _lib.EE_PATH_STATE), dtype=torch.float64, device=dev); self.path_state[:, 0] = -1.0
             self.own.append(self.path_state)
@@ -1186,11 +1260,12 @@ class Session:
                     self.req = torch.zeros_like(contact); self.req_end = torch.full_like(contact, 2); self.req_rows = torch.zeros_like(self.pl_rows)
             self._place_link = p["sp"]["link"] if sp is not None else (_lib.SPAWN_GROUND_MAP if o["ground_map"] is True else 0)
 
-        if rz is not None or sp is not None or tl is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
+        if rz is not None or sp is not None or tl is not None or p["pd"] is not None:   # every robot's first episode begins right before the first solve (after the restore of the start image)
             with torch.cuda.stream(stream):
                 self.ep_rows = torch.zeros((B, _lib.EPISODE), dtype=torch.float64, device=dev) if rz is not None else None
                 self.sp_rows = torch.zeros((B, _lib.SPAWN), dtype=torch.float64, device=dev) if sp is not None else None
                 self.tl_rows = torch.zeros((B, tl["n"], _lib.TIMELINE_CMD), dtype=torch.float64, device=dev) if tl is not None else None
+                self.pd_rows = torch.zeros((B, _lib.EE_PATH_MAX, 8), dtype=torch.float64, device=dev) if p["pd"] is not None else None
                 if rs is None:
                     self._begin(torch.ones(B, dtype=torch.int32, device=dev), torch.zeros(B, dtype=torch.int32, device=dev))
                 else:
@@ -1257,7 +1332,7 @@ class Session:
         rows = torch.arange(self.B, device=self.device); e = self.episode.long()
         self.ep_level[rows, e] = torch.where(mask.bool(), self.cu_level, self.ep_level[rows, e])
 
-    def _begin(self, mask, idx, placed=None):   # the masked robots begin episode idx: their plant's draw, then their spawn or place, then their command timeline
+    def _begin(self, mask, idx, placed=None):   # the masked robots begin episode idx: their plant's draw, their spawn or place, their command timeline, their path
         p, solver, s = self._spec, self.solver, self._s
         if p["rz"] is not None:
             self._draw(mask, idx)
@@ -1271,6 +1346,8 @@ class Session:
             self.acc_st.bitwise_or_(self.pl_st)
         if p["tl"] is not None:
             solver.timeline_sample_dev(mask, idx, self.tl_rows, s)
+        if p["pd"] is not None:   # last: its pending start is applied after the timeline's rows due on the first tick (the restore dropped any pending command)
+            solver.ee_path_sample_dev(mask, idx, self.pd_rows, s)
 
     def _record_spawn(self, mask, placed):   # the masked robots' new episode's spawn row: placed, drawn, or the start's; NaN where a place was rejected
         import torch
@@ -1595,8 +1672,8 @@ class Session:
 
     def finish(self):
         """Close every robot's open episode (end 0) and return run's end-of-run keys as numpy arrays, from the device state: contact, q, v, start_base,
-        start_ee, and as run gives them gait_templates, episode_level, curriculum_state, episode_params, spawn_params, timeline_params, episode_metrics
-        and metrics_layout.  Synchronises self.stream; the session takes no more steps."""
+        start_ee, and as run gives them gait_templates, episode_level, curriculum_state, episode_params, spawn_params, timeline_params, ee_path_params,
+        episode_metrics and metrics_layout.  Synchronises self.stream; the session takes no more steps."""
         import torch
         if not self._open or self._finished:
             raise ValueError("closed_loop.Session.finish: the session is not open (enter it with `with`; finish() ends it)")
@@ -1624,6 +1701,10 @@ class Session:
                     out[kind + "_params"] = np.full(had.shape + shape, np.nan); out[kind + "_params"][rb, re_] = rows
             if tl is not None:   # on the episode's clock: exact for drawn times in [t_start / 2, 2 t_start]
                 out["timeline_params"][..., 0] -= self.t_start
+        if p["pd"] is not None:   # tau counts from the path's start, the episode's first MPC tick
+            rb, re_ = np.nonzero(had)
+            _, way = solver.curriculum_draw("ee_path", rb, re_, el[rb, re_]) if "ee_path" in self._tops else solver.ee_path_draw(rb, re_)
+            out["ee_path_params"] = np.full(had.shape + (p["pd"]["n"], 8), np.nan); out["ee_path_params"][rb, re_] = way[:, :p["pd"]["n"]]
         if self._placing and int(self.pl_any.item()):   # placed rows are not draws: the device record holds every episode's row
             out["spawn_params"] = self.sp_rec[:, :had.shape[1]].cpu().numpy()
         if self._mt:   # trimmed to the most episodes of any robot

@@ -24,6 +24,7 @@
 #include "kernels/spawn_api.cuh"
 #include "kernels/metrics_api.cuh"
 #include "kernels/timeline_api.cuh"
+#include "kernels/ee_path_draw_api.cuh"
 #include "kernels/curriculum_api.cuh"
 
 namespace qmb {
@@ -46,7 +47,7 @@ struct RobotArray {
   const double* dev() const { return host.empty() ? nullptr : d; }
 };
 
-// Per-robot ranges of a per-episode draw (capi_episode.inc, capi_spawn.inc, capi_timeline.inc): lo, hi [B][width] (empty: none set), their device copies (dalloc: freed
+// Per-robot ranges of a per-episode draw (capi_episode.inc, capi_spawn.inc, capi_timeline.inc, capi_ee_path_draw.inc): lo, hi [B][width] (empty: none set), their device copies (dalloc: freed
 // with allocs) and the seed; attached: a curriculum owns them (capi_curriculum.inc), on_device: its update wrote the device copies, ranges_sync refreshes lo, hi
 struct DrawRanges {
   int width; std::vector<double> lo, hi; double *d_lo = nullptr, *d_hi = nullptr; uint64_t seed = 0; bool attached = false, on_device = false;
@@ -90,8 +91,9 @@ struct qmb200_handle {
     std::vector<int32_t> host; int32_t* d = nullptr; uint64_t gen = 0; bool on_device = false;
     const int32_t* dev() const { return host.empty() ? nullptr : d; }
   } ee_frame;
-  struct {   // the end-effector path table (qmb200_set_ee_paths): host copies (n_way empty = none) and device copies of n_way [n] and way [n][EE_PATH_MAX][8]
-    std::vector<int32_t> n_way; std::vector<double> way; int32_t* d_n_way = nullptr; double* d_way = nullptr;
+  struct {   // the end-effector path table (qmb200_set_ee_paths): host copies (n_way empty = none) and device copies of n_way [n] and way [n][EE_PATH_MAX][8];
+             // drawn: the rows the path sampler owns after them on the device (B while ee path ranges are set, else 0; capi_ee_path_draw.inc)
+    std::vector<int32_t> n_way; std::vector<double> way; int32_t* d_n_way = nullptr; double* d_way = nullptr; int drawn = 0;
   } ee_path;
   qmb200_payload_est_params est_prm{}; FilterState est{EST_DBL, "payload estimator", "qmb200_payload_est_reset"};   // payload estimator (capi_est.inc)
   qmb200_sensor_params sensor_prm{};                               // sensor noise of qmb200_sim_read_sensors (capi_state_est.inc)
@@ -120,6 +122,7 @@ struct qmb200_handle {
                                          // ranges: whether any robot weighs an end-effector kind, one past the highest gait_set bit
     int n_cmd = 0; bool ee = false; int gait_bits = 0;
   } timeline{{TL_DBL}};
+  DrawRanges ee_draw{EPR_DBL};   // per-episode end-effector paths (capi_ee_path_draw.inc)
   struct {   // per-robot curriculum (capi_curriculum.inc): the rule, the rows [B][CU_DBL] and the state [B][CUS_INT] (host copies, empty: none set; on_device:
              // an update wrote the device state) with their device copies, and each kind's base and top boxes (host copies, empty: not attached) with
              // their device copy d [4][B][width] (base lo, base hi, top lo, top hi)
@@ -351,7 +354,7 @@ int model_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb
 int plant_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->plant_on_device, {&h->mu, &h->payload}); }
 int tuning_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->tuning_on_device, {&h->tuning}); }
 int terrain_rows_sync(const qmb200_handle* hc) { qmb200_handle* h = const_cast<qmb200_handle*>(hc); return rows_sync(h, h->terrain_on_device, {&h->terrain, &h->se_ground}); }
-// The ranged draws' set / get / draw path (qmb200_<kind>_set_ranges, _get_ranges, _draw; kind: "episode", "spawn" or "timeline").
+// The ranged draws' set / get / draw path (qmb200_<kind>_set_ranges, _get_ranges, _draw; kind: "episode", "spawn", "timeline" or "ee_path").
 // Set: NULL lo and hi clear the ranges once no queued draw reads them; else error() checks them ("" when valid), the device copies are allocated, then
 // prepare() makes sure the rows the sampler writes exist (it may fail, leaving the ranges as they were), and the ranges are copied and stored.
 // Refused while a curriculum is attached to the ranges (qmb200_curriculum_attach), whose update writes them.
@@ -581,4 +584,5 @@ int qmb200_wbc_set_iteration_caps(qmb200_handle* h, int32_t level0_passes, int32
 #include "capi_spawn.inc"
 #include "capi_metrics.inc"
 #include "capi_timeline.inc"
+#include "capi_ee_path_draw.inc"
 #include "capi_curriculum.inc"

@@ -13,6 +13,7 @@
 #include "episode_api.cuh"
 #include "spawn_api.cuh"
 #include "timeline_api.cuh"
+#include "ee_path_draw_api.cuh"
 #include "../../../include/qmb200.h"
 
 namespace qmb {
@@ -20,7 +21,7 @@ namespace qmb {
 // a curriculum row [CU_DBL] (_lib.CURRICULUM_LAYOUT) and a state row [CUS_INT] (_lib.CURRICULUM_STATE_LAYOUT)
 constexpr int CU_START = 0, CU_UP_AFTER = 1, CU_DOWN_AFTER = 2, CU_THRESHOLD = 3, CU_DBL = 7;
 constexpr int CUS_LEVEL = 0, CUS_PASS_RUN = 1, CUS_FAIL_RUN = 2, CUS_UPDATES = 3, CUS_INT = 4;
-constexpr int CU_KINDS = 3;
+constexpr int CU_KINDS = 4;
 
 // One column at `level` of n_levels: base at level 0 and top at the last level, byte for byte; between them base where both ends are equal (-0.0
 // included; fma would turn -0.0 into +0.0), else fma(f, top - base, base) with f = level / (n_levels - 1), rounded to the nearest integer
@@ -94,6 +95,16 @@ inline std::string curriculum_timeline_ends_error(const double* base_lo, const d
   }
   return "";
 }
+// The ee path's columns that are not interpolated, n_way and q*, must be equal in the base and top boxes lo, hi [B][EPR_DBL] ("" when they are)
+inline std::string curriculum_ee_path_ends_error(const double* base_lo, const double* base_hi, const double* top_lo, const double* top_hi, size_t B) {
+  static const char* const names[5] = {"n_way", "qx", "qy", "qz", "qw"};
+  static const int cols[5] = {EPR_N_WAY, EPR_QUAT, EPR_QUAT + 1, EPR_QUAT + 2, EPR_QUAT + 3};
+  for (size_t b = 0; b < B; ++b) for (int j = 0; j < 5; ++j) {
+    const size_t i = b * EPR_DBL + cols[j];
+    if (!(top_lo[i] == base_lo[i] && top_hi[i] == base_hi[i])) return std::string("ee_path ") + names[j] + " of robot " + std::to_string(b) + ": must be equal in the base and top boxes";
+  }
+  return "";
+}
 // The first level of n_levels whose boxes lo, hi [B][width] between base and top fail check(lo, hi) (a message naming the field and the robot, "" when
 // valid): "<kind> level <l>: <message>", "" when every level passes
 template <class Check>
@@ -115,7 +126,7 @@ std::string curriculum_levels_error(const char* kind, const double* base_lo, con
 struct CurriculumKind { const double *base_lo, *base_hi, *top_lo, *top_hi; double *lo, *hi; };
 struct CurriculumArgs {
   qmb200_curriculum_rule rule; const double* rows; int32_t* state;   // the rule, the curriculum rows [B][CU_DBL], the state [B][CUS_INT]
-  CurriculumKind kind[CU_KINDS];                                     // QMB200_CURRICULUM_EPISODE, _SPAWN, _TIMELINE
+  CurriculumKind kind[CU_KINDS];                                     // QMB200_CURRICULUM_EPISODE, _SPAWN, _TIMELINE, _EE_PATH
 };
 // one thread per robot: the masked robots with end 1 or 2 update their state from end and (with conditions) metrics[b][episode[b]]
 int launch_curriculum_update(int B, const CurriculumArgs& a, const int32_t* mask, const int32_t* end, const int32_t* episode, const double* metrics, int n_episodes,

@@ -11,7 +11,7 @@ constexpr int CU_THREADS = 128;
 
 // robot b's box of one kind of width W (round_col: the integer column, -1 none) at `level` into the kind's ranges
 template <int W, int ROUND_COL>
-__device__ __forceinline__ void write_box(const CurriculumKind& k, size_t b, int level, int n_levels) {
+__device__ __forceinline__ void write_box(const CurriculumKind k, size_t b, int level, int n_levels) {
   const size_t o = b * W;
 #pragma unroll
   for (int c = 0; c < W; ++c) {
@@ -44,6 +44,7 @@ __global__ void __launch_bounds__(CU_THREADS) curriculum_update_kernel(int B, co
   if (a.kind[QMB200_CURRICULUM_EPISODE].lo) write_box<EP_DBL, -1>(a.kind[QMB200_CURRICULUM_EPISODE], b, s[CUS_LEVEL], a.rule.n_levels);
   if (a.kind[QMB200_CURRICULUM_SPAWN].lo) write_box<SP_DBL, SP_TILE>(a.kind[QMB200_CURRICULUM_SPAWN], b, s[CUS_LEVEL], a.rule.n_levels);
   if (a.kind[QMB200_CURRICULUM_TIMELINE].lo) write_box<TL_DBL, -1>(a.kind[QMB200_CURRICULUM_TIMELINE], b, s[CUS_LEVEL], a.rule.n_levels);
+  if (a.kind[QMB200_CURRICULUM_EE_PATH].lo) write_box<EPR_DBL, -1>(a.kind[QMB200_CURRICULUM_EE_PATH], b, s[CUS_LEVEL], a.rule.n_levels);
 }
 }  // namespace
 

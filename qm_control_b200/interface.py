@@ -944,6 +944,39 @@ class Solver:
         self._call("timeline_draw", len(robot), _p(robot), _p(episode), _p(rows))
         return rows
 
+    # ---------------- per-episode end-effector paths (include/qmb200.h: qmb200_ee_path_*; DESIGN.md §4.21) ----------------
+    def ee_path_set_ranges(self, lo=None, hi=None, seed=0):
+        """Per-robot ranges lo, hi [B, EE_PATH_RANGES] (columns _lib.EE_PATH_RANGES_LAYOUT) and a 64-bit seed of the per-episode end-effector paths; None
+        clears them.  While they are set, robot b's drawn path is row P + b of the path table (P: set_ee_paths' paths), and set_ee_paths refuses.
+        Synchronous."""
+        self._ranges_set("ee_path", _lib.EE_PATH_RANGES, lo, hi, seed)
+
+    def ee_path_get_ranges(self):
+        """→ dict(lo [B, EE_PATH_RANGES], hi [B, EE_PATH_RANGES], seed) of the stored ranges, or None when none are set."""
+        return self._ranges_get("ee_path", _lib.EE_PATH_RANGES)
+
+    def ee_path_sample(self, mask, episode, rows=None):
+        """Host variant of ee_path_sample_dev: mask [B], episode [B] → rows [B, EE_PATH_MAX, 8] (rows of unmasked robots and past n_way as given, zeros by
+        default)."""
+        B = self.batch; shape = (B, _lib.EE_PATH_MAX, 8)
+        rows = np.zeros(shape) if rows is None else _f64(rows, shape).copy()
+        mask = _i32(np.broadcast_to(np.asarray(mask), (B,)), (B,)); episode = _i32(np.broadcast_to(np.asarray(episode), (B,)), (B,))
+        self._call("ee_path_sample", _p(mask), _p(episode), _p(rows))
+        return rows
+
+    def ee_path_sample_dev(self, mask, episode, rows, stream=None):
+        """Every robot with mask[b] != 0 (int32 [B] device tensor) draws episode[b]'s path (int32 [B]) into rows[b, :n_way] ([B, EE_PATH_MAX, 8] float64
+        device tensor; the rest of the row is not written) and into its row of the path table, and its pending command becomes a start of that row, applied by its next gait step.
+        Needs the device gait schedule.  One launch, no synchronisation."""
+        self._call("ee_path_sample_dev", _p(mask), _p(episode), _p(rows), stream)
+
+    def ee_path_draw(self, robot, episode):
+        """Host only: robot [n] (in [0, B)), episode [n] → (n_way [n], way [n, EE_PATH_MAX, 8]) the sampler draws for them on the stored ranges and seed."""
+        robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape)
+        n_way = np.zeros(len(robot), dtype=np.int32); way = np.zeros((len(robot), _lib.EE_PATH_MAX, 8))
+        self._call("ee_path_draw", len(robot), _p(robot), _p(episode), _p(n_way), _p(way))
+        return n_way, way
+
     # ---------------- per-robot curricula (include/qmb200.h: qmb200_curriculum_*; DESIGN.md §4.15) ----------------
     def curriculum_set(self, n_levels=None, rows=None, conditions=()):
         """A curriculum of n_levels levels: per-robot rows [B, CURRICULUM] (_lib.CURRICULUM_LAYOUT) and up to CURRICULUM_MAX_COND conditions (column, op,
@@ -961,9 +994,9 @@ class Solver:
         self._call("curriculum_set", C.byref(rule), _p(_f64(rows, (self.batch, _lib.CURRICULUM))))
 
     def curriculum_attach(self, kind, lo_top, hi_top):
-        """Attach kind ("episode", "spawn" or "timeline"): its ranges in force become level 0, lo_top / hi_top [B, width] the last level, and each robot's
+        """Attach kind ("episode", "spawn", "timeline" or "ee_path"): its ranges in force become level 0, lo_top / hi_top [B, width] the last level, and each robot's
         box at its level is written into the kind's ranges.  Synchronous."""
-        width = dict(episode=_lib.EPISODE, spawn=_lib.SPAWN, timeline=_lib.TIMELINE)[kind]
+        width = dict(episode=_lib.EPISODE, spawn=_lib.SPAWN, timeline=_lib.TIMELINE, ee_path=_lib.EE_PATH_RANGES)[kind]
         shape = (self.batch, width)
         self._call("curriculum_attach", _lib.CURRICULUM_KINDS.index(kind), _p(_f64(lo_top, shape)), _p(_f64(hi_top, shape)))
 
@@ -994,12 +1027,15 @@ class Solver:
         self._call("curriculum_update_dev", _p(mask), _p(end), _p(episode), _p(rows), 1 if rows is None else int(rows.shape[1]), _p(level), _p(status), stream)
 
     def curriculum_draw(self, kind, robot, episode, level):
-        """Host only: robot [n], episode [n], level [n] → the rows attached kind's sampler draws for them at those levels ([n, EPISODE], [n, SPAWN] or
-        [n, n_cmd, TIMELINE_CMD])."""
+        """Host only: robot [n], episode [n], level [n] → the rows attached kind's sampler draws for them at those levels ([n, EPISODE], [n, SPAWN],
+        [n, n_cmd, TIMELINE_CMD], or for "ee_path" (n_way [n], way [n, EE_PATH_MAX, 8]) as ee_path_draw gives them)."""
         robot = _i32(np.ravel(robot)); episode = _i32(np.ravel(episode), robot.shape); level = _i32(np.ravel(level), robot.shape)
-        shape = dict(episode=(_lib.EPISODE,), spawn=(_lib.SPAWN,), timeline=(self._timeline_n(), _lib.TIMELINE_CMD))[kind]
+        shape = dict(episode=(_lib.EPISODE,), spawn=(_lib.SPAWN,), timeline=(self._timeline_n(), _lib.TIMELINE_CMD),
+                     ee_path=(1 + _lib.EE_PATH_MAX * 8,))[kind]
         rows = np.zeros((len(robot),) + shape)
         self._call("curriculum_draw", _lib.CURRICULUM_KINDS.index(kind), len(robot), _p(robot), _p(episode), _p(level), _p(rows))
+        if kind == "ee_path":
+            return rows[:, 0].astype(np.int32), rows[:, 1:].reshape(len(robot), _lib.EE_PATH_MAX, 8)
         return rows
 
     # ---------------- per-episode metrics (include/qmb200.h: qmb200_metrics_*; DESIGN.md §4.13) ----------------

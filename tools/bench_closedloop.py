@@ -449,6 +449,77 @@ def ee_paths_main(args, duration=4.0, t_first=0.5, gap=0.75):
     print(json.dumps(out))
 
 
+def ee_path_draw_main(args, track_s=4.0, box=0.05):
+    """Per-episode end-effector paths (DESIGN.md §4.21): the sampler's device time for one draw of every robot against one 1 ms plant step of the batch
+    (alternated blocks of CUDA events, medians); the wall seconds per simulated second of --duration respawning runs of --gait at --vx (respawn after
+    0.1 s fallen or 1 s) with and without a heading-frame path draw per episode, alternated twice after a warm-up pair; and 256 standing heading robots on
+    drawn 4-waypoint paths in a +-box m box about the standing hand: the hand's position error against p(t) from the first to the last waypoint, p50 / p95."""
+    import torch
+    import qm_control_b200 as q
+    from qm_control_b200 import closed_loop
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_closedloop.py: no CUDA device — the product path has no CPU fallback")
+    dev = torch.device("cuda", 0); B = args.batch; solver = q.Solver(batch=B, device=0); st = torch.cuda.Stream(device=dev)
+    xy = np.zeros((B, 3)); xy[:, 0] = 2.0 * (np.arange(B) % 64); xy[:, 1] = 2.0 * (np.arange(B) // 64)
+    r = closed_loop.run(solver, duration=0.5, gait="stance", xy_yaw=xy, ee_frame="heading")
+    hand = np.r_[r["ee"][-1, 0, :2] - r["base"][-1, 0, :2], r["ee"][-1, 0, 2:7]]   # robot 0's standing hand relative to its base (yaw 0)
+    spec = dict(seed=1, n=4, tau_first=(0.5, 0.6), gap=(0.6, 0.8), yaw=(-0.3, 0.3), quat=hand[3:7], **{c: (hand[i] - box, hand[i] + box) for i, c in enumerate("xyz")})
+    # per call: the sampler on a running device gait schedule, and the plant step
+    pd = closed_loop._ee_path_draw_spec(B, solver.time_horizon, spec)
+    solver.gait_dev_set_templates(closed_loop.gait_template_names()); solver.gait_dev_reset(np.zeros(B, dtype=np.int32), np.full(B, 10.0))
+    solver.ee_path_set_ranges(*closed_loop._ee_path_box(pd, B), 1)
+    q0, v0 = solver.sim_standing_state(xy); qq = torch.as_tensor(q0, device=dev); vv = torch.as_tensor(v0, device=dev)
+    eff = torch.zeros((B, 18), dtype=torch.float64, device=dev); rbd = torch.zeros((B, 55), dtype=torch.float64, device=dev)
+    contact = torch.zeros(B, dtype=torch.int32, device=dev); sst = torch.zeros_like(contact)
+    every = torch.ones_like(contact); episode = torch.zeros_like(contact); rows = torch.zeros((B, _lib.EE_PATH_MAX, 8), dtype=torch.float64, device=dev)
+    calls_of = {"ee_path_sample": lambda: (episode.add_(1), solver.ee_path_sample_dev(every, episode, rows, st.cuda_stream)),
+                "plant": lambda: solver.sim_step_dev(1e-3, eff, qq, vv, rbd, contact, sst, st.cuda_stream)}
+    times = {k: [] for k in calls_of}; reps, calls = 7, 20
+    with torch.cuda.stream(st):
+        for rep in range(reps + 1):   # the first round warms up
+            for mode, call in calls_of.items():
+                torch.cuda.synchronize(dev)
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True); a.record(st)
+                for _ in range(calls):
+                    call()
+                b.record(st); torch.cuda.synchronize(dev)
+                if rep:
+                    times[mode].append(a.elapsed_time(b) / calls)
+    solver.ee_path_set_ranges(None); solver.gait_dev_stop()
+    per_call = {"label": "device time per call on %d robots (every robot drawing 4 waypoints), median of %d alternated blocks of %d calls" % (B, reps, calls),
+                **{"ms_per_%s" % k: float(np.median(v)) for k, v in times.items()}, "spread_ee_path_sample": [float(min(times["ee_path_sample"])), float(max(times["ee_path_sample"]))]}
+    # wall time of a respawning trot with and without the draws
+    kw = dict(gait=args.gait, cmd_vel=np.array([args.vx, 0.0, 0.0, 0.0]), xy_yaw=xy, ee_frame="heading", respawn=dict(hold=0.1, every=1.0))
+    wall = {"without_draw": [], "with_draw": []}
+    for rep in range(3):   # the first round warms up
+        for name, extra in (("without_draw", {}), ("with_draw", dict(ee_path_draw=spec))):
+            solver.mpc_reset(); solver.wbc_set_input_last(None); torch.cuda.synchronize(dev); t0 = time.perf_counter()
+            closed_loop.run(solver, duration=args.duration, **kw, **extra); torch.cuda.synchronize(dev)
+            if rep:
+                wall[name].append((time.perf_counter() - t0) / args.duration)
+    # tracking: 256 standing heading robots on drawn paths
+    n = min(B, 256); s2 = q.Solver(batch=n, device=0); xy2 = xy[:n]
+    with closed_loop.Session(s2, track_s, gait="stance", xy_yaw=xy2, ee_frame="heading", ee_path_draw=spec) as ss:
+        rec = ss.step(ss.windows); ss.stream.synchronize(); p = ss.path_state.cpu().numpy(); end = ss.finish()
+    rec = {k: (v if isinstance(v, np.ndarray) else v.cpu().numpy()) for k, v in rec.items()}
+    way = end["ee_path_params"][:, 0]; t = rec["t"]; ref = np.zeros((len(t), n, 3))
+    for b in range(n):
+        for c in range(3):
+            ref[:, b, c] = np.interp(t - p[b, 1], way[b, :, 0], way[b, :, 1 + c])
+    cs, sn = np.cos(p[:, 4]), np.sin(p[:, 4])
+    world = np.stack([cs * ref[..., 0] - sn * ref[..., 1] + p[:, 2], sn * ref[..., 0] + cs * ref[..., 1] + p[:, 3], ref[..., 2]], -1)
+    err = np.linalg.norm(rec["ee"][..., :3] - world, axis=-1) * 1e3
+    along = (t[:, None] >= p[None, :, 1] + way[None, :, 0, 0]) & (t[:, None] <= p[None, :, 1] + way[None, :, -1, 0])
+    base = rec["base"]; up = np.all(np.isfinite(base), axis=(0, 2)) & (np.min(base[:, :, 2], axis=0) > 0.3)
+    name, limit = card()
+    print(json.dumps({"metric": "ee_path_draw", "gpu": name, "power_limit": limit, "batch": B, "per_call": per_call,
+                      "wall_s_per_sim_s": {"label": "%s at %.2f m/s, heading frame, respawn after 0.1 s fallen or 1 s, runs of %.1f s, two alternated pairs after a "
+                                                    "warm-up pair" % (args.gait, args.vx, args.duration), **wall},
+                      "tracking": {"robots": n, "frame": "heading", "box_m": box, "waypoints": 4, "fallen": int(np.sum(~up)),
+                                   "status_robots": int(np.sum(np.any(rec["status"] != 0, axis=0))),
+                                   "along_path_mm_p50_p95": [float(v) for v in np.percentile(err[along], [50, 95])]}}))
+
+
 def ee_frame_main(args, sweep_s=4.0):
     """End-effector targets in the heading frame (DESIGN.md §4.19): the target call of the whole batch (kinds 0 / 1 / 2 / -1 mixed) with no frame rows,
     all-world rows and all-heading rows, alternated blocks of CUDA events, medians; then the turning sweep (start yaws over [-pi, pi], yaw rates
@@ -1406,7 +1477,11 @@ def main():
     ap.add_argument("--ee-frame", action="store_true", help="end-effector targets in the heading frame: the target call's time with no, all-world and all-heading "
                                                             "frame rows, and a turning sweep over start yaws and yaw rates in both frames; with --respawn: "
                                                             "that run with every robot's targets in its heading frame")
+    ap.add_argument("--ee-path-draw", action="store_true", help="per-episode end-effector paths: the sampler's time against the plant step, a respawning run "
+                    "with and without draws, and the hand error against drawn 4-waypoint paths of 256 standing robots")
     args = ap.parse_args()
+    if args.ee_path_draw:
+        return ee_path_draw_main(args)
     if args.ee_frame and not args.respawn:
         return ee_frame_main(args)
     if args.ee_paths:
