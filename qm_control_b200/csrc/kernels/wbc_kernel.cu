@@ -26,7 +26,9 @@ namespace qmb {
 constexpr int LDM = 25;   // leading dimension of 24-column matrices (odd → conflict-free column walks)
 constexpr int LDZ = 37;   // leading dimension of 36-column / 36-row matrices
 constexpr int LZ = 19;    // leading dimension of matrices in null-space coordinates (at most 18 columns: level 0 always has 18 independent rows)
-constexpr int MAXR = 24;  // max rows of one level's equality task (22 in flight mode) or 18 + violated rows at level 0
+constexpr int MAXR = 24;  // max rows of one level's equality task (22 in flight mode)
+constexpr int MAXR0 = 32; // max rows of level 0's least squares: its 18 task rows + up to 14 violated inequalities (w_qrcp factors at most 32 columns)
+constexpr int KG0 = 27;   // max rank of a rank-deficient level-0 pass of more than MAXR rows that forms its Gram (behind the rows); above it the pass solves on its independent rows
 constexpr int LJC = 9;    // pitch of a compact foot-Jacobian row
 constexpr int MAXW = 20;  // max size of the inequality working set
 #ifndef QMB_WBC_WARPS
@@ -44,20 +46,25 @@ struct EeWs { double Jee[6 * LDM], djv_ee[6], ee_m_pos[3], ee_m_vel[3], ee_m_rot
 //   * levels >= 1 iterate in null-space coordinates on the projected rows A_p Z (<= 22 x 18), so the 36-wide rows are only a build area that the
 //     factorisation workspaces of the level reuse; working-set rows are regenerated from M / J instead of being cached.
 struct QpWs {
-  union ZA { struct Q { double Z[36 * LZ];        // orthonormal basis of the current null space, active columns [off, nzc)
+  union ZA { struct Q { double Z[36 * LZ];        // orthonormal basis of the current null space, active columns [off, nzc).  Level 0, a pass with more than MAXR
+                                                  //   rows: its rows (up to MAXR0, reaching into AR) and the Gram scratch behind row MAXR0
                         double AR[MAXR * LDZ];    // level 0: task rows / their in-place QR.  levels >= 1: raw task rows while they are built, then the
                       } q;                        //   step workspace W1 (LZ x MAXR, at AR) and the working-set factorisation Wc (LZ x MAXW, behind it)
              RbdWs rbd;                           // rigid-body passes (before the hierarchy starts)
              __device__ ZA() {} } za;
   union AH { double Ah[MAXR * LZ];                // projected task rows A_p Z (rows x nz, pitch LZ) = column-major nz x rows for the null-space QR of the level
              EeWs ee; __device__ AH() {} } ah;
-  double G[18 * 19 / 2 + 1];                      // normal equations (packed lower triangle) of an overdetermined / rank-deficient step (k <= 18 at levels >= 1; level 0 borrows Z)
+  union GL { double G[18 * 19 / 2 + 1];           // normal equations (packed lower triangle) of an overdetermined / rank-deficient step (k <= 18 at levels >= 1)
+             struct L0 { double b[MAXR0], tau[MAXR0], t18[MAXR0]; int perm[MAXR0]; } l0;   // level 0: right-hand side and QR scratch of its MAXR0 rows
+             __device__ GL() {} } gl;
   double tau[MAXR], tauc[MAXW];
   double xbar[36], dx[36], g[36], y[36], s[36], zac[LZ + 1], rhs[MAXR], bp[MAXR], bh[MAXR], lam[MAXW], t18[MAXR];
   int perm[MAXR], permc[MAXW], wset[MAXW];
 };
 static_assert(LZ * MAXR + LZ * MAXW <= MAXR * LDZ, "W1 and Wc share the row build area");
 static_assert(sizeof(RbdWs) <= sizeof(double) * (36 * LZ + MAXR * LDZ), "rigid-body workspace overlays Z + AR only");
+static_assert(MAXR0 * LDZ + KG0 * (KG0 + 1) / 2 <= 36 * LZ + MAXR * LDZ, "level 0's rows and the Gram of a rank-deficient pass fit in Z + AR");
+static_assert(MAXR0 <= 32, "w_qrcp factors at most 32 columns");
 
 struct WbcSmem {
   double q[NQ], v[NQ], qd[NQ], vd[NQ];
@@ -116,43 +123,50 @@ __device__ __forceinline__ double ineq_row_elem(const IneqCtx& c, int i, int k) 
 
 // ---------------------------------------------------------------------------------------------------------
 // Minimum-norm least squares  min || Abar y - rhs ||  with Abar^T stored column-wise in W (n x r, leading dimension ldw): COD.
-// On exit y[0..n) holds the solution in the coordinates of W's rows; returns rank.  Uses qp.tau/perm/t18 and the scratch G (k(k+1)/2 doubles).
-__device__ int cod_lstsq(QpWs& qp, double* W, int n, int r, int ldw, const double* rhs, double* y, double* G, int lane) {
-  const int k = w_qrcp(W, n, r, ldw, qp.tau, qp.perm, 1e-11, lane);
+// On exit y[0..n) holds the solution in the coordinates of W's rows; returns rank.  Rank-deficient rows of a rank above kg (no room for their Gram) are solved on
+// their k independent rows, which is the same solution when the dependent rows are consistent with them; otherwise y holds that solution and returns -1.
+// Scratch: tau / perm (r entries), t (k) and G (k(k+1)/2 doubles, k <= kg).
+__device__ int cod_lstsq(double* W, int n, int r, int ldw, const double* rhs, double* y, double* G, int kg, double* tau, int* perm, double* t, int lane) {
+  const int k = w_qrcp(W, n, r, ldw, tau, perm, 1e-11, lane);
   // Abar = P R^T Q^T  →  residual_c = sum_{i<=min(c,k-1)} R[i][c] y_i - rhs[perm[c]]
   for (int i = lane; i < n; i += 32) y[i] = 0.0;
   __syncwarp();
   if (k == 0) return 0;
-  if (k == r) {   // square lower-triangular system R11^T y1 = P^T rhs
+  if (k == r || k > kg) {   // square lower-triangular system R11^T y1 = P^T rhs
     for (int c = 0; c < k; ++c) {
       double part = 0.0; if (lane < c) part = W[lane + c * ldw] * y[lane];
       const double s = warp_sum(part);
-      if (lane == 0) y[c] = (rhs[qp.perm[c]] - s) / W[c + c * ldw];
+      if (lane == 0) y[c] = (rhs[perm[c]] - s) / W[c + c * ldw];
       __syncwarp();
+    }
+    if (k < r) {   // the dependent rows must hold at that solution (lane = row, r <= 32)
+      bool off = false;
+      if (lane >= k && lane < r) { double s = 0.0; for (int i = 0; i < k; ++i) s += W[i + lane * ldw] * y[i]; const double b = rhs[perm[lane]]; off = fabs(s - b) > 1e-9 * (1.0 + fabs(b)); }
+      if (__any_sync(FULL, off)) { w_apply_q(W, n, k, ldw, tau, y, lane); return -1; }   // y: the solution on the independent rows, in x coordinates
     }
   } else {        // overdetermined / rank deficient: normal equations on the k x k triangular factor, G = R R^T as a packed lower triangle
     { int a = 0, b = lane; while (b > a) { b -= a + 1; ++a; }   // entry number `lane` of the packed triangle; the lane then strides by 32 entries
       while (a < k) { double s = 0.0; for (int c = a; c < r; ++c) s += W[a + c * ldw] * W[b + c * ldw]; G[tri(a) + b] = s;
         b += 32; while (b > a) { b -= a + 1; ++a; } } }
-    if (lane < k) { double s = 0.0; for (int c = lane; c < r; ++c) s += W[lane + c * ldw] * rhs[qp.perm[c]]; qp.t18[lane] = s; }
+    if (lane < k) { double s = 0.0; for (int c = lane; c < r; ++c) s += W[lane + c * ldw] * rhs[perm[c]]; t[lane] = s; }
     __syncwarp();
     w_cholesky(G, k, lane);
-    w_chol_solve(G, k, qp.t18, lane);
-    if (lane < k) y[lane] = qp.t18[lane];
+    w_chol_solve(G, k, t, lane);
+    if (lane < k) y[lane] = t[lane];
     __syncwarp();
   }
-  w_apply_q(W, n, k, ldw, qp.tau, y, lane);
+  w_apply_q(W, n, k, ldw, tau, y, lane);
   return k;
 }
 
-// Build the task rows of one hierarchy level into the row build area qp.za.q.AR (pitch LDZ) / qp.bp.  Returns the row count.
+// Build the task rows of one hierarchy level into the row build area qp.za.q.AR (pitch LDZ) / qp.bp (level 0: qp.gl.l0.b).  Returns the row count.
 //   level 0: floating-base EoM + no-contact-motion + swing zero-force           (WbcBase.cpp:338-356, 386-401, 407-415)
 //   level 1: HierarchicalWbc: height, base angular, EE linear, EE angular, 100*swing (t>=10) | arm joint tracking (t<10)
 //            HierarchicalMpcWbc: height, base angular, base linear, 100*swing
 //   level 2: contact force + base linear | contact force
 __device__ int build_level(WbcSmem& sm, const Tuning* __restrict__ tn, int level, int mode, int variant, bool init_phase, int ffp, int lane) {
   QpWs& qp = sm.qp; double* Ap = qp.za.q.AR; const EeWs& ee = qp.ah.ee; int nc = 0; for (int f = 0; f < 4; ++f) nc += contact_flag(mode, f);
-  int rows = 0;
+  double* b0 = qp.gl.l0.b; int rows = 0;
   if (level == 0) rows = 18;
   else if (level == 1) rows = (variant == 0) ? (init_phase ? 6 : 10 + 3 * (4 - nc)) : (6 + 3 * (4 - nc));
   else rows = (variant == 0) ? 14 : 12;
@@ -160,10 +174,10 @@ __device__ int build_level(WbcSmem& sm, const Tuning* __restrict__ tn, int level
   __syncwarp();
   if (level == 0) {
     for (int e = lane; e < 6 * 36; e += 32) { const int r = e / 36, k = e % 36; Ap[r * LDZ + k] = (k < NQ) ? sm.M[r * LDM + k] : -sm.Jc[(k - NQ) * LJC + r]; }
-    if (lane < 6) qp.bp[lane] = -sm.nle[lane];
+    if (lane < 6) b0[lane] = -sm.nle[lane];
     int row = 6;
-    for (int f = 0; f < 4; ++f) if (contact_flag(mode, f)) { if (lane < 27) { const int a = lane / 9, c = lane - 9 * a; Ap[(row + a) * LDZ + (c < 6 ? c : foot_first(ffp, f) + c)] = sm.Jc[(3 * f + a) * LJC + c]; } if (lane < 3) qp.bp[row + lane] = -sm.djv_f[3 * f + lane]; row += 3; }
-    for (int f = 0; f < 4; ++f) if (!contact_flag(mode, f)) { if (lane < 3) { Ap[(row + lane) * LDZ + NQ + 3 * f + lane] = 1.0; qp.bp[row + lane] = 0.0; } row += 3; }
+    for (int f = 0; f < 4; ++f) if (contact_flag(mode, f)) { if (lane < 27) { const int a = lane / 9, c = lane - 9 * a; Ap[(row + a) * LDZ + (c < 6 ? c : foot_first(ffp, f) + c)] = sm.Jc[(3 * f + a) * LJC + c]; } if (lane < 3) b0[row + lane] = -sm.djv_f[3 * f + lane]; row += 3; }
+    for (int f = 0; f < 4; ++f) if (!contact_flag(mode, f)) { if (lane < 3) { Ap[(row + lane) * LDZ + NQ + 3 * f + lane] = 1.0; b0[row + lane] = 0.0; } row += 3; }
   } else if (level == 1) {
     int row = 0;
     if (variant == 0 && init_phase) {   // formulateArmJointNomalTrackingTask (WbcBase.cpp:439-465)
@@ -258,7 +272,7 @@ __device__ int solve_level(WbcSmem& sm, const IneqCtx& ic, int rows, int off, in
     const int nfree = nz - kc;
     for (int i = lane; i < nz; i += 32) qp.s[i] = 0.0;
     __syncwarp();
-    if (nfree > 0) cod_lstsq(qp, W1 + kc, nfree, rows, LZ, qp.rhs, qp.s + kc, qp.G, lane);
+    if (nfree > 0) cod_lstsq(W1 + kc, nfree, rows, LZ, qp.rhs, qp.s + kc, qp.gl.G, 18, qp.tau, qp.perm, qp.t18, lane);
     if (kc > 0) w_apply_q(Wc, nz, kc, LZ, qp.tauc, qp.s, lane);
     for (int i = lane; i < 36; i += 32) { double d = 0.0; for (int c = 0; c < nz; ++c) d = fma(Z[i * LZ + off + c], qp.s[c], d); qp.dx[i] = d; }
     __syncwarp();
@@ -410,7 +424,7 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   const Tuning* tn = TUNED ? &sm.tun : tuning_of(mdl, nullptr, 0);
   QpWs& qp = sm.qp; IneqCtx ic{&sm, mode, nc, TUNED ? tuning[(size_t)b * TUNING_DBL + 1] : mdl->wbc_friction, lfp, ffp}; int status = 0;
   const bool init_phase = time < 10.0;   // HierarchicalWbc.cpp:32
-  double* AR = qp.za.q.AR; double* Z = qp.za.q.Z;
+  double* AR = qp.za.q.AR; double* Z = qp.za.q.Z; QpWs::GL::L0& l0 = qp.gl.l0;
   for (int i = lane; i < 36; i += 32) qp.xbar[i] = 0.0;
   __syncwarp();
   // level 0: min ||A0 x - b0||^2 + ||(D0 x - f0)_+||^2  — semismooth iteration on the violated set V.  The rows are factorised IN PLACE (row i of the task is
@@ -420,11 +434,16 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   int k0 = 0;
   for (int it = 0; it < cap0; ++it) {
     int r = build_level(sm, tn, 0, mode, variant, init_phase, ffp, lane); it0 = it + 1;
+    // a pass with more than MAXR rows moves the task rows to the start of Z (not in use before level 0 ends) and lets the violated rows run on into AR;
+    // every other pass works in AR and keeps Z as the scratch of the rank-deficient branch, so the last pass of a robot whose set stays empty leaves the QR of A0 in AR
+    const bool big = r + __popc(vmask0) + __popc(vmask1) > MAXR; double* W = big ? Z : AR;
+    if (big) { for (int e = lane; e < r * LDZ; e += 32) W[e] = AR[e]; __syncwarp(); }
     // append violated rows
-    for (int i = 0; i < nineq; ++i) { const bool in = (i < 32) ? ((vmask0 >> i) & 1u) : ((vmask1 >> (i - 32)) & 1u); if (in) { if (r >= MAXR) { status |= ST_TOO_MANY_ROWS; break; }
-        for (int k = lane; k < 36; k += 32) AR[r * LDZ + k] = ineq_row_elem(ic, i, k); if (lane == 0) qp.bp[r] = ineq_rhs(ic, i); ++r; } }
+    for (int i = 0; i < nineq; ++i) { const bool in = (i < 32) ? ((vmask0 >> i) & 1u) : ((vmask1 >> (i - 32)) & 1u); if (in) { if (r >= MAXR0) { status |= ST_TOO_MANY_ROWS; break; }
+        for (int k = lane; k < 36; k += 32) W[r * LDZ + k] = ineq_row_elem(ic, i, k); if (lane == 0) l0.b[r] = ineq_rhs(ic, i); ++r; } }
     __syncwarp();
-    k0 = cod_lstsq(qp, AR, 36, r, LDZ, qp.bp, qp.xbar, Z, lane);   // Z is not in use yet: scratch of the rank-deficient branch
+    k0 = cod_lstsq(W, 36, r, LDZ, l0.b, qp.xbar, big ? Z + MAXR0 * LDZ : Z, big ? KG0 : 36, l0.tau, l0.perm, l0.t18, lane);
+    if (k0 < 0) { status |= ST_TOO_MANY_ROWS; break; }
     __syncwarp();
     unsigned n0 = 0, n1 = 0;   // next violated set: strictly violated rows, plus rows of V sitting on their boundary
     for (int i = lane; i < nineq; i += 32) { const double val = ineq_row_dot(ic, i, qp.xbar) - ineq_rhs(ic, i); const double sc = 1e-9 * (1.0 + fabs(ineq_rhs(ic, i)));
@@ -442,11 +461,11 @@ __global__ void __launch_bounds__(32 * WBC_WARPS) wbc_update_kernel(const DevMod
   {
     if (vmask0 | vmask1) {   // the last factorisation contains violated rows: factor A0 alone (otherwise the one in AR already is the QR of A0')
       const int rows0 = build_level(sm, tn, 0, mode, variant, init_phase, ffp, lane);
-      k0 = w_qrcp(AR, 36, rows0, LDZ, qp.tau, qp.perm, 1e-11, lane);
+      k0 = w_qrcp(AR, 36, rows0, LDZ, l0.tau, l0.perm, 1e-11, lane);
     }
     nzc = 36 - k0;
     if (nzc > LZ - 1) { status |= ST_TOO_MANY_ROWS; nzc = 0; }   // (A0 has 18 independent rows for every physical model: the mass matrix and a contact Jacobian)
-    else w_form_q_tail(AR, 36, k0, LDZ, qp.tau, Z, LZ, lane);
+    else w_form_q_tail(AR, 36, k0, LDZ, l0.tau, Z, LZ, lane);
   }
   // levels 1 and 2
   for (int level = 1; level <= 2 && nzc > 0; ++level) {

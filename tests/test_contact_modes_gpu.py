@@ -198,12 +198,12 @@ def test_wbc_on_all_16_masks(oracle, variant, time):
     assert compared >= 60 or (variant == 0 and time >= 10), (compared, oracle_off)          # the oracle is certified on most swing-foot robots (tests/test_contact_modes_cpu.py lists where it is not)
 
 
-def _level_certificate(oracle, g, variant, time, x_des, u_des, rbd, mode, period, il, x):
+def _level_certificate(oracle, g, variant, time, x_des, u_des, rbd, mode, period, il, x, mu=0.3):
     """KKT certificate of a WBC result x against the literal level problems of one robot → dict(ok, e0, viol, r1, r2, obj1, obj2).
     e0: distance of A0 x from the level-0 optimum A0 x0 (unique), viol: worst violation of a level-0 inequality (slack included), r1 / r2: NNLS KKT residuals
-    of levels 1 and 2 at x, obj1 / obj2: the level objectives."""
+    of levels 1 and 2 at x, obj1 / obj2: the level objectives.  mu: the robot's friction pyramid (the oracle's task file must hold the same)."""
     dbg = oracle.wbc_debug(x_des, u_des, rbd, int(mode), period, time, input_last=il, variant=variant)
-    (A0, b0, D0, f0), (A1, b1), (A2, b2), _ = tw._tasks(oracle, dbg, u_des, int(mode), time if variant == 0 else 12.0, g)   # HierarchicalMpcWbc has no init branch
+    (A0, b0, D0, f0), (A1, b1), (A2, b2), _ = tw._tasks(oracle, dbg, u_des, int(mode), time if variant == 0 else 12.0, g, mu)   # HierarchicalMpcWbc has no init branch
     if variant == 1:                                                    # HierarchicalMpcWbc.cpp:23-28: height + base angular + base linear + 100 swing, then the forces
         A1, b1, A2, b2 = np.r_[A1[:4], A2[12:14], A1[10:]], np.r_[b1[:4], b2[12:14], b1[10:]], A2[:12], b2[:12]
     x0 = dbg["levels"][0]; fcap = f0 + np.maximum(0.0, D0 @ x0 - f0)

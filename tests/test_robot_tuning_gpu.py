@@ -188,8 +188,8 @@ def test_neutral_rows_are_bit_identical_to_no_rows_and_a_permuted_batch_follows_
 
 
 def test_told_friction_pyramid_is_enforced():
-    """wbc_friction 0.15 / 0.3 / 0.6 on stance states whose desired forces push 30 % sideways: every foot force of a robot without a WBC status bit lies in its
-    own pyramid |Fx|, |Fy| <= mu_b Fz (to 1e-9 of the force scale), and at 0.15 the pyramid binds on some foot, so the check is not vacuous."""
+    """wbc_friction 0.15 / 0.3 / 0.6 on stance states whose desired forces push 30 % sideways: every robot comes out without a WBC status bit, every foot
+    force lies in its own pyramid |Fx|, |Fy| <= mu_b Fz (to 1e-9 of the force scale), and at 0.15 the pyramid binds on some foot, so the check is not vacuous."""
     prob, wbc = _inputs(); mus = np.array([0.15, 0.3, 0.6])[np.arange(B) % 3]
     s = _solver()
     try:
@@ -198,7 +198,7 @@ def test_told_friction_pyramid_is_enforced():
         u_des = np.zeros((B, 30)); u_des[:, 2:12:3] = 80.0; u_des[:, 0:12:3] = rng.uniform(-24.0, 24.0, (B, 4)); u_des[:, 1:12:3] = rng.uniform(-24.0, 24.0, (B, 4))
         cmd, st = s.wbc_update(prob["x0"], u_des, wbc["rbd"], np.full(B, 15, dtype=np.int32), wbc["period"], wbc["time"] + 12.0)
         F = cmd[:, 24:36].reshape(B, 4, 3); scale = np.max(np.abs(F), axis=(1, 2))
-        ok = (st & 0xFF) == 0; assert ok.sum() >= B // 2
+        ok = (st & 0xFF) == 0; assert np.all(ok), np.unique(st)
         excess = np.maximum(np.abs(F[:, :, 0]), np.abs(F[:, :, 1])) - mus[:, None] * F[:, :, 2]
         assert np.all(excess[ok] <= 1e-9 * scale[ok, None]), np.max(excess[ok] / scale[ok, None])
         low = ok & (mus == 0.15); assert np.any(excess[low] >= -1e-9 * scale[low, None])   # a pyramid row is active

@@ -42,8 +42,8 @@ def _rot_err(Rl, Rr):   # rotationErrorInWorld(lhs, rhs): rotation vector of lhs
     return Rotation.from_matrix(Rl @ Rr.T).as_rotvec()
 
 
-def _tasks(oracle, dbg, u_des, mode, time, g):
-    """WbcBase formulators → (A0, b0, D0, f0), (A1, b1), (A2, b2) exactly as HierarchicalWbc::update stacks them."""
+def _tasks(oracle, dbg, u_des, mode, time, g, mu=0.3):
+    """WbcBase formulators → (A0, b0, D0, f0), (A1, b1), (A2, b2) exactly as HierarchicalWbc::update stacks them; mu: the friction pyramid's coefficient."""
     qm, vm, qd, vd, bacc = dbg["q_meas"], dbg["v_meas"], dbg["q_des"], dbg["v_des"], dbg["base_acc"]
     M = oracle.rbd(qm, vm); D = oracle.rbd(qd, vd); info = oracle.model_info()
     flags = [(mode >> (3 - f)) & 1 for f in range(4)]; nc = sum(flags)
@@ -60,7 +60,7 @@ def _tasks(oracle, dbg, u_des, mode, time, g):
     for i in range(4):
         if not flags[i]:
             a_fr[3 * j:3 * j + 3, NQ + 3 * i:NQ + 3 * i + 3] = np.eye(3); j += 1
-    mu = 0.3; pyr = np.array([[0, 0, -1], [1, 0, -mu], [-1, 0, -mu], [0, 1, -mu], [0, -1, -mu]], dtype=float)
+    pyr = np.array([[0, 0, -1], [1, 0, -mu], [-1, 0, -mu], [0, 1, -mu], [0, -1, -mu]], dtype=float)
     d_fr = np.zeros((5 * nc + 3 * (4 - nc), NDEC)); j = 0
     for i in range(4):
         if flags[i]:
@@ -112,11 +112,11 @@ def _certificate(g, A_eq, D_act):
     return rnorm / (1.0 + np.linalg.norm(g))
 
 
-def assert_levels_are_kkt_points(oracle, g, x_des, u_des, rbd, mode, period, time, il, tag=None):
+def assert_levels_are_kkt_points(oracle, g, x_des, u_des, rbd, mode, period, time, il, tag=None, mu=0.3):
     """The three HoQp levels of the oracle's WBC (variant 0) for one robot: level 0 stationary, levels 1 and 2 in the null space of the
     higher-priority tasks, feasible for their inequalities and KKT points with NNLS multipliers; the command follows by updateCmd."""
     dbg = oracle.wbc_debug(x_des, u_des, rbd, int(mode), period, time, input_last=il)
-    (A0, b0, D0, f0), (A1, b1), (A2, b2), M = _tasks(oracle, dbg, u_des, int(mode), time, g)
+    (A0, b0, D0, f0), (A1, b1), (A2, b2), M = _tasks(oracle, dbg, u_des, int(mode), time, g, mu)
     x0, x1, x2 = dbg["levels"]
     # level 0: smooth problem (slack eliminated): A0'(A0 x - b0) + D0' (D0 x - f0)_+ = 0
     v0 = np.maximum(0.0, D0 @ x0 - f0); g0 = A0.T @ (A0 @ x0 - b0) + D0.T @ v0
